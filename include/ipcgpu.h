@@ -117,6 +117,10 @@ int ipcgpu_capture_begin(ipcgpu_ctx* ctx);
 int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id);
 int ipcgpu_graph_launch(ipcgpu_ctx* ctx, int graph_id);
 int ipcgpu_graph_destroy(ipcgpu_ctx* ctx, int graph_id);
+/* kernel nodes of a captured graph at the high and at the low stream priority; a replay keeps each node's priority.  The step-bound chain
+ * runs at the high one and the derivative chain (gradient, Hessian, CSR assembly) at the low one -- the other way round in a graph that
+ * copies derivative results to the host (ipcgpu_download_range_async), where the derivative chain and its copy are the critical path */
+int ipcgpu_graph_kernel_priorities(ipcgpu_ctx* ctx, int graph_id, int* n_high, int* n_low);
 
 /* ---- scene (once per scene; replaces what Mesh<3> precomputes, Mesh.cpp:415-527, :661-671) ------- */
 int ipcgpu_set_mesh(ipcgpu_ctx* ctx, int nV, int nT,

@@ -2,8 +2,9 @@
 //
 // Execution model.  Every stage enqueues its kernels (and, with several ranks, its NCCL reductions) on the context's stream and leaves
 // its scalar results in the device-resident iteration state (kernels.h: IterState).  An entry point synchronises with the host only if
-// the caller hands it a host output pointer; with NULL outputs a whole Newton iteration is one uninterrupted stream, read back once by
-// ipcgpu_fetch_iteration.  The synchronous forms are the same code followed by that read-back.
+// the caller hands it a host output pointer; with NULL outputs a whole Newton iteration runs without a host synchronisation, read back
+// once by ipcgpu_fetch_iteration, its derivative chain on a stream of its own next to the step-bound chain (see enter() below).  The
+// synchronous forms are the same code followed by that read-back.
 #include "../../include/ipcgpu.h"
 #include "context.h"
 #include <algorithm>
@@ -98,6 +99,62 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
     ctx->copy_pending = false;
     return IPCGPU_OK;
 }
+
+// ---- the two chains of an iteration --------------------------------------------------------------------------------------
+// A device-resident iteration is two chains of work that share no written data: the DERIVATIVE chain (value-array clear, per-tet
+// gradient/Hessian kernel, energy reduce/store, gradient gather, CSR assembly + diagonal, barrier gradient, barrier Hessian scatter:
+// wide HBM/FP64-bound grids) and the STEP-BOUND chain (step set, inversion filter, partial CCD, swept broad phase, full CCD: strings of
+// short latency-bound kernels and the Tight-Inclusion passes, the critical path).  The first derivative call in its NULL-output form
+// forks the low-priority stream `deriv` off the main stream; the step-bound calls keep running on the high-priority main stream next
+// to it.  While `deriv` is open only these entry points may run:
+//   - ipcgpu_step_bound_set, ipcgpu_inversion_step, ipcgpu_ccd_partial_ti, ipcgpu_hash_build_swept, ipcgpu_ccd_full_ti with every host
+//     argument NULL (a host search direction rewrites `dir`, a host step reads back);
+//   - the derivative calls in their NULL-output form (they enqueue on `deriv`);
+//   - ipcgpu_allreduce_grad_hess on one rank (a no-op), and ipcgpu_download_range_async, whose copy waits on `deriv` as well.
+// Every other entry point that touches the device calls enter(ctx, kSerial) first, which joins `deriv` into the main stream (the pure
+// host-side getters need not).  The chains stay on one stream with several ranks (the gradient sum and the step-bound min-reductions
+// must keep one order per communicator), while the stage timers are on (each stage is timed alone), and in the synchronous host-output
+// forms.
+//
+// Why the allowed calls cannot race the derivative chain (written by one side / read or written by the other):
+//   - ContactWork::counters: ccd_full clears and counts words 8-9 (broad-phase pairs); the barrier kernels read words 0 and 2 (list sizes,
+//     written by the constraint set before the fork) and the pair-Hessian build clears and counts word 12.  Separate words, and each
+//     cudaMemsetAsync covers only its own.
+//   - IterState: the derivative chain writes energy[0] and flags[FLAG_SET_CAPACITY] / flags[FLAG_PATTERN]; the step-bound chain writes
+//     step_ord, inv_ord, ccd_ord, cand_range, n_full_cand, max_t, alpha_grid, radius, ref_lo, ref_inv_h, alpha_stage, ref_count,
+//     grid_axis_cells, ccd_stats and flags[FLAG_ZERO_CCD_DISTANCE] / [FLAG_CCD_CAPACITY] / [FLAG_TI_WARNINGS].  Aligned words of their own;
+//     nothing clears the struct while `deriv` is open (the fetch clears the flags after joining).
+//   - contact lists: the barrier kernels read act / para / para_e (written by the constraint set before the fork); the step-bound chain
+//     reads ContactWork::cand and writes the grid arrays (vbox, ebox, tbox, bounds, grid, cell_cnt, cell_off, key_tmp, val_tmp, ckeys,
+//     cvals, centries, cub_tmp), bp_pairs and the CcdWork buffers, none of which the derivative chain touches.
+//   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither.  g, a, gcont, hblk, hcon, e_partials2, scalar_out[0], bHraw, brows,
+//     bpsd: derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
+enum Chain { kSerial, kStepBound, kDerivative };
+
+static int join_deriv(ipcgpu_ctx* ctx)
+{
+    if (!ctx->deriv_open) return IPCGPU_OK;
+    ctx->deriv_open = false;
+    CK(cudaEventRecord(ctx->ev_deriv_done, ctx->deriv));
+    CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_deriv_done, 0));
+    return IPCGPU_OK;
+}
+
+static int enter(ipcgpu_ctx* ctx, Chain chain)
+{
+    if (chain == kStepBound) return IPCGPU_OK;
+    if (chain == kSerial || ctx->nranks > 1 || ctx->profiling) return join_deriv(ctx);
+    if (ctx->deriv_open) return IPCGPU_OK;
+    CK(cudaEventRecord(ctx->ev_deriv_fork, ctx->stream)); // everything enqueued so far (positions, contact lists) precedes the chain
+    CK(cudaStreamWaitEvent(ctx->deriv, ctx->ev_deriv_fork, 0));
+    ctx->deriv_open = true;
+    return IPCGPU_OK;
+}
+#define ENTER(chain)                                                                              \
+    do {                                                                                          \
+        int re_ = enter(ctx, (chain));                                                            \
+        if (re_) return re_;                                                                      \
+    } while (0)
 
 // one D2H copy of the iteration state + stream synchronisation
 int fetch_iter_state(ipcgpu_ctx* ctx)
@@ -345,6 +402,25 @@ static int status_from_flags(ipcgpu_ctx* ctx, const int* f)
     return IPCGPU_OK;
 }
 
+// f(node, priority attribute) on every kernel node of a graph, until one returns an error
+template <typename F>
+static cudaError_t for_each_kernel_node(cudaGraph_t g, F f)
+{
+    size_t n = 0;
+    cudaError_t e = cudaGraphGetNodes(g, nullptr, &n);
+    std::vector<cudaGraphNode_t> nodes(n);
+    if (e == cudaSuccess && n) e = cudaGraphGetNodes(g, nodes.data(), &n);
+    for (size_t i = 0; e == cudaSuccess && i < n; ++i) {
+        cudaGraphNodeType type;
+        e = cudaGraphNodeGetType(nodes[i], &type);
+        if (e != cudaSuccess || type != cudaGraphNodeTypeKernel) continue;
+        cudaKernelNodeAttrValue v;
+        e = cudaGraphKernelNodeGetAttribute(nodes[i], cudaKernelNodeAttributePriority, &v);
+        if (e == cudaSuccess) e = f(nodes[i], v);
+    }
+    return e;
+}
+
 extern "C" {
 
 int ipcgpu_create(int device, ipcgpu_ctx** out)
@@ -358,10 +434,14 @@ int ipcgpu_create(int device, ipcgpu_ctx** out)
     ipcgpu_ctx* ctx = new ipcgpu_ctx();
     ctx->device = device;
     void* hi = nullptr;
-    if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess || cudaMallocHost(&ctx->h_scalar, 512) != cudaSuccess
+    if (cudaDeviceGetStreamPriorityRange(&ctx->prio_low, &ctx->prio_high) != cudaSuccess
+        || cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, ctx->prio_high) != cudaSuccess
+        || cudaStreamCreateWithPriority(&ctx->deriv, cudaStreamNonBlocking, ctx->prio_low) != cudaSuccess
+        || cudaEventCreateWithFlags(&ctx->ev_deriv_fork, cudaEventDisableTiming) != cudaSuccess
+        || cudaEventCreateWithFlags(&ctx->ev_deriv_done, cudaEventDisableTiming) != cudaSuccess || cudaMallocHost(&ctx->h_scalar, 512) != cudaSuccess
         || cudaMallocHost(&hi, sizeof(IterState)) != cudaSuccess || !ctx->flag.reserve(4) || !ctx->scalar_out.reserve(32) || !ctx->iter.reserve(1)
         || cudaMemsetAsync(ctx->iter.p, 0, sizeof(IterState), ctx->stream) != cudaSuccess) {
-        delete ctx;
+        ipcgpu_destroy(ctx);
         return IPCGPU_ERR_CUDA;
     }
     ctx->h_iter = static_cast<IterState*>(hi);
@@ -370,8 +450,8 @@ int ipcgpu_create(int device, ipcgpu_ctx** out)
         const char* e = std::getenv("IPCGPU_HESS_LAYOUT");
         if (e) ctx->hess_layout = std::atoi(e) == 0 ? 0 : 1;
     }
-    {   // side stream for the pair-Hessian build + projection (IPCGPU_BARRIER_OVERLAP=0 keeps everything on one stream).  Replayed from a
-        // graph the overlap wins 0.12 ms per iteration (H100 SXM, 400 W, C5: 3.83 -> 3.71 ms)
+    {   // side stream for the pair-Hessian build + projection (IPCGPU_BARRIER_OVERLAP=0 keeps it on the stream of the derivative chain).
+        // Replayed from a graph it wins 0.13 ms per iteration next to the overlapped derivative chain (H100 SXM, 700 W, C5: 3.39 -> 3.25 ms)
         const char* e = std::getenv("IPCGPU_BARRIER_OVERLAP");
         if (!(e && std::atoi(e) == 0)) {
             if (cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&ctx->ev_inputs, cudaEventDisableTiming) != cudaSuccess
@@ -392,6 +472,7 @@ void ipcgpu_destroy(ipcgpu_ctx* ctx)
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     if (ctx->side) cudaStreamSynchronize(ctx->side);
+    if (ctx->deriv) cudaStreamSynchronize(ctx->deriv);
     if (ctx->copy) {
         cudaStreamSynchronize(ctx->copy);
         cudaStreamDestroy(ctx->copy);
@@ -407,6 +488,9 @@ void ipcgpu_destroy(ipcgpu_ctx* ctx)
     if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
     if (ctx->ev_scatter) cudaEventDestroy(ctx->ev_scatter);
     if (ctx->side) cudaStreamDestroy(ctx->side);
+    if (ctx->ev_deriv_fork) cudaEventDestroy(ctx->ev_deriv_fork);
+    if (ctx->ev_deriv_done) cudaEventDestroy(ctx->ev_deriv_done);
+    if (ctx->deriv) cudaStreamDestroy(ctx->deriv);
     for (auto& v : ctx->prof)
         for (auto& pr : v) {
             cudaEventDestroy(pr.first);
@@ -426,6 +510,7 @@ int ipcgpu_host_alloc(void** ptr, uint64_t bytes) { return cudaMallocHost(ptr, b
 int ipcgpu_host_free(void* ptr) { return cudaFreeHost(ptr) == cudaSuccess ? IPCGPU_OK : IPCGPU_ERR_CUDA; }
 int ipcgpu_sync(ipcgpu_ctx* ctx)
 {
+    ENTER(kSerial);
     int rcj = join_copy_stream(ctx);
     if (rcj) return rcj;
     CK(cudaStreamSynchronize(ctx->stream));
@@ -442,6 +527,7 @@ int ipcgpu_comm_unique_id(void* id128)
 
 int ipcgpu_comm_init(ipcgpu_ctx* ctx, int rank, int nranks, const void* id128)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(nranks >= 1 && rank >= 0 && rank < nranks, IPCGPU_ERR_ARG, "bad rank/nranks");
     CK(cudaSetDevice(ctx->device));
@@ -482,6 +568,7 @@ int ipcgpu_partition_info(ipcgpu_ctx* ctx, int* rank, int* nranks, int* tet_begi
 int ipcgpu_set_mesh(ipcgpu_ctx* ctx, int nV, int nT, const double* Vrest, const int* tets, const double* restTriInv, const double* vol,
     const double* mu, const double* lam, const double* mass, const uint8_t* dbc, int energy)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(nV > 0 && nT >= 0 && Vrest && tets && restTriInv && vol && mu && lam, IPCGPU_ERR_ARG, "ipcgpu_set_mesh: null or empty input");
     REQUIRE(energy == IPCGPU_NEOHOOKEAN || energy == IPCGPU_FIXED_COROT, IPCGPU_ERR_ARG, "unknown energy type");
@@ -520,6 +607,7 @@ int ipcgpu_set_mesh(ipcgpu_ctx* ctx, int nV, int nT, const double* Vrest, const 
 
 int ipcgpu_set_csr(ipcgpu_ctx* ctx, int n_rows, const int* ia, const int* ja, int index_base)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(n_rows > 0 && ia && ja && (index_base == 0 || index_base == 1), IPCGPU_ERR_ARG, "ipcgpu_set_csr: bad arguments");
     REQUIRE(ctx->nV > 0 && n_rows == 3 * ctx->nV, IPCGPU_ERR_ARG, "ipcgpu_set_csr: n_rows must be 3*nV of the mesh set before");
@@ -545,6 +633,7 @@ int ipcgpu_set_state(ipcgpu_ctx* ctx, const double* V)
 {
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     if (V) CK(cudaMemcpyAsync(ctx->V.p, V, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     ctx->mark_inputs();
     return IPCGPU_OK;
@@ -553,6 +642,7 @@ int ipcgpu_set_state(ipcgpu_ctx* ctx, const double* V)
 int ipcgpu_save_state(ipcgpu_ctx* ctx)
 {
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    ENTER(kSerial);
     CK(cudaMemcpyAsync(ctx->Vsaved.p, ctx->V.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
     ctx->state_saved = true;
     return IPCGPU_OK;
@@ -592,6 +682,7 @@ int ipcgpu_set_search_dir(ipcgpu_ctx* ctx, const double* p)
 {
     REQUIRE(ctx->nV > 0 && p, IPCGPU_ERR_ARG, "ipcgpu_set_search_dir: mesh and p required");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     return upload_dir(ctx, p);
 }
 
@@ -600,6 +691,7 @@ int ipcgpu_step_forward(ipcgpu_ctx* ctx, const double* p, double alpha)
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     REQUIRE(ctx->state_saved, IPCGPU_ERR_STATE, "ipcgpu_save_state must precede ipcgpu_step_forward");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc = upload_dir(ctx, p);
     if (rc) return rc;
     step_forward(ctx->nV, ctx->Vsaved.p, ctx->dir.p, alpha, ctx->V.p, ctx->stream);
@@ -613,6 +705,7 @@ int ipcgpu_elastic_energy(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, double*
 {
     REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_ELASTIC_ENERGY);
     elastic_energy(ctx->eargs(), ctx->e_per_tet.p, ctx->partials.p, coef, ctx->scalar_out.p, ctx->stream);
     ctx->prof_end(pe);
@@ -636,10 +729,13 @@ int ipcgpu_elastic_energy(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, double*
 // zero the part of the value array this rank writes (everything after a cross-rank completion has filled the other rows)
 static int zero_values(ipcgpu_ctx* ctx)
 {
+    cudaStream_t st = ctx->deriv_stream(); // (zero_words, not a memset: kernels.h)
     if (ctx->nranks > 1 && !ctx->a_all_dirty) {
-        if (ctx->a_end > ctx->a_begin) CK(cudaMemsetAsync(ctx->a.p + ctx->a_begin, 0, (size_t)(ctx->a_end - ctx->a_begin) * sizeof(double), ctx->stream));
+        if (ctx->a_end > ctx->a_begin) zero_words(ctx->a.p + ctx->a_begin, (size_t)(ctx->a_end - ctx->a_begin) * 2, st);
     }
-    else CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)ctx->nnz * sizeof(double), ctx->stream));
+    else zero_words(ctx->a.p, (size_t)ctx->nnz * 2, st);
+    ++ctx->launches;
+    CK(cudaGetLastError());
     ctx->a_all_dirty = false;
     return IPCGPU_OK;
 }
@@ -651,6 +747,7 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
         int rc = ensure_offsets(ctx);
         if (rc) return rc;
     }
+    cudaStream_t st = ctx->deriv_stream(); // (stage timers are only on when it is the main stream)
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_ELASTIC_TET);
     double* e_part = nullptr;
     if (with_energy) { // psi * vol per CTA, summed in fixed order below (computeEnergyVal at the same state: the SVD is shared)
@@ -658,14 +755,14 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
         e_part = ctx->e_partials2.p;
     }
     const bool slot_major = need_h && ctx->hess_layout == 1;
-    elastic_grad_hess(ctx->eargs(), coef, projectSPD, need_g, need_h, ctx->gcont.p, ctx->hblk.p, ctx->stream, e_part, slot_major ? ctx->hdst.p : nullptr, ctx->hcon.p);
+    elastic_grad_hess(ctx->eargs(), coef, projectSPD, need_g, need_h, ctx->gcont.p, ctx->hblk.p, st, e_part, slot_major ? ctx->hdst.p : nullptr, ctx->hcon.p);
     ctx->hblk_valid = need_h && !slot_major;
     ctx->prof_end(pe);
     ++ctx->launches;
     if (with_energy) {
         pe = ctx->prof_begin(IPCGPU_STAGE_ELASTIC_ENERGY);
-        reduce_sum(e_part, elastic_grad_hess_blocks(ctx->n_list), coef, ctx->scalar_out.p, ctx->stream);
-        energy_store(ctx->iter.p, 0, ctx->scalar_out.p, ctx->stream);
+        reduce_sum(e_part, elastic_grad_hess_blocks(ctx->n_list), coef, ctx->scalar_out.p, st);
+        energy_store(ctx->iter.p, 0, ctx->scalar_out.p, st);
         ctx->prof_end(pe);
         ctx->launches += 2;
         ctx->energy_local[0] = ctx->nranks > 1;
@@ -673,7 +770,7 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
     if (need_g) {
         // owned vertices gather their complete sums (every incident tet is in this rank's list); the other rows are written as zeros
         pe = ctx->prof_begin(IPCGPU_STAGE_GATHER_GRADIENT);
-        gather_gradient(ctx->nV, ctx->inc_ptr.p, ctx->inc.p, ctx->gcont.p, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, 0, ctx->g.p, ctx->stream);
+        gather_gradient(ctx->nV, ctx->inc_ptr.p, ctx->inc.p, ctx->gcont.p, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, 0, ctx->g.p, st);
         ctx->prof_end(pe);
         ++ctx->launches;
     }
@@ -681,13 +778,13 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
         pe = ctx->prof_begin(IPCGPU_STAGE_ASSEMBLE_CSR);
         if (slot_major)
             assemble_slot_major(ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->slot_off.p, ctx->cbase.p, ctx->hcon.p, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, 1, ctx->a.p,
-                ctx->stream);
+                st);
         else
             assemble_csr(ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->slot_off.p, ctx->con_ptr.p, ctx->con_src.p, ctx->hblk.p,
-                ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, nullptr, 1, ctx->a.p, ctx->stream);
+                ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, nullptr, 1, ctx->a.p, st);
         // per-vertex diagonal terms (mass, Dirichlet identity) of the owned rows
         const double* m = (add_mass && ctx->has_mass) ? ctx->mass.p : nullptr;
-        diag_mass_dbc_range(ctx->v_begin, ctx->v_end, ctx->ia.p, ctx->index_base, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, m, ctx->a.p, ctx->stream);
+        diag_mass_dbc_range(ctx->v_begin, ctx->v_end, ctx->ia.p, ctx->index_base, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, m, ctx->a.p, st);
         ctx->prof_end(pe);
         ctx->launches += 2;
     }
@@ -698,6 +795,7 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
 int ipcgpu_elastic_gradient(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, int projectDBC, double* g)
 {
     CK(cudaSetDevice(ctx->device));
+    ENTER(g ? kSerial : kDerivative);
     int rc = run_grad_hess(ctx, coef, 1, projectDBC, true, false, 0);
     if (rc) return rc;
     if (ctx->nranks > 1 && g) { // host result requested: complete it across ranks; NULL = deferred (ipcgpu_allreduce_grad_hess)
@@ -733,6 +831,7 @@ int ipcgpu_elastic_hessian(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, int pr
 {
     CK(cudaSetDevice(ctx->device));
     REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
+    ENTER(a_inout ? kSerial : kDerivative);
     int rc;
     if (a_inout && (rc = upload_values(ctx, a_inout))) return rc;
     if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, false, true, 0))) return rc;
@@ -744,6 +843,7 @@ int ipcgpu_elastic_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int p
 {
     CK(cudaSetDevice(ctx->device));
     REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
+    ENTER(g || a ? kSerial : kDerivative);
     // the value array is rebuilt from scratch (LinSysSolver::setZero, then addCoeff of every term): slots that no local tet touches
     // -- contact-only blocks of the augmented pattern -- must not keep last iteration's values
     int rc = zero_values(ctx);
@@ -763,6 +863,7 @@ int ipcgpu_elastic_energy_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD
 {
     CK(cudaSetDevice(ctx->device));
     REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
+    ENTER(E || g || a ? kSerial : kDerivative);
     // the value array is rebuilt from scratch (LinSysSolver::setZero, then addCoeff of every term): slots that no local tet touches
     // -- contact-only blocks of the augmented pattern -- must not keep last iteration's values
     int rc = zero_values(ctx);
@@ -793,6 +894,7 @@ int ipcgpu_step_bound_set(ipcgpu_ctx* ctx, double alpha)
 {
     REQUIRE(alpha >= 0.0, IPCGPU_ERR_ARG, "the step must be non-negative");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kStepBound);
     step_set(ctx->iter.p, alpha, ctx->stream);
     ++ctx->launches;
     CK(cudaGetLastError());
@@ -803,6 +905,7 @@ int ipcgpu_inversion_step(ipcgpu_ctx* ctx, const double* p, double slack, double
 {
     REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(p || alpha_inout ? kSerial : kStepBound);
     int rc = upload_dir(ctx, p);
     if (rc) return rc;
     if (alpha_inout && (rc = ipcgpu_step_bound_set(ctx, *alpha_inout))) return rc;
@@ -821,6 +924,7 @@ int ipcgpu_inversion_step(ipcgpu_ctx* ctx, const double* p, double slack, double
 // ---- contact ---------------------------------------------------------------------------------------------
 int ipcgpu_set_surface(ipcgpu_ctx* ctx, int nSV, const int* SVI, int nSE, const int* SE, int nSF, const int* SF, const int* vCoDim)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     REQUIRE(nSV >= 0 && nSE >= 0 && nSF >= 0 && (nSV == 0 || SVI) && (nSE == 0 || SE) && (nSF == 0 || SF), IPCGPU_ERR_ARG, "ipcgpu_set_surface: bad arguments");
@@ -845,6 +949,7 @@ int ipcgpu_set_surface(ipcgpu_ctx* ctx, int nSV, const int* SVI, int nSE, const 
 
 int ipcgpu_set_obstacle_tail(ipcgpu_ctx* ctx, int first_obstacle_vertex, int ee_through_vf_routine)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (the pair rules change)
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     if (first_obstacle_vertex < 0 || first_obstacle_vertex >= ctx->nV) { // no obstacle
@@ -873,6 +978,7 @@ int ipcgpu_set_obstacle_positions(ipcgpu_ctx* ctx, const double* Vo_soa)
     REQUIRE(ctx->nV > 0 && ctx->nVdof < ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_obstacle_tail first");
     REQUIRE(Vo_soa, IPCGPU_ERR_ARG, "null argument");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     const size_t nVo = (size_t)(ctx->nV - ctx->nVdof);
     // current AND rest positions: the obstacle has no rest shape of its own, compute_eps_x takes its current edge lengths
     // (MeshCollisionUtils.hpp:2976-2981); SoA with the stride of the whole vertex array
@@ -886,6 +992,7 @@ int ipcgpu_set_obstacle_positions(ipcgpu_ctx* ctx, const double* Vo_soa)
 
 int ipcgpu_set_ccd_capacity(ipcgpu_ctx* ctx, uint64_t capacity)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(capacity > 0 && capacity < 0xffffffffull, IPCGPU_ERR_ARG, "capacity out of range");
     ctx->ccd_capacity = (size_t)capacity;
@@ -935,6 +1042,7 @@ int ipcgpu_ccd_partial_ti(ipcgpu_ctx* ctx, const double* p, double tol, const do
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(err_vf && err_ee, IPCGPU_ERR_ARG, "null argument");
     CK(cudaSetDevice(ctx->device));
+    ENTER(p || alpha_inout ? kSerial : kStepBound);
     int rc = upload_dir(ctx, p);
     if (rc) return rc;
     if (alpha_inout && (rc = ipcgpu_step_bound_set(ctx, *alpha_inout))) return rc;
@@ -952,6 +1060,7 @@ int ipcgpu_hash_build_swept(ipcgpu_ctx* ctx, const double* p, double* alpha_inou
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(h > 0.0, IPCGPU_ERR_ARG, "bad arguments");
     CK(cudaSetDevice(ctx->device));
+    ENTER(p || alpha_inout ? kSerial : kStepBound);
     int rc = upload_dir(ctx, p);
     if (rc) return rc;
     REQUIRE(ctx->pSize_surface, IPCGPU_ERR_STATE, "the search direction was uploaded before ipcgpu_set_surface: upload it again");
@@ -966,6 +1075,7 @@ int ipcgpu_ccd_full_ti(ipcgpu_ctx* ctx, double tol, const double err_vf[3], cons
     REQUIRE(ctx->surface_ready && ctx->ccd.swept_ready, IPCGPU_ERR_STATE, "ipcgpu_hash_build_swept first");
     REQUIRE(err_vf && err_ee, IPCGPU_ERR_ARG, "null argument");
     CK(cudaSetDevice(ctx->device));
+    ENTER(alpha_inout || n_candidates ? kSerial : kStepBound);
     int rc;
     // (the swept grid was built for the step the chain held then; a host step that differs from it only lowers max_t)
     if (alpha_inout && (rc = ipcgpu_step_bound_set(ctx, *alpha_inout))) return rc;
@@ -1008,6 +1118,7 @@ int ipcgpu_ccd_stats_timing(ipcgpu_ctx* ctx, uint64_t* longest_pair_cycles, uint
 
 int ipcgpu_set_hessian_layout(ipcgpu_ctx* ctx, int layout)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (another kernel pair)
     REQUIRE(layout == 0 || layout == 1, IPCGPU_ERR_ARG, "layout: 0 tile-major (per-tet blocks downloadable), 1 slot-major");
     ctx->hess_layout = layout;
@@ -1016,6 +1127,7 @@ int ipcgpu_set_hessian_layout(ipcgpu_ctx* ctx, int layout)
 
 int ipcgpu_set_exchange_capacity(ipcgpu_ctx* ctx, int pairs_per_rank)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (the message buffers change)
     REQUIRE(pairs_per_rank > 0, IPCGPU_ERR_ARG, "capacity must be positive");
     ctx->exchange_capacity = pairs_per_rank;
@@ -1025,6 +1137,7 @@ int ipcgpu_set_exchange_capacity(ipcgpu_ctx* ctx, int pairs_per_rank)
 
 int ipcgpu_set_pair_capacity(ipcgpu_ctx* ctx, int capacity)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(capacity > 0, IPCGPU_ERR_ARG, "capacity must be positive");
     ctx->pair_capacity = capacity;
@@ -1037,6 +1150,7 @@ int ipcgpu_constraint_set(ipcgpu_ctx* ctx, double dHat, int getPTEE, int* nC, in
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(dHat > 0.0, IPCGPU_ERR_ARG, "dHat must be positive");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc = contact_constraint_set(ctx, dHat, getPTEE, nC, nPara, nCand);
     ctx->lists_local = (rc == 0) && ctx->partition_contact && ctx->nranks > 1;
     ctx->cw.lists_global = false;
@@ -1059,6 +1173,7 @@ int ipcgpu_constraint_set(ipcgpu_ctx* ctx, double dHat, int getPTEE, int* nC, in
 
 int ipcgpu_set_canonical_order(ipcgpu_ctx* ctx, int enable)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     ctx->canonical_order = enable != 0;
     return IPCGPU_OK;
@@ -1066,6 +1181,7 @@ int ipcgpu_set_canonical_order(ipcgpu_ctx* ctx, int enable)
 
 int ipcgpu_set_contact_partition(ipcgpu_ctx* ctx, int enable)
 {
+    ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     ctx->partition_contact = enable != 0;
     return IPCGPU_OK;
@@ -1074,6 +1190,7 @@ int ipcgpu_set_contact_partition(ipcgpu_ctx* ctx, int enable)
 int ipcgpu_get_constraint_set(ipcgpu_ctx* ctx, int* mm, int* para, int* para_e, int* cand)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    ENTER(kSerial);
     ContactWork& w = ctx->cw;
     if (w.nC < 0) { // built without a read-back: fetch the sizes now
         int rc = contact_sync_counts(ctx);
@@ -1090,6 +1207,7 @@ int ipcgpu_get_constraint_set(ipcgpu_ctx* ctx, int* mm, int* para, int* para_e, 
 int ipcgpu_constraint_set_sizes(ipcgpu_ctx* ctx, int* nC, int* nPara, int* nCand)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    ENTER(kSerial);
     ContactWork& w = ctx->cw;
     if (w.nC < 0) {
         int rc = contact_sync_counts(ctx);
@@ -1104,6 +1222,7 @@ int ipcgpu_constraint_set_sizes(ipcgpu_ctx* ctx, int* nC, int* nPara, int* nCand
 int ipcgpu_set_constraint_set(ipcgpu_ctx* ctx, int nC, const int* mm, int nP, const int* para, const int* para_e, int nK, const int* cand)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    ENTER(kSerial);
     ContactWork& w = ctx->cw;
     REQUIRE(nC >= 0 && nP >= 0 && nK >= 0 && nC <= w.cap && nP <= w.cap && nK <= 4 * w.cap, IPCGPU_ERR_CAPACITY, "set exceeds the pair capacity");
     if (nC) CK(cudaMemcpyAsync(w.act.p, mm, (size_t)nC * sizeof(int4), cudaMemcpyHostToDevice, ctx->stream));
@@ -1149,6 +1268,7 @@ int ipcgpu_barrier_energy(ipcgpu_ctx* ctx, double dHat, double kappa, double* E)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     BarrierArgs p = barrier_args(ctx, dHat, kappa, 0);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     barrier_energy(p, ctx->cw.bpartials.p, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE], ctx->stream);
@@ -1181,12 +1301,13 @@ int ipcgpu_barrier_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(g_inout ? kSerial : kDerivative);
     if (g_inout) {
         if (ctx->rank == 0) CK(cudaMemcpyAsync(ctx->g.p, g_inout, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
         else CK(cudaMemsetAsync(ctx->g.p, 0, (size_t)3 * ctx->nV * sizeof(double), ctx->stream));
     }
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
-    barrier_gradient(barrier_args(ctx, dHat, kappa, 0), ctx->g.p, ctx->stream);
+    barrier_gradient(barrier_args(ctx, dHat, kappa, 0), ctx->g.p, ctx->deriv_stream());
     ctx->prof_end(pe);
     ++ctx->launches;
     CK(cudaGetLastError());
@@ -1223,6 +1344,7 @@ int ipcgpu_evaluate_constraints(ipcgpu_ctx* ctx, double* val, int n)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     ContactWork& w = ctx->cw;
     if (w.nC < 0) {
         int rc = contact_sync_counts(ctx);
@@ -1245,6 +1367,7 @@ int ipcgpu_constraint_jacobian_t(ipcgpu_ctx* ctx, const double* input, int n, do
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(g_inout != nullptr, IPCGPU_ERR_ARG, "null gradient");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     ContactWork& w = ctx->cw;
     if (w.nC < 0) {
         int rc = contact_sync_counts(ctx);
@@ -1269,6 +1392,7 @@ int ipcgpu_para_ee_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(g_inout != nullptr, IPCGPU_ERR_ARG, "null gradient");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc = gradient_roundtrip_begin(ctx, g_inout);
     if (rc) return rc;
     para_gradient(barrier_args(ctx, dHat, kappa, 0), ctx->g.p, ctx->stream);
@@ -1282,23 +1406,25 @@ int ipcgpu_barrier_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int proje
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(a_inout ? kSerial : kDerivative);
     int rc;
     if (a_inout && (rc = upload_values(ctx, a_inout))) return rc;
     ContactWork& w = ctx->cw;
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     const BarrierArgs bp = barrier_args(ctx, dHat, kappa, projectDBC);
+    cudaStream_t st = ctx->deriv_stream();
     if (ctx->side && ctx->inputs_marked) {
         // build + projection on the side stream, ordered after the last change of their inputs (positions, contact sets) -- i.e. next to
-        // whatever the main stream has queued since (the elastic assembly); the scatter joins the main stream, after the elastic writes
+        // whatever has been queued since (the elastic assembly); the scatter joins the derivative chain, after the elastic writes
         CK(cudaStreamWaitEvent(ctx->side, ctx->ev_inputs, 0));
         if (ctx->scatter_marked) CK(cudaStreamWaitEvent(ctx->side, ctx->ev_scatter, 0)); // back-to-back calls: the last scatter still reads the buffers
         barrier_hessian_build_project(bp, ctx->iter.p->flags, w.bHraw.p, w.brows.p, w.bpsd.p, w.counters.p + 12, w.cap, ctx->side);
         CK(cudaEventRecord(ctx->ev_join, ctx->side));
-        CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+        CK(cudaStreamWaitEvent(st, ctx->ev_join, 0));
     }
-    else barrier_hessian_build_project(bp, ctx->iter.p->flags, w.bHraw.p, w.brows.p, w.bpsd.p, w.counters.p + 12, w.cap, ctx->stream);
-    barrier_hessian_scatter(bp, ctx->a.p, ctx->iter.p->flags, w.bHraw.p, w.brows.p, w.bpsd.p, w.counters.p + 12, w.cap, ctx->stream);
-    if (ctx->side && ctx->ev_scatter) ctx->scatter_marked = (cudaEventRecord(ctx->ev_scatter, ctx->stream) == cudaSuccess);
+    else barrier_hessian_build_project(bp, ctx->iter.p->flags, w.bHraw.p, w.brows.p, w.bpsd.p, w.counters.p + 12, w.cap, st);
+    barrier_hessian_scatter(bp, ctx->a.p, ctx->iter.p->flags, w.bHraw.p, w.brows.p, w.bpsd.p, w.counters.p + 12, w.cap, st);
+    if (ctx->side && ctx->ev_scatter) ctx->scatter_marked = (cudaEventRecord(ctx->ev_scatter, st) == cudaSuccess);
     ctx->prof_end(pe);
     ctx->launches += 3;
     CK(cudaGetLastError());
@@ -1322,6 +1448,7 @@ int ipcgpu_set_prev_state(ipcgpu_ctx* ctx, const double* V_prev_soa)
 {
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     ALLOC(ctx->Vprev, (size_t)3 * ctx->nV);
     if (V_prev_soa) CK(cudaMemcpyAsync(ctx->Vprev.p, V_prev_soa, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     else CK(cudaMemcpyAsync(ctx->Vprev.p, ctx->V.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream)); // V_prev = V at the start of a step
@@ -1346,6 +1473,7 @@ int ipcgpu_friction_lag(ipcgpu_ctx* ctx, double dHat, double kappa, int* n_pairs
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc = friction_alloc(ctx);
     if (rc) return rc;
     ContactWork& w = ctx->cw;
@@ -1380,6 +1508,7 @@ int ipcgpu_get_friction_data(ipcgpu_ctx* ctx, int* n_pairs, int* mmcvid4, double
 {
     REQUIRE(ctx->cw.fr_ready, IPCGPU_ERR_STATE, "ipcgpu_friction_lag / ipcgpu_set_friction_data first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc = friction_host_count(ctx);
     if (rc) return rc;
     ContactWork& w = ctx->cw;
@@ -1399,6 +1528,7 @@ int ipcgpu_set_friction_data(ipcgpu_ctx* ctx, int n_pairs, const int* mmcvid4, c
     REQUIRE(n_pairs >= 0 && n_pairs <= ctx->pair_capacity, IPCGPU_ERR_CAPACITY, "friction set larger than the pair capacity");
     REQUIRE(n_pairs == 0 || (mmcvid4 && lambda && coord2 && basis6), IPCGPU_ERR_ARG, "null friction arrays");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc = friction_alloc(ctx);
     if (rc) return rc;
     ContactWork& w = ctx->cw;
@@ -1438,6 +1568,7 @@ int ipcgpu_friction_energy(ipcgpu_ctx* ctx, double eps2, double coef, double* E)
     REQUIRE_FRICTION();
     REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     friction_energy(friction_args(ctx, eps2, coef, 0), ctx->cw.fr_partials.p, ctx->stream);
     reduce_sum(ctx->cw.fr_partials.p, friction_energy_blocks(), coef, ctx->scalar_out.p + 2, ctx->stream);
@@ -1464,6 +1595,7 @@ int ipcgpu_friction_gradient(ipcgpu_ctx* ctx, double eps2, double coef, double* 
     REQUIRE_FRICTION();
     REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc;
     if (g_inout && (rc = gradient_roundtrip_begin(ctx, g_inout))) return rc;
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
@@ -1481,6 +1613,7 @@ int ipcgpu_friction_hessian(ipcgpu_ctx* ctx, double eps2, double coef, int proje
     REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive");
     REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc;
     if (a_inout && (rc = upload_values(ctx, a_inout))) return rc;
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
@@ -1507,6 +1640,7 @@ int ipcgpu_set_xtilde(ipcgpu_ctx* ctx, const double* xtilde_soa)
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     REQUIRE(xtilde_soa != nullptr, IPCGPU_ERR_ARG, "null xTilta");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     ALLOC(ctx->xtilde, (size_t)3 * ctx->nV);
     CK(cudaMemcpyAsync(ctx->xtilde.p, xtilde_soa, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     ctx->xtilde_set = true;
@@ -1517,6 +1651,7 @@ int ipcgpu_inertia_energy(ipcgpu_ctx* ctx, double* E)
 {
     REQUIRE(ctx->xtilde_set && ctx->has_mass, IPCGPU_ERR_STATE, "ipcgpu_set_xtilde and a mass diagonal (ipcgpu_set_mesh) first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     // vertex blocks [nV r / N, nV (r+1) / N): every vertex exactly once across the ranks
     const int v0 = (int)((long long)ctx->nV * ctx->rank / ctx->nranks), v1 = (int)((long long)ctx->nV * (ctx->rank + 1) / ctx->nranks);
     ALLOC(ctx->in_partials, (size_t)inertia_energy_blocks(ctx->nV) + 8);
@@ -1545,6 +1680,7 @@ int ipcgpu_inertia_gradient(ipcgpu_ctx* ctx, int projectDBC, double* g_inout)
 {
     REQUIRE(ctx->xtilde_set && ctx->has_mass, IPCGPU_ERR_STATE, "ipcgpu_set_xtilde and a mass diagonal (ipcgpu_set_mesh) first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     if (g_inout) CK(cudaMemcpyAsync(ctx->g.p, g_inout, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     // Device-resident form with several ranks: the gradient is summed over the ranks later (ipcgpu_allreduce_grad_hess), so only rank 0 adds
     // the per-vertex term.  Host form: every rank holds the caller's vector and adds the full term -- no reduction needed.
@@ -1599,8 +1735,10 @@ int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
     REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is already in progress");
     REQUIRE(!ctx->profiling, IPCGPU_ERR_STATE, "switch the stage timers off (ipcgpu_profile(ctx, 0)) before capturing");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     ctx->inputs_marked = false;  // the side-stream fork of the pair Hessians must hang on an event recorded INSIDE the capture
     ctx->scatter_marked = false;
+    ctx->deriv_copied = false;
     ctx->launches_at_capture = ctx->launches;
     ctx->dirty_at_capture = ctx->a_all_dirty;
     CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
@@ -1612,8 +1750,9 @@ int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id)
 {
     REQUIRE(ctx->capturing, IPCGPU_ERR_STATE, "no capture in progress");
     REQUIRE(graph_id != nullptr, IPCGPU_ERR_ARG, "null graph id");
+    ENTER(kSerial); // forked branches (derivative chain, copies) must rejoin the capturing stream
     {
-        int rcj = join_copy_stream(ctx); // a forked copy branch must rejoin the capturing stream
+        int rcj = join_copy_stream(ctx);
         if (rcj) return rcj;
     }
     ctx->capturing = false;
@@ -1624,7 +1763,22 @@ int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id)
         ctx->err = std::string("stream capture failed (a call inside the capture synchronised or copied to the host? use NULL outputs): ") + cudaGetErrorString(e);
         return IPCGPU_ERR_CUDA;
     }
-    e = cudaGraphInstantiate(&rec.exec, rec.graph, 0);
+    if (ctx->deriv_copied) {
+        // the sequence hands the derivative chain's results to the host: that chain and the copy behind it (longer than the step-bound
+        // chain) are now the critical path, so in this graph the two chains trade priorities
+        e = for_each_kernel_node(rec.graph, [&](cudaGraphNode_t node, cudaKernelNodeAttrValue v) {
+            v.priority = (v.priority == ctx->prio_high) ? ctx->prio_low : ctx->prio_high;
+            return cudaGraphKernelNodeSetAttribute(node, cudaKernelNodeAttributePriority, &v);
+        });
+        if (e != cudaSuccess) {
+            cudaGraphDestroy(rec.graph);
+            ctx->err = std::string("kernel node priorities: ") + cudaGetErrorString(e);
+            return IPCGPU_ERR_CUDA;
+        }
+    }
+    // kernel nodes carry the priority of the stream they were captured from; without this flag a replay would run every node at the
+    // priority of the stream it is launched into
+    e = cudaGraphInstantiateWithFlags(&rec.exec, rec.graph, cudaGraphInstantiateFlagUseNodePriority);
     if (e != cudaSuccess) {
         cudaGraphDestroy(rec.graph);
         ctx->err = std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e);
@@ -1649,6 +1803,7 @@ int ipcgpu_graph_launch(ipcgpu_ctx* ctx, int graph_id)
     const ipcgpu_ctx::GraphRec& rec = ctx->graphs[graph_id];
     REQUIRE(rec.epoch == ctx->epoch, IPCGPU_ERR_STATE, "the scene, pattern, partition or capacities changed since this graph was captured: capture it again");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     if (ctx->a_all_dirty && !rec.dirty_at_begin) // a cross-rank completion filled rows the captured clear does not cover
         CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)ctx->nnz * sizeof(double), ctx->stream));
     CK(cudaGraphLaunch(rec.exec, ctx->stream));
@@ -1661,11 +1816,26 @@ int ipcgpu_graph_launch(ipcgpu_ctx* ctx, int graph_id)
 int ipcgpu_graph_destroy(ipcgpu_ctx* ctx, int graph_id)
 {
     REQUIRE(graph_id >= 0 && graph_id < (int)ctx->graphs.size(), IPCGPU_ERR_ARG, "unknown graph id");
+    ENTER(kSerial);
     ipcgpu_ctx::GraphRec& rec = ctx->graphs[graph_id];
     if (rec.exec) cudaGraphExecDestroy(rec.exec);
     if (rec.graph) cudaGraphDestroy(rec.graph);
     rec.exec = nullptr;
     rec.graph = nullptr;
+    return IPCGPU_OK;
+}
+
+int ipcgpu_graph_kernel_priorities(ipcgpu_ctx* ctx, int graph_id, int* n_high, int* n_low)
+{
+    REQUIRE(graph_id >= 0 && graph_id < (int)ctx->graphs.size() && ctx->graphs[graph_id].graph, IPCGPU_ERR_ARG, "unknown graph id");
+    REQUIRE(n_high && n_low, IPCGPU_ERR_ARG, "null argument");
+    CK(cudaSetDevice(ctx->device));
+    *n_high = *n_low = 0;
+    CK(for_each_kernel_node(ctx->graphs[graph_id].graph, [&](cudaGraphNode_t, cudaKernelNodeAttrValue v) {
+        if (v.priority == ctx->prio_high) ++*n_high;
+        else if (v.priority == ctx->prio_low) ++*n_low;
+        return cudaSuccess;
+    }));
     return IPCGPU_OK;
 }
 
@@ -1684,6 +1854,7 @@ int ipcgpu_check_inversion(ipcgpu_ctx* ctx, int* n_inverted)
 {
     REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc = safeguard_inversion(ctx);
     REQUIRE(rc == 0, rc, "inversion check launch failed");
     ctx->checks_local = true;
@@ -1700,6 +1871,7 @@ int ipcgpu_intersection_free(ipcgpu_ctx* ctx, int* ok)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_HASH);
     int rc = safeguard_intersections(ctx);
     ctx->prof_end(pe);
@@ -1721,6 +1893,7 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
     REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the built-in solver runs on one rank (a distributed solver takes each rank's rows: ipcgpu_partition_info)");
     REQUIRE(rel_tol > 0.0 && max_iter > 0, IPCGPU_ERR_ARG, "bad tolerance / iteration limit");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     if (!ctx->full_pattern_ready) { // once per sparsity pattern: rows of both triangles, gathered through a position map
         std::vector<int> ia((size_t)ctx->n_rows + 1), ja((size_t)ctx->nnz);
         CK(cudaMemcpyAsync(ia.data(), ctx->ia.p, ia.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1750,6 +1923,7 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
 int ipcgpu_csr_set_zero(ipcgpu_ctx* ctx)
 {
     REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
+    ENTER(kSerial);
     return zero_values(ctx);
 }
 
@@ -1757,6 +1931,7 @@ int ipcgpu_allreduce_grad_hess(ipcgpu_ctx* ctx, int with_gradient, int with_hess
 {
     if (ctx->nranks <= 1) return IPCGPU_OK;
     REQUIRE(ctx->nccl_comm != nullptr, IPCGPU_ERR_STATE, "ipcgpu_comm_init first");
+    ENTER(kSerial);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_ALLREDUCE);
     if (with_gradient) { // elastic part: every rank holds the complete rows it owns (zeros elsewhere); barrier part: partial sums
         int r = g_nccl.AllReduce(ctx->g.p, ctx->g.p, (size_t)3 * ctx->nV, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
@@ -1777,6 +1952,7 @@ int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
 {
     REQUIRE(out != nullptr, IPCGPU_ERR_ARG, "null output");
     CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     if (ctx->nranks > 1) {
         // complete the deferred scalars across ranks in ONE collective: locally summed energies, the error flags (so that every rank
         // returns the same status) and the safeguard counts (round 2, first half: up to six separate NCCL calls here)
@@ -1830,6 +2006,7 @@ int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
 int ipcgpu_profile(ipcgpu_ctx* ctx, int enable)
 {
     REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "stage timers cannot be switched inside a capture");
+    ENTER(kSerial);
     CK(cudaStreamSynchronize(ctx->stream));
     for (int s = 0; s < IPCGPU_STAGE_COUNT; ++s) {
         for (auto& pr : ctx->prof[s]) {
@@ -1845,6 +2022,7 @@ int ipcgpu_profile(ipcgpu_ctx* ctx, int enable)
 int ipcgpu_profile_read(ipcgpu_ctx* ctx, int stage, double* total_ms, int* count)
 {
     REQUIRE(stage >= 0 && stage < IPCGPU_STAGE_COUNT && total_ms && count, IPCGPU_ERR_ARG, "bad stage");
+    ENTER(kSerial);
     CK(cudaStreamSynchronize(ctx->stream));
     double tot = 0.0;
     for (auto& pr : ctx->prof[stage]) {
@@ -1859,6 +2037,7 @@ int ipcgpu_profile_read(ipcgpu_ctx* ctx, int stage, double* total_ms, int* count
 
 int ipcgpu_timer_start(ipcgpu_ctx* ctx)
 {
+    ENTER(kSerial);
     if (!ctx->timer_a) {
         CK(cudaEventCreate(&ctx->timer_a));
         CK(cudaEventCreate(&ctx->timer_b));
@@ -1870,6 +2049,7 @@ int ipcgpu_timer_start(ipcgpu_ctx* ctx)
 int ipcgpu_timer_stop(ipcgpu_ctx* ctx, double* ms)
 {
     REQUIRE(ctx->timer_a && ms, IPCGPU_ERR_STATE, "ipcgpu_timer_start first");
+    ENTER(kSerial);
     CK(cudaEventRecord(ctx->timer_b, ctx->stream));
     CK(cudaEventSynchronize(ctx->timer_b));
     float f = 0.f;
@@ -1908,9 +2088,15 @@ int ipcgpu_download_range_async(ipcgpu_ctx* ctx, int which, uint64_t offset, uin
         CK(cudaEventCreateWithFlags(&ctx->ev_copy_join, cudaEventDisableTiming));
     }
     if (count == 0) return IPCGPU_OK;
-    // everything enqueued so far produces the buffer: the copy starts after it and runs next to whatever follows on the main stream
+    // everything enqueued so far, on the main stream and on an open derivative stream, produces the buffer: the copy starts after it and
+    // runs next to whatever follows on the main stream (this call does not join the derivative chain, see enter())
     CK(cudaEventRecord(ctx->ev_copy_fork, ctx->stream));
     CK(cudaStreamWaitEvent(ctx->copy, ctx->ev_copy_fork, 0));
+    if (ctx->deriv_open) {
+        CK(cudaEventRecord(ctx->ev_deriv_done, ctx->deriv));
+        CK(cudaStreamWaitEvent(ctx->copy, ctx->ev_deriv_done, 0));
+        if (ctx->capturing) ctx->deriv_copied = true;
+    }
     CK(cudaMemcpyAsync(dst_pinned, p + offset, count * sizeof(double), cudaMemcpyDeviceToHost, ctx->copy));
     ctx->copy_pending = true;
     return IPCGPU_OK;
@@ -1926,6 +2112,7 @@ int ipcgpu_download_range(ipcgpu_ctx* ctx, int which, uint64_t offset, uint64_t 
         REQUIRE(bi == 0, IPCGPU_ERR_ARG, "unknown buffer id");
     }
     REQUIRE((dst || count == 0) && offset + count <= n, IPCGPU_ERR_ARG, "download: bad destination or range");
+    ENTER(kSerial);
     if (count) CK(cudaMemcpyAsync(dst, p + offset, count * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return IPCGPU_OK;

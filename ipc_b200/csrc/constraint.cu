@@ -933,7 +933,7 @@ static int build_grids(ipcgpu_ctx* ctx, int nT, int nE, int nV, const int* vmin,
     w.built_vertices = nV;
     if (n <= 0) return 0;
     const size_t nTab = (size_t)3 * kGridCells + 1;
-    cudaMemsetAsync(w.cell_cnt.p, 0, nTab * sizeof(int), st);
+    zero_words(w.cell_cnt.p, nTab, st); // (kernels.h: not a memset)
     k_cell_count<<<nblk(n, 256), 256, 0, st>>>(nT, nE, nV, w.tbox.p, w.ebox.p, w.vbox.p, w.grid.p, w.cell_cnt.p, w.key_tmp.p, w.val_tmp.p);
     size_t bytes = w.cub_tmp.n;
     cudaError_t e = cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, bytes, w.cell_cnt.p, w.cell_off.p, (int)nTab, st);
@@ -944,7 +944,7 @@ static int build_grids(ipcgpu_ctx* ctx, int nT, int nE, int nV, const int* vmin,
     k_cell_scatter<<<nblk(n, 256), 256, 0, st>>>(nT, nE, nV, w.tbox.p, w.ebox.p, w.vbox.p, w.grid.p, w.cell_off.p, w.key_tmp.p, w.val_tmp.p, w.ckeys.p, w.cvals.p,
         reinterpret_cast<uint4*>(w.centries.p), surf_args(ctx), vmin, vmax);
     w.built_voxel_entries = vmin != nullptr;
-    ctx->launches += 4;
+    ctx->launches += 5;
     return 0;
 }
 // views of the combined sorted array: triangles are entries [0, nSF), edges [nSF, nSF + nSE) (positions are absolute in both views)

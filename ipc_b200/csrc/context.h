@@ -101,9 +101,19 @@ struct CcdWork {
 
 struct ipcgpu_ctx {
     int device = 0;
+    // main stream, high priority: everything except the derivative chain, in particular the step-bound chain (the critical path)
     cudaStream_t stream = nullptr;
-    // side stream: the build + projection of the pair Hessians (latency-bound, a fraction of one wave) run next to the elastic assembly;
-    // ev_inputs marks, on the main stream, the last point at which their inputs (positions, contact sets) changed
+    // derivative stream, low priority: the elastic gradient/Hessian, its CSR assembly and the barrier gradient / Hessian scatter of the
+    // device-resident iteration run here next to the step-bound chain (api.cu: enter / join_deriv).  deriv_open: work has been forked
+    // onto it that the main stream has not joined yet; deriv_copied: the capture in progress copies derivative results to the host
+    cudaStream_t deriv = nullptr;
+    cudaEvent_t ev_deriv_fork = nullptr, ev_deriv_done = nullptr;
+    bool deriv_open = false, deriv_copied = false;
+    int prio_low = 0, prio_high = 0; // the device's stream priority range (numerically lower = higher priority)
+    cudaStream_t deriv_stream() const { return deriv_open ? deriv : stream; }
+    // side stream: the build + projection of the pair Hessians (latency-bound, a fraction of one wave) run next to the elastic assembly
+    // and join the stream of the derivative chain before the scatter; ev_inputs marks, on the main stream, the last point at which their
+    // inputs (positions, contact sets) changed
     cudaStream_t side = nullptr;
     // copy stream: ipcgpu_download_range_async forks it off the main stream, so that a result (gradient, CSR values) travels to the host
     // while the later stages of the iteration run; joined by ipcgpu_fetch_iteration / ipcgpu_sync / ipcgpu_capture_end

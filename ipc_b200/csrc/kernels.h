@@ -145,5 +145,9 @@ void step_forward(int nV, const double* x0_soa, const double* p_interleaved, dou
 int inertia_energy_blocks(int nV);
 void inertia_energy(int v0, int v1, int nV, const double* x_soa, const double* xtilde_soa, const double* mass, double* partials, cudaStream_t st);
 void inertia_gradient(int nV, const double* x_soa, const double* xtilde_soa, const double* mass, const uint8_t* dbc, int projectDBC, double* g, cudaStream_t st);
+// zero n_words 4-byte words.  A kernel rather than cudaMemsetAsync where the two chains of an iteration overlap (api.cu): replayed from a
+// graph, a memset node has no priority of its own and queues behind whatever low-priority grids are pending, which held the step-bound
+// chain up for the length of the CSR assembly
+void zero_words(void* p, size_t n_words, cudaStream_t st);
 
 } // namespace ipcgpu

@@ -1,6 +1,7 @@
 // misc.cu -- small per-vertex kernels the Newton driver runs between the hot stages.
 #include "common.cuh"
 #include "kernels.h"
+#include <algorithm>
 
 namespace ipcgpu {
 
@@ -64,6 +65,15 @@ void inertia_energy(int v0, int v1, int nV, const double* x, const double* xt, c
 void inertia_gradient(int nV, const double* x, const double* xt, const double* mass, const uint8_t* dbc, int projectDBC, double* g, cudaStream_t st)
 {
     if (nV > 0) k_inertia_gradient<<<(nV + 255) / 256, 256, 0, st>>>(nV, x, xt, mass, dbc, projectDBC, g);
+}
+
+__global__ void __launch_bounds__(256) k_zero_words(size_t n, unsigned* __restrict__ p)
+{
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = 0u;
+}
+void zero_words(void* p, size_t n_words, cudaStream_t st)
+{
+    if (n_words) k_zero_words<<<(unsigned)std::min<size_t>((n_words + 255) / 256, (size_t)kSMs * 16), 256, 0, st>>>(n_words, static_cast<unsigned*>(p));
 }
 
 } // namespace ipcgpu

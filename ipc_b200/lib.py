@@ -91,6 +91,7 @@ SIGNATURES = {
     "ipcgpu_capture_end": (C.c_int, [_ctxp, _ip]),
     "ipcgpu_graph_launch": (C.c_int, [_ctxp, C.c_int]),
     "ipcgpu_graph_destroy": (C.c_int, [_ctxp, C.c_int]),
+    "ipcgpu_graph_kernel_priorities": (C.c_int, [_ctxp, C.c_int, _ip, _ip]),
     "ipcgpu_csr_set_zero": (C.c_int, [_ctxp]),
     "ipcgpu_solve_pcg": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
     "ipcgpu_allreduce_grad_hess": (C.c_int, [_ctxp, C.c_int, C.c_int]),
@@ -328,6 +329,12 @@ class Context:
 
     def graph_destroy(self, gid):
         self._ck(self.lib.ipcgpu_graph_destroy(self.h, int(gid)))
+
+    def graph_kernel_priorities(self, gid):
+        """(kernel nodes at the high stream priority, kernel nodes at the low one) of a captured graph"""
+        a, b = C.c_int(), C.c_int()
+        self._ck(self.lib.ipcgpu_graph_kernel_priorities(self.h, int(gid), C.byref(a), C.byref(b)))
+        return a.value, b.value
 
     # ---- friction / inertia -------------------------------------------------------------------
     def set_prev_state(self, V_prev_soa=None):
