@@ -317,6 +317,10 @@ int ipcgpu_ccd_stats_timing(ipcgpu_ctx* ctx, uint64_t* longest_pair_cycles, uint
  * depends on scheduling.  toi >= 0 makes every later narrow phase start as if some pair had already reported `toi` (the step on entry,
  * i.e. max_t of every pair, is unchanged; the result is min(toi, the pairs' impacts)); toi < 0 switches the hook off. */
 int ipcgpu_ccd_debug_seed_bound(ipcgpu_ctx* ctx, double toi);
+/* TEST HOOK.  boxes >= 0: a thread may evaluate this many boxes of a search in the thread-level pass before it hands the pair on to the
+ * warp-level pass, in every later narrow phase of this context (0 hands on every search that does not end at its root box); boxes < 0
+ * restores the default (IPCGPU_TI_BUDGET, else 32).  The step bound does not depend on it. */
+int ipcgpu_ccd_debug_thread_budget(ipcgpu_ctx* ctx, int64_t boxes);
 
 /* ---- linear-solve hand-off with the Hessian resident in HBM (LinSysSolver::factorize/solve, LinSysSolver.hpp:230-236; Optimizer.cpp:2324-2355) ----
  * The production binding is a sparse Cholesky on the device arrays (cuDSS: INTEGRATION.md; ipcgpu_device_ptr / the ia, ja uploaded by

@@ -1037,6 +1037,12 @@ int ipcgpu_ccd_debug_seed_bound(ipcgpu_ctx* ctx, double toi)
     return IPCGPU_OK;
 }
 
+int ipcgpu_ccd_debug_thread_budget(ipcgpu_ctx* ctx, int64_t boxes)
+{
+    ctx->debug_ti_budget = boxes;
+    return IPCGPU_OK;
+}
+
 int ipcgpu_ccd_partial_ti(ipcgpu_ctx* ctx, const double* p, double tol, const double err_vf[3], const double err_ee[3], double* alpha_inout)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");

@@ -1007,319 +1007,7 @@ __device__ int pair_ccd(bool vf, const TiPair& P, const NarrowArgs& a, DBox* buf
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// group pass: EIGHT LANES per surviving pair (four pairs per warp).  A lane is one corner of the parameter box being evaluated, the
-// co-domain interval of a coordinate is a 3-step shuffle min/max inside the group -- the same corner-parallel evaluation as the narrow
-// levels of the warp-level pass, with the same arithmetic per corner, hence the same decisions and the same time of impact.  What
-// changes is the concurrency: the interval search is a chain of short dependent steps (evaluate a level, pick K1/K2, split), and one
-// warp per pair left three quarters of its lanes idle on the 1-4 box levels that make up almost every search, at 24 pairs in flight
-// per SM.  Four pairs per warp quadruple the searches in flight for the same registers and shared memory.  Levels are walked one box
-// at a time per group; the split pass handles eight boxes per round.  A pair whose level outgrows the group's buffer (kGrpCap boxes)
-// is handed to the warp-level pass, which restarts it.
-// ------------------------------------------------------------------------------------------------------------------
-constexpr int kGrpCap = 44;       // boxes per level buffer per group (two buffers per group: 4 x 2 x 44 x 32 B = 11.3 KB per warp; static smem stays < 48 KB)
-constexpr int kGrpWarpsPerCta = 4;
-
-__device__ int ti_root_finder_grp(bool vf, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err, double ms, int max_itr, DBox* sA, DBox* sB,
-    int gl, unsigned gmask, double& toi, double& out_tol, int* __restrict__ warn, const unsigned long long* best)
-{
-    const bool check_t = (max_t != 1.0);
-    const double INF = __longlong_as_double(0x7ff0000000000000ll);
-    const int ci = gl >> 2, cj = (gl >> 1) & 1, cl = gl & 1;
-    DBox* cur = sA;
-    DBox* nxt = sB;
-    if (gl == 0) cur[0] = DBox{ 0ull, 0ull, 0ull, 0u, 0u };
-    __syncwarp(gmask);
-    int n = 1;
-    double toi_skip = INF;
-    bool use_skip = false;
-    long long refine = 0;
-    double temp_toi = INF, temp_out_tol = co_tol;
-    out_tol = co_tol;
-    toi = INF;
-    unsigned long long bo_cur = best ? *reinterpret_cast<const volatile unsigned long long*>(best) : 0ull;
-    while (n > 0) {
-        Key3 k1 = { INF, INF, INF }, k2 = { INF, INF, INF };
-        unsigned p1 = 0, p2 = 0;
-        double a1max = 0.0;
-        int visited = 0;
-        // exact pruning against the running device-wide minimum (see ti_root_finder); the value used here was requested one level ago
-        double t_prune = INF;
-        if (best) {
-            t_prune = fmax(ord_to_dbl(bo_cur), 1e-6);
-            bo_cur = *reinterpret_cast<const volatile unsigned long long*>(best);
-        }
-        for (int bI = 0; bI < n; ++bI) { // one box at a time, its 8 corners on the 8 lanes (every branch below is uniform over the group)
-            const DBox b = cur[bI];
-            const int tk = b.kk & 0xff, uk = (b.kk >> 8) & 0xff, vk = (b.kk >> 16) & 0xff;
-            const double tlo = dy_lo(b.tn, tk);
-            unsigned flags = 0;
-            if (tlo < toi_skip && tlo < t_prune) {
-                ++visited;
-                const double tv = ci ? dy_hi(b.tn, tk) : tlo;
-                const double uv = cj ? dy_hi(b.un, uk) : dy_lo(b.un, uk);
-                const double vv = cl ? dy_hi(b.vn, vk) : dy_lo(b.vn, vk);
-                bool excl = false, inside = true, tolc = true;
-                double tmax = 0.0;
-#pragma unroll
-                for (int cc = 0; cc < 3; ++cc) {
-                    double pp[4];
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) pp[k] = (P.x1[3 * k + cc] - P.x0[3 * k + cc]) * tv + P.x0[3 * k + cc];
-                    double f;
-                    if (vf) {
-                        const double pt = ((pp[2] - pp[1]) * uv + (pp[3] - pp[1]) * vv) + pp[1];
-                        f = pp[0] - pt;
-                    }
-                    else {
-                        const double pa = (pp[1] - pp[0]) * uv + pp[0];
-                        const double pb = (pp[3] - pp[2]) * vv + pp[2];
-                        f = pa - pb;
-                    }
-                    double mn = f, mx = f;
-#pragma unroll
-                    for (int o = 1; o < 8; o <<= 1) {
-                        mn = fmin(mn, __shfl_xor_sync(gmask, mn, o, 8));
-                        mx = fmax(mx, __shfl_xor_sync(gmask, mx, o, 8));
-                    }
-                    const double e = err[cc] + ms;
-                    const double tt = mx - mn;
-                    excl = excl || (mn > e || mx < -e);
-                    inside = inside && (mn >= -e && mx <= e);
-                    tolc = tolc && !(tt > co_tol);
-                    tmax = (cc == 0) ? tt : fmax(tmax, tt);
-                }
-                if (!excl) { // the co-domain box contains the origin
-                    flags = F_ZERO;
-                    const bool cond1 = pow2neg(tk) <= tol[0] && pow2neg(uk) <= tol[1] && pow2neg(vk) <= tol[2];
-                    const Key3 key = { tlo, dy_lo(b.un, uk), dy_lo(b.vn, vk) };
-                    const bool flagged = tolc || inside || cond1;
-                    if (key_less(key, k1)) { k1 = key; p1 = flagged ? 1u : 0u; a1max = tmax; }
-                    if (flagged && key_less(key, k2)) { k2 = key; p2 = cond1 ? 1u : 0u; }
-                }
-            }
-            if (gl == 0) cur[bI].kk = (b.kk & 0x00ffffffu) | flags;
-        }
-        __syncwarp(gmask);
-        if (k1.t == INF) break; // search space exhausted
-        if (p1 & 1u) { toi = k1.t; return 1; }
-        const bool has_k2 = k2.t != INF;
-        if (has_k2 && (p2 & 1u)) { toi = k2.t; return 1; }
-        if (gl == 0) atomicAdd(reinterpret_cast<unsigned long long*>(warn + 5), (unsigned long long)visited); // diagnostics: boxes of this pass
-        if (max_itr > 0) {
-            temp_toi = k1.t;
-            temp_out_tol = fmax(a1max, co_tol);
-            refine += visited;
-            if (refine > max_itr) {
-                if (gl == 0) atomicAdd(warn, 1);
-                toi = temp_toi;
-                out_tol = temp_out_tol;
-                return 1;
-            }
-        }
-        if (has_k2) {
-            if (k2.t < toi_skip) toi_skip = k2.t;
-            use_skip = true;
-        }
-        int nn = 0;
-        bool over = false, deep = false;
-        for (int base = 0; base < n; base += 8) { // split pass: one box per lane of the group
-            const int i = base + gl;
-            int nchild = 0;
-            DBox c0, c1;
-            if (i < n) {
-                const DBox b = cur[i];
-                if (b.kk & F_ZERO) {
-                    const int tk = b.kk & 0xff, uk = (b.kk >> 8) & 0xff, vk = (b.kk >> 16) & 0xff;
-                    const Key3 key = { dy_lo(b.tn, tk), dy_lo(b.un, uk), dy_lo(b.vn, vk) };
-                    if (!has_k2 || key_less(key, k2)) {
-                        const double w[3] = { pow2neg(tk), pow2neg(uk), pow2neg(vk) };
-                        int split = -1;
-                        double bestr = -1.0;
-#pragma unroll
-                        for (int d = 0; d < 3; ++d)
-                            if (w[d] > tol[d]) {
-                                const double r = inv_tol[d] * w[d]; // = w[d] / tol[d] bit for bit: w[d] is a power of two (see ti_ccd)
-                                if (r > bestr) { bestr = r; split = d; }
-                            }
-                        const int pk = split == 0 ? tk : (split == 1 ? uk : vk);
-                        if (split < 0 || pk >= 60) deep = true;
-                        else {
-                            const unsigned long long pn = split == 0 ? b.tn : (split == 1 ? b.un : b.vn);
-#pragma unroll
-                            for (int half = 0; half < 2; ++half) {
-                                const unsigned long long hn = 2 * pn + half;
-                                const int hk = pk + 1;
-                                bool keep = true;
-                                if (split == 0) { if (check_t) keep = !(dy_hi(hn, hk) < 0.0 || dy_lo(hn, hk) > max_t); }
-                                else if (vf) keep = (split == 1) ? sum_le_1(hn, hk, b.vn, vk) : sum_le_1(hn, hk, b.un, uk);
-                                if (keep) {
-                                    DBox ch = b;
-                                    ch.kk &= 0x00ffffffu;
-                                    if (split == 0) { ch.tn = hn; ch.kk = (ch.kk & ~0xffu) | (unsigned)hk; }
-                                    else if (split == 1) { ch.un = hn; ch.kk = (ch.kk & ~0xff00u) | ((unsigned)hk << 8); }
-                                    else { ch.vn = hn; ch.kk = (ch.kk & ~0xff0000u) | ((unsigned)hk << 16); }
-                                    if (nchild == 0) c0 = ch;
-                                    else c1 = ch;
-                                    ++nchild;
-                                }
-                            }
-                        }
-                    }
-                }
-            }
-            int incl = nchild; // inclusive scan over the 8 lanes of the group
-#pragma unroll
-            for (int o = 1; o < 8; o <<= 1) {
-                const int y = __shfl_up_sync(gmask, incl, o, 8);
-                if (gl >= o) incl += y;
-            }
-            const int total = __shfl_sync(gmask, incl, 7, 8);
-            const int off = nn + incl - nchild;
-            if (nn + total > kGrpCap) over = true;
-            else {
-                if (nchild > 0) nxt[off] = c0;
-                if (nchild > 1) nxt[off + 1] = c1;
-            }
-            nn += total;
-            if (__any_sync(gmask, over || deep)) break;
-        }
-        if (__any_sync(gmask, deep)) { // bisection depth exhausted: the conservative per-level estimate, like the other passes
-            if (gl == 0) atomicAdd(warn, 1);
-            toi = temp_toi;
-            out_tol = temp_out_tol;
-            return 1;
-        }
-        if (__any_sync(gmask, over)) return 2; // the level outgrew the group's buffer: hand the pair to the warp-level pass
-        __syncwarp(gmask);
-        DBox* tsw = cur; cur = nxt; nxt = tsw;
-        n = nn;
-    }
-    if (use_skip) { toi = toi_skip; return 1; }
-    return 0;
-}
-
-// vertexFaceCCD_double / edgeEdgeCCD_double incl. the no_zero_toi refinement loop, for one 8-lane group; 0 / 1 / 2 (deferred)
-__device__ int ti_ccd_grp(bool vf, const TiPair& P, const double* err, double ms, double tolerance, double t_max, int max_itr, DBox* sA, DBox* sB, int gl, unsigned gmask,
-    double& toi, int* __restrict__ warn, const unsigned long long* best)
-{
-    double tolerance_in = tolerance, ms_in = ms, out_tol = tolerance;
-    bool is_impacting = false, tmp = false;
-    unsigned iter = 0;
-    do {
-        double tol[3];
-        width_tolerances(vf, P, tolerance_in, tol);
-        double inv_tol[3];
-        for (int d = 0; d < 3; ++d) inv_tol[d] = 1.0 / tol[d];
-        const int rc = ti_root_finder_grp(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, sA, sB, gl, gmask, toi, out_tol, warn, best);
-        if (rc == 2) return 2;
-        tmp = rc == 1;
-        if (iter == 0) is_impacting = tmp;
-        else toi = tmp ? toi : t_max;
-        if (tmp && toi == 0.0) {
-            if (out_tol > tolerance_in) t_max *= 0.9;
-            else if (10 * tolerance_in < ms_in) ms_in *= 0.5;
-            else tolerance_in *= 0.1;
-        }
-        ++iter;
-    } while (iter < 0x7fffffffu && tmp && toi == 0.0);
-    return is_impacting ? 1 : 0;
-}
-
-__global__ void __launch_bounds__(32 * kGrpWarpsPerCta, 4) k_ti_groups(NarrowArgs a, const unsigned* __restrict__ survivors, const unsigned* __restrict__ nSurvPtr,
-    unsigned* __restrict__ work, unsigned* __restrict__ deferred, unsigned* __restrict__ nDeferred, unsigned long long* __restrict__ min_ord, int* __restrict__ warn)
-{
-    __shared__ DBox sLevels[kGrpWarpsPerCta][4][2][kGrpCap];
-    __shared__ TiPair sPair[kGrpWarpsPerCta][4];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const int grp = lane >> 3, gl = lane & 7;
-    const unsigned gmask = 0xffu << (8 * grp);
-    DBox* sA = sLevels[wib][grp][0];
-    DBox* sB = sLevels[wib][grp][1];
-    TiPair& Ps = sPair[wib][grp];
-    const unsigned nSurv = *nSurvPtr;
-    const double max_t = a.st->max_t;
-    const unsigned long long* best = &a.st->ccd_ord;
-    for (;;) {
-        unsigned w = 0;
-        if (gl == 0) w = atomicAdd(work, 1u);
-        w = __shfl_sync(gmask, w, 0, 8);
-        if (w >= nSurv) break;
-        const unsigned idx = survivors[w];
-        bool vf;
-        {
-            int v[4];
-            TiPair Pl;
-            load_pair(a.s, a.dir, a.cand[idx], vf, v, Pl);
-            if (gl == 0) Ps = Pl;
-            __syncwarp(gmask);
-        }
-        const TiPair& P = Ps;
-        const double d = pair_distance_sqrt(vf, P);
-        const double ms = fmin(0.2 * d, 1e-6);
-        const double* err = vf_metric(vf, P) ? a.err_vf : a.err_ee;
-        double toi;
-        int hit = ti_ccd_grp(vf, P, err, ms, a.tol, max_t, a.max_itr, sA, sB, gl, gmask, toi, warn, best);
-        if (hit == 1 && toi < 1e-6) { // :759-781 (no pruning here: the result is rescaled by 0.8, see pair_ccd)
-            hit = ti_ccd_grp(vf, P, err, 0.0, a.tol, max_t, a.max_itr, sA, sB, gl, gmask, toi, warn, nullptr);
-            if (hit == 1) toi *= 0.8;
-        }
-        if (gl == 0) {
-            if (hit == 2) deferred[atomicAdd(nDeferred, 1u)] = idx;
-            else if (hit == 1) atomicMin(min_ord, dbl_to_ord(toi));
-        }
-        __syncwarp(gmask);
-    }
-}
-
-// stage 1.5: one THREAD per surviving pair with a small private level buffer; pairs whose search outgrows it are deferred
-constexpr int kThreadCap = 12;
-template <int CAP, int OCC, bool SMEM = false>
-__global__ void __launch_bounds__(128, OCC) k_ti_stage15(NarrowArgs a, const unsigned* __restrict__ survivors, const unsigned* __restrict__ nSurvPtr,
-    unsigned* __restrict__ deferred, unsigned* __restrict__ nDeferred, long long budget, unsigned long long* __restrict__ min_ord, int* __restrict__ warn)
-{
-    const unsigned nSurv = *nSurvPtr;
-    const unsigned stride = gridDim.x * blockDim.x;
-    // grid-stride over whole warps so that the warp-aggregated append below always has all 32 lanes present
-    for (unsigned base = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); base < nSurv; base += stride) {
-        const unsigned i = base + (threadIdx.x & 31);
-        bool defer = false;
-        unsigned idx = 0;
-        if (i < nSurv) {
-            idx = survivors[i];
-            bool vf;
-            int v[4];
-            TiPair P;
-            load_pair(a.s, a.dir, a.cand[idx], vf, v, P);
-            // level buffers: in LOCAL memory they cost ~20 % of this kernel's stall samples (ncu source view: the flag test and the
-            // integer->double conversions right behind the box loads; 100 KB of stack per CTA thrashes the L1).  SMEM = true keeps them in
-            // shared memory, one padded slab per thread ((CAP * 32 + 8)-byte stride: the lanes' 64-bit words fall into distinct bank pairs).
-            DBox lA[SMEM ? 1 : CAP], lB[SMEM ? 1 : CAP];
-            DBox* bufA = lA;
-            DBox* bufB = lB;
-            if (SMEM) {
-                extern __shared__ __align__(16) unsigned char s_lvl[];
-                constexpr int kSlab = CAP * (int)sizeof(DBox) + 8;
-                bufA = reinterpret_cast<DBox*>(s_lvl + (size_t)threadIdx.x * kSlab);
-                bufB = reinterpret_cast<DBox*>(s_lvl + (size_t)(blockDim.x + threadIdx.x) * kSlab);
-            }
-            double toi;
-            const int hit = pair_ccd<1>(vf, P, a, bufA, bufB, CAP, 0, toi, warn, nullptr, nullptr, budget);
-            if (hit == 2) defer = true;
-            else if (hit == 1) atomicMin(min_ord, dbl_to_ord(toi));
-        }
-        const unsigned m = __ballot_sync(0xffffffffu, defer);
-        if (m) {
-            const int lane = threadIdx.x & 31;
-            unsigned b0 = 0;
-            if (lane == __ffs(m) - 1) b0 = atomicAdd(nDeferred, __popc(m));
-            b0 = __shfl_sync(0xffffffffu, b0, __ffs(m) - 1);
-            if (defer) deferred[b0 + __popc(m & ((1u << lane) - 1))] = idx;
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Thread pass with LANE-LEVEL REFILL (round 2, second half).  ncu on k_ti_stage15: 7.4 of 32 lanes active per issued instruction -- a lane whose
+// Thread pass with LANE-LEVEL REFILL (round 2, second half).  With one pair per lane and grid-stride round, ncu showed 7.4 of 32 lanes active per issued instruction -- a lane whose
 // search ended after two boxes waited for the lane of its warp that used its whole 24-box budget.  Here the search is a resumable state
 // machine: one loop iteration = ONE LEVEL of one lane's breadth-first search (the body of ti_root_finder's level loop, same arithmetic, same
 // decisions); a lane whose pair is finished takes the next survivor from a work counter in the same iteration.  The no_zero_toi loop of
@@ -1557,7 +1245,7 @@ __global__ void __launch_bounds__(128, 2) k_ti_stage15_refill(NarrowArgs a, cons
     }
 }
 
-__global__ void __launch_bounds__(128, 3) k_ti_stage2(NarrowArgs a, const unsigned* __restrict__ survivors, const unsigned* __restrict__ nSurvPtr, unsigned* __restrict__ work,
+__global__ void __launch_bounds__(128, 2) k_ti_stage2(NarrowArgs a, const unsigned* __restrict__ survivors, const unsigned* __restrict__ nSurvPtr, unsigned* __restrict__ work,
     DBox* __restrict__ scratch, int cap, unsigned long long* __restrict__ min_ord, int* __restrict__ warn)
 {
     __shared__ DBox sLevels[kStage2WarpsPerCtaDev][2][kSmemLevel];
@@ -1668,18 +1356,11 @@ void cell_pairs_pt(const ipcgpu::Grid* gp, const ipcgpu::SortedGrid& vg, const i
     const ipcgpu::IterState* vox, int first, int last, const ipcgpu::PairOut& out, cudaStream_t st);
 SortedGrid vertex_grid(const ipcgpu_ctx* ctx);
 
-static bool refill_mode() // thread pass with lane-level refill (IPCGPU_TI_REFILL=0: one pair per lane and grid-stride round)
-{
-    static const bool v = [] { const char* e = std::getenv("IPCGPU_TI_REFILL"); return e ? std::atoi(e) != 0 : true; }();
-    return v;
-}
-static bool lvl_smem() // level buffers of the thread pass in shared memory (IPCGPU_TI_LVL_SMEM=0: thread-local memory)
-{
-    static const bool v = [] { const char* e = std::getenv("IPCGPU_TI_LVL_SMEM"); return e ? std::atoi(e) != 0 : true; }();
-    return v;
-}
 constexpr int kStage2WarpsPerCta = 4;
-constexpr int kStage2Ctas = kSMs * 6;// persistent: 6 CTAs x 4 warps per SM
+// persistent: 2 CTAs x 4 warps per SM, compiled for 2 CTAs per SM (230 registers, no spill; for 3 per SM it spilled 226 B per thread).  Fewer
+// warps of this pass per SM leave room for the derivative chain that runs next to it (H100 SXM, 700 W, C5, iteration ms with budget 32:
+// 1 CTA per SM 3.19, 2 -> 3.15, 3 -> 3.16; 6 CTAs of the 3-per-SM build 3.21)
+constexpr int kStage2Ctas = kSMs * 2;
 constexpr int kLevelCap = 4096;      // boxes per BFS level buffer (2 buffers per warp)
 
 int ccd_alloc(ipcgpu_ctx* ctx)
@@ -1718,7 +1399,7 @@ int ccd_narrow(ipcgpu_ctx* ctx, const int2* cand, const int* n32, const unsigned
     IterState* ist = ctx->iter.p;
     unsigned* nSurv = reinterpret_cast<unsigned*>(w.counters.p);
     unsigned* work = nSurv + 1;
-    int* flags = w.counters.p + 2; // [0] zero distance, [1] warnings, [2] deferred, [4] longest, [5] total cycles, [6..7] / [8..9] boxes
+    int* flags = w.counters.p + 2; // [0] zero distance, [1] warnings, [2] deferred, [3] pass A's work counter, [4] longest, [5] total cycles, [6..7] / [8..9] boxes
     static const int wide_env = [] { const char* e = std::getenv("IPCGPU_TI_WIDE_LEVEL"); return e ? std::atoi(e) : 0; }();
     if (wide_env > 0 && !w.wide_level_set) {
         CKD(cudaMemcpyToSymbolAsync(c_wide_level, &wide_env, sizeof(int), 0, cudaMemcpyHostToDevice, st));
@@ -1729,70 +1410,29 @@ int ccd_narrow(ipcgpu_ctx* ctx, const int2* cand, const int* n32, const unsigned
     {
         // the candidate count lives on the device: every pass is a grid-stride / persistent kernel that reads it there
         // pass 1 (thread per candidate): the root box only;
-        // pass A (thread per survivor, 10-box budget): the shallow majority dies here without holding its warp hostage;
+        // pass A (thread per survivor, box budget): the shallow majority dies here without holding its warp hostage;
         // pass B (warp per pair, corner-parallel box evaluation): the deep searches, compacted.
-        // (a three-tier split -- 3-box, then 12-box thread passes -- was measured slower: the per-pair set-up dominates pass A)
+        // (measured slower or wrong, and deleted: a three-tier split -- 3-box, then 12-box thread passes; an 8-lanes-per-pair group pass between
+        // A and B, or instead of A; both passes fused into one persistent kernel that starts the deep searches while the thread pass still runs:
+        // DESIGN.md §3.1, §7)
         cudaEvent_t pe1 = ctx->prof_begin(IPCGPU_STAGE_CCD_ROOT_FILTER);
         k_ti_stage1<<<kSMs * 16, 128, 0, st>>>(a, w.surv.p, nSurv, flags);
         ctx->prof_end(pe1);
         unsigned* nDefA = reinterpret_cast<unsigned*>(flags + 2);
-        // pass A (thread per survivor, 24-box budget): the shallow majority (2-3 boxes) at 32 pairs per warp;
-        // pass G (8 lanes per pair, 4 pairs per warp): the searches pass A gave up on, unless a level outgrows the group's 44-box buffer;
-        // pass B (warp per pair): those wide searches.  IPCGPU_TI_MODE: 0 = A + B (default), 1 = G + B, 2 = A + G + B, 3 = A + A(48-box levels) + B.
-        // Narrow phase per iteration (H100 SXM, 400 W, C5): A + B 1.03 ms, G + B 2.34 ms -- the four groups of a warp diverge and the hardware runs
-        // divergent paths of one warp one after the other, so pass G buys no latency hiding (kept for the record).  A + G + B ran in 0.80 ms
-        // but returned a different, larger step bound than every other mode and the oracle (0.377 instead of 0.133): not a usable mode.
-        static const int ti_mode = [] { const char* e = std::getenv("IPCGPU_TI_MODE"); return e ? std::atoi(e) : 0; }();
-        unsigned* grp_work = reinterpret_cast<unsigned*>(flags + 3);
-        unsigned* nDefB = reinterpret_cast<unsigned*>(flags + 10);
-        if (ti_mode == 1) {
-            k_ti_groups<<<kSMs * 4, 32 * kGrpWarpsPerCta, 0, st>>>(a, w.surv.p, nSurv, grp_work, w.surv2.p, nDefA, &ist->ccd_ord, flags + 1);
-            k_ti_stage2<<<kStage2Ctas, 32 * kStage2WarpsPerCta, 0, st>>>(a, w.surv2.p, nDefA, work, reinterpret_cast<DBox*>(w.scratch.p), kLevelCap, &ist->ccd_ord, flags + 1);
-        }
-        else {
-            static const long long budgetA = [] { const char* e = std::getenv("IPCGPU_TI_BUDGET"); return e ? std::atoll(e) : 24ll; }(); // boxes a thread may evaluate before it hands its pair on
-            // (H100 SXM, 400 W, C5, narrow phase per iteration: 10 -> 1.36 ms, 16 -> 1.11, 24 -> 1.03, 32 -> 1.04, 64 -> 1.09)
-            static const int occA = [] { const char* e = std::getenv("IPCGPU_TI_OCC"); return e ? std::atoi(e) : 2; }(); // CTAs/SM the thread pass is compiled for (2: 255 regs, 3: 168 regs + spills)
-            static const int capA = [] { const char* e = std::getenv("IPCGPU_TI_CAP"); return e ? std::atoi(e) : 8; }(); // boxes per level buffer of the thread pass
-            // (H100 SXM, 400 W, C5, narrow phase per iteration, 8 boxes: refill 1.03 ms; no refill, shared memory 1.04, thread-local memory 1.07)
-            if (occA == 3) k_ti_stage15<kThreadCap, 3><<<kSMs * 16, 128, 0, st>>>(a, w.surv.p, nSurv, w.surv2.p, nDefA, budgetA, &ist->ccd_ord, flags + 1);
-            else if (refill_mode()) {
-                constexpr int bytes = 2 * 128 * (8 * (int)sizeof(DBox) + 8);
-                static bool attr = false;
-                if (!attr) { cudaFuncSetAttribute(k_ti_stage15_refill<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); attr = true; }
-                static const int batch = [] { const char* e = std::getenv("IPCGPU_TI_REFILL_BATCH"); return e ? std::atoi(e) : 16; }(); // (H100 SXM, 400 W, C5: batch 1 / 8 / 16 / 32 -> 1.06 / 1.05 / 1.03 / 1.03 ms)
-                k_ti_stage15_refill<8><<<kSMs * 2, 128, bytes, st>>>(a, w.surv.p, nSurv, grp_work, w.surv2.p, nDefA, budgetA, &ist->ccd_ord, flags + 1, batch);
-            }
-            else if (lvl_smem() && capA == 8) {
-                constexpr int bytes = 2 * 128 * (8 * (int)sizeof(DBox) + 8);
-                static bool attr = false;
-                if (!attr) { cudaFuncSetAttribute(k_ti_stage15<8, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); attr = true; }
-                k_ti_stage15<8, 2, true><<<kSMs * 16, 128, bytes, st>>>(a, w.surv.p, nSurv, w.surv2.p, nDefA, budgetA, &ist->ccd_ord, flags + 1);
-            }
-            else if (lvl_smem() && capA == kThreadCap) {
-                constexpr int bytes = 2 * 128 * (kThreadCap * (int)sizeof(DBox) + 8);
-                static bool attr = false;
-                if (!attr) { cudaFuncSetAttribute(k_ti_stage15<kThreadCap, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); attr = true; }
-                k_ti_stage15<kThreadCap, 2, true><<<kSMs * 16, 128, bytes, st>>>(a, w.surv.p, nSurv, w.surv2.p, nDefA, budgetA, &ist->ccd_ord, flags + 1);
-            }
-            else if (capA == 8) k_ti_stage15<8, 2><<<kSMs * 16, 128, 0, st>>>(a, w.surv.p, nSurv, w.surv2.p, nDefA, budgetA, &ist->ccd_ord, flags + 1);
-            else if (capA == 6) k_ti_stage15<6, 2><<<kSMs * 16, 128, 0, st>>>(a, w.surv.p, nSurv, w.surv2.p, nDefA, budgetA, &ist->ccd_ord, flags + 1);
-            else if (capA == 16) k_ti_stage15<16, 2><<<kSMs * 16, 128, 0, st>>>(a, w.surv.p, nSurv, w.surv2.p, nDefA, budgetA, &ist->ccd_ord, flags + 1);
-            else k_ti_stage15<kThreadCap, 2><<<kSMs * 16, 128, 0, st>>>(a, w.surv.p, nSurv, w.surv2.p, nDefA, budgetA, &ist->ccd_ord, flags + 1);
-            if (ti_mode == 2) { // the survivor list is dead after pass A: pass G's own deferrals go there
-                k_ti_groups<<<kSMs * 4, 32 * kGrpWarpsPerCta, 0, st>>>(a, w.surv2.p, nDefA, grp_work, w.surv.p, nDefB, &ist->ccd_ord, flags + 1);
-                k_ti_stage2<<<kStage2Ctas, 32 * kStage2WarpsPerCta, 0, st>>>(a, w.surv.p, nDefB, work, reinterpret_cast<DBox*>(w.scratch.p), kLevelCap, &ist->ccd_ord, flags + 1);
-                ++ctx->launches;
-            }
-            else if (ti_mode == 3) { // second thread pass over the compacted deferrals: 48-box levels in local memory, 256-box budget
-                static const long long budgetA2 = [] { const char* e = std::getenv("IPCGPU_TI_BUDGET2"); return e ? std::atoll(e) : 256ll; }();
-                k_ti_stage15<48, 2><<<kSMs * 8, 128, 0, st>>>(a, w.surv2.p, nDefA, w.surv.p, nDefB, budgetA2, &ist->ccd_ord, flags + 1);
-                k_ti_stage2<<<kStage2Ctas, 32 * kStage2WarpsPerCta, 0, st>>>(a, w.surv.p, nDefB, work, reinterpret_cast<DBox*>(w.scratch.p), kLevelCap, &ist->ccd_ord, flags + 1);
-                ++ctx->launches;
-            }
-            else
-                k_ti_stage2<<<kStage2Ctas, 32 * kStage2WarpsPerCta, 0, st>>>(a, w.surv2.p, nDefA, work, reinterpret_cast<DBox*>(w.scratch.p), kLevelCap, &ist->ccd_ord, flags + 1);
-        }
+        unsigned* refill_work = reinterpret_cast<unsigned*>(flags + 3);
+        // pass A (thread per survivor): the shallow majority (2-3 boxes) at 32 pairs per warp; pass B (warp per pair): the searches pass A hands on.
+        // boxes a thread may evaluate before it hands its pair on (H100 SXM, 700 W, C5, iteration ms with the warp pass above: 24 -> 3.26 (2,871 pairs
+        // handed on in the full CCD), 32 -> 3.15 (950), 40 -> 3.14, 64 -> 3.16; the narrow phase alone barely moves, the iteration gains because
+        // the shorter warp pass leaves the SMs to the derivative chain sooner)
+        static const long long budget_env = [] { const char* e = std::getenv("IPCGPU_TI_BUDGET"); return e ? std::atoll(e) : 32ll; }();
+        const long long budget = ctx->debug_ti_budget >= 0 ? ctx->debug_ti_budget : budget_env;
+        constexpr int bytes = 2 * 128 * (8 * (int)sizeof(DBox) + 8);
+        static bool attr = false;
+        if (!attr) { CKD(cudaFuncSetAttribute(k_ti_stage15_refill<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); attr = true; }
+        // idle lanes of a warp refill together once this many are idle (H100 SXM, 400 W, C5: batch 1 / 8 / 16 / 32 -> 1.06 / 1.05 / 1.03 / 1.03 ms)
+        static const int batch = [] { const char* e = std::getenv("IPCGPU_TI_REFILL_BATCH"); return e ? std::atoi(e) : 16; }();
+        k_ti_stage15_refill<8><<<kSMs * 2, 128, bytes, st>>>(a, w.surv.p, nSurv, refill_work, w.surv2.p, nDefA, budget, &ist->ccd_ord, flags + 1, batch);
+        k_ti_stage2<<<kStage2Ctas, 32 * kStage2WarpsPerCta, 0, st>>>(a, w.surv2.p, nDefA, work, reinterpret_cast<DBox*>(w.scratch.p), kLevelCap, &ist->ccd_ord, flags + 1);
     }
     k_ccd_finish<<<1, 32, 0, st>>>(ist, nSurv, flags, overflow, stage == 3);
     ctx->prof_end(pe);

@@ -173,6 +173,7 @@ struct ipcgpu_ctx {
     size_t ccd_capacity = (size_t)1 << 23; // candidate pairs
     std::vector<int> h_SVI;                // host copy (pSize of the swept build is a serial host sum, SpatialHash.hpp:603-612)
     double debug_prune_seed = -1.0;        // test hook, see ipcgpu_ccd_debug_seed_bound
+    long long debug_ti_budget = -1;        // test hook, see ipcgpu_ccd_debug_thread_budget
 
     // gradient gather map (local tets)
     ipcgpu::DevBuf<int> inc_ptr, inc;

@@ -38,6 +38,7 @@ SIGNATURES = {
     "ipcgpu_intersection_free": (C.c_int, [_ctxp, _ip]),
     "ipcgpu_constraint_set_sizes": (C.c_int, [_ctxp, _ip, _ip, _ip]),
     "ipcgpu_ccd_debug_seed_bound": (C.c_int, [_ctxp, C.c_double]),
+    "ipcgpu_ccd_debug_thread_budget": (C.c_int, [_ctxp, C.c_int64]),
     "ipcgpu_download_range": (C.c_int, [_ctxp, C.c_int, C.c_uint64, C.c_uint64, _dp]),
     "ipcgpu_download_range_async": (C.c_int, [_ctxp, C.c_int, C.c_uint64, C.c_uint64, _dp]),
     "ipcgpu_set_mesh": (C.c_int, [_ctxp, C.c_int, C.c_int, _dp, _ip, _dp, _dp, _dp, _dp, _dp, _u8p, C.c_int]),
@@ -302,6 +303,9 @@ class Context:
 
     def ccd_debug_seed_bound(self, toi):
         self._ck(self.lib.ipcgpu_ccd_debug_seed_bound(self.h, float(toi)))
+
+    def ccd_debug_thread_budget(self, boxes):
+        self._ck(self.lib.ipcgpu_ccd_debug_thread_budget(self.h, int(boxes)))
 
     def constraint_set_sizes(self):
         nC, nP, nK = C.c_int(), C.c_int(), C.c_int()
