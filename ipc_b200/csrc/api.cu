@@ -117,16 +117,16 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 // forms.
 //
 // Why the allowed calls cannot race the derivative chain (written by one side / read or written by the other):
-//   - ContactWork::counters: ccd_full clears and counts words 8-9 (broad-phase pairs); the barrier kernels read words 0 and 2 (list sizes,
-//     written by the constraint set before the fork) and the pair-Hessian build clears and counts word 12.  Separate words, and each
-//     cudaMemsetAsync covers only its own.
+//   - ContactWork::counters: the barrier kernels read words 0 and 2 (list sizes, written by the constraint set before the fork) and the
+//     pair-Hessian build clears and counts word 12; the step-bound chain reads word 3 (partial-CCD candidates).  The step-bound chain
+//     writes no ContactWork buffer.
 //   - IterState: the derivative chain writes energy[0] and flags[FLAG_SET_CAPACITY] / flags[FLAG_PATTERN]; the step-bound chain writes
-//     step_ord, inv_ord, ccd_ord, cand_range, n_full_cand, max_t, alpha_grid, radius, ref_lo, ref_inv_h, alpha_stage, ref_count,
-//     grid_axis_cells, ccd_stats and flags[FLAG_ZERO_CCD_DISTANCE] / [FLAG_CCD_CAPACITY] / [FLAG_TI_WARNINGS].  Aligned words of their own;
-//     nothing clears the struct while `deriv` is open (the fetch clears the flags after joining).
+//     step_ord, inv_ord, ccd_ord, cand_range, n_full_cand, max_t, alpha_grid, ref_lo, ref_inv_h, alpha_stage, ref_count, ccd_stats and
+//     flags[FLAG_ZERO_CCD_DISTANCE] / [FLAG_CCD_CAPACITY] / [FLAG_TI_WARNINGS].  Aligned words of their own; nothing clears the struct
+//     while `deriv` is open (the fetch clears the flags after joining).
 //   - contact lists: the barrier kernels read act / para / para_e (written by the constraint set before the fork); the step-bound chain
-//     reads ContactWork::cand and writes the grid arrays (vbox, ebox, tbox, bounds, grid, cell_cnt, cell_off, key_tmp, val_tmp, ckeys,
-//     cvals, centries, cub_tmp), bp_pairs and the CcdWork buffers, none of which the derivative chain touches.
+//     reads ContactWork::cand and writes only the CcdWork buffers (among them the swept grid: cells, sw_keys, sw_ent, sw_cnt, sw_off,
+//     sw_tmp), which the derivative chain does not touch.
 //   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither.  g, a, gcont, hblk, hcon, e_partials2, scalar_out[0], bHraw, brows,
 //     bpsd: derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };

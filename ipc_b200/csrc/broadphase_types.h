@@ -17,4 +17,10 @@ struct QEntry {
 struct Box {
     double lo[3], hi[3];
 };
+// swept grid of the CCD on the reference voxel lattice (ccd.cu): K x K x K voxels per cell, n cells per axis; lmax / hmax: the longest voxel
+// range of any primitive and the largest voxel index per axis, from which K is chosen on the device
+struct SweptCells {
+    int K, n[3];
+    int lmax, hmax[3];
+};
 } // namespace ipcgpu

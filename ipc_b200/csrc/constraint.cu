@@ -20,12 +20,6 @@ namespace ipcgpu {
 // ------------------------------------------------------------------------------------------------------------
 // boxes + global bounds.  bounds[0..2] = min (flipped order), bounds[3..5] = max, bounds[6] = max extent
 // ------------------------------------------------------------------------------------------------------------
-DEV V3 moved(const SurfArgs& s, const double* __restrict__ dir, double alpha, int v)
-{
-    V3 x = load_vertex(s.V, s.nV, v);
-    if (dir) x = x + alpha * V3{ __ldg(dir + 3 * (size_t)v), __ldg(dir + 3 * (size_t)v + 1), __ldg(dir + 3 * (size_t)v + 2) };
-    return x;
-}
 DEV void grow(Box& b, V3 x)
 {
     b.lo[0] = fmin(b.lo[0], x.x); b.hi[0] = fmax(b.hi[0], x.x);
@@ -39,11 +33,9 @@ DEV Box empty_box()
     return b;
 }
 
-// prim: 0 = surface vertices, 1 = edges, 2 = triangles.  swept: include x + alpha*dir
-__global__ void __launch_bounds__(256) k_boxes(SurfArgs s, int prim, const double* __restrict__ dir, const double* __restrict__ alpha_ptr, Box* __restrict__ boxes,
-    unsigned long long* __restrict__ bounds)
+// prim: 0 = surface vertices, 1 = edges, 2 = triangles
+__global__ void __launch_bounds__(256) k_boxes(SurfArgs s, int prim, Box* __restrict__ boxes, unsigned long long* __restrict__ bounds)
 {
-    const double alpha = alpha_ptr ? *alpha_ptr : 0.0; // sweep length: device resident (IterState::alpha_grid)
     const int n = prim == 0 ? s.nSV : (prim == 1 ? s.nSE : s.nSF);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     Box b = empty_box();
@@ -53,10 +45,7 @@ __global__ void __launch_bounds__(256) k_boxes(SurfArgs s, int prim, const doubl
         if (prim == 0) { v[0] = s.SVI[i]; nv = 1; }
         else if (prim == 1) { v[0] = s.SE[2 * i]; v[1] = s.SE[2 * i + 1]; nv = 2; }
         else { v[0] = s.SF[i]; v[1] = s.SF[(size_t)s.nSF + i]; v[2] = s.SF[(size_t)2 * s.nSF + i]; nv = 3; }
-        for (int k = 0; k < nv; ++k) {
-            grow(b, load_vertex(s.V, s.nV, v[k]));
-            if (dir) grow(b, moved(s, dir, alpha, v[k]));
-        }
+        for (int k = 0; k < nv; ++k) grow(b, load_vertex(s.V, s.nV, v[k]));
         boxes[i] = b;
         ext = fmax(fmax(b.hi[0] - b.lo[0], b.hi[1] - b.lo[1]), b.hi[2] - b.lo[2]);
     }
@@ -93,11 +82,9 @@ __global__ void k_bounds_init(unsigned long long* bounds)
 // grow when the scene would need more: the grid is only an accelerator, any cell size >= the largest inflated box is valid).  The
 // number of cells per axis the scene WANTS goes to the iteration state; the host re-tunes axis_bits from it after every fetch, so that
 // in the steady state the radix sort runs 2 passes (16 key bits) instead of 4.
-__global__ void k_grid_params(const unsigned long long* __restrict__ bounds, double radius_val, const double* __restrict__ radius_ptr, int axis_bits, Grid* __restrict__ g,
-    IterState* __restrict__ st)
+__global__ void k_grid_params(const unsigned long long* __restrict__ bounds, double radius, int axis_bits, Grid* __restrict__ g, IterState* __restrict__ st)
 {
     if (threadIdx.x != 0) return;
-    const double radius = radius_ptr ? *radius_ptr : radius_val;
     double lo[3], hi[3];
     for (int a = 0; a < 3; ++a) { lo[a] = unflip_ord(bounds[a]) - radius; hi[a] = unflip_ord(bounds[3 + a]) + radius; }
     double ext = unflip_ord(bounds[6]);
@@ -147,7 +134,7 @@ __global__ void __launch_bounds__(256) k_cell_count(int nT, int nE, int nV, cons
 }
 __global__ void __launch_bounds__(256) k_cell_scatter(int nT, int nE, int nV, const Box* __restrict__ tboxes, const Box* __restrict__ eboxes, const Box* __restrict__ vboxes,
     const Grid* __restrict__ gp, const int* __restrict__ off, const unsigned* __restrict__ key_of, const int* __restrict__ slot_of, unsigned* __restrict__ keys,
-    int* __restrict__ ids, uint4* __restrict__ sorted, SurfArgs s, const int* __restrict__ vmin, const int* __restrict__ vmax)
+    int* __restrict__ ids, uint4* __restrict__ sorted)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nT + nE + nV) return;
@@ -155,26 +142,7 @@ __global__ void __launch_bounds__(256) k_cell_scatter(int nT, int nE, int nV, co
     const int id = type == 2 ? i - nT - nE : (type == 1 ? i - nT : i);
     const unsigned key = key_of[i];
     const int pos = off[key] + slot_of[i];
-    QBox q;
-    if (vmin) {
-        // swept (CCD) grid: the entry's box IS the primitive's range of REFERENCE voxels (SpatialHash.hpp:642-697: the cells the reference
-        // registers it in), so the overlap test of the pair kernels is exactly the reference's hash-query condition -- not a superset of it
-        int vs[3], nv;
-        if (type == 2) { vs[0] = s.SVI[id]; nv = 1; }
-        else if (type == 1) { vs[0] = s.SE[2 * id]; vs[1] = s.SE[2 * id + 1]; nv = 2; }
-        else { vs[0] = s.SF[id]; vs[1] = s.SF[(size_t)s.nSF + id]; vs[2] = s.SF[(size_t)2 * s.nSF + id]; nv = 3; }
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            int lo = vmin[3 * (size_t)vs[0] + c], hi = vmax[3 * (size_t)vs[0] + c];
-            for (int k = 1; k < nv; ++k) {
-                lo = min(lo, vmin[3 * (size_t)vs[k] + c]);
-                hi = max(hi, vmax[3 * (size_t)vs[k] + c]);
-            }
-            q.lo[c] = min(max(lo, 0), 65535); // (clamping can only widen the overlap: still a superset on absurdly fine grids)
-            q.hi[c] = min(max(hi, 0), 65535);
-        }
-    }
-    else q = quantize_box(*gp, type == 2 ? vboxes[id] : (type == 1 ? eboxes[id] : tboxes[id]));
+    const QBox q = quantize_box(*gp, type == 2 ? vboxes[id] : (type == 1 ? eboxes[id] : tboxes[id]));
     keys[pos] = key;
     ids[pos] = id;
     sorted[pos] = make_uint4((unsigned)q.lo[0] | ((unsigned)q.lo[1] << 16), (unsigned)q.lo[2] | ((unsigned)q.hi[0] << 16), (unsigned)q.hi[1] | ((unsigned)q.hi[2] << 16), (unsigned)id);
@@ -299,8 +267,8 @@ DEV void warp_stage_flush(WarpStage& ws, const PairOut& o, int lane, unsigned th
     if (lane == 0) ws.count = 0;
     __syncwarp();
 }
-__global__ void __launch_bounds__(32 * kCellPairWarps) k_cell_pairs_ee(const Grid* __restrict__ gp, SortedGrid eg, const int* __restrict__ SE, double radius_val,
-    const double* __restrict__ radius_ptr, const IterState* __restrict__ vox, int first, int last, PairOut out)
+__global__ void __launch_bounds__(32 * kCellPairWarps) k_cell_pairs_ee(const Grid* __restrict__ gp, SortedGrid eg, const int* __restrict__ SE, double radius, int first,
+    int last, PairOut out)
 {
     __shared__ WarpStage sStage[kCellPairWarps];
     __shared__ AEntry sA[kCellPairWarps][32];
@@ -310,19 +278,10 @@ __global__ void __launch_bounds__(32 * kCellPairWarps) k_cell_pairs_ee(const Gri
     if (lane == 0) stage.count = 0;
     __syncwarp();
     const Grid g = *gp;
-    // Two kinds of entry boxes (k_cell_scatter): quantised double boxes (static grid: the query is inflated by `radius` in lattice steps) or
-    // ranges of reference voxels (swept grid, vox != nullptr: ranges overlap <=> the reference's hash query pairs the two primitives, no
-    // inflation).  Either way lattice coordinate q maps to accelerator cell floor(q * S + O[axis]).
-    const double radius = radius_ptr ? *radius_ptr : radius_val;
-    const bool voxel = vox != nullptr;
-    const unsigned rq = voxel ? 0u : (unsigned)min((int)ceil(radius * g.q_inv) + 1, 65535);
+    // the query is inflated by `radius` in lattice steps of the quantised entry boxes; lattice coordinate q lies in accelerator cell floor(q * S)
+    const unsigned rq = (unsigned)min((int)ceil(radius * g.q_inv) + 1, 65535);
     const unsigned rq2 = rq | (rq << 16);
-    double S = g.inv_h / g.q_inv, O[3] = { 0.0, 0.0, 0.0 }, padLo = 0.0, padHi = 0.0, bias = 0.0;
-    if (voxel) { // a swept box lies inside its voxel range [vmin, vmax + 1) and is inflated by one voxel: cells of [vmin - 1, vmax + 2)
-        S = g.inv_h / vox->ref_inv_h;
-        O[0] = (vox->ref_lo[0] - g.ox) * g.inv_h; O[1] = (vox->ref_lo[1] - g.oy) * g.inv_h; O[2] = (vox->ref_lo[2] - g.oz) * g.inv_h;
-        padLo = -1.0; padHi = 2.0; bias = 1e-6;
-    }
+    const double S = g.inv_h / g.q_inv;
     const uint4* __restrict__ ent = reinterpret_cast<const uint4*>(eg.ent);
     AEntry* A = sA[wib];
     const int pos = first + (blockIdx.x * kCellPairWarps + wib) * 32 + lane;
@@ -346,9 +305,9 @@ __global__ void __launch_bounds__(32 * kCellPairWarps) k_cell_pairs_ee(const Gri
             a.pad0 = av.x; a.pad1 = av.y;
         }
         A[lane] = a;
-        cl[0] = (int)floor(((double)(a.L01 & 0xffffu) + padLo) * S + O[0] - bias); ch[0] = (int)floor(((double)(a.H01 & 0xffffu) + padHi) * S + O[0] + bias);
-        cl[1] = (int)floor(((double)(a.L01 >> 16) + padLo) * S + O[1] - bias);     ch[1] = (int)floor(((double)(a.H01 >> 16) + padHi) * S + O[1] + bias);
-        cl[2] = (int)floor(((double)a.lo2 + padLo) * S + O[2] - bias);             ch[2] = (int)floor(((double)a.hi2 + padHi) * S + O[2] + bias);
+        cl[0] = (int)floor((double)(a.L01 & 0xffffu) * S); ch[0] = (int)floor((double)(a.H01 & 0xffffu) * S);
+        cl[1] = (int)floor((double)(a.L01 >> 16) * S);     ch[1] = (int)floor((double)(a.H01 >> 16) * S);
+        cl[2] = (int)floor((double)a.lo2 * S);             ch[2] = (int)floor((double)a.hi2 * S);
     }
     __syncwarp();
     unsigned remaining = __ballot_sync(full, valid);
@@ -440,7 +399,7 @@ __global__ void __launch_bounds__(32 * kCellPairWarps) k_cell_pairs_ee(const Gri
 // Rows are walked one after the other (a row of three cells holds about one warp-load of triangles); the first load of the next row is
 // issued before the current row is tested.
 __global__ void __launch_bounds__(32 * kCellPairWarps) k_cell_pairs_pt(const Grid* __restrict__ gp, SortedGrid vg, SortedGrid tg, const int* __restrict__ SVI,
-    const int* __restrict__ SF, int nSF, double radius_val, const double* __restrict__ radius_ptr, const IterState* __restrict__ vox, int first, int last, PairOut out)
+    const int* __restrict__ SF, int nSF, double radius, int first, int last, PairOut out)
 {
     __shared__ WarpStage sStage[kCellPairWarps];
     __shared__ AEntry sA[kCellPairWarps][32];
@@ -450,19 +409,10 @@ __global__ void __launch_bounds__(32 * kCellPairWarps) k_cell_pairs_pt(const Gri
     if (lane == 0) stage.count = 0;
     __syncwarp();
     const Grid g = *gp;
-    // Two kinds of entry boxes (k_cell_scatter): quantised double boxes (static grid: the query is inflated by `radius` in lattice steps) or
-    // ranges of reference voxels (swept grid, vox != nullptr: ranges overlap <=> the reference's hash query pairs the two primitives, no
-    // inflation).  Either way lattice coordinate q maps to accelerator cell floor(q * S + O[axis]).
-    const double radius = radius_ptr ? *radius_ptr : radius_val;
-    const bool voxel = vox != nullptr;
-    const unsigned rq = voxel ? 0u : (unsigned)min((int)ceil(radius * g.q_inv) + 1, 65535);
+    // the query is inflated by `radius` in lattice steps of the quantised entry boxes; lattice coordinate q lies in accelerator cell floor(q * S)
+    const unsigned rq = (unsigned)min((int)ceil(radius * g.q_inv) + 1, 65535);
     const unsigned rq2 = rq | (rq << 16);
-    double S = g.inv_h / g.q_inv, O[3] = { 0.0, 0.0, 0.0 }, padLo = 0.0, padHi = 0.0, bias = 0.0;
-    if (voxel) { // a swept box lies inside its voxel range [vmin, vmax + 1) and is inflated by one voxel: cells of [vmin - 1, vmax + 2)
-        S = g.inv_h / vox->ref_inv_h;
-        O[0] = (vox->ref_lo[0] - g.ox) * g.inv_h; O[1] = (vox->ref_lo[1] - g.oy) * g.inv_h; O[2] = (vox->ref_lo[2] - g.oz) * g.inv_h;
-        padLo = -1.0; padHi = 2.0; bias = 1e-6;
-    }
+    const double S = g.inv_h / g.q_inv;
     const uint4* __restrict__ ent = reinterpret_cast<const uint4*>(tg.ent);
     AEntry* A = sA[wib];
     const int pos = first + (blockIdx.x * kCellPairWarps + wib) * 32 + lane;
@@ -483,9 +433,9 @@ __global__ void __launch_bounds__(32 * kCellPairWarps) k_cell_pairs_pt(const Gri
         a.pad0 = __ldg(SVI + a.id); // the vertex itself: a triangle that contains it is no partner (:2184), and those are most overlapping boxes
         a.pad1 = 0;
         A[lane] = a;
-        cl[0] = (int)floor(((double)(a.L01 & 0xffffu) + padLo) * S + O[0] - bias); ch[0] = (int)floor(((double)(a.H01 & 0xffffu) + padHi) * S + O[0] + bias);
-        cl[1] = (int)floor(((double)(a.L01 >> 16) + padLo) * S + O[1] - bias);     ch[1] = (int)floor(((double)(a.H01 >> 16) + padHi) * S + O[1] + bias);
-        cl[2] = (int)floor(((double)a.lo2 + padLo) * S + O[2] - bias);             ch[2] = (int)floor(((double)a.hi2 + padHi) * S + O[2] + bias);
+        cl[0] = (int)floor((double)(a.L01 & 0xffffu) * S); ch[0] = (int)floor((double)(a.H01 & 0xffffu) * S);
+        cl[1] = (int)floor((double)(a.L01 >> 16) * S);     ch[1] = (int)floor((double)(a.H01 >> 16) * S);
+        cl[2] = (int)floor((double)a.lo2 * S);             ch[2] = (int)floor((double)a.hi2 * S);
     }
     __syncwarp();
     unsigned remaining = __ballot_sync(full, valid);
@@ -808,22 +758,18 @@ using namespace ipcgpu;
 
 static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
 // IPCGPU_PAIRS_MODE: 1 (default) = cell-centric edge-edge pair finding, 0 = the warp-per-query kernel of round 1
-int pairs_mode()
+static int pairs_mode()
 {
     static const int mode = [] { const char* e = std::getenv("IPCGPU_PAIRS_MODE"); return e ? std::atoi(e) : 1; }();
     return mode;
 }
-// vox != nullptr: the grid's entries are reference-voxel ranges (swept grid of the CCD), see k_cell_scatter
-void cell_pairs_pt(const Grid* gp, const SortedGrid& vg, const SortedGrid& tg, const SurfArgs& s, double radius_val, const double* radius_ptr, const IterState* vox, int first,
-    int last, const PairOut& out, cudaStream_t st)
+static void cell_pairs_pt(const Grid* gp, const SortedGrid& vg, const SortedGrid& tg, const SurfArgs& s, double radius, int first, int last, const PairOut& out, cudaStream_t st)
 {
-    if (last > first)
-        k_cell_pairs_pt<<<nblk(last - first, 32 * kCellPairWarps), 32 * kCellPairWarps, 0, st>>>(gp, vg, tg, s.SVI, s.SF, s.nSF, radius_val, radius_ptr, vox, first, last, out);
+    if (last > first) k_cell_pairs_pt<<<nblk(last - first, 32 * kCellPairWarps), 32 * kCellPairWarps, 0, st>>>(gp, vg, tg, s.SVI, s.SF, s.nSF, radius, first, last, out);
 }
-void cell_pairs_ee(const Grid* gp, const SortedGrid& eg, const SurfArgs& s, double radius_val, const double* radius_ptr, const IterState* vox, int first, int last,
-    const PairOut& out, cudaStream_t st)
+static void cell_pairs_ee(const Grid* gp, const SortedGrid& eg, const SurfArgs& s, double radius, int first, int last, const PairOut& out, cudaStream_t st)
 {
-    if (last > first) k_cell_pairs_ee<<<nblk(last - first, 32 * kCellPairWarps), 32 * kCellPairWarps, 0, st>>>(gp, eg, s.SE, radius_val, radius_ptr, vox, first, last, out);
+    if (last > first) k_cell_pairs_ee<<<nblk(last - first, 32 * kCellPairWarps), 32 * kCellPairWarps, 0, st>>>(gp, eg, s.SE, radius, first, last, out);
 }
 
 // stable radix sort of (keys, idx) pairs, result back in (keys, idx)
@@ -925,7 +871,7 @@ int contact_alloc(ipcgpu_ctx* ctx)
 // build the sorted grids of the triangles and the edges in ONE pass: one emit, one radix sort (cell key + type bit), one gather of the
 // quantised entries, one cell table
 SurfArgs surf_args(const ipcgpu_ctx* ctx);
-static int build_grids(ipcgpu_ctx* ctx, int nT, int nE, int nV, const int* vmin, const int* vmax)
+static int build_grids(ipcgpu_ctx* ctx, int nT, int nE, int nV)
 {
     ContactWork& w = ctx->cw;
     cudaStream_t st = ctx->stream;
@@ -942,8 +888,7 @@ static int build_grids(ipcgpu_ctx* ctx, int nT, int nE, int nV, const int* vmin,
         return IPCGPU_ERR_CUDA;
     }
     k_cell_scatter<<<nblk(n, 256), 256, 0, st>>>(nT, nE, nV, w.tbox.p, w.ebox.p, w.vbox.p, w.grid.p, w.cell_off.p, w.key_tmp.p, w.val_tmp.p, w.ckeys.p, w.cvals.p,
-        reinterpret_cast<uint4*>(w.centries.p), surf_args(ctx), vmin, vmax);
-    w.built_voxel_entries = vmin != nullptr;
+        reinterpret_cast<uint4*>(w.centries.p));
     ctx->launches += 5;
     return 0;
 }
@@ -975,22 +920,19 @@ SurfArgs surf_args(const ipcgpu_ctx* ctx)
     return s;
 }
 
-// boxes of vertices/edges/triangles (optionally swept by alpha*dir), grid parameters, and the two sorted grids
-// dir == nullptr: static boxes.  alpha_ptr / radius_ptr (device) override the by-value radius: the swept build takes both from the
-// device-resident iteration state
-int boxes_and_grid(ipcgpu_ctx* ctx, const double* dir, const double* alpha_ptr, double radius, const double* radius_ptr, bool with_vertex_boxes, const int* vmin, const int* vmax)
+// boxes of vertices/edges/triangles at the current positions, grid parameters, and the sorted grids
+int boxes_and_grid(ipcgpu_ctx* ctx, double radius, bool with_vertex_boxes)
 {
     ContactWork& w = ctx->cw;
     cudaStream_t st = ctx->stream;
     const SurfArgs s = surf_args(ctx);
     k_bounds_init<<<1, 32, 0, st>>>(w.bounds.p);
-    if (with_vertex_boxes && s.nSV > 0) k_boxes<<<nblk(s.nSV, 256), 256, 0, st>>>(s, 0, dir, alpha_ptr, w.vbox.p, w.bounds.p);
-    if (s.nSE > 0) k_boxes<<<nblk(s.nSE, 256), 256, 0, st>>>(s, 1, dir, alpha_ptr, w.ebox.p, w.bounds.p);
-    if (s.nSF > 0) k_boxes<<<nblk(s.nSF, 256), 256, 0, st>>>(s, 2, dir, alpha_ptr, w.tbox.p, w.bounds.p);
-    k_grid_params<<<1, 32, 0, st>>>(w.bounds.p, radius, radius_ptr, w.axis_bits, w.grid.p, ctx->iter.p);
+    if (with_vertex_boxes && s.nSV > 0) k_boxes<<<nblk(s.nSV, 256), 256, 0, st>>>(s, 0, w.vbox.p, w.bounds.p);
+    if (s.nSE > 0) k_boxes<<<nblk(s.nSE, 256), 256, 0, st>>>(s, 1, w.ebox.p, w.bounds.p);
+    if (s.nSF > 0) k_boxes<<<nblk(s.nSF, 256), 256, 0, st>>>(s, 2, w.tbox.p, w.bounds.p);
+    k_grid_params<<<1, 32, 0, st>>>(w.bounds.p, radius, w.axis_bits, w.grid.p, ctx->iter.p);
     ctx->launches += 5;
-    const bool cells = pairs_mode() != 0; // (the warp-per-query kernels of round 1 test inflated double boxes: no voxel-range entries for them)
-    return build_grids(ctx, s.nSF, s.nSE, (with_vertex_boxes && cells) ? s.nSV : 0, cells ? vmin : nullptr, cells ? vmax : nullptr);
+    return build_grids(ctx, s.nSF, s.nSE, (with_vertex_boxes && pairs_mode() != 0) ? s.nSV : 0);
 }
 
 // pack this rank's lists, allgather, rebuild the global lists (called by api.cu around its ncclAllGather)
@@ -1036,7 +978,7 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
     const double radius = sqrt(dHat);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_HASH);
     int rc;
-    if ((rc = boxes_and_grid(ctx, nullptr, nullptr, radius, nullptr, pairs_mode() != 0, nullptr, nullptr))) return rc; // (vertex entries for the cell-centric PT kernel)
+    if ((rc = boxes_and_grid(ctx, radius, pairs_mode() != 0))) return rc; // (vertex entries for the cell-centric PT kernel)
     ctx->prof_end(pe);
 
     pe = ctx->prof_begin(IPCGPU_STAGE_CONSTRAINT_SET);
@@ -1061,13 +1003,13 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
     PairOut ppt{ w.bp_pairs.p, nPairs, (unsigned)w.bp_cap, w.counters.p + 4 }, pee{ w.bp_pairs.p + w.bp_cap, nPairs + 1, (unsigned)w.bp_cap, w.counters.p + 4 };
     if (v1 > v0 && s.nSF > 0) {
         if (pairs_mode() == 0 || w.built_vertices != s.nSV) k_pairs_pt<<<nblk(v1 - v0, 8 * kPairQueriesPerWarp), 256, 0, st>>>(s, w.grid.p, tg, dHat, radius, v0, v1, ppt);
-        else cell_pairs_pt(w.grid.p, vertex_grid(ctx), tg, s, radius, nullptr, nullptr, s.nSF + s.nSE + v0, s.nSF + s.nSE + v1, ppt, st); // vertex entries: by sorted position
+        else cell_pairs_pt(w.grid.p, vertex_grid(ctx), tg, s, radius, s.nSF + s.nSE + v0, s.nSF + s.nSE + v1, ppt, st); // vertex entries: by sorted position
         k_classify_pt<<<kSMs * 8, 128, 0, st>>>(s, ppt.pairs, ppt.n, ppt.cap, dHat, wantCand, out);
         ctx->launches += 2;
     }
     if (e1 > e0 && s.nSE > 1) {
         if (pairs_mode() == 0) k_pairs_ee<<<nblk(e1 - e0, 8 * kPairQueriesPerWarp), 256, 0, st>>>(w.grid.p, eg, w.ebox.p, dHat, radius, s.nSF + e0, s.nSF + e1, pee); // edge entries sit behind the triangles
-        else cell_pairs_ee(w.grid.p, eg, s, radius, nullptr, nullptr, s.nSF + e0, s.nSF + e1, pee, st);
+        else cell_pairs_ee(w.grid.p, eg, s, radius, s.nSF + e0, s.nSF + e1, pee, st);
         k_classify_ee<<<kSMs * 8, 128, 0, st>>>(s, pee.pairs, pee.n, pee.cap, dHat, wantCand, out);
         ctx->launches += 2;
     }

@@ -63,7 +63,6 @@ struct ContactWork {
     int axis_bits = 10;         // key bits per axis of the grid sorts (re-tuned from IterState::grid_axis_cells at every fetch)
     int built_axis_bits = 10;   // ... of the grids that are currently built (position of the type bit)
     int built_vertices = 0;     // surface-vertex entries in the combined sorted array (0: the build carried none)
-    bool built_voxel_entries = false; // the entries of the current grid carry reference-voxel ranges (swept grid) instead of quantised boxes
     // barrier stage workspace, sized by the pair capacity
     DevBuf<double> bHraw, bpartials, bval; // (bval: per-constraint values of ipcgpu_evaluate_constraints / inputs of ..._jacobian_t)
     DevBuf<int> brows, bpsd;
@@ -90,6 +89,13 @@ struct CcdWork {
     bool wide_level_set = false;
     DevBuf<unsigned char> scratch;
     DevBuf<unsigned long long> ncand, bounds;
+    // swept grid on the reference voxel lattice (ccd.cu): geometry, per-entry cell keys and entries (sorted by key), dense per-(type, cell)
+    // counters and their exclusive prefix sum, scan scratch
+    DevBuf<SweptCells> cells;
+    DevBuf<unsigned> sw_keys;
+    DevBuf<uint4> sw_ent;
+    DevBuf<int> sw_cnt, sw_off;
+    DevBuf<unsigned char> sw_tmp;
     bool swept_ready = false; // (the reference swept-grid geometry of the last build lives in IterState)
     unsigned last_survivors = 0;
     unsigned long long last_deferred = 0, last_longest_cycles = 0, last_total_cycles = 0;

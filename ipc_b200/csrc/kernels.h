@@ -15,7 +15,6 @@ struct IterState {
     unsigned long long n_full_cand;   // candidates of the last full CCD (this rank)
     double max_t;                     // step on entry of the narrow phase in flight (max_t of every pair, SURVEY 8a row 10)
     double alpha_grid;                // sweep length of the last swept grid (after the span rescale of SpatialHash.hpp:603-618)
-    double radius;                    // query inflation of the swept broad phase = one reference voxel
     double ref_lo[3], ref_inv_h;      // reference swept-grid geometry (SpatialHash.hpp:589-640)
     double alpha_stage[4];            // step after: inversion filter, partial CCD, swept-grid rescale, full CCD
     double energy[4];                 // elastic, barrier, friction, inertia (cross-rank sums once reduced)

@@ -256,8 +256,7 @@ using namespace ipcgpu;
 
 SurfArgs surf_args(const ipcgpu_ctx* ctx); // constraint.cu
 SortedGrid edge_grid(const ipcgpu_ctx* ctx);
-int boxes_and_grid(ipcgpu_ctx* ctx, const double* dir, const double* alpha_ptr, double radius, const double* radius_ptr, bool with_vertex_boxes, const int* vmin,
-    const int* vmax); // constraint.cu
+int boxes_and_grid(ipcgpu_ctx* ctx, double radius, bool with_vertex_boxes); // constraint.cu
 
 static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
 
@@ -284,7 +283,7 @@ int safeguard_intersections(ipcgpu_ctx* ctx)
     int* cnt = &ctx->iter.p->checks[1];
     if (cudaMemsetAsync(cnt, 0, sizeof(int), st) != cudaSuccess) return IPCGPU_ERR_CUDA;
     if (s.nSF == 0 || s.nSE == 0) return 0;
-    int rc = boxes_and_grid(ctx, nullptr, nullptr, 0.0, nullptr, false, nullptr, nullptr);
+    int rc = boxes_and_grid(ctx, 0.0, false);
     if (rc) return rc;
     const SortedGrid eg = edge_grid(ctx);
     const int f0 = (int)((long long)s.nSF * ctx->rank / ctx->nranks), f1 = (int)((long long)s.nSF * (ctx->rank + 1) / ctx->nranks);
