@@ -112,7 +112,8 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 //   - the derivative calls in their NULL-output form (they enqueue on `deriv`);
 //   - ipcgpu_allreduce_grad_hess on one rank (a no-op), and ipcgpu_download_range_async, whose copy waits on `deriv` as well.
 // Every other entry point that touches the device calls enter(ctx, kSerial) first, which joins `deriv` into the main stream (the pure
-// host-side getters need not).  The chains stay on one stream with several ranks (the gradient sum and the step-bound min-reductions
+// host-side getters need not).  Among them ipcgpu_update_pattern: it rewrites ia, ja and slot_off, which the derivative chain reads, so it
+// runs between ipcgpu_constraint_set and the first derivative call, before the fork.  The chains stay on one stream with several ranks (the gradient sum and the step-bound min-reductions
 // must keep one order per communicator), while the stage timers are on (each stage is timed alone), and in the synchronous host-output
 // forms.
 //
@@ -127,7 +128,7 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 //   - contact lists: the barrier kernels read act / para / para_e (written by the constraint set before the fork); the step-bound chain
 //     reads ContactWork::cand and writes only the CcdWork buffers (among them the swept grid: cells, sw_keys, sw_ent, sw_cnt, sw_off,
 //     sw_tmp), which the derivative chain does not touch.
-//   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither.  g, a, gcont, hblk, hcon, e_partials2, scalar_out[0], bHraw, brows,
+//   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, hcon, e_partials2, scalar_out[0], bHraw, brows,
 //     bpsd: derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };
 
@@ -358,6 +359,31 @@ static int ensure_offsets(ipcgpu_ctx* ctx)
     return IPCGPU_OK;
 }
 
+// device-built pattern: bring the host mirrors (nnz, h_ia, owned value range) up to the device's pattern; h_iter must be fresh
+static int refresh_pattern_mirror(ipcgpu_ctx* ctx)
+{
+    if (!ctx->device_pattern) return IPCGPU_OK;
+    ctx->pat_pending = false;
+    const IterState& h = *ctx->h_iter;
+    ctx->pat_changed_host = h.pat_changed;
+    if (h.pat_version == ctx->pat_seen_version) return IPCGPU_OK;
+    ctx->pat_seen_version = h.pat_version;
+    ctx->nnz = (int)h.pat_nnz;
+    CK(cudaMemcpyAsync(ctx->h_ia.data(), ctx->ia.p, ctx->h_ia.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->full_pattern_ready = false;
+    owned_value_range(ctx);
+    return IPCGPU_OK;
+}
+int fetch_iter_state(ipcgpu_ctx* ctx);
+// ... before a host-side use of them, when an update was enqueued since (synchronises)
+static int sync_pattern_mirror(ipcgpu_ctx* ctx)
+{
+    if (!ctx->device_pattern || !ctx->pat_pending) return IPCGPU_OK;
+    int rc = fetch_iter_state(ctx);
+    return rc ? rc : refresh_pattern_mirror(ctx);
+}
+
 // C++ linkage helpers implemented in constraint.cu / ccd.cu
 int contact_alloc(ipcgpu_ctx* ctx);
 int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, int* nPara, int* nCand);
@@ -373,6 +399,8 @@ int ccd_read_back(ipcgpu_ctx* ctx, double* alpha_out);
 int solver_build_full_pattern(ipcgpu_ctx* ctx, const int* ia, const int* ja); // solve.cu
 int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int* iters_out, double* rel_res_out);
 int solver_adopt_direction(ipcgpu_ctx* ctx);
+int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity); // pattern.cu
+int pattern_update(ipcgpu_ctx* ctx, const BarrierArgs& lists, bool with_friction);
 int safeguard_inversion(ipcgpu_ctx* ctx);     // safeguard.cu
 int safeguard_intersections(ipcgpu_ctx* ctx); // safeguard.cu
 
@@ -393,6 +421,10 @@ static int status_from_flags(ipcgpu_ctx* ctx, const int* f)
     }
     if (f[FLAG_CCD_CAPACITY]) {
         ctx->err = "CCD candidate capacity exceeded (raise it with ipcgpu_set_ccd_capacity)";
+        return IPCGPU_ERR_CAPACITY;
+    }
+    if (f[FLAG_PATTERN_CAPACITY]) {
+        ctx->err = "device-built sparsity pattern exceeds its capacity (raise it with ipcgpu_enable_device_pattern); the previous pattern is kept";
         return IPCGPU_ERR_CAPACITY;
     }
     if (f[FLAG_PATTERN]) {
@@ -581,6 +613,7 @@ int ipcgpu_set_mesh(ipcgpu_ctx* ctx, int nV, int nT, const double* Vrest, const 
     ctx->h_T.assign(tets, tets + (size_t)4 * nT);
     ctx->h_ia.clear();
     ctx->nnz = 0;
+    ctx->device_pattern = ctx->pat_pending = false;
     ctx->surface_ready = false;
     ctx->dir_valid = false;
     // Dm^-1: reference layout is per-tet column-major; device layout is SoA over the row-major index q=3i+j
@@ -617,6 +650,7 @@ int ipcgpu_set_csr(ipcgpu_ctx* ctx, int n_rows, const int* ia, const int* ja, in
     ctx->n_rows = n_rows;
     ctx->nnz = nnz;
     ctx->index_base = index_base;
+    ctx->device_pattern = ctx->pat_pending = false; // host mode again
     ctx->h_ia.assign(ia, ia + (size_t)n_rows + 1);
     bool ok = ctx->ia.upload(ia, (size_t)n_rows + 1, ctx->stream) && ctx->ja.upload(ja, (size_t)nnz, ctx->stream) && ctx->a.reserve((size_t)std::max(nnz, 1));
     REQUIRE(ok, IPCGPU_ERR_CUDA, "CSR upload failed");
@@ -730,7 +764,11 @@ int ipcgpu_elastic_energy(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, double*
 static int zero_values(ipcgpu_ctx* ctx)
 {
     cudaStream_t st = ctx->deriv_stream(); // (zero_words, not a memset: kernels.h)
-    if (ctx->nranks > 1 && !ctx->a_all_dirty) {
+    if (ctx->device_pattern) { // the range follows the device's row starts (the host mirror may lag an update in flight)
+        const bool owned = ctx->nranks > 1 && !ctx->a_all_dirty;
+        zero_csr_rows(ctx->ia.p, ctx->index_base, owned ? 3 * ctx->v_begin : 0, owned ? 3 * ctx->v_end : 3 * ctx->nV, ctx->a.p, st);
+    }
+    else if (ctx->nranks > 1 && !ctx->a_all_dirty) {
         if (ctx->a_end > ctx->a_begin) zero_words(ctx->a.p + ctx->a_begin, (size_t)(ctx->a_end - ctx->a_begin) * 2, st);
     }
     else zero_words(ctx->a.p, (size_t)ctx->nnz * 2, st);
@@ -812,12 +850,18 @@ int ipcgpu_elastic_gradient(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, int p
 // host value array in (addCoeff semantics): rank 0 contributes it, everybody else starts from zero
 static int upload_values(ipcgpu_ctx* ctx, const double* a_host)
 {
+    int rc = sync_pattern_mirror(ctx);
+    if (rc) return rc;
     if (ctx->rank == 0) CK(cudaMemcpyAsync(ctx->a.p, a_host, (size_t)ctx->nnz * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     else CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)ctx->nnz * sizeof(double), ctx->stream));
     return IPCGPU_OK;
 }
 static int download_values(ipcgpu_ctx* ctx, double* a_host)
 {
+    {
+        int rc = sync_pattern_mirror(ctx);
+        if (rc) return rc;
+    }
     if (ctx->nranks > 1) {
         int rc = ipcgpu_allreduce_grad_hess(ctx, 0, 1);
         if (rc) return rc;
@@ -846,8 +890,8 @@ int ipcgpu_elastic_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int p
     ENTER(g || a ? kSerial : kDerivative);
     // the value array is rebuilt from scratch (LinSysSolver::setZero, then addCoeff of every term): slots that no local tet touches
     // -- contact-only blocks of the augmented pattern -- must not keep last iteration's values
-    int rc = zero_values(ctx);
-    if (rc) return rc;
+    int rc = a ? sync_pattern_mirror(ctx) : 0; // (the host array holds the current pattern's values)
+    if (rc || (rc = zero_values(ctx))) return rc;
     if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, true, true, add_mass))) return rc;
     if (ctx->nranks > 1 && (g || a)) {
         rc = ipcgpu_allreduce_grad_hess(ctx, g ? 1 : 0, a ? 1 : 0);
@@ -866,8 +910,8 @@ int ipcgpu_elastic_energy_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD
     ENTER(E || g || a ? kSerial : kDerivative);
     // the value array is rebuilt from scratch (LinSysSolver::setZero, then addCoeff of every term): slots that no local tet touches
     // -- contact-only blocks of the augmented pattern -- must not keep last iteration's values
-    int rc = zero_values(ctx);
-    if (rc) return rc;
+    int rc = a ? sync_pattern_mirror(ctx) : 0;
+    if (rc || (rc = zero_values(ctx))) return rc;
     if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, true, true, add_mass, true))) return rc;
     if (ctx->nranks > 1 && (g || a)) {
         rc = ipcgpu_allreduce_grad_hess(ctx, g ? 1 : 0, a ? 1 : 0);
@@ -944,6 +988,7 @@ int ipcgpu_set_surface(ipcgpu_ctx* ctx, int nSV, const int* SVI, int nSE, const 
     if (rc) return rc;
     if ((rc = ccd_alloc(ctx))) return rc;
     ctx->surface_ready = true;
+    if (ctx->device_pattern) return ipcgpu_enable_device_pattern(ctx, ctx->index_base, ctx->pw.requested_cap); // new surface edges
     return IPCGPU_OK;
 }
 
@@ -956,6 +1001,7 @@ int ipcgpu_set_obstacle_tail(ipcgpu_ctx* ctx, int first_obstacle_vertex, int ee_
         ctx->nVdof = 0x7fffffff;
         ctx->ee_as_vf = ee_through_vf_routine ? 1 : 0;
         ctx->pSize_surface = false;
+        if (ctx->device_pattern) return ipcgpu_enable_device_pattern(ctx, ctx->index_base, ctx->pw.requested_cap); // the tail's pairs return
         return IPCGPU_OK;
     }
     REQUIRE(first_obstacle_vertex > 0, IPCGPU_ERR_ARG, "the mesh needs at least one vertex of its own");
@@ -970,6 +1016,7 @@ int ipcgpu_set_obstacle_tail(ipcgpu_ctx* ctx, int first_obstacle_vertex, int ee_
     ctx->nVdof = first_obstacle_vertex;
     ctx->ee_as_vf = ee_through_vf_routine ? 1 : 0;
     ctx->pSize_surface = false; // the mean |p| of the swept build is taken over the MESH's surface vertices: upload the direction again
+    if (ctx->device_pattern) return ipcgpu_enable_device_pattern(ctx, ctx->index_base, ctx->pw.requested_cap); // the tail's pairs leave
     return IPCGPU_OK;
 }
 
@@ -1268,6 +1315,77 @@ static BarrierArgs barrier_args(ipcgpu_ctx* ctx, double dHat, double kappa, int 
     p.dHat = dHat; p.kappa = kappa; p.projectDBC = projectDBC;
     p.ia = ctx->ia.p; p.ja = ctx->ja.p; p.base = ctx->index_base;
     return p;
+}
+
+// ---- device-built sparsity pattern (pattern.cu) -------------------------------------------------------------------------
+int ipcgpu_enable_device_pattern(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity)
+{
+    ENTER(kSerial);
+    ++ctx->epoch; // graphs captured before this call are refused (ja / a may be reallocated)
+    REQUIRE(ctx->maps_ready && ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    REQUIRE(index_base == 0 || index_base == 1, IPCGPU_ERR_ARG, "index_base must be 0 or 1");
+    CK(cudaSetDevice(ctx->device));
+    ctx->device_pattern = false;
+    int rc = pattern_enable(ctx, index_base, nnz_capacity);
+    if (rc) return rc;
+    ctx->device_pattern = true;
+    ctx->pat_pending = false;
+    ctx->pat_seen_version = 0;
+    ctx->pat_changed_host = 0;
+    ctx->a_all_dirty = false;
+    ctx->offsets_ready = false;
+    ctx->full_pattern_ready = false;
+    owned_value_range(ctx);
+    return ensure_offsets(ctx);
+}
+
+int ipcgpu_update_pattern(ipcgpu_ctx* ctx, int with_friction, int* changed, int64_t* nnz)
+{
+    REQUIRE(ctx->device_pattern, IPCGPU_ERR_STATE, "ipcgpu_enable_device_pattern first");
+    REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    REQUIRE(!with_friction || ctx->cw.fr_ready, IPCGPU_ERR_STATE, "with_friction: ipcgpu_friction_lag / ipcgpu_set_friction_data first");
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    int rc = pattern_update(ctx, barrier_args(ctx, 1.0, 1.0, 0), with_friction != 0);
+    if (rc) return rc;
+    ctx->pat_pending = true;
+    if (!changed && !nnz) return IPCGPU_OK;
+    if ((rc = sync_pattern_mirror(ctx))) return rc;
+    if (changed) *changed = ctx->pat_changed_host;
+    if (nnz) *nnz = ctx->nnz;
+    if (ctx->h_iter->flags[FLAG_PATTERN_CAPACITY]) {
+        clear_flag(ctx, FLAG_PATTERN_CAPACITY);
+        int only[8] = { 0 };
+        only[FLAG_PATTERN_CAPACITY] = 1;
+        return status_from_flags(ctx, only);
+    }
+    return IPCGPU_OK;
+}
+
+int ipcgpu_pattern_info(ipcgpu_ctx* ctx, int* changed, int64_t* nnz, uint64_t* version)
+{
+    REQUIRE(ctx->device_pattern, IPCGPU_ERR_STATE, "ipcgpu_enable_device_pattern first");
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    int rc = sync_pattern_mirror(ctx);
+    if (rc) return rc;
+    if (changed) *changed = ctx->pat_changed_host;
+    if (nnz) *nnz = ctx->nnz;
+    if (version) *version = ctx->pat_seen_version;
+    return IPCGPU_OK;
+}
+
+int ipcgpu_get_pattern(ipcgpu_ctx* ctx, int* ia, int* ja)
+{
+    REQUIRE(ctx->n_rows > 0, IPCGPU_ERR_STATE, "no pattern: ipcgpu_set_csr or ipcgpu_enable_device_pattern first");
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    int rc = sync_pattern_mirror(ctx);
+    if (rc) return rc;
+    if (ia) CK(cudaMemcpyAsync(ia, ctx->ia.p, ((size_t)ctx->n_rows + 1) * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    if (ja) CK(cudaMemcpyAsync(ja, ctx->ja.p, (size_t)ctx->nnz * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IPCGPU_OK;
 }
 
 int ipcgpu_barrier_energy(ipcgpu_ctx* ctx, double dHat, double kappa, double* E)
@@ -1747,6 +1865,8 @@ int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
     ctx->deriv_copied = false;
     ctx->launches_at_capture = ctx->launches;
     ctx->dirty_at_capture = ctx->a_all_dirty;
+    ctx->pat_pending_at_capture = ctx->pat_pending;
+    ctx->pat_pending = false;
     CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
     ctx->capturing = true;
     return IPCGPU_OK;
@@ -1793,6 +1913,8 @@ int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id)
     rec.launches = ctx->launches - ctx->launches_at_capture;
     rec.epoch = ctx->epoch;
     rec.dirty_at_begin = ctx->dirty_at_capture;
+    rec.updates_pattern = ctx->pat_pending;
+    ctx->pat_pending = ctx->pat_pending_at_capture; // nothing ran yet
     rec.hs = snapshot_host_state(ctx);
     ctx->launches = ctx->launches_at_capture; // nothing ran yet
     ctx->inputs_marked = false;
@@ -1811,8 +1933,9 @@ int ipcgpu_graph_launch(ipcgpu_ctx* ctx, int graph_id)
     CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     if (ctx->a_all_dirty && !rec.dirty_at_begin) // a cross-rank completion filled rows the captured clear does not cover
-        CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)ctx->nnz * sizeof(double), ctx->stream));
+        CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)(ctx->device_pattern ? ctx->pw.nnz_cap : ctx->nnz) * sizeof(double), ctx->stream));
     CK(cudaGraphLaunch(rec.exec, ctx->stream));
+    if (rec.updates_pattern) ctx->pat_pending = true;
     ctx->a_all_dirty = false;
     apply_host_state(ctx, rec.hs);
     ctx->launches += rec.launches;
@@ -1900,6 +2023,10 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
     REQUIRE(rel_tol > 0.0 && max_iter > 0, IPCGPU_ERR_ARG, "bad tolerance / iteration limit");
     CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
+    {
+        int rcp = sync_pattern_mirror(ctx);
+        if (rcp) return rcp;
+    }
     if (!ctx->full_pattern_ready) { // once per sparsity pattern: rows of both triangles, gathered through a position map
         std::vector<int> ia((size_t)ctx->n_rows + 1), ja((size_t)ctx->nnz);
         CK(cudaMemcpyAsync(ia.data(), ctx->ia.p, ia.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1946,7 +2073,9 @@ int ipcgpu_allreduce_grad_hess(ipcgpu_ctx* ctx, int with_gradient, int with_hess
     if (with_hessian) {
         // The rows a rank owns are already complete (row-owner assembly): this only matters to a caller that wants the WHOLE matrix on
         // every rank.  Non-owned rows are zero, so a sum completes it.
-        int r = g_nccl.AllReduce(ctx->a.p, ctx->a.p, (size_t)ctx->nnz, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
+        // (device-built pattern: the whole capacity -- the count is fixed when the call is captured, the pattern may grow at replay)
+        const size_t n = ctx->device_pattern ? (size_t)ctx->pw.nnz_cap : (size_t)ctx->nnz;
+        int r = g_nccl.AllReduce(ctx->a.p, ctx->a.p, n, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
         REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(csr values) failed");
         ctx->a_all_dirty = true; // the next rebuild must clear every row, not only the owned ones
     }
@@ -1977,7 +2106,7 @@ int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
     }
     ctx->checks_local = false;
     int rc = ccd_read_back(ctx, nullptr);
-    if (rc) return rc;
+    if (rc || (rc = refresh_pattern_mirror(ctx))) return rc;
     const IterState& h = *ctx->h_iter;
     out->energy_elastic = h.energy[0];
     out->energy_barrier = h.energy[1];
@@ -2086,6 +2215,8 @@ int ipcgpu_download_range_async(ipcgpu_ctx* ctx, int which, uint64_t offset, uin
     uint64_t n;
     REQUIRE(buf_info(ctx, which, &p, &n) == 0, IPCGPU_ERR_ARG, "unknown buffer id");
     REQUIRE((dst_pinned || count == 0) && offset + count <= n, IPCGPU_ERR_ARG, "download: bad destination or range");
+    REQUIRE(!(ctx->capturing && ctx->device_pattern && which == IPCGPU_BUF_CSR_VALUES), IPCGPU_ERR_STATE,
+        "with the device-built pattern the CSR values cannot be copied from inside a graph: the range is fixed at capture, the pattern may change at replay");
     CK(cudaSetDevice(ctx->device));
     if (!ctx->copy) {
         REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "call ipcgpu_download_range_async once outside a capture first (it creates the copy stream)");
@@ -2113,6 +2244,10 @@ int ipcgpu_download_range(ipcgpu_ctx* ctx, int which, uint64_t offset, uint64_t 
     double* p;
     uint64_t n;
     {
+        int rcp = sync_pattern_mirror(ctx);
+        if (rcp) return rcp;
+    }
+    {
         const int bi = buf_info(ctx, which, &p, &n);
         REQUIRE(bi != 2, IPCGPU_ERR_STATE, "the per-tet Hessian blocks are only kept by the tile-major layout: ipcgpu_set_hessian_layout(ctx, 0) before the Hessian call");
         REQUIRE(bi == 0, IPCGPU_ERR_ARG, "unknown buffer id");
@@ -2126,6 +2261,8 @@ int ipcgpu_download_range(ipcgpu_ctx* ctx, int which, uint64_t offset, uint64_t 
 
 void* ipcgpu_device_ptr(ipcgpu_ctx* ctx, int which)
 {
+    if (which == IPCGPU_BUF_CSR_ROW_STARTS) return ctx->ia.p;
+    if (which == IPCGPU_BUF_CSR_COLUMNS) return ctx->ja.p;
     double* p;
     uint64_t n;
     return buf_info(ctx, which, &p, &n) == 0 ? p : nullptr;

@@ -103,6 +103,20 @@ struct CcdWork {
     unsigned long long last_candidates = 0, last_boxes_thread = 0, last_boxes_warp = 0;
 };
 
+// device-built sparsity pattern (pattern.cu, ipcgpu_enable_device_pattern): the static mesh part (vNeighbor, upper neighbours only) and
+// the per-update workspace.  Extra blocks (contact neighbours that are not mesh neighbours) are bucketed by their lower vertex.
+struct PatternWork {
+    DevBuf<int> mptr, mnbr;           // mesh part: upper neighbours u > v of vertex v in mnbr[mptr[v], mptr[v+1]), ascending
+    DevBuf<int> row_cnt, row_off;     // raw extra keys per lower vertex (nV + 1, last entry 0) and their exclusive scan
+    DevBuf<int> bucket;               // raw extra keys, upper vertex ids grouped by lower vertex (key_cap entries)
+    DevBuf<int> ucnt, uoff;           // distinct extra neighbours per vertex (nV + 1) and their exclusive scan
+    DevBuf<int> prev_ptr, prev_nbr;   // extra neighbours of the pattern currently in ia / ja (what the next update compares with)
+    DevBuf<unsigned char> scan_tmp;
+    size_t scan_bytes = 0;
+    long long mesh_pairs = 0, mesh_nnz = 0, nnz_cap = 0, key_cap = 0;
+    uint64_t requested_cap = 0;       // what the caller asked for (0 = default), kept to rebuild after a surface / obstacle change
+};
+
 } // namespace ipcgpu
 
 struct ipcgpu_ctx {
@@ -197,6 +211,13 @@ struct ipcgpu_ctx {
     ipcgpu::DevBuf<int> ia, ja;
     ipcgpu::DevBuf<double> a;
     ipcgpu::DevBuf<int> flag; // device error flag
+    // device-built pattern mode (ipcgpu_enable_device_pattern; ipcgpu_set_csr returns to host mode).  The host mirrors nnz / h_ia / a_begin,
+    // a_end follow the device at every fetch (or wherever a host result needs them, see sync_pattern_mirror in api.cu); pat_pending: an
+    // update was enqueued since they were last refreshed
+    bool device_pattern = false, pat_pending = false;
+    uint64_t pat_seen_version = 0;
+    int pat_changed_host = 0;
+    ipcgpu::PatternWork pw;
     // device-resident linear solve (solve.cu): full-row structure of the symmetric matrix + PCG workspace
     ipcgpu::DevBuf<int> fia, fja, fpos;
     bool full_pattern_ready = false;
@@ -218,10 +239,11 @@ struct ipcgpu_ctx {
         cudaGraph_t graph = nullptr;
         uint64_t launches = 0, epoch = 0;
         bool dirty_at_begin = false;
+        bool updates_pattern = false; // the sequence contains ipcgpu_update_pattern
         HostState hs;
     };
     std::vector<GraphRec> graphs;
-    bool capturing = false;
+    bool capturing = false, pat_pending_at_capture = false;
     uint64_t epoch = 0, launches_at_capture = 0;
     bool dirty_at_capture = false;
     double* h_scalar = nullptr; // pinned staging for scalars

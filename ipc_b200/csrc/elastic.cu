@@ -455,10 +455,10 @@ __global__ void __launch_bounds__(256) k_diag_mass_dbc(int v0, int nV, const int
 
 // slot -> CSR offsets (binary search of column 3u in rows 3v, 3v+1, 3v+2)
 __global__ void __launch_bounds__(256) k_slot_offsets(int nSlots, const int* __restrict__ slot_v, const int* __restrict__ slot_u,
-    const int* __restrict__ ia, const int* __restrict__ ja, int base, int* __restrict__ slot_off, int* __restrict__ err)
+    const int* __restrict__ ia, const int* __restrict__ ja, int base, int* __restrict__ slot_off, int* __restrict__ err, const int* __restrict__ gate)
 {
     const int sIdx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (sIdx >= nSlots) return;
+    if (sIdx >= nSlots || (gate && !*gate)) return;
     const int v = slot_v[sIdx], u = slot_u[sIdx];
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
@@ -739,10 +739,10 @@ void diag_mass_dbc_range(int v0, int v1, const int* ia, int base, const uint8_t*
 {
     if (v1 > v0 && (dbc || mass)) k_diag_mass_dbc<<<(v1 - v0 + 255) / 256, 256, 0, st>>>(v0, v1, ia, base, dbc, projectDBC, mass, a);
 }
-void slot_offsets(int nSlots, const int* slot_v, const int* slot_u, const int* ia, const int* ja, int base, int* slot_off, int* err, cudaStream_t st)
+void slot_offsets(int nSlots, const int* slot_v, const int* slot_u, const int* ia, const int* ja, int base, int* slot_off, int* err, cudaStream_t st, const int* gate)
 {
     if (nSlots <= 0) return;
-    k_slot_offsets<<<(nSlots + 255) / 256, 256, 0, st>>>(nSlots, slot_v, slot_u, ia, ja, base, slot_off, err);
+    k_slot_offsets<<<(nSlots + 255) / 256, 256, 0, st>>>(nSlots, slot_v, slot_u, ia, ja, base, slot_off, err, gate);
 }
 void inversion_step(const ElasticArgs& p, const double* dir, double slack, double* per_tet, IterState* st_dev, cudaStream_t st)
 {

@@ -25,8 +25,16 @@ struct IterState {
     int pad_;
     int checks[2];                    // line-search safeguards: inverted tets, surface triangles crossed by an edge (this rank's share, then sums)
     unsigned long long ccd_stats[8];  // survivors, warnings, deferred, longest / total pair cycles, boxes (thread pass, warp pass), candidates
+    // device-built sparsity pattern (pattern.cu): result of the last ipcgpu_update_pattern and its per-update control words
+    long long pat_nnz;                // nnz of the pattern in ia / ja
+    unsigned long long pat_version;   // bumped by every update that rewrote the pattern
+    int pat_changed;                  // the last update rewrote the pattern
+    int pat_ok;                       // the raw contact keys of the update in flight fit the key buffer
+    int pat_diff;                     // the extra blocks of the update in flight differ from the previous ones
+    int pat_pad_;
 };
-enum { FLAG_NONPOSITIVE_DISTANCE = 0, FLAG_SET_CAPACITY = 1, FLAG_CCD_CAPACITY = 2, FLAG_ZERO_CCD_DISTANCE = 3, FLAG_PATTERN = 4, FLAG_TI_WARNINGS = 5, FLAG_EXCHANGE_CAPACITY = 6 };
+enum { FLAG_NONPOSITIVE_DISTANCE = 0, FLAG_SET_CAPACITY = 1, FLAG_CCD_CAPACITY = 2, FLAG_ZERO_CCD_DISTANCE = 3, FLAG_PATTERN = 4, FLAG_TI_WARNINGS = 5, FLAG_EXCHANGE_CAPACITY = 6,
+    FLAG_PATTERN_CAPACITY = 7 };
 
 struct ElasticArgs {
     int nV, nT;
@@ -57,7 +65,9 @@ void gather_gradient(int nV, const int* inc_ptr, const int* inc, const double* g
 void assemble_csr(int nSlots, const int* slot_v, const int* slot_u, const int* slot_off, const int* con_ptr, const unsigned* con_src,
     const double* hblk, const uint8_t* dbc, int projectDBC, const double* mass, int accumulate, double* a, cudaStream_t st);
 void diag_mass_dbc(int nV, const int* ia, int base, const uint8_t* dbc, int projectDBC, const double* mass, double* a, cudaStream_t st);
-void slot_offsets(int nSlots, const int* slot_v, const int* slot_u, const int* ia, const int* ja, int base, int* slot_off, int* err, cudaStream_t st);
+// gate != nullptr: the kernel does nothing unless *gate is nonzero (the device-built pattern recomputes the offsets only when it changed)
+void slot_offsets(int nSlots, const int* slot_v, const int* slot_u, const int* ia, const int* ja, int base, int* slot_off, int* err, cudaStream_t st,
+    const int* gate = nullptr);
 void diag_mass_dbc_range(int v0, int v1, const int* ia, int base, const uint8_t* dbc, int projectDBC, const double* mass, double* a, cudaStream_t st);
 void inversion_step(const ElasticArgs& p, const double* dir, double slack, double* per_tet, IterState* st_dev, cudaStream_t st);
 void inversion_apply(IterState* st_dev, int nT, cudaStream_t st);          // Energy.cpp:576-579 on the device-resident step
@@ -135,6 +145,8 @@ void friction_energy(const FrictionArgs& p, double* partials, cudaStream_t st);
 int friction_energy_blocks();
 void friction_gradient(const FrictionArgs& p, double* g, cudaStream_t st);
 void friction_hessian(const FrictionArgs& p, double* a, int* err, cudaStream_t st);
+// pattern.cu: a[ia[row0] - base, ia[row1] - base) = 0 with the range read on the device (the value-array clear of the device-built pattern)
+void zero_csr_rows(const int* ia, int base, int row0, int row1, double* a, cudaStream_t st);
 // elastic.cu (shared fixed-order reduction)
 void reduce_sum(const double* partials, int n, double scale, double* out, cudaStream_t st);
 

@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libipcgpu.so")
 ERR_NAMES = {0: "OK", 1: "CUDA", 2: "ARG", 3: "PATTERN", 4: "NONPOSITIVE_DISTANCE", 5: "CAPACITY", 6: "NCCL", 7: "STATE"}
 
 BUF_GRADIENT, BUF_CSR_VALUES, BUF_ENERGY_PER_TET, BUF_TET_HESSIANS, BUF_TET_GRADIENTS, BUF_INVERSION_STEPS = range(6)
+BUF_CSR_ROW_STARTS, BUF_CSR_COLUMNS = 6, 7  # ipcgpu_device_ptr only
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
@@ -43,6 +44,10 @@ SIGNATURES = {
     "ipcgpu_download_range_async": (C.c_int, [_ctxp, C.c_int, C.c_uint64, C.c_uint64, _dp]),
     "ipcgpu_set_mesh": (C.c_int, [_ctxp, C.c_int, C.c_int, _dp, _ip, _dp, _dp, _dp, _dp, _dp, _u8p, C.c_int]),
     "ipcgpu_set_csr": (C.c_int, [_ctxp, C.c_int, _ip, _ip, C.c_int]),
+    "ipcgpu_enable_device_pattern": (C.c_int, [_ctxp, C.c_int, C.c_uint64]),
+    "ipcgpu_update_pattern": (C.c_int, [_ctxp, C.c_int, _ip, C.POINTER(C.c_int64)]),
+    "ipcgpu_pattern_info": (C.c_int, [_ctxp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]),
+    "ipcgpu_get_pattern": (C.c_int, [_ctxp, _ip, _ip]),
     "ipcgpu_set_state": (C.c_int, [_ctxp, _dp]),
     "ipcgpu_save_state": (C.c_int, [_ctxp]),
     "ipcgpu_set_search_dir": (C.c_int, [_ctxp, _dp]),
@@ -226,6 +231,38 @@ class Context:
         ia, ja = i32(ia), i32(ja)
         self.nnz = int(ia[-1]) - index_base
         self._ck(self.lib.ipcgpu_set_csr(self.h, ia.size - 1, _i(ia), _i(ja), index_base))
+
+    def enable_device_pattern(self, index_base=1, nnz_capacity=0):
+        """the device builds the sparsity pattern from here on (mesh part now, contact part at every update_pattern)"""
+        self._ck(self.lib.ipcgpu_enable_device_pattern(self.h, int(index_base), int(nnz_capacity)))
+        self.nnz = self.pattern_info()[1]
+
+    def update_pattern(self, with_friction=0, want=True):
+        """want=True: (changed, nnz) after one synchronisation; want=False: enqueued only (read it with fetch_iteration / pattern_info)"""
+        if not want:
+            self._ck(self.lib.ipcgpu_update_pattern(self.h, int(with_friction), None, None))
+            return None
+        ch, n = C.c_int(), C.c_int64()
+        self._ck(self.lib.ipcgpu_update_pattern(self.h, int(with_friction), C.byref(ch), C.byref(n)))
+        self.nnz = n.value
+        return ch.value, n.value
+
+    def pattern_info(self):
+        """(changed, nnz, version) of the last pattern update"""
+        ch, n, ver = C.c_int(), C.c_int64(), C.c_uint64()
+        self._ck(self.lib.ipcgpu_pattern_info(self.h, C.byref(ch), C.byref(n), C.byref(ver)))
+        self.nnz = n.value
+        return ch.value, n.value, ver.value
+
+    def get_pattern(self):
+        """(ia, ja) of the current pattern"""
+        nnz = self.pattern_info()[1]
+        ia, ja = np.empty(3 * self.nV + 1, np.int32), np.empty(max(nnz, 1), np.int32)
+        self._ck(self.lib.ipcgpu_get_pattern(self.h, _i(ia), _i(ja)))
+        return ia, ja[:nnz]
+
+    def device_ptr(self, which):
+        return self.lib.ipcgpu_device_ptr(self.h, int(which))
 
     def set_state(self, V_soa):
         self._ck(self.lib.ipcgpu_set_state(self.h, _d(f64(V_soa).ravel()) if V_soa is not None else None))
