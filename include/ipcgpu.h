@@ -47,7 +47,9 @@ enum {
     IPCGPU_ERR_NONPOSITIVE_DISTANCE = 4, /* Optimizer.cpp:3296-3306 would exit(0) */
     IPCGPU_ERR_CAPACITY = 5,
     IPCGPU_ERR_NCCL = 6,
-    IPCGPU_ERR_STATE = 7
+    IPCGPU_ERR_STATE = 7,
+    IPCGPU_ERR_LINE_SEARCH = 8 /* step 0: a line search whose entry state fails a safeguard (the reference loops forever, Optimizer.cpp:2710-2811),
+                                  or a zero step bound (Optimizer.cpp:2031-2033 would exit(-1)) */
 };
 
 enum { IPCGPU_NEOHOOKEAN = 0, IPCGPU_FIXED_COROT = 1 };
@@ -302,6 +304,52 @@ int ipcgpu_hash_build_swept(ipcgpu_ctx* ctx, const double* p_interleaved /* NULL
 /* largestFeasibleStepSize_CCD_TightInclusion (SelfCollisionHandler.cpp:1370-1630) over the candidates of the swept hash.
  * n_candidates (may be NULL) receives the number of PT+EE pairs sent to the narrow phase. */
 int ipcgpu_ccd_full_ti(ipcgpu_ctx* ctx, double tolerance, const double err_vf[3], const double err_ee[3], double* alpha_inout, uint64_t* n_candidates);
+
+/* ---- step control: the CFL branch of the step bound and the line search (DESIGN.md section 3.11, INTEGRATION.md section 4) ---------------
+ * Both run their data-dependent decisions on the device.  Inside ipcgpu_capture_begin / _end they become conditional graph nodes (CUDA 12.4
+ * or newer; IPCGPU_ERR_CUDA without driver support) and nothing synchronises.  OUTSIDE a capture the host drives the loops and reads each
+ * decision back: one synchronisation per decision, also with alpha_inout == NULL (the one exception to "NULL outputs never synchronise"; it is
+ * also the eager run that makes the lazy allocations before a capture).  Single rank only (IPCGPU_ERR_STATE with several). */
+/* CFL_FOR_CCD == 2 (Optimizer.cpp:1947-2027; src/Utils/Types.hpp:34).  Call it after ipcgpu_ccd_partial_ti, in place of
+ * ipcgpu_hash_build_swept + ipcgpu_ccd_full_ti: alpha_CFL = sqrt(dHat) / (2 max_i |p_SVI[i]|) over the mesh's surface vertices (inf for p = 0);
+ * if (first_iteration && alpha > alpha_CFL) || alpha > 2 alpha_CFL: swept hash + full CCD, then alpha = max(alpha, alpha_CFL); otherwise
+ * alpha = min(alpha, alpha_CFL) (the swept-grid and full-CCD stages of ipcgpu_iteration then report that step).  A zero step raises
+ * IPCGPU_ERR_LINE_SEARCH (ipcgpu_step_control_info; returned directly by the host-output form). */
+int ipcgpu_ccd_cfl_ti(ipcgpu_ctx* ctx, double dHat, int first_iteration, double voxel_size, double tolerance, const double err_vf[3], const double err_ee[3],
+    double* alpha_inout /* NULL: device-resident step */);
+/* the energy of a line-search trial, ((E_el + E_in) + E_b) + E_f in the order of Optimizer::computeEnergyVal (Optimizer.cpp:3199-3378) */
+typedef struct ipcgpu_line_search_terms {
+    double elastic_coef;          /* dt^2 * energyParams[0] (BE) or dt^2 * beta_NM * energyParams[0] */
+    int    inertia;               /* != 0: + sum m|x - xtilde|^2 / 2 (ipcgpu_set_xtilde) */
+    double dHat, kappa;           /* + kappa * sum b(d) over the sets rebuilt at every trial */
+    double fric_eps2, fric_coef;  /* fric_coef > 0: + friction energy of the lagged set (ipcgpu_friction_lag) */
+} ipcgpu_line_search_terms;
+/* Optimizer::lineSearch (Optimizer.cpp:2662-2916) with armijoParam = 0 and lowerBound = 0, the only values the reference passes (:2059, :2614),
+ * from the device-resident step (alpha_inout == NULL) or *alpha_inout, along the search direction held (ipcgpu_set_search_dir / ipcgpu_solve_pcg).
+ *   V0 := V into the saved state (this OVERWRITES what ipcgpu_save_state saved), E0 := E(V) with the contact sets held;
+ *   V = V0 + alpha p; Neo-Hookean meshes only: while a tet is inverted, alpha /= 2 and step again (:2710-2715);
+ *   while not intersection-free, alpha /= 2 and step again (:2720-2733);  constraint set (getPTEE = 1), E_t = E(V);
+ *   while E_t > E0: alpha /= 2 (alpha == 0: stopped), step, constraint set, E_t = E(V) (:2761-2797);
+ *   if alpha dropped: while not intersection-free, alpha /= 2 and step, then the constraint set again if that loop ran (:2799-2811).
+ * The accepted step becomes the device-resident step (ipcgpu_fetch_iteration().alpha).  An entry step of 0 runs nothing; every loop also ends
+ * at alpha == 0 and then reports IPCGPU_ERR_LINE_SEARCH with V = V0; d <= 0 in a trial ends the search with IPCGPU_ERR_NONPOSITIVE_DISTANCE.
+ * Results: ipcgpu_step_control_info; the host-output form returns the status directly.  Inside a capture the contact lists must be in
+ * arbitrary order (ipcgpu_set_canonical_order(ctx, 0)). */
+int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* terms, double* alpha_inout);
+typedef struct ipcgpu_step_control {
+    double alpha_cfl;             /* last ipcgpu_ccd_cfl_ti */
+    double alpha_feasible;        /* last line search: the step after the inversion guard and the intersection pre-check (LFStepSize, :2750) */
+    double alpha;                 /* ... the accepted step */
+    double energy_start, energy;  /* ... E0 and E_t of the last trial (lastEnergyVal, :2898) */
+    int full_ccd;                 /* last ipcgpu_ccd_cfl_ti took the full CCD */
+    int stopped;                  /* the Armijo loop halved the step to 0 (lineSearch's return value) */
+    int halvings_inversion, halvings_intersection, halvings_armijo, halvings_post_check;
+    int post_check_rebuilt;       /* the post-check halved the step and the constraint set was rebuilt */
+    int status;                   /* IPCGPU_OK, IPCGPU_ERR_LINE_SEARCH or IPCGPU_ERR_NONPOSITIVE_DISTANCE */
+} ipcgpu_step_control;
+/* synchronises only when a CFL branch or a line search was enqueued since the last read; returns out->status */
+int ipcgpu_step_control_info(ipcgpu_ctx* ctx, ipcgpu_step_control* out);
+
 /* ---- kinematic mesh obstacle: MeshCO<3> (src/CollisionObject/MeshCO.hpp:39-233; SURVEY 8 row f3, barrier / Tight-Inclusion path) --------------------
  * An obstacle is a triangle mesh without degrees of freedom (MeshCO's Base::V, edges, Base::F).  It rides at the TAIL of the mesh's arrays: the
  * caller appends the obstacle's vertices to the vertex arrays of ipcgpu_set_mesh (rest = current positions, Dirichlet flag 1, mass 0, no

@@ -434,21 +434,30 @@ static int status_from_flags(ipcgpu_ctx* ctx, const int* f)
     return IPCGPU_OK;
 }
 
-// f(node, priority attribute) on every kernel node of a graph, until one returns an error
+// f(node, priority attribute) on every kernel node of a graph and of the bodies of its conditional nodes, until one returns an error
 template <typename F>
-static cudaError_t for_each_kernel_node(cudaGraph_t g, F f)
+static cudaError_t for_each_kernel_node(cudaGraph_t top, const std::vector<cudaGraph_t>& bodies, F f)
 {
-    size_t n = 0;
-    cudaError_t e = cudaGraphGetNodes(g, nullptr, &n);
-    std::vector<cudaGraphNode_t> nodes(n);
-    if (e == cudaSuccess && n) e = cudaGraphGetNodes(g, nodes.data(), &n);
-    for (size_t i = 0; e == cudaSuccess && i < n; ++i) {
-        cudaGraphNodeType type;
-        e = cudaGraphNodeGetType(nodes[i], &type);
-        if (e != cudaSuccess || type != cudaGraphNodeTypeKernel) continue;
-        cudaKernelNodeAttrValue v;
-        e = cudaGraphKernelNodeGetAttribute(nodes[i], cudaKernelNodeAttributePriority, &v);
-        if (e == cudaSuccess) e = f(nodes[i], v);
+    cudaError_t e = cudaSuccess;
+    for (size_t b = 0; e == cudaSuccess && b <= bodies.size(); ++b) {
+        cudaGraph_t g = b == 0 ? top : bodies[b - 1];
+        size_t n = 0;
+        e = cudaGraphGetNodes(g, nullptr, &n);
+        std::vector<cudaGraphNode_t> nodes(n);
+        if (e == cudaSuccess && n) e = cudaGraphGetNodes(g, nodes.data(), &n);
+        for (size_t i = 0; e == cudaSuccess && i < n; ++i) {
+            // (the runtime reports no type for a conditional node: cudaErrorUnknown, not sticky, but left as the last error, which a later
+            // cub call would pick up -- cleared here; the node's body is in `bodies`)
+            cudaGraphNodeType type;
+            if (cudaGraphNodeGetType(nodes[i], &type) != cudaSuccess) {
+                cudaGetLastError();
+                continue;
+            }
+            if (type != cudaGraphNodeTypeKernel) continue;
+            cudaKernelNodeAttrValue v;
+            e = cudaGraphKernelNodeGetAttribute(nodes[i], cudaKernelNodeAttributePriority, &v);
+            if (e == cudaSuccess) e = f(nodes[i], v);
+        }
     }
     return e;
 }
@@ -523,6 +532,8 @@ void ipcgpu_destroy(ipcgpu_ctx* ctx)
     if (ctx->ev_deriv_fork) cudaEventDestroy(ctx->ev_deriv_fork);
     if (ctx->ev_deriv_done) cudaEventDestroy(ctx->ev_deriv_done);
     if (ctx->deriv) cudaStreamDestroy(ctx->deriv);
+    for (cudaStream_t s : ctx->cond_streams)
+        if (s) cudaStreamDestroy(s);
     for (auto& v : ctx->prof)
         for (auto& pr : v) {
             cudaEventDestroy(pr.first);
@@ -1867,6 +1878,9 @@ int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
     ctx->dirty_at_capture = ctx->a_all_dirty;
     ctx->pat_pending_at_capture = ctx->pat_pending;
     ctx->pat_pending = false;
+    ctx->sc_pending_at_capture = ctx->sc_pending;
+    ctx->sc_pending = false;
+    ctx->capture_bodies.clear();
     CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
     ctx->capturing = true;
     return IPCGPU_OK;
@@ -1892,7 +1906,7 @@ int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id)
     if (ctx->deriv_copied) {
         // the sequence hands the derivative chain's results to the host: that chain and the copy behind it (longer than the step-bound
         // chain) are now the critical path, so in this graph the two chains trade priorities
-        e = for_each_kernel_node(rec.graph, [&](cudaGraphNode_t node, cudaKernelNodeAttrValue v) {
+        e = for_each_kernel_node(rec.graph, ctx->capture_bodies, [&](cudaGraphNode_t node, cudaKernelNodeAttrValue v) {
             v.priority = (v.priority == ctx->prio_high) ? ctx->prio_low : ctx->prio_high;
             return cudaGraphKernelNodeSetAttribute(node, cudaKernelNodeAttributePriority, &v);
         });
@@ -1915,6 +1929,9 @@ int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id)
     rec.dirty_at_begin = ctx->dirty_at_capture;
     rec.updates_pattern = ctx->pat_pending;
     ctx->pat_pending = ctx->pat_pending_at_capture; // nothing ran yet
+    rec.step_control = ctx->sc_pending;
+    ctx->sc_pending = ctx->sc_pending_at_capture;
+    rec.bodies.swap(ctx->capture_bodies);
     rec.hs = snapshot_host_state(ctx);
     ctx->launches = ctx->launches_at_capture; // nothing ran yet
     ctx->inputs_marked = false;
@@ -1936,6 +1953,7 @@ int ipcgpu_graph_launch(ipcgpu_ctx* ctx, int graph_id)
         CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)(ctx->device_pattern ? ctx->pw.nnz_cap : ctx->nnz) * sizeof(double), ctx->stream));
     CK(cudaGraphLaunch(rec.exec, ctx->stream));
     if (rec.updates_pattern) ctx->pat_pending = true;
+    if (rec.step_control) ctx->sc_pending = true;
     ctx->a_all_dirty = false;
     apply_host_state(ctx, rec.hs);
     ctx->launches += rec.launches;
@@ -1960,7 +1978,7 @@ int ipcgpu_graph_kernel_priorities(ipcgpu_ctx* ctx, int graph_id, int* n_high, i
     REQUIRE(n_high && n_low, IPCGPU_ERR_ARG, "null argument");
     CK(cudaSetDevice(ctx->device));
     *n_high = *n_low = 0;
-    CK(for_each_kernel_node(ctx->graphs[graph_id].graph, [&](cudaGraphNode_t, cudaKernelNodeAttrValue v) {
+    CK(for_each_kernel_node(ctx->graphs[graph_id].graph, ctx->graphs[graph_id].bodies, [&](cudaGraphNode_t, cudaKernelNodeAttrValue v) {
         if (v.priority == ctx->prio_high) ++*n_high;
         else if (v.priority == ctx->prio_low) ++*n_low;
         return cudaSuccess;
@@ -2013,6 +2031,245 @@ int ipcgpu_intersection_free(ipcgpu_ctx* ctx, int* ok)
         *ok = ctx->h_iter->checks[1] == 0 ? 1 : 0;
     }
     return IPCGPU_OK;
+}
+
+// ---- step control: CFL branch and line search (step_control.cu holds the decision kernel) ----------------------------------------
+// Each loop body and loop condition is written once: a sequence of the entry points above plus one step_decide.  Outside a capture the
+// host loops and reads the decision word (one synchronisation per decision); inside one the body is captured into a conditional node.
+static int decide(ipcgpu_ctx* ctx, int op, double a, int b, cudaGraphConditionalHandle h, bool* word)
+{
+    step_decide(ctx->iter.p, op, a, b, (unsigned long long)h, ctx->stream);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    if (word) {
+        int* hw = reinterpret_cast<int*>(ctx->h_scalar + 40); // pinned staging slot of its own
+        CK(cudaMemcpyAsync(hw, &ctx->iter.p->ls_cond, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        *word = *hw != 0;
+    }
+    return IPCGPU_OK;
+}
+
+} // extern "C"
+
+// if (decision) body  /  while (decision) body, where the decision is step_decide(op) before the node and, for a loop, at the end of each pass.
+// Captured: the handle is created on the graph being captured, the decision before the node sets it, the node is added behind the
+// capture's current dependencies, and the body is captured into the node's body graph on a stream of its own (ctx->stream points to it
+// meanwhile, so that the entry points the body calls enqueue there).
+template <typename Body>
+static int cond_node(ipcgpu_ctx* ctx, bool loop, int op, double a, int b, Body body)
+{
+    int rc;
+    if (!ctx->capturing) {
+        bool go = false;
+        if ((rc = decide(ctx, op, a, b, 0, &go))) return rc;
+        while (go) {
+            if ((rc = body())) return rc;
+            if (!loop) break;
+            if ((rc = decide(ctx, op, a, b, 0, &go))) return rc;
+        }
+        return IPCGPU_OK;
+    }
+    REQUIRE(ctx->cond_depth < ipcgpu_ctx::kCondDepth, IPCGPU_ERR_STATE, "conditional nodes nested too deeply");
+    cudaStreamCaptureStatus cs;
+    cudaGraph_t g = nullptr;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t nd = 0;
+    CK(cudaStreamGetCaptureInfo(ctx->stream, &cs, nullptr, &g, &deps, &nd));
+    cudaGraphConditionalHandle h = 0;
+    const cudaError_t eh = cudaGraphConditionalHandleCreate(&h, g, 0, 0);
+    if (eh != cudaSuccess) {
+        cudaGetLastError();
+        ctx->err = std::string("conditional graph nodes need CUDA 12.4 or newer in the driver: ") + cudaGetErrorString(eh);
+        return IPCGPU_ERR_CUDA;
+    }
+    if ((rc = decide(ctx, op, a, b, h, nullptr))) return rc;
+    CK(cudaStreamGetCaptureInfo(ctx->stream, &cs, nullptr, &g, &deps, &nd));
+    cudaGraphNodeParams np = {};
+    np.type = cudaGraphNodeTypeConditional;
+    np.conditional.handle = h;
+    np.conditional.type = loop ? cudaGraphCondTypeWhile : cudaGraphCondTypeIf;
+    np.conditional.size = 1;
+    cudaGraphNode_t node;
+    CK(cudaGraphAddNode(&node, g, deps, nd, &np));
+    cudaGraph_t bg = np.conditional.phGraph_out[0];
+    ctx->capture_bodies.push_back(bg);
+    cudaStream_t outer = ctx->stream, inner = ctx->cond_streams[ctx->cond_depth];
+    CK(cudaStreamBeginCaptureToGraph(inner, bg, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    ctx->stream = inner;
+    ++ctx->cond_depth;
+    ctx->inputs_marked = false;
+    rc = body();
+    if (!rc && loop) rc = decide(ctx, op, a, b, h, nullptr);
+    --ctx->cond_depth;
+    ctx->stream = outer;
+    cudaGraph_t captured = nullptr;
+    const cudaError_t ee = cudaStreamEndCapture(inner, &captured);
+    if (rc) return rc;
+    CK(ee);
+    CK(cudaStreamUpdateCaptureDependencies(outer, &node, 1, cudaStreamSetCaptureDependencies));
+    ctx->mark_inputs(); // an event recorded inside the body cannot be waited on out here: the positions / sets changed at this node
+    return IPCGPU_OK;
+}
+
+extern "C" {
+
+static int step_control_prepare(ipcgpu_ctx* ctx)
+{
+    REQUIRE(ctx->surface_ready && ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh and ipcgpu_set_surface first");
+    REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the CFL branch and the line search run on one rank");
+    REQUIRE(ctx->dir_valid && ctx->pSize_surface, IPCGPU_ERR_STATE, "no search direction for this surface: ipcgpu_set_search_dir first");
+    if (!ctx->cond_streams[0]) {
+        REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "run the CFL branch / line search once outside a capture first (it creates its streams)");
+        for (cudaStream_t& s : ctx->cond_streams) CK(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, ctx->prio_high));
+    }
+    return IPCGPU_OK;
+}
+
+static int step_control_status(ipcgpu_ctx* ctx, int status)
+{
+    if (status == IPCGPU_ERR_LINE_SEARCH)
+        ctx->err = "step 0: the line search's entry state fails a safeguard (inversion / intersection), or the step bound or the entry step is 0";
+    else if (status == IPCGPU_ERR_NONPOSITIVE_DISTANCE)
+        ctx->err = "a line-search trial has a constraint with d <= 0 (the reference exits here, Optimizer.cpp:3296-3306)";
+    return status;
+}
+
+// host-output form: read the state back, hand out the step and the status
+static int step_control_host_result(ipcgpu_ctx* ctx, double* alpha_inout)
+{
+    int rc = fetch_iter_state(ctx);
+    if (rc) return rc;
+    ctx->sc_pending = false;
+    std::memcpy(alpha_inout, &ctx->h_iter->step_ord, sizeof(double));
+    return step_control_status(ctx, ctx->h_iter->sc_status);
+}
+
+int ipcgpu_ccd_cfl_ti(ipcgpu_ctx* ctx, double dHat, int first_iteration, double voxel_size, double tol, const double err_vf[3], const double err_ee[3], double* alpha_inout)
+{
+    REQUIRE(err_vf && err_ee, IPCGPU_ERR_ARG, "null argument");
+    REQUIRE(dHat > 0.0 && voxel_size > 0.0, IPCGPU_ERR_ARG, "dHat and the voxel size must be positive");
+    CK(cudaSetDevice(ctx->device));
+    int rc = step_control_prepare(ctx);
+    if (rc) return rc;
+    ENTER(alpha_inout ? kSerial : kStepBound);
+    if (alpha_inout && (rc = ipcgpu_step_bound_set(ctx, *alpha_inout))) return rc;
+    cfl_pmax(ctx->nSV, ctx->SVI.p, ctx->nVdof, ctx->dir.p, ctx->iter.p, ctx->stream);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    rc = cond_node(ctx, false, kCflBranch, dHat, first_iteration ? 1 : 0, [&]() {
+        int r = ccd_build_swept(ctx, voxel_size);
+        if (!r) r = ccd_full(ctx, tol, err_vf, err_ee);
+        if (!r) r = decide(ctx, kCflClamp, 0.0, 0, 0, nullptr);
+        return r;
+    });
+    if (rc) return rc;
+    ctx->sc_pending = true;
+    return alpha_inout ? step_control_host_result(ctx, alpha_inout) : IPCGPU_OK;
+}
+
+// one trial's energy: E_el, E_in, E_b, E_f into IterState::energy (summed by the decision that reads them)
+static int ls_energy(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
+{
+    int rc = ipcgpu_elastic_energy(ctx, t.elastic_coef, 1, nullptr);
+    if (!rc && t.inertia) rc = ipcgpu_inertia_energy(ctx, nullptr);
+    if (!rc) rc = ipcgpu_barrier_energy(ctx, t.dHat, t.kappa, nullptr);
+    if (!rc && t.fric_coef > 0.0) rc = ipcgpu_friction_energy(ctx, t.fric_eps2, t.fric_coef, nullptr);
+    return rc;
+}
+// V = V0 + alpha p with the device-resident step
+static int ls_step(ipcgpu_ctx* ctx)
+{
+    step_forward(ctx->nV, ctx->Vsaved.p, ctx->dir.p, 0.0, ctx->V.p, ctx->stream, &ctx->iter.p->step_ord);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    ctx->mark_inputs();
+    return IPCGPU_OK;
+}
+
+static int line_search_body(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
+{
+    const int terms = (t.inertia ? kTermInertia : 0) | (t.fric_coef > 0.0 ? kTermFriction : 0);
+    CK(cudaMemcpyAsync(ctx->Vsaved.p, ctx->V.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream)); // :2692
+    ctx->state_saved = true;
+    int rc = ls_energy(ctx, t); // :2681
+    if (!rc) rc = decide(ctx, kLsStart, 0.0, terms, 0, nullptr);
+    if (!rc) rc = ls_step(ctx); // :2709
+    if (!rc && ctx->energy == IPCGPU_NEOHOOKEAN) { // getNeedElemInvSafeGuard() (:2710)
+        rc = ipcgpu_check_inversion(ctx, nullptr);
+        if (!rc) rc = cond_node(ctx, true, kLsInversion, 0.0, 0, [&]() {
+            int r = ls_step(ctx);
+            return r ? r : ipcgpu_check_inversion(ctx, nullptr);
+        });
+    }
+    if (!rc) rc = ipcgpu_intersection_free(ctx, nullptr); // :2720
+    if (!rc) rc = cond_node(ctx, true, kLsIntersection, 0.0, 0, [&]() {
+        int r = ls_step(ctx);
+        return r ? r : ipcgpu_intersection_free(ctx, nullptr);
+    });
+    if (!rc) rc = ipcgpu_constraint_set(ctx, t.dHat, 1, nullptr, nullptr, nullptr); // :2741
+    if (!rc) rc = ls_energy(ctx, t);                                                 // :2744
+    if (!rc) rc = cond_node(ctx, true, kLsArmijo, 0.0, terms, [&]() {
+        int r = ls_step(ctx);
+        if (!r) r = ipcgpu_constraint_set(ctx, t.dHat, 1, nullptr, nullptr, nullptr);
+        return r ? r : ls_energy(ctx, t);
+    });
+    if (!rc) rc = cond_node(ctx, false, kLsPostCheck, 0.0, 0, [&]() {
+        int r = ipcgpu_intersection_free(ctx, nullptr);
+        if (!r) r = cond_node(ctx, true, kLsPostLoop, 0.0, 0, [&]() {
+            int q = ls_step(ctx);
+            return q ? q : ipcgpu_intersection_free(ctx, nullptr);
+        });
+        if (!r) r = cond_node(ctx, false, kLsRebuild, 0.0, 0, [&]() { return ipcgpu_constraint_set(ctx, t.dHat, 1, nullptr, nullptr, nullptr); });
+        return r;
+    });
+    return rc;
+}
+
+int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* t, double* alpha_inout)
+{
+    REQUIRE(t != nullptr, IPCGPU_ERR_ARG, "null terms");
+    REQUIRE(t->dHat > 0.0 && t->kappa >= 0.0, IPCGPU_ERR_ARG, "dHat must be positive");
+    REQUIRE(!t->inertia || (ctx->xtilde_set && ctx->has_mass), IPCGPU_ERR_STATE, "inertia: ipcgpu_set_xtilde and a mass diagonal first");
+    REQUIRE(!(t->fric_coef > 0.0) || (ctx->cw.fr_ready && ctx->prev_set && t->fric_eps2 > 0.0), IPCGPU_ERR_STATE,
+        "friction: ipcgpu_friction_lag, ipcgpu_set_prev_state and fric_eps2 > 0 first");
+    REQUIRE(!(ctx->capturing && ctx->canonical_order), IPCGPU_ERR_STATE, "inside a capture the line search needs ipcgpu_set_canonical_order(ctx, 0)");
+    CK(cudaSetDevice(ctx->device));
+    int rc = step_control_prepare(ctx);
+    if (rc) return rc;
+    ENTER(kSerial);
+    if (alpha_inout && (rc = ipcgpu_step_bound_set(ctx, *alpha_inout))) return rc;
+    if ((rc = cond_node(ctx, false, kLsEntry, 0.0, 0, [&]() { return line_search_body(ctx, *t); }))) return rc;
+    ctx->sc_pending = true;
+    return alpha_inout ? step_control_host_result(ctx, alpha_inout) : IPCGPU_OK;
+}
+
+int ipcgpu_step_control_info(ipcgpu_ctx* ctx, ipcgpu_step_control* out)
+{
+    REQUIRE(out != nullptr, IPCGPU_ERR_ARG, "null output");
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is in progress");
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->sc_pending) {
+        ENTER(kSerial);
+        int rc = fetch_iter_state(ctx);
+        if (rc) return rc;
+        ctx->sc_pending = false;
+    }
+    const IterState& h = *ctx->h_iter;
+    out->alpha_cfl = h.sc_alpha_cfl;
+    out->alpha_feasible = h.ls_LF;
+    std::memcpy(&out->alpha, &h.step_ord, sizeof(double));
+    out->energy_start = h.ls_E0;
+    out->energy = h.ls_Et;
+    out->full_ccd = h.sc_full_ccd;
+    out->stopped = h.ls_stopped;
+    out->halvings_inversion = h.ls_count[0];
+    out->halvings_intersection = h.ls_count[1];
+    out->halvings_armijo = h.ls_count[2];
+    out->halvings_post_check = h.ls_count[3];
+    out->post_check_rebuilt = h.ls_rebuilt;
+    out->status = h.sc_status;
+    return step_control_status(ctx, h.sc_status);
 }
 
 // ---- device-resident linear solve hand-off (SURVEY 8(f) rank 1) ----------------------------------------------------------

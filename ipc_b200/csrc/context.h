@@ -240,9 +240,17 @@ struct ipcgpu_ctx {
         uint64_t launches = 0, epoch = 0;
         bool dirty_at_begin = false;
         bool updates_pattern = false; // the sequence contains ipcgpu_update_pattern
+        bool step_control = false;    // ... a CFL branch or a line search
+        std::vector<cudaGraph_t> bodies; // bodies of its conditional nodes (owned by `graph`)
         HostState hs;
     };
     std::vector<GraphRec> graphs;
+    std::vector<cudaGraph_t> capture_bodies; // conditional-node bodies of the capture in progress
+    // step control (api.cu: cond_node): the bodies of nested conditional nodes are captured on these high-priority streams, one per depth
+    static constexpr int kCondDepth = 3;
+    cudaStream_t cond_streams[kCondDepth] = { nullptr, nullptr, nullptr };
+    int cond_depth = 0;
+    bool sc_pending = false, sc_pending_at_capture = false; // a CFL branch / line search was enqueued since ipcgpu_step_control_info read it
     bool capturing = false, pat_pending_at_capture = false;
     uint64_t epoch = 0, launches_at_capture = 0;
     bool dirty_at_capture = false;

@@ -25,6 +25,15 @@ struct IterState {
     int pad_;
     int checks[2];                    // line-search safeguards: inverted tets, surface triangles crossed by an edge (this rank's share, then sums)
     unsigned long long ccd_stats[8];  // survivors, warnings, deferred, longest / total pair cycles, boxes (thread pass, warp pass), candidates
+    // step control (step_control.cu): the CFL branch of the step bound and the line search
+    unsigned long long sc_pmax_ord;   // max |p| over the mesh's surface vertices
+    double sc_alpha_cfl;              // sqrt(dHat) / (2 max |p|)
+    double ls_E0, ls_Et, ls_LF;       // energy on entry, energy of the last trial, step after the safeguards (LFStepSize)
+    int sc_full_ccd;                  // the CFL branch took the full CCD
+    int sc_status;                    // IPCGPU_OK or the IPCGPU_ERR_* code that ended the last CFL branch / line search
+    int ls_count[4];                  // halvings: inversion guard, intersection pre-check, Armijo loop, post-check
+    int ls_stopped, ls_rebuilt, ls_post_ran;
+    int ls_cond;                      // the decision word of the last step_decide
     // device-built sparsity pattern (pattern.cu): result of the last ipcgpu_update_pattern and its per-update control words
     long long pat_nnz;                // nnz of the pattern in ia / ja
     unsigned long long pat_version;   // bumped by every update that rewrote the pattern
@@ -33,6 +42,9 @@ struct IterState {
     int pat_diff;                     // the extra blocks of the update in flight differ from the previous ones
     int pat_pad_;
 };
+// step_decide operations (step_control.cu) and the energy terms of a line search
+enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersection, kLsArmijo, kLsPostCheck, kLsPostLoop, kLsRebuild };
+enum { kTermInertia = 1, kTermFriction = 2 };
 enum { FLAG_NONPOSITIVE_DISTANCE = 0, FLAG_SET_CAPACITY = 1, FLAG_CCD_CAPACITY = 2, FLAG_ZERO_CCD_DISTANCE = 3, FLAG_PATTERN = 4, FLAG_TI_WARNINGS = 5, FLAG_EXCHANGE_CAPACITY = 6,
     FLAG_PATTERN_CAPACITY = 7 };
 
@@ -150,8 +162,13 @@ void zero_csr_rows(const int* ia, int base, int row0, int row1, double* a, cudaS
 // elastic.cu (shared fixed-order reduction)
 void reduce_sum(const double* partials, int n, double scale, double* out, cudaStream_t st);
 
-// misc.cu
-void step_forward(int nV, const double* x0_soa, const double* p_interleaved, double alpha, double* x_soa, cudaStream_t st);
+// misc.cu.  alpha_ord != nullptr: the step is read on the device from there (an IterState::step_ord) instead of `alpha`
+void step_forward(int nV, const double* x0_soa, const double* p_interleaved, double alpha, double* x_soa, cudaStream_t st,
+    const unsigned long long* alpha_ord = nullptr);
+// step_control.cu: IterState::sc_pmax_ord = max |p| over the surface vertices below nVdof; one decision of the step control (handle != 0:
+// also the value of that conditional graph node)
+void cfl_pmax(int nSV, const int* SVI, int nVdof, const double* dir, IterState* st_dev, cudaStream_t st);
+void step_decide(IterState* st_dev, int op, double a, int b, unsigned long long handle, cudaStream_t st);
 // inertia term of Optimizer::computeEnergyVal / computeGradient (Optimizer.cpp:3227-3239, :3439-3450)
 int inertia_energy_blocks(int nV);
 void inertia_energy(int v0, int v1, int nV, const double* x_soa, const double* xtilde_soa, const double* mass, double* partials, cudaStream_t st);

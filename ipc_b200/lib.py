@@ -11,7 +11,8 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libipcgpu.so")
 
-ERR_NAMES = {0: "OK", 1: "CUDA", 2: "ARG", 3: "PATTERN", 4: "NONPOSITIVE_DISTANCE", 5: "CAPACITY", 6: "NCCL", 7: "STATE"}
+ERR_NAMES = {0: "OK", 1: "CUDA", 2: "ARG", 3: "PATTERN", 4: "NONPOSITIVE_DISTANCE", 5: "CAPACITY", 6: "NCCL", 7: "STATE", 8: "LINE_SEARCH"}
+ERR_NONPOSITIVE_DISTANCE, ERR_STATE, ERR_LINE_SEARCH = 4, 7, 8
 
 BUF_GRADIENT, BUF_CSR_VALUES, BUF_ENERGY_PER_TET, BUF_TET_HESSIANS, BUF_TET_GRADIENTS, BUF_INVERSION_STEPS = range(6)
 BUF_CSR_ROW_STARTS, BUF_CSR_COLUMNS = 6, 7  # ipcgpu_device_ptr only
@@ -107,6 +108,9 @@ SIGNATURES = {
     "ipcgpu_profile_read": (C.c_int, [_ctxp, C.c_int, _dp, _ip]),
     "ipcgpu_timer_start": (C.c_int, [_ctxp]),
     "ipcgpu_timer_stop": (C.c_int, [_ctxp, _dp]),
+    "ipcgpu_ccd_cfl_ti": (C.c_int, [_ctxp, C.c_double, C.c_int, C.c_double, C.c_double, _dp, _dp, _dp]),
+    "ipcgpu_line_search": (C.c_int, [_ctxp, C.c_void_p, _dp]),
+    "ipcgpu_step_control_info": (C.c_int, [_ctxp, C.c_void_p]),
 }
 
 STAGES = ["elastic_energy", "elastic_tet", "gather_gradient", "assemble_csr", "inversion", "hash", "constraint_set", "barrier",
@@ -121,6 +125,19 @@ class Iteration(C.Structure):
                 ("alpha_swept_grid", C.c_double), ("alpha_full_ccd", C.c_double), ("alpha", C.c_double), ("n_active", C.c_int), ("n_mollified", C.c_int),
                 ("n_candidates", C.c_int), ("status", C.c_int), ("n_full_ccd_candidates", C.c_uint64), ("ti_warnings", C.c_uint64),
                 ("n_inverted_tets", C.c_int), ("n_intersected_triangles", C.c_int), ("energy_friction", C.c_double), ("energy_inertia", C.c_double)]
+
+
+class LineSearchTerms(C.Structure):
+    """ipcgpu_line_search_terms (include/ipcgpu.h)"""
+    _fields_ = [("elastic_coef", C.c_double), ("inertia", C.c_int), ("dHat", C.c_double), ("kappa", C.c_double), ("fric_eps2", C.c_double),
+                ("fric_coef", C.c_double)]
+
+
+class StepControl(C.Structure):
+    """ipcgpu_step_control (include/ipcgpu.h)"""
+    _fields_ = [("alpha_cfl", C.c_double), ("alpha_feasible", C.c_double), ("alpha", C.c_double), ("energy_start", C.c_double), ("energy", C.c_double),
+                ("full_ccd", C.c_int), ("stopped", C.c_int), ("halvings_inversion", C.c_int), ("halvings_intersection", C.c_int),
+                ("halvings_armijo", C.c_int), ("halvings_post_check", C.c_int), ("post_check_rebuilt", C.c_int), ("status", C.c_int)]
 
 
 class IpcGpuError(RuntimeError):
@@ -519,6 +536,29 @@ class Context:
         self._ck(self.lib.ipcgpu_ccd_partial_ti(self.h, _d(f64(p)) if p is not None else None, tol, _d(f64(err_vf)), _d(f64(err_ee)),
                                                 C.byref(a) if alpha is not None else None))
         return a.value if alpha is not None else None
+
+    def ccd_cfl(self, dHat, first_iteration, voxel_size, tol, err_vf, err_ee, alpha):
+        """CFL branch of the step bound (CFL_FOR_CCD == 2) after ccd_partial; alpha=None: the device-resident step"""
+        a = C.c_double(alpha if alpha is not None else 0.0)
+        self._ck(self.lib.ipcgpu_ccd_cfl_ti(self.h, float(dHat), int(first_iteration), float(voxel_size), float(tol), _d(f64(err_vf)), _d(f64(err_ee)),
+                                            C.byref(a) if alpha is not None else None))
+        return a.value if alpha is not None else None
+
+    def line_search(self, elastic_coef, dHat, kappa, inertia=False, fric_eps2=0.0, fric_coef=0.0, alpha=None, check=True):
+        """Optimizer::lineSearch (armijoParam = 0) along the held search direction; alpha=None: from / into the device-resident step.
+        Returns the status code (check=True raises on an error instead)"""
+        t = LineSearchTerms(float(elastic_coef), int(bool(inertia)), float(dHat), float(kappa), float(fric_eps2), float(fric_coef))
+        a = C.c_double(alpha if alpha is not None else 0.0)
+        rc = self.lib.ipcgpu_line_search(self.h, C.byref(t), C.byref(a) if alpha is not None else None)
+        if check:
+            self._ck(rc)
+        return (rc, a.value) if alpha is not None else rc
+
+    def step_control_info(self):
+        """ipcgpu_step_control of the last CFL branch / line search (its status is out.status, not raised)"""
+        out = StepControl()
+        self.lib.ipcgpu_step_control_info(self.h, C.byref(out))
+        return out
 
     def hash_build_swept(self, p, alpha, h):
         a = C.c_double(alpha if alpha is not None else 0.0)
