@@ -101,6 +101,12 @@ typedef struct ipcgpu_iteration {
     int n_inverted_tets;                     /* last ipcgpu_check_inversion (summed over ranks) */
     int n_intersected_triangles;             /* last ipcgpu_intersection_free: surface triangles crossed by an edge (summed over ranks) */
     double energy_friction, energy_inertia;  /* last ipcgpu_friction_energy / ipcgpu_inertia_energy (summed over ranks) */
+    /* half-space collision objects (ipcgpu_set_halfspaces; all 0 without planes) */
+    double energy_halfspace;                 /* last ipcgpu_halfspace_energy (summed over ranks) */
+    double energy_halfspace_friction;        /* last ipcgpu_halfspace_friction_energy (summed over ranks) */
+    double alpha_halfspace;                  /* the step after the last ipcgpu_halfspace_step */
+    int n_halfspace_active;                  /* size of the last plane active set (every rank holds all of it) */
+    int n_halfspace_crossings;               /* last ipcgpu_halfspace_crossings (summed over ranks) */
 } ipcgpu_iteration;
 /* Synchronises once, completes the deferred cross-rank scalars (collective: every rank must call it), fills `out`, clears the
  * deferred error flags and returns out->status. */
@@ -378,6 +384,47 @@ int ipcgpu_set_obstacle_tail(ipcgpu_ctx* ctx, int first_obstacle_vertex, int ee_
  * edge lengths, MeshCollisionUtils.hpp:2976-2981).  The state saved by ipcgpu_save_state keeps the tail it was saved with: move the obstacle between
  * line searches (as the reference does, Optimizer.cpp: the scripted motion runs before the Newton loop of a time step) or save the state again. */
 int ipcgpu_set_obstacle_positions(ipcgpu_ctx* ctx, const double* Vo_soa);
+
+/* ---- analytic half-space collision objects: HalfSpace<3> (src/CollisionObject/HalfSpace.cpp, CollisionObject.h; script tokens `ground` /
+ * `halfSpace`, Config.cpp:425-447; DESIGN.md section 3.12, INTEGRATION.md section 8) ----------------------------------------------------------
+ * Entries are (plane, vertex) pairs.  Every call below has a NULL-output form that is deferred and capturable; the parameters of the planes live
+ * in device memory, so moving a plane between time steps (new origin / velocitydt: the caller's HalfSpace::move) needs no new capture -- only a
+ * change of their number does.  Without planes (n = 0) every call returns at once and launches nothing.  Several ranks: the active set, the
+ * lagged set and the step bound are replicated (each rank walks all of SVI: no collective); gradient and Hessian rows, energies and crossing
+ * counts go by row owner (the counts and energies are summed by ipcgpu_fetch_iteration's single collective). */
+/* HalfSpace::init (HalfSpace.cpp:42-52) for up to 8 planes: normal normalised, D = -n.origin; velocitydt (3n, NULL = 0) and friction per plane.
+ * The ground token is origin (0, y, 0), normal (0, 1, 0).  n = 0 removes all planes. */
+int ipcgpu_set_halfspaces(ipcgpu_ctx* ctx, int n, const double* origin, const double* normal, const double* velocitydt, const double* friction);
+/* CollisionObject::computeConstraintSet (CollisionObject.h:323-352) of every plane in one pass: SVI vertices, not Dirichlet, codimension 3,
+ * d = (n.x + D)^2 < dHat; plane-major, SVI order inside a plane (activeSet[coI] over coI).  n_active NULL: deferred. */
+int ipcgpu_halfspace_constraint_set(ipcgpu_ctx* ctx, double dHat, int* n_active);
+/* kappa sum b(d) (Optimizer.cpp:3254-3267); d <= 0 raises IPCGPU_ERR_NONPOSITIVE_DISTANCE as ipcgpu_barrier_energy does */
+int ipcgpu_halfspace_energy(ipcgpu_ctx* ctx, double dHat, double kappa, double* E);
+/* HalfSpace::leftMultiplyConstraintJacobianT (HalfSpace.cpp:121-143) with input b'(d) (Optimizer.cpp:3465-3472): g += kappa b'(d) 2 dist n.
+ * g_inout as in ipcgpu_barrier_gradient; the NULL form runs on the derivative chain */
+int ipcgpu_halfspace_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* g_inout);
+/* HalfSpace::augmentIPHessian (HalfSpace.cpp:169-213): the vertex's diagonal block += kappa param n n^T where param = 4 b'' d + 2 b' > 0;
+ * a_inout as in ipcgpu_barrier_hessian */
+int ipcgpu_halfspace_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC, double* a_inout);
+/* HalfSpace::largestFeasibleStepSize (HalfSpace.cpp:242-269; slackness_a = 0.9 at Optimizer.cpp:1886-1890, after the inversion filter, before the
+ * partial CCD): alpha = min(alpha, 1, -dist / (n.p) slackness over the non-Dirichlet SVI vertices with n.p < 0).  A bound <= 0 stores step 0
+ * and reports IPCGPU_ERR_LINE_SEARCH (returned by the host form, else by ipcgpu_fetch_iteration).  p NULL: the held search direction;
+ * alpha_inout NULL: the device-resident step (step-bound chain). */
+int ipcgpu_halfspace_step(ipcgpu_ctx* ctx, const double* p_interleaved, double slackness, double* alpha_inout);
+/* CollisionObject::isIntersected (CollisionObject.h:386-401): number of (plane, vertex) with d <= 0 over every codimension-3, non-Dirichlet
+ * vertex.  The test is on the SQUARED distance, as in the reference: a vertex that tunnelled behind a plane is not counted.  n NULL: deferred. */
+int ipcgpu_halfspace_crossings(ipcgpu_ctx* ctx, int* n);
+/* the friction update of Optimizer.cpp:1555-1572: the active entries of the planes with friction > 0 become the lagged set, with
+ * lambda = -kappa 2 sqrt(d) b'(d).  n_lagged NULL: deferred. */
+int ipcgpu_halfspace_friction_lag(ipcgpu_ctx* ctx, double dHat, double kappa, int* n_lagged);
+/* HalfSpace::computeFrictionEnergy / augmentFrictionGradient / augmentFrictionHessian (HalfSpace.cpp:272-380, coef 1.0 as Optimizer.cpp:3361
+ * passes it) against result.V_prev (ipcgpu_set_prev_state); eps2 = fricDHat.  Outputs as in the barrier calls above. */
+int ipcgpu_halfspace_friction_energy(ipcgpu_ctx* ctx, double eps2, double* E);
+int ipcgpu_halfspace_friction_gradient(ipcgpu_ctx* ctx, double eps2, double* g_inout);
+int ipcgpu_halfspace_friction_hessian(ipcgpu_ctx* ctx, double eps2, int projectDBC, double* a_inout);
+/* copies of the active set (plane, vertex interleaved), the lagged set and its lambda (activeSet / activeSet_lastH / lambda_lastH, split by
+ * plane); any pointer may be NULL (call once with NULL arrays for the sizes) */
+int ipcgpu_get_halfspace_sets(ipcgpu_ctx* ctx, int* n_active, int* active2, int* n_lagged, int* lagged2, double* lambda);
 
 /* diagnostics of the last narrow phase: candidates tested, pairs surviving the root box, conservative early-outs (should be 0) */
 int ipcgpu_ccd_stats(ipcgpu_ctx* ctx, uint64_t* candidates, uint64_t* survivors, uint64_t* warnings);

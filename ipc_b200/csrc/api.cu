@@ -9,6 +9,7 @@
 #include "context.h"
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstring>
 #include <dlfcn.h>
 #include <numeric>
@@ -107,9 +108,10 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 // short latency-bound kernels and the Tight-Inclusion passes, the critical path).  The first derivative call in its NULL-output form
 // forks the low-priority stream `deriv` off the main stream; the step-bound calls keep running on the high-priority main stream next
 // to it.  While `deriv` is open only these entry points may run:
-//   - ipcgpu_step_bound_set, ipcgpu_inversion_step, ipcgpu_ccd_partial_ti, ipcgpu_hash_build_swept, ipcgpu_ccd_full_ti with every host
-//     argument NULL (a host search direction rewrites `dir`, a host step reads back);
-//   - the derivative calls in their NULL-output form (they enqueue on `deriv`);
+//   - ipcgpu_step_bound_set, ipcgpu_inversion_step, ipcgpu_halfspace_step, ipcgpu_ccd_partial_ti, ipcgpu_hash_build_swept, ipcgpu_ccd_full_ti
+//     with every host argument NULL (a host search direction rewrites `dir`, a host step reads back);
+//   - the derivative calls in their NULL-output form (they enqueue on `deriv`), among them ipcgpu_halfspace_gradient / _hessian and
+//     ipcgpu_halfspace_friction_gradient / _hessian;
 //   - ipcgpu_allreduce_grad_hess on one rank (a no-op), and ipcgpu_download_range_async, whose copy waits on `deriv` as well.
 // Every other entry point that touches the device calls enter(ctx, kSerial) first, which joins `deriv` into the main stream (the pure
 // host-side getters need not).  Among them ipcgpu_update_pattern: it rewrites ia, ja and slot_off, which the derivative chain reads, so it
@@ -128,6 +130,10 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 //   - contact lists: the barrier kernels read act / para / para_e (written by the constraint set before the fork); the step-bound chain
 //     reads ContactWork::cand and writes only the CcdWork buffers (among them the swept grid: cells, sw_keys, sw_ent, sw_cnt, sw_off,
 //     sw_tmp), which the derivative chain does not touch.
+//   - half-space planes: the plane constraint set, lag, energies and crossing check are kSerial (they write hs_act, hs_lag, hs_lam, hs_cnt,
+//     hs_pstart and IterState::hs_energy, hs_n_*, hs_crossings); the plane derivative calls read hs_par, hs_act, hs_lag, hs_lam, hs_cnt,
+//     Vprev (written before the fork) and write g / a only; ipcgpu_halfspace_step reads hs_par, SVI, dir and writes IterState::step_ord,
+//     hs_alpha, hs_zero_step only (the derivative chain touches none of them).
 //   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, hcon, e_partials2, scalar_out[0], bHraw, brows,
 //     bpsd: derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };
@@ -480,7 +486,7 @@ int ipcgpu_create(int device, ipcgpu_ctx** out)
         || cudaStreamCreateWithPriority(&ctx->deriv, cudaStreamNonBlocking, ctx->prio_low) != cudaSuccess
         || cudaEventCreateWithFlags(&ctx->ev_deriv_fork, cudaEventDisableTiming) != cudaSuccess
         || cudaEventCreateWithFlags(&ctx->ev_deriv_done, cudaEventDisableTiming) != cudaSuccess || cudaMallocHost(&ctx->h_scalar, 512) != cudaSuccess
-        || cudaMallocHost(&hi, sizeof(IterState)) != cudaSuccess || !ctx->flag.reserve(4) || !ctx->scalar_out.reserve(32) || !ctx->iter.reserve(1)
+        || cudaMallocHost(&hi, sizeof(IterState)) != cudaSuccess || !ctx->flag.reserve(4) || !ctx->scalar_out.reserve(40) || !ctx->iter.reserve(1)
         || cudaMemsetAsync(ctx->iter.p, 0, sizeof(IterState), ctx->stream) != cudaSuccess) {
         ipcgpu_destroy(ctx);
         return IPCGPU_ERR_CUDA;
@@ -620,6 +626,7 @@ int ipcgpu_set_mesh(ipcgpu_ctx* ctx, int nV, int nT, const double* Vrest, const 
     ctx->nV = nV;
     ctx->nT = nT;
     ctx->energy = energy;
+    ctx->hs_set_built = ctx->hs_lag_ready = false; // the plane sets index the old vertices
     ctx->nVdof = 0x7fffffff; // a new mesh has no obstacle tail until ipcgpu_set_obstacle_tail names one
     ctx->h_T.assign(tets, tets + (size_t)4 * nT);
     ctx->h_ia.clear();
@@ -994,6 +1001,7 @@ int ipcgpu_set_surface(ipcgpu_ctx* ctx, int nSV, const int* SVI, int nSE, const 
     if (vCoDim) REQUIRE(ctx->vCoDim.upload(vCoDim, ctx->nV, ctx->stream), IPCGPU_ERR_CUDA, "codim upload failed");
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->h_SVI.assign(SVI, SVI + nSV);
+    ctx->hs_set_built = ctx->hs_lag_ready = false; // the plane sets index the old surface (and halfspace_alloc may reallocate them)
     ctx->pSize_surface = false; // pSize belongs to the surface
     int rc = contact_alloc(ctx);
     if (rc) return rc;
@@ -1831,6 +1839,323 @@ int ipcgpu_inertia_gradient(ipcgpu_ctx* ctx, int projectDBC, double* g_inout)
     return IPCGPU_OK;
 }
 
+// ---- analytic half-space collision objects (halfspace.cu; which chain each call runs on: see enter()) ------------------------------------
+static HalfSpaceArgs halfspace_args(ipcgpu_ctx* ctx)
+{
+    HalfSpaceArgs p;
+    p.nV = ctx->nV; p.nSV = ctx->nSV; p.nP = ctx->n_hs;
+    p.SVI = ctx->SVI.p; p.V = ctx->V.p; p.Vt = ctx->Vprev.p;
+    p.dbc = ctx->has_dbc ? ctx->dbc.p : nullptr; p.vCoDim = ctx->has_codim ? ctx->vCoDim.p : nullptr;
+    p.par = ctx->hs_par.p;
+    p.act = ctx->hs_act.p; p.n_act = ctx->hs_cnt.p;
+    p.lag = ctx->hs_lag.p; p.lam = ctx->hs_lam.p; p.n_lag = ctx->hs_cnt.p + 1;
+    p.row_lo = ctx->nranks > 1 ? ctx->v_begin : 0;
+    p.row_hi = ctx->nranks > 1 ? ctx->v_end : ctx->nV;
+    p.ia = ctx->ia.p; p.base = ctx->index_base;
+    return p;
+}
+
+int ipcgpu_set_halfspaces(ipcgpu_ctx* ctx, int n, const double* origin, const double* normal, const double* velocitydt, const double* friction)
+{
+    REQUIRE(n >= 0 && n <= kMaxPlanes, IPCGPU_ERR_ARG, "at most 8 half-spaces");
+    REQUIRE(n == 0 || (origin && normal && friction), IPCGPU_ERR_ARG, "null half-space arrays");
+    REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    std::vector<double> par((size_t)kPlaneStride * std::max(n, 1), 0.0);
+    for (int k = 0; k < n; ++k) {
+        const double* o = origin + 3 * k;
+        const double* nr = normal + 3 * k;
+        const double z = (nr[0] * nr[0] + nr[1] * nr[1]) + nr[2] * nr[2]; // normal.normalize() (HalfSpace.cpp:49)
+        REQUIRE(z > 0.0, IPCGPU_ERR_ARG, "half-space normal is zero");
+        const double s = std::sqrt(z);
+        double* q = par.data() + kPlaneStride * k;
+        for (int r = 0; r < 3; ++r) q[r] = nr[r] / s;
+        q[3] = -((q[0] * o[0] + q[1] * o[1]) + q[2] * o[2]); // D = -normal.dot(origin) (:51)
+        for (int r = 0; r < 3; ++r) q[4 + r] = velocitydt ? velocitydt[3 * k + r] : 0.0;
+        q[7] = friction[k];
+    }
+    if (n != ctx->n_hs) {
+        ++ctx->epoch; // the graphs captured with the old number of planes are refused (launch shapes and calls change)
+        ctx->hs_set_built = ctx->hs_lag_ready = false;
+        CK(cudaMemsetAsync(&ctx->iter.p->hs_energy[0], 0, offsetof(IterState, pat_nnz) - offsetof(IterState, hs_energy), ctx->stream));
+    }
+    ctx->n_hs = n;
+    if (n > 0) {
+        ALLOC(ctx->hs_par, (size_t)kPlaneStride * kMaxPlanes);
+        CK(cudaMemcpyAsync(ctx->hs_par.p, par.data(), par.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    CK(cudaStreamSynchronize(ctx->stream)); // `par` lives on this stack
+    return IPCGPU_OK;
+}
+
+// allocations sized by the surface (lazy: the first call after ipcgpu_set_surface, which refuses older graphs, must run outside a capture)
+static int halfspace_alloc(ipcgpu_ctx* ctx)
+{
+    const size_t n = (size_t)kMaxPlanes * std::max(ctx->nSV, 1);
+    ALLOC(ctx->hs_flags, n);
+    ALLOC(ctx->hs_offs, n);
+    ALLOC(ctx->hs_act, n);
+    ALLOC(ctx->hs_lag, n);
+    ALLOC(ctx->hs_lam, n);
+    ALLOC(ctx->hs_cnt, 2);
+    ALLOC(ctx->hs_pstart, kMaxPlanes + 1);
+    ALLOC(ctx->hs_partials, (size_t)halfspace_energy_blocks() + 8);
+    // the scan's temporary storage grows with its length (decoupled look-back tile state): sized for the scan this surface and this number of
+    // planes run, at every call (a host-only query), and the size handed to cub is that one
+    ctx->hs_scan_bytes = halfspace_scan_bytes(ctx->n_hs * ctx->nSV);
+    ALLOC(ctx->hs_scan, ctx->hs_scan_bytes);
+    return IPCGPU_OK;
+}
+
+static int halfspace_sync_counts(ipcgpu_ctx* ctx)
+{
+    CK(cudaMemcpyAsync(ctx->h_scalar + 44, ctx->hs_cnt.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IPCGPU_OK;
+}
+
+int ipcgpu_halfspace_constraint_set(ipcgpu_ctx* ctx, double dHat, int* n_active)
+{
+    if (n_active) *n_active = 0;
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE(ctx->surface_ready && ctx->nSV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_surface with surface vertices first");
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    int rc = halfspace_alloc(ctx);
+    if (rc) return rc;
+    const HalfSpaceArgs p = halfspace_args(ctx);
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_CONSTRAINT_SET);
+    CK(halfspace_active_set(p, dHat, ctx->hs_flags.p, ctx->hs_offs.p, ctx->hs_scan.p, ctx->hs_scan_bytes, ctx->hs_act.p, ctx->hs_cnt.p, ctx->hs_pstart.p,
+        ctx->iter.p, ctx->stream));
+    ctx->prof_end(pe);
+    ctx->launches += 3;
+    ctx->hs_set_built = true;
+    ctx->mark_inputs();
+    if (n_active) {
+        if ((rc = halfspace_sync_counts(ctx))) return rc;
+        *n_active = reinterpret_cast<int*>(ctx->h_scalar + 44)[0];
+    }
+    return IPCGPU_OK;
+}
+
+#define REQUIRE_HS_SET() REQUIRE(ctx->hs_set_built, IPCGPU_ERR_STATE, "ipcgpu_halfspace_constraint_set first")
+
+int ipcgpu_halfspace_energy(ipcgpu_ctx* ctx, double dHat, double kappa, double* E)
+{
+    if (E) *E = 0.0;
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE_HS_SET();
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    const HalfSpaceArgs p = halfspace_args(ctx);
+    double* out = &ctx->iter.p->hs_energy[0];
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
+    halfspace_energy(p, dHat, ctx->hs_partials.p, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE], ctx->stream);
+    reduce_sum(ctx->hs_partials.p, halfspace_energy_blocks(), kappa, out, ctx->stream);
+    ctx->prof_end(pe);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    ctx->hs_local[0] = ctx->nranks > 1 && !E;
+    if (!E) return IPCGPU_OK;
+    if (ctx->nranks > 1) {
+        int r = g_nccl.AllReduce(out, out, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
+        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(half-space energy) failed");
+    }
+    int rc = fetch_iter_state(ctx);
+    if (rc) return rc;
+    *E = ctx->h_iter->hs_energy[0];
+    if (ctx->h_iter->flags[FLAG_NONPOSITIVE_DISTANCE]) {
+        clear_flag(ctx, FLAG_NONPOSITIVE_DISTANCE);
+        int only[8] = { 0 };
+        only[FLAG_NONPOSITIVE_DISTANCE] = 1;
+        return status_from_flags(ctx, only);
+    }
+    return IPCGPU_OK;
+}
+
+} // extern "C"
+
+// NULL output: the term on the derivative chain; host output: the caller's vector in, the term added on the main stream, the (rank-summed)
+// vector out
+template <typename Launch>
+static int halfspace_gradient_call(ipcgpu_ctx* ctx, double* g_inout, Launch launch)
+{
+    CK(cudaSetDevice(ctx->device));
+    ENTER(g_inout ? kSerial : kDerivative);
+    int rc;
+    if (g_inout && (rc = gradient_roundtrip_begin(ctx, g_inout))) return rc;
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
+    launch(ctx->deriv_stream());
+    ctx->prof_end(pe);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    return g_inout ? gradient_roundtrip_end(ctx, g_inout) : IPCGPU_OK;
+}
+template <typename Launch>
+static int halfspace_hessian_call(ipcgpu_ctx* ctx, double* a_inout, Launch launch)
+{
+    REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
+    CK(cudaSetDevice(ctx->device));
+    ENTER(a_inout ? kSerial : kDerivative);
+    int rc;
+    if (a_inout && (rc = upload_values(ctx, a_inout))) return rc;
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
+    launch(ctx->deriv_stream());
+    ctx->prof_end(pe);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    return a_inout ? download_values(ctx, a_inout) : IPCGPU_OK;
+}
+
+extern "C" {
+
+int ipcgpu_halfspace_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* g_inout)
+{
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE_HS_SET();
+    const HalfSpaceArgs p = halfspace_args(ctx);
+    return halfspace_gradient_call(ctx, g_inout, [&](cudaStream_t st) { halfspace_gradient(p, dHat, kappa, ctx->g.p, st); });
+}
+
+int ipcgpu_halfspace_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC, double* a_inout)
+{
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE_HS_SET();
+    const HalfSpaceArgs p = halfspace_args(ctx);
+    return halfspace_hessian_call(ctx, a_inout, [&](cudaStream_t st) { halfspace_hessian(p, dHat, kappa, projectDBC, ctx->a.p, st); });
+}
+
+int ipcgpu_halfspace_step(ipcgpu_ctx* ctx, const double* p_dir, double slackness, double* alpha_inout)
+{
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    CK(cudaSetDevice(ctx->device));
+    ENTER(p_dir || alpha_inout ? kSerial : kStepBound);
+    int rc = upload_dir(ctx, p_dir);
+    if (rc) return rc;
+    if (alpha_inout && (rc = ipcgpu_step_bound_set(ctx, *alpha_inout))) return rc;
+    halfspace_step(halfspace_args(ctx), ctx->dir.p, slackness, ctx->iter.p, ctx->stream);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    if (!alpha_inout) return IPCGPU_OK;
+    if ((rc = ccd_read_back(ctx, alpha_inout))) return rc;
+    if (ctx->h_iter->hs_zero_step) {
+        CK(cudaMemsetAsync(&ctx->iter.p->hs_zero_step, 0, sizeof(int), ctx->stream));
+        ctx->err = "step 0: a vertex is at or behind a half-space and moves further into it (Optimizer.cpp:2031-2033 would exit(-1))";
+        return IPCGPU_ERR_LINE_SEARCH;
+    }
+    return IPCGPU_OK;
+}
+
+int ipcgpu_halfspace_crossings(ipcgpu_ctx* ctx, int* n)
+{
+    if (n) *n = 0;
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    halfspace_crossings(halfspace_args(ctx), ctx->iter.p, ctx->stream);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    ctx->hs_local[2] = ctx->nranks > 1 && !n;
+    if (!n) return IPCGPU_OK;
+    if (ctx->nranks > 1) {
+        int r = g_nccl.AllReduce(&ctx->iter.p->hs_crossings, &ctx->iter.p->hs_crossings, 1, kNcclInt32, kNcclSum, ctx->nccl_comm, ctx->stream);
+        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(half-space crossings) failed");
+    }
+    int rc = fetch_iter_state(ctx);
+    if (rc) return rc;
+    *n = ctx->h_iter->hs_crossings;
+    return IPCGPU_OK;
+}
+
+int ipcgpu_halfspace_friction_lag(ipcgpu_ctx* ctx, double dHat, double kappa, int* n_lagged)
+{
+    if (n_lagged) *n_lagged = 0;
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE_HS_SET();
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    halfspace_lag(halfspace_args(ctx), dHat, kappa, ctx->hs_pstart.p, ctx->hs_lag.p, ctx->hs_lam.p, ctx->hs_cnt.p + 1, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE],
+        ctx->iter.p, ctx->stream);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    ctx->hs_lag_ready = true;
+    if (n_lagged) {
+        int rc = halfspace_sync_counts(ctx);
+        if (rc) return rc;
+        *n_lagged = reinterpret_cast<int*>(ctx->h_scalar + 44)[1];
+    }
+    return IPCGPU_OK;
+}
+
+#define REQUIRE_HS_LAG()                                                                                            \
+    REQUIRE(ctx->hs_lag_ready, IPCGPU_ERR_STATE, "ipcgpu_halfspace_friction_lag first");                          \
+    REQUIRE(ctx->prev_set, IPCGPU_ERR_STATE, "ipcgpu_set_prev_state first");                                       \
+    REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive")
+
+int ipcgpu_halfspace_friction_energy(ipcgpu_ctx* ctx, double eps2, double* E)
+{
+    if (E) *E = 0.0;
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE_HS_LAG();
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    double* out = &ctx->iter.p->hs_energy[1];
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
+    halfspace_friction_energy(halfspace_args(ctx), eps2, ctx->hs_partials.p, ctx->stream);
+    reduce_sum(ctx->hs_partials.p, halfspace_energy_blocks(), 1.0, out, ctx->stream);
+    ctx->prof_end(pe);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    ctx->hs_local[1] = ctx->nranks > 1 && !E;
+    if (!E) return IPCGPU_OK;
+    if (ctx->nranks > 1) {
+        int r = g_nccl.AllReduce(out, out, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
+        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(half-space friction energy) failed");
+    }
+    int rc = fetch_iter_state(ctx);
+    if (rc) return rc;
+    *E = ctx->h_iter->hs_energy[1];
+    return IPCGPU_OK;
+}
+
+int ipcgpu_halfspace_friction_gradient(ipcgpu_ctx* ctx, double eps2, double* g_inout)
+{
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE_HS_LAG();
+    const HalfSpaceArgs p = halfspace_args(ctx);
+    return halfspace_gradient_call(ctx, g_inout, [&](cudaStream_t st) { halfspace_friction_gradient(p, eps2, ctx->g.p, st); });
+}
+
+int ipcgpu_halfspace_friction_hessian(ipcgpu_ctx* ctx, double eps2, int projectDBC, double* a_inout)
+{
+    if (ctx->n_hs == 0) return IPCGPU_OK;
+    REQUIRE_HS_LAG();
+    const HalfSpaceArgs p = halfspace_args(ctx);
+    return halfspace_hessian_call(ctx, a_inout, [&](cudaStream_t st) { halfspace_friction_hessian(p, eps2, projectDBC, ctx->a.p, st); });
+}
+
+int ipcgpu_get_halfspace_sets(ipcgpu_ctx* ctx, int* n_active, int* active2, int* n_lagged, int* lagged2, double* lambda)
+{
+    if (n_active) *n_active = 0;
+    if (n_lagged) *n_lagged = 0;
+    if (ctx->n_hs == 0 || !ctx->hs_set_built) return IPCGPU_OK;
+    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
+    int rc = halfspace_sync_counts(ctx);
+    if (rc) return rc;
+    const int* h = reinterpret_cast<int*>(ctx->h_scalar + 44);
+    const size_t na = (size_t)h[0], nl = ctx->hs_lag_ready ? (size_t)h[1] : 0;
+    if (n_active) *n_active = (int)na;
+    if (n_lagged) *n_lagged = (int)nl;
+    if (na && active2) CK(cudaMemcpyAsync(active2, ctx->hs_act.p, na * sizeof(int2), cudaMemcpyDeviceToHost, ctx->stream));
+    if (nl && lagged2) CK(cudaMemcpyAsync(lagged2, ctx->hs_lag.p, nl * sizeof(int2), cudaMemcpyDeviceToHost, ctx->stream));
+    if (nl && lambda) CK(cudaMemcpyAsync(lambda, ctx->hs_lam.p, nl * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IPCGPU_OK;
+}
+
 // ---- CUDA graphs of device-resident call sequences ----------------------------------------------------------------------------
 // An iteration in the NULL-output form is ~65 launches whose arguments do not change while the scene, the pattern, dHat / kappa and
 // the tolerances stay the same: positions, search direction, list sizes and step bounds all live in device memory.  Enqueued one by
@@ -1849,6 +2174,9 @@ static ipcgpu_ctx::HostState snapshot_host_state(const ipcgpu_ctx* ctx)
     h.inputs_marked = false; // events recorded inside a capture cannot be waited on outside of it
     h.scatter_marked = false;
     h.nC = ctx->cw.nC; h.nP = ctx->cw.nP; h.nK = ctx->cw.nK; h.fr_host_n = ctx->cw.fr_host_n;
+    for (int s = 0; s < 3; ++s) h.hs_local[s] = ctx->hs_local[s];
+    h.hs_set_built = ctx->hs_set_built;
+    h.hs_lag_ready = ctx->hs_lag_ready;
     return h;
 }
 static void apply_host_state(ipcgpu_ctx* ctx, const ipcgpu_ctx::HostState& h)
@@ -1863,6 +2191,9 @@ static void apply_host_state(ipcgpu_ctx* ctx, const ipcgpu_ctx::HostState& h)
     ctx->inputs_marked = h.inputs_marked;
     ctx->scatter_marked = h.scatter_marked;
     ctx->cw.nC = h.nC; ctx->cw.nP = h.nP; ctx->cw.nK = h.nK; ctx->cw.fr_host_n = h.fr_host_n;
+    for (int s = 0; s < 3; ++s) ctx->hs_local[s] = h.hs_local[s];
+    ctx->hs_set_built = h.hs_set_built;
+    ctx->hs_lag_ready = h.hs_lag_ready;
 }
 
 int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
@@ -2168,14 +2499,37 @@ int ipcgpu_ccd_cfl_ti(ipcgpu_ctx* ctx, double dHat, int first_iteration, double 
     return alpha_inout ? step_control_host_result(ctx, alpha_inout) : IPCGPU_OK;
 }
 
-// one trial's energy: E_el, E_in, E_b, E_f into IterState::energy (summed by the decision that reads them)
+// the energy terms of a line search: with planes set, their barrier energy, and their friction when fricDHat > 0 and a lagged plane set exists
+// (Optimizer.cpp:3355-3365)
+static int ls_terms(const ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
+{
+    int terms = (t.inertia ? kTermInertia : 0) | (t.fric_coef > 0.0 ? kTermFriction : 0);
+    if (ctx->n_hs > 0) terms |= kTermHalfSpace;
+    if (ctx->n_hs > 0 && ctx->hs_lag_ready && t.fric_eps2 > 0.0) terms |= kTermHalfSpaceFriction;
+    return terms;
+}
+// one trial's energy: E_el, E_in, E_b, E_f (and the planes' terms) into IterState (summed by the decision that reads them)
 static int ls_energy(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
 {
+    const int terms = ls_terms(ctx, t);
     int rc = ipcgpu_elastic_energy(ctx, t.elastic_coef, 1, nullptr);
     if (!rc && t.inertia) rc = ipcgpu_inertia_energy(ctx, nullptr);
     if (!rc) rc = ipcgpu_barrier_energy(ctx, t.dHat, t.kappa, nullptr);
+    if (!rc && (terms & kTermHalfSpace)) rc = ipcgpu_halfspace_energy(ctx, t.dHat, t.kappa, nullptr);
+    if (!rc && (terms & kTermHalfSpaceFriction)) rc = ipcgpu_halfspace_friction_energy(ctx, t.fric_eps2, nullptr);
     if (!rc && t.fric_coef > 0.0) rc = ipcgpu_friction_energy(ctx, t.fric_eps2, t.fric_coef, nullptr);
     return rc;
+}
+// a trial's constraint sets: the self-contact set and the planes' (isIntersected and computeConstraintSet cover every collision object)
+static int ls_constraint_set(ipcgpu_ctx* ctx, double dHat)
+{
+    int rc = ipcgpu_constraint_set(ctx, dHat, 1, nullptr, nullptr, nullptr);
+    return rc ? rc : ipcgpu_halfspace_constraint_set(ctx, dHat, nullptr);
+}
+static int ls_intersection(ipcgpu_ctx* ctx)
+{
+    int rc = ipcgpu_intersection_free(ctx, nullptr);
+    return rc ? rc : ipcgpu_halfspace_crossings(ctx, nullptr);
 }
 // V = V0 + alpha p with the device-resident step
 static int ls_step(ipcgpu_ctx* ctx)
@@ -2189,7 +2543,7 @@ static int ls_step(ipcgpu_ctx* ctx)
 
 static int line_search_body(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
 {
-    const int terms = (t.inertia ? kTermInertia : 0) | (t.fric_coef > 0.0 ? kTermFriction : 0);
+    const int terms = ls_terms(ctx, t);
     CK(cudaMemcpyAsync(ctx->Vsaved.p, ctx->V.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream)); // :2692
     ctx->state_saved = true;
     int rc = ls_energy(ctx, t); // :2681
@@ -2202,25 +2556,25 @@ static int line_search_body(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
             return r ? r : ipcgpu_check_inversion(ctx, nullptr);
         });
     }
-    if (!rc) rc = ipcgpu_intersection_free(ctx, nullptr); // :2720
-    if (!rc) rc = cond_node(ctx, true, kLsIntersection, 0.0, 0, [&]() {
+    if (!rc) rc = ls_intersection(ctx); // :2720
+    if (!rc) rc = cond_node(ctx, true, kLsIntersection, 0.0, terms, [&]() {
         int r = ls_step(ctx);
-        return r ? r : ipcgpu_intersection_free(ctx, nullptr);
+        return r ? r : ls_intersection(ctx);
     });
-    if (!rc) rc = ipcgpu_constraint_set(ctx, t.dHat, 1, nullptr, nullptr, nullptr); // :2741
-    if (!rc) rc = ls_energy(ctx, t);                                                 // :2744
+    if (!rc) rc = ls_constraint_set(ctx, t.dHat); // :2741
+    if (!rc) rc = ls_energy(ctx, t);              // :2744
     if (!rc) rc = cond_node(ctx, true, kLsArmijo, 0.0, terms, [&]() {
         int r = ls_step(ctx);
-        if (!r) r = ipcgpu_constraint_set(ctx, t.dHat, 1, nullptr, nullptr, nullptr);
+        if (!r) r = ls_constraint_set(ctx, t.dHat);
         return r ? r : ls_energy(ctx, t);
     });
     if (!rc) rc = cond_node(ctx, false, kLsPostCheck, 0.0, 0, [&]() {
-        int r = ipcgpu_intersection_free(ctx, nullptr);
-        if (!r) r = cond_node(ctx, true, kLsPostLoop, 0.0, 0, [&]() {
+        int r = ls_intersection(ctx);
+        if (!r) r = cond_node(ctx, true, kLsPostLoop, 0.0, terms, [&]() {
             int q = ls_step(ctx);
-            return q ? q : ipcgpu_intersection_free(ctx, nullptr);
+            return q ? q : ls_intersection(ctx);
         });
-        if (!r) r = cond_node(ctx, false, kLsRebuild, 0.0, 0, [&]() { return ipcgpu_constraint_set(ctx, t.dHat, 1, nullptr, nullptr, nullptr); });
+        if (!r) r = cond_node(ctx, false, kLsRebuild, 0.0, 0, [&]() { return ls_constraint_set(ctx, t.dHat); });
         return r;
     });
     return rc;
@@ -2233,6 +2587,8 @@ int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* t, doubl
     REQUIRE(!t->inertia || (ctx->xtilde_set && ctx->has_mass), IPCGPU_ERR_STATE, "inertia: ipcgpu_set_xtilde and a mass diagonal first");
     REQUIRE(!(t->fric_coef > 0.0) || (ctx->cw.fr_ready && ctx->prev_set && t->fric_eps2 > 0.0), IPCGPU_ERR_STATE,
         "friction: ipcgpu_friction_lag, ipcgpu_set_prev_state and fric_eps2 > 0 first");
+    REQUIRE(ctx->n_hs == 0 || ctx->hs_set_built, IPCGPU_ERR_STATE, "half-spaces: ipcgpu_halfspace_constraint_set first (E0 takes the sets held on entry)");
+    REQUIRE(!(ls_terms(ctx, *t) & kTermHalfSpaceFriction) || ctx->prev_set, IPCGPU_ERR_STATE, "half-space friction: ipcgpu_set_prev_state first");
     REQUIRE(!(ctx->capturing && ctx->canonical_order), IPCGPU_ERR_STATE, "inside a capture the line search needs ipcgpu_set_canonical_order(ctx, 0)");
     CK(cudaSetDevice(ctx->device));
     int rc = step_control_prepare(ctx);
@@ -2352,15 +2708,21 @@ int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
         for (int s = 0; s < 4; ++s)
             if (ctx->energy_local[s]) mask |= 1u << s;
         if (ctx->checks_local) mask |= 1u << 4;
+        unsigned hs_mask = 0; // with planes: their energies and crossing count ride in the same collective, 3 doubles behind the 14
+        for (int s = 0; s < 3; ++s)
+            if (ctx->n_hs > 0 && ctx->hs_local[s]) hs_mask |= 1u << s;
         cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_ALLREDUCE);
         pack_scalars(ctx->iter.p, mask, ctx->scalar_out.p + 16, ctx->stream);
-        int r = g_nccl.AllReduce(ctx->scalar_out.p + 16, ctx->scalar_out.p + 16, 14, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
+        if (ctx->n_hs > 0) halfspace_pack(ctx->iter.p, hs_mask, ctx->scalar_out.p + 30, ctx->stream);
+        int r = g_nccl.AllReduce(ctx->scalar_out.p + 16, ctx->scalar_out.p + 16, ctx->n_hs > 0 ? 17 : 14, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
         unpack_scalars(ctx->iter.p, mask, ctx->scalar_out.p + 16, ctx->stream);
+        if (ctx->n_hs > 0) halfspace_unpack(ctx->iter.p, hs_mask, ctx->scalar_out.p + 30, ctx->stream);
         ctx->prof_end(pe);
-        ctx->launches += 2;
+        ctx->launches += ctx->n_hs > 0 ? 4 : 2;
         REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(iteration scalars) failed");
         for (int s = 0; s < 4; ++s) ctx->energy_local[s] = false;
     }
+    for (int s = 0; s < 3; ++s) ctx->hs_local[s] = false;
     ctx->checks_local = false;
     int rc = ccd_read_back(ctx, nullptr);
     if (rc || (rc = refresh_pattern_mirror(ctx))) return rc;
@@ -2381,11 +2743,21 @@ int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
     out->ti_warnings = (uint64_t)h.flags[FLAG_TI_WARNINGS];
     out->n_inverted_tets = h.checks[0];
     out->n_intersected_triangles = h.checks[1];
+    out->energy_halfspace = h.hs_energy[0];
+    out->energy_halfspace_friction = h.hs_energy[1];
+    out->alpha_halfspace = h.hs_alpha;
+    out->n_halfspace_active = h.hs_n_active;
+    out->n_halfspace_crossings = h.hs_crossings;
     ContactWork& w = ctx->cw;
     w.nC = h.n_set[0]; w.nP = h.n_set[1]; w.nK = h.n_set[2];
-    const int status = status_from_flags(ctx, h.flags);
+    int status = status_from_flags(ctx, h.flags);
+    if (status == IPCGPU_OK && h.hs_zero_step) {
+        ctx->err = "step 0: a vertex is at or behind a half-space and moves further into it (Optimizer.cpp:2031-2033 would exit(-1))";
+        status = IPCGPU_ERR_LINE_SEARCH;
+    }
     out->status = status;
     CK(cudaMemsetAsync(ctx->iter.p->flags, 0, 8 * sizeof(int), ctx->stream)); // flags are per fetch
+    if (h.hs_zero_step) CK(cudaMemsetAsync(&ctx->iter.p->hs_zero_step, 0, sizeof(int), ctx->stream));
     if (h.grid_axis_cells > 0) { // sort width of the next iteration's grid builds: enough bits for 1.5x the cells this one wanted
         int bits = 3;
         while (bits < 10 && (1 << bits) - 2 < (h.grid_axis_cells * 3) / 2 + 2) ++bits;

@@ -190,6 +190,16 @@ struct ipcgpu_ctx {
     bool partition_contact = false, lists_local = false; // multi-rank: build only this rank's share of the contact sets
     ipcgpu::ContactWork cw;
     ipcgpu::CcdWork ccd;
+    // half-space collision objects (halfspace.cu, ipcgpu_set_halfspaces): parameters, flags / scan of the (plane, SVI index) range, active and
+    // lagged (plane, vertex) lists, per-plane starts of the active list, energy partials
+    int n_hs = 0;
+    ipcgpu::DevBuf<double> hs_par, hs_lam, hs_partials;
+    ipcgpu::DevBuf<int> hs_flags, hs_offs, hs_cnt, hs_pstart; // hs_cnt: [0] active, [1] lagged
+    ipcgpu::DevBuf<int2> hs_act, hs_lag;
+    ipcgpu::DevBuf<unsigned char> hs_scan;
+    size_t hs_scan_bytes = 0;
+    bool hs_set_built = false, hs_lag_ready = false;
+    bool hs_local[3] = { false, false, false }; // IterState::hs_energy[0], [1], hs_crossings still hold this rank's share
     size_t ccd_capacity = (size_t)1 << 23; // candidate pairs
     std::vector<int> h_SVI;                // host copy (pSize of the swept build is a serial host sum, SpatialHash.hpp:603-612)
     double debug_prune_seed = -1.0;        // test hook, see ipcgpu_ccd_debug_seed_bound
@@ -232,6 +242,7 @@ struct ipcgpu_ctx {
     // capture and re-applied at every replay.  `epoch` is bumped by every call that may reallocate or re-partition: older graphs are refused.
     struct HostState {
         bool energy_local[4], checks_local, lists_local, lists_global, want_cand, swept_ready, fr_ready, inputs_marked, scatter_marked;
+        bool hs_local[3], hs_set_built, hs_lag_ready;
         int nC, nP, nK, fr_host_n;
     };
     struct GraphRec {

@@ -34,6 +34,12 @@ struct IterState {
     int ls_count[4];                  // halvings: inversion guard, intersection pre-check, Armijo loop, post-check
     int ls_stopped, ls_rebuilt, ls_post_ran;
     int ls_cond;                      // the decision word of the last step_decide
+    // half-space collision objects (halfspace.cu)
+    double hs_energy[2];              // barrier, friction of the planes (this rank's share, then sums)
+    double hs_alpha;                  // step after the plane bound
+    int hs_n_active, hs_n_lagged;     // sizes of the plane active set / lagged set (replicated on every rank)
+    int hs_crossings;                 // vertices with d <= 0 of the last crossing check (this rank's share, then sums)
+    int hs_zero_step;                 // the plane bound (or the step entering it) was 0; cleared by ipcgpu_fetch_iteration
     // device-built sparsity pattern (pattern.cu): result of the last ipcgpu_update_pattern and its per-update control words
     long long pat_nnz;                // nnz of the pattern in ia / ja
     unsigned long long pat_version;   // bumped by every update that rewrote the pattern
@@ -44,7 +50,7 @@ struct IterState {
 };
 // step_decide operations (step_control.cu) and the energy terms of a line search
 enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersection, kLsArmijo, kLsPostCheck, kLsPostLoop, kLsRebuild };
-enum { kTermInertia = 1, kTermFriction = 2 };
+enum { kTermInertia = 1, kTermFriction = 2, kTermHalfSpace = 4, kTermHalfSpaceFriction = 8 };
 enum { FLAG_NONPOSITIVE_DISTANCE = 0, FLAG_SET_CAPACITY = 1, FLAG_CCD_CAPACITY = 2, FLAG_ZERO_CCD_DISTANCE = 3, FLAG_PATTERN = 4, FLAG_TI_WARNINGS = 5, FLAG_EXCHANGE_CAPACITY = 6,
     FLAG_PATTERN_CAPACITY = 7 };
 
@@ -173,6 +179,39 @@ void step_decide(IterState* st_dev, int op, double a, int b, unsigned long long 
 int inertia_energy_blocks(int nV);
 void inertia_energy(int v0, int v1, int nV, const double* x_soa, const double* xtilde_soa, const double* mass, double* partials, cudaStream_t st);
 void inertia_gradient(int nV, const double* x_soa, const double* xtilde_soa, const double* mass, const uint8_t* dbc, int projectDBC, double* g, cudaStream_t st);
+// halfspace.cu -- analytic planes (HalfSpace<3>).  par: kPlaneStride doubles per plane [n0 n1 n2 D v0 v1 v2 mu]; act / lag: (plane, vertex)
+constexpr int kPlaneStride = 8;
+constexpr int kMaxPlanes = 8;
+struct HalfSpaceArgs {
+    int nV, nSV, nP;
+    const int* SVI;
+    const double* V;        // current positions (SoA)
+    const double* Vt;       // result.V_prev (SoA), friction only
+    const uint8_t* dbc;     // nullable
+    const int* vCoDim;      // nullable (=> 3)
+    const double* par;
+    const int2* act; const int* n_act;        // active set and its device-resident size
+    const int2* lag; const double* lam; const int* n_lag; // lagged set (friction planes only), lambda, size
+    int row_lo, row_hi;     // rows (energies, gradient, Hessian, crossings) this rank owns
+    const int* ia; int base;
+};
+int halfspace_energy_blocks();
+size_t halfspace_scan_bytes(int n);
+// n_act: the device-resident size the per-entry kernels read (also left in IterState::hs_n_active); pstart: first entry of each plane (nP + 1)
+cudaError_t halfspace_active_set(const HalfSpaceArgs& p, double dHat, int* flags, int* offs, void* scan_tmp, size_t scan_bytes, int2* act, int* n_act,
+    int* pstart, IterState* st_dev, cudaStream_t st);
+void halfspace_energy(const HalfSpaceArgs& p, double dHat, double* partials, int* bad, cudaStream_t st);
+void halfspace_gradient(const HalfSpaceArgs& p, double dHat, double kappa, double* g, cudaStream_t st);
+void halfspace_hessian(const HalfSpaceArgs& p, double dHat, double kappa, int projectDBC, double* a, cudaStream_t st);
+void halfspace_step(const HalfSpaceArgs& p, const double* dir, double slack, IterState* st_dev, cudaStream_t st);
+void halfspace_crossings(const HalfSpaceArgs& p, IterState* st_dev, cudaStream_t st);
+void halfspace_lag(const HalfSpaceArgs& p, double dHat, double kappa, const int* pstart, int2* lag, double* lam, int* n_lag, int* bad, IterState* st_dev, cudaStream_t st);
+void halfspace_friction_energy(const HalfSpaceArgs& p, double eps2, double* partials, cudaStream_t st);
+void halfspace_friction_gradient(const HalfSpaceArgs& p, double eps2, double* g, cudaStream_t st);
+void halfspace_friction_hessian(const HalfSpaceArgs& p, double eps2, int projectDBC, double* a, cudaStream_t st);
+void halfspace_pack(const IterState* st_dev, unsigned mask, double* buf, cudaStream_t st);   // 3 doubles behind pack_scalars' 14
+void halfspace_unpack(IterState* st_dev, unsigned mask, const double* buf, cudaStream_t st);
+
 // zero n_words 4-byte words.  A kernel rather than cudaMemsetAsync where the two chains of an iteration overlap (api.cu): replayed from a
 // graph, a memset node has no priority of its own and queues behind whatever low-priority grids are pending, which held the step-bound
 // chain up for the length of the CSR assembly

@@ -111,6 +111,18 @@ SIGNATURES = {
     "ipcgpu_ccd_cfl_ti": (C.c_int, [_ctxp, C.c_double, C.c_int, C.c_double, C.c_double, _dp, _dp, _dp]),
     "ipcgpu_line_search": (C.c_int, [_ctxp, C.c_void_p, _dp]),
     "ipcgpu_step_control_info": (C.c_int, [_ctxp, C.c_void_p]),
+    "ipcgpu_set_halfspaces": (C.c_int, [_ctxp, C.c_int, _dp, _dp, _dp, _dp]),
+    "ipcgpu_halfspace_constraint_set": (C.c_int, [_ctxp, C.c_double, _ip]),
+    "ipcgpu_halfspace_energy": (C.c_int, [_ctxp, C.c_double, C.c_double, _dp]),
+    "ipcgpu_halfspace_gradient": (C.c_int, [_ctxp, C.c_double, C.c_double, _dp]),
+    "ipcgpu_halfspace_hessian": (C.c_int, [_ctxp, C.c_double, C.c_double, C.c_int, _dp]),
+    "ipcgpu_halfspace_step": (C.c_int, [_ctxp, _dp, C.c_double, _dp]),
+    "ipcgpu_halfspace_crossings": (C.c_int, [_ctxp, _ip]),
+    "ipcgpu_halfspace_friction_lag": (C.c_int, [_ctxp, C.c_double, C.c_double, _ip]),
+    "ipcgpu_halfspace_friction_energy": (C.c_int, [_ctxp, C.c_double, _dp]),
+    "ipcgpu_halfspace_friction_gradient": (C.c_int, [_ctxp, C.c_double, _dp]),
+    "ipcgpu_halfspace_friction_hessian": (C.c_int, [_ctxp, C.c_double, C.c_int, _dp]),
+    "ipcgpu_get_halfspace_sets": (C.c_int, [_ctxp, _ip, _ip, _ip, _ip, _dp]),
 }
 
 STAGES = ["elastic_energy", "elastic_tet", "gather_gradient", "assemble_csr", "inversion", "hash", "constraint_set", "barrier",
@@ -124,7 +136,9 @@ class Iteration(C.Structure):
     _fields_ = [("energy_elastic", C.c_double), ("energy_barrier", C.c_double), ("alpha_inversion", C.c_double), ("alpha_partial_ccd", C.c_double),
                 ("alpha_swept_grid", C.c_double), ("alpha_full_ccd", C.c_double), ("alpha", C.c_double), ("n_active", C.c_int), ("n_mollified", C.c_int),
                 ("n_candidates", C.c_int), ("status", C.c_int), ("n_full_ccd_candidates", C.c_uint64), ("ti_warnings", C.c_uint64),
-                ("n_inverted_tets", C.c_int), ("n_intersected_triangles", C.c_int), ("energy_friction", C.c_double), ("energy_inertia", C.c_double)]
+                ("n_inverted_tets", C.c_int), ("n_intersected_triangles", C.c_int), ("energy_friction", C.c_double), ("energy_inertia", C.c_double),
+                ("energy_halfspace", C.c_double), ("energy_halfspace_friction", C.c_double), ("alpha_halfspace", C.c_double),
+                ("n_halfspace_active", C.c_int), ("n_halfspace_crossings", C.c_int)]
 
 
 class LineSearchTerms(C.Structure):
@@ -439,6 +453,73 @@ class Context:
     def inertia_gradient(self, projectDBC=1, g_inout=None):
         self._ck(self.lib.ipcgpu_inertia_gradient(self.h, projectDBC, _d(g_inout)))
         return g_inout
+
+    # ---- half-space collision objects (HalfSpace<3>) -----------------------------------------------
+    def set_halfspaces(self, origin, normal, velocitydt=None, friction=None):
+        """up to 8 planes: origin, normal (n, 3), velocitydt (n, 3) or None, friction (n,); an empty list removes them"""
+        o = f64(np.asarray(origin, dtype=np.float64).reshape(-1, 3))
+        n = len(o)
+        nr = f64(np.asarray(normal, dtype=np.float64).reshape(-1, 3))
+        v = None if velocitydt is None else f64(np.asarray(velocitydt, dtype=np.float64).reshape(-1, 3))
+        fr = f64(np.zeros(n) if friction is None else np.asarray(friction, dtype=np.float64).reshape(-1))
+        self._ck(self.lib.ipcgpu_set_halfspaces(self.h, n, _d(o) if n else None, _d(nr) if n else None, _d(v) if n else None, _d(fr) if n else None))
+
+    def halfspace_constraint_set(self, dHat, want=True):
+        n = C.c_int()
+        self._ck(self.lib.ipcgpu_halfspace_constraint_set(self.h, float(dHat), C.byref(n) if want else None))
+        return n.value if want else None
+
+    def halfspace_energy(self, dHat, kappa, want=True):
+        E = C.c_double()
+        self._ck(self.lib.ipcgpu_halfspace_energy(self.h, float(dHat), float(kappa), C.byref(E) if want else None))
+        return E.value if want else None
+
+    def halfspace_gradient(self, dHat, kappa, g_inout=None):
+        self._ck(self.lib.ipcgpu_halfspace_gradient(self.h, float(dHat), float(kappa), _d(g_inout)))
+        return g_inout
+
+    def halfspace_hessian(self, dHat, kappa, projectDBC=1, a_inout=None):
+        self._ck(self.lib.ipcgpu_halfspace_hessian(self.h, float(dHat), float(kappa), int(projectDBC), _d(a_inout)))
+        return a_inout
+
+    def halfspace_step(self, p, slackness, alpha):
+        """alpha=None: the device-resident step (step-bound chain); p=None: the held search direction"""
+        a = C.c_double(alpha if alpha is not None else 0.0)
+        rc = self.lib.ipcgpu_halfspace_step(self.h, _d(f64(p)) if p is not None else None, float(slackness), C.byref(a) if alpha is not None else None)
+        if rc != ERR_LINE_SEARCH:
+            self._ck(rc)
+        return (a.value if alpha is not None else None), rc
+
+    def halfspace_crossings(self, want=True):
+        n = C.c_int()
+        self._ck(self.lib.ipcgpu_halfspace_crossings(self.h, C.byref(n) if want else None))
+        return n.value if want else None
+
+    def halfspace_friction_lag(self, dHat, kappa, want=True):
+        n = C.c_int()
+        self._ck(self.lib.ipcgpu_halfspace_friction_lag(self.h, float(dHat), float(kappa), C.byref(n) if want else None))
+        return n.value if want else None
+
+    def halfspace_friction_energy(self, eps2, want=True):
+        E = C.c_double()
+        self._ck(self.lib.ipcgpu_halfspace_friction_energy(self.h, float(eps2), C.byref(E) if want else None))
+        return E.value if want else None
+
+    def halfspace_friction_gradient(self, eps2, g_inout=None):
+        self._ck(self.lib.ipcgpu_halfspace_friction_gradient(self.h, float(eps2), _d(g_inout)))
+        return g_inout
+
+    def halfspace_friction_hessian(self, eps2, projectDBC=1, a_inout=None):
+        self._ck(self.lib.ipcgpu_halfspace_friction_hessian(self.h, float(eps2), int(projectDBC), _d(a_inout)))
+        return a_inout
+
+    def get_halfspace_sets(self):
+        """(active (n, 2) [plane, vertex], lagged (m, 2), lambda (m,))"""
+        na, nl = C.c_int(), C.c_int()
+        self._ck(self.lib.ipcgpu_get_halfspace_sets(self.h, C.byref(na), None, C.byref(nl), None, None))
+        act, lag, lam = np.empty((max(na.value, 1), 2), np.int32), np.empty((max(nl.value, 1), 2), np.int32), np.empty(max(nl.value, 1))
+        self._ck(self.lib.ipcgpu_get_halfspace_sets(self.h, C.byref(na), _i(act), C.byref(nl), _i(lag), _d(lam)))
+        return act[:na.value], lag[:nl.value], lam[:nl.value]
 
     # ---- contact ------------------------------------------------------------------------------
     def set_surface(self, SVI, SFEdges, SF_soa, vCoDim=None):
