@@ -4,7 +4,7 @@
 // its scalar results in the device-resident iteration state (kernels.h: IterState).  An entry point synchronises with the host only if
 // the caller hands it a host output pointer; with NULL outputs a whole Newton iteration runs without a host synchronisation, read back
 // once by ipcgpu_fetch_iteration, its derivative chain on a stream of its own next to the step-bound chain (see enter() below).  The
-// synchronous forms are the same code followed by that read-back.
+// synchronous forms are the same code followed by that read-back (energy_result, gradient_call / hessian_call, flag_status).
 #include "../../include/ipcgpu.h"
 #include "context.h"
 #include <algorithm>
@@ -123,7 +123,7 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 //   - ContactWork::counters: the barrier kernels read words 0 and 2 (list sizes, written by the constraint set before the fork) and the
 //     pair-Hessian build clears and counts word 12; the step-bound chain reads word 3 (partial-CCD candidates).  The step-bound chain
 //     writes no ContactWork buffer.
-//   - IterState: the derivative chain writes energy[0] and flags[FLAG_SET_CAPACITY] / flags[FLAG_PATTERN]; the step-bound chain writes
+//   - IterState: the derivative chain writes energy[kEnergyElastic] and flags[FLAG_SET_CAPACITY] / flags[FLAG_PATTERN]; the step-bound chain writes
 //     step_ord, inv_ord, ccd_ord, cand_range, n_full_cand, max_t, alpha_grid, ref_lo, ref_inv_h, alpha_stage, ref_count, ccd_stats and
 //     flags[FLAG_ZERO_CCD_DISTANCE] / [FLAG_CCD_CAPACITY] / [FLAG_TI_WARNINGS].  Aligned words of their own; nothing clears the struct
 //     while `deriv` is open (the fetch clears the flags after joining).
@@ -131,11 +131,11 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 //     reads ContactWork::cand and writes only the CcdWork buffers (among them the swept grid: cells, sw_keys, sw_ent, sw_cnt, sw_off,
 //     sw_tmp), which the derivative chain does not touch.
 //   - half-space planes: the plane constraint set, lag, energies and crossing check are kSerial (they write hs_act, hs_lag, hs_lam, hs_cnt,
-//     hs_pstart and IterState::hs_energy, hs_n_*, hs_crossings); the plane derivative calls read hs_par, hs_act, hs_lag, hs_lam, hs_cnt,
+//     hs_pstart and IterState::energy[kEnergyPlaneBarrier / kEnergyPlaneFriction], hs_n_*, hs_crossings); the plane derivative calls read hs_par, hs_act, hs_lag, hs_lam, hs_cnt,
 //     Vprev (written before the fork) and write g / a only; ipcgpu_halfspace_step reads hs_par, SVI, dir and writes IterState::step_ord,
 //     hs_alpha, hs_zero_step only (the derivative chain touches none of them).
-//   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, hcon, e_partials2, scalar_out[0], bHraw, brows,
-//     bpsd: derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
+//   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, hcon, e_partials2, bHraw, brows, bpsd:
+//     derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };
 
 static int join_deriv(ipcgpu_ctx* ctx)
@@ -147,8 +147,11 @@ static int join_deriv(ipcgpu_ctx* ctx)
     return IPCGPU_OK;
 }
 
+// first call of every entry point that touches the device: the context's device, then the chain (only ipcgpu_download_range_async,
+// ipcgpu_graph_kernel_priorities and ipcgpu_step_control_info without a pending result set the device themselves instead)
 static int enter(ipcgpu_ctx* ctx, Chain chain)
 {
+    CK(cudaSetDevice(ctx->device));
     if (chain == kStepBound) return IPCGPU_OK;
     if (chain == kSerial || ctx->nranks > 1 || ctx->profiling) return join_deriv(ctx);
     if (ctx->deriv_open) return IPCGPU_OK;
@@ -172,11 +175,6 @@ int fetch_iter_state(ipcgpu_ctx* ctx)
     }
     CK(cudaMemcpyAsync(ctx->h_iter, ctx->iter.p, sizeof(IterState), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    return IPCGPU_OK;
-}
-static int clear_flag(ipcgpu_ctx* ctx, int idx)
-{
-    CK(cudaMemsetAsync(&ctx->iter.p->flags[idx], 0, sizeof(int), ctx->stream));
     return IPCGPU_OK;
 }
 
@@ -440,6 +438,134 @@ static int status_from_flags(ipcgpu_ctx* ctx, const int* f)
     return IPCGPU_OK;
 }
 
+// ---- the tails the synchronous forms share --------------------------------------------------------------------------------
+// the flags of `mask` that the (fresh) h_iter shows raised: cleared on the device, returned as a status
+static int flag_status(ipcgpu_ctx* ctx, unsigned mask)
+{
+    int f[8] = { 0 };
+    for (int i = 0; i < 8; ++i)
+        if (((mask >> i) & 1u) && ctx->h_iter->flags[i]) {
+            f[i] = ctx->h_iter->flags[i];
+            CK(cudaMemsetAsync(&ctx->iter.p->flags[i], 0, sizeof(int), ctx->stream));
+        }
+    return status_from_flags(ctx, f);
+}
+
+static void set_local(ipcgpu_ctx* ctx, unsigned bits, bool local)
+{
+    ctx->local_scalars = local ? (ctx->local_scalars | bits) : (ctx->local_scalars & ~bits);
+}
+
+// IterState::energy[slot] once reduced.  Host E: summed across the ranks in place and read back, either the one double or (`fetch`) the
+// whole iteration state, after which the flags of `check` are the status.  NULL: this rank's share, completed by the fetch's collective.
+static int energy_result(ipcgpu_ctx* ctx, int slot, double* E, bool fetch = false, unsigned check = 0)
+{
+    set_local(ctx, 1u << slot, ctx->nranks > 1 && !E);
+    if (!E) return IPCGPU_OK;
+    double* out = &ctx->iter.p->energy[slot];
+    if (ctx->nranks > 1) {
+        int r = g_nccl.AllReduce(out, out, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
+        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(energy) failed");
+    }
+    if (fetch) {
+        int rc = fetch_iter_state(ctx);
+        if (rc) return rc;
+        *E = ctx->h_iter->energy[slot];
+        return flag_status(ctx, check);
+    }
+    CK(cudaMemcpyAsync(ctx->h_scalar, out, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    *E = ctx->h_scalar[0];
+    return IPCGPU_OK;
+}
+// the tail of an energy term on the main stream: its partial sums reduced into the slot, the stage timer `pe` stopped, energy_result
+static int energy_tail(ipcgpu_ctx* ctx, int slot, const double* partials, int n_partials, double scale, cudaEvent_t pe, double* E, bool fetch = false,
+    unsigned check = 0)
+{
+    reduce_sum(partials, n_partials, scale, &ctx->iter.p->energy[slot], ctx->stream);
+    ctx->prof_end(pe);
+    ctx->launches += 2; // the term's partial kernel and the reduce
+    CK(cudaGetLastError());
+    return energy_result(ctx, slot, E, fetch, check);
+}
+
+// host gradient in/out around a kernel that accumulates into the device gradient (addCoeff-like semantics: rank 0 contributes the input)
+static int gradient_roundtrip_begin(ipcgpu_ctx* ctx, const double* g_in)
+{
+    if (ctx->rank == 0) CK(cudaMemcpyAsync(ctx->g.p, g_in, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    else CK(cudaMemsetAsync(ctx->g.p, 0, (size_t)3 * ctx->nV * sizeof(double), ctx->stream));
+    return IPCGPU_OK;
+}
+static int gradient_roundtrip_end(ipcgpu_ctx* ctx, double* g_out)
+{
+    if (ctx->nranks > 1) {
+        int rc = ipcgpu_allreduce_grad_hess(ctx, 1, 0);
+        if (rc) return rc;
+    }
+    CK(cudaMemcpyAsync(g_out, ctx->g.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IPCGPU_OK;
+}
+// the same for the value array
+static int upload_values(ipcgpu_ctx* ctx, const double* a_host)
+{
+    int rc = sync_pattern_mirror(ctx);
+    if (rc) return rc;
+    if (ctx->rank == 0) CK(cudaMemcpyAsync(ctx->a.p, a_host, (size_t)ctx->nnz * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    else CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)ctx->nnz * sizeof(double), ctx->stream));
+    return IPCGPU_OK;
+}
+static int download_values(ipcgpu_ctx* ctx, double* a_host)
+{
+    int rc = sync_pattern_mirror(ctx);
+    if (rc) return rc;
+    if (ctx->nranks > 1 && (rc = ipcgpu_allreduce_grad_hess(ctx, 0, 1))) return rc;
+    CK(cudaMemcpyAsync(a_host, ctx->a.p, (size_t)ctx->nnz * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IPCGPU_OK;
+}
+
+// A gradient / Hessian term.  NULL output: the term on `chain`; host output: the caller's array in, the term added on the main stream,
+// the rank-completed array out and, for a Hessian, the flags of `check` it may raise returned as its status.
+template <typename Launch>
+static int gradient_call(ipcgpu_ctx* ctx, Chain chain, double* g_inout, Launch launch)
+{
+    ENTER(g_inout ? kSerial : chain);
+    int rc;
+    if (g_inout && (rc = gradient_roundtrip_begin(ctx, g_inout))) return rc;
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
+    launch(ctx->deriv_stream());
+    ctx->prof_end(pe);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    return g_inout ? gradient_roundtrip_end(ctx, g_inout) : IPCGPU_OK;
+}
+static int hessian_begin(ipcgpu_ctx* ctx, Chain chain, const double* a_inout)
+{
+    REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
+    ENTER(a_inout ? kSerial : chain);
+    return a_inout ? upload_values(ctx, a_inout) : IPCGPU_OK;
+}
+static int hessian_end(ipcgpu_ctx* ctx, double* a_inout, unsigned check)
+{
+    if (!a_inout) return IPCGPU_OK;
+    int rc = download_values(ctx, a_inout);
+    if (rc || !check || (rc = fetch_iter_state(ctx))) return rc;
+    return flag_status(ctx, check);
+}
+template <typename Launch>
+static int hessian_call(ipcgpu_ctx* ctx, Chain chain, double* a_inout, unsigned check, Launch launch)
+{
+    int rc = hessian_begin(ctx, chain, a_inout);
+    if (rc) return rc;
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
+    launch(ctx->deriv_stream());
+    ctx->prof_end(pe);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    return hessian_end(ctx, a_inout, check);
+}
+
 // f(node, priority attribute) on every kernel node of a graph and of the bodies of its conditional nodes, until one returns an error
 template <typename F>
 static cudaError_t for_each_kernel_node(cudaGraph_t top, const std::vector<cudaGraph_t>& bodies, F f)
@@ -486,7 +612,7 @@ int ipcgpu_create(int device, ipcgpu_ctx** out)
         || cudaStreamCreateWithPriority(&ctx->deriv, cudaStreamNonBlocking, ctx->prio_low) != cudaSuccess
         || cudaEventCreateWithFlags(&ctx->ev_deriv_fork, cudaEventDisableTiming) != cudaSuccess
         || cudaEventCreateWithFlags(&ctx->ev_deriv_done, cudaEventDisableTiming) != cudaSuccess || cudaMallocHost(&ctx->h_scalar, 512) != cudaSuccess
-        || cudaMallocHost(&hi, sizeof(IterState)) != cudaSuccess || !ctx->flag.reserve(4) || !ctx->scalar_out.reserve(40) || !ctx->iter.reserve(1)
+        || cudaMallocHost(&hi, sizeof(IterState)) != cudaSuccess || !ctx->flag.reserve(4) || !ctx->packed_scalars.reserve(kPackedScalars) || !ctx->iter.reserve(1)
         || cudaMemsetAsync(ctx->iter.p, 0, sizeof(IterState), ctx->stream) != cudaSuccess) {
         ipcgpu_destroy(ctx);
         return IPCGPU_ERR_CUDA;
@@ -579,7 +705,6 @@ int ipcgpu_comm_init(ipcgpu_ctx* ctx, int rank, int nranks, const void* id128)
     ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(nranks >= 1 && rank >= 0 && rank < nranks, IPCGPU_ERR_ARG, "bad rank/nranks");
-    CK(cudaSetDevice(ctx->device));
     ctx->rank = rank;
     ctx->nranks = nranks;
     if (nranks > 1) {
@@ -621,7 +746,6 @@ int ipcgpu_set_mesh(ipcgpu_ctx* ctx, int nV, int nT, const double* Vrest, const 
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(nV > 0 && nT >= 0 && Vrest && tets && restTriInv && vol && mu && lam, IPCGPU_ERR_ARG, "ipcgpu_set_mesh: null or empty input");
     REQUIRE(energy == IPCGPU_NEOHOOKEAN || energy == IPCGPU_FIXED_COROT, IPCGPU_ERR_ARG, "unknown energy type");
-    CK(cudaSetDevice(ctx->device));
     for (size_t i = 0; i < (size_t)4 * nT; ++i) REQUIRE(tets[i] >= 0 && tets[i] < nV, IPCGPU_ERR_ARG, "tet vertex index out of range");
     ctx->nV = nV;
     ctx->nT = nT;
@@ -662,7 +786,6 @@ int ipcgpu_set_csr(ipcgpu_ctx* ctx, int n_rows, const int* ia, const int* ja, in
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(n_rows > 0 && ia && ja && (index_base == 0 || index_base == 1), IPCGPU_ERR_ARG, "ipcgpu_set_csr: bad arguments");
     REQUIRE(ctx->nV > 0 && n_rows == 3 * ctx->nV, IPCGPU_ERR_ARG, "ipcgpu_set_csr: n_rows must be 3*nV of the mesh set before");
-    CK(cudaSetDevice(ctx->device));
     const int nnz = ia[n_rows] - index_base;
     REQUIRE(nnz >= 0, IPCGPU_ERR_ARG, "ipcgpu_set_csr: negative nnz");
     ctx->n_rows = n_rows;
@@ -684,7 +807,6 @@ int ipcgpu_set_csr(ipcgpu_ctx* ctx, int n_rows, const int* ia, const int* ja, in
 int ipcgpu_set_state(ipcgpu_ctx* ctx, const double* V)
 {
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     if (V) CK(cudaMemcpyAsync(ctx->V.p, V, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     ctx->mark_inputs();
@@ -733,7 +855,6 @@ static int upload_dir(ipcgpu_ctx* ctx, const double* p)
 int ipcgpu_set_search_dir(ipcgpu_ctx* ctx, const double* p)
 {
     REQUIRE(ctx->nV > 0 && p, IPCGPU_ERR_ARG, "ipcgpu_set_search_dir: mesh and p required");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     return upload_dir(ctx, p);
 }
@@ -742,7 +863,6 @@ int ipcgpu_step_forward(ipcgpu_ctx* ctx, const double* p, double alpha)
 {
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     REQUIRE(ctx->state_saved, IPCGPU_ERR_STATE, "ipcgpu_save_state must precede ipcgpu_step_forward");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = upload_dir(ctx, p);
     if (rc) return rc;
@@ -756,26 +876,10 @@ int ipcgpu_step_forward(ipcgpu_ctx* ctx, const double* p, double alpha)
 int ipcgpu_elastic_energy(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, double* E)
 {
     REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_ELASTIC_ENERGY);
-    elastic_energy(ctx->eargs(), ctx->e_per_tet.p, ctx->partials.p, coef, ctx->scalar_out.p, ctx->stream);
-    ctx->prof_end(pe);
-    ctx->launches += 2;
-    if (ctx->nranks > 1 && E) { // host result requested: complete it now; NULL = local sum, reduced by ipcgpu_fetch_iteration
-        int r = g_nccl.AllReduce(ctx->scalar_out.p, ctx->scalar_out.p, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
-        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(energy) failed");
-    }
-    energy_store(ctx->iter.p, 0, ctx->scalar_out.p, ctx->stream);
-    ++ctx->launches;
-    ctx->energy_local[0] = (ctx->nranks > 1 && !E);
-    CK(cudaGetLastError());
-    if (E) {
-        CK(cudaMemcpyAsync(ctx->h_scalar, ctx->scalar_out.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *E = ctx->h_scalar[0];
-    }
-    return IPCGPU_OK;
+    elastic_energy(ctx->eargs(), ctx->e_per_tet.p, ctx->partials.p, ctx->stream);
+    return energy_tail(ctx, kEnergyElastic, ctx->partials.p, elastic_energy_blocks(ctx->t_end - ctx->t_begin), coef, pe, E);
 }
 
 // zero the part of the value array this rank writes (everything after a cross-rank completion has filled the other rows)
@@ -815,13 +919,11 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
     ctx->hblk_valid = need_h && !slot_major;
     ctx->prof_end(pe);
     ++ctx->launches;
-    if (with_energy) {
+    if (with_energy) { // (which rank's share it is: energy_result, once the call knows whether the host wants it)
         pe = ctx->prof_begin(IPCGPU_STAGE_ELASTIC_ENERGY);
-        reduce_sum(e_part, elastic_grad_hess_blocks(ctx->n_list), coef, ctx->scalar_out.p, st);
-        energy_store(ctx->iter.p, 0, ctx->scalar_out.p, st);
+        reduce_sum(e_part, elastic_grad_hess_blocks(ctx->n_list), coef, &ctx->iter.p->energy[kEnergyElastic], st);
         ctx->prof_end(pe);
-        ctx->launches += 2;
-        ctx->energy_local[0] = ctx->nranks > 1;
+        ++ctx->launches;
     }
     if (need_g) {
         // owned vertices gather their complete sums (every incident tet is in this rank's list); the other rows are written as zeros
@@ -850,112 +952,52 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
 
 int ipcgpu_elastic_gradient(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, int projectDBC, double* g)
 {
-    CK(cudaSetDevice(ctx->device));
     ENTER(g ? kSerial : kDerivative);
     int rc = run_grad_hess(ctx, coef, 1, projectDBC, true, false, 0);
-    if (rc) return rc;
-    if (ctx->nranks > 1 && g) { // host result requested: complete it across ranks; NULL = deferred (ipcgpu_allreduce_grad_hess)
-        rc = ipcgpu_allreduce_grad_hess(ctx, 1, 0);
-        if (rc) return rc;
-    }
-    if (g) {
-        CK(cudaMemcpyAsync(g, ctx->g.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    return IPCGPU_OK;
-}
-
-// host value array in (addCoeff semantics): rank 0 contributes it, everybody else starts from zero
-static int upload_values(ipcgpu_ctx* ctx, const double* a_host)
-{
-    int rc = sync_pattern_mirror(ctx);
-    if (rc) return rc;
-    if (ctx->rank == 0) CK(cudaMemcpyAsync(ctx->a.p, a_host, (size_t)ctx->nnz * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    else CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)ctx->nnz * sizeof(double), ctx->stream));
-    return IPCGPU_OK;
-}
-static int download_values(ipcgpu_ctx* ctx, double* a_host)
-{
-    {
-        int rc = sync_pattern_mirror(ctx);
-        if (rc) return rc;
-    }
-    if (ctx->nranks > 1) {
-        int rc = ipcgpu_allreduce_grad_hess(ctx, 0, 1);
-        if (rc) return rc;
-    }
-    CK(cudaMemcpyAsync(a_host, ctx->a.p, (size_t)ctx->nnz * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return IPCGPU_OK;
+    return rc || !g ? rc : gradient_roundtrip_end(ctx, g); // (the gradient is written, not accumulated: no roundtrip_begin)
 }
 
 int ipcgpu_elastic_hessian(ipcgpu_ctx* ctx, double coef, int /*redoSVD*/, int projectSPD, int projectDBC, double* a_inout)
 {
-    CK(cudaSetDevice(ctx->device));
+    int rc = hessian_begin(ctx, kDerivative, a_inout);
+    if (rc || (rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, false, true, 0))) return rc;
+    return hessian_end(ctx, a_inout, 0);
+}
+
+static int elastic_derivatives(ipcgpu_ctx* ctx, double coef, int projectSPD, int projectDBC, int add_mass, bool with_energy, double* E, double* g, double* a)
+{
     REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
-    ENTER(a_inout ? kSerial : kDerivative);
-    int rc;
-    if (a_inout && (rc = upload_values(ctx, a_inout))) return rc;
-    if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, false, true, 0))) return rc;
-    if (a_inout) return download_values(ctx, a_inout);
+    ENTER(E || g || a ? kSerial : kDerivative);
+    // the value array is rebuilt from scratch (LinSysSolver::setZero, then addCoeff of every term): slots that no local tet touches
+    // -- contact-only blocks of the augmented pattern -- must not keep last iteration's values
+    int rc = a ? sync_pattern_mirror(ctx) : 0; // (the host array holds the current pattern's values)
+    if (rc || (rc = zero_values(ctx))) return rc;
+    if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, true, true, add_mass, with_energy))) return rc;
+    if (ctx->nranks > 1 && (g || a)) {
+        rc = ipcgpu_allreduce_grad_hess(ctx, g ? 1 : 0, a ? 1 : 0);
+        if (rc) return rc;
+    }
+    if (g) CK(cudaMemcpyAsync(g, ctx->g.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    if (a) CK(cudaMemcpyAsync(a, ctx->a.p, (size_t)ctx->nnz * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    if (with_energy && (rc = energy_result(ctx, kEnergyElastic, E))) return rc; // (a host E synchronises)
+    if (!E && (g || a)) CK(cudaStreamSynchronize(ctx->stream));
     return IPCGPU_OK;
 }
 
 int ipcgpu_elastic_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int projectDBC, int add_mass, double* g, double* a)
 {
-    CK(cudaSetDevice(ctx->device));
-    REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
-    ENTER(g || a ? kSerial : kDerivative);
-    // the value array is rebuilt from scratch (LinSysSolver::setZero, then addCoeff of every term): slots that no local tet touches
-    // -- contact-only blocks of the augmented pattern -- must not keep last iteration's values
-    int rc = a ? sync_pattern_mirror(ctx) : 0; // (the host array holds the current pattern's values)
-    if (rc || (rc = zero_values(ctx))) return rc;
-    if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, true, true, add_mass))) return rc;
-    if (ctx->nranks > 1 && (g || a)) {
-        rc = ipcgpu_allreduce_grad_hess(ctx, g ? 1 : 0, a ? 1 : 0);
-        if (rc) return rc;
-    }
-    if (g) CK(cudaMemcpyAsync(g, ctx->g.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    if (a) CK(cudaMemcpyAsync(a, ctx->a.p, (size_t)ctx->nnz * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    if (g || a) CK(cudaStreamSynchronize(ctx->stream));
-    return IPCGPU_OK;
+    return elastic_derivatives(ctx, coef, projectSPD, projectDBC, add_mass, false, nullptr, g, a);
 }
 
 int ipcgpu_elastic_energy_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int projectDBC, int add_mass, double* E, double* g, double* a)
 {
-    CK(cudaSetDevice(ctx->device));
-    REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
-    ENTER(E || g || a ? kSerial : kDerivative);
-    // the value array is rebuilt from scratch (LinSysSolver::setZero, then addCoeff of every term): slots that no local tet touches
-    // -- contact-only blocks of the augmented pattern -- must not keep last iteration's values
-    int rc = a ? sync_pattern_mirror(ctx) : 0;
-    if (rc || (rc = zero_values(ctx))) return rc;
-    if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, true, true, add_mass, true))) return rc;
-    if (ctx->nranks > 1 && (g || a)) {
-        rc = ipcgpu_allreduce_grad_hess(ctx, g ? 1 : 0, a ? 1 : 0);
-        if (rc) return rc;
-    }
-    if (g) CK(cudaMemcpyAsync(g, ctx->g.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    if (a) CK(cudaMemcpyAsync(a, ctx->a.p, (size_t)ctx->nnz * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    if (E) { // host result requested: complete it across the ranks now
-        if (ctx->nranks > 1) {
-            int r = g_nccl.AllReduce(&ctx->iter.p->energy[0], &ctx->iter.p->energy[0], 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
-            REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(energy) failed");
-            ctx->energy_local[0] = false;
-        }
-        CK(cudaMemcpyAsync(ctx->h_scalar, &ctx->iter.p->energy[0], sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *E = ctx->h_scalar[0];
-    }
-    else if (g || a) CK(cudaStreamSynchronize(ctx->stream));
-    return IPCGPU_OK;
+    return elastic_derivatives(ctx, coef, projectSPD, projectDBC, add_mass, true, E, g, a);
 }
 
 // ---- step bound: device-resident chain ---------------------------------------------------------------------
 int ipcgpu_step_bound_set(ipcgpu_ctx* ctx, double alpha)
 {
     REQUIRE(alpha >= 0.0, IPCGPU_ERR_ARG, "the step must be non-negative");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kStepBound);
     step_set(ctx->iter.p, alpha, ctx->stream);
     ++ctx->launches;
@@ -966,7 +1008,6 @@ int ipcgpu_step_bound_set(ipcgpu_ctx* ctx, double alpha)
 int ipcgpu_inversion_step(ipcgpu_ctx* ctx, const double* p, double slack, double* alpha_inout)
 {
     REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(p || alpha_inout ? kSerial : kStepBound);
     int rc = upload_dir(ctx, p);
     if (rc) return rc;
@@ -990,7 +1031,6 @@ int ipcgpu_set_surface(ipcgpu_ctx* ctx, int nSV, const int* SVI, int nSE, const 
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     REQUIRE(nSV >= 0 && nSE >= 0 && nSF >= 0 && (nSV == 0 || SVI) && (nSE == 0 || SE) && (nSF == 0 || SF), IPCGPU_ERR_ARG, "ipcgpu_set_surface: bad arguments");
-    CK(cudaSetDevice(ctx->device));
     for (int i = 0; i < nSV; ++i) REQUIRE(SVI[i] >= 0 && SVI[i] < ctx->nV, IPCGPU_ERR_ARG, "SVI out of range");
     for (int i = 0; i < 2 * nSE; ++i) REQUIRE(SE[i] >= 0 && SE[i] < ctx->nV, IPCGPU_ERR_ARG, "SFEdges out of range");
     for (size_t i = 0; i < (size_t)3 * nSF; ++i) REQUIRE(SF[i] >= 0 && SF[i] < ctx->nV, IPCGPU_ERR_ARG, "SF out of range");
@@ -1043,7 +1083,6 @@ int ipcgpu_set_obstacle_positions(ipcgpu_ctx* ctx, const double* Vo_soa)
 {
     REQUIRE(ctx->nV > 0 && ctx->nVdof < ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_obstacle_tail first");
     REQUIRE(Vo_soa, IPCGPU_ERR_ARG, "null argument");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     const size_t nVo = (size_t)(ctx->nV - ctx->nVdof);
     // current AND rest positions: the obstacle has no rest shape of its own, compute_eps_x takes its current edge lengths
@@ -1113,7 +1152,6 @@ int ipcgpu_ccd_partial_ti(ipcgpu_ctx* ctx, const double* p, double tol, const do
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(err_vf && err_ee, IPCGPU_ERR_ARG, "null argument");
-    CK(cudaSetDevice(ctx->device));
     ENTER(p || alpha_inout ? kSerial : kStepBound);
     int rc = upload_dir(ctx, p);
     if (rc) return rc;
@@ -1131,7 +1169,6 @@ int ipcgpu_hash_build_swept(ipcgpu_ctx* ctx, const double* p, double* alpha_inou
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(h > 0.0, IPCGPU_ERR_ARG, "bad arguments");
-    CK(cudaSetDevice(ctx->device));
     ENTER(p || alpha_inout ? kSerial : kStepBound);
     int rc = upload_dir(ctx, p);
     if (rc) return rc;
@@ -1146,7 +1183,6 @@ int ipcgpu_ccd_full_ti(ipcgpu_ctx* ctx, double tol, const double err_vf[3], cons
 {
     REQUIRE(ctx->surface_ready && ctx->ccd.swept_ready, IPCGPU_ERR_STATE, "ipcgpu_hash_build_swept first");
     REQUIRE(err_vf && err_ee, IPCGPU_ERR_ARG, "null argument");
-    CK(cudaSetDevice(ctx->device));
     ENTER(alpha_inout || n_candidates ? kSerial : kStepBound);
     int rc;
     // (the swept grid was built for the step the chain held then; a host step that differs from it only lowers max_t)
@@ -1155,12 +1191,7 @@ int ipcgpu_ccd_full_ti(ipcgpu_ctx* ctx, double tol, const double err_vf[3], cons
     if (alpha_inout || n_candidates) {
         if ((rc = ccd_read_back(ctx, alpha_inout))) return rc;
         if (n_candidates) *n_candidates = ctx->h_iter->n_full_cand;
-        if (ctx->h_iter->flags[FLAG_CCD_CAPACITY]) {
-            clear_flag(ctx, FLAG_CCD_CAPACITY);
-            int only[8] = { 0 };
-            only[FLAG_CCD_CAPACITY] = 1;
-            return status_from_flags(ctx, only);
-        }
+        return flag_status(ctx, 1u << FLAG_CCD_CAPACITY);
     }
     return IPCGPU_OK;
 }
@@ -1221,7 +1252,6 @@ int ipcgpu_constraint_set(ipcgpu_ctx* ctx, double dHat, int getPTEE, int* nC, in
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(dHat > 0.0, IPCGPU_ERR_ARG, "dHat must be positive");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = contact_constraint_set(ctx, dHat, getPTEE, nC, nPara, nCand);
     ctx->lists_local = (rc == 0) && ctx->partition_contact && ctx->nranks > 1;
@@ -1343,7 +1373,6 @@ int ipcgpu_enable_device_pattern(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_c
     ++ctx->epoch; // graphs captured before this call are refused (ja / a may be reallocated)
     REQUIRE(ctx->maps_ready && ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     REQUIRE(index_base == 0 || index_base == 1, IPCGPU_ERR_ARG, "index_base must be 0 or 1");
-    CK(cudaSetDevice(ctx->device));
     ctx->device_pattern = false;
     int rc = pattern_enable(ctx, index_base, nnz_capacity);
     if (rc) return rc;
@@ -1363,7 +1392,6 @@ int ipcgpu_update_pattern(ipcgpu_ctx* ctx, int with_friction, int* changed, int6
     REQUIRE(ctx->device_pattern, IPCGPU_ERR_STATE, "ipcgpu_enable_device_pattern first");
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(!with_friction || ctx->cw.fr_ready, IPCGPU_ERR_STATE, "with_friction: ipcgpu_friction_lag / ipcgpu_set_friction_data first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = pattern_update(ctx, barrier_args(ctx, 1.0, 1.0, 0), with_friction != 0);
     if (rc) return rc;
@@ -1372,19 +1400,12 @@ int ipcgpu_update_pattern(ipcgpu_ctx* ctx, int with_friction, int* changed, int6
     if ((rc = sync_pattern_mirror(ctx))) return rc;
     if (changed) *changed = ctx->pat_changed_host;
     if (nnz) *nnz = ctx->nnz;
-    if (ctx->h_iter->flags[FLAG_PATTERN_CAPACITY]) {
-        clear_flag(ctx, FLAG_PATTERN_CAPACITY);
-        int only[8] = { 0 };
-        only[FLAG_PATTERN_CAPACITY] = 1;
-        return status_from_flags(ctx, only);
-    }
-    return IPCGPU_OK;
+    return flag_status(ctx, 1u << FLAG_PATTERN_CAPACITY);
 }
 
 int ipcgpu_pattern_info(ipcgpu_ctx* ctx, int* changed, int64_t* nnz, uint64_t* version)
 {
     REQUIRE(ctx->device_pattern, IPCGPU_ERR_STATE, "ipcgpu_enable_device_pattern first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = sync_pattern_mirror(ctx);
     if (rc) return rc;
@@ -1397,7 +1418,6 @@ int ipcgpu_pattern_info(ipcgpu_ctx* ctx, int* changed, int64_t* nnz, uint64_t* v
 int ipcgpu_get_pattern(ipcgpu_ctx* ctx, int* ia, int* ja)
 {
     REQUIRE(ctx->n_rows > 0, IPCGPU_ERR_STATE, "no pattern: ipcgpu_set_csr or ipcgpu_enable_device_pattern first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = sync_pattern_mirror(ctx);
     if (rc) return rc;
@@ -1410,83 +1430,24 @@ int ipcgpu_get_pattern(ipcgpu_ctx* ctx, int* ia, int* ja)
 int ipcgpu_barrier_energy(ipcgpu_ctx* ctx, double dHat, double kappa, double* E)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     BarrierArgs p = barrier_args(ctx, dHat, kappa, 0);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     barrier_energy(p, ctx->cw.bpartials.p, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE], ctx->stream);
-    reduce_sum(ctx->cw.bpartials.p, barrier_energy_blocks(), kappa, ctx->scalar_out.p + 1, ctx->stream);
-    ctx->prof_end(pe);
-    ctx->launches += 2;
-    if (ctx->nranks > 1 && E) {
-        int r = g_nccl.AllReduce(ctx->scalar_out.p + 1, ctx->scalar_out.p + 1, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
-        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(barrier energy) failed");
-    }
-    energy_store(ctx->iter.p, 1, ctx->scalar_out.p + 1, ctx->stream);
-    ++ctx->launches;
-    ctx->energy_local[1] = (ctx->nranks > 1 && !E);
-    CK(cudaGetLastError());
-    if (E) { // synchronous form: the d <= 0 flag is checked right here (every rank checks its own share of the pairs)
-        int rc = fetch_iter_state(ctx);
-        if (rc) return rc;
-        *E = ctx->h_iter->energy[1];
-        if (ctx->h_iter->flags[FLAG_NONPOSITIVE_DISTANCE]) {
-            clear_flag(ctx, FLAG_NONPOSITIVE_DISTANCE);
-            int only[8] = { 0 };
-            only[FLAG_NONPOSITIVE_DISTANCE] = 1;
-            return status_from_flags(ctx, only);
-        }
-    }
-    return IPCGPU_OK;
+    // synchronous form: the d <= 0 flag is checked right here (every rank checks its own share of the pairs)
+    return energy_tail(ctx, kEnergyBarrier, ctx->cw.bpartials.p, barrier_energy_blocks(), kappa, pe, E, true, 1u << FLAG_NONPOSITIVE_DISTANCE);
 }
 
 int ipcgpu_barrier_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* g_inout)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
-    CK(cudaSetDevice(ctx->device));
-    ENTER(g_inout ? kSerial : kDerivative);
-    if (g_inout) {
-        if (ctx->rank == 0) CK(cudaMemcpyAsync(ctx->g.p, g_inout, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-        else CK(cudaMemsetAsync(ctx->g.p, 0, (size_t)3 * ctx->nV * sizeof(double), ctx->stream));
-    }
-    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
-    barrier_gradient(barrier_args(ctx, dHat, kappa, 0), ctx->g.p, ctx->deriv_stream());
-    ctx->prof_end(pe);
-    ++ctx->launches;
-    CK(cudaGetLastError());
-    if (g_inout && ctx->nranks > 1) {
-        int rc = ipcgpu_allreduce_grad_hess(ctx, 1, 0);
-        if (rc) return rc;
-    }
-    if (g_inout) {
-        CK(cudaMemcpyAsync(g_inout, ctx->g.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    return IPCGPU_OK;
-}
-
-// host gradient in/out around a kernel that accumulates into the device gradient (addCoeff-like semantics: rank 0 contributes the input)
-static int gradient_roundtrip_begin(ipcgpu_ctx* ctx, const double* g_in)
-{
-    if (ctx->rank == 0) CK(cudaMemcpyAsync(ctx->g.p, g_in, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    else CK(cudaMemsetAsync(ctx->g.p, 0, (size_t)3 * ctx->nV * sizeof(double), ctx->stream));
-    return IPCGPU_OK;
-}
-static int gradient_roundtrip_end(ipcgpu_ctx* ctx, double* g_out)
-{
-    if (ctx->nranks > 1) {
-        int rc = ipcgpu_allreduce_grad_hess(ctx, 1, 0);
-        if (rc) return rc;
-    }
-    CK(cudaMemcpyAsync(g_out, ctx->g.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return IPCGPU_OK;
+    const BarrierArgs p = barrier_args(ctx, dHat, kappa, 0);
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { barrier_gradient(p, ctx->g.p, st); });
 }
 
 int ipcgpu_evaluate_constraints(ipcgpu_ctx* ctx, double* val, int n)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     ContactWork& w = ctx->cw;
     if (w.nC < 0) {
@@ -1509,7 +1470,6 @@ int ipcgpu_constraint_jacobian_t(ipcgpu_ctx* ctx, const double* input, int n, do
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(g_inout != nullptr, IPCGPU_ERR_ARG, "null gradient");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     ContactWork& w = ctx->cw;
     if (w.nC < 0) {
@@ -1534,7 +1494,6 @@ int ipcgpu_para_ee_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(g_inout != nullptr, IPCGPU_ERR_ARG, "null gradient");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = gradient_roundtrip_begin(ctx, g_inout);
     if (rc) return rc;
@@ -1547,11 +1506,8 @@ int ipcgpu_para_ee_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
 int ipcgpu_barrier_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC, double* a_inout)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
-    REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
-    CK(cudaSetDevice(ctx->device));
-    ENTER(a_inout ? kSerial : kDerivative);
-    int rc;
-    if (a_inout && (rc = upload_values(ctx, a_inout))) return rc;
+    int rc = hessian_begin(ctx, kDerivative, a_inout);
+    if (rc) return rc;
     ContactWork& w = ctx->cw;
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     const BarrierArgs bp = barrier_args(ctx, dHat, kappa, projectDBC);
@@ -1571,26 +1527,13 @@ int ipcgpu_barrier_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int proje
     ctx->prof_end(pe);
     ctx->launches += 3;
     CK(cudaGetLastError());
-    if (a_inout) { // synchronous form: complete across ranks, download, check the pattern flag now
-        if ((rc = download_values(ctx, a_inout))) return rc;
-        if ((rc = fetch_iter_state(ctx))) return rc;
-        if (ctx->h_iter->flags[FLAG_PATTERN] || ctx->h_iter->flags[FLAG_SET_CAPACITY]) {
-            int only[8] = { 0 };
-            only[FLAG_PATTERN] = ctx->h_iter->flags[FLAG_PATTERN];
-            only[FLAG_SET_CAPACITY] = ctx->h_iter->flags[FLAG_SET_CAPACITY];
-            clear_flag(ctx, FLAG_PATTERN);
-            clear_flag(ctx, FLAG_SET_CAPACITY);
-            return status_from_flags(ctx, only);
-        }
-    }
-    return IPCGPU_OK;
+    return hessian_end(ctx, a_inout, (1u << FLAG_PATTERN) | (1u << FLAG_SET_CAPACITY));
 }
 
 // ---- lagged friction of the self-contact pairs (SURVEY 8 f4) --------------------------------------------------------------
 int ipcgpu_set_prev_state(ipcgpu_ctx* ctx, const double* V_prev_soa)
 {
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     ALLOC(ctx->Vprev, (size_t)3 * ctx->nV);
     if (V_prev_soa) CK(cudaMemcpyAsync(ctx->Vprev.p, V_prev_soa, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
@@ -1615,7 +1558,6 @@ static int friction_alloc(ipcgpu_ctx* ctx)
 int ipcgpu_friction_lag(ipcgpu_ctx* ctx, double dHat, double kappa, int* n_pairs)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = friction_alloc(ctx);
     if (rc) return rc;
@@ -1650,7 +1592,6 @@ static int friction_host_count(ipcgpu_ctx* ctx)
 int ipcgpu_get_friction_data(ipcgpu_ctx* ctx, int* n_pairs, int* mmcvid4, double* lambda, double* coord2, double* basis6)
 {
     REQUIRE(ctx->cw.fr_ready, IPCGPU_ERR_STATE, "ipcgpu_friction_lag / ipcgpu_set_friction_data first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = friction_host_count(ctx);
     if (rc) return rc;
@@ -1670,7 +1611,6 @@ int ipcgpu_set_friction_data(ipcgpu_ctx* ctx, int n_pairs, const int* mmcvid4, c
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     REQUIRE(n_pairs >= 0 && n_pairs <= ctx->pair_capacity, IPCGPU_ERR_CAPACITY, "friction set larger than the pair capacity");
     REQUIRE(n_pairs == 0 || (mmcvid4 && lambda && coord2 && basis6), IPCGPU_ERR_ARG, "null friction arrays");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = friction_alloc(ctx);
     if (rc) return rc;
@@ -1710,71 +1650,27 @@ int ipcgpu_friction_energy(ipcgpu_ctx* ctx, double eps2, double coef, double* E)
 {
     REQUIRE_FRICTION();
     REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     friction_energy(friction_args(ctx, eps2, coef, 0), ctx->cw.fr_partials.p, ctx->stream);
-    reduce_sum(ctx->cw.fr_partials.p, friction_energy_blocks(), coef, ctx->scalar_out.p + 2, ctx->stream);
-    ctx->prof_end(pe);
-    ctx->launches += 2;
-    if (ctx->nranks > 1 && E) {
-        int r = g_nccl.AllReduce(ctx->scalar_out.p + 2, ctx->scalar_out.p + 2, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
-        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(friction energy) failed");
-    }
-    energy_store(ctx->iter.p, 2, ctx->scalar_out.p + 2, ctx->stream);
-    ++ctx->launches;
-    ctx->energy_local[2] = (ctx->nranks > 1 && !E);
-    CK(cudaGetLastError());
-    if (E) {
-        CK(cudaMemcpyAsync(ctx->h_scalar, ctx->scalar_out.p + 2, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *E = ctx->h_scalar[0];
-    }
-    return IPCGPU_OK;
+    return energy_tail(ctx, kEnergyFriction, ctx->cw.fr_partials.p, friction_energy_blocks(), coef, pe, E);
 }
 
 int ipcgpu_friction_gradient(ipcgpu_ctx* ctx, double eps2, double coef, double* g_inout)
 {
     REQUIRE_FRICTION();
     REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive");
-    CK(cudaSetDevice(ctx->device));
-    ENTER(kSerial);
-    int rc;
-    if (g_inout && (rc = gradient_roundtrip_begin(ctx, g_inout))) return rc;
-    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
-    friction_gradient(friction_args(ctx, eps2, coef, 0), ctx->g.p, ctx->stream);
-    ctx->prof_end(pe);
-    ++ctx->launches;
-    CK(cudaGetLastError());
-    if (g_inout) return gradient_roundtrip_end(ctx, g_inout);
-    return IPCGPU_OK;
+    const FrictionArgs p = friction_args(ctx, eps2, coef, 0);
+    return gradient_call(ctx, kSerial, g_inout, [&](cudaStream_t st) { friction_gradient(p, ctx->g.p, st); });
 }
 
 int ipcgpu_friction_hessian(ipcgpu_ctx* ctx, double eps2, double coef, int projectDBC, double* a_inout)
 {
     REQUIRE_FRICTION();
     REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive");
-    REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
-    CK(cudaSetDevice(ctx->device));
-    ENTER(kSerial);
-    int rc;
-    if (a_inout && (rc = upload_values(ctx, a_inout))) return rc;
-    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
-    friction_hessian(friction_args(ctx, eps2, coef, projectDBC), ctx->a.p, ctx->iter.p->flags + FLAG_PATTERN, ctx->stream);
-    ctx->prof_end(pe);
-    ++ctx->launches;
-    CK(cudaGetLastError());
-    if (a_inout) {
-        if ((rc = download_values(ctx, a_inout))) return rc;
-        if ((rc = fetch_iter_state(ctx))) return rc;
-        if (ctx->h_iter->flags[FLAG_PATTERN]) {
-            int only[8] = { 0 };
-            only[FLAG_PATTERN] = 1;
-            clear_flag(ctx, FLAG_PATTERN);
-            return status_from_flags(ctx, only);
-        }
-    }
-    return IPCGPU_OK;
+    const FrictionArgs p = friction_args(ctx, eps2, coef, projectDBC);
+    return hessian_call(ctx, kSerial, a_inout, 1u << FLAG_PATTERN,
+        [&](cudaStream_t st) { friction_hessian(p, ctx->a.p, ctx->iter.p->flags + FLAG_PATTERN, st); });
 }
 
 // ---- inertia term (Optimizer.cpp:3227-3239, :3439-3450) ---------------------------------------------------------------------
@@ -1782,7 +1678,6 @@ int ipcgpu_set_xtilde(ipcgpu_ctx* ctx, const double* xtilde_soa)
 {
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     REQUIRE(xtilde_soa != nullptr, IPCGPU_ERR_ARG, "null xTilta");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     ALLOC(ctx->xtilde, (size_t)3 * ctx->nV);
     CK(cudaMemcpyAsync(ctx->xtilde.p, xtilde_soa, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
@@ -1793,40 +1688,23 @@ int ipcgpu_set_xtilde(ipcgpu_ctx* ctx, const double* xtilde_soa)
 int ipcgpu_inertia_energy(ipcgpu_ctx* ctx, double* E)
 {
     REQUIRE(ctx->xtilde_set && ctx->has_mass, IPCGPU_ERR_STATE, "ipcgpu_set_xtilde and a mass diagonal (ipcgpu_set_mesh) first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     // vertex blocks [nV r / N, nV (r+1) / N): every vertex exactly once across the ranks
     const int v0 = (int)((long long)ctx->nV * ctx->rank / ctx->nranks), v1 = (int)((long long)ctx->nV * (ctx->rank + 1) / ctx->nranks);
     ALLOC(ctx->in_partials, (size_t)inertia_energy_blocks(ctx->nV) + 8);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_ELASTIC_ENERGY);
     inertia_energy(v0, v1, ctx->nV, ctx->V.p, ctx->xtilde.p, ctx->mass.p, ctx->in_partials.p, ctx->stream);
-    reduce_sum(ctx->in_partials.p, inertia_energy_blocks(v1 - v0), 1.0, ctx->scalar_out.p + 3, ctx->stream);
-    ctx->prof_end(pe);
-    ctx->launches += 2;
-    if (ctx->nranks > 1 && E) {
-        int r = g_nccl.AllReduce(ctx->scalar_out.p + 3, ctx->scalar_out.p + 3, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
-        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(inertia energy) failed");
-    }
-    energy_store(ctx->iter.p, 3, ctx->scalar_out.p + 3, ctx->stream);
-    ++ctx->launches;
-    ctx->energy_local[3] = (ctx->nranks > 1 && !E);
-    CK(cudaGetLastError());
-    if (E) {
-        CK(cudaMemcpyAsync(ctx->h_scalar, ctx->scalar_out.p + 3, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *E = ctx->h_scalar[0];
-    }
-    return IPCGPU_OK;
+    return energy_tail(ctx, kEnergyInertia, ctx->in_partials.p, inertia_energy_blocks(v1 - v0), 1.0, pe, E);
 }
 
 int ipcgpu_inertia_gradient(ipcgpu_ctx* ctx, int projectDBC, double* g_inout)
 {
     REQUIRE(ctx->xtilde_set && ctx->has_mass, IPCGPU_ERR_STATE, "ipcgpu_set_xtilde and a mass diagonal (ipcgpu_set_mesh) first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     if (g_inout) CK(cudaMemcpyAsync(ctx->g.p, g_inout, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     // Device-resident form with several ranks: the gradient is summed over the ranks later (ipcgpu_allreduce_grad_hess), so only rank 0 adds
-    // the per-vertex term.  Host form: every rank holds the caller's vector and adds the full term -- no reduction needed.
+    // the per-vertex term.  Host form: every rank holds the caller's vector and adds the full term -- no reduction needed, which is why this
+    // is not a gradient_call (whose host form sums the ranks' vectors).
     if (g_inout || ctx->nranks == 1 || ctx->rank == 0) {
         inertia_gradient(ctx->nV, ctx->V.p, ctx->xtilde.p, ctx->mass.p, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, ctx->g.p, ctx->stream);
         ++ctx->launches;
@@ -1860,7 +1738,6 @@ int ipcgpu_set_halfspaces(ipcgpu_ctx* ctx, int n, const double* origin, const do
     REQUIRE(n >= 0 && n <= kMaxPlanes, IPCGPU_ERR_ARG, "at most 8 half-spaces");
     REQUIRE(n == 0 || (origin && normal && friction), IPCGPU_ERR_ARG, "null half-space arrays");
     REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     std::vector<double> par((size_t)kPlaneStride * std::max(n, 1), 0.0);
     for (int k = 0; k < n; ++k) {
@@ -1878,7 +1755,12 @@ int ipcgpu_set_halfspaces(ipcgpu_ctx* ctx, int n, const double* origin, const do
     if (n != ctx->n_hs) {
         ++ctx->epoch; // the graphs captured with the old number of planes are refused (launch shapes and calls change)
         ctx->hs_set_built = ctx->hs_lag_ready = false;
-        CK(cudaMemsetAsync(&ctx->iter.p->hs_energy[0], 0, offsetof(IterState, pat_nnz) - offsetof(IterState, hs_energy), ctx->stream));
+        // the plane energies and the hs_* words start from zero, and no rank-local share of the old planes is left for the fetch to sum
+        IterState* ist = ctx->iter.p;
+        CK(cudaMemsetAsync(&ist->energy[kEnergyPlaneBarrier], 0, sizeof(double), ctx->stream));
+        CK(cudaMemsetAsync(&ist->energy[kEnergyPlaneFriction], 0, sizeof(double), ctx->stream));
+        CK(cudaMemsetAsync(&ist->hs_alpha, 0, offsetof(IterState, pat_nnz) - offsetof(IterState, hs_alpha), ctx->stream));
+        set_local(ctx, (1u << kEnergyPlaneBarrier) | (1u << kEnergyPlaneFriction) | kLocalCrossings, false);
     }
     ctx->n_hs = n;
     if (n > 0) {
@@ -1920,7 +1802,6 @@ int ipcgpu_halfspace_constraint_set(ipcgpu_ctx* ctx, double dHat, int* n_active)
     if (n_active) *n_active = 0;
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE(ctx->surface_ready && ctx->nSV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_surface with surface vertices first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = halfspace_alloc(ctx);
     if (rc) return rc;
@@ -1946,76 +1827,19 @@ int ipcgpu_halfspace_energy(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
     if (E) *E = 0.0;
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_SET();
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     const HalfSpaceArgs p = halfspace_args(ctx);
-    double* out = &ctx->iter.p->hs_energy[0];
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     halfspace_energy(p, dHat, ctx->hs_partials.p, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE], ctx->stream);
-    reduce_sum(ctx->hs_partials.p, halfspace_energy_blocks(), kappa, out, ctx->stream);
-    ctx->prof_end(pe);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
-    ctx->hs_local[0] = ctx->nranks > 1 && !E;
-    if (!E) return IPCGPU_OK;
-    if (ctx->nranks > 1) {
-        int r = g_nccl.AllReduce(out, out, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
-        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(half-space energy) failed");
-    }
-    int rc = fetch_iter_state(ctx);
-    if (rc) return rc;
-    *E = ctx->h_iter->hs_energy[0];
-    if (ctx->h_iter->flags[FLAG_NONPOSITIVE_DISTANCE]) {
-        clear_flag(ctx, FLAG_NONPOSITIVE_DISTANCE);
-        int only[8] = { 0 };
-        only[FLAG_NONPOSITIVE_DISTANCE] = 1;
-        return status_from_flags(ctx, only);
-    }
-    return IPCGPU_OK;
+    return energy_tail(ctx, kEnergyPlaneBarrier, ctx->hs_partials.p, halfspace_energy_blocks(), kappa, pe, E, true, 1u << FLAG_NONPOSITIVE_DISTANCE);
 }
-
-} // extern "C"
-
-// NULL output: the term on the derivative chain; host output: the caller's vector in, the term added on the main stream, the (rank-summed)
-// vector out
-template <typename Launch>
-static int halfspace_gradient_call(ipcgpu_ctx* ctx, double* g_inout, Launch launch)
-{
-    CK(cudaSetDevice(ctx->device));
-    ENTER(g_inout ? kSerial : kDerivative);
-    int rc;
-    if (g_inout && (rc = gradient_roundtrip_begin(ctx, g_inout))) return rc;
-    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
-    launch(ctx->deriv_stream());
-    ctx->prof_end(pe);
-    ++ctx->launches;
-    CK(cudaGetLastError());
-    return g_inout ? gradient_roundtrip_end(ctx, g_inout) : IPCGPU_OK;
-}
-template <typename Launch>
-static int halfspace_hessian_call(ipcgpu_ctx* ctx, double* a_inout, Launch launch)
-{
-    REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
-    CK(cudaSetDevice(ctx->device));
-    ENTER(a_inout ? kSerial : kDerivative);
-    int rc;
-    if (a_inout && (rc = upload_values(ctx, a_inout))) return rc;
-    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
-    launch(ctx->deriv_stream());
-    ctx->prof_end(pe);
-    ++ctx->launches;
-    CK(cudaGetLastError());
-    return a_inout ? download_values(ctx, a_inout) : IPCGPU_OK;
-}
-
-extern "C" {
 
 int ipcgpu_halfspace_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* g_inout)
 {
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_SET();
     const HalfSpaceArgs p = halfspace_args(ctx);
-    return halfspace_gradient_call(ctx, g_inout, [&](cudaStream_t st) { halfspace_gradient(p, dHat, kappa, ctx->g.p, st); });
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { halfspace_gradient(p, dHat, kappa, ctx->g.p, st); });
 }
 
 int ipcgpu_halfspace_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC, double* a_inout)
@@ -2023,14 +1847,13 @@ int ipcgpu_halfspace_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int pro
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_SET();
     const HalfSpaceArgs p = halfspace_args(ctx);
-    return halfspace_hessian_call(ctx, a_inout, [&](cudaStream_t st) { halfspace_hessian(p, dHat, kappa, projectDBC, ctx->a.p, st); });
+    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) { halfspace_hessian(p, dHat, kappa, projectDBC, ctx->a.p, st); });
 }
 
 int ipcgpu_halfspace_step(ipcgpu_ctx* ctx, const double* p_dir, double slackness, double* alpha_inout)
 {
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(p_dir || alpha_inout ? kSerial : kStepBound);
     int rc = upload_dir(ctx, p_dir);
     if (rc) return rc;
@@ -2052,12 +1875,11 @@ int ipcgpu_halfspace_crossings(ipcgpu_ctx* ctx, int* n)
 {
     if (n) *n = 0;
     if (ctx->n_hs == 0) return IPCGPU_OK;
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     halfspace_crossings(halfspace_args(ctx), ctx->iter.p, ctx->stream);
     ctx->launches += 2;
     CK(cudaGetLastError());
-    ctx->hs_local[2] = ctx->nranks > 1 && !n;
+    set_local(ctx, kLocalCrossings, ctx->nranks > 1 && !n);
     if (!n) return IPCGPU_OK;
     if (ctx->nranks > 1) {
         int r = g_nccl.AllReduce(&ctx->iter.p->hs_crossings, &ctx->iter.p->hs_crossings, 1, kNcclInt32, kNcclSum, ctx->nccl_comm, ctx->stream);
@@ -2074,7 +1896,6 @@ int ipcgpu_halfspace_friction_lag(ipcgpu_ctx* ctx, double dHat, double kappa, in
     if (n_lagged) *n_lagged = 0;
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_SET();
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     halfspace_lag(halfspace_args(ctx), dHat, kappa, ctx->hs_pstart.p, ctx->hs_lag.p, ctx->hs_lam.p, ctx->hs_cnt.p + 1, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE],
         ctx->iter.p, ctx->stream);
@@ -2099,25 +1920,10 @@ int ipcgpu_halfspace_friction_energy(ipcgpu_ctx* ctx, double eps2, double* E)
     if (E) *E = 0.0;
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_LAG();
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
-    double* out = &ctx->iter.p->hs_energy[1];
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     halfspace_friction_energy(halfspace_args(ctx), eps2, ctx->hs_partials.p, ctx->stream);
-    reduce_sum(ctx->hs_partials.p, halfspace_energy_blocks(), 1.0, out, ctx->stream);
-    ctx->prof_end(pe);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
-    ctx->hs_local[1] = ctx->nranks > 1 && !E;
-    if (!E) return IPCGPU_OK;
-    if (ctx->nranks > 1) {
-        int r = g_nccl.AllReduce(out, out, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
-        REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(half-space friction energy) failed");
-    }
-    int rc = fetch_iter_state(ctx);
-    if (rc) return rc;
-    *E = ctx->h_iter->hs_energy[1];
-    return IPCGPU_OK;
+    return energy_tail(ctx, kEnergyPlaneFriction, ctx->hs_partials.p, halfspace_energy_blocks(), 1.0, pe, E, true);
 }
 
 int ipcgpu_halfspace_friction_gradient(ipcgpu_ctx* ctx, double eps2, double* g_inout)
@@ -2125,7 +1931,7 @@ int ipcgpu_halfspace_friction_gradient(ipcgpu_ctx* ctx, double eps2, double* g_i
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_LAG();
     const HalfSpaceArgs p = halfspace_args(ctx);
-    return halfspace_gradient_call(ctx, g_inout, [&](cudaStream_t st) { halfspace_friction_gradient(p, eps2, ctx->g.p, st); });
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { halfspace_friction_gradient(p, eps2, ctx->g.p, st); });
 }
 
 int ipcgpu_halfspace_friction_hessian(ipcgpu_ctx* ctx, double eps2, int projectDBC, double* a_inout)
@@ -2133,7 +1939,7 @@ int ipcgpu_halfspace_friction_hessian(ipcgpu_ctx* ctx, double eps2, int projectD
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_LAG();
     const HalfSpaceArgs p = halfspace_args(ctx);
-    return halfspace_hessian_call(ctx, a_inout, [&](cudaStream_t st) { halfspace_friction_hessian(p, eps2, projectDBC, ctx->a.p, st); });
+    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) { halfspace_friction_hessian(p, eps2, projectDBC, ctx->a.p, st); });
 }
 
 int ipcgpu_get_halfspace_sets(ipcgpu_ctx* ctx, int* n_active, int* active2, int* n_lagged, int* lagged2, double* lambda)
@@ -2141,7 +1947,6 @@ int ipcgpu_get_halfspace_sets(ipcgpu_ctx* ctx, int* n_active, int* active2, int*
     if (n_active) *n_active = 0;
     if (n_lagged) *n_lagged = 0;
     if (ctx->n_hs == 0 || !ctx->hs_set_built) return IPCGPU_OK;
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = halfspace_sync_counts(ctx);
     if (rc) return rc;
@@ -2164,8 +1969,7 @@ int ipcgpu_get_halfspace_sets(ipcgpu_ctx* ctx, int* n_active, int* active2, int*
 static ipcgpu_ctx::HostState snapshot_host_state(const ipcgpu_ctx* ctx)
 {
     ipcgpu_ctx::HostState h;
-    for (int s = 0; s < 4; ++s) h.energy_local[s] = ctx->energy_local[s];
-    h.checks_local = ctx->checks_local;
+    h.local_scalars = ctx->local_scalars;
     h.lists_local = ctx->lists_local;
     h.lists_global = ctx->cw.lists_global;
     h.want_cand = ctx->cw.want_cand;
@@ -2174,15 +1978,13 @@ static ipcgpu_ctx::HostState snapshot_host_state(const ipcgpu_ctx* ctx)
     h.inputs_marked = false; // events recorded inside a capture cannot be waited on outside of it
     h.scatter_marked = false;
     h.nC = ctx->cw.nC; h.nP = ctx->cw.nP; h.nK = ctx->cw.nK; h.fr_host_n = ctx->cw.fr_host_n;
-    for (int s = 0; s < 3; ++s) h.hs_local[s] = ctx->hs_local[s];
     h.hs_set_built = ctx->hs_set_built;
     h.hs_lag_ready = ctx->hs_lag_ready;
     return h;
 }
 static void apply_host_state(ipcgpu_ctx* ctx, const ipcgpu_ctx::HostState& h)
 {
-    for (int s = 0; s < 4; ++s) ctx->energy_local[s] = h.energy_local[s];
-    ctx->checks_local = h.checks_local;
+    ctx->local_scalars = h.local_scalars;
     ctx->lists_local = h.lists_local;
     ctx->cw.lists_global = h.lists_global;
     ctx->cw.want_cand = h.want_cand;
@@ -2191,7 +1993,6 @@ static void apply_host_state(ipcgpu_ctx* ctx, const ipcgpu_ctx::HostState& h)
     ctx->inputs_marked = h.inputs_marked;
     ctx->scatter_marked = h.scatter_marked;
     ctx->cw.nC = h.nC; ctx->cw.nP = h.nP; ctx->cw.nK = h.nK; ctx->cw.fr_host_n = h.fr_host_n;
-    for (int s = 0; s < 3; ++s) ctx->hs_local[s] = h.hs_local[s];
     ctx->hs_set_built = h.hs_set_built;
     ctx->hs_lag_ready = h.hs_lag_ready;
 }
@@ -2200,7 +2001,6 @@ int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
 {
     REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is already in progress");
     REQUIRE(!ctx->profiling, IPCGPU_ERR_STATE, "switch the stage timers off (ipcgpu_profile(ctx, 0)) before capturing");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     ctx->inputs_marked = false;  // the side-stream fork of the pair Hessians must hang on an event recorded INSIDE the capture
     ctx->scatter_marked = false;
@@ -2278,7 +2078,6 @@ int ipcgpu_graph_launch(ipcgpu_ctx* ctx, int graph_id)
     REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is in progress");
     const ipcgpu_ctx::GraphRec& rec = ctx->graphs[graph_id];
     REQUIRE(rec.epoch == ctx->epoch, IPCGPU_ERR_STATE, "the scene, pattern, partition or capacities changed since this graph was captured: capture it again");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     if (ctx->a_all_dirty && !rec.dirty_at_begin) // a cross-rank completion filled rows the captured clear does not cover
         CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)(ctx->device_pattern ? ctx->pw.nnz_cap : ctx->nnz) * sizeof(double), ctx->stream));
@@ -2320,22 +2119,21 @@ int ipcgpu_graph_kernel_priorities(ipcgpu_ctx* ctx, int graph_id, int* n_high, i
 // ---- line-search safeguards (SURVEY 8(f) rank 2) -----------------------------------------------------------------------
 static int reduce_checks(ipcgpu_ctx* ctx)
 {
-    if (ctx->nranks > 1 && ctx->checks_local) {
+    if (ctx->nranks > 1 && (ctx->local_scalars & kLocalChecks)) {
         int r = g_nccl.AllReduce(ctx->iter.p->checks, ctx->iter.p->checks, 2, kNcclInt32, kNcclSum, ctx->nccl_comm, ctx->stream);
         REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(safeguard counts) failed");
     }
-    ctx->checks_local = false;
+    set_local(ctx, kLocalChecks, false);
     return IPCGPU_OK;
 }
 
 int ipcgpu_check_inversion(ipcgpu_ctx* ctx, int* n_inverted)
 {
     REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     int rc = safeguard_inversion(ctx);
     REQUIRE(rc == 0, rc, "inversion check launch failed");
-    ctx->checks_local = true;
+    set_local(ctx, kLocalChecks, true);
     if (n_inverted) {
         CK(cudaMemsetAsync(&ctx->iter.p->checks[1], 0, sizeof(int), ctx->stream)); // (the partner count is not pending: keep the sum clean)
         if ((rc = reduce_checks(ctx))) return rc;
@@ -2348,13 +2146,12 @@ int ipcgpu_check_inversion(ipcgpu_ctx* ctx, int* n_inverted)
 int ipcgpu_intersection_free(ipcgpu_ctx* ctx, int* ok)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_HASH);
     int rc = safeguard_intersections(ctx);
     ctx->prof_end(pe);
     REQUIRE(rc == 0, rc, "intersection check launch failed");
-    ctx->checks_local = true;
+    set_local(ctx, kLocalChecks, true);
     if (ok) {
         CK(cudaMemsetAsync(&ctx->iter.p->checks[0], 0, sizeof(int), ctx->stream));
         if ((rc = reduce_checks(ctx))) return rc;
@@ -2480,10 +2277,9 @@ int ipcgpu_ccd_cfl_ti(ipcgpu_ctx* ctx, double dHat, int first_iteration, double 
 {
     REQUIRE(err_vf && err_ee, IPCGPU_ERR_ARG, "null argument");
     REQUIRE(dHat > 0.0 && voxel_size > 0.0, IPCGPU_ERR_ARG, "dHat and the voxel size must be positive");
-    CK(cudaSetDevice(ctx->device));
+    ENTER(alpha_inout ? kSerial : kStepBound);
     int rc = step_control_prepare(ctx);
     if (rc) return rc;
-    ENTER(alpha_inout ? kSerial : kStepBound);
     if (alpha_inout && (rc = ipcgpu_step_bound_set(ctx, *alpha_inout))) return rc;
     cfl_pmax(ctx->nSV, ctx->SVI.p, ctx->nVdof, ctx->dir.p, ctx->iter.p, ctx->stream);
     ctx->launches += 2;
@@ -2590,10 +2386,9 @@ int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* t, doubl
     REQUIRE(ctx->n_hs == 0 || ctx->hs_set_built, IPCGPU_ERR_STATE, "half-spaces: ipcgpu_halfspace_constraint_set first (E0 takes the sets held on entry)");
     REQUIRE(!(ls_terms(ctx, *t) & kTermHalfSpaceFriction) || ctx->prev_set, IPCGPU_ERR_STATE, "half-space friction: ipcgpu_set_prev_state first");
     REQUIRE(!(ctx->capturing && ctx->canonical_order), IPCGPU_ERR_STATE, "inside a capture the line search needs ipcgpu_set_canonical_order(ctx, 0)");
-    CK(cudaSetDevice(ctx->device));
+    ENTER(kSerial);
     int rc = step_control_prepare(ctx);
     if (rc) return rc;
-    ENTER(kSerial);
     if (alpha_inout && (rc = ipcgpu_step_bound_set(ctx, *alpha_inout))) return rc;
     if ((rc = cond_node(ctx, false, kLsEntry, 0.0, 0, [&]() { return line_search_body(ctx, *t); }))) return rc;
     ctx->sc_pending = true;
@@ -2604,13 +2399,13 @@ int ipcgpu_step_control_info(ipcgpu_ctx* ctx, ipcgpu_step_control* out)
 {
     REQUIRE(out != nullptr, IPCGPU_ERR_ARG, "null output");
     REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is in progress");
-    CK(cudaSetDevice(ctx->device));
     if (ctx->sc_pending) {
         ENTER(kSerial);
         int rc = fetch_iter_state(ctx);
         if (rc) return rc;
         ctx->sc_pending = false;
     }
+    else CK(cudaSetDevice(ctx->device)); // (reads the host mirror: no need to join the derivative chain)
     const IterState& h = *ctx->h_iter;
     out->alpha_cfl = h.sc_alpha_cfl;
     out->alpha_feasible = h.ls_LF;
@@ -2634,7 +2429,6 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
     REQUIRE(ctx->nnz > 0 && ctx->n_rows == 3 * ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
     REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the built-in solver runs on one rank (a distributed solver takes each rank's rows: ipcgpu_partition_info)");
     REQUIRE(rel_tol > 0.0 && max_iter > 0, IPCGPU_ERR_ARG, "bad tolerance / iteration limit");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     {
         int rcp = sync_pattern_mirror(ctx);
@@ -2699,38 +2493,27 @@ int ipcgpu_allreduce_grad_hess(ipcgpu_ctx* ctx, int with_gradient, int with_hess
 int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
 {
     REQUIRE(out != nullptr, IPCGPU_ERR_ARG, "null output");
-    CK(cudaSetDevice(ctx->device));
     ENTER(kSerial);
     if (ctx->nranks > 1) {
-        // complete the deferred scalars across ranks in ONE collective: locally summed energies, the error flags (so that every rank
-        // returns the same status) and the safeguard counts (round 2, first half: up to six separate NCCL calls here)
-        unsigned mask = 0;
-        for (int s = 0; s < 4; ++s)
-            if (ctx->energy_local[s]) mask |= 1u << s;
-        if (ctx->checks_local) mask |= 1u << 4;
-        unsigned hs_mask = 0; // with planes: their energies and crossing count ride in the same collective, 3 doubles behind the 14
-        for (int s = 0; s < 3; ++s)
-            if (ctx->n_hs > 0 && ctx->hs_local[s]) hs_mask |= 1u << s;
+        // complete the deferred scalars across ranks in ONE collective: the shares still local (local_scalars) and the error flags (so
+        // that every rank returns the same status)
+        double* buf = ctx->packed_scalars.p;
         cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_ALLREDUCE);
-        pack_scalars(ctx->iter.p, mask, ctx->scalar_out.p + 16, ctx->stream);
-        if (ctx->n_hs > 0) halfspace_pack(ctx->iter.p, hs_mask, ctx->scalar_out.p + 30, ctx->stream);
-        int r = g_nccl.AllReduce(ctx->scalar_out.p + 16, ctx->scalar_out.p + 16, ctx->n_hs > 0 ? 17 : 14, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
-        unpack_scalars(ctx->iter.p, mask, ctx->scalar_out.p + 16, ctx->stream);
-        if (ctx->n_hs > 0) halfspace_unpack(ctx->iter.p, hs_mask, ctx->scalar_out.p + 30, ctx->stream);
+        pack_scalars(ctx->iter.p, ctx->local_scalars, buf, ctx->stream);
+        int r = g_nccl.AllReduce(buf, buf, kPackedScalars, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream);
+        unpack_scalars(ctx->iter.p, ctx->local_scalars, buf, ctx->stream);
         ctx->prof_end(pe);
-        ctx->launches += ctx->n_hs > 0 ? 4 : 2;
+        ctx->launches += 2;
         REQUIRE(r == 0, IPCGPU_ERR_NCCL, "ncclAllReduce(iteration scalars) failed");
-        for (int s = 0; s < 4; ++s) ctx->energy_local[s] = false;
     }
-    for (int s = 0; s < 3; ++s) ctx->hs_local[s] = false;
-    ctx->checks_local = false;
+    ctx->local_scalars = 0;
     int rc = ccd_read_back(ctx, nullptr);
     if (rc || (rc = refresh_pattern_mirror(ctx))) return rc;
     const IterState& h = *ctx->h_iter;
-    out->energy_elastic = h.energy[0];
-    out->energy_barrier = h.energy[1];
-    out->energy_friction = h.energy[2];
-    out->energy_inertia = h.energy[3];
+    out->energy_elastic = h.energy[kEnergyElastic];
+    out->energy_barrier = h.energy[kEnergyBarrier];
+    out->energy_friction = h.energy[kEnergyFriction];
+    out->energy_inertia = h.energy[kEnergyInertia];
     out->alpha_inversion = h.alpha_stage[0];
     out->alpha_partial_ccd = h.alpha_stage[1];
     out->alpha_swept_grid = h.alpha_stage[2];
@@ -2743,8 +2526,8 @@ int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
     out->ti_warnings = (uint64_t)h.flags[FLAG_TI_WARNINGS];
     out->n_inverted_tets = h.checks[0];
     out->n_intersected_triangles = h.checks[1];
-    out->energy_halfspace = h.hs_energy[0];
-    out->energy_halfspace_friction = h.hs_energy[1];
+    out->energy_halfspace = h.energy[kEnergyPlaneBarrier];
+    out->energy_halfspace_friction = h.energy[kEnergyPlaneFriction];
     out->alpha_halfspace = h.hs_alpha;
     out->n_halfspace_active = h.hs_n_active;
     out->n_halfspace_crossings = h.hs_crossings;
@@ -2872,6 +2655,7 @@ int ipcgpu_download_range(ipcgpu_ctx* ctx, int which, uint64_t offset, uint64_t 
 {
     double* p;
     uint64_t n;
+    ENTER(kSerial);
     {
         int rcp = sync_pattern_mirror(ctx);
         if (rcp) return rcp;
@@ -2882,7 +2666,6 @@ int ipcgpu_download_range(ipcgpu_ctx* ctx, int which, uint64_t offset, uint64_t 
         REQUIRE(bi == 0, IPCGPU_ERR_ARG, "unknown buffer id");
     }
     REQUIRE((dst || count == 0) && offset + count <= n, IPCGPU_ERR_ARG, "download: bad destination or range");
-    ENTER(kSerial);
     if (count) CK(cudaMemcpyAsync(dst, p + offset, count * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return IPCGPU_OK;

@@ -163,9 +163,8 @@ struct ipcgpu_ctx {
     ipcgpu::IterState* h_iter = nullptr;
     double pSize = 0.0;     // mean |p| over the surface vertices (SpatialHash.hpp:603-612), computed when p is uploaded
     bool dir_valid = false, pSize_surface = false;
-    bool energy_local[4] = { false, false, false, false }; // IterState::energy[s] still holds this rank's partial sum
+    unsigned local_scalars = 0;              // kLocal* bits (kernels.h): IterState scalars that still hold this rank's share
     bool a_all_dirty = false;                // a cross-rank completion filled rows this rank does not own
-    bool checks_local = false;               // IterState::checks still holds this rank's partial counts
     std::vector<int> h_ia;                   // host copy of the CSR row starts (value range of the owned rows)
 
     // mesh
@@ -199,7 +198,6 @@ struct ipcgpu_ctx {
     ipcgpu::DevBuf<unsigned char> hs_scan;
     size_t hs_scan_bytes = 0;
     bool hs_set_built = false, hs_lag_ready = false;
-    bool hs_local[3] = { false, false, false }; // IterState::hs_energy[0], [1], hs_crossings still hold this rank's share
     size_t ccd_capacity = (size_t)1 << 23; // candidate pairs
     std::vector<int> h_SVI;                // host copy (pSize of the swept build is a serial host sum, SpatialHash.hpp:603-612)
     double debug_prune_seed = -1.0;        // test hook, see ipcgpu_ccd_debug_seed_bound
@@ -234,15 +232,16 @@ struct ipcgpu_ctx {
     ipcgpu::DevBuf<double> sol, pcg_b, pcg_r, pcg_p, pcg_q, pcg_minv, pcg_scal, pcg_hist;
 
     // work / result buffers
-    ipcgpu::DevBuf<double> gcont, hblk, g, e_per_tet, partials, scalar_out, inv_steps, dir, in_partials, e_partials2;
+    ipcgpu::DevBuf<double> gcont, hblk, g, e_per_tet, partials, inv_steps, dir, in_partials, e_partials2;
+    ipcgpu::DevBuf<double> packed_scalars; // the fetch's cross-rank sum (kPackedScalars)
     ipcgpu::DevBuf<double> pSize_dev; // mean |p| of the uploaded search direction, read by the swept-grid kernel from device memory (graph replay)
 
     // CUDA graphs of device-resident call sequences (ipcgpu_capture_begin / _end / ipcgpu_graph_launch).  A captured sequence mutates a
     // few host-side state words (which scalars are still rank-local, which lists are global ...); they are snapshotted at the end of the
     // capture and re-applied at every replay.  `epoch` is bumped by every call that may reallocate or re-partition: older graphs are refused.
     struct HostState {
-        bool energy_local[4], checks_local, lists_local, lists_global, want_cand, swept_ready, fr_ready, inputs_marked, scatter_marked;
-        bool hs_local[3], hs_set_built, hs_lag_ready;
+        unsigned local_scalars;
+        bool lists_local, lists_global, want_cand, swept_ready, fr_ready, inputs_marked, scatter_marked, hs_set_built, hs_lag_ready;
         int nC, nP, nK, fr_host_n;
     };
     struct GraphRec {

@@ -578,10 +578,6 @@ __global__ void k_step_set(IterState* st, double alpha)
 {
     if (threadIdx.x == 0) st->step_ord = dbl_to_ord(alpha);
 }
-__global__ void k_energy_store(IterState* st, int slot, const double* __restrict__ src)
-{
-    if (threadIdx.x == 0) st->energy[slot] = *src;
-}
 
 __global__ void __launch_bounds__(256) k_inversion_step(ElasticArgs p, const double* __restrict__ dir /* interleaved 3nV */, double slack,
     double* __restrict__ per_tet, unsigned long long* __restrict__ min_ord)
@@ -633,18 +629,12 @@ __global__ void __launch_bounds__(256) k_inversion_step(ElasticArgs p, const dou
 // ---------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------
-template <int ENERGY>
-static void launch_energy(const ElasticArgs& p, double* e_per_tet, double* partials, double coef, double* out, cudaStream_t st)
+void elastic_energy(const ElasticArgs& p, double* e_per_tet, double* partials, cudaStream_t st)
 {
-    const int n = p.t_end - p.t_begin;
-    const int nb = (n + 255) / 256;
-    if (nb > 0) k_elastic_energy<ENERGY><<<nb, 256, 0, st>>>(p, e_per_tet, partials);
-    k_reduce_sum<<<1, 1024, 0, st>>>(partials, nb, coef, out);
-}
-void elastic_energy(const ElasticArgs& p, double* e_per_tet, double* partials, double coef, double* out, cudaStream_t st)
-{
-    if (p.energy == 0) launch_energy<0>(p, e_per_tet, partials, coef, out, st);
-    else launch_energy<1>(p, e_per_tet, partials, coef, out, st);
+    const int nb = elastic_energy_blocks(p.t_end - p.t_begin);
+    if (nb <= 0) return;
+    if (p.energy == 0) k_elastic_energy<0><<<nb, 256, 0, st>>>(p, e_per_tet, partials);
+    else k_elastic_energy<1><<<nb, 256, 0, st>>>(p, e_per_tet, partials);
 }
 int elastic_energy_blocks(int nTets) { return (nTets + 255) / 256; }
 void reduce_sum(const double* partials, int n, double scale, double* out, cudaStream_t st) { k_reduce_sum<<<1, 1024, 0, st>>>(partials, n, scale, out); }
@@ -753,24 +743,26 @@ void inversion_step(const ElasticArgs& p, const double* dir, double slack, doubl
 }
 void inversion_apply(IterState* st_dev, int nT, cudaStream_t st) { k_inversion_apply<<<1, 32, 0, st>>>(st_dev, nT); }
 void step_set(IterState* st_dev, double alpha, cudaStream_t st) { k_step_set<<<1, 32, 0, st>>>(st_dev, alpha); }
-void energy_store(IterState* st_dev, int slot, const double* src, cudaStream_t st) { k_energy_store<<<1, 32, 0, st>>>(st_dev, slot, src); }
 
-// Deferred cross-rank scalars of one iteration in ONE collective: the energies that are still local sums, the error flags and the
-// safeguard counts are packed into 14 doubles, sum-all-reduced, and unpacked (a flag is raised iff any rank raised it; integer counts
-// are exact in a double).  local_mask bit s: energy s is a local partial sum; bit 4: the safeguard counts are local.
+// Deferred cross-rank scalars of one iteration in ONE collective (kernels.h: kPackedScalars): buf = the energies, the flags, the checks and
+// the crossing count; a scalar that is not a local share (local_mask) packs as 0 and keeps its value.
+constexpr int kFlags = kEnergySlots, kChecks = kFlags + 8, kCrossings = kChecks + 2;
+static_assert(kCrossings + 1 == kPackedScalars && kPackedScalars <= 32, "one warp packs the scalars");
 __global__ void k_pack_scalars(const IterState* __restrict__ st, unsigned local_mask, double* __restrict__ buf)
 {
     const int i = threadIdx.x;
-    if (i < 4) buf[i] = ((local_mask >> i) & 1u) ? st->energy[i] : 0.0;
-    else if (i < 12) buf[i] = (double)st->flags[i - 4];
-    else if (i < 14) buf[i] = ((local_mask >> 4) & 1u) ? (double)st->checks[i - 12] : 0.0;
+    if (i < kFlags) buf[i] = ((local_mask >> i) & 1u) ? st->energy[i] : 0.0;
+    else if (i < kChecks) buf[i] = (double)st->flags[i - kFlags];
+    else if (i < kCrossings) buf[i] = (local_mask & kLocalChecks) ? (double)st->checks[i - kChecks] : 0.0;
+    else if (i == kCrossings) buf[i] = (local_mask & kLocalCrossings) ? (double)st->hs_crossings : 0.0;
 }
 __global__ void k_unpack_scalars(IterState* __restrict__ st, unsigned local_mask, const double* __restrict__ buf)
 {
     const int i = threadIdx.x;
-    if (i < 4) { if ((local_mask >> i) & 1u) st->energy[i] = buf[i]; }
-    else if (i < 12) st->flags[i - 4] = (int)fmin(buf[i], 2147483647.0);
-    else if (i < 14) { if ((local_mask >> 4) & 1u) st->checks[i - 12] = (int)buf[i]; }
+    if (i < kFlags) { if ((local_mask >> i) & 1u) st->energy[i] = buf[i]; }
+    else if (i < kChecks) st->flags[i - kFlags] = (int)fmin(buf[i], 2147483647.0);
+    else if (i < kCrossings) { if (local_mask & kLocalChecks) st->checks[i - kChecks] = (int)buf[i]; }
+    else if (i == kCrossings) { if (local_mask & kLocalCrossings) st->hs_crossings = (int)buf[i]; }
 }
 void pack_scalars(const IterState* st_dev, unsigned local_mask, double* buf, cudaStream_t st) { k_pack_scalars<<<1, 32, 0, st>>>(st_dev, local_mask, buf); }
 void unpack_scalars(IterState* st_dev, unsigned local_mask, const double* buf, cudaStream_t st) { k_unpack_scalars<<<1, 32, 0, st>>>(st_dev, local_mask, buf); }

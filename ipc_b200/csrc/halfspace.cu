@@ -289,20 +289,6 @@ __global__ void __launch_bounds__(128) k_hs_fric_hessian(HalfSpaceArgs p, double
     }
 }
 
-// the plane scalars of the fetch's single cross-rank sum: buf[0..2] = barrier energy, friction energy, crossings (mask bits 0..2: still local)
-__global__ void k_hs_pack(const IterState* __restrict__ st, unsigned mask, double* __restrict__ buf)
-{
-    const int i = threadIdx.x;
-    if (i < 2) buf[i] = ((mask >> i) & 1u) ? st->hs_energy[i] : 0.0;
-    else if (i == 2) buf[i] = ((mask >> 2) & 1u) ? (double)st->hs_crossings : 0.0;
-}
-__global__ void k_hs_unpack(IterState* __restrict__ st, unsigned mask, const double* __restrict__ buf)
-{
-    const int i = threadIdx.x;
-    if (i < 2) { if ((mask >> i) & 1u) st->hs_energy[i] = buf[i]; }
-    else if (i == 2) { if ((mask >> 2) & 1u) st->hs_crossings = (int)buf[i]; }
-}
-
 constexpr int kHsEnergyBlocks = kSMs;
 int grid_for(long long n, int threads) { return (int)std::max(1LL, std::min((n + threads - 1) / threads, (long long)kSMs * 8)); }
 
@@ -365,7 +351,5 @@ void halfspace_friction_hessian(const HalfSpaceArgs& p, double eps2, int project
 {
     k_hs_fric_hessian<<<kSMs, 128, 0, st>>>(p, eps2, projectDBC, a);
 }
-void halfspace_pack(const IterState* st_dev, unsigned mask, double* buf, cudaStream_t st) { k_hs_pack<<<1, 32, 0, st>>>(st_dev, mask, buf); }
-void halfspace_unpack(IterState* st_dev, unsigned mask, const double* buf, cudaStream_t st) { k_hs_unpack<<<1, 32, 0, st>>>(st_dev, mask, buf); }
 
 } // namespace ipcgpu

@@ -5,6 +5,9 @@
 
 namespace ipcgpu {
 
+// slots of IterState::energy
+enum { kEnergyElastic = 0, kEnergyBarrier, kEnergyFriction, kEnergyInertia, kEnergyPlaneBarrier, kEnergyPlaneFriction, kEnergySlots };
+
 // Device-resident scalars of one Newton iteration.  Every stage reads its inputs from here and leaves its outputs here, so a whole
 // iteration is one stream of launches (and in-stream NCCL reductions) with a single read-back at the end (ipcgpu_fetch_iteration).
 struct IterState {
@@ -17,7 +20,7 @@ struct IterState {
     double alpha_grid;                // sweep length of the last swept grid (after the span rescale of SpatialHash.hpp:603-618)
     double ref_lo[3], ref_inv_h;      // reference swept-grid geometry (SpatialHash.hpp:589-640)
     double alpha_stage[4];            // step after: inversion filter, partial CCD, swept-grid rescale, full CCD
-    double energy[4];                 // elastic, barrier, friction, inertia (cross-rank sums once reduced)
+    double energy[kEnergySlots];      // kEnergy* slots (this rank's share, then cross-rank sums)
     int ref_count[3];
     int n_set[3];                     // active / mollified / candidate counts of the last constraint set (this rank's lists)
     int flags[8];                     // IPCGPU_FLAG_* slots (nonzero = raised); cleared by ipcgpu_fetch_iteration
@@ -35,7 +38,6 @@ struct IterState {
     int ls_stopped, ls_rebuilt, ls_post_ran;
     int ls_cond;                      // the decision word of the last step_decide
     // half-space collision objects (halfspace.cu)
-    double hs_energy[2];              // barrier, friction of the planes (this rank's share, then sums)
     double hs_alpha;                  // step after the plane bound
     int hs_n_active, hs_n_lagged;     // sizes of the plane active set / lagged set (replicated on every rank)
     int hs_crossings;                 // vertices with d <= 0 of the last crossing check (this rank's share, then sums)
@@ -53,6 +55,11 @@ enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersect
 enum { kTermInertia = 1, kTermFriction = 2, kTermHalfSpace = 4, kTermHalfSpaceFriction = 8 };
 enum { FLAG_NONPOSITIVE_DISTANCE = 0, FLAG_SET_CAPACITY = 1, FLAG_CCD_CAPACITY = 2, FLAG_ZERO_CCD_DISTANCE = 3, FLAG_PATTERN = 4, FLAG_TI_WARNINGS = 5, FLAG_EXCHANGE_CAPACITY = 6,
     FLAG_PATTERN_CAPACITY = 7 };
+// Scalars that may still hold this rank's share (ipcgpu_ctx::local_scalars): bit s = energy[s], then checks and hs_crossings.  The fetch
+// completes them in one sum-allreduce of kPackedScalars doubles: the energies, the 8 flags (a flag is raised iff any rank raised it), the
+// 2 checks and the crossing count (integer counts are exact in a double).
+enum : unsigned { kLocalChecks = 1u << kEnergySlots, kLocalCrossings = 1u << (kEnergySlots + 1) };
+constexpr int kPackedScalars = kEnergySlots + 8 + 2 + 1;
 
 struct ElasticArgs {
     int nV, nT;
@@ -70,7 +77,7 @@ struct ElasticArgs {
 };
 
 // elastic.cu
-void elastic_energy(const ElasticArgs& p, double* e_per_tet, double* partials, double coef, double* out, cudaStream_t st);
+void elastic_energy(const ElasticArgs& p, double* e_per_tet, double* partials, cudaStream_t st); // elastic_energy_blocks partial sums of psi * vol
 int elastic_energy_blocks(int nTets);
 // e_partials != nullptr: the kernel also leaves one partial sum of psi * vol per CTA there (elastic_grad_hess_blocks of them)
 // hdst != nullptr: the Hessian blocks go to the SLOT-MAJOR intermediate hcon (destination offsets hdst, 10 per local tet) instead of the tile-major hblk
@@ -90,8 +97,7 @@ void diag_mass_dbc_range(int v0, int v1, const int* ia, int base, const uint8_t*
 void inversion_step(const ElasticArgs& p, const double* dir, double slack, double* per_tet, IterState* st_dev, cudaStream_t st);
 void inversion_apply(IterState* st_dev, int nT, cudaStream_t st);          // Energy.cpp:576-579 on the device-resident step
 void step_set(IterState* st_dev, double alpha, cudaStream_t st);           // step_ord = alpha
-void energy_store(IterState* st_dev, int slot, const double* src, cudaStream_t st);
-void pack_scalars(const IterState* st_dev, unsigned local_mask, double* buf, cudaStream_t st);   // deferred cross-rank scalars -> 14 doubles
+void pack_scalars(const IterState* st_dev, unsigned local_mask, double* buf, cudaStream_t st);   // deferred cross-rank scalars -> kPackedScalars doubles
 void unpack_scalars(IterState* st_dev, unsigned local_mask, const double* buf, cudaStream_t st);
 
 
@@ -209,8 +215,6 @@ void halfspace_lag(const HalfSpaceArgs& p, double dHat, double kappa, const int*
 void halfspace_friction_energy(const HalfSpaceArgs& p, double eps2, double* partials, cudaStream_t st);
 void halfspace_friction_gradient(const HalfSpaceArgs& p, double eps2, double* g, cudaStream_t st);
 void halfspace_friction_hessian(const HalfSpaceArgs& p, double eps2, int projectDBC, double* a, cudaStream_t st);
-void halfspace_pack(const IterState* st_dev, unsigned mask, double* buf, cudaStream_t st);   // 3 doubles behind pack_scalars' 14
-void halfspace_unpack(IterState* st_dev, unsigned mask, const double* buf, cudaStream_t st);
 
 // zero n_words 4-byte words.  A kernel rather than cudaMemsetAsync where the two chains of an iteration overlap (api.cu): replayed from a
 // graph, a memset node has no priority of its own and queues behind whatever low-priority grids are pending, which held the step-bound

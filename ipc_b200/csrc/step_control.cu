@@ -49,11 +49,11 @@ DEV int halve_while(IterState* st, bool bad, int counter)
 // ((E_el + E_in) + (E_b + E_plane_b)) + E_plane_f + E_f: both barrier parts are one kappa bVals.sum() (:3352), plane friction comes first (:3355-3377)
 DEV double energy_sum(const IterState* st, int terms)
 {
-    double e = st->energy[0];
-    if (terms & kTermInertia) e += st->energy[3];
-    e += (terms & kTermHalfSpace) ? st->energy[1] + st->hs_energy[0] : st->energy[1];
-    if (terms & kTermHalfSpaceFriction) e += st->hs_energy[1];
-    if (terms & kTermFriction) e += st->energy[2];
+    double e = st->energy[kEnergyElastic];
+    if (terms & kTermInertia) e += st->energy[kEnergyInertia];
+    e += (terms & kTermHalfSpace) ? st->energy[kEnergyBarrier] + st->energy[kEnergyPlaneBarrier] : st->energy[kEnergyBarrier];
+    if (terms & kTermHalfSpaceFriction) e += st->energy[kEnergyPlaneFriction];
+    if (terms & kTermFriction) e += st->energy[kEnergyFriction];
     return e;
 }
 // the intersection safeguard: surface triangles crossed by an edge, and with half-spaces the vertices with d <= 0 (isIntersected, :2627-2642)
