@@ -194,12 +194,6 @@ int ipcgpu_elastic_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int p
  * (one SVD per tet and iteration instead of two).  E NULL: the energy stays on the device (ipcgpu_fetch_iteration). */
 int ipcgpu_elastic_energy_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int projectDBC, int add_mass,
     double* E, double* g, double* a);
-/* Layout of the per-tet Hessian blocks between the per-tet kernel and the CSR assembly.  0 (default): tile-major (DESIGN.md section 2), one
- * TMA bulk store per tile and block slot, the assembly gathers the 72-byte blocks through an index list; the only layout in which
- * ipcgpu_download(IPCGPU_BUF_TET_HESSIANS) is available.  1: slot-major -- every block is written where the contributions of its CSR block
- * slot are contiguous and the assembly streams them (slower on C5, H100 SXM at 400 W: the scattered block writes take the per-tet kernel from
- * 0.46 to 0.94 ms and the assembly gains nothing).  Results are identical bit for bit. */
-int ipcgpu_set_hessian_layout(ipcgpu_ctx* ctx, int layout);
 /* Energy::filterStepSize (Energy.cpp:565-581); alpha_inout == NULL: the device-resident step */
 int ipcgpu_inversion_step(ipcgpu_ctx* ctx, const double* p_interleaved, double slack, double* alpha_inout);
 
@@ -438,7 +432,7 @@ int ipcgpu_ccd_stats_timing(ipcgpu_ctx* ctx, uint64_t* longest_pair_cycles, uint
 int ipcgpu_ccd_debug_seed_bound(ipcgpu_ctx* ctx, double toi);
 /* TEST HOOK.  boxes >= 0: a thread may evaluate this many boxes of a search in the thread-level pass before it hands the pair on to the
  * warp-level pass, in every later narrow phase of this context (0 hands on every search that does not end at its root box); boxes < 0
- * restores the default (IPCGPU_TI_BUDGET, else 32).  The step bound does not depend on it. */
+ * restores the default, 32.  The step bound does not depend on it. */
 int ipcgpu_ccd_debug_thread_budget(ipcgpu_ctx* ctx, int64_t boxes);
 
 /* ---- linear-solve hand-off with the Hessian resident in HBM (LinSysSolver::factorize/solve, LinSysSolver.hpp:230-236; Optimizer.cpp:2324-2355) ----

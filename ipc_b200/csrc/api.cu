@@ -134,7 +134,7 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 //     hs_pstart and IterState::energy[kEnergyPlaneBarrier / kEnergyPlaneFriction], hs_n_*, hs_crossings); the plane derivative calls read hs_par, hs_act, hs_lag, hs_lam, hs_cnt,
 //     Vprev (written before the fork) and write g / a only; ipcgpu_halfspace_step reads hs_par, SVI, dir and writes IterState::step_ord,
 //     hs_alpha, hs_zero_step only (the derivative chain touches none of them).
-//   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, hcon, e_partials2, bHraw, brows, bpsd:
+//   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, e_partials2, bHraw, brows, bpsd:
 //     derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };
 
@@ -248,7 +248,6 @@ static int build_maps(ipcgpu_ctx* ctx)
         uint64_t key;
         unsigned src;
         unsigned tet;
-        unsigned slot10; // block slot of the tet: 0..3 diagonal blocks, 4..9 the vertex pairs (0,1)(0,2)(0,3)(1,2)(1,3)(2,3)
     };
     std::vector<KS> ks;
     ks.reserve((size_t)10 * nL);
@@ -260,15 +259,15 @@ static int build_maps(ipcgpu_ctx* ctx)
         // tile-major block addresses (elastic.cu): (l/64)*64*78 + o*64 + (l%64)*len
         const unsigned tl = (unsigned)l, tile_base = (tl / 64u) * (64u * 78u), tin = tl % 64u;
         for (int a = 0; a < 4; ++a)
-            if (v[a] >= vb && v[a] < ve) ks.push_back({ ((uint64_t)v[a] << 32) | (uint32_t)v[a], tile_base + 6u * a * 64u + tin * 6u, tl, (unsigned)a });
+            if (v[a] >= vb && v[a] < ve) ks.push_back({ ((uint64_t)v[a] << 32) | (uint32_t)v[a], tile_base + 6u * a * 64u + tin * 6u, tl });
         for (int q = 0; q < 6; ++q) {
             const int lo = std::min(v[pa[q]], v[pb[q]]), hi = std::max(v[pa[q]], v[pb[q]]);
-            if (lo >= vb && lo < ve) ks.push_back({ ((uint64_t)lo << 32) | (uint32_t)hi, tile_base + (24u + 9u * q) * 64u + tin * 9u, tl, 4u + (unsigned)q });
+            if (lo >= vb && lo < ve) ks.push_back({ ((uint64_t)lo << 32) | (uint32_t)hi, tile_base + (24u + 9u * q) * 64u + tin * 9u, tl });
         }
     }
     std::sort(ks.begin(), ks.end(), [](const KS& a, const KS& b) { return a.key < b.key || (a.key == b.key && (a.tet < b.tet || (a.tet == b.tet && a.src < b.src))); });
     std::vector<int> sv, su, cptr;
-    std::vector<unsigned> csrc(std::max<size_t>(ks.size(), 1)), cwho(std::max<size_t>(ks.size(), 1)); // cwho: 10 * local tet + block slot of the contribution
+    std::vector<unsigned> csrc(std::max<size_t>(ks.size(), 1));
     for (size_t i = 0; i < ks.size(); ++i) {
         if (i == 0 || ks[i].key != ks[i - 1].key) {
             sv.push_back((int)(ks[i].key >> 32));
@@ -276,7 +275,6 @@ static int build_maps(ipcgpu_ctx* ctx)
             cptr.push_back((int)i);
         }
         csrc[i] = ks[i].src;
-        cwho[i] = ks[i].tet * 10u + ks[i].slot10;
     }
     cptr.push_back((int)ks.size());
     {
@@ -292,7 +290,7 @@ static int build_maps(ipcgpu_ctx* ctx)
         for (size_t i = 0; i < nS; ++i)
             if (sv[i] == su[i]) order.push_back((int)i);
         std::vector<int> sv2(nS), su2(nS), cptr2;
-        std::vector<unsigned> csrc2(csrc.size()), cwho2(cwho.size());
+        std::vector<unsigned> csrc2(csrc.size());
         cptr2.reserve(nS + 1);
         size_t pos = 0;
         for (size_t k = 0; k < nS; ++k) {
@@ -300,38 +298,19 @@ static int build_maps(ipcgpu_ctx* ctx)
             sv2[k] = sv[i];
             su2[k] = su[i];
             cptr2.push_back((int)pos);
-            for (int c = cptr[i]; c < cptr[i + 1]; ++c) { csrc2[pos] = csrc[c]; cwho2[pos] = cwho[c]; ++pos; }
+            for (int c = cptr[i]; c < cptr[i + 1]; ++c) csrc2[pos++] = csrc[c];
         }
         cptr2.push_back((int)pos);
-        sv.swap(sv2); su.swap(su2); cptr.swap(cptr2); csrc.swap(csrc2); cwho.swap(cwho2);
-    }
-    // slot-major intermediate: the contributions of a slot are contiguous (ascending tet order inside the slot), 6 doubles per diagonal and
-    // 9 per off-diagonal contribution; hdst tells the per-tet kernel where each of a tet's ten blocks goes (0xffffffff: a row this rank does
-    // not own), cbase where a slot's run starts
-    std::vector<unsigned> hdst((size_t)10 * std::max(nL, 1), 0xffffffffu), cbase(sv.size() + 1, 0u);
-    {
-        uint64_t run = 0;
-        for (size_t k = 0; k < sv.size() && !ks.empty(); ++k) {
-            cbase[k] = (unsigned)run;
-            const unsigned len = (sv[k] == su[k]) ? 6u : 9u;
-            for (int c = cptr[k]; c < cptr[k + 1]; ++c) {
-                hdst[cwho[c]] = (unsigned)run;
-                run += len;
-            }
-        }
-        cbase[sv.size()] = (unsigned)run;
-        REQUIRE(run < 0xffffffffull, IPCGPU_ERR_CAPACITY, "slot-major intermediate too large for 32-bit offsets");
+        sv.swap(sv2); su.swap(su2); cptr.swap(cptr2); csrc.swap(csrc2);
     }
     ctx->nSlots = (int)sv.size();
     if (sv.empty()) { sv.push_back(0); su.push_back(0); } // keep the uploads non-empty
     bool ok = ctx->slot_v.upload(sv.data(), sv.size(), ctx->stream) && ctx->slot_u.upload(su.data(), su.size(), ctx->stream)
         && ctx->con_ptr.upload(cptr.data(), cptr.size(), ctx->stream) && ctx->con_src.upload(csrc.data(), csrc.size(), ctx->stream)
-        && ctx->slot_off.reserve((size_t)3 * std::max(1, ctx->nSlots)) && ctx->hdst.upload(hdst.data(), hdst.size(), ctx->stream)
-        && ctx->cbase.upload(cbase.data(), cbase.size(), ctx->stream);
+        && ctx->slot_off.reserve((size_t)3 * std::max(1, ctx->nSlots));
     REQUIRE(ok, IPCGPU_ERR_CUDA, "upload of Hessian scatter map failed");
     ALLOC(ctx->gcont, (size_t)12 * std::max(1, nL));
     ALLOC(ctx->hblk, (size_t)78 * 64 * ((size_t)(std::max(1, nL) + 63) / 64));
-    ALLOC(ctx->hcon, (size_t)78 * std::max(1, nL));
     ALLOC(ctx->partials, (size_t)std::max(1, elastic_energy_blocks(ctx->t_end - ctx->t_begin)) + 8);
     CK(cudaStreamSynchronize(ctx->stream)); // host vectors go out of scope
     ctx->maps_ready = true;
@@ -611,7 +590,12 @@ int ipcgpu_create(int device, ipcgpu_ctx** out)
         || cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, ctx->prio_high) != cudaSuccess
         || cudaStreamCreateWithPriority(&ctx->deriv, cudaStreamNonBlocking, ctx->prio_low) != cudaSuccess
         || cudaEventCreateWithFlags(&ctx->ev_deriv_fork, cudaEventDisableTiming) != cudaSuccess
-        || cudaEventCreateWithFlags(&ctx->ev_deriv_done, cudaEventDisableTiming) != cudaSuccess || cudaMallocHost(&ctx->h_scalar, 512) != cudaSuccess
+        || cudaEventCreateWithFlags(&ctx->ev_deriv_done, cudaEventDisableTiming) != cudaSuccess
+        // side stream for the pair-Hessian build + projection.  Replayed from a graph it wins 0.13 ms per iteration next to the overlapped
+        // derivative chain (H100 SXM, 700 W, C5: 3.39 -> 3.25 ms)
+        || cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&ctx->ev_inputs, cudaEventDisableTiming) != cudaSuccess
+        || cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ctx->ev_scatter, cudaEventDisableTiming) != cudaSuccess
+        || cudaMallocHost(&ctx->h_scalar, 512) != cudaSuccess
         || cudaMallocHost(&hi, sizeof(IterState)) != cudaSuccess || !ctx->flag.reserve(4) || !ctx->packed_scalars.reserve(kPackedScalars) || !ctx->iter.reserve(1)
         || cudaMemsetAsync(ctx->iter.p, 0, sizeof(IterState), ctx->stream) != cudaSuccess) {
         ipcgpu_destroy(ctx);
@@ -619,22 +603,6 @@ int ipcgpu_create(int device, ipcgpu_ctx** out)
     }
     ctx->h_iter = static_cast<IterState*>(hi);
     std::memset(ctx->h_iter, 0, sizeof(IterState));
-    {
-        const char* e = std::getenv("IPCGPU_HESS_LAYOUT");
-        if (e) ctx->hess_layout = std::atoi(e) == 0 ? 0 : 1;
-    }
-    {   // side stream for the pair-Hessian build + projection (IPCGPU_BARRIER_OVERLAP=0 keeps it on the stream of the derivative chain).
-        // Replayed from a graph it wins 0.13 ms per iteration next to the overlapped derivative chain (H100 SXM, 700 W, C5: 3.39 -> 3.25 ms)
-        const char* e = std::getenv("IPCGPU_BARRIER_OVERLAP");
-        if (!(e && std::atoi(e) == 0)) {
-            if (cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&ctx->ev_inputs, cudaEventDisableTiming) != cudaSuccess
-                || cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming) != cudaSuccess
-                || cudaEventCreateWithFlags(&ctx->ev_scatter, cudaEventDisableTiming) != cudaSuccess) {
-                if (ctx->side) cudaStreamDestroy(ctx->side);
-                ctx->side = nullptr; // fall back to the single-stream order
-            }
-        }
-    }
     step_set(ctx->iter.p, 1.0, ctx->stream);
     *out = ctx;
     return IPCGPU_OK;
@@ -914,9 +882,8 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
         ALLOC(ctx->e_partials2, (size_t)elastic_grad_hess_blocks(ctx->n_list) + 8);
         e_part = ctx->e_partials2.p;
     }
-    const bool slot_major = need_h && ctx->hess_layout == 1;
-    elastic_grad_hess(ctx->eargs(), coef, projectSPD, need_g, need_h, ctx->gcont.p, ctx->hblk.p, st, e_part, slot_major ? ctx->hdst.p : nullptr, ctx->hcon.p);
-    ctx->hblk_valid = need_h && !slot_major;
+    elastic_grad_hess(ctx->eargs(), coef, projectSPD, need_g, need_h, ctx->gcont.p, ctx->hblk.p, st, e_part);
+    ctx->hblk_valid = need_h;
     ctx->prof_end(pe);
     ++ctx->launches;
     if (with_energy) { // (which rank's share it is: energy_result, once the call knows whether the host wants it)
@@ -934,12 +901,8 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
     }
     if (need_h) {
         pe = ctx->prof_begin(IPCGPU_STAGE_ASSEMBLE_CSR);
-        if (slot_major)
-            assemble_slot_major(ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->slot_off.p, ctx->cbase.p, ctx->hcon.p, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, 1, ctx->a.p,
-                st);
-        else
-            assemble_csr(ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->slot_off.p, ctx->con_ptr.p, ctx->con_src.p, ctx->hblk.p,
-                ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, nullptr, 1, ctx->a.p, st);
+        assemble_csr(ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->slot_off.p, ctx->con_ptr.p, ctx->con_src.p, ctx->hblk.p,
+            ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, nullptr, 1, ctx->a.p, st);
         // per-vertex diagonal terms (mass, Dirichlet identity) of the owned rows
         const double* m = (add_mass && ctx->has_mass) ? ctx->mass.p : nullptr;
         diag_mass_dbc_range(ctx->v_begin, ctx->v_end, ctx->ia.p, ctx->index_base, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, m, ctx->a.p, st);
@@ -1216,15 +1179,6 @@ int ipcgpu_ccd_stats_timing(ipcgpu_ctx* ctx, uint64_t* longest_pair_cycles, uint
 {
     if (longest_pair_cycles) *longest_pair_cycles = ctx->ccd.last_longest_cycles;
     if (total_pair_cycles) *total_pair_cycles = ctx->ccd.last_total_cycles;
-    return IPCGPU_OK;
-}
-
-int ipcgpu_set_hessian_layout(ipcgpu_ctx* ctx, int layout)
-{
-    ENTER(kSerial);
-    ++ctx->epoch; // graphs captured before this call are refused (another kernel pair)
-    REQUIRE(layout == 0 || layout == 1, IPCGPU_ERR_ARG, "layout: 0 tile-major (per-tet blocks downloadable), 1 slot-major");
-    ctx->hess_layout = layout;
     return IPCGPU_OK;
 }
 
@@ -1512,7 +1466,7 @@ int ipcgpu_barrier_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int proje
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     const BarrierArgs bp = barrier_args(ctx, dHat, kappa, projectDBC);
     cudaStream_t st = ctx->deriv_stream();
-    if (ctx->side && ctx->inputs_marked) {
+    if (ctx->inputs_marked) {
         // build + projection on the side stream, ordered after the last change of their inputs (positions, contact sets) -- i.e. next to
         // whatever has been queued since (the elastic assembly); the scatter joins the derivative chain, after the elastic writes
         CK(cudaStreamWaitEvent(ctx->side, ctx->ev_inputs, 0));
@@ -1523,7 +1477,7 @@ int ipcgpu_barrier_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int proje
     }
     else barrier_hessian_build_project(bp, ctx->iter.p->flags, w.bHraw.p, w.brows.p, w.bpsd.p, w.counters.p + 12, w.cap, st);
     barrier_hessian_scatter(bp, ctx->a.p, ctx->iter.p->flags, w.bHraw.p, w.brows.p, w.bpsd.p, w.counters.p + 12, w.cap, st);
-    if (ctx->side && ctx->ev_scatter) ctx->scatter_marked = (cudaEventRecord(ctx->ev_scatter, st) == cudaSuccess);
+    ctx->scatter_marked = (cudaEventRecord(ctx->ev_scatter, st) == cudaSuccess);
     ctx->prof_end(pe);
     ctx->launches += 3;
     CK(cudaGetLastError());
@@ -2662,7 +2616,7 @@ int ipcgpu_download_range(ipcgpu_ctx* ctx, int which, uint64_t offset, uint64_t 
     }
     {
         const int bi = buf_info(ctx, which, &p, &n);
-        REQUIRE(bi != 2, IPCGPU_ERR_STATE, "the per-tet Hessian blocks are only kept by the tile-major layout: ipcgpu_set_hessian_layout(ctx, 0) before the Hessian call");
+        REQUIRE(bi != 2, IPCGPU_ERR_STATE, "no per-tet Hessian blocks: the last elastic gradient/Hessian call computed no Hessian");
         REQUIRE(bi == 0, IPCGPU_ERR_ARG, "unknown buffer id");
     }
     REQUIRE((dst || count == 0) && offset + count <= n, IPCGPU_ERR_ARG, "download: bad destination or range");

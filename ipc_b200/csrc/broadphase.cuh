@@ -176,58 +176,13 @@ DEV void warp_scan_candidates(const Grid& g, const SortedGrid& sg, const Box& qb
     }
 }
 
-// Pair output of the warp-per-query kernels.  A single global counter hit once per warp and iteration serialises in the L2
-// (~0.6M same-address atomics per launch), so pairs are staged in shared memory per CTA and flushed with ONE global atomic and
-// coalesced stores.
+// Pair output of the broad phase: a list, its device-resident size, its capacity and the overflow flag.
 struct PairOut {
     int2* pairs;
     unsigned* n;
     unsigned cap;
     int* overflow;
 };
-constexpr int kPairStageCap = 4096;     // pairs staged per CTA (32 KB)
-constexpr int kPairQueriesPerWarp = 8;  // queries handled by one warp of the pair-finding kernels
-struct PairStage {
-    int2 buf[kPairStageCap];
-    unsigned count;
-    unsigned base;
-};
-DEV void pair_stage_init(PairStage& st)
-{
-    if (threadIdx.x == 0) st.count = 0;
-    __syncthreads();
-}
-// must be called by all 32 lanes of the warp
-DEV void warp_push_pair(PairStage& st, const PairOut& o, bool want, int a, int b, int lane)
-{
-    const unsigned m = __ballot_sync(0xffffffffu, want);
-    if (m == 0) return;
-    const int leader = __ffs(m) - 1;
-    unsigned base = 0;
-    if (lane == leader) base = atomicAdd(&st.count, (unsigned)__popc(m));
-    base = __shfl_sync(0xffffffffu, base, leader);
-    if (want) {
-        const unsigned i = base + __popc(m & ((1u << lane) - 1u));
-        if (i < (unsigned)kPairStageCap) st.buf[i] = make_int2(a, b);
-        else { // stage full (very dense neighbourhood): straight to the global list
-            const unsigned gi = atomicAdd(o.n, 1u);
-            if (gi < o.cap) o.pairs[gi] = make_int2(a, b);
-            else atomicExch(o.overflow, 1);
-        }
-    }
-}
-// must be called by every thread of the CTA
-DEV void pair_stage_flush(PairStage& st, const PairOut& o)
-{
-    __syncthreads();
-    const unsigned n = min(st.count, (unsigned)kPairStageCap);
-    if (threadIdx.x == 0) st.base = (n > 0) ? atomicAdd(o.n, n) : 0u;
-    __syncthreads();
-    const unsigned base = st.base;
-    for (unsigned i = threadIdx.x; i < n; i += blockDim.x) {
-        if (base + i < o.cap) o.pairs[base + i] = st.buf[i];
-        else atomicExch(o.overflow, 1);
-    }
-}
+constexpr int kPairQueriesPerWarp = 8; // queries handled by one warp of a warp-per-query kernel (warp_scan_candidates)
 
 } // namespace ipcgpu

@@ -179,51 +179,15 @@ DEV double box_gap2(const Box& a, const Box& b)
 DEV bool is_dbc_v(const SurfArgs& s, int v) { return s.dbc && s.dbc[v] != 0; }
 DEV int codim_v(const SurfArgs& s, int v) { return s.vCoDim ? s.vCoDim[v] : 3; }
 
-// ---- phase 1: broad phase proper.  One WARP per query primitive scans the grid and appends (query, partner) pairs whose boxes are
-// closer than sqrt(dHat).  Only boxes are touched here, so the kernel needs few registers and runs at high occupancy.
-
-__global__ void __launch_bounds__(256) k_pairs_pt(SurfArgs s, const Grid* __restrict__ gp, SortedGrid tg, double dHat, double radius, int first, int last, PairOut out)
-{
-    __shared__ PairStage stage;
-    pair_stage_init(stage);
-    const int lane = threadIdx.x & 31;
-    const Grid g = *gp;
-    const int q0 = first + (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * kPairQueriesPerWarp;
-    for (int svI = q0; svI < min(q0 + kPairQueriesPerWarp, last); ++svI) {
-        const V3 p = load_vertex(s.V, s.nV, s.SVI[svI]);
-        Box qb;
-        qb.lo[0] = p.x - radius; qb.lo[1] = p.y - radius; qb.lo[2] = p.z - radius;
-        qb.hi[0] = p.x + radius; qb.hi[1] = p.y + radius; qb.hi[2] = p.z + radius;
-        warp_scan_candidates(g, tg, qb, lane, [&](bool hit, int sfI) { warp_push_pair(stage, out, hit, svI, sfI, lane); });
-    }
-    pair_stage_flush(stage, out);
-}
-
-// queries are the entries of the sorted edge grid itself ([first, last) = sorted positions); each walks only the entries behind it
-__global__ void __launch_bounds__(256) k_pairs_ee(const Grid* __restrict__ gp, SortedGrid eg, const Box* __restrict__ eboxes, double dHat, double radius, int first, int last, PairOut out)
-{
-    __shared__ PairStage stage;
-    pair_stage_init(stage);
-    const int lane = threadIdx.x & 31;
-    const Grid g = *gp;
-    const int q0 = first + (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * kPairQueriesPerWarp;
-    for (int i = q0; i < min(q0 + kPairQueriesPerWarp, last); ++i) {
-        const int eI = eg.ids[i];
-        Box qb = eboxes[eI];
-        for (int k = 0; k < 3; ++k) { qb.lo[k] -= radius; qb.hi[k] += radius; }
-        warp_scan_candidates(g, eg, qb, lane, [&](bool hit, int eJ) { warp_push_pair(stage, out, hit, min(eI, eJ), max(eI, eJ), lane); }, i);
-    }
-    pair_stage_flush(stage, out);
-}
-
-// ---- cell-centric edge-edge pair finding (round 2, second half) ------------------------------------------------------------------
-// The warp-per-query kernels above spend ~2 warp instructions per box test (flattened-index arithmetic, entry load, ballot/append per
-// 32 tests plus ~150 instructions of set-up per query) and are ISSUE-bound (542 K edge queries x ~450 instructions; on C5 with H100 SXM
-// at 400 W the constraint set takes 0.69 ms with them against 0.35 ms with the kernels below).  Here a
+// ---- phase 1: broad phase proper, cell-centric pair finding (round 2, second half) ------------------------------------------------
+// Only boxes are touched here: the pairs whose boxes are closer than sqrt(dHat) go to a list that phase 2 classifies.  A warp per
+// query (warp_scan_candidates, the round-1 form) spends ~2 warp instructions per box test (flattened-index arithmetic, entry load,
+// ballot/append per 32 tests plus ~150 instructions of set-up per query) and is ISSUE-bound (542 K edge queries x ~450 instructions;
+// on C5 with H100 SXM at 400 W the constraint set took 0.69 ms with it against 0.35 ms with the kernels below).  Here a
 // warp takes 32 CONSECUTIVE entries of the sorted edge grid as queries ("A"); consecutive entries share their cell, so the partner
 // entries ("B") of a whole run of queries are fetched once: a lane holds one B entry and tests it against every query of the run, whose
 // inflated quantised boxes sit in shared memory (one broadcast LDS.128 + LDS.64 and ~8 integer instructions per test, 16-bit SIMD min for
-// two axes at a time).  Hits are rare and appended lane by lane.  One-sided like the query kernels: a pair is reported from the entry with
+// two axes at a time).  Hits are rare and appended lane by lane.  One-sided: a pair is reported from the entry with
 // the smaller sorted position, so only cells at or behind the run's own cell are visited.
 //   Which cells: a query registered in cell c (lower corner of its box) and inflated by `radius` covers cells c0'..c1' with
 //   c - 1 <= c0' <= c and c1' <= c0' + 1; its partners are registered in [c0' - 1, c1'] (broadphase.cuh).  The run uses the union over
@@ -757,12 +721,6 @@ using namespace ipcgpu;
     } while (0)
 
 static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
-// IPCGPU_PAIRS_MODE: 1 (default) = cell-centric edge-edge pair finding, 0 = the warp-per-query kernel of round 1
-static int pairs_mode()
-{
-    static const int mode = [] { const char* e = std::getenv("IPCGPU_PAIRS_MODE"); return e ? std::atoi(e) : 1; }();
-    return mode;
-}
 static void cell_pairs_pt(const Grid* gp, const SortedGrid& vg, const SortedGrid& tg, const SurfArgs& s, double radius, int first, int last, const PairOut& out, cudaStream_t st)
 {
     if (last > first) k_cell_pairs_pt<<<nblk(last - first, 32 * kCellPairWarps), 32 * kCellPairWarps, 0, st>>>(gp, vg, tg, s.SVI, s.SF, s.nSF, radius, first, last, out);
@@ -932,7 +890,7 @@ int boxes_and_grid(ipcgpu_ctx* ctx, double radius, bool with_vertex_boxes)
     if (s.nSF > 0) k_boxes<<<nblk(s.nSF, 256), 256, 0, st>>>(s, 2, w.tbox.p, w.bounds.p);
     k_grid_params<<<1, 32, 0, st>>>(w.bounds.p, radius, w.axis_bits, w.grid.p, ctx->iter.p);
     ctx->launches += 5;
-    return build_grids(ctx, s.nSF, s.nSE, (with_vertex_boxes && pairs_mode() != 0) ? s.nSV : 0);
+    return build_grids(ctx, s.nSF, s.nSE, with_vertex_boxes ? s.nSV : 0);
 }
 
 // pack this rank's lists, allgather, rebuild the global lists (called by api.cu around its ncclAllGather)
@@ -978,7 +936,7 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
     const double radius = sqrt(dHat);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_HASH);
     int rc;
-    if ((rc = boxes_and_grid(ctx, radius, pairs_mode() != 0))) return rc; // (vertex entries for the cell-centric PT kernel)
+    if ((rc = boxes_and_grid(ctx, radius, true))) return rc; // (vertex entries for the cell-centric PT kernel)
     ctx->prof_end(pe);
 
     pe = ctx->prof_begin(IPCGPU_STAGE_CONSTRAINT_SET);
@@ -1002,14 +960,12 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
     unsigned* nPairs = reinterpret_cast<unsigned*>(w.counters.p + 8); // [8] PT pairs, [9] EE pairs
     PairOut ppt{ w.bp_pairs.p, nPairs, (unsigned)w.bp_cap, w.counters.p + 4 }, pee{ w.bp_pairs.p + w.bp_cap, nPairs + 1, (unsigned)w.bp_cap, w.counters.p + 4 };
     if (v1 > v0 && s.nSF > 0) {
-        if (pairs_mode() == 0 || w.built_vertices != s.nSV) k_pairs_pt<<<nblk(v1 - v0, 8 * kPairQueriesPerWarp), 256, 0, st>>>(s, w.grid.p, tg, dHat, radius, v0, v1, ppt);
-        else cell_pairs_pt(w.grid.p, vertex_grid(ctx), tg, s, radius, s.nSF + s.nSE + v0, s.nSF + s.nSE + v1, ppt, st); // vertex entries: by sorted position
+        cell_pairs_pt(w.grid.p, vertex_grid(ctx), tg, s, radius, s.nSF + s.nSE + v0, s.nSF + s.nSE + v1, ppt, st); // vertex entries: by sorted position
         k_classify_pt<<<kSMs * 8, 128, 0, st>>>(s, ppt.pairs, ppt.n, ppt.cap, dHat, wantCand, out);
         ctx->launches += 2;
     }
     if (e1 > e0 && s.nSE > 1) {
-        if (pairs_mode() == 0) k_pairs_ee<<<nblk(e1 - e0, 8 * kPairQueriesPerWarp), 256, 0, st>>>(w.grid.p, eg, w.ebox.p, dHat, radius, s.nSF + e0, s.nSF + e1, pee); // edge entries sit behind the triangles
-        else cell_pairs_ee(w.grid.p, eg, s, radius, s.nSF + e0, s.nSF + e1, pee, st);
+        cell_pairs_ee(w.grid.p, eg, s, radius, s.nSF + e0, s.nSF + e1, pee, st); // edge entries sit behind the triangles
         k_classify_ee<<<kSMs * 8, 128, 0, st>>>(s, pee.pairs, pee.n, pee.cap, dHat, wantCand, out);
         ctx->launches += 2;
     }

@@ -86,7 +86,6 @@ struct CcdWork {
     DevBuf<int> vmin, vmax, counters;
     DevBuf<int2> cand;
     DevBuf<unsigned> surv, surv2;
-    bool wide_level_set = false;
     DevBuf<unsigned char> scratch;
     DevBuf<unsigned long long> ncand, bounds;
     // swept grid on the reference voxel lattice (ccd.cu): geometry, per-entry cell keys and entries (sorted by key), dense per-(type, cell)
@@ -145,7 +144,7 @@ struct ipcgpu_ctx {
     bool inputs_marked = false;
     void mark_inputs()
     {
-        if (ev_inputs) inputs_marked = (cudaEventRecord(ev_inputs, stream) == cudaSuccess);
+        inputs_marked = (cudaEventRecord(ev_inputs, stream) == cudaSuccess);
     }
     std::string err;
     uint64_t launches = 0;
@@ -208,10 +207,8 @@ struct ipcgpu_ctx {
     // Hessian slots (mesh-topology vertex pairs v<=u touched by local tets) and contributions
     int nSlots = 0;
     ipcgpu::DevBuf<int> slot_v, slot_u, slot_off, con_ptr;
-    ipcgpu::DevBuf<unsigned> con_src, hdst, cbase; // hdst / cbase: slot-major intermediate (destination of each tet block / start of each slot's run)
-    ipcgpu::DevBuf<double> hcon;                   // the slot-major intermediate itself: contributions of a CSR block slot contiguous
-    int hess_layout = 0;                           // 0 tile-major hblk + index-list assembly (default: faster), 1 slot-major hcon + streaming assembly
-    bool hblk_valid = false;
+    ipcgpu::DevBuf<unsigned> con_src;
+    bool hblk_valid = false; // the last gradient/Hessian call left the per-tet Hessian blocks in hblk
     bool maps_ready = false, offsets_ready = false;
 
     // CSR

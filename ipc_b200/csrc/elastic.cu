@@ -20,7 +20,6 @@
 //    store (cp.async.bulk.global.shared::cta), so HBM sees only full-line writes.
 #include "elastic.cuh"
 #include "kernels.h"
-#include <cstdlib>
 
 namespace ipcgpu {
 
@@ -132,24 +131,19 @@ DEV void tma_store_tile(void* gdst, const void* ssrc, unsigned bytes)
 // shared-memory occupancy limit of the first version of this kernel.
 // block slots of a tet in emission order: (a, b) local vertex pair, offset of the slot inside a tile (in units of 64 doubles), length
 
-// TILES 64-tet tiles per CTA: the warps of a CTA walk the (6.6 k instruction) body in step -- every slot ends in a CTA barrier -- so a larger CTA
-// means fewer distinct instruction streams per SM competing for the instruction caches (ncu, round 1: "no instruction" 1.9 stalls per issue
-// with eight independent 64-thread CTAs per SM).  The tile layout of the output does not change: half-CTA h works on tile blockIdx.x * TILES + h.
-template <int ENERGY, bool NEED_G, bool NEED_H, int TILES, int MINB = 8>
-__global__ void __launch_bounds__(kHessTile * TILES, MINB / TILES) k_elastic_grad_hess(ElasticArgs p, double coef, int projectSPD,
-    double* __restrict__ gcont /* 12 per LOCAL tet */, double* __restrict__ hblk /* tile-major, 78 per LOCAL tet */, double* __restrict__ e_partials /* nullable */,
-    const unsigned* __restrict__ hdst /* nullable: slot-major destinations, 10 per LOCAL tet */, double* __restrict__ hcon)
+// One 64-tet tile per CTA, compiled for 8 CTAs per SM (128 registers).  DESIGN.md ("Defaults re-checked on H100") keeps the timings
+// of 2- and 4-tile CTAs and of 6, 10 and 12 CTAs per SM: none was faster.
+template <int ENERGY, bool NEED_G, bool NEED_H>
+__global__ void __launch_bounds__(kHessTile, 8) k_elastic_grad_hess(ElasticArgs p, double coef, int projectSPD,
+    double* __restrict__ gcont /* 12 per LOCAL tet */, double* __restrict__ hblk /* tile-major, 78 per LOCAL tet */, double* __restrict__ e_partials /* nullable */)
 {
-    __shared__ unsigned sDst[TILES][kHessTile]; // slot-major output: destination of this slot's block of every tet of the tile
     double e_tet = 0.0; // fused energy: psi * vol of this thread's tet (computeEnergyVal at the same state shares the SVD, like the reference's cache)
-    extern __shared__ __align__(128) double smem_all[];
-    const int sub = threadIdx.x / kHessTile, tx = threadIdx.x % kHessTile; // tile of this CTA, thread inside the tile
-    constexpr int kSmemPerTile = kHessTile * ((NEED_H ? 18 : 0) + (NEED_G ? 12 : 0));
-    double* smem = smem_all + sub * kSmemPerTile;
+    extern __shared__ __align__(128) double smem[];
+    const int tx = threadIdx.x;
     double* sHb[2] = { smem, smem + kHessTile * 9 };          // two slot buffers (ping-pong)
     double* sG = smem + (NEED_H ? 2 * kHessTile * 9 : 0);     // kHessTile * 12
     const int nLocal = p.n_list;
-    const int tileI = blockIdx.x * TILES + sub;
+    const int tileI = blockIdx.x;
     const int tile0 = tileI * kHessTile;
     const int t = tile0 + tx;
     const bool active = t < nLocal;
@@ -282,22 +276,6 @@ __global__ void __launch_bounds__(kHessTile * TILES, MINB / TILES) k_elastic_gra
                             }
                     }
                 }
-                if (hdst) {
-                    // SLOT-MAJOR output (round 2, second half): every block goes to the place where the contributions of its CSR block slot
-                    // are contiguous, so the assembly streams them instead of gathering 72-byte pieces through an index list.  The tile's
-                    // blocks of this slot sit in shared memory; 64 threads write them out element by element (a warp store covers 3.5
-                    // blocks = 3.5 contiguous runs).
-                    const int kSlotIdx = (a == b) ? a : (a == 0 ? 3 + b : (a == 1 ? 5 + b : 9)); // (folded after unrolling; the order of build_maps)
-                    sDst[sub][tx] = active ? __ldg(hdst + (size_t)t * 10 + kSlotIdx) : 0xffffffffu;
-                    __syncthreads();
-                    for (int e = tx; e < kHessTile * len; e += kHessTile) {
-                        const int tt = e / len, q = e - tt * len;
-                        const unsigned d = sDst[sub][tt];
-                        if (d != 0xffffffffu) hcon[(size_t)d + q] = buf[e];
-                    }
-                    __syncthreads();
-                }
-                else {
                 // ship this slot: generic-proxy writes -> async-proxy fence -> CTA barrier -> one elected TMA store
                 asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
                 __syncthreads();
@@ -306,7 +284,6 @@ __global__ void __launch_bounds__(kHessTile * TILES, MINB / TILES) k_elastic_gra
                     asm volatile("cp.async.bulk.wait_group.read 1;\n" ::: "memory"); // the other buffer's store has been read out
                 }
                 __syncthreads();
-                }
                 ++slot;
             }
         }
@@ -318,14 +295,14 @@ __global__ void __launch_bounds__(kHessTile * TILES, MINB / TILES) k_elastic_gra
         asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory");
     }
     if (e_partials) { // fixed-order CTA sum: warp sums, then warp 0 adds them in warp order
-        __shared__ double sE[2 * TILES];
+        __shared__ double sE[2];
         const double ws = warp_sum(e_tet);
         if ((threadIdx.x & 31) == 0) sE[threadIdx.x >> 5] = ws;
         __syncthreads();
         if (threadIdx.x == 0) {
             double acc = 0.0;
 #pragma unroll
-            for (int i = 0; i < 2 * TILES; ++i) acc += sE[i];
+            for (int i = 0; i < 2; ++i) acc += sE[i];
             e_partials[blockIdx.x] = acc;
         }
     }
@@ -366,7 +343,6 @@ __global__ void __launch_bounds__(256) k_gather_gradient(int nV, const int* __re
 // one thread per block-slot (vertex pair v<=u of the mesh topology); contributions are summed in
 // ascending tet order (the reference's vFLoc order), then written to the three CSR rows.
 // ---------------------------------------------------------------------------------------------
-template <int UNROLL>
 __global__ void __launch_bounds__(288) k_assemble_csr(int nSlots, const int* __restrict__ slot_v, const int* __restrict__ slot_u,
     const int* __restrict__ slot_off /* 3 per slot */, const int* __restrict__ con_ptr, const unsigned* __restrict__ con_src,
     const double* __restrict__ hblk, const uint8_t* __restrict__ dbc, int projectDBC, const double* __restrict__ mass,
@@ -387,7 +363,7 @@ __global__ void __launch_bounds__(288) k_assemble_csr(int nSlots, const int* __r
     if (!dropped) {
         const int b = con_ptr[sIdx], e = con_ptr[sIdx + 1];
         // (round 1: an explicit 8-deep load batch was slower -- but slot lists were then mixed 5- and 23-long inside a warp)
-#pragma unroll UNROLL
+#pragma unroll 4
         for (int k = b; k < e; ++k) h += hblk[__ldg(con_src + k) + q];
     }
     int r, c;
@@ -400,41 +376,6 @@ __global__ void __launch_bounds__(288) k_assemble_csr(int nSlots, const int* __r
     }
     else a[o] = h;
     (void)mass;
-}
-
-// The same over the SLOT-MAJOR intermediate: the contributions of slot s are the `cnt` consecutive blocks at cbase[s] (6 doubles each for a
-// diagonal slot, 9 otherwise), in ascending tet order -- a streaming read (every line is used completely by the 3.5 slots of a warp), no
-// index list, the loads of consecutive contributions independent of each other.
-template <int UNROLL>
-__global__ void __launch_bounds__(288) k_assemble_slot_major(int nSlots, const int* __restrict__ slot_v, const int* __restrict__ slot_u, const int* __restrict__ slot_off /* 3 per slot */,
-    const unsigned* __restrict__ cbase, const double* __restrict__ hcon, const uint8_t* __restrict__ dbc, int projectDBC, int accumulate, double* __restrict__ a)
-{
-    const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int sIdx = (int)(tid / 9), q = (int)(tid - 9ll * sIdx);
-    if (sIdx >= nSlots) return;
-    const int v = slot_v[sIdx], u = slot_u[sIdx];
-    const bool diag = (v == u);
-    if (diag && q >= 6) return;
-    const bool pv = dbc && (dbc[v] == 1 || (dbc[v] == 2 && projectDBC));
-    const bool pu = dbc && (dbc[u] == 1 || (dbc[u] == 2 && projectDBC));
-    const bool dropped = pv || pu;
-    double h = 0.0;
-    if (!dropped) {
-        const int len = diag ? 6 : 9;
-        const double* src = hcon + cbase[sIdx] + q;
-        const double* end = hcon + cbase[sIdx + 1];
-#pragma unroll UNROLL
-        for (; src < end; src += len) h += *src;
-    }
-    int r, c;
-    if (diag) { r = (q < 3) ? 0 : (q < 5 ? 1 : 2); c = (q < 3) ? q : (q < 5 ? q - 3 : 0); }
-    else { r = q / 3; c = q - 3 * r; }
-    const int o = slot_off[3 * sIdx + r] + c;
-    if (accumulate) {
-        if (!dropped) a[o] += h;
-        else if (diag) a[o] = 0.0;
-    }
-    else a[o] = h;
 }
 
 // per-vertex diagonal terms of computePrecondMtr (Optimizer.cpp:3638-3668): mass on free vertices, identity on projected
@@ -639,63 +580,31 @@ void elastic_energy(const ElasticArgs& p, double* e_per_tet, double* partials, c
 int elastic_energy_blocks(int nTets) { return (nTets + 255) / 256; }
 void reduce_sum(const double* partials, int n, double scale, double* out, cudaStream_t st) { k_reduce_sum<<<1, 1024, 0, st>>>(partials, n, scale, out); }
 
-static int tet_tiles()
-{
-    static const int tiles = [] { const char* e = std::getenv("IPCGPU_TET_TILES"); const int v = e ? std::atoi(e) : 1; return (v == 1 || v == 2 || v == 4) ? v : 1; }();
-    return tiles; // 64-tet tiles per CTA of the gradient/Hessian kernel (H100 SXM, 400 W, C5: 1 / 2 / 4 -> kernel 0.46 / 0.46 / 0.44 ms, iteration 3.71 / 3.78 / 3.72 ms)
-}
-int elastic_grad_hess_blocks(int n_list)
-{
-    const int nb = (n_list + kHessTile - 1) / kHessTile, t = tet_tiles();
-    return (nb + t - 1) / t;
-}
+int elastic_grad_hess_blocks(int n_list) { return (n_list + kHessTile - 1) / kHessTile; }
 template <int ENERGY, bool G, bool H>
-static void launch_gh(const ElasticArgs& p, double coef, int projectSPD, double* gcont, double* hblk, cudaStream_t st, double* e_partials, const unsigned* hdst, double* hcon)
+static void launch_gh(const ElasticArgs& p, double coef, int projectSPD, double* gcont, double* hblk, cudaStream_t st, double* e_partials)
 {
     const int n = p.n_list;
     if (n <= 0) return;
-    const int nb = (n + kHessTile - 1) / kHessTile;
     const size_t smem = (size_t)kHessTile * 8 * ((H ? 18 : 0) + (G ? 12 : 0));
-    const int tiles = tet_tiles();
     static bool attr_set = false;
     if (!attr_set) {
-        cudaFuncSetAttribute(k_elastic_grad_hess<ENERGY, G, H, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        cudaFuncSetAttribute(k_elastic_grad_hess<ENERGY, G, H, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * smem));
-        cudaFuncSetAttribute(k_elastic_grad_hess<ENERGY, G, H, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * smem));
+        cudaFuncSetAttribute(k_elastic_grad_hess<ENERGY, G, H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_set = true;
     }
-    static const int minb = [] { const char* e = std::getenv("IPCGPU_TET_MINB"); return e ? std::atoi(e) : 8; }(); // CTAs/SM the kernel is compiled for: 8 = 128 registers
-    // (H100 SXM, 400 W, C5: 6 / 8 / 10 / 12 -> kernel 0.47 / 0.46 / 0.58 / 0.79 ms)
-    if (tiles == 1 && minb == 10) {
-        static bool a10 = false;
-        if (!a10) { cudaFuncSetAttribute(k_elastic_grad_hess<ENERGY, G, H, 1, 10>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); a10 = true; }
-        k_elastic_grad_hess<ENERGY, G, H, 1, 10><<<nb, kHessTile, smem, st>>>(p, coef, projectSPD, gcont, hblk, e_partials, hdst, hcon);
-    }
-    else if (tiles == 1 && minb == 12) {
-        static bool a12 = false;
-        if (!a12) { cudaFuncSetAttribute(k_elastic_grad_hess<ENERGY, G, H, 1, 12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); a12 = true; }
-        k_elastic_grad_hess<ENERGY, G, H, 1, 12><<<nb, kHessTile, smem, st>>>(p, coef, projectSPD, gcont, hblk, e_partials, hdst, hcon);
-    }
-    else if (tiles == 1 && minb == 6) {
-        static bool a6 = false;
-        if (!a6) { cudaFuncSetAttribute(k_elastic_grad_hess<ENERGY, G, H, 1, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); a6 = true; }
-        k_elastic_grad_hess<ENERGY, G, H, 1, 6><<<nb, kHessTile, smem, st>>>(p, coef, projectSPD, gcont, hblk, e_partials, hdst, hcon);
-    }
-    else if (tiles == 1) k_elastic_grad_hess<ENERGY, G, H, 1><<<nb, kHessTile, smem, st>>>(p, coef, projectSPD, gcont, hblk, e_partials, hdst, hcon);
-    else if (tiles == 2) k_elastic_grad_hess<ENERGY, G, H, 2><<<(nb + 1) / 2, 2 * kHessTile, 2 * smem, st>>>(p, coef, projectSPD, gcont, hblk, e_partials, hdst, hcon);
-    else k_elastic_grad_hess<ENERGY, G, H, 4><<<(nb + 3) / 4, 4 * kHessTile, 4 * smem, st>>>(p, coef, projectSPD, gcont, hblk, e_partials, hdst, hcon);
+    k_elastic_grad_hess<ENERGY, G, H><<<elastic_grad_hess_blocks(n), kHessTile, smem, st>>>(p, coef, projectSPD, gcont, hblk, e_partials);
 }
-void elastic_grad_hess(const ElasticArgs& p, double coef, int projectSPD, bool need_g, bool need_h, double* gcont, double* hblk, cudaStream_t st, double* e_partials, const unsigned* hdst, double* hcon)
+void elastic_grad_hess(const ElasticArgs& p, double coef, int projectSPD, bool need_g, bool need_h, double* gcont, double* hblk, cudaStream_t st, double* e_partials)
 {
     if (p.energy == 0) {
-        if (need_g && need_h) launch_gh<0, true, true>(p, coef, projectSPD, gcont, hblk, st, e_partials, hdst, hcon);
-        else if (need_g) launch_gh<0, true, false>(p, coef, projectSPD, gcont, hblk, st, e_partials, hdst, hcon);
-        else if (need_h) launch_gh<0, false, true>(p, coef, projectSPD, gcont, hblk, st, e_partials, hdst, hcon);
+        if (need_g && need_h) launch_gh<0, true, true>(p, coef, projectSPD, gcont, hblk, st, e_partials);
+        else if (need_g) launch_gh<0, true, false>(p, coef, projectSPD, gcont, hblk, st, e_partials);
+        else if (need_h) launch_gh<0, false, true>(p, coef, projectSPD, gcont, hblk, st, e_partials);
     }
     else {
-        if (need_g && need_h) launch_gh<1, true, true>(p, coef, projectSPD, gcont, hblk, st, e_partials, hdst, hcon);
-        else if (need_g) launch_gh<1, true, false>(p, coef, projectSPD, gcont, hblk, st, e_partials, hdst, hcon);
-        else if (need_h) launch_gh<1, false, true>(p, coef, projectSPD, gcont, hblk, st, e_partials, hdst, hcon);
+        if (need_g && need_h) launch_gh<1, true, true>(p, coef, projectSPD, gcont, hblk, st, e_partials);
+        else if (need_g) launch_gh<1, true, false>(p, coef, projectSPD, gcont, hblk, st, e_partials);
+        else if (need_h) launch_gh<1, false, true>(p, coef, projectSPD, gcont, hblk, st, e_partials);
     }
 }
 
@@ -708,17 +617,8 @@ void assemble_csr(int nSlots, const int* slot_v, const int* slot_u, const int* s
     const double* hblk, const uint8_t* dbc, int projectDBC, const double* mass, int accumulate, double* a, cudaStream_t st)
 {
     if (nSlots <= 0) return;
-    static const int unroll = [] { const char* e = std::getenv("IPCGPU_ASM_UNROLL"); return e ? std::atoi(e) : 4; }();
     const int nb = (int)(((long long)nSlots * 9 + 287) / 288);
-    if (unroll >= 4) k_assemble_csr<4><<<nb, 288, 0, st>>>(nSlots, slot_v, slot_u, slot_off, con_ptr, con_src, hblk, dbc, projectDBC, mass, accumulate, a);
-    else k_assemble_csr<1><<<nb, 288, 0, st>>>(nSlots, slot_v, slot_u, slot_off, con_ptr, con_src, hblk, dbc, projectDBC, mass, accumulate, a);
-}
-void assemble_slot_major(int nSlots, const int* slot_v, const int* slot_u, const int* slot_off, const unsigned* cbase, const double* hcon, const uint8_t* dbc, int projectDBC,
-    int accumulate, double* a, cudaStream_t st)
-{
-    if (nSlots <= 0) return;
-    const int nb = (int)(((long long)nSlots * 9 + 287) / 288);
-    k_assemble_slot_major<4><<<nb, 288, 0, st>>>(nSlots, slot_v, slot_u, slot_off, cbase, hcon, dbc, projectDBC, accumulate, a);
+    k_assemble_csr<<<nb, 288, 0, st>>>(nSlots, slot_v, slot_u, slot_off, con_ptr, con_src, hblk, dbc, projectDBC, mass, accumulate, a);
 }
 void diag_mass_dbc(int nV, const int* ia, int base, const uint8_t* dbc, int projectDBC, const double* mass, double* a, cudaStream_t st)
 {

@@ -80,11 +80,7 @@ struct ElasticArgs {
 void elastic_energy(const ElasticArgs& p, double* e_per_tet, double* partials, cudaStream_t st); // elastic_energy_blocks partial sums of psi * vol
 int elastic_energy_blocks(int nTets);
 // e_partials != nullptr: the kernel also leaves one partial sum of psi * vol per CTA there (elastic_grad_hess_blocks of them)
-// hdst != nullptr: the Hessian blocks go to the SLOT-MAJOR intermediate hcon (destination offsets hdst, 10 per local tet) instead of the tile-major hblk
-void elastic_grad_hess(const ElasticArgs& p, double coef, int projectSPD, bool need_g, bool need_h, double* gcont, double* hblk, cudaStream_t st, double* e_partials = nullptr,
-    const unsigned* hdst = nullptr, double* hcon = nullptr);
-void assemble_slot_major(int nSlots, const int* slot_v, const int* slot_u, const int* slot_off, const unsigned* cbase, const double* hcon, const uint8_t* dbc, int projectDBC,
-    int accumulate, double* a, cudaStream_t st);
+void elastic_grad_hess(const ElasticArgs& p, double coef, int projectSPD, bool need_g, bool need_h, double* gcont, double* hblk, cudaStream_t st, double* e_partials = nullptr);
 int elastic_grad_hess_blocks(int n_list);
 void gather_gradient(int nV, const int* inc_ptr, const int* inc, const double* gcont, const uint8_t* dbc, int projectDBC, int accumulate, double* g, cudaStream_t st);
 void assemble_csr(int nSlots, const int* slot_v, const int* slot_u, const int* slot_off, const int* con_ptr, const unsigned* con_src,

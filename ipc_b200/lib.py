@@ -62,7 +62,6 @@ SIGNATURES = {
     "ipcgpu_set_surface": (C.c_int, [_ctxp, C.c_int, _ip, C.c_int, _ip, C.c_int, _ip, _ip]),
     "ipcgpu_set_pair_capacity": (C.c_int, [_ctxp, C.c_int]),
     "ipcgpu_set_exchange_capacity": (C.c_int, [_ctxp, C.c_int]),
-    "ipcgpu_set_hessian_layout": (C.c_int, [_ctxp, C.c_int]),
     "ipcgpu_constraint_set": (C.c_int, [_ctxp, C.c_double, C.c_int, _ip, _ip, _ip]),
     "ipcgpu_set_contact_partition": (C.c_int, [_ctxp, C.c_int]),
     "ipcgpu_set_canonical_order": (C.c_int, [_ctxp, C.c_int]),
@@ -540,10 +539,6 @@ class Context:
 
     def set_contact_partition(self, enable):
         self._ck(self.lib.ipcgpu_set_contact_partition(self.h, int(enable)))
-
-    def set_hessian_layout(self, layout):
-        """0 tile-major (default; per-tet blocks downloadable), 1 slot-major"""
-        self._ck(self.lib.ipcgpu_set_hessian_layout(self.h, int(layout)))
 
     def set_exchange_capacity(self, pairs_per_rank):
         self._ck(self.lib.ipcgpu_set_exchange_capacity(self.h, int(pairs_per_rank)))
