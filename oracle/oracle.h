@@ -30,6 +30,10 @@ extern "C" {
 /* ---- elastic (oracle/elastic.cpp) ---------------------------------------- */
 /* AutoFlipSVD / JIXIE implicit-QR 3x3 SVD (ImplicitQRSVD.h:687-850). Row-major. */
 int orc_svd3(const double F[9], double U[9], double S[3], double V[9]);
+/* Which way the same SVD left: *exit_id = 0..4 for the beta_2, beta_1, alpha_2, alpha_3, alpha_1 exits (in the order they are tested);
+ * *sort_id = 0 / 1 for the sort after process(0) / process(1); *reordered = 1 when that sort took its swapping branch rather than the
+ * early return. Returns the QR sweep count. */
+int orc_svd3_branch(const double F[9], int* exit_id, int* sort_id, int* reordered);
 
 /* energy_type: 0 = NeoHookean, 1 = FixedCoRot */
 void orc_psi(int energy_type, const double S[3], double mu, double lam, double* E);

@@ -102,6 +102,18 @@ def svd3(F):
     return U.reshape(3, 3), S, V.reshape(3, 3)
 
 
+SVD3_EXITS = ("beta_2", "beta_1", "alpha_2", "alpha_3", "alpha_1")
+
+
+def svd3_branch(F):
+    """(exit, sort, reordered) of the restated SVD on F: the exit's name (SVD3_EXITS, in the order the exits are tested), which sort ran
+    (0 after process(0), 1 after process(1)) and whether that sort took its swapping branch instead of the early return"""
+    F = np.ascontiguousarray(F, dtype=np.float64).ravel()
+    ex, so, re = C.c_int(), C.c_int(), C.c_int()
+    lib().orc_svd3_branch(d(F), C.byref(ex), C.byref(so), C.byref(re))
+    return SVD3_EXITS[ex.value], so.value, bool(re.value)
+
+
 def psi(et, S, mu, lam):
     S = np.ascontiguousarray(S, dtype=np.float64)
     E = C.c_double()
