@@ -111,7 +111,8 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 //   - ipcgpu_step_bound_set, ipcgpu_inversion_step, ipcgpu_halfspace_step, ipcgpu_ccd_partial_ti, ipcgpu_hash_build_swept, ipcgpu_ccd_full_ti
 //     with every host argument NULL (a host search direction rewrites `dir`, a host step reads back);
 //   - the derivative calls in their NULL-output form (they enqueue on `deriv`), among them ipcgpu_halfspace_gradient / _hessian and
-//     ipcgpu_halfspace_friction_gradient / _hessian;
+//     ipcgpu_halfspace_friction_gradient / _hessian, ipcgpu_damping_gradient / _hessian, ipcgpu_neumann_gradient and
+//     ipcgpu_dirichlet_gradient / _hessian;
 //   - ipcgpu_allreduce_grad_hess on one rank (a no-op), and ipcgpu_download_range_async, whose copy waits on `deriv` as well.
 // Every other entry point that touches the device calls enter(ctx, kSerial) first, which joins `deriv` into the main stream (the pure
 // host-side getters need not).  Among them ipcgpu_update_pattern: it rewrites ia, ja and slot_off, which the derivative chain reads, so it
@@ -134,6 +135,12 @@ static int join_copy_stream(ipcgpu_ctx* ctx)
 //     hs_pstart and IterState::energy[kEnergyPlaneBarrier / kEnergyPlaneFriction], hs_n_*, hs_crossings); the plane derivative calls read hs_par, hs_act, hs_lag, hs_lam, hs_cnt,
 //     Vprev (written before the fork) and write g / a only; ipcgpu_halfspace_step reads hs_par, SVI, dir and writes IterState::step_ord,
 //     hs_alpha, hs_zero_step only (the derivative chain touches none of them).
+//   - damping, Neumann forces, Dirichlet penalty (damping.cu): the gradient / Hessian calls in their NULL form (ipcgpu_damping_gradient /
+//     _hessian, ipcgpu_neumann_gradient, ipcgpu_dirichlet_gradient / _hessian) run on the derivative chain; they read damp_D, damp_inc_ptr,
+//     damp_inc, slot_v, slot_u, slot_off, Vprev, nbc_f, mass, dbc_vid, dbc_tgt, dbc_lam and IterState::dbc_rho (all written before the fork,
+//     by kSerial calls: ipcgpu_damping_update, ipcgpu_set_neumann_forces, ipcgpu_set_dirichlet_targets / _penalty / _update_lambda) and
+//     write g / a only; their energies and ipcgpu_dirichlet_completed_step (IterState::energy[kEnergyDamping / kEnergyNeumann /
+//     kEnergyDirichlet], dbc_step, damp_partials, nbc_partials, dbc_partials) are kSerial.  The step-bound chain touches none of them.
 //   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, e_partials2, bHraw, brows, bpsd:
 //     derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };
@@ -315,6 +322,12 @@ static int build_maps(ipcgpu_ctx* ctx)
     CK(cudaStreamSynchronize(ctx->stream)); // host vectors go out of scope
     ctx->maps_ready = true;
     ctx->offsets_ready = false;
+    // D and its incidence follow the slots, the Neumann forces and Dirichlet targets the vertices: a new mesh or partition removes them
+    ctx->damp_on = ctx->damp_inc_ready = ctx->nbc_on = false;
+    ctx->n_dbc = 0;
+    for (int slot : { kEnergyDamping, kEnergyNeumann, kEnergyDirichlet }) // (the fetch reports 0 for a term that is not set)
+        CK(cudaMemsetAsync(&ctx->iter.p->energy[slot], 0, sizeof(double), ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     return IPCGPU_OK;
 }
 
@@ -506,13 +519,14 @@ static int download_values(ipcgpu_ctx* ctx, double* a_host)
 
 // A gradient / Hessian term.  NULL output: the term on `chain`; host output: the caller's array in, the term added on the main stream,
 // the rank-completed array out and, for a Hessian, the flags of `check` it may raise returned as its status.
+// `stage`: the stage timer the term is counted under.
 template <typename Launch>
-static int gradient_call(ipcgpu_ctx* ctx, Chain chain, double* g_inout, Launch launch)
+static int gradient_call(ipcgpu_ctx* ctx, Chain chain, double* g_inout, Launch launch, int stage = IPCGPU_STAGE_BARRIER)
 {
     ENTER(g_inout ? kSerial : chain);
     int rc;
     if (g_inout && (rc = gradient_roundtrip_begin(ctx, g_inout))) return rc;
-    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
+    cudaEvent_t pe = ctx->prof_begin(stage);
     launch(ctx->deriv_stream());
     ctx->prof_end(pe);
     ++ctx->launches;
@@ -533,11 +547,11 @@ static int hessian_end(ipcgpu_ctx* ctx, double* a_inout, unsigned check)
     return flag_status(ctx, check);
 }
 template <typename Launch>
-static int hessian_call(ipcgpu_ctx* ctx, Chain chain, double* a_inout, unsigned check, Launch launch)
+static int hessian_call(ipcgpu_ctx* ctx, Chain chain, double* a_inout, unsigned check, Launch launch, int stage = IPCGPU_STAGE_BARRIER)
 {
     int rc = hessian_begin(ctx, chain, a_inout);
     if (rc) return rc;
-    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
+    cudaEvent_t pe = ctx->prof_begin(stage);
     launch(ctx->deriv_stream());
     ctx->prof_end(pe);
     ++ctx->launches;
@@ -1671,6 +1685,285 @@ int ipcgpu_inertia_gradient(ipcgpu_ctx* ctx, int projectDBC, double* g_inout)
     return IPCGPU_OK;
 }
 
+// ---- Rayleigh damping, Neumann forces, augmented-Lagrangian Dirichlet penalty (damping.cu; which chain each call runs on: see enter()) ------
+#define REQUIRE_ONE_RANK() REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "damping, Neumann forces and the Dirichlet penalty run on one rank")
+
+// a term switched on or off: graphs that bake the line search's set of terms in are refused, and the term's energy slot reads 0 while it is off
+static int term_switched(ipcgpu_ctx* ctx, int slot)
+{
+    ++ctx->epoch;
+    CK(cudaMemsetAsync(&ctx->iter.p->energy[slot], 0, sizeof(double), ctx->stream));
+    return IPCGPU_OK;
+}
+
+static DampingArgs damping_args(ipcgpu_ctx* ctx)
+{
+    DampingArgs p;
+    p.nV = ctx->nV; p.nSlots = ctx->nSlots;
+    p.slot_v = ctx->slot_v.p; p.slot_u = ctx->slot_u.p;
+    p.inc_ptr = ctx->damp_inc_ptr.p; p.inc = ctx->damp_inc.p;
+    p.D = ctx->damp_D.p;
+    p.V = ctx->V.p; p.Vprev = ctx->Vprev.p;
+    p.dbc = ctx->has_dbc ? ctx->dbc.p : nullptr;
+    return p;
+}
+
+// the slot incidence of every vertex (once per mesh): the slots in which it is slot_v (entry 2s), then those in which it is the slot_u of an
+// off-diagonal slot (2s + 1), each group in slot order
+static int damping_incidence(ipcgpu_ctx* ctx)
+{
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "run ipcgpu_damping_update once outside a capture first (it builds the slot incidence)");
+    const int nS = ctx->nSlots, nV = ctx->nV;
+    std::vector<int> sv((size_t)std::max(nS, 1)), su((size_t)std::max(nS, 1));
+    CK(cudaMemcpyAsync(sv.data(), ctx->slot_v.p, (size_t)nS * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(su.data(), ctx->slot_u.p, (size_t)nS * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::vector<int> ptr((size_t)nV + 1, 0);
+    for (int s = 0; s < nS; ++s) {
+        ++ptr[(size_t)sv[s] + 1];
+        if (sv[s] != su[s]) ++ptr[(size_t)su[s] + 1];
+    }
+    for (int v = 0; v < nV; ++v) ptr[(size_t)v + 1] += ptr[v];
+    std::vector<int> inc((size_t)std::max(ptr[nV], 1)), cur(ptr.begin(), ptr.end() - 1);
+    for (int s = 0; s < nS; ++s) inc[(size_t)cur[sv[s]]++] = 2 * s;
+    for (int s = 0; s < nS; ++s)
+        if (sv[s] != su[s]) inc[(size_t)cur[su[s]]++] = 2 * s + 1;
+    REQUIRE(ctx->damp_inc_ptr.upload(ptr.data(), ptr.size(), ctx->stream) && ctx->damp_inc.upload(inc.data(), inc.size(), ctx->stream), IPCGPU_ERR_CUDA,
+        "upload of the damping incidence failed");
+    CK(cudaStreamSynchronize(ctx->stream)); // host vectors go out of scope
+    ctx->damp_inc_ready = true;
+    return IPCGPU_OK;
+}
+
+int ipcgpu_damping_update(ipcgpu_ctx* ctx, double coef)
+{
+    REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    REQUIRE_ONE_RANK();
+    ENTER(kSerial);
+    int rc;
+    if (coef == 0.0) { // no damping term
+        if (ctx->damp_on && (rc = term_switched(ctx, kEnergyDamping))) return rc;
+        ctx->damp_on = false;
+        return IPCGPU_OK;
+    }
+    if (!ctx->damp_inc_ready && (rc = damping_incidence(ctx))) return rc;
+    ALLOC(ctx->damp_D, (size_t)9 * std::max(ctx->nSlots, 1));
+    ALLOC(ctx->damp_partials, (size_t)damping_energy_blocks(ctx->nSlots) + 8);
+    // computeDampingMtr (Optimizer.cpp:3723-3734): the elastic Hessian at the current state, coef, projected (projectSPD = projectDBC = 1)
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_DAMPING_BC);
+    elastic_grad_hess(ctx->eargs(), coef, 1, false, true, ctx->gcont.p, ctx->hblk.p, ctx->stream);
+    ctx->hblk_valid = true; // (IPCGPU_BUF_TET_HESSIANS now holds the damping's per-tet blocks)
+    damping_assemble(ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->con_ptr.p, ctx->con_src.p, ctx->hblk.p, ctx->has_dbc ? ctx->dbc.p : nullptr,
+        ctx->damp_D.p, ctx->stream);
+    ctx->prof_end(pe);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    if (!ctx->damp_on && (rc = term_switched(ctx, kEnergyDamping))) return rc;
+    ctx->damp_on = true;
+    return IPCGPU_OK;
+}
+
+#define REQUIRE_DAMPING()                                                                                                \
+    REQUIRE(ctx->damp_on, IPCGPU_ERR_STATE, "ipcgpu_damping_update with a nonzero coefficient first");                  \
+    REQUIRE(ctx->prev_set, IPCGPU_ERR_STATE, "ipcgpu_set_prev_state first");                                              \
+    REQUIRE_ONE_RANK()
+
+int ipcgpu_damping_energy(ipcgpu_ctx* ctx, double* E)
+{
+    REQUIRE_DAMPING();
+    ENTER(kSerial);
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_DAMPING_BC);
+    damping_energy(damping_args(ctx), ctx->damp_partials.p, ctx->stream);
+    return energy_tail(ctx, kEnergyDamping, ctx->damp_partials.p, damping_energy_blocks(ctx->nSlots), 0.5, pe, E);
+}
+
+int ipcgpu_damping_gradient(ipcgpu_ctx* ctx, int projectDBC, double* g_inout)
+{
+    REQUIRE_DAMPING();
+    const DampingArgs p = damping_args(ctx);
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { damping_gradient(p, projectDBC, ctx->g.p, st); }, IPCGPU_STAGE_DAMPING_BC);
+}
+
+int ipcgpu_damping_hessian(ipcgpu_ctx* ctx, double* a_inout)
+{
+    REQUIRE_DAMPING();
+    REQUIRE(ctx->nnz > 0, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
+    if (!ctx->offsets_ready) { // (the slot offsets of a new host pattern: one synchronising check, as the first elastic Hessian does)
+        ENTER(kSerial);
+        int rc = ensure_offsets(ctx);
+        if (rc) return rc;
+    }
+    const DampingArgs p = damping_args(ctx);
+    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) { damping_hessian(p, ctx->slot_off.p, ctx->a.p, st); }, IPCGPU_STAGE_DAMPING_BC);
+}
+
+int ipcgpu_set_neumann_forces(ipcgpu_ctx* ctx, double coef, const double* f)
+{
+    REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    REQUIRE(!f || ctx->has_mass, IPCGPU_ERR_STATE, "Neumann forces need the mass diagonal (ipcgpu_set_mesh)");
+    REQUIRE_ONE_RANK();
+    ENTER(kSerial);
+    int rc;
+    if (f) {
+        ALLOC(ctx->nbc_f, (size_t)3 * ctx->nV);
+        ALLOC(ctx->nbc_partials, (size_t)vertex_energy_blocks(ctx->nV) + 8);
+        CK(cudaMemcpyAsync(ctx->nbc_f.p, f, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream)); // (f is the caller's: the upload completes here)
+    }
+    set_double(&ctx->iter.p->nbc_coef, coef, ctx->stream); // (read at run time, like the forces: a new dt needs no new capture)
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    if ((f != nullptr) != ctx->nbc_on && (rc = term_switched(ctx, kEnergyNeumann))) return rc;
+    ctx->nbc_on = f != nullptr;
+    return IPCGPU_OK;
+}
+
+#define REQUIRE_NEUMANN()                                                                                   \
+    REQUIRE(ctx->nbc_on, IPCGPU_ERR_STATE, "ipcgpu_set_neumann_forces first");                             \
+    REQUIRE_ONE_RANK()
+
+int ipcgpu_neumann_energy(ipcgpu_ctx* ctx, double* E)
+{
+    REQUIRE_NEUMANN();
+    ENTER(kSerial);
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_DAMPING_BC);
+    neumann_energy(ctx->nV, ctx->V.p, ctx->nbc_f.p, ctx->mass.p, ctx->has_dbc ? ctx->dbc.p : nullptr, &ctx->iter.p->nbc_coef, ctx->nbc_partials.p, ctx->stream);
+    return energy_tail(ctx, kEnergyNeumann, ctx->nbc_partials.p, vertex_energy_blocks(ctx->nV), 1.0, pe, E);
+}
+
+int ipcgpu_neumann_gradient(ipcgpu_ctx* ctx, double* g_inout)
+{
+    REQUIRE_NEUMANN();
+    const uint8_t* dbc = ctx->has_dbc ? ctx->dbc.p : nullptr;
+    const double* coef = &ctx->iter.p->nbc_coef;
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { neumann_gradient(ctx->nV, ctx->nbc_f.p, ctx->mass.p, dbc, coef, ctx->g.p, st); },
+        IPCGPU_STAGE_DAMPING_BC);
+}
+
+static DirichletArgs dirichlet_args(ipcgpu_ctx* ctx)
+{
+    DirichletArgs p;
+    p.n = ctx->n_dbc; p.nV = ctx->nV;
+    p.vid = ctx->dbc_vid.p; p.tgt = ctx->dbc_tgt.p; p.lam = ctx->dbc_lam.p;
+    p.V = ctx->V.p; p.mass = ctx->mass.p;
+    p.rho = &ctx->iter.p->dbc_rho;
+    return p;
+}
+
+int ipcgpu_set_dirichlet_targets(ipcgpu_ctx* ctx, int n, const int* vid, const double* target, const double* lambda, double dist2Tol)
+{
+    REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    REQUIRE(n >= 0 && (n == 0 || (vid && target)), IPCGPU_ERR_ARG, "ipcgpu_set_dirichlet_targets: bad arguments");
+    REQUIRE(n == 0 || ctx->has_mass, IPCGPU_ERR_STATE, "the Dirichlet penalty needs the mass diagonal (ipcgpu_set_mesh)");
+    {
+        // targetPos is a map: one target per vertex (the gradient / Hessian kernels update a vertex's rows from one thread)
+        std::vector<char> seen((size_t)ctx->nV, 0);
+        for (int i = 0; i < n; ++i) {
+            REQUIRE(vid[i] >= 0 && vid[i] < ctx->nV, IPCGPU_ERR_ARG, "Dirichlet target vertex out of range");
+            REQUIRE(!seen[(size_t)vid[i]], IPCGPU_ERR_ARG, "Dirichlet target vertices must be distinct");
+            seen[(size_t)vid[i]] = 1;
+        }
+    }
+    REQUIRE_ONE_RANK();
+    ENTER(kSerial);
+    if (n > 0) {
+        ALLOC(ctx->dbc_vid, (size_t)n);
+        ALLOC(ctx->dbc_tgt, (size_t)3 * n);
+        ALLOC(ctx->dbc_lam, (size_t)3 * n);
+        ALLOC(ctx->dbc_partials, (size_t)vertex_energy_blocks(n) + 8);
+        CK(cudaMemcpyAsync(ctx->dbc_vid.p, vid, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->dbc_tgt.p, target, (size_t)3 * n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        if (lambda) CK(cudaMemcpyAsync(ctx->dbc_lam.p, lambda, (size_t)3 * n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        else CK(cudaMemsetAsync(ctx->dbc_lam.p, 0, (size_t)3 * n * sizeof(double), ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream)); // (the arrays are the caller's: the upload completes here)
+    }
+    // the number of targets is a launch shape (a new number needs a new capture); the same number with new values does not
+    if (n != ctx->n_dbc) {
+        int rc = term_switched(ctx, kEnergyDirichlet);
+        if (rc) return rc;
+    }
+    ctx->n_dbc = n;
+    set_double(&ctx->iter.p->dbc_tol, n ? dist2Tol : 0.0, ctx->stream); // (stream order: a new dist2Tol per time step needs no new capture)
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    return IPCGPU_OK;
+}
+
+int ipcgpu_set_dirichlet_penalty(ipcgpu_ctx* ctx, double rho)
+{
+    REQUIRE_ONE_RANK();
+    ENTER(kSerial);
+    set_double(&ctx->iter.p->dbc_rho, rho, ctx->stream);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    return IPCGPU_OK;
+}
+
+int ipcgpu_get_dirichlet_lambda(ipcgpu_ctx* ctx, double* lambda)
+{
+    REQUIRE(lambda != nullptr, IPCGPU_ERR_ARG, "null output");
+    REQUIRE_ONE_RANK();
+    ENTER(kSerial);
+    if (ctx->n_dbc > 0) CK(cudaMemcpyAsync(lambda, ctx->dbc_lam.p, (size_t)3 * ctx->n_dbc * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IPCGPU_OK;
+}
+
+#define REQUIRE_DIRICHLET()                                                                                                   \
+    REQUIRE_ONE_RANK();                                                                                                        \
+    if (ctx->n_dbc == 0) return IPCGPU_OK
+
+int ipcgpu_dirichlet_energy(ipcgpu_ctx* ctx, double* E)
+{
+    if (E) *E = 0.0;
+    REQUIRE_DIRICHLET();
+    ENTER(kSerial);
+    cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_DAMPING_BC);
+    dirichlet_energy(dirichlet_args(ctx), ctx->dbc_partials.p, ctx->stream);
+    return energy_tail(ctx, kEnergyDirichlet, ctx->dbc_partials.p, vertex_energy_blocks(ctx->n_dbc), 1.0, pe, E);
+}
+
+int ipcgpu_dirichlet_gradient(ipcgpu_ctx* ctx, int projectDBC, double* g_inout)
+{
+    REQUIRE_DIRICHLET();
+    if (projectDBC) return IPCGPU_OK; // (Optimizer.cpp:3542)
+    const DirichletArgs p = dirichlet_args(ctx);
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { dirichlet_gradient(p, ctx->g.p, st); }, IPCGPU_STAGE_DAMPING_BC);
+}
+
+int ipcgpu_dirichlet_hessian(ipcgpu_ctx* ctx, int projectDBC, double* a_inout)
+{
+    REQUIRE_DIRICHLET();
+    if (projectDBC) return IPCGPU_OK; // (:3711)
+    const DirichletArgs p = dirichlet_args(ctx);
+    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) { dirichlet_hessian(p, ctx->ia.p, ctx->index_base, ctx->a.p, st); }, IPCGPU_STAGE_DAMPING_BC);
+}
+
+int ipcgpu_dirichlet_update_lambda(ipcgpu_ctx* ctx)
+{
+    REQUIRE_DIRICHLET();
+    ENTER(kSerial);
+    dirichlet_update_lambda(dirichlet_args(ctx), ctx->dbc_lam.p, ctx->stream);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    return IPCGPU_OK;
+}
+
+int ipcgpu_dirichlet_completed_step(ipcgpu_ctx* ctx, double* s)
+{
+    REQUIRE_ONE_RANK();
+    ENTER(kSerial);
+    ALLOC(ctx->dbc_partials, (size_t)vertex_energy_blocks(ctx->n_dbc) + 8);
+    dirichlet_completed_step(dirichlet_args(ctx), &ctx->iter.p->dbc_tol, ctx->dbc_partials.p, &ctx->iter.p->dbc_step, ctx->stream);
+    ctx->launches += ctx->n_dbc ? 3 : 2;
+    CK(cudaGetLastError());
+    if (!s) return IPCGPU_OK;
+    CK(cudaMemcpyAsync(ctx->h_scalar, &ctx->iter.p->dbc_step, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    *s = ctx->h_scalar[0];
+    return IPCGPU_OK;
+}
+
 // ---- analytic half-space collision objects (halfspace.cu; which chain each call runs on: see enter()) ------------------------------------
 static HalfSpaceArgs halfspace_args(ipcgpu_ctx* ctx)
 {
@@ -2256,9 +2549,14 @@ static int ls_terms(const ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
     int terms = (t.inertia ? kTermInertia : 0) | (t.fric_coef > 0.0 ? kTermFriction : 0);
     if (ctx->n_hs > 0) terms |= kTermHalfSpace;
     if (ctx->n_hs > 0 && ctx->hs_lag_ready && t.fric_eps2 > 0.0) terms |= kTermHalfSpaceFriction;
+    // damping, Neumann forces and the Dirichlet penalty whenever they are set (ipcgpu_damping_update, _set_neumann_forces, _set_dirichlet_targets)
+    if (ctx->damp_on) terms |= kTermDamping;
+    if (ctx->nbc_on) terms |= kTermNeumann;
+    if (ctx->n_dbc > 0) terms |= kTermDirichlet;
     return terms;
 }
-// one trial's energy: E_el, E_in, E_b, E_f (and the planes' terms) into IterState (summed by the decision that reads them)
+// one trial's energy: E_el, E_in, E_b, E_f (and the planes', damping, Neumann and Dirichlet-penalty terms) into IterState (summed by the decision
+// that reads them)
 static int ls_energy(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
 {
     const int terms = ls_terms(ctx, t);
@@ -2268,6 +2566,9 @@ static int ls_energy(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
     if (!rc && (terms & kTermHalfSpace)) rc = ipcgpu_halfspace_energy(ctx, t.dHat, t.kappa, nullptr);
     if (!rc && (terms & kTermHalfSpaceFriction)) rc = ipcgpu_halfspace_friction_energy(ctx, t.fric_eps2, nullptr);
     if (!rc && t.fric_coef > 0.0) rc = ipcgpu_friction_energy(ctx, t.fric_eps2, t.fric_coef, nullptr);
+    if (!rc && (terms & kTermDamping)) rc = ipcgpu_damping_energy(ctx, nullptr);
+    if (!rc && (terms & kTermNeumann)) rc = ipcgpu_neumann_energy(ctx, nullptr);
+    if (!rc && (terms & kTermDirichlet)) rc = ipcgpu_dirichlet_energy(ctx, nullptr);
     return rc;
 }
 // a trial's constraint sets: the self-contact set and the planes' (isIntersected and computeConstraintSet cover every collision object)
@@ -2339,6 +2640,7 @@ int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* t, doubl
         "friction: ipcgpu_friction_lag, ipcgpu_set_prev_state and fric_eps2 > 0 first");
     REQUIRE(ctx->n_hs == 0 || ctx->hs_set_built, IPCGPU_ERR_STATE, "half-spaces: ipcgpu_halfspace_constraint_set first (E0 takes the sets held on entry)");
     REQUIRE(!(ls_terms(ctx, *t) & kTermHalfSpaceFriction) || ctx->prev_set, IPCGPU_ERR_STATE, "half-space friction: ipcgpu_set_prev_state first");
+    REQUIRE(!ctx->damp_on || ctx->prev_set, IPCGPU_ERR_STATE, "damping: ipcgpu_set_prev_state first");
     REQUIRE(!(ctx->capturing && ctx->canonical_order), IPCGPU_ERR_STATE, "inside a capture the line search needs ipcgpu_set_canonical_order(ctx, 0)");
     ENTER(kSerial);
     int rc = step_control_prepare(ctx);
@@ -2485,6 +2787,10 @@ int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
     out->alpha_halfspace = h.hs_alpha;
     out->n_halfspace_active = h.hs_n_active;
     out->n_halfspace_crossings = h.hs_crossings;
+    out->energy_damping = h.energy[kEnergyDamping];
+    out->energy_neumann = h.energy[kEnergyNeumann];
+    out->energy_dirichlet = h.energy[kEnergyDirichlet];
+    out->dirichlet_completed_step = h.dbc_step;
     ContactWork& w = ctx->cw;
     w.nC = h.n_set[0]; w.nP = h.n_set[1]; w.nK = h.n_set[2];
     int status = status_from_flags(ctx, h.flags);

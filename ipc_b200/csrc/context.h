@@ -197,6 +197,13 @@ struct ipcgpu_ctx {
     ipcgpu::DevBuf<unsigned char> hs_scan;
     size_t hs_scan_bytes = 0;
     bool hs_set_built = false, hs_lag_ready = false;
+    // Rayleigh damping, Neumann forces and the Dirichlet penalty (damping.cu): D in slot order (9 doubles per slot) and its per-vertex slot
+    // incidence (built once per mesh, at the first ipcgpu_damping_update); the summed Neumann force per vertex (interleaved); the Dirichlet
+    // targets (vertex, target, multiplier).  A new mesh (build_maps) removes all three.
+    bool damp_on = false, damp_inc_ready = false, nbc_on = false;
+    int n_dbc = 0;
+    ipcgpu::DevBuf<double> damp_D, damp_partials, nbc_f, nbc_partials, dbc_tgt, dbc_lam, dbc_partials;
+    ipcgpu::DevBuf<int> damp_inc_ptr, damp_inc, dbc_vid;
     size_t ccd_capacity = (size_t)1 << 23; // candidate pairs
     std::vector<int> h_SVI;                // host copy (pSize of the swept build is a serial host sum, SpatialHash.hpp:603-612)
     double debug_prune_seed = -1.0;        // test hook, see ipcgpu_ccd_debug_seed_bound

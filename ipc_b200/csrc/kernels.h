@@ -6,7 +6,8 @@
 namespace ipcgpu {
 
 // slots of IterState::energy
-enum { kEnergyElastic = 0, kEnergyBarrier, kEnergyFriction, kEnergyInertia, kEnergyPlaneBarrier, kEnergyPlaneFriction, kEnergySlots };
+enum { kEnergyElastic = 0, kEnergyBarrier, kEnergyFriction, kEnergyInertia, kEnergyPlaneBarrier, kEnergyPlaneFriction, kEnergyDamping, kEnergyNeumann,
+    kEnergyDirichlet, kEnergySlots };
 
 // Device-resident scalars of one Newton iteration.  Every stage reads its inputs from here and leaves its outputs here, so a whole
 // iteration is one stream of launches (and in-stream NCCL reductions) with a single read-back at the end (ipcgpu_fetch_iteration).
@@ -37,6 +38,11 @@ struct IterState {
     int ls_count[4];                  // halvings: inversion guard, intersection pre-check, Armijo loop, post-check
     int ls_stopped, ls_rebuilt, ls_post_ran;
     int ls_cond;                      // the decision word of the last step_decide
+    // Dirichlet penalty and Neumann forces (damping.cu; before the half-space words, which ipcgpu_set_halfspaces clears as one range)
+    double dbc_rho;                   // rho_DBC (ipcgpu_set_dirichlet_penalty), read by the penalty kernels at run time
+    double dbc_step;                  // the last computeCompletedStepSize
+    double dbc_tol;                   // dist2Tol of the targets (ipcgpu_set_dirichlet_targets; 0 without targets), read at run time
+    double nbc_coef;                  // dt^2 of the Neumann term (ipcgpu_set_neumann_forces)
     // half-space collision objects (halfspace.cu)
     double hs_alpha;                  // step after the plane bound
     int hs_n_active, hs_n_lagged;     // sizes of the plane active set / lagged set (replicated on every rank)
@@ -52,7 +58,7 @@ struct IterState {
 };
 // step_decide operations (step_control.cu) and the energy terms of a line search
 enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersection, kLsArmijo, kLsPostCheck, kLsPostLoop, kLsRebuild };
-enum { kTermInertia = 1, kTermFriction = 2, kTermHalfSpace = 4, kTermHalfSpaceFriction = 8 };
+enum { kTermInertia = 1, kTermFriction = 2, kTermHalfSpace = 4, kTermHalfSpaceFriction = 8, kTermDamping = 16, kTermNeumann = 32, kTermDirichlet = 64 };
 enum { FLAG_NONPOSITIVE_DISTANCE = 0, FLAG_SET_CAPACITY = 1, FLAG_CCD_CAPACITY = 2, FLAG_ZERO_CCD_DISTANCE = 3, FLAG_PATTERN = 4, FLAG_TI_WARNINGS = 5, FLAG_EXCHANGE_CAPACITY = 6,
     FLAG_PATTERN_CAPACITY = 7 };
 // Scalars that may still hold this rank's share (ipcgpu_ctx::local_scalars): bit s = energy[s], then checks and hs_crossings.  The fetch
@@ -211,6 +217,37 @@ void halfspace_lag(const HalfSpaceArgs& p, double dHat, double kappa, const int*
 void halfspace_friction_energy(const HalfSpaceArgs& p, double eps2, double* partials, cudaStream_t st);
 void halfspace_friction_gradient(const HalfSpaceArgs& p, double eps2, double* g, cudaStream_t st);
 void halfspace_friction_hessian(const HalfSpaceArgs& p, double eps2, int projectDBC, double* a, cudaStream_t st);
+
+// damping.cu -- Rayleigh damping (D in elastic slot order, 9 doubles per slot), Neumann forces, augmented-Lagrangian Dirichlet penalty
+struct DampingArgs {
+    int nV, nSlots;
+    const int* slot_v; const int* slot_u;
+    const int* inc_ptr; const int* inc;   // slot incidence per vertex (nV + 1 starts; entry 2s: as slot_v, 2s + 1: as slot_u of an off-diagonal slot)
+    const double* D;
+    const double* V; const double* Vprev; // SoA
+    const uint8_t* dbc;                   // nullable
+};
+struct DirichletArgs {
+    int n, nV;
+    const int* vid; const double* tgt; const double* lam; // targets: vertex, target position and multiplier (3 per target, interleaved)
+    const double* V; const double* mass;
+    const double* rho;                    // device-resident rho_DBC (IterState::dbc_rho)
+};
+void damping_assemble(int nSlots, const int* slot_v, const int* slot_u, const int* con_ptr, const unsigned* con_src, const double* hblk, const uint8_t* dbc,
+    double* D, cudaStream_t st);
+int damping_energy_blocks(int nSlots);
+void damping_energy(const DampingArgs& p, double* partials, cudaStream_t st);
+void damping_gradient(const DampingArgs& p, int projectDBC, double* g, cudaStream_t st);
+void damping_hessian(const DampingArgs& p, const int* slot_off, double* a, cudaStream_t st);
+int vertex_energy_blocks(int n); // partials of the per-vertex / per-target energies below
+void neumann_energy(int nV, const double* x, const double* f, const double* mass, const uint8_t* dbc, const double* coef, double* partials, cudaStream_t st);
+void neumann_gradient(int nV, const double* f, const double* mass, const uint8_t* dbc, const double* coef, double* g, cudaStream_t st);
+void dirichlet_energy(const DirichletArgs& p, double* partials, cudaStream_t st);
+void dirichlet_gradient(const DirichletArgs& p, double* g, cudaStream_t st);
+void dirichlet_hessian(const DirichletArgs& p, const int* ia, int base, double* a, cudaStream_t st);
+void dirichlet_update_lambda(const DirichletArgs& p, double* lam, cudaStream_t st);
+void dirichlet_completed_step(const DirichletArgs& p, const double* dist2Tol, double* partials, double* out, cudaStream_t st); // 3 launches (dist2Tol: device)
+void set_double(double* p, double v, cudaStream_t st); // a device double in stream order
 
 // zero n_words 4-byte words.  A kernel rather than cudaMemsetAsync where the two chains of an iteration overlap (api.cu): replayed from a
 // graph, a memset node has no priority of its own and queues behind whatever low-priority grids are pending, which held the step-bound

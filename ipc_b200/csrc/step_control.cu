@@ -46,14 +46,19 @@ DEV int halve_while(IterState* st, bool bad, int counter)
     return 1;
 }
 // E = ((E_el + E_in) + E_b) + E_f, the accumulation order of Optimizer::computeEnergyVal (Optimizer.cpp:3199-3378); with half-spaces
-// ((E_el + E_in) + (E_b + E_plane_b)) + E_plane_f + E_f: both barrier parts are one kappa bVals.sum() (:3352), plane friction comes first (:3355-3377)
+// ((E_el + E_in) + (E_b + E_plane_b)) + E_plane_f + E_f: both barrier parts are one kappa bVals.sum() (:3352), plane friction comes first (:3355-3377).
+// The Neumann forces come right after the inertia term (:3241-3250), damping (:3381-3400) and the Dirichlet penalty (:3402-3404) last:
+// ((((((E_el + E_in) + E_nbc) + E_b) + E_plane_f) + E_f) + E_damp) + E_dbc.  A term that is not set adds nothing (not even a 0).
 DEV double energy_sum(const IterState* st, int terms)
 {
     double e = st->energy[kEnergyElastic];
     if (terms & kTermInertia) e += st->energy[kEnergyInertia];
+    if (terms & kTermNeumann) e += st->energy[kEnergyNeumann];
     e += (terms & kTermHalfSpace) ? st->energy[kEnergyBarrier] + st->energy[kEnergyPlaneBarrier] : st->energy[kEnergyBarrier];
     if (terms & kTermHalfSpaceFriction) e += st->energy[kEnergyPlaneFriction];
     if (terms & kTermFriction) e += st->energy[kEnergyFriction];
+    if (terms & kTermDamping) e += st->energy[kEnergyDamping];
+    if (terms & kTermDirichlet) e += st->energy[kEnergyDirichlet];
     return e;
 }
 // the intersection safeguard: surface triangles crossed by an edge, and with half-spaces the vertices with d <= 0 (isIntersected, :2627-2642)

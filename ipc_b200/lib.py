@@ -122,10 +122,25 @@ SIGNATURES = {
     "ipcgpu_halfspace_friction_gradient": (C.c_int, [_ctxp, C.c_double, _dp]),
     "ipcgpu_halfspace_friction_hessian": (C.c_int, [_ctxp, C.c_double, C.c_int, _dp]),
     "ipcgpu_get_halfspace_sets": (C.c_int, [_ctxp, _ip, _ip, _ip, _ip, _dp]),
+    "ipcgpu_damping_update": (C.c_int, [_ctxp, C.c_double]),
+    "ipcgpu_damping_energy": (C.c_int, [_ctxp, _dp]),
+    "ipcgpu_damping_gradient": (C.c_int, [_ctxp, C.c_int, _dp]),
+    "ipcgpu_damping_hessian": (C.c_int, [_ctxp, _dp]),
+    "ipcgpu_set_neumann_forces": (C.c_int, [_ctxp, C.c_double, _dp]),
+    "ipcgpu_neumann_energy": (C.c_int, [_ctxp, _dp]),
+    "ipcgpu_neumann_gradient": (C.c_int, [_ctxp, _dp]),
+    "ipcgpu_set_dirichlet_targets": (C.c_int, [_ctxp, C.c_int, _ip, _dp, _dp, C.c_double]),
+    "ipcgpu_set_dirichlet_penalty": (C.c_int, [_ctxp, C.c_double]),
+    "ipcgpu_get_dirichlet_lambda": (C.c_int, [_ctxp, _dp]),
+    "ipcgpu_dirichlet_energy": (C.c_int, [_ctxp, _dp]),
+    "ipcgpu_dirichlet_gradient": (C.c_int, [_ctxp, C.c_int, _dp]),
+    "ipcgpu_dirichlet_hessian": (C.c_int, [_ctxp, C.c_int, _dp]),
+    "ipcgpu_dirichlet_update_lambda": (C.c_int, [_ctxp]),
+    "ipcgpu_dirichlet_completed_step": (C.c_int, [_ctxp, _dp]),
 }
 
 STAGES = ["elastic_energy", "elastic_tet", "gather_gradient", "assemble_csr", "inversion", "hash", "constraint_set", "barrier",
-          "ccd_broad", "ccd_narrow", "allreduce", "ccd_root_filter"]
+          "ccd_broad", "ccd_narrow", "allreduce", "ccd_root_filter", "damping_bc"]
 
 _lib = None
 
@@ -137,7 +152,8 @@ class Iteration(C.Structure):
                 ("n_candidates", C.c_int), ("status", C.c_int), ("n_full_ccd_candidates", C.c_uint64), ("ti_warnings", C.c_uint64),
                 ("n_inverted_tets", C.c_int), ("n_intersected_triangles", C.c_int), ("energy_friction", C.c_double), ("energy_inertia", C.c_double),
                 ("energy_halfspace", C.c_double), ("energy_halfspace_friction", C.c_double), ("alpha_halfspace", C.c_double),
-                ("n_halfspace_active", C.c_int), ("n_halfspace_crossings", C.c_int)]
+                ("n_halfspace_active", C.c_int), ("n_halfspace_crossings", C.c_int), ("energy_damping", C.c_double), ("energy_neumann", C.c_double),
+                ("energy_dirichlet", C.c_double), ("dirichlet_completed_step", C.c_double)]
 
 
 class LineSearchTerms(C.Structure):
@@ -519,6 +535,76 @@ class Context:
         act, lag, lam = np.empty((max(na.value, 1), 2), np.int32), np.empty((max(nl.value, 1), 2), np.int32), np.empty(max(nl.value, 1))
         self._ck(self.lib.ipcgpu_get_halfspace_sets(self.h, C.byref(na), _i(act), C.byref(nl), _i(lag), _d(lam)))
         return act[:na.value], lag[:nl.value], lam[:nl.value]
+
+    # ---- damping, Neumann forces, Dirichlet penalty --------------------------------------------------
+    def damping_update(self, coef):
+        """computeDampingMtr at the current state (coef = energyParams[0] dampingStiff / dt); 0 removes the term"""
+        self._ck(self.lib.ipcgpu_damping_update(self.h, float(coef)))
+
+    def damping_energy(self, want=True):
+        E = C.c_double()
+        self._ck(self.lib.ipcgpu_damping_energy(self.h, C.byref(E) if want else None))
+        return E.value if want else None
+
+    def damping_gradient(self, projectDBC=1, g_inout=None):
+        self._ck(self.lib.ipcgpu_damping_gradient(self.h, int(projectDBC), _d(g_inout)))
+        return g_inout
+
+    def damping_hessian(self, a_inout=None):
+        self._ck(self.lib.ipcgpu_damping_hessian(self.h, _d(a_inout)))
+        return a_inout
+
+    def set_neumann_forces(self, coef, f):
+        """f: per-vertex summed force of the active NBCs (nV, 3) or None (removes the term); coef = dt^2"""
+        f = None if f is None else f64(np.asarray(f, dtype=np.float64).reshape(-1))
+        self._ck(self.lib.ipcgpu_set_neumann_forces(self.h, float(coef), _d(f)))
+
+    def neumann_energy(self, want=True):
+        E = C.c_double()
+        self._ck(self.lib.ipcgpu_neumann_energy(self.h, C.byref(E) if want else None))
+        return E.value if want else None
+
+    def neumann_gradient(self, g_inout=None):
+        self._ck(self.lib.ipcgpu_neumann_gradient(self.h, _d(g_inout)))
+        return g_inout
+
+    def set_dirichlet_targets(self, vid, target, lam=None, dist2Tol=0.0):
+        """targetPos: vertices (n,), target positions (n, 3), multipliers (n, 3) or None (0); an empty list removes the term"""
+        vid = i32(np.asarray(vid).reshape(-1))
+        n = int(vid.size)
+        t = f64(np.asarray(target, dtype=np.float64).reshape(-1))
+        lam = None if lam is None else f64(np.asarray(lam, dtype=np.float64).reshape(-1))
+        self._ck(self.lib.ipcgpu_set_dirichlet_targets(self.h, n, _i(vid) if n else None, _d(t) if n else None, _d(lam) if n else None, float(dist2Tol)))
+        self.n_dbc = n
+
+    def set_dirichlet_penalty(self, rho):
+        self._ck(self.lib.ipcgpu_set_dirichlet_penalty(self.h, float(rho)))
+
+    def get_dirichlet_lambda(self):
+        out = np.empty(3 * max(getattr(self, "n_dbc", 0), 1))
+        self._ck(self.lib.ipcgpu_get_dirichlet_lambda(self.h, _d(out)))
+        return out[:3 * getattr(self, "n_dbc", 0)].reshape(-1, 3)
+
+    def dirichlet_energy(self, want=True):
+        E = C.c_double()
+        self._ck(self.lib.ipcgpu_dirichlet_energy(self.h, C.byref(E) if want else None))
+        return E.value if want else None
+
+    def dirichlet_gradient(self, projectDBC=0, g_inout=None):
+        self._ck(self.lib.ipcgpu_dirichlet_gradient(self.h, int(projectDBC), _d(g_inout)))
+        return g_inout
+
+    def dirichlet_hessian(self, projectDBC=0, a_inout=None):
+        self._ck(self.lib.ipcgpu_dirichlet_hessian(self.h, int(projectDBC), _d(a_inout)))
+        return a_inout
+
+    def dirichlet_update_lambda(self):
+        self._ck(self.lib.ipcgpu_dirichlet_update_lambda(self.h))
+
+    def dirichlet_completed_step(self, want=True):
+        s = C.c_double()
+        self._ck(self.lib.ipcgpu_dirichlet_completed_step(self.h, C.byref(s) if want else None))
+        return s.value if want else None
 
     # ---- contact ------------------------------------------------------------------------------
     def set_surface(self, SVI, SFEdges, SF_soa, vCoDim=None):
