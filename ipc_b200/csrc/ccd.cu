@@ -23,8 +23,7 @@
 //                 origin and the first "terminal" box, which is all the sequential semantics depend on.
 //   reduction   : atomicMin on the order-preserving uint64 image of the (non-negative) time of impact.
 #include "broadphase.cuh"
-#include "context.h"
-#include "../../include/ipcgpu.h"
+#include "abi.h"
 #include <cub/cub.cuh>
 
 namespace ipcgpu {
@@ -1561,17 +1560,6 @@ __global__ void k_ccd_commit(IterState* st, int stage)
 
 using namespace ipcgpu;
 
-#define CKD(call)                                                      \
-    do {                                                               \
-        cudaError_t e_ = (call);                                       \
-        if (e_ != cudaSuccess) {                                       \
-            ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
-            return IPCGPU_ERR_CUDA;                                    \
-        }                                                              \
-    } while (0)
-
-static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
-SurfArgs surf_args(const ipcgpu_ctx* ctx); // constraint.cu
 
 constexpr int kStage2WarpsPerCta = 4;
 // persistent: 2 CTAs x 4 warps per SM, compiled for 2 CTAs per SM (230 registers, no spill; for 3 per SM it spilled 226 B per thread).  Fewer
@@ -1598,10 +1586,6 @@ int ccd_alloc(ipcgpu_ctx* ctx)
     }
     return 0;
 }
-
-// cross-rank min of the running minimum (api.cu; no-op on one rank)
-int nccl_min_u64(ipcgpu_ctx* ctx, unsigned long long* word);
-int fetch_iter_state(ipcgpu_ctx* ctx); // api.cu: one D2H copy of the iteration state + stream synchronisation
 
 // Narrow phase over a device-resident candidate list.  The step is read from and written back to the device-resident iteration state
 // (IterState::step_ord): nothing is read back here.  n32 / n64: device-resident list size; share: walk only this rank's contiguous
@@ -1646,14 +1630,14 @@ int ccd_narrow(ipcgpu_ctx* ctx, const int2* cand, const int* n32, const unsigned
         const long long budget = ctx->debug_ti_budget >= 0 ? ctx->debug_ti_budget : kThreadBudget;
         constexpr int bytes = 2 * 128 * (kThreadLevel * (int)sizeof(DBox) + 8);
         static bool attr = false;
-        if (!attr) { CKD(cudaFuncSetAttribute(k_ti_stage15_refill, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); attr = true; }
+        if (!attr) { CK(cudaFuncSetAttribute(k_ti_stage15_refill, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); attr = true; }
         k_ti_stage15_refill<<<kSMs * 2, 128, bytes, st>>>(a, w.surv.p, nSurv, refill_work, w.surv2.p, nDefA, budget, &ist->ccd_ord, flags + 1);
         k_ti_stage2<<<kStage2Ctas, 32 * kStage2WarpsPerCta, 0, st>>>(a, w.surv2.p, nDefA, work, reinterpret_cast<DBox*>(w.scratch.p), kLevelCap, &ist->ccd_ord, flags + 1);
     }
     k_ccd_finish<<<1, 32, 0, st>>>(ist, nSurv, flags, overflow, stage == 3);
     ctx->prof_end(pe);
     ctx->launches += 5;
-    CKD(cudaGetLastError());
+    CK(cudaGetLastError());
     int rc = nccl_min_u64(ctx, &ist->ccd_ord); // min over ranks of the step; a zero-distance flag travels as step 0
     if (rc) return rc;
     k_ccd_commit<<<1, 32, 0, st>>>(ist, stage);
@@ -1708,12 +1692,12 @@ int ccd_build_swept(ipcgpu_ctx* ctx, double h)
         zero_words(w.sw_cnt.p, nTab, st); // (kernels.h: not a memset)
         k_swept_count<<<nblk(nPrim, 256), 256, 0, st>>>(s, w.vmin.p, w.vmax.p, w.cells.p, w.sw_cnt.p);
         size_t bytes = w.sw_tmp.n;
-        CKD(cub::DeviceScan::ExclusiveSum(w.sw_tmp.p, bytes, w.sw_cnt.p, w.sw_off.p, (int)nTab, st));
+        CK(cub::DeviceScan::ExclusiveSum(w.sw_tmp.p, bytes, w.sw_cnt.p, w.sw_off.p, (int)nTab, st));
         k_swept_scatter<<<nblk(nPrim, 256), 256, 0, st>>>(s, w.vmin.p, w.vmax.p, w.cells.p, w.sw_cnt.p, w.sw_off.p, w.sw_keys.p, w.sw_ent.p);
         ctx->launches += 7;
     }
     ctx->prof_end(pe);
-    CKD(cudaGetLastError());
+    CK(cudaGetLastError());
     w.swept_ready = true;
     return 0;
 }
@@ -1724,8 +1708,8 @@ int ccd_full(ipcgpu_ctx* ctx, double tol, const double* err_vf, const double* er
     cudaStream_t st = ctx->stream;
     const SurfArgs s = surf_args(ctx);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_CCD_BROAD);
-    CKD(cudaMemsetAsync(w.ncand.p, 0, 2 * sizeof(unsigned long long), st));
-    CKD(cudaMemsetAsync(w.counters.p + 14, 0, sizeof(int), st));
+    CK(cudaMemsetAsync(w.ncand.p, 0, 2 * sizeof(unsigned long long), st));
+    CK(cudaMemsetAsync(w.counters.p + 14, 0, sizeof(int), st));
     SweptArgs a{ s, ctx->dir.p, ctx->iter.p, w.vmin.p, w.vmax.p, w.cells.p, w.sw_keys.p, w.sw_ent.p, w.sw_off.p, 0, 0,
         CandOut{ w.cand.p, w.ncand.p, (unsigned long long)ctx->ccd_capacity, w.counters.p + 14 } };
     // multi-GPU: every rank keeps a disjoint share of the pairs -- PT by the surface vertex, EE by the smaller edge id (the reference's own

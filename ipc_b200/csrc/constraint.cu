@@ -11,8 +11,7 @@
 // The output ORDER is canonical (sorted), unlike the reference whose order depends on unordered_set iteration and TBB
 // scheduling (:2176, :2282 "different constraint order will result in numerically different results").
 #include "broadphase.cuh"
-#include "context.h"
-#include "../../include/ipcgpu.h"
+#include "abi.h"
 #include <cub/cub.cuh>
 
 namespace ipcgpu {
@@ -711,16 +710,6 @@ __global__ void k_dup_emit(unsigned size, const unsigned long long* __restrict__
 
 using namespace ipcgpu;
 
-#define CKC(call)                                                      \
-    do {                                                               \
-        cudaError_t e_ = (call);                                       \
-        if (e_ != cudaSuccess) {                                       \
-            ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
-            return IPCGPU_ERR_CUDA;                                    \
-        }                                                              \
-    } while (0)
-
-static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
 static void cell_pairs_pt(const Grid* gp, const SortedGrid& vg, const SortedGrid& tg, const SurfArgs& s, double radius, int first, int last, const PairOut& out, cudaStream_t st)
 {
     if (last > first) k_cell_pairs_pt<<<nblk(last - first, 32 * kCellPairWarps), 32 * kCellPairWarps, 0, st>>>(gp, vg, tg, s.SVI, s.SF, s.nSF, radius, first, last, out);
@@ -763,10 +752,10 @@ static int sort_lex(ipcgpu_ctx* ctx, int4* data, int2* comp, int n, int4* tmp4, 
     k_key_from4<<<nblk(n, 256), 256, 0, st>>>(n, data, w.sidx.p, 1, w.skey.p);
     if ((rc = sort_pass(ctx, n))) return rc;
     k_gather<int4><<<nblk(n, 256), 256, 0, st>>>(n, data, w.sidx.p, tmp4);
-    CKC(cudaMemcpyAsync(data, tmp4, (size_t)n * sizeof(int4), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(data, tmp4, (size_t)n * sizeof(int4), cudaMemcpyDeviceToDevice, st));
     if (comp) {
         k_gather<int2><<<nblk(n, 256), 256, 0, st>>>(n, comp, w.sidx.p, tmp2);
-        CKC(cudaMemcpyAsync(comp, tmp2, (size_t)n * sizeof(int2), cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(comp, tmp2, (size_t)n * sizeof(int2), cudaMemcpyDeviceToDevice, st));
     }
     ctx->launches += 6;
     return 0;
@@ -782,7 +771,7 @@ static int sort_int2(ipcgpu_ctx* ctx, int2* data, int n, int2* tmp2)
     int rc;
     if ((rc = sort_pass(ctx, n))) return rc;
     k_gather<int2><<<nblk(n, 256), 256, 0, st>>>(n, data, w.sidx.p, tmp2);
-    CKC(cudaMemcpyAsync(data, tmp2, (size_t)n * sizeof(int2), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(data, tmp2, (size_t)n * sizeof(int2), cudaMemcpyDeviceToDevice, st));
     ctx->launches += 3;
     return 0;
 }
@@ -828,7 +817,6 @@ int contact_alloc(ipcgpu_ctx* ctx)
 
 // build the sorted grids of the triangles and the edges in ONE pass: one emit, one radix sort (cell key + type bit), one gather of the
 // quantised entries, one cell table
-SurfArgs surf_args(const ipcgpu_ctx* ctx);
 static int build_grids(ipcgpu_ctx* ctx, int nT, int nE, int nV)
 {
     ContactWork& w = ctx->cw;
@@ -893,7 +881,7 @@ int boxes_and_grid(ipcgpu_ctx* ctx, double radius, bool with_vertex_boxes)
     return build_grids(ctx, s.nSF, s.nSE, with_vertex_boxes ? s.nSV : 0);
 }
 
-// pack this rank's lists, allgather, rebuild the global lists (called by api.cu around its ncclAllGather)
+// pack this rank's lists, allgather, rebuild the global lists (called by ipcgpu_constraint_set around its all-gather)
 void contact_pack_lists(ipcgpu_ctx* ctx)
 {
     ContactWork& w = ctx->cw;
@@ -912,9 +900,9 @@ void contact_unpack_lists(ipcgpu_ctx* ctx)
 int contact_sync_counts(ipcgpu_ctx* ctx)
 {
     ContactWork& w = ctx->cw;
-    int* h = reinterpret_cast<int*>(ctx->h_scalar);
-    CKC(cudaMemcpyAsync(h, w.counters.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    CKC(cudaStreamSynchronize(ctx->stream));
+    int* h = ctx->staging->contact;
+    CK(cudaMemcpyAsync(h, w.counters.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     if (h[4]) {
         ctx->err = "constraint-set capacity exceeded (raise it with ipcgpu_set_pair_capacity)";
         return IPCGPU_ERR_CAPACITY;
@@ -940,7 +928,7 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
     ctx->prof_end(pe);
 
     pe = ctx->prof_begin(IPCGPU_STAGE_CONSTRAINT_SET);
-    CKC(cudaMemsetAsync(w.counters.p, 0, 16 * sizeof(int), st));
+    CK(cudaMemsetAsync(w.counters.p, 0, 16 * sizeof(int), st));
     CsOut out;
     out.act = w.act.p; out.nAct = w.counters.p + 0; out.capAct = w.cap;
     out.dup = w.dup.p; out.nDup = w.counters.p + 1; out.capDup = w.cap;
@@ -972,8 +960,8 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
     // merge PP/PE duplicates into the active list with negative multiplicities (:2434-2476)
     const bool hashed_merge = ctx->nV < (1 << 21) - 2;
     if (hashed_merge) { // (x,y,z) packs into one 64-bit key: fixed-size table, no host-side size needed
-        CKC(cudaMemsetAsync(w.skey.p, 0xff, (size_t)w.dup_tab * sizeof(unsigned long long), st));
-        CKC(cudaMemsetAsync(w.sidx.p, 0, (size_t)w.dup_tab * sizeof(int), st));
+        CK(cudaMemsetAsync(w.skey.p, 0xff, (size_t)w.dup_tab * sizeof(unsigned long long), st));
+        CK(cudaMemsetAsync(w.sidx.p, 0, (size_t)w.dup_tab * sizeof(int), st));
         k_dup_insert<<<kSMs * 2, 256, 0, st>>>(w.counters.p + 1, w.cap, w.dup.p, w.skey.p, w.sidx.p, w.dup_tab - 1, w.counters.p + 4);
         k_dup_emit<<<nblk(w.dup_tab, 256), 256, 0, st>>>(w.dup_tab, w.skey.p, w.sidx.p, w.act.p, w.counters.p + 0, w.cap, w.counters.p + 4);
         ctx->launches += 2;
@@ -982,10 +970,10 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
     w.nC = w.nP = w.nK = -1; // unknown on the host until somebody asks
     const bool need_host = !hashed_merge || ctx->canonical_order || nC || nPara || nCand;
     if (need_host) {
-        int* h = reinterpret_cast<int*>(ctx->h_scalar);
+        int* h = ctx->staging->contact;
         if (!hashed_merge) { // huge meshes: sort-based merge, sized on the host
-            CKC(cudaMemcpyAsync(h, w.counters.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
-            CKC(cudaStreamSynchronize(st));
+            CK(cudaMemcpyAsync(h, w.counters.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
             const int nDup = std::min(h[1], w.cap);
             if (nDup > 0) {
                 if ((rc = sort_lex(ctx, w.dup.p, nullptr, nDup, w.tmp4.p, nullptr))) return rc;

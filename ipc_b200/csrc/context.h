@@ -116,6 +116,19 @@ struct PatternWork {
     uint64_t requested_cap = 0;       // what the caller asked for (0 = default), kept to rebuild after a surface / obstacle change
 };
 
+// pinned host memory of the scalars the entry points copy between host and device, one member per use.  Allocated once per context
+// (cudaMallocHost(sizeof(HostStaging))), freed by ipcgpu_destroy: every member keeps its own address for the context's lifetime, since a
+// captured graph or a copy nobody waits on may still hold it.
+struct HostStaging {
+    double scalar;   // a read-back double: energy_result, ipcgpu_dirichlet_completed_step
+    int count;       // a read-back count: the lagged friction pairs
+    int contact[16]; // ContactWork::counters read back (contact_sync_counts, the sort-based duplicate merge) or uploaded (ipcgpu_set_constraint_set)
+    double pcg[8];   // the PCG scalars (solve.cu), then its residual history entry
+    double pSize;    // source of upload_dir's asynchronous H2D copy into pSize_dev, which nothing waits on: never reused for anything else
+    int decision;    // the step-control decision word (IterState::ls_cond) of the host loop of a CFL branch / line search
+    int hs_count[2]; // half-space counts: [0] active, [1] lagged
+};
+
 } // namespace ipcgpu
 
 struct ipcgpu_ctx {
@@ -123,7 +136,7 @@ struct ipcgpu_ctx {
     // main stream, high priority: everything except the derivative chain, in particular the step-bound chain (the critical path)
     cudaStream_t stream = nullptr;
     // derivative stream, low priority: the elastic gradient/Hessian, its CSR assembly and the barrier gradient / Hessian scatter of the
-    // device-resident iteration run here next to the step-bound chain (api.cu: enter / join_deriv).  deriv_open: work has been forked
+    // device-resident iteration run here next to the step-bound chain (abi.h: enter / join_deriv).  deriv_open: work has been forked
     // onto it that the main stream has not joined yet; deriv_copied: the capture in progress copies derivative results to the host
     cudaStream_t deriv = nullptr;
     cudaEvent_t ev_deriv_fork = nullptr, ev_deriv_done = nullptr;
@@ -260,7 +273,7 @@ struct ipcgpu_ctx {
     };
     std::vector<GraphRec> graphs;
     std::vector<cudaGraph_t> capture_bodies; // conditional-node bodies of the capture in progress
-    // step control (api.cu: cond_node): the bodies of nested conditional nodes are captured on these high-priority streams, one per depth
+    // step control (api_step.cu: cond_node): the bodies of nested conditional nodes are captured on these high-priority streams, one per depth
     static constexpr int kCondDepth = 3;
     cudaStream_t cond_streams[kCondDepth] = { nullptr, nullptr, nullptr };
     int cond_depth = 0;
@@ -268,7 +281,7 @@ struct ipcgpu_ctx {
     bool capturing = false, pat_pending_at_capture = false;
     uint64_t epoch = 0, launches_at_capture = 0;
     bool dirty_at_capture = false;
-    double* h_scalar = nullptr; // pinned staging for scalars
+    ipcgpu::HostStaging* staging = nullptr; // pinned staging for scalars
 
     // profiling: event pairs per stage (only when enabled)
     bool profiling = false;

@@ -2,7 +2,7 @@
 // Rayleigh damping 1/2 d^T D d (Optimizer.cpp:3381-3400, :3519-3540, :3707-3709, D from computeDampingMtr :3723-3734), the Neumann forces
 // (:3241-3250, :3452-3461) and the augmented-Lagrangian Dirichlet penalty (AnimScripter.cpp:2286-2344).
 //
-// D is held once, in the elastic slot order of api.cu's build_maps: one full 3x3 row-major block per mesh vertex pair (slot_v <= slot_u),
+// D is held once, in the elastic slot order of api_mesh.cu's build_maps: one full 3x3 row-major block per mesh vertex pair (slot_v <= slot_u),
 // so it does not depend on the system's sparsity pattern (host- or device-built); slot_off places a block in the CSR.  Every sum is in a
 // fixed order (per-CTA partials, then k_reduce_sum; the per-vertex gather walks a slot incidence list built once per mesh): no atomics,
 // the results are bitwise reproducible and an eager and a replayed line search take the same Armijo decisions.

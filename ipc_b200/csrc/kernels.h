@@ -1,4 +1,4 @@
-// kernels.h -- launcher declarations shared between the .cu translation units and the C-ABI (api.cu)
+// kernels.h -- launcher declarations shared between the .cu translation units and the C-ABI (api*.cu)
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -249,7 +249,7 @@ void dirichlet_update_lambda(const DirichletArgs& p, double* lam, cudaStream_t s
 void dirichlet_completed_step(const DirichletArgs& p, const double* dist2Tol, double* partials, double* out, cudaStream_t st); // 3 launches (dist2Tol: device)
 void set_double(double* p, double v, cudaStream_t st); // a device double in stream order
 
-// zero n_words 4-byte words.  A kernel rather than cudaMemsetAsync where the two chains of an iteration overlap (api.cu): replayed from a
+// zero n_words 4-byte words.  A kernel rather than cudaMemsetAsync where the two chains of an iteration overlap (abi.h: enter): replayed from a
 // graph, a memset node has no priority of its own and queues behind whatever low-priority grids are pending, which held the step-bound
 // chain up for the length of the CSR assembly
 void zero_words(void* p, size_t n_words, cudaStream_t st);

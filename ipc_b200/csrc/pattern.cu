@@ -18,8 +18,7 @@
 //      next comparison; k_slot_offsets (elastic.cu) recomputes the CSR offsets of the elastic block slots.
 // Every launch has a size fixed by nV and the capacities and reads its counts and gates from device memory, so an update is capturable.
 #include "common.cuh"
-#include "context.h"
-#include "../../include/ipcgpu.h"
+#include "abi.h"
 #include <algorithm>
 #include <cstddef>
 #include <cub/cub.cuh>
@@ -191,15 +190,6 @@ void zero_csr_rows(const int* ia, int base, int row0, int row1, double* a, cudaS
 
 using namespace ipcgpu;
 
-#define CKP(call)                                                          \
-    do {                                                                   \
-        cudaError_t e_ = (call);                                           \
-        if (e_ != cudaSuccess) {                                           \
-            ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
-            return IPCGPU_ERR_CUDA;                                        \
-        }                                                                  \
-    } while (0)
-
 // Mesh part + buffers + the mesh-only pattern in ia / ja (host, once per enable).  The caller refreshes the host mirrors.
 int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity)
 {
@@ -219,8 +209,8 @@ int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity)
             for (int j = i + 1; j < 4; ++j) add(T[(size_t)i * nT + t], T[(size_t)j * nT + t]);
     if (ctx->surface_ready && ctx->nSE > 0) {
         std::vector<int> se((size_t)2 * ctx->nSE);
-        CKP(cudaMemcpyAsync(se.data(), ctx->SE.p, se.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        CKP(cudaStreamSynchronize(ctx->stream));
+        CK(cudaMemcpyAsync(se.data(), ctx->SE.p, se.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
         for (int e = 0; e < ctx->nSE; ++e) add(se[2 * (size_t)e], se[2 * (size_t)e + 1]);
     }
     std::sort(keys.begin(), keys.end());
@@ -268,14 +258,14 @@ int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity)
         ctx->err = "ipcgpu_enable_device_pattern: allocation or upload failed";
         return IPCGPU_ERR_CUDA;
     }
-    CKP(cudaMemcpyAsync(ctx->ja.p, ja.data(), ja.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-    CKP(cudaMemsetAsync(ctx->a.p, 0, (size_t)cap * sizeof(double), ctx->stream));
-    for (int* p : { w.row_cnt.p, w.ucnt.p, w.prev_ptr.p }) CKP(cudaMemsetAsync(p, 0, n1 * sizeof(int), ctx->stream)); // no extra blocks yet
+    CK(cudaMemcpyAsync(ctx->ja.p, ja.data(), ja.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(ctx->a.p, 0, (size_t)cap * sizeof(double), ctx->stream));
+    for (int* p : { w.row_cnt.p, w.ucnt.p, w.prev_ptr.p }) CK(cudaMemsetAsync(p, 0, n1 * sizeof(int), ctx->stream)); // no extra blocks yet
     {   // result of the "last update": the mesh pattern, unchanged, version 0
         struct { long long nnz; unsigned long long version; int changed, ok, diff, pad; } r = { mesh_nnz, 0ull, 0, 1, 0, 0 };
         static_assert(sizeof(r) == sizeof(IterState) - offsetof(IterState, pat_nnz), "IterState pattern words");
-        CKP(cudaMemcpyAsync(reinterpret_cast<char*>(ctx->iter.p) + offsetof(IterState, pat_nnz), &r, sizeof(r), cudaMemcpyHostToDevice, ctx->stream));
-        CKP(cudaStreamSynchronize(ctx->stream)); // (host vectors and r go out of scope)
+        CK(cudaMemcpyAsync(reinterpret_cast<char*>(ctx->iter.p) + offsetof(IterState, pat_nnz), &r, sizeof(r), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream)); // (host vectors and r go out of scope)
     }
     w.scan_bytes = scan_bytes;
     w.mesh_pairs = nPairs;
@@ -307,17 +297,17 @@ int pattern_update(ipcgpu_ctx* ctx, const BarrierArgs& lists, bool with_friction
     const int gv = (nV + 255) / 256;
     size_t bytes = w.scan_bytes;
     k_pattern_keys<false><<<kSMs * 4, 256, 0, st>>>(p, w.row_cnt.p, w.row_off.p, w.bucket.p, it);
-    CKP(cub::DeviceScan::ExclusiveSum(w.scan_tmp.p, bytes, w.row_cnt.p, w.row_off.p, nV + 1, st));
+    CK(cub::DeviceScan::ExclusiveSum(w.scan_tmp.p, bytes, w.row_cnt.p, w.row_off.p, nV + 1, st));
     k_pattern_check<<<1, 1, 0, st>>>(w.row_off.p + nV, w.key_cap, it);
     k_pattern_keys<true><<<kSMs * 4, 256, 0, st>>>(p, w.row_cnt.p, w.row_off.p, w.bucket.p, it);
     k_pattern_rows<<<gv, 256, 0, st>>>(nV, w.row_off.p, w.bucket.p, w.ucnt.p, w.prev_ptr.p, w.prev_nbr.p, it);
     bytes = w.scan_bytes;
-    CKP(cub::DeviceScan::ExclusiveSum(w.scan_tmp.p, bytes, w.ucnt.p, w.uoff.p, nV + 1, st));
+    CK(cub::DeviceScan::ExclusiveSum(w.scan_tmp.p, bytes, w.ucnt.p, w.uoff.p, nV + 1, st));
     k_pattern_commit<<<1, 1, 0, st>>>(nV, w.mptr.p + nV, w.uoff.p + nV, w.nnz_cap, it);
     k_pattern_write<<<gv, 256, 0, st>>>(nV, ctx->index_base, w.mptr.p, w.mnbr.p, w.row_off.p, w.bucket.p, w.ucnt.p, w.uoff.p, ctx->ia.p, ctx->ja.p, w.prev_ptr.p,
         w.prev_nbr.p, it);
     slot_offsets(ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->ia.p, ctx->ja.p, ctx->index_base, ctx->slot_off.p, ctx->flag.p, st, &it->pat_changed);
     ctx->launches += 9;
-    CKP(cudaGetLastError());
+    CK(cudaGetLastError());
     return IPCGPU_OK;
 }

@@ -11,8 +11,7 @@
 // (a handful per million tests) go through an exact evaluation with floating-point expansions held in thread-local memory
 // (two-sum, two-product via the explicit fma intrinsic, grow-expansion, scale-expansion -- Shewchuk 1997, figs. 6, 7, 13).
 #include "broadphase.cuh"
-#include "context.h"
-#include "../../include/ipcgpu.h"
+#include "abi.h"
 
 namespace ipcgpu {
 
@@ -253,12 +252,6 @@ __global__ void __launch_bounds__(256) k_count_inverted(ElasticArgs p, int* __re
 } // namespace ipcgpu
 
 using namespace ipcgpu;
-
-SurfArgs surf_args(const ipcgpu_ctx* ctx); // constraint.cu
-SortedGrid edge_grid(const ipcgpu_ctx* ctx);
-int boxes_and_grid(ipcgpu_ctx* ctx, double radius, bool with_vertex_boxes); // constraint.cu
-
-static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
 
 // enqueue the inversion count of this rank's tets into IterState::checks[0]
 int safeguard_inversion(ipcgpu_ctx* ctx)

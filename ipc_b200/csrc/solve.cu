@@ -12,8 +12,7 @@
 // (col index + position of the value inside the upper-triangular array for every entry of both triangles), so the product is a plain
 // deterministic row-parallel CSR SpMV that gathers a[] through that position map -- no atomics, no transposed pass.
 #include "common.cuh"
-#include "context.h"
-#include "../../include/ipcgpu.h"
+#include "abi.h"
 #include <algorithm>
 #include <cmath>
 #include <vector>
@@ -153,17 +152,6 @@ __global__ void __launch_bounds__(256) k_psize(int nSV, const int* __restrict__ 
 
 using namespace ipcgpu;
 
-#define CKS(call)                                                      \
-    do {                                                               \
-        cudaError_t e_ = (call);                                       \
-        if (e_ != cudaSuccess) {                                       \
-            ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
-            return IPCGPU_ERR_CUDA;                                    \
-        }                                                              \
-    } while (0)
-
-static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
-
 // full row structure of the symmetric matrix from its upper-triangular CSR (host, once per pattern)
 int solver_build_full_pattern(ipcgpu_ctx* ctx, const int* ia, const int* ja)
 {
@@ -193,7 +181,7 @@ int solver_build_full_pattern(ipcgpu_ctx* ctx, const int* ia, const int* ja)
         ctx->err = "upload of the full-row pattern failed";
         return IPCGPU_ERR_CUDA;
     }
-    CKS(cudaStreamSynchronize(ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     ctx->full_pattern_ready = true;
     return 0;
 }
@@ -209,13 +197,13 @@ int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_t
         ctx->err = "PCG workspace allocation failed";
         return IPCGPU_ERR_CUDA;
     }
-    CKS(cudaMemsetAsync(ctx->pcg_scal.p, 0, 8 * sizeof(double), st));
+    CK(cudaMemsetAsync(ctx->pcg_scal.p, 0, 8 * sizeof(double), st));
     k_block_jacobi<<<nblk(nV, 256), 256, 0, st>>>(nV, ctx->ia.p, ctx->index_base, ctx->a.p, ctx->pcg_minv.p);
     k_pcg_init<<<nblk(nV, 256), 256, 0, st>>>(nV, rhs_dev, sign, ctx->pcg_minv.p, ctx->sol.p, ctx->pcg_r.p, ctx->pcg_p.p, ctx->pcg_scal.p);
     ctx->launches += 2;
-    double* h = ctx->h_scalar;
-    CKS(cudaMemcpyAsync(h, ctx->pcg_scal.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CKS(cudaStreamSynchronize(st));
+    double* h = ctx->staging->pcg;
+    CK(cudaMemcpyAsync(h, ctx->pcg_scal.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     const double bb = h[4];
     int it = 0;
     double rr = bb;
@@ -230,14 +218,14 @@ int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_t
                 k_pcg_roll<<<1, 32, 0, st>>>(ctx->pcg_scal.p, ctx->pcg_hist.p, it);
                 ctx->launches += 4;
             }
-            CKS(cudaMemcpyAsync(h, ctx->pcg_hist.p + (it - 1), sizeof(double), cudaMemcpyDeviceToHost, st));
-            CKS(cudaStreamSynchronize(st));
+            CK(cudaMemcpyAsync(h, ctx->pcg_hist.p + (it - 1), sizeof(double), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
             rr = h[0];
             if (!(rr == rr)) break; // NaN: the matrix was not positive definite
             if (std::sqrt(rr) <= rel_tol * std::sqrt(bb)) break;
         }
     }
-    CKS(cudaGetLastError());
+    CK(cudaGetLastError());
     if (iters_out) *iters_out = it;
     if (rel_res_out) *rel_res_out = bb > 0.0 ? std::sqrt(rr / bb) : 0.0;
     return 0;
@@ -247,7 +235,7 @@ int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_t
 int solver_adopt_direction(ipcgpu_ctx* ctx)
 {
     cudaStream_t st = ctx->stream;
-    CKS(cudaMemcpyAsync(ctx->dir.p, ctx->sol.p, (size_t)ctx->n_rows * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(ctx->dir.p, ctx->sol.p, (size_t)ctx->n_rows * sizeof(double), cudaMemcpyDeviceToDevice, st));
     double pSize = 0.0;
     if (ctx->nSV > 0) {
         const int nb = 64;
@@ -255,8 +243,8 @@ int solver_adopt_direction(ipcgpu_ctx* ctx)
         k_psize<<<nb, 256, 0, st>>>(ctx->nSV, ctx->SVI.p, ctx->nVdof, ctx->dir.p, ctx->partials.p);
         ++ctx->launches;
         std::vector<double> hp(nb);
-        CKS(cudaMemcpyAsync(hp.data(), ctx->partials.p, nb * sizeof(double), cudaMemcpyDeviceToHost, st));
-        CKS(cudaStreamSynchronize(st));
+        CK(cudaMemcpyAsync(hp.data(), ctx->partials.p, nb * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
         for (double v : hp) pSize += v;
         long long nMeshSV = 0;
         for (int v : ctx->h_SVI) nMeshSV += v < ctx->nVdof ? 1 : 0;
@@ -264,8 +252,8 @@ int solver_adopt_direction(ipcgpu_ctx* ctx)
     }
     ctx->pSize = pSize;
     if (!ctx->pSize_dev.reserve(1)) return IPCGPU_ERR_CUDA;
-    CKS(cudaMemcpyAsync(ctx->pSize_dev.p, &ctx->pSize, sizeof(double), cudaMemcpyHostToDevice, st));
-    CKS(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(ctx->pSize_dev.p, &ctx->pSize, sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));
     ctx->pSize_surface = ctx->surface_ready;
     ctx->dir_valid = true;
     return 0;

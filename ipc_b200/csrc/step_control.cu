@@ -5,7 +5,7 @@
 //
 // Every decision is one single-thread kernel that reads IterState (energies, safeguard counts, flags), computes the next step in place
 // (IterState::step_ord) and writes the decision word IterState::ls_cond.  Outside a capture the host reads that word; inside one the kernel
-// also hands it to the conditional graph node that runs the loop body (cudaGraphSetConditional).  api.cu holds the two drivers.
+// also hands it to the conditional graph node that runs the loop body (cudaGraphSetConditional).  api_step.cu holds the two drivers.
 #include "common.cuh"
 #include "kernels.h"
 #include "../../include/ipcgpu.h"

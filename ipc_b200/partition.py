@@ -1,4 +1,4 @@
-"""Host-side mirror of the multi-rank partition rule that libipcgpu.so applies (csrc/api.cu: build_maps), for callers that need to know
+"""Host-side mirror of the multi-rank partition rule that libipcgpu.so applies (csrc/api_mesh.cu: build_maps), for callers that need to know
 who owns what (which CSR rows to fetch from which rank) and for the CPU-side tests of the rule.
 
   tets      : block partition [nT*r/N, nT*(r+1)/N)            -- energy, inversion filter: every tet exactly once

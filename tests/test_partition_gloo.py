@@ -21,7 +21,7 @@ def _worker(rank, world, port, q):
     m = M.Mesh(V, T, energy=0)
     M.deform(m, 3)
     ia, ja = m.csr_pattern(1)
-    tb, te = m.nT * rank // world, m.nT * (rank + 1) // world  # the context's partition rule (api.cu)
+    tb, te = m.nT * rank // world, m.nT * (rank + 1) // world  # the context's partition rule (api_mesh.cu)
     sub = M.Mesh.__new__(M.Mesh)
     sub.__dict__.update(m.__dict__)
     sub.T, sub.nT = m.T[tb:te], te - tb
@@ -53,7 +53,7 @@ def test_tet_partition_allreduce_gloo():
 
 
 def _contact_worker(rank, world, port, q):
-    """Contact stage under the context's partition rules (api.cu / constraint.cu / ccd.cu): every rank keeps a contiguous share of the
+    """Contact stage under the context's partition rules (api_contact.cu / constraint.cu / ccd.cu): every rank keeps a contiguous share of the
     pair lists and of the CCD candidates; SUM of the barrier energy / gradient / CSR values and MIN of the step reproduce one rank."""
     sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
     import oracle as orc
@@ -102,7 +102,7 @@ def test_contact_partition_allreduce_gloo():
 
 
 def _row_owner_worker(rank, world, port, q):
-    """The row-owner rule (ipc_b200/partition.py = csrc/api.cu build_maps): every rank assembles the tets that touch its vertex range and
+    """The row-owner rule (ipc_b200/partition.py = csrc/api_mesh.cu build_maps): every rank assembles the tets that touch its vertex range and
     keeps only the CSR rows (and gradient rows) it owns; the kept pieces are DISJOINT and their union is the single-process result -- no
     reduction of the Hessian, only a gather."""
     sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
