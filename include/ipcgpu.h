@@ -65,7 +65,12 @@ enum {
     /* ipcgpu_device_ptr only (int arrays): the CSR row starts (n_rows + 1) and column indices (nnz) in the context's index base -- with
      * the device-built pattern they change when ipcgpu_pattern_info reports `changed` (a device solver re-points its matrix then) */
     IPCGPU_BUF_CSR_ROW_STARTS = 6,
-    IPCGPU_BUF_CSR_COLUMNS = 7
+    IPCGPU_BUF_CSR_COLUMNS = 7,
+    /* the state a time step leaves on the device (ipcgpu_end_time_step / ipcgpu_warm_start / the line search), for the frame a binding writes
+     * out: positions result.V (SoA, 3*nV), the search direction (interleaved, 3*nV; the warm start's predictor), xTilta (SoA, 3*nV) */
+    IPCGPU_BUF_POSITIONS = 8,
+    IPCGPU_BUF_SEARCH_DIR = 9,
+    IPCGPU_BUF_XTILDE = 10
 };
 
 /* ---- lifetime ---------------------------------------------------------------------------------- */
@@ -278,6 +283,31 @@ int ipcgpu_set_xtilde(ipcgpu_ctx* ctx, const double* xtilde_soa);
 int ipcgpu_inertia_energy(ipcgpu_ctx* ctx, double* E);
 /* g_v += m_v (x_v - xtilde_v) for every vertex that is not a projected Dirichlet vertex; g_inout NULL = the device-resident gradient */
 int ipcgpu_inertia_gradient(ipcgpu_ctx* ctx, int projectDBC, double* g_inout);
+
+/* ---- time integration: the frame of a time step around its Newton iterations (DESIGN.md section 3.14, INTEGRATION.md section 10) -------------
+ * Per-vertex kernels over every vertex, obstacle tail included; "Dirichlet" is Mesh::isDBCVertex (dbc_type != 0).  Every expression keeps the
+ * reference's evaluation order and rounding (no fused multiply-add).  No communication: every rank holds all vertices, so the calls work at any
+ * rank count, except the warm start (single rank). */
+/* Optimizer::setTime (Optimizer.cpp:421-428) and Config's time-integration tokens: type 0 = TIT_BE, 1 = TIT_NM (beta, gamma: Config.hpp:96).
+ * Held in device memory: a replayed graph uses the current values, so changing dt needs no new capture. */
+int ipcgpu_set_time_integration(ipcgpu_ctx* ctx, int type, double dt, double beta, double gamma, const double gravity[3]);
+/* Optimizer's dynamic state (:175-177, restart :203-230): velocity 3nV interleaved, acceleration and dx_Elastic nV x 3 SoA; NULL = zero */
+int ipcgpu_set_dynamics(ipcgpu_ctx* ctx, const double* velocity, const double* acceleration_soa, const double* dx_elastic_soa);
+int ipcgpu_get_dynamics(ipcgpu_ctx* ctx, double* velocity, double* acceleration_soa, double* dx_elastic_soa); /* any NULL skipped; synchronises */
+/* computeXTilta (:1236-1278) from V_prev (ipcgpu_set_prev_state) and the dynamic state, into the x~ the inertia term reads.  Capturable. */
+int ipcgpu_compute_xtilde(ipcgpu_ctx* ctx);
+/* end of a time step (:572-590): dx_Elastic, velocity, acceleration, V_prev = V, x~.  Capturable. */
+int ipcgpu_end_time_step(ipcgpu_ctx* ctx);
+/* initX(option) (:925-1233) for option 0-4: the predictor becomes the search direction (mean |p| of the swept build: the fixed-order device sum
+ * of a direction adopted on the device, as ipcgpu_solve_pcg's).  Option 0: p = 0, nothing moves, the step is 0.  Options >= 1: from step 1,
+ * the inversion filter (Neo-Hookean meshes), the planes' step with slackness 0.9, the swept hash with voxel_size (avgEdgeLen / 3) and the full
+ * Tight-Inclusion CCD; V0 := V into the saved state, V = V0 + alpha p; while a tet is inverted (Neo-Hookean), alpha /= 2; while not
+ * intersection-free (isIntersected, :2627-2659), alpha /= 2.  A bound of 0 is not an error (the reference only logs it, :1186-1188); an entry
+ * state that fails a check at step 0 gives IPCGPU_ERR_LINE_SEARCH with V = V0.  Results: the stage steps in ipcgpu_iteration (alpha_inversion,
+ * alpha_halfspace, alpha_swept_grid, alpha_full_ccd), the accepted step as the device-resident step, the halvings and the status in
+ * ipcgpu_step_control (alpha_feasible = alpha = the accepted step).  alpha_out NULL: deferred and capturable (conditional nodes; run it once
+ * outside a capture first); otherwise synchronises and returns the accepted step.  Option 5 or out of range: IPCGPU_ERR_ARG.  Single rank. */
+int ipcgpu_warm_start(ipcgpu_ctx* ctx, int option, double voxel_size, double tolerance, const double err_vf[3], const double err_ee[3], double* alpha_out);
 
 /* ---- Rayleigh damping, Neumann forces and the augmented-Lagrangian Dirichlet penalty: the last terms of Optimizer::computeEnergyVal /
  * computeGradient / computePrecondMtr (DESIGN.md section 3.13, INTEGRATION.md section 9) ------------------------------------------------

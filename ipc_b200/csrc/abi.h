@@ -65,6 +65,9 @@ static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
 //     by kSerial calls: ipcgpu_damping_update, ipcgpu_set_neumann_forces, ipcgpu_set_dirichlet_targets / _penalty / _update_lambda) and
 //     write g / a only; their energies and ipcgpu_dirichlet_completed_step (IterState::energy[kEnergyDamping / kEnergyNeumann /
 //     kEnergyDirichlet], dbc_step, damp_partials, nbc_partials, dbc_partials) are kSerial.  The step-bound chain touches none of them.
+//   - time integration (timestep.cu): ipcgpu_compute_xtilde, ipcgpu_end_time_step and ipcgpu_warm_start write xtilde, Vprev, V, dir and the
+//     dynamic state (vel, acc, dxe), which the derivative chain reads (inertia, damping, friction) or the step-bound chain does (dir): all
+//     three are kSerial.
 //   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, e_partials2, bHraw, brows, bpsd:
 //     derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };
@@ -124,6 +127,9 @@ void owned_value_range(ipcgpu_ctx* ctx);
 int ensure_offsets(ipcgpu_ctx* ctx);
 int upload_dir(ipcgpu_ctx* ctx, const double* p);
 
+// ---- api_terms.cu: checks the time-integration state, sizes the dynamic state and x~, fills the kernels' arguments ----------------------
+int timestep_prepare(ipcgpu_ctx* ctx, ipcgpu::DynamicsArgs* p);
+
 // ---- constraint.cu ----------------------------------------------------------------------------------------------------------
 namespace ipcgpu {
 struct SortedGrid; // broadphase.cuh
@@ -148,7 +154,7 @@ int ccd_read_back(ipcgpu_ctx* ctx, double* alpha_out);
 // ---- solve.cu, pattern.cu, safeguard.cu -------------------------------------------------------------------------------------
 int solver_build_full_pattern(ipcgpu_ctx* ctx, const int* ia, const int* ja);
 int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int* iters_out, double* rel_res_out);
-int solver_adopt_direction(ipcgpu_ctx* ctx);
+int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src); // src NULL: the direction already in ctx->dir
 int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity);
 int pattern_update(ipcgpu_ctx* ctx, const ipcgpu::BarrierArgs& lists, bool with_friction);
 int safeguard_inversion(ipcgpu_ctx* ctx);

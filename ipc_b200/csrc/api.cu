@@ -424,6 +424,9 @@ static int buf_info(ipcgpu_ctx* ctx, int which, double** p, uint64_t* n)
     case IPCGPU_BUF_TET_HESSIANS: *p = ctx->hblk.p; *n = 78 * 64 * ((nL + 63) / 64); return ctx->hblk_valid ? 0 : 2; /* tile-major, see elastic.cu */
     case IPCGPU_BUF_TET_GRADIENTS: *p = ctx->gcont.p; *n = 12 * nL; return 0;
     case IPCGPU_BUF_INVERSION_STEPS: *p = ctx->inv_steps.p; *n = (uint64_t)ctx->nT; return 0;
+    case IPCGPU_BUF_POSITIONS: *p = ctx->V.p; *n = (uint64_t)3 * ctx->nV; return 0;
+    case IPCGPU_BUF_SEARCH_DIR: *p = ctx->dir.p; *n = ctx->dir_valid ? (uint64_t)3 * ctx->nV : 0; return 0;
+    case IPCGPU_BUF_XTILDE: *p = ctx->xtilde.p; *n = ctx->xtilde_set ? (uint64_t)3 * ctx->nV : 0; return 0;
     default: return 1;
     }
 }

@@ -488,7 +488,7 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
     }
     int rc = solver_pcg(ctx, rhs_dev, sign, rel_tol, max_iter, iters, rel_residual);
     if (rc) return rc;
-    if (adopt_as_search_dir && (rc = solver_adopt_direction(ctx))) return rc;
+    if (adopt_as_search_dir && (rc = solver_adopt_direction(ctx, ctx->sol.p))) return rc;
     if (x) {
         CK(cudaMemcpyAsync(x, ctx->sol.p, (size_t)ctx->n_rows * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));

@@ -478,6 +478,52 @@ int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* t, doubl
     return alpha_inout ? step_control_host_result(ctx, alpha_inout) : IPCGPU_OK;
 }
 
+// Optimizer::initX (:925-1233) for options 0-4 with the barrier solver (solveIP): the predictor becomes the search direction, its step is
+// bounded (inversion filter, planes with slackness 0.9, swept hash + full CCD: initX always takes the full CCD, :1132) and applied with the
+// two backtracking loops of the line search (kLsInversion, kLsIntersection).  Nothing here synchronises outside the host loops of cond_node.
+int ipcgpu_warm_start(ipcgpu_ctx* ctx, int option, double voxel_size, double tol, const double err_vf[3], const double err_ee[3], double* alpha_out)
+{
+    REQUIRE(option >= 0 && option <= 4, IPCGPU_ERR_ARG, "warm start option 0-4 (initX option 5, Jacobi, is not supported)");
+    REQUIRE(option == 0 || (err_vf && err_ee && voxel_size > 0.0), IPCGPU_ERR_ARG, "the warm start needs the Tight-Inclusion errors and a positive voxel size");
+    REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the warm start runs on one rank");
+    REQUIRE(ctx->surface_ready && ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh and ipcgpu_set_surface first");
+    ENTER(kSerial);
+    DynamicsArgs dyn;
+    int rc = timestep_prepare(ctx, &dyn);
+    if (rc) return rc;
+    timestep_predictor(dyn, option, ctx->dir.p, ctx->stream);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    if ((rc = solver_adopt_direction(ctx, nullptr)) || (rc = step_control_prepare(ctx))) return rc;
+    if ((rc = decide(ctx, kWsEntry, option ? 1.0 : 0.0, 0, 0, nullptr))) return rc; // stepSize = 1.0 (:1123)
+    if (option) {
+        if (ctx->energy == IPCGPU_NEOHOOKEAN && (rc = ipcgpu_inversion_step(ctx, nullptr, 0.2, nullptr))) return rc; // filterStepSize (:1124)
+        if ((rc = ipcgpu_halfspace_step(ctx, nullptr, 0.9, nullptr))) return rc; // slackness_a (:1123, :1130-1131)
+        if (ctx->n_hs > 0) CK(cudaMemsetAsync(&ctx->iter.p->hs_zero_step, 0, sizeof(int), ctx->stream)); // a zero bound is no error here
+        if ((rc = ipcgpu_hash_build_swept(ctx, nullptr, nullptr, voxel_size))) return rc; // :1135
+        if ((rc = ipcgpu_ccd_full_ti(ctx, tol, err_vf, err_ee, nullptr, nullptr))) return rc;
+        CK(cudaMemcpyAsync(ctx->Vsaved.p, ctx->V.p, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream)); // V0 (:1191)
+        ctx->state_saved = true;
+        rc = ls_step(ctx); // :1192
+        if (!rc && ctx->energy == IPCGPU_NEOHOOKEAN) { // getNeedElemInvSafeGuard() (:1194-1200)
+            rc = ipcgpu_check_inversion(ctx, nullptr);
+            if (!rc) rc = cond_node(ctx, true, kLsInversion, 0.0, 0, [&]() {
+                int r = ls_step(ctx);
+                return r ? r : ipcgpu_check_inversion(ctx, nullptr);
+            });
+        }
+        const int terms = ctx->n_hs > 0 ? kTermHalfSpace : 0;
+        if (!rc) rc = ls_intersection(ctx); // isIntersected (:1203-1210)
+        if (!rc) rc = cond_node(ctx, true, kLsIntersection, 0.0, terms, [&]() {
+            int r = ls_step(ctx);
+            return r ? r : ls_intersection(ctx);
+        });
+        if (rc) return rc;
+    }
+    ctx->sc_pending = true;
+    return alpha_out ? step_control_host_result(ctx, alpha_out) : IPCGPU_OK;
+}
+
 int ipcgpu_step_control_info(ipcgpu_ctx* ctx, ipcgpu_step_control* out)
 {
     REQUIRE(out != nullptr, IPCGPU_ERR_ARG, "null output");

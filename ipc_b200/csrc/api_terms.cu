@@ -8,6 +8,37 @@
 
 using namespace ipcgpu;
 
+// the dynamic state for the current mesh, zero when it was never set for a mesh of this size
+static int dynamics_alloc(ipcgpu_ctx* ctx)
+{
+    if (ctx->dyn_nV == ctx->nV) return IPCGPU_OK;
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "set the dynamic state (ipcgpu_set_dynamics) outside a capture first");
+    const size_t n = (size_t)3 * ctx->nV;
+    ALLOC(ctx->vel, n);
+    ALLOC(ctx->acc, n);
+    ALLOC(ctx->dxe, n);
+    for (double* b : { ctx->vel.p, ctx->acc.p, ctx->dxe.p }) CK(cudaMemsetAsync(b, 0, n * sizeof(double), ctx->stream));
+    ctx->dyn_nV = ctx->nV;
+    return IPCGPU_OK;
+}
+
+// the state every per-vertex time-integration call needs: the parameters, V_prev of this mesh, and the dynamic state
+int timestep_prepare(ipcgpu_ctx* ctx, DynamicsArgs* p)
+{
+    REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    REQUIRE(ctx->time_set, IPCGPU_ERR_STATE, "ipcgpu_set_time_integration first");
+    REQUIRE(ctx->prev_set && ctx->Vprev.n >= (size_t)3 * ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_prev_state first");
+    int rc = dynamics_alloc(ctx);
+    if (rc) return rc;
+    ALLOC(ctx->xtilde, (size_t)3 * ctx->nV);
+    p->nV = ctx->nV;
+    p->tp = ctx->tparams.p;
+    p->dbc = ctx->has_dbc ? ctx->dbc.p : nullptr;
+    p->vel = ctx->vel.p; p->acc = ctx->acc.p; p->dxe = ctx->dxe.p;
+    p->V = ctx->V.p; p->Vprev = ctx->Vprev.p; p->xtilde = ctx->xtilde.p;
+    return IPCGPU_OK;
+}
+
 extern "C" {
 
 // ---- inertia term (Optimizer.cpp:3227-3239, :3439-3450) ---------------------------------------------------------------------
@@ -19,6 +50,88 @@ int ipcgpu_set_xtilde(ipcgpu_ctx* ctx, const double* xtilde_soa)
     ALLOC(ctx->xtilde, (size_t)3 * ctx->nV);
     CK(cudaMemcpyAsync(ctx->xtilde.p, xtilde_soa, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     ctx->xtilde_set = true;
+    return IPCGPU_OK;
+}
+
+// ---- time integration (timestep.cu): Optimizer::setTime (:421-428), computeXTilta (:1236-1278), the end of a time step (:572-590) -------------
+int ipcgpu_set_time_integration(ipcgpu_ctx* ctx, int type, double dt, double beta, double gamma, const double gravity[3])
+{
+    REQUIRE(type == 0 || type == 1, IPCGPU_ERR_ARG, "time integration type: 0 (TIT_BE) or 1 (TIT_NM)");
+    REQUIRE(gravity != nullptr, IPCGPU_ERR_ARG, "null gravity");
+    REQUIRE(dt > 0.0 && (type == 0 || beta > 0.0), IPCGPU_ERR_ARG, "dt, and beta of a Newmark integration, must be positive");
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "set the time integration outside a capture (a replay reads the values held on the device)");
+    ENTER(kSerial);
+    TimeParams q = {};
+    q.type = type;
+    q.dt = dt;
+    q.dtSq = dt * dt;
+    q.beta = beta;
+    q.gamma = gamma;
+    for (int d = 0; d < 3; ++d) {
+        q.gravity[d] = gravity[d];
+        q.gDtSq[d] = q.dtSq * gravity[d];
+    }
+    ALLOC(ctx->tparams, 1);
+    CK(cudaMemcpyAsync(ctx->tparams.p, &q, sizeof q, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream)); // `q` lives on this stack
+    ctx->time_set = true;
+    return IPCGPU_OK;
+}
+
+int ipcgpu_set_dynamics(ipcgpu_ctx* ctx, const double* velocity, const double* acceleration_soa, const double* dx_elastic_soa)
+{
+    REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is in progress");
+    ENTER(kSerial);
+    ctx->dyn_nV = 0; // (re)sized and zeroed, then the given arrays
+    int rc = dynamics_alloc(ctx);
+    if (rc) return rc;
+    const size_t bytes = (size_t)3 * ctx->nV * sizeof(double);
+    if (velocity) CK(cudaMemcpyAsync(ctx->vel.p, velocity, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (acceleration_soa) CK(cudaMemcpyAsync(ctx->acc.p, acceleration_soa, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (dx_elastic_soa) CK(cudaMemcpyAsync(ctx->dxe.p, dx_elastic_soa, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream)); // (the arrays are the caller's: the upload completes here)
+    return IPCGPU_OK;
+}
+
+int ipcgpu_get_dynamics(ipcgpu_ctx* ctx, double* velocity, double* acceleration_soa, double* dx_elastic_soa)
+{
+    REQUIRE(ctx->nV > 0, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is in progress");
+    ENTER(kSerial);
+    int rc = dynamics_alloc(ctx);
+    if (rc) return rc;
+    const size_t bytes = (size_t)3 * ctx->nV * sizeof(double);
+    if (velocity) CK(cudaMemcpyAsync(velocity, ctx->vel.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (acceleration_soa) CK(cudaMemcpyAsync(acceleration_soa, ctx->acc.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (dx_elastic_soa) CK(cudaMemcpyAsync(dx_elastic_soa, ctx->dxe.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IPCGPU_OK;
+}
+
+int ipcgpu_compute_xtilde(ipcgpu_ctx* ctx)
+{
+    ENTER(kSerial);
+    DynamicsArgs p;
+    int rc = timestep_prepare(ctx, &p);
+    if (rc) return rc;
+    timestep_xtilde(p, ctx->stream);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    ctx->xtilde_set = true;
+    return IPCGPU_OK;
+}
+
+int ipcgpu_end_time_step(ipcgpu_ctx* ctx)
+{
+    REQUIRE(ctx->xtilde_set, IPCGPU_ERR_STATE, "no xTilta for the step that ends: ipcgpu_compute_xtilde (or ipcgpu_set_xtilde) first");
+    ENTER(kSerial);
+    DynamicsArgs p;
+    int rc = timestep_prepare(ctx, &p);
+    if (rc) return rc;
+    timestep_end(p, ctx->stream);
+    ++ctx->launches;
+    CK(cudaGetLastError());
     return IPCGPU_OK;
 }
 

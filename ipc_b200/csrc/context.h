@@ -217,6 +217,12 @@ struct ipcgpu_ctx {
     int n_dbc = 0;
     ipcgpu::DevBuf<double> damp_D, damp_partials, nbc_f, nbc_partials, dbc_tgt, dbc_lam, dbc_partials;
     ipcgpu::DevBuf<int> damp_inc_ptr, damp_inc, dbc_vid;
+    // time integration (timestep.cu): the parameters of ipcgpu_set_time_integration in device memory, and Optimizer's dynamic state --
+    // velocity (interleaved), acceleration and dx_Elastic (SoA) -- for dyn_nV vertices (zeroed at the first use on a mesh of another size)
+    ipcgpu::DevBuf<ipcgpu::TimeParams> tparams;
+    ipcgpu::DevBuf<double> vel, acc, dxe;
+    bool time_set = false;
+    int dyn_nV = 0;
     size_t ccd_capacity = (size_t)1 << 23; // candidate pairs
     std::vector<int> h_SVI;                // host copy (pSize of the swept build is a serial host sum, SpatialHash.hpp:603-612)
     double debug_prune_seed = -1.0;        // test hook, see ipcgpu_ccd_debug_seed_bound

@@ -57,7 +57,7 @@ struct IterState {
     int pat_pad_;
 };
 // step_decide operations (step_control.cu) and the energy terms of a line search
-enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersection, kLsArmijo, kLsPostCheck, kLsPostLoop, kLsRebuild };
+enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersection, kLsArmijo, kLsPostCheck, kLsPostLoop, kLsRebuild, kWsEntry };
 enum { kTermInertia = 1, kTermFriction = 2, kTermHalfSpace = 4, kTermHalfSpaceFriction = 8, kTermDamping = 16, kTermNeumann = 32, kTermDirichlet = 64 };
 enum { FLAG_NONPOSITIVE_DISTANCE = 0, FLAG_SET_CAPACITY = 1, FLAG_CCD_CAPACITY = 2, FLAG_ZERO_CCD_DISTANCE = 3, FLAG_PATTERN = 4, FLAG_TI_WARNINGS = 5, FLAG_EXCHANGE_CAPACITY = 6,
     FLAG_PATTERN_CAPACITY = 7 };
@@ -248,6 +248,29 @@ void dirichlet_hessian(const DirichletArgs& p, const int* ia, int base, double* 
 void dirichlet_update_lambda(const DirichletArgs& p, double* lam, cudaStream_t st);
 void dirichlet_completed_step(const DirichletArgs& p, const double* dist2Tol, double* partials, double* out, cudaStream_t st); // 3 launches (dist2Tol: device)
 void set_double(double* p, double v, cudaStream_t st); // a device double in stream order
+
+// timestep.cu -- time integration (Optimizer::setTime / computeXTilta / solve's end of step / initX).  TimeParams lives in device memory
+// (ipcgpu_set_time_integration): a replayed graph reads the current values.
+struct TimeParams {
+    double dt, dtSq, beta, gamma;      // dtSq = dt * dt (setTime, Optimizer.cpp:423)
+    double gravity[3], gDtSq[3];       // gravityDtSq = dtSq * gravity (:427)
+    int type;                          // 0 TIT_BE, 1 TIT_NM
+    int pad_;
+};
+struct DynamicsArgs {
+    int nV;
+    const TimeParams* tp;
+    const uint8_t* dbc;                // nullable: isDBCVertex = dbc != 0
+    double* vel;                       // velocity, interleaved 3 nV
+    double* acc;                       // acceleration, nV x 3 column-major (SoA)
+    double* dxe;                       // dx_Elastic, nV x 3 column-major (SoA)
+    const double* V;                   // SoA
+    double* Vprev;                     // result.V_prev, SoA
+    double* xtilde;                    // xTilta, SoA
+};
+void timestep_xtilde(const DynamicsArgs& p, cudaStream_t st);
+void timestep_end(const DynamicsArgs& p, cudaStream_t st);
+void timestep_predictor(const DynamicsArgs& p, int option, double* dir, cudaStream_t st); // option 0-4 into dir (interleaved)
 
 // zero n_words 4-byte words.  A kernel rather than cudaMemsetAsync where the two chains of an iteration overlap (abi.h: enter): replayed from a
 // graph, a memset node has no priority of its own and queues behind whatever low-priority grids are pending, which held the step-bound

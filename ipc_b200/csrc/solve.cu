@@ -147,6 +147,14 @@ __global__ void __launch_bounds__(256) k_psize(int nSV, const int* __restrict__ 
         partials[blockIdx.x] = t;
     }
 }
+// ... then the partials in block order, over the 3 nMeshSV components (0 without mesh surface vertices)
+__global__ void k_psize_mean(const double* __restrict__ partials, int n, long long n3, double* __restrict__ out)
+{
+    if (threadIdx.x != 0) return;
+    double s = 0.0;
+    for (int b = 0; b < n; ++b) s += partials[b];
+    *out = n3 > 0 ? s / (double)n3 : 0.0;
+}
 
 } // namespace ipcgpu
 
@@ -231,29 +239,20 @@ int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_t
     return 0;
 }
 
-// the device-resident solution becomes the search direction of the step-bound stages (pSize by a fixed-order device sum)
-int solver_adopt_direction(ipcgpu_ctx* ctx)
+// a direction produced on the device (src, or `dir` itself when src is NULL) becomes the search direction of the step-bound stages: pSize
+// by a fixed-order device sum into pSize_dev.  Nothing synchronises, so a captured sequence may adopt a direction (the warm start's predictor).
+int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src)
 {
     cudaStream_t st = ctx->stream;
-    CK(cudaMemcpyAsync(ctx->dir.p, ctx->sol.p, (size_t)ctx->n_rows * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    double pSize = 0.0;
-    if (ctx->nSV > 0) {
-        const int nb = 64;
-        if (!ctx->pcg_scal.reserve(8) || !ctx->partials.reserve(nb + 8)) return IPCGPU_ERR_CUDA;
-        k_psize<<<nb, 256, 0, st>>>(ctx->nSV, ctx->SVI.p, ctx->nVdof, ctx->dir.p, ctx->partials.p);
-        ++ctx->launches;
-        std::vector<double> hp(nb);
-        CK(cudaMemcpyAsync(hp.data(), ctx->partials.p, nb * sizeof(double), cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        for (double v : hp) pSize += v;
-        long long nMeshSV = 0;
-        for (int v : ctx->h_SVI) nMeshSV += v < ctx->nVdof ? 1 : 0;
-        pSize = nMeshSV > 0 ? pSize / (double)(nMeshSV * 3) : 0.0;
-    }
-    ctx->pSize = pSize;
-    if (!ctx->pSize_dev.reserve(1)) return IPCGPU_ERR_CUDA;
-    CK(cudaMemcpyAsync(ctx->pSize_dev.p, &ctx->pSize, sizeof(double), cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));
+    if (src) CK(cudaMemcpyAsync(ctx->dir.p, src, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    const int nb = ctx->nSV > 0 ? 64 : 0;
+    if (!ctx->partials.reserve(nb + 8) || !ctx->pSize_dev.reserve(1)) return IPCGPU_ERR_CUDA;
+    long long nMeshSV = 0;
+    for (int v : ctx->h_SVI) nMeshSV += v < ctx->nVdof ? 1 : 0;
+    if (nb) k_psize<<<nb, 256, 0, st>>>(ctx->nSV, ctx->SVI.p, ctx->nVdof, ctx->dir.p, ctx->partials.p);
+    k_psize_mean<<<1, 32, 0, st>>>(ctx->partials.p, nb, nMeshSV * 3, ctx->pSize_dev.p);
+    ctx->launches += nb ? 2 : 1;
+    CK(cudaGetLastError());
     ctx->pSize_surface = ctx->surface_ready;
     ctx->dir_valid = true;
     return 0;

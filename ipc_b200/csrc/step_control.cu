@@ -1,6 +1,6 @@
 // step_control.cu -- the data-dependent decisions of a Newton iteration on the device (sm_90a): the CFL branch of the step bound
 // (Optimizer.cpp:1947-2027, CFL_FOR_CCD == 2) and the loop conditions of Optimizer::lineSearch (Optimizer.cpp:2662-2916, armijoParam = 0,
-// lowerBound = 0).
+// lowerBound = 0), and the entry of a warm start (Optimizer::initX, Optimizer.cpp:1120-1215), whose two loops are the line search's first two.
 //   *** compiled with --fmad=false (NOFMA_FILES): |p| = sqrt((x*x + y*y) + z*z) rounds like the CPU oracle ***
 //
 // Every decision is one single-thread kernel that reads IterState (energies, safeguard counts, flags), computes the next step in place
@@ -135,6 +135,17 @@ __global__ void k_step_decide(IterState* st, int op, double a, int b, cudaGraphC
     case kLsRebuild: // :2808-2810
         cond = ok && st->ls_post_ran;
         st->ls_rebuilt = cond;
+        break;
+    case kWsEntry: // initX (:1123): a warm start begins at stepSize = a (1.0; 0.0 for option 0).  Its counters are per call, as a line
+                   // search's are, but a step bound of 0 is not an error here ("CCD gives 0 in initX()" is only logged, :1186-1188): the loops
+                   // then run at step 0 and only a failing entry state ends the call with IPCGPU_ERR_LINE_SEARCH (halve_while).
+        for (int k = 0; k < 4; ++k) st->ls_count[k] = 0;
+        st->ls_stopped = st->ls_rebuilt = st->ls_post_ran = 0;
+        st->sc_status = 0;
+        st->ls_E0 = st->ls_Et = 0.0;
+        st->step_ord = dbl_to_ord(a);
+        st->ls_LF = a;
+        st->alpha_stage[0] = a; // the step the inversion filter starts from (it lowers it on Neo-Hookean meshes; no filter otherwise)
         break;
     }
     st->ls_cond = cond;

@@ -16,6 +16,7 @@ ERR_NONPOSITIVE_DISTANCE, ERR_STATE, ERR_LINE_SEARCH = 4, 7, 8
 
 BUF_GRADIENT, BUF_CSR_VALUES, BUF_ENERGY_PER_TET, BUF_TET_HESSIANS, BUF_TET_GRADIENTS, BUF_INVERSION_STEPS = range(6)
 BUF_CSR_ROW_STARTS, BUF_CSR_COLUMNS = 6, 7  # ipcgpu_device_ptr only
+BUF_POSITIONS, BUF_SEARCH_DIR, BUF_XTILDE = 8, 9, 10
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
@@ -137,7 +138,14 @@ SIGNATURES = {
     "ipcgpu_dirichlet_hessian": (C.c_int, [_ctxp, C.c_int, _dp]),
     "ipcgpu_dirichlet_update_lambda": (C.c_int, [_ctxp]),
     "ipcgpu_dirichlet_completed_step": (C.c_int, [_ctxp, _dp]),
+    "ipcgpu_set_time_integration": (C.c_int, [_ctxp, C.c_int, C.c_double, C.c_double, C.c_double, _dp]),
+    "ipcgpu_set_dynamics": (C.c_int, [_ctxp, _dp, _dp, _dp]),
+    "ipcgpu_get_dynamics": (C.c_int, [_ctxp, _dp, _dp, _dp]),
+    "ipcgpu_compute_xtilde": (C.c_int, [_ctxp]),
+    "ipcgpu_end_time_step": (C.c_int, [_ctxp]),
+    "ipcgpu_warm_start": (C.c_int, [_ctxp, C.c_int, C.c_double, C.c_double, _dp, _dp, _dp]),
 }
+TIT_BE, TIT_NM = 0, 1
 
 STAGES = ["elastic_energy", "elastic_tet", "gather_gradient", "assemble_csr", "inversion", "hash", "constraint_set", "barrier",
           "ccd_broad", "ccd_narrow", "allreduce", "ccd_root_filter", "damping_bc"]
@@ -468,6 +476,39 @@ class Context:
     def inertia_gradient(self, projectDBC=1, g_inout=None):
         self._ck(self.lib.ipcgpu_inertia_gradient(self.h, projectDBC, _d(g_inout)))
         return g_inout
+
+    # ---- time integration (Optimizer::setTime / computeXTilta / end of a time step / initX) ------------------
+    def set_time_integration(self, type, dt, beta=0.25, gamma=0.5, gravity=(0.0, -9.81, 0.0)):
+        """type TIT_BE (0) or TIT_NM (1); the values live in device memory (a replayed graph reads the current ones)"""
+        g = f64(np.asarray(gravity, dtype=np.float64).reshape(3))
+        self._ck(self.lib.ipcgpu_set_time_integration(self.h, int(type), float(dt), float(beta), float(gamma), _d(g)))
+
+    def set_dynamics(self, velocity=None, acceleration_soa=None, dx_elastic_soa=None):
+        """velocity 3nV interleaved, acceleration and dx_Elastic nV x 3 SoA (3nV); None = zero"""
+        v, a, dx = (None if x is None else f64(np.asarray(x, dtype=np.float64).ravel()) for x in (velocity, acceleration_soa, dx_elastic_soa))
+        self._ck(self.lib.ipcgpu_set_dynamics(self.h, _d(v), _d(a), _d(dx)))
+
+    def get_dynamics(self):
+        """(velocity interleaved, acceleration SoA, dx_Elastic SoA), 3nV doubles each"""
+        v, a, dx = np.empty(3 * self.nV), np.empty(3 * self.nV), np.empty(3 * self.nV)
+        self._ck(self.lib.ipcgpu_get_dynamics(self.h, _d(v), _d(a), _d(dx)))
+        return v, a, dx
+
+    def compute_xtilde(self):
+        self._ck(self.lib.ipcgpu_compute_xtilde(self.h))
+
+    def end_time_step(self):
+        self._ck(self.lib.ipcgpu_end_time_step(self.h))
+
+    def warm_start(self, option, voxel_size, tol, err_vf, err_ee, want=True, check=True):
+        """initX(option): want=True returns (status, accepted step) after one synchronisation (check=True raises on an error instead);
+        want=False: deferred and capturable, returns the status of the enqueue"""
+        a = C.c_double()
+        evf, eee = (None if e is None else f64(e) for e in (err_vf, err_ee))
+        rc = self.lib.ipcgpu_warm_start(self.h, int(option), float(voxel_size), float(tol), _d(evf), _d(eee), C.byref(a) if want else None)
+        if check:
+            self._ck(rc)
+        return (rc, a.value) if want else rc
 
     # ---- half-space collision objects (HalfSpace<3>) -----------------------------------------------
     def set_halfspaces(self, origin, normal, velocitydt=None, friction=None):
