@@ -151,9 +151,11 @@ int ccd_build_swept(ipcgpu_ctx* ctx, double h);
 int ccd_full(ipcgpu_ctx* ctx, double tol, const double* err_vf, const double* err_ee);
 int ccd_read_back(ipcgpu_ctx* ctx, double* alpha_out);
 
-// ---- solve.cu, pattern.cu, safeguard.cu -------------------------------------------------------------------------------------
+// ---- solve.cu, multilevel.cu, pattern.cu, safeguard.cu ----------------------------------------------------------------------
 int solver_build_full_pattern(ipcgpu_ctx* ctx, const int* ia, const int* ja);
 int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int* iters_out, double* rel_res_out);
+int solver_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int* iters_out, double* rel_res_out);
+int solver_multilevel_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count);
 int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src); // src NULL: the direction already in ctx->dir
 int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity);
 int pattern_update(ipcgpu_ctx* ctx, const ipcgpu::BarrierArgs& lists, bool with_friction);

@@ -427,6 +427,7 @@ static int buf_info(ipcgpu_ctx* ctx, int which, double** p, uint64_t* n)
     case IPCGPU_BUF_POSITIONS: *p = ctx->V.p; *n = (uint64_t)3 * ctx->nV; return 0;
     case IPCGPU_BUF_SEARCH_DIR: *p = ctx->dir.p; *n = ctx->dir_valid ? (uint64_t)3 * ctx->nV : 0; return 0;
     case IPCGPU_BUF_XTILDE: *p = ctx->xtilde.p; *n = ctx->xtilde_set ? (uint64_t)3 * ctx->nV : 0; return 0;
+    case IPCGPU_BUF_MULTILEVEL_INVERSES: *p = ctx->ml.inv.p; *n = ctx->ml.built ? (uint64_t)ctx->ml.tiles * 96 * 96 : 0; return 0;
     default: return 1;
     }
 }

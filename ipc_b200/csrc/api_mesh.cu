@@ -460,7 +460,8 @@ int ipcgpu_inversion_step(ipcgpu_ctx* ctx, const double* p, double slack, double
 }
 
 // ---- device-resident linear solve hand-off (SURVEY 8(f) rank 1) ----------------------------------------------------------
-int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
+// (both built-in solvers: the preconditioner is the only difference)
+static int solve_pcg(ipcgpu_ctx* ctx, bool multilevel, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
 {
     REQUIRE(ctx->nnz > 0 && ctx->n_rows == 3 * ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
     REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the built-in solver runs on one rank (a distributed solver takes each rank's rows: ipcgpu_partition_info)");
@@ -486,7 +487,7 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
         rhs_dev = ctx->pcg_b.p;
         sign = 1.0;
     }
-    int rc = solver_pcg(ctx, rhs_dev, sign, rel_tol, max_iter, iters, rel_residual);
+    int rc = (multilevel ? solver_pcg_multilevel : solver_pcg)(ctx, rhs_dev, sign, rel_tol, max_iter, iters, rel_residual);
     if (rc) return rc;
     if (adopt_as_search_dir && (rc = solver_adopt_direction(ctx, ctx->sol.p))) return rc;
     if (x) {
@@ -494,6 +495,34 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
         CK(cudaStreamSynchronize(ctx->stream));
     }
     return IPCGPU_OK;
+}
+
+int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
+{
+    return solve_pcg(ctx, false, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
+}
+
+int ipcgpu_solve_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
+{
+    return solve_pcg(ctx, true, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
+}
+
+int ipcgpu_multilevel_info(ipcgpu_ctx* ctx, int* levels, int64_t* domains_per_level, uint64_t* bytes)
+{
+    const ipcgpu::MultilevelWork& w = ctx->ml;
+    REQUIRE(w.built, IPCGPU_ERR_STATE, "ipcgpu_solve_pcg_multilevel first (a call that failed leaves no hierarchy)");
+    if (levels) *levels = w.levels;
+    if (domains_per_level)
+        for (int l = 0; l < ipcgpu::kMultilevelMax; ++l) domains_per_level[l] = l < w.levels ? w.domains[l] : 0;
+    if (bytes) *bytes = (uint64_t)w.tiles * 96 * 96 * sizeof(double);
+    return IPCGPU_OK;
+}
+
+int ipcgpu_multilevel_debug_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count)
+{
+    REQUIRE(ctx->ml.built, IPCGPU_ERR_STATE, "ipcgpu_solve_pcg_multilevel first");
+    ENTER(kSerial);
+    return solver_multilevel_matrices(ctx, dst, count);
 }
 
 int ipcgpu_csr_set_zero(ipcgpu_ctx* ctx)

@@ -116,6 +116,21 @@ struct PatternWork {
     uint64_t requested_cap = 0;       // what the caller asked for (0 = default), kept to rebuild after a surface / obstacle change
 };
 
+// multilevel additive Schwarz preconditioner (multilevel.cu): the Morton order of the vertices, the stored inverses of the domain matrices
+// (96 x 96 doubles per domain, the levels one after the other) and the per-level restricted / coarse-solved vectors (96 per domain)
+constexpr int kMultilevelMax = 8; // levels: 32^8 vertices and more are out of reach of an int
+struct MultilevelWork {
+    DevBuf<double> box, inv, R, Y, part, chunk; // (part: per-CTA partials of the dot products; chunk: per-chunk shares of a level's assembly)
+    DevBuf<unsigned> code, code_sorted;
+    DevBuf<int> id, order, rank;
+    DevBuf<unsigned char> sort_tmp, fixed; // (fixed: 1 for a vertex without degrees of freedom -- Dirichlet or obstacle tail)
+    bool built = false;                   // the last solve built the whole hierarchy (every pivot positive)
+    int levels = 0;
+    long long domains[kMultilevelMax] = {};
+    size_t tile_off[kMultilevelMax] = {}, tiles = 0; // first domain of every level, domains in all
+    bool smem_opted = false;              // the inversion kernel's dynamic shared memory has been opted in
+};
+
 // pinned host memory of the scalars the entry points copy between host and device, one member per use.  Allocated once per context
 // (cudaMallocHost(sizeof(HostStaging))), freed by ipcgpu_destroy: every member keeps its own address for the context's lifetime, since a
 // captured graph or a copy nobody waits on may still hold it.
@@ -253,6 +268,7 @@ struct ipcgpu_ctx {
     ipcgpu::DevBuf<int> fia, fja, fpos;
     bool full_pattern_ready = false;
     ipcgpu::DevBuf<double> sol, pcg_b, pcg_r, pcg_p, pcg_q, pcg_minv, pcg_scal, pcg_hist;
+    ipcgpu::MultilevelWork ml;
 
     // work / result buffers
     ipcgpu::DevBuf<double> gcont, hblk, g, e_per_tet, partials, inv_steps, dir, in_partials, e_partials2;

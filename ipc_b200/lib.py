@@ -11,12 +11,13 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libipcgpu.so")
 
-ERR_NAMES = {0: "OK", 1: "CUDA", 2: "ARG", 3: "PATTERN", 4: "NONPOSITIVE_DISTANCE", 5: "CAPACITY", 6: "NCCL", 7: "STATE", 8: "LINE_SEARCH"}
-ERR_NONPOSITIVE_DISTANCE, ERR_STATE, ERR_LINE_SEARCH = 4, 7, 8
+ERR_NAMES = {0: "OK", 1: "CUDA", 2: "ARG", 3: "PATTERN", 4: "NONPOSITIVE_DISTANCE", 5: "CAPACITY", 6: "NCCL", 7: "STATE", 8: "LINE_SEARCH", 9: "SOLVE"}
+ERR_NONPOSITIVE_DISTANCE, ERR_STATE, ERR_LINE_SEARCH, ERR_SOLVE = 4, 7, 8, 9
 
 BUF_GRADIENT, BUF_CSR_VALUES, BUF_ENERGY_PER_TET, BUF_TET_HESSIANS, BUF_TET_GRADIENTS, BUF_INVERSION_STEPS = range(6)
 BUF_CSR_ROW_STARTS, BUF_CSR_COLUMNS = 6, 7  # ipcgpu_device_ptr only
 BUF_POSITIONS, BUF_SEARCH_DIR, BUF_XTILDE = 8, 9, 10
+BUF_MULTILEVEL_INVERSES = 11
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
@@ -101,6 +102,9 @@ SIGNATURES = {
     "ipcgpu_graph_kernel_priorities": (C.c_int, [_ctxp, C.c_int, _ip, _ip]),
     "ipcgpu_csr_set_zero": (C.c_int, [_ctxp]),
     "ipcgpu_solve_pcg": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
+    "ipcgpu_solve_pcg_multilevel": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
+    "ipcgpu_multilevel_info": (C.c_int, [_ctxp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]),
+    "ipcgpu_multilevel_debug_matrices": (C.c_int, [_ctxp, _dp, C.c_uint64]),
     "ipcgpu_allreduce_grad_hess": (C.c_int, [_ctxp, C.c_int, C.c_int]),
     "ipcgpu_download": (C.c_int, [_ctxp, C.c_int, _dp, C.c_uint64]),
     "ipcgpu_device_ptr": (C.c_void_p, [_ctxp, C.c_int]),
@@ -820,6 +824,27 @@ class Context:
         self._ck(self.lib.ipcgpu_solve_pcg(self.h, _d(f64(rhs)) if rhs is not None else None, rel_tol, int(max_iter), _d(x) if want_x else None, int(adopt),
                                            C.byref(it), C.byref(res)))
         return x, it.value, res.value
+
+    def solve_pcg_multilevel(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False):
+        """solve_pcg with the multilevel additive Schwarz preconditioner (rebuilt from the resident matrix and positions at every call)"""
+        x = np.empty(3 * self.nV) if want_x else None
+        it, res = C.c_int(), C.c_double()
+        self._ck(self.lib.ipcgpu_solve_pcg_multilevel(self.h, _d(f64(rhs)) if rhs is not None else None, rel_tol, int(max_iter), _d(x) if want_x else None,
+                                                      int(adopt), C.byref(it), C.byref(res)))
+        return x, it.value, res.value
+
+    def multilevel_info(self):
+        """(domains per level, bytes of the stored inverses) of the last multilevel solve"""
+        lv, dom, nb = C.c_int(), (C.c_int64 * 8)(), C.c_uint64()
+        self._ck(self.lib.ipcgpu_multilevel_info(self.h, C.byref(lv), dom, C.byref(nb)))
+        return list(dom[: lv.value]), nb.value
+
+    def multilevel_debug_matrices(self):
+        """test hook: the level matrices before inversion, one (domains, 96, 96) array per level; the stored inverses are lost"""
+        domains, _ = self.multilevel_info()
+        out = np.empty(9216 * sum(domains))
+        self._ck(self.lib.ipcgpu_multilevel_debug_matrices(self.h, _d(out), out.size))
+        return [a.reshape(-1, 96, 96) for a in np.split(out, np.cumsum([9216 * d for d in domains])[:-1])]
 
     def csr_set_zero(self):
         self._ck(self.lib.ipcgpu_csr_set_zero(self.h))
