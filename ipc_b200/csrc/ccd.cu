@@ -644,6 +644,8 @@ struct NarrowArgs {
     // device-resident: cand_range = the slice of `cand` this rank walks, max_t = the step on entry (every pair's max_t), ccd_ord = the
     // running device-wide minimum (ordered-uint image): boxes starting at or after it cannot lower the result
     const IterState* st;
+    DBox* arena;     // overflow arena of the warp-level pass (ti_root_finder_arena) and its lock
+    int* arena_lock;
 };
 
 __global__ void __launch_bounds__(128) k_ti_stage1(NarrowArgs a, unsigned* __restrict__ survivors, unsigned* __restrict__ nSurv, int* __restrict__ zero_flag)
@@ -720,10 +722,20 @@ DEV bool sum_le_1(unsigned long long an, int ak, unsigned long long bn, int bk)
 }
 
 constexpr unsigned F_ZERO = 1u << 24; // zero_in flag stored in DBox::kk
+constexpr unsigned F_VIS = 1u << 25;  // the box was evaluated at this level (the library counts it towards max_itr)
 
 constexpr int kStage2WarpsPerCtaDev = 4;
 constexpr int kSmemLevel = 184; // boxes per level buffer kept in shared memory by the warp-level pass
 constexpr int kWideLevel = 10; // levels with at least this many boxes are evaluated box-parallel, narrower ones corner-parallel
+// Boxes per level buffer of the overflow arena.  A level only splits boxes the library has counted, and it leaves before the count
+// exceeds max_itr (1e6), so no level holds more than 2 max_itr boxes: a search in the arena never outgrows it.
+constexpr int kArenaLevel = 2000000;
+
+DEV Key3 box_key(const DBox& b)
+{
+    const int tk = b.kk & 0xff, uk = (b.kk >> 8) & 0xff, vk = (b.kk >> 16) & 0xff;
+    return Key3{ dy_lo(b.tn, tk), dy_lo(b.un, uk), dy_lo(b.vn, vk) };
+}
 
 // warp inclusive prefix sum of v
 DEV int warp_incl_scan(int v, int lane)
@@ -736,7 +748,38 @@ DEV int warp_incl_scan(int v, int lane)
     return v;
 }
 
-// box-parallel root finder of the warp-level pass, one box per lane, level buffers in global memory: 0 no collision, 1 collision (toi set)
+// Does the library leave this level through max_itr?  It walks the level in key order, counting every evaluated box, and leaves at the
+// first box containing the origin whose count exceeds max_itr -- unless a terminal box comes first.  The last box it can leave at is the
+// last one containing the origin before K2 when K2 is terminal, up to and including K2 when K2 only stops the level's splitting, or the
+// last one of the level.  room = max_itr - (boxes counted at earlier levels).
+DEV bool library_leaves_at_max_itr(const DBox* cur, int n, int lane, bool has_k2, bool k2_terminal, const Key3& k2, long long room)
+{
+    const double INF = __longlong_as_double(0x7ff0000000000000ll);
+    Key3 nz = { INF, INF, INF }; // the last candidate box, as the minimum of the negated keys
+    unsigned pay = 0;
+    double aux = 0.0;
+    for (int base = 0; base < n; base += 32) {
+        const int i = base + lane;
+        Key3 mk = { INF, INF, INF };
+        if (i < n && (cur[i].kk & F_ZERO)) {
+            const Key3 key = box_key(cur[i]);
+            if (!has_k2 || key_less(key, k2) || (!k2_terminal && !key_less(k2, key))) mk = Key3{ -key.t, -key.u, -key.v };
+        }
+        warp_min_key(mk, pay, aux);
+        if (key_less(mk, nz)) nz = mk;
+    }
+    if (nz.t == INF) return false;
+    const Key3 z = { -nz.t, -nz.u, -nz.v };
+    long long count = 0; // the library's count when it reaches z
+    for (int base = 0; base < n; base += 32) {
+        const int i = base + lane;
+        count += __popc(__ballot_sync(0xffffffffu, i < n && (cur[i].kk & F_VIS) && !key_less(z, box_key(cur[i]))));
+    }
+    return count > room;
+}
+
+// box-parallel root finder of the warp-level pass, one box per lane, level buffers in global memory: 0 no collision, 1 collision (toi set),
+// -1 a level outgrew the buffers (toi / out_tol hold the conservative estimate of the level before)
 __device__ int ti_root_finder(bool VF, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err, double ms, int max_itr, DBox* bufA,
     DBox* bufB, int cap, int lane, double& toi, double& out_tol, int* __restrict__ warn, const unsigned long long* best)
 {
@@ -781,10 +824,11 @@ __device__ int ti_root_finder(bool VF, const TiPair& P, const double* tol, const
                 unsigned flags = 0;
                 if (tlo < toi_skip && tlo < t_prune) {
                     vis = true;
+                    flags = F_VIS;
                     bool box_in;
                     double tt[3];
                     if (origin_in_box(VF, P, b, err, ms, box_in, tt)) {
-                        flags = F_ZERO;
+                        flags |= F_ZERO;
                         const bool tol_cond = tt[0] <= co_tol && tt[1] <= co_tol && tt[2] <= co_tol;
                         const bool cond1 = pow2neg(tk) <= tol[0] && pow2neg(uk) <= tol[1] && pow2neg(vk) <= tol[2];
                         const Key3 key = { tlo, dy_lo(b.un, uk), dy_lo(b.vn, vk) };
@@ -816,36 +860,40 @@ __device__ int ti_root_finder(bool VF, const TiPair& P, const double* tol, const
             return 1;
         }
         const bool has_k2 = k2.t != INF;
-        if (has_k2 && (p2 & 1u)) { // a later box already below the width tolerances (condition 1)
-            // boxes between K1 and K2 do not matter: the library returns here
-            toi = k2.t;
-            return 1;
-        }
         if (lane == 0) atomicAdd(reinterpret_cast<unsigned long long*>(warn + 7), (unsigned long long)visited); // diagnostics: boxes evaluated
         if (max_itr > 0) {
             temp_toi = k1.t;
             temp_out_tol = fmax(a1, co_tol);
-            refine += visited;
-            if (refine > max_itr) { // conservative early-out (the library returns its per-level estimate here as well)
+            // the library's own early-out, at the box where its count crosses max_itr; it can only cross where the count of every
+            // evaluated box does, which levels of the per-warp buffers never reach (181 levels x 4,096 boxes < 1e6)
+            if (refine + visited > max_itr && library_leaves_at_max_itr(cur, n, lane, has_k2, (p2 & 1u) != 0, k2, max_itr - refine)) {
                 if (lane == 0) atomicAdd(warn, 1);
                 toi = temp_toi;
                 out_tol = temp_out_tol;
                 return 1;
             }
         }
+        if (has_k2 && (p2 & 1u)) { // a later box already below the width tolerances (condition 1)
+            // boxes between K1 and K2 do not matter: the library returns here
+            toi = k2.t;
+            return 1;
+        }
         if (has_k2) {
             if (k2.t < toi_skip) toi_skip = k2.t;
             use_skip = true;
         }
-        // ---- pass 2: split every box that contains the origin and precedes K2 ------------------------------------------
+        // ---- pass 2: split every box that contains the origin and precedes K2; count the boxes the library evaluated (up to K2) --
         int nn = 0;
-        bool over = false;
+        long long counted = 0;
+        bool over = false, full = false;
         for (int base = 0; base < n; base += 32) {
             const int i = base + lane;
             int nchild = 0;
             DBox c0, c1;
+            bool cnt = false;
             if (i < n) {
                 const DBox b = cur[i];
+                if (b.kk & F_VIS) cnt = !has_k2 || !key_less(k2, box_key(b));
                 if (b.kk & F_ZERO) {
                     const int tk = b.kk & 0xff, uk = (b.kk >> 8) & 0xff, vk = (b.kk >> 16) & 0xff;
                     const Key3 key = { dy_lo(b.tn, tk), dy_lo(b.un, uk), dy_lo(b.vn, vk) };
@@ -885,24 +933,30 @@ __device__ int ti_root_finder(bool VF, const TiPair& P, const double* tol, const
                     }
                 }
             }
+            counted += __popc(__ballot_sync(0xffffffffu, cnt));
             // warp exclusive scan of nchild
             const int incl = warp_incl_scan(nchild, lane), total = __shfl_sync(0xffffffffu, incl, 31);
             const int off = nn + incl - nchild;
-            if (nn + total > cap) over = true;
+            if (nn + total > cap) full = true;
             else {
                 if (nchild > 0) nxt[off] = c0;
                 if (nchild > 1) nxt[off + 1] = c1;
             }
             nn += total;
-            if (__any_sync(0xffffffffu, over)) { over = true; break; }
+            if (__any_sync(0xffffffffu, over || full)) break;
         }
-        if (__any_sync(0xffffffffu, over)) {
-            // level buffer / bisection depth exhausted: return the conservative per-level estimate (earliest box containing the origin)
-            if (lane == 0) atomicAdd(warn, 1);
+        if (__any_sync(0xffffffffu, over || full)) {
+            // bisection depth exhausted: return the conservative per-level estimate (earliest box containing the origin); a level that
+            // outgrew the buffers returns the same estimate as -1, and the caller runs the search again in larger ones
             toi = temp_toi;
             out_tol = temp_out_tol;
-            return 1;
+            if (__any_sync(0xffffffffu, over)) {
+                if (lane == 0) atomicAdd(warn, 1);
+                return 1;
+            }
+            return -1;
         }
+        refine += counted;
         __syncwarp();
         DBox* t = cur; cur = nxt; nxt = t;
         n = nn;
@@ -1175,10 +1229,35 @@ __device__ __noinline__ int ti_root_finder_warp_call(bool vf, const TiPair& P, c
     return ti_root_finder(vf, P, tol, inv_tol, co_tol, max_t, err, ms, max_itr, bufA, bufB, cap, lane, toi, out_tol, warn, best);
 }
 
+// A search that outgrows the per-warp level buffers runs again in the context's overflow arena (two levels of kArenaLevel boxes), which one
+// warp holds at a time: such searches are rare, and the library itself runs them to max_itr.  The arena run does not prune against the
+// running minimum, so its count of evaluated boxes -- and with it the max_itr exit -- is the library's own.
+__device__ __noinline__ int ti_root_finder_arena(bool vf, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err,
+    double ms, int max_itr, DBox* arena, int* arena_lock, int lane, double& toi, double& out_tol, int* __restrict__ warn)
+{
+    if (lane == 0) {
+        while (atomicCAS(arena_lock, 0, 1) != 0) __nanosleep(1000);
+        __threadfence();
+    }
+    __syncwarp();
+    int rc = ti_root_finder_warp_call(vf, P, tol, inv_tol, co_tol, max_t, err, ms, max_itr, arena, arena + kArenaLevel, kArenaLevel, lane, toi, out_tol, warn, nullptr);
+    __syncwarp();
+    if (lane == 0) {
+        __threadfence();
+        atomicExch(arena_lock, 0);
+    }
+    if (rc == -1) { // cannot happen (see kArenaLevel); keep the conservative estimate and report it
+        if (lane == 0) atomicAdd(warn, 1);
+        rc = 1;
+    }
+    return rc;
+}
+
 // vertexFaceCCD_double / edgeEdgeCCD_double including the no_zero_toi refinement loop; returns 0 / 1.  The corner-parallel root finder runs
-// in the shared-memory level buffers sA / sB; a search that outgrows them restarts box-parallel in the global buffers bufA / bufB.
+// in the shared-memory level buffers sA / sB; a search that outgrows them restarts box-parallel in the global buffers bufA / bufB, and one
+// that outgrows those in the overflow arena.
 __device__ int ti_ccd(bool vf, const TiPair& P, const double* err, double ms, double tolerance, double t_max, int max_itr, DBox* bufA, DBox* bufB, int cap, int lane,
-    double& toi, int* __restrict__ warn, DBox* sA, DBox* sB, const unsigned long long* best)
+    double& toi, int* __restrict__ warn, DBox* sA, DBox* sB, const unsigned long long* best, DBox* arena, int* arena_lock)
 {
     double tolerance_in = tolerance, ms_in = ms, out_tol = tolerance;
     bool is_impacting = false, tmp = false;
@@ -1193,6 +1272,7 @@ __device__ int ti_ccd(bool vf, const TiPair& P, const double* err, double ms, do
         for (int d = 0; d < 3; ++d) inv_tol[d] = 1.0 / tol[d];
         int rc = ti_root_finder_cp_call(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, sA, sB, lane, toi, out_tol, warn, best);
         if (rc == -1) rc = ti_root_finder_warp_call(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, bufA, bufB, cap, lane, toi, out_tol, warn, best);
+        if (rc == -1) rc = ti_root_finder_arena(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, arena, arena_lock, lane, toi, out_tol, warn);
         tmp = rc == 1;
         if (iter == 0) is_impacting = tmp;
         else toi = tmp ? toi : t_max;
@@ -1220,7 +1300,7 @@ __device__ int pair_ccd(bool vf, const TiPair& P, const NarrowArgs& a, DBox* buf
     for (int attempt = 0; attempt < 2; ++attempt) {
         const double ms = attempt ? 0.0 : fmin(0.2 * d, 1e-6);
         const unsigned long long* best = attempt ? nullptr : &a.st->ccd_ord;
-        hit = ti_ccd(vf, P, err, ms, a.tol, max_t, a.max_itr, bufA, bufB, cap, lane, toi, warn, sA, sB, best);
+        hit = ti_ccd(vf, P, err, ms, a.tol, max_t, a.max_itr, bufA, bufB, cap, lane, toi, warn, sA, sB, best, a.arena, a.arena_lock);
         if (attempt == 1) {
             if (hit) toi *= 0.8;
             break;
@@ -1576,7 +1656,13 @@ int ccd_alloc(ipcgpu_ctx* ctx)
     const size_t nEnt = (size_t)8 * std::max(ctx->nSF + ctx->nSE + ctx->nSV, 1);
     size_t scan_bytes = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int*)nullptr, (int*)nullptr, (int)(3 * kGridCells + 1));
-    bool ok = w.vmin.reserve((size_t)3 * ctx->nV) && w.vmax.reserve((size_t)3 * ctx->nV) && w.cand.reserve(ctx->ccd_capacity) && w.surv.reserve(ctx->ccd_capacity) && w.surv2.reserve(ctx->ccd_capacity)
+    if (!w.arena_lock.p) {
+        if (!w.arena_lock.reserve(1) || cudaMemsetAsync(w.arena_lock.p, 0, sizeof(int), ctx->stream) != cudaSuccess) {
+            ctx->err = "CCD workspace allocation failed";
+            return IPCGPU_ERR_CUDA;
+        }
+    }
+    bool ok = w.arena.reserve((size_t)2 * kArenaLevel * sizeof(DBox)) && w.vmin.reserve((size_t)3 * ctx->nV) && w.vmax.reserve((size_t)3 * ctx->nV) && w.cand.reserve(ctx->ccd_capacity) && w.surv.reserve(ctx->ccd_capacity) && w.surv2.reserve(ctx->ccd_capacity)
         && w.scratch.reserve(warps * 2 * kLevelCap * sizeof(DBox)) && w.counters.reserve(16) && w.ncand.reserve(2) && w.bounds.reserve(8) && w.cells.reserve(1)
         && w.sw_keys.reserve(nEnt) && w.sw_ent.reserve(nEnt) && w.sw_cnt.reserve((size_t)3 * kGridCells + 1) && w.sw_off.reserve((size_t)3 * kGridCells + 1)
         && w.sw_tmp.reserve(scan_bytes + 256);
@@ -1603,6 +1689,8 @@ int ccd_narrow(ipcgpu_ctx* ctx, const int2* cand, const int* n32, const unsigned
     a.tol = tol;
     a.max_itr = 1000000;    // TIGHT_INCLUSION_MAX_ITER (CCDUtils.hpp:14)
     a.st = ctx->iter.p;
+    a.arena = reinterpret_cast<DBox*>(w.arena.p);
+    a.arena_lock = w.arena_lock.p;
     IterState* ist = ctx->iter.p;
     unsigned* nSurv = reinterpret_cast<unsigned*>(w.counters.p);
     unsigned* work = nSurv + 1;

@@ -86,7 +86,8 @@ struct CcdWork {
     DevBuf<int> vmin, vmax, counters;
     DevBuf<int2> cand;
     DevBuf<unsigned> surv, surv2;
-    DevBuf<unsigned char> scratch;
+    DevBuf<unsigned char> scratch, arena; // per-warp level buffers of the narrow phase's warp pass; overflow arena shared by its warps
+    DevBuf<int> arena_lock;
     DevBuf<unsigned long long> ncand, bounds;
     // swept grid on the reference voxel lattice (ccd.cu): geometry, per-entry cell keys and entries (sorted by key), dense per-(type, cell)
     // counters and their exclusive prefix sum, scan scratch

@@ -153,6 +153,27 @@ extern "C" void orc_ti_stats(long long* out72, int reset)
 static std::atomic<int> g_tie_reversed{ 0 };
 extern "C" void orc_ti_debug_tie_order(int reversed) { g_tie_reversed.store(reversed ? 1 : 0); }
 
+/* orc_ti_debug_level_cap(n), n > 0: emulates a root finder whose level buffers hold n boxes and which, when the next level would outgrow
+ * them, returns the per-level estimate of the current level (the estimate of the max_itr exit).  The CUDA narrow phase did this with
+ * n = 4096 before it continued such searches in an overflow arena; 0 (the default) is the library, which has no such cap.  Kept so that
+ * tests can show what that rule does to a search (tests/test_ccd_regimes.py). */
+static std::atomic<long long> g_level_cap{ 0 };
+extern "C" void orc_ti_debug_level_cap(long long n) { g_level_cap.store(n > 0 ? n : 0); }
+
+/* How a search went (orc_ti_trace).  Exits of the root finder: */
+enum TiExit { EXIT_EXHAUSTED = 0, EXIT_K1 = 1, EXIT_K2 = 2, EXIT_SKIP = 3, EXIT_MAX_ITR = 4, EXIT_DEPTH = 5, EXIT_LEVEL_CAP = 6, EXIT_UNFINISHED = 7 };
+struct TiTrace {
+    long long trip_cap, box_cap;   /* limits: no_zero_toi trips per ti_ccd call, boxes per trace */
+    long long exits[8];            /* root-finder calls per exit */
+    int last_exit;
+    long long levels, width, boxes;
+    long long trips[3];            /* no_zero_toi trips: t_max *= 0.9, ms *= 0.5, tolerance *= 0.1 */
+    double ms, tolerance, t_max;   /* of the last root-finder call */
+    int retry;                     /* pair_ccd ran its ms = 0 retry */
+    int unfinished;
+};
+static thread_local TiTrace* g_trace = nullptr;
+
 /* interval_root_finder_double_horizontal_tree with the canonical in-level order */
 bool root_finder(bool vf, const double* x0, const double* x1, const double tol[3], double co_tol, double max_t, const double err[3], double ms,
     int max_itr, double& toi, double& out_tol)
@@ -167,6 +188,10 @@ bool root_finder(bool vf, const double* x0, const double* x1, const double tol[3
     out_tol = co_tol;
     toi = std::numeric_limits<double>::infinity();
     bool overflow = false;
+    int why = EXIT_MAX_ITR;
+    TiTrace* tr = g_trace;
+    const long long level_cap = g_level_cap.load(std::memory_order_relaxed);
+    auto exit_as = [tr](int e) { if (tr) { tr->exits[e]++; tr->last_exit = e; } };
     TiStat stat;
     /* diagnostics only (sizing the GPU passes, never set by tests): ORC_TI_DIAG_PRUNE=<t> skips boxes that start at or after max(t, 1e-6), the
      * GPU's pruning rule against the running minimum in the limit of an instantly known final step */
@@ -174,6 +199,10 @@ bool root_finder(bool vf, const double* x0, const double* x1, const double tol[3
     while (!level.empty() && !overflow) {
         ++stat.levels;
         stat.width = std::max<long long>(stat.width, (long long)level.size());
+        if (tr) {
+            ++tr->levels;
+            tr->width = std::max<long long>(tr->width, (long long)level.size());
+        }
         const bool rev = g_tie_reversed.load(std::memory_order_relaxed) != 0;
         std::sort(level.begin(), level.end(), [rev](const Box3& a, const Box3& b) {
             double ta = lo_of(a.t), tb = lo_of(b.t);
@@ -182,7 +211,7 @@ bool root_finder(bool vf, const double* x0, const double* x1, const double tol[3
             if (ua != ub) return rev ? ua > ub : ua < ub;
             return rev ? lo_of(a.v) > lo_of(b.v) : lo_of(a.v) < lo_of(b.v);
         });
-        bool this_level_less_tol = true, find_level_root = false;
+        bool this_level_less_tol = true, find_level_root = false, origin_seen = false;
         next.clear();
         for (const Box3& cur : level) {
             const double t_lo = lo_of(cur.t);
@@ -190,9 +219,17 @@ bool root_finder(bool vf, const double* x0, const double* x1, const double tol[3
             if (diag_prune >= 0.0 && !(t_lo < std::max(diag_prune, 1e-6))) continue;
             ++refine;
             ++stat.boxes;
+            if (tr && ++tr->boxes > tr->box_cap) {
+                tr->unfinished = 1;
+                exit_as(EXIT_UNFINISHED);
+                toi = 0.0;
+                return true;
+            }
             bool box_in;
             double true_tol[3];
             if (!origin_in_box(vf, x0, x1, cur, err, ms, box_in, true_tol)) continue;
+            const bool first_origin = !origin_seen;
+            origin_seen = true;
             const double w[3] = { width_of(cur.t), width_of(cur.u), width_of(cur.v) };
             const bool tol_cond = true_tol[0] <= co_tol && true_tol[1] <= co_tol && true_tol[2] <= co_tol;
             const bool cond1 = w[0] <= tol[0] && w[1] <= tol[1] && w[2] <= tol[2];
@@ -200,6 +237,7 @@ bool root_finder(bool vf, const double* x0, const double* x1, const double tol[3
             if (!tol_cond) this_level_less_tol = false;
             const bool cond3 = this_level_less_tol;
             if (cond1 || cond2 || cond3) {
+                exit_as(first_origin ? EXIT_K1 : EXIT_K2);
                 toi = t_lo;
                 return true;
             }
@@ -231,6 +269,7 @@ bool root_finder(bool vf, const double* x0, const double* x1, const double tol[3
             const Dy parent = cur.*mem;
             if (parent.k >= 60) { /* bisection overflow */
                 overflow = true;
+                why = EXIT_DEPTH;
                 break;
             }
             const Dy h1 = { parent.n * 2, parent.k + 1 }, h2 = { parent.n * 2 + 1, parent.k + 1 };
@@ -246,17 +285,24 @@ bool root_finder(bool vf, const double* x0, const double* x1, const double tol[3
                 }
             }
         }
+        if (!overflow && level_cap > 0 && (long long)next.size() > level_cap) {
+            overflow = true;
+            why = EXIT_LEVEL_CAP;
+        }
         level.swap(next);
     }
     if (overflow) {
+        exit_as(why);
         toi = temp_toi;
         out_tol = temp_out_tol;
         return true;
     }
     if (use_skip) {
+        exit_as(EXIT_SKIP);
         toi = toi_skip;
         return true;
     }
+    exit_as(EXIT_EXHAUSTED);
     return false;
 }
 
@@ -271,12 +317,24 @@ bool ti_ccd(bool vf, const double* x0, const double* x1, const double err[3], do
         double tol[3];
         width_tolerances(vf, x0, x1, tolerance_in, tol);
         tmp = root_finder(vf, x0, x1, tol, tolerance_in, t_max, err, ms_in, max_itr, toi, out_tol);
+        if (g_trace) {
+            g_trace->ms = ms_in;
+            g_trace->tolerance = tolerance_in;
+            g_trace->t_max = t_max;
+            if (g_trace->unfinished) break;
+        }
         if (iter == 0) is_impacting = tmp;
         else toi = tmp ? toi : t_max;
         if (tmp && toi == 0 && no_zero_toi) {
-            if (out_tol > tolerance_in) t_max *= 0.9;
-            else if (10 * tolerance_in < ms_in) ms_in *= 0.5;
+            if (g_trace && g_trace->trips[0] + g_trace->trips[1] + g_trace->trips[2] >= g_trace->trip_cap) {
+                g_trace->unfinished = 1;
+                break;
+            }
+            const int branch = out_tol > tolerance_in ? 0 : (10 * tolerance_in < ms_in ? 1 : 2);
+            if (branch == 0) t_max *= 0.9;
+            else if (branch == 1) ms_in *= 0.5;
             else tolerance_in *= 0.1;
+            if (g_trace) ++g_trace->trips[branch];
         }
         ++iter;
     } while (no_zero_toi && iter < 0x7fffffffu && tmp && toi == 0);
@@ -292,6 +350,8 @@ inline void vert_of(const orc_surf* s, int v, double* out)
 inline bool is_dbc(const orc_surf* s, int v) { return s->dbc && s->dbc[v] != 0; }
 inline int codim(const orc_surf* s, int v) { return s->vCoDim ? s->vCoDim[v] : 3; }
 
+int pair_ccd_x(bool vf, const double* x0, const double* x1, double tol, const double err[3], double max_t, double* toi_out);
+
 /* one candidate: SelfCollisionHandler.cpp:725-790 (EE) / :795-861 (PT). returns -1 when d==0 (stepSize := 0) */
 int pair_ccd(bool vf, const int v[4], const orc_surf* s, const double* p, double tol, const double err[3], double max_t, double* toi_out)
 {
@@ -300,6 +360,12 @@ int pair_ccd(bool vf, const int v[4], const orc_surf* s, const double* p, double
         vert_of(s, v[k], x0 + 3 * k);
         for (int c = 0; c < 3; ++c) x1[3 * k + c] = x0[3 * k + c] + p[3 * (size_t)v[k] + c];
     }
+    return pair_ccd_x(vf, x0, x1, tol, err, max_t, toi_out);
+}
+
+/* the same from the pair's coordinates (x1 = x0 + p already formed) */
+int pair_ccd_x(bool vf, const double* x0, const double* x1, double tol, const double err[3], double max_t, double* toi_out)
+{
     double d;
     if (vf) orc_point_tri_d(x0, &d);
     else orc_edge_edge_d(x0, &d);
@@ -307,7 +373,8 @@ int pair_ccd(bool vf, const int v[4], const orc_surf* s, const double* p, double
     if (d == 0) return -1;
     double toi, out_tol;
     bool hit = ti_ccd(vf, x0, x1, err, std::min(0.2 * d, 1e-6), tol, max_t, 1000000, true, toi, out_tol);
-    if (hit && toi < 1e-6) {
+    if (hit && toi < 1e-6 && !(g_trace && g_trace->unfinished)) {
+        if (g_trace) g_trace->retry = 1;
         hit = ti_ccd(vf, x0, x1, err, 0.0, tol, max_t, 1000000, true, toi, out_tol);
         if (hit) toi *= 0.8;
     }
@@ -329,6 +396,39 @@ int orc_ti_vf(const double* x0, const double* x1, const double err[3], double ms
 int orc_ti_ee(const double* x0, const double* x1, const double err[3], double ms, double tol, double max_t, int max_itr, int no_zero_toi, double* toi, double* out_tol)
 {
     return ti_ccd(false, x0, x1, err, ms, tol, max_t, max_itr, no_zero_toi != 0, *toi, *out_tol) ? 1 : 0;
+}
+
+/* One pair as the narrow phase runs it (pair_ccd: ms = min(0.2 d, 1e-6), max_itr = 1e6, no_zero_toi, the ms = 0 retry), traced.
+ * vf = 1: point-triangle (p, t0, t1, t2), 0: edge-edge (a0, a1, b0, b1); x1 = x0 + p as the caller formed it.  The search gives up once
+ * a ti_ccd call takes trip_cap no_zero_toi trips or the pair evaluates box_cap boxes (out_i[9] = 1, "did not finish").
+ * Returns what pair_ccd returns: -1 zero initial distance, 0 no impact, 1 impact (*toi set).
+ * out_i[0..7]: root-finder calls per exit (exhausted, terminal K1, terminal K2, TOI_SKIP, max_itr, depth 60, level cap, unfinished);
+ * out_i[8]: exit of the last call; [9] unfinished; [10] retry ran; [11] levels; [12] widest level; [13] boxes evaluated;
+ * [14..16] no_zero_toi trips taking t_max *= 0.9, ms *= 0.5, tolerance *= 0.1.
+ * out_d[0..2]: ms, tolerance and t_max of the last root-finder call. */
+int orc_ti_trace(int vf, const double* x0, const double* x1, const double err[3], double tol, double max_t, long long trip_cap, long long box_cap, double* toi,
+    long long* out_i, double* out_d)
+{
+    TiTrace tr{};
+    tr.trip_cap = trip_cap;
+    tr.box_cap = box_cap;
+    tr.last_exit = -1;
+    g_trace = &tr;
+    *toi = std::numeric_limits<double>::quiet_NaN();
+    const int r = pair_ccd_x(vf != 0, x0, x1, tol, err, max_t, toi);
+    g_trace = nullptr;
+    for (int e = 0; e < 8; ++e) out_i[e] = tr.exits[e];
+    out_i[8] = tr.last_exit;
+    out_i[9] = tr.unfinished;
+    out_i[10] = tr.retry;
+    out_i[11] = tr.levels;
+    out_i[12] = tr.width;
+    out_i[13] = tr.boxes;
+    for (int b = 0; b < 3; ++b) out_i[14 + b] = tr.trips[b];
+    out_d[0] = tr.ms;
+    out_d[1] = tr.tolerance;
+    out_d[2] = tr.t_max;
+    return r;
 }
 
 /* CCDUtils.cpp:21-87: world bbox of V (and V+p), inflated to centre +- 10*radius*(1,1,1)/sqrt(3), then

@@ -164,6 +164,11 @@ int orc_ti_ee(const double* x0, const double* x1, const double err[3], double ms
     double max_t, int max_itr, int no_zero_toi, double* toi, double* out_tol);
 /* diagnostics: 1 = boxes of a level with equal t_lo are visited in DESCENDING (u_lo, v_lo) instead of the canonical ascending order */
 void orc_ti_debug_tie_order(int reversed);
+/* diagnostics: n > 0 emulates level buffers of n boxes that return the per-level estimate when a level outgrows them; 0 = the library */
+void orc_ti_debug_level_cap(long long n);
+/* one pair as the narrow phase runs it (pair_ccd, with its ms = 0 retry), with a trace of how the search went; see ccd.cpp */
+int orc_ti_trace(int vf, const double* x0, const double* x1, const double err[3], double tol, double max_t, long long trip_cap, long long box_cap,
+    double* toi, long long* out_i, double* out_d);
 /* SelfCollisionHandler.cpp:690-866 with canonical max_t = alpha on entry */
 int orc_ccd_partial(const orc_surf* s, const double* p, const int* cand, int nCand, double tol,
     const double err_vf[3], const double err_ee[3], double* alpha_inout, int nthreads);

@@ -365,6 +365,30 @@ def ti(kind, x0, x1, err, ms, tol=1e-6, max_t=1.0, max_itr=1000000, no_zero_toi=
     return bool(hit), toi.value, ot.value
 
 
+TI_EXITS = ("exhausted", "k1", "k2", "skip", "max_itr", "depth60", "level_cap", "unfinished")
+
+
+def ti_trace(kind, x0, x1, err, tol=1e-6, max_t=1.0, trip_cap=1000, box_cap=1 << 24, level_cap=0):
+    """One pair as the narrow phase runs it (ms from the initial distance, max_itr 1e6, no_zero_toi, the ms = 0 retry), traced.
+    level_cap > 0 emulates level buffers that return the per-level estimate when a level outgrows them.
+    Returns (r, toi, trace): r = -1 zero distance / 0 no impact / 1 impact."""
+    x0 = np.ascontiguousarray(x0, dtype=np.float64).ravel(); x1 = np.ascontiguousarray(x1, dtype=np.float64).ravel()
+    err = np.ascontiguousarray(err, dtype=np.float64)
+    toi = C.c_double()
+    oi = np.zeros(17, dtype=np.int64); od = np.zeros(3)
+    lib().orc_ti_debug_level_cap(C.c_longlong(int(level_cap)))
+    try:
+        r = lib().orc_ti_trace(int(kind == "vf"), d(x0), d(x1), d(err), C.c_double(tol), C.c_double(max_t), C.c_longlong(int(trip_cap)),
+                               C.c_longlong(int(box_cap)), C.byref(toi), oi.ctypes.data_as(C.POINTER(C.c_longlong)), d(od))
+    finally:
+        lib().orc_ti_debug_level_cap(C.c_longlong(0))
+    tr = dict(exits={TI_EXITS[e]: int(oi[e]) for e in range(8)}, last_exit=TI_EXITS[oi[8]] if oi[8] >= 0 else None, unfinished=bool(oi[9]),
+              retry=bool(oi[10]), levels=int(oi[11]), width=int(oi[12]), boxes=int(oi[13]), trips=[int(x) for x in oi[14:17]],
+              ms=float(od[0]), tolerance=float(od[1]), t_max=float(od[2]))
+    tr["early_outs"] = tr["exits"]["max_itr"] + tr["exits"]["depth60"] + tr["exits"]["level_cap"]
+    return int(r), toi.value, tr
+
+
 def ti_error(V_soa, nV, p=None):
     V_soa = np.ascontiguousarray(V_soa, dtype=np.float64)
     evf, eee = np.empty(3), np.empty(3)
