@@ -108,15 +108,17 @@ int build_maps(ipcgpu_ctx* ctx)
     }
     cptr.push_back((int)ks.size());
     {
-        // Slot order = work order of k_assemble_csr (9 threads per slot, a warp covers ~3.5 slots and runs as long as its longest
-        // contribution list).  In key order every 7th slot is a diagonal block with ~23 contributions against ~5 for an off-diagonal
-        // one, so half of the warps idled most lanes for 20 iterations.  Off-diagonal slots first, then the diagonal ones (key order
-        // inside each group keeps the CSR writes local): warps see uniform list lengths.
+        // Slot order = work order of k_assemble_csr (one thread per stored entry: 9 per off-diagonal slot, 6 per diagonal one; a warp
+        // covers ~3.5 / ~5.3 slots and runs as long as its longest contribution list).  In key order every 7th slot is a diagonal block
+        // with ~23 contributions against ~5 for an off-diagonal one, so half of the warps idled most lanes for 20 iterations.
+        // Off-diagonal slots first, then the diagonal ones (key order inside each group keeps the CSR writes local): warps see uniform
+        // list lengths, and the kernel knows from nOffSlots where the 6-thread slots begin.
         const size_t nS = sv.size();
         std::vector<int> order;
         order.reserve(nS);
         for (size_t i = 0; i < nS; ++i)
             if (sv[i] != su[i]) order.push_back((int)i);
+        ctx->nOffSlots = (int)order.size();
         for (size_t i = 0; i < nS; ++i)
             if (sv[i] == su[i]) order.push_back((int)i);
         std::vector<int> sv2(nS), su2(nS), cptr2;
@@ -340,7 +342,9 @@ static int zero_values(ipcgpu_ctx* ctx)
     return IPCGPU_OK;
 }
 
-static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int projectDBC, bool need_g, bool need_h, int add_mass, bool with_energy = false)
+// cleared: the value array holds zeros at every entry of the slots (zero_values), so the assembly writes its sums instead of adding them
+static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int projectDBC, bool need_g, bool need_h, int add_mass, bool with_energy = false,
+    bool cleared = false)
 {
     REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
     if (need_h) {
@@ -373,8 +377,8 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
     }
     if (need_h) {
         pe = ctx->prof_begin(IPCGPU_STAGE_ASSEMBLE_CSR);
-        assemble_csr(ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->slot_off.p, ctx->con_ptr.p, ctx->con_src.p, ctx->hblk.p,
-            ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, nullptr, 1, ctx->a.p, st);
+        assemble_csr(ctx->nOffSlots, ctx->nSlots, ctx->slot_v.p, ctx->slot_u.p, ctx->slot_off.p, ctx->con_ptr.p, ctx->con_src.p, ctx->hblk.p,
+            ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, nullptr, cleared ? 0 : 1, ctx->a.p, st);
         // per-vertex diagonal terms (mass, Dirichlet identity) of the owned rows
         const double* m = (add_mass && ctx->has_mass) ? ctx->mass.p : nullptr;
         diag_mass_dbc_range(ctx->v_begin, ctx->v_end, ctx->ia.p, ctx->index_base, ctx->has_dbc ? ctx->dbc.p : nullptr, projectDBC, m, ctx->a.p, st);
@@ -407,7 +411,7 @@ static int elastic_derivatives(ipcgpu_ctx* ctx, double coef, int projectSPD, int
     // -- contact-only blocks of the augmented pattern -- must not keep last iteration's values
     int rc = a ? sync_pattern_mirror(ctx) : 0; // (the host array holds the current pattern's values)
     if (rc || (rc = zero_values(ctx))) return rc;
-    if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, true, true, add_mass, with_energy))) return rc;
+    if ((rc = run_grad_hess(ctx, coef, projectSPD, projectDBC, true, true, add_mass, with_energy, true))) return rc;
     if (ctx->nranks > 1 && (g || a)) {
         rc = ipcgpu_allreduce_grad_hess(ctx, g ? 1 : 0, a ? 1 : 0);
         if (rc) return rc;

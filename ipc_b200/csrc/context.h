@@ -247,7 +247,7 @@ struct ipcgpu_ctx {
     // gradient gather map (local tets)
     ipcgpu::DevBuf<int> inc_ptr, inc;
     // Hessian slots (mesh-topology vertex pairs v<=u touched by local tets) and contributions
-    int nSlots = 0;
+    int nSlots = 0, nOffSlots = 0; // (the off-diagonal slots come first: [0, nOffSlots))
     ipcgpu::DevBuf<int> slot_v, slot_u, slot_off, con_ptr;
     ipcgpu::DevBuf<unsigned> con_src;
     bool hblk_valid = false; // the last gradient/Hessian call left the per-tet Hessian blocks in hblk

@@ -340,18 +340,28 @@ __global__ void __launch_bounds__(256) k_gather_gradient(int nV, const int* __re
 
 // ---------------------------------------------------------------------------------------------
 // CSR assembly (Energy.cpp:317-330 -> IglUtils::addBlockToMatrix -> LinSysSolver::addCoeff):
-// one thread per block-slot (vertex pair v<=u of the mesh topology); contributions are summed in
+// one thread per entry of a block-slot (vertex pair v<=u of the mesh topology); contributions are summed in
 // ascending tet order (the reference's vFLoc order), then written to the three CSR rows.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(288) k_assemble_csr(int nSlots, const int* __restrict__ slot_v, const int* __restrict__ slot_u,
+__global__ void __launch_bounds__(288) k_assemble_csr(int nOff, int nSlots, const int* __restrict__ slot_v, const int* __restrict__ slot_u,
     const int* __restrict__ slot_off /* 3 per slot */, const int* __restrict__ con_ptr, const unsigned* __restrict__ con_src,
     const double* __restrict__ hblk, const uint8_t* __restrict__ dbc, int projectDBC, const double* __restrict__ mass,
     int accumulate, double* __restrict__ a)
 {
-    // 9 consecutive threads per slot: thread q sums entry q of every contributing block (ascending tet order: the reference's
-    // vFLoc order, so the sum is bitwise reproducible); the 9 loads of one block are one contiguous 72-byte run
-    const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int sIdx = (int)(tid / 9), q = (int)(tid - 9ll * sIdx);
+    // Consecutive threads per slot, one per stored entry: 9 for the off-diagonal slots [0, nOff), 6 for the diagonal ones after them
+    // (build_maps orders them so; a diagonal block stores its 6 upper entries).  Thread q sums entry q of every contributing block
+    // (ascending tet order: the reference's vFLoc order, so the sum is bitwise reproducible); the loads of one block are one contiguous run
+    const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, tOff = 9ll * nOff;
+    int sIdx, q;
+    if (tid < tOff) {
+        sIdx = (int)(tid / 9);
+        q = (int)(tid - 9ll * sIdx);
+    }
+    else {
+        const int k = (int)((tid - tOff) / 6);
+        sIdx = nOff + k;
+        q = (int)(tid - tOff - 6ll * k);
+    }
     if (sIdx >= nSlots) return;
     const int v = slot_v[sIdx], u = slot_u[sIdx];
     const bool diag = (v == u);
@@ -370,6 +380,7 @@ __global__ void __launch_bounds__(288) k_assemble_csr(int nSlots, const int* __r
     if (diag) { r = (q < 3) ? 0 : (q < 5 ? 1 : 2); c = (q < 3) ? q : (q < 5 ? q - 3 : 0); }
     else { r = q / 3; c = q - 3 * r; }
     const int o = slot_off[3 * sIdx + r] + c;
+    // accumulate == 0: the value array was cleared before, so a[o] = h is 0 + h without reading a[o] (a sum from +0.0 is never -0.0)
     if (accumulate) {
         if (!dropped) a[o] += h;
         else if (diag) a[o] = 0.0;
@@ -613,12 +624,12 @@ void gather_gradient(int nV, const int* inc_ptr, const int* inc, const double* g
     if (nV <= 0) return;
     k_gather_gradient<<<(nV + 255) / 256, 256, 0, st>>>(nV, inc_ptr, inc, gcont, dbc, projectDBC, accumulate, g);
 }
-void assemble_csr(int nSlots, const int* slot_v, const int* slot_u, const int* slot_off, const int* con_ptr, const unsigned* con_src,
+void assemble_csr(int nOff, int nSlots, const int* slot_v, const int* slot_u, const int* slot_off, const int* con_ptr, const unsigned* con_src,
     const double* hblk, const uint8_t* dbc, int projectDBC, const double* mass, int accumulate, double* a, cudaStream_t st)
 {
     if (nSlots <= 0) return;
-    const int nb = (int)(((long long)nSlots * 9 + 287) / 288);
-    k_assemble_csr<<<nb, 288, 0, st>>>(nSlots, slot_v, slot_u, slot_off, con_ptr, con_src, hblk, dbc, projectDBC, mass, accumulate, a);
+    const int nb = (int)(((long long)nOff * 9 + (long long)(nSlots - nOff) * 6 + 287) / 288);
+    k_assemble_csr<<<nb, 288, 0, st>>>(nOff, nSlots, slot_v, slot_u, slot_off, con_ptr, con_src, hblk, dbc, projectDBC, mass, accumulate, a);
 }
 void diag_mass_dbc(int nV, const int* ia, int base, const uint8_t* dbc, int projectDBC, const double* mass, double* a, cudaStream_t st)
 {

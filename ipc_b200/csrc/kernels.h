@@ -89,7 +89,9 @@ int elastic_energy_blocks(int nTets);
 void elastic_grad_hess(const ElasticArgs& p, double coef, int projectSPD, bool need_g, bool need_h, double* gcont, double* hblk, cudaStream_t st, double* e_partials = nullptr);
 int elastic_grad_hess_blocks(int n_list);
 void gather_gradient(int nV, const int* inc_ptr, const int* inc, const double* gcont, const uint8_t* dbc, int projectDBC, int accumulate, double* g, cudaStream_t st);
-void assemble_csr(int nSlots, const int* slot_v, const int* slot_u, const int* slot_off, const int* con_ptr, const unsigned* con_src,
+// nOff: the off-diagonal slots come first (slots [0, nOff)), the diagonal ones after them.  accumulate == 0: a[] holds zeros at the slots'
+// entries (written, not added)
+void assemble_csr(int nOff, int nSlots, const int* slot_v, const int* slot_u, const int* slot_off, const int* con_ptr, const unsigned* con_src,
     const double* hblk, const uint8_t* dbc, int projectDBC, const double* mass, int accumulate, double* a, cudaStream_t st);
 void diag_mass_dbc(int nV, const int* ia, int base, const uint8_t* dbc, int projectDBC, const double* mass, double* a, cudaStream_t st);
 // gate != nullptr: the kernel does nothing unless *gate is nonzero (the device-built pattern recomputes the offsets only when it changed)
