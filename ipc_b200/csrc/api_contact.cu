@@ -24,12 +24,13 @@ int ipcgpu_set_surface(ipcgpu_ctx* ctx, int nSV, const int* SVI, int nSE, const 
     REQUIRE(ok, IPCGPU_ERR_CUDA, "surface upload failed");
     ctx->has_codim = vCoDim != nullptr;
     if (vCoDim) REQUIRE(ctx->vCoDim.upload(vCoDim, ctx->nV, ctx->stream), IPCGPU_ERR_CUDA, "codim upload failed");
+    int rc = safeguard_set_points(ctx, vCoDim);
+    if (rc) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->h_SVI.assign(SVI, SVI + nSV);
     ctx->hs_set_built = ctx->hs_lag_ready = false; // the plane sets index the old surface (and halfspace_alloc may reallocate them)
     ctx->pSize_surface = false; // pSize belongs to the surface
-    int rc = contact_alloc(ctx);
-    if (rc) return rc;
+    if ((rc = contact_alloc(ctx))) return rc;
     if ((rc = ccd_alloc(ctx))) return rc;
     ctx->surface_ready = true;
     if (ctx->device_pattern) return ipcgpu_enable_device_pattern(ctx, ctx->index_base, ctx->pw.requested_cap); // new surface edges

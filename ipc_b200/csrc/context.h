@@ -132,6 +132,22 @@ struct MultilevelWork {
     bool smem_opted = false;              // the inversion kernel's dynamic shared memory has been opted in
 };
 
+// point-in-tetrahedron half of the intersection check (safeguard.cu): the codimension-0 vertices (vCoDim == 0) of ipcgpu_set_surface, and
+// a grid over them rebuilt at every check -- cell key per point, the (key, vertex) pairs sorted by key, the grid's geometry, sort scratch
+struct PointGrid {
+    double o[3], inv_h;
+    int n[3];
+    double lo[3], hi[3]; // box of the points: a tetrahedron whose box misses it scans nothing
+};
+struct PointTetWork {
+    int n = 0; // codimension-0 vertices; 0 = the check launches nothing
+    DevBuf<int> pts, id, id_sorted;
+    DevBuf<unsigned> key, key_sorted;
+    DevBuf<PointGrid> grid;
+    DevBuf<unsigned char> sort_tmp;
+    size_t sort_bytes = 0;
+};
+
 // pinned host memory of the scalars the entry points copy between host and device, one member per use.  Allocated once per context
 // (cudaMallocHost(sizeof(HostStaging))), freed by ipcgpu_destroy: every member keeps its own address for the context's lifetime, since a
 // captured graph or a copy nobody waits on may still hold it.
@@ -217,6 +233,7 @@ struct ipcgpu_ctx {
     bool partition_contact = false, lists_local = false; // multi-rank: build only this rank's share of the contact sets
     ipcgpu::ContactWork cw;
     ipcgpu::CcdWork ccd;
+    ipcgpu::PointTetWork pit;
     // half-space collision objects (halfspace.cu, ipcgpu_set_halfspaces): parameters, flags / scan of the (plane, SVI index) range, active and
     // lagged (plane, vertex) lists, per-plane starts of the active list, energy partials
     int n_hs = 0;

@@ -377,6 +377,8 @@ class Context:
         return n.value if want else None
 
     def intersection_free(self, want=True):
+        """checkEdgeTriIntersectionIfAny: no surface edge crosses a surface triangle and no codimension-0 vertex (vCoDim == 0) lies in a
+        tetrahedron (faces included).  want=False: deferred, the count comes back with fetch_iteration (n_intersected_triangles)."""
         ok = C.c_int()
         self._ck(self.lib.ipcgpu_intersection_free(self.h, C.byref(ok) if want else None))
         return bool(ok.value) if want else None
