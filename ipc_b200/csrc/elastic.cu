@@ -565,8 +565,11 @@ __global__ void __launch_bounds__(256) k_inversion_step(ElasticArgs p, const dou
         out = (r >= 0) ? r : 1e20;
         if (per_tet) per_tet[tt] = out;
     }
-    // min over the CTA; negative/zero roots are impossible here (r>=0 or 1e20), so the ordered-uint trick is valid
-    double m = warp_min(out);
+    // min over the CTA of out + 0.0.  A bound is r >= 0 or 1e20, but r can be -0.0 (-0/c in the linear exit, +0/(2a) with a < 0 in the
+    // quadratic one), whose bits would order above every positive bound.  Energy.cpp:576-579 takes minCoeff with `<`, where either zero is
+    // the minimum wherever it lies and fails `0 < min`; adding +0.0 makes both zeros +0.0, the smallest key of the ordered-uint atomicMin
+    // (here and across ranks), so k_inversion_apply rejects it the same way.  per_tet keeps the signed value.
+    double m = warp_min(__dadd_rn(out, 0.0));
     __shared__ double sm[8];
     if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
     __syncthreads();

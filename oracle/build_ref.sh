@@ -1,7 +1,10 @@
 #!/bin/sh
 # Builds oracle/_ref/libref_pairs.so from the REFERENCE's own scalar code (MATLAB-codegen bodies of the
 # pair-distance gradients/Hessians, the EE cross-norm derivatives, the mollifier polynomial and the C2 barrier)
-# compiled from the sources where they lie under /root/reference.  The line ranges below are the pure-`double`
+# compiled from the sources where they lie under /root/reference, and oracle/_ref/libref_cubic.so from its
+# inversion-filter root finders (getSmallestPositiveRealQuadRoot / getSmallestPositiveRealCubicRoot, pure double and
+# std::complex) and its absolute-coordinate coefficient lines (a, b, c, d of computeInjectiveStepSize_3d), the latter
+# inside a shim that declares the scalars they read.  The line ranges below are the pure-`double`
 # overloads (no Eigen inside); they are streamed through sed into a scratch file OUTSIDE the repo, compiled, and
 # the scratch file is deleted -- no reference source is ever copied into this repository.  Only the .so lands in
 # oracle/_ref/ (git-ignored, travels to the GPU box).  The rest of the reference (Eigen/TBB/libigl/CCD-Wrapper
@@ -41,3 +44,28 @@ SHIM
 } > "$TMP/ref_pairs.cpp"
 $CXX -O2 -std=c++17 -fPIC -ffp-contract=off -shared -o "$OUT/libref_pairs.so" "$TMP/ref_pairs.cpp"
 echo "built $OUT/libref_pairs.so"
+G="$REF/Utils/get_feasible_steps.cpp"
+{
+  echo '#include <cmath>'
+  echo '#include <complex>'
+  echo 'namespace refsrc {'
+  echo 'using namespace std;'
+  sed -n '9,28p;75,108p' "$G"
+  echo 'void coefs(const double* X, const double* P, double slackness, double* out) {'
+  echo 'const double x1 = X[0], y1 = X[1], z1 = X[2], x2 = X[3], y2 = X[4], z2 = X[5], x3 = X[6], y3 = X[7], z3 = X[8], x4 = X[9], y4 = X[10], z4 = X[11];'
+  echo 'const double p1 = P[0], q1 = P[1], r1 = P[2], p2 = P[3], q2 = P[4], r2 = P[5], p3 = P[6], q3 = P[7], r3 = P[8], p4 = P[9], q4 = P[10], r4 = P[11];'
+  echo 'double a, b, c, d;'
+  sed -n '158,161p' "$G"
+  echo 'out[0] = a; out[1] = b; out[2] = c; out[3] = d;'
+  echo '}'
+  echo '}'
+  cat <<'SHIM'
+extern "C" {
+double ref_quad_root(double a, double b, double c, double tol) { return refsrc::getSmallestPositiveRealQuadRoot(a, b, c, tol); }
+double ref_cubic_root(double a, double b, double c, double d, double tol) { return refsrc::getSmallestPositiveRealCubicRoot(a, b, c, d, tol); }
+void ref_inversion_coefs(const double* X, const double* P, double slackness, double* out) { refsrc::coefs(X, P, slackness, out); }
+}
+SHIM
+} > "$TMP/ref_cubic.cpp"
+$CXX -O2 -std=c++17 -fPIC -ffp-contract=off -shared -o "$OUT/libref_cubic.so" "$TMP/ref_cubic.cpp"
+echo "built $OUT/libref_cubic.so"

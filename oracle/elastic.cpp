@@ -798,41 +798,75 @@ void orc_elastic_hessian_csr(const orc_mesh* m, double coef, int projectSPD, int
 }
 
 /* get_feasible_steps.cpp:9-28, :75-108 */
-static double quadRoot(double a, double b, double c, double tol)
+/* br (optional, see orc_cubic_branch): br[0] the exit, br[1] the |C| == 0 fallback, br[2] the mask of Cardano roots that pass the filter,
+ * br[3] the root kept (1..3, 0 for none) */
+static double quadRoot(double a, double b, double c, double tol, int* br = nullptr)
 {
     double t;
-    if (std::abs(a) <= tol) t = -c / b;
+    if (std::abs(a) <= tol) {
+        t = -c / b;
+        if (br) br[0] = 0;
+    }
     else {
         double desc = b * b - 4 * a * c;
         if (desc > 0) {
             t = (-b - std::sqrt(desc)) / (2 * a);
-            if (t < 0) t = (-b + std::sqrt(desc)) / (2 * a);
+            if (br) br[0] = 1;
+            if (t < 0) {
+                t = (-b + std::sqrt(desc)) / (2 * a);
+                if (br) br[0] = 2;
+            }
         }
-        else t = -1;
+        else {
+            t = -1;
+            if (br) br[0] = 3;
+        }
     }
     return t;
 }
-static double cubicRoot(double a, double b, double c, double d, double tol)
+static double cubicRoot(double a, double b, double c, double d, double tol, int* br = nullptr)
 {
     double t = -1;
-    if (std::abs(a) <= tol) t = quadRoot(b, c, d, tol);
+    if (br) br[0] = br[1] = br[2] = br[3] = 0;
+    if (std::abs(a) <= tol) t = quadRoot(b, c, d, tol, br);
     else {
         typedef std::complex<double> cd;
         cd i(0, 1);
         cd delta0(b * b - 3 * a * c, 0);
         cd delta1(2 * b * b * b - 9 * a * b * c + 27 * a * a * d, 0);
-        cd C = std::pow((delta1 + std::sqrt(delta1 * delta1 - 4.0 * delta0 * delta0 * delta0)) / 2.0, 1.0 / 3.0);
-        if (std::abs(C) == 0.0) C = std::pow((delta1 - std::sqrt(delta1 * delta1 - 4.0 * delta0 * delta0 * delta0)) / 2.0, 1.0 / 3.0);
+        cd rad = (delta1 + std::sqrt(delta1 * delta1 - 4.0 * delta0 * delta0 * delta0)) / 2.0;
+        cd C = std::pow(rad, 1.0 / 3.0);
+        if (std::abs(C) == 0.0) {
+            rad = (delta1 - std::sqrt(delta1 * delta1 - 4.0 * delta0 * delta0 * delta0)) / 2.0;
+            C = std::pow(rad, 1.0 / 3.0);
+            if (br) br[1] = 1;
+        }
+        if (br) br[0] = (std::imag(rad) == 0.0 && std::real(rad) > 0.0) ? 4 : 5; /* libstdc++'s real pow, or the complex log/polar path */
         cd u2 = (-1.0 + std::sqrt(3.0) * i) / 2.0;
         cd u3 = (-1.0 - std::sqrt(3.0) * i) / 2.0;
         cd t1 = (b + C + delta0 / C) / (-3.0 * a);
         cd t2 = (b + u2 * C + delta0 / (u2 * C)) / (-3.0 * a);
         cd t3 = (b + u3 * C + delta0 / (u3 * C)) / (-3.0 * a);
-        if ((std::abs(std::imag(t1)) < tol) && (std::real(t1) > 0)) t = std::real(t1);
-        if ((std::abs(std::imag(t2)) < tol) && (std::real(t2) > 0) && ((std::real(t2) < t) || (t < 0))) t = std::real(t2);
-        if ((std::abs(std::imag(t3)) < tol) && (std::real(t3) > 0) && ((std::real(t3) < t) || (t < 0))) t = std::real(t3);
+        const bool p1 = (std::abs(std::imag(t1)) < tol) && (std::real(t1) > 0);
+        const bool p2 = (std::abs(std::imag(t2)) < tol) && (std::real(t2) > 0);
+        const bool p3 = (std::abs(std::imag(t3)) < tol) && (std::real(t3) > 0);
+        int k = 0;
+        if (p1) t = std::real(t1), k = 1;
+        if (p2 && ((std::real(t2) < t) || (t < 0))) t = std::real(t2), k = 2;
+        if (p3 && ((std::real(t3) < t) || (t < 0))) t = std::real(t3), k = 3;
+        if (br) br[2] = (int)p1 | (int)p2 << 1 | (int)p3 << 2, br[3] = k;
     }
     return t;
+}
+
+int orc_cubic_branch(double a, double b, double c, double d, double tol, double* t, int* fallback, int* passed, int* kept)
+{
+    int br[4];
+    *t = cubicRoot(a, b, c, d, tol, br);
+    *fallback = br[1];
+    *passed = br[2];
+    *kept = br[3];
+    return br[0];
 }
 static inline double det3c(const double* a, const double* b, const double* c)
 {

@@ -71,6 +71,11 @@ void orc_elastic_hessian_csr(const orc_mesh* m, double coef, int projectSPD, int
     const int* ia, const int* ja, int index_base, double* a, int nthreads);
 /* get_feasible_steps.cpp:110-172 + Energy.cpp:565-581 ; p interleaved */
 void orc_inversion_step(const orc_mesh* m, const double* p, double slack, double* per_tet /*nullable*/, double* alpha_inout);
+/* getSmallestPositiveRealCubicRoot (get_feasible_steps.cpp:75-108) on given coefficients: the root in *t (negative for none) and the exit
+ * taken: 0 linear (|a|, |b| <= tol), 1 / 2 the quadratic's first / second root, 3 the quadratic without a real root (desc <= 0), 4 / 5
+ * Cardano with C from the real pow of a positive real radicand / from the complex pow.  fallback: the |C| == 0 branch ran; passed: mask of
+ * the Cardano roots t1..t3 with |Im t| < tol and Re t > 0; kept: the one returned (1..3, 0 for none). */
+int orc_cubic_branch(double a, double b, double c, double d, double tol, double* t, int* fallback, int* passed, int* kept);
 
 /* LinSysSolver.hpp:46-150: builds the upper-triangular block CSR pattern from vertex
  * adjacency given as CSR (nbr_ptr/nbr sorted ascending, no self). Returns nnz; if ia==NULL only counts. */

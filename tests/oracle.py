@@ -114,6 +114,20 @@ def svd3_branch(F):
     return SVD3_EXITS[ex.value], so.value, bool(re.value)
 
 
+CUBIC_EXITS = ("linear", "quad_first", "quad_second", "quad_none", "cardano_real", "cardano_complex")
+
+
+def cubic_branch(a, b, c, d, tol=1e-6):
+    """(t, exit, fallback, passed, kept) of the restated getSmallestPositiveRealCubicRoot on the given coefficients: the root (negative
+    for none), the exit's name (CUBIC_EXITS), whether the |C| == 0 fallback ran, the mask of Cardano roots with |Im t| < tol and Re t > 0,
+    and the root kept (1..3, 0 for none)"""
+    t, fb, ps, kp = C.c_double(), C.c_int(), C.c_int(), C.c_int()
+    f = lib().orc_cubic_branch
+    f.argtypes = [C.c_double] * 5 + [_dp, _ip, _ip, _ip]
+    ex = f(a, b, c, d, tol, C.byref(t), C.byref(fb), C.byref(ps), C.byref(kp))
+    return t.value, CUBIC_EXITS[ex], bool(fb.value), ps.value, kp.value
+
+
 def psi(et, S, mu, lam):
     S = np.ascontiguousarray(S, dtype=np.float64)
     E = C.c_double()
