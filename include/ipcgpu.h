@@ -371,6 +371,11 @@ int ipcgpu_check_inversion(ipcgpu_ctx* ctx, int* n_inverted);
  * positions; without codimension-0 vertices the second test launches nothing.  With several ranks each rank tests its own triangles and
  * tets.  NULL: deferred, reported by ipcgpu_fetch_iteration. */
 int ipcgpu_intersection_free(ipcgpu_ctx* ctx, int* ok);
+/* TEST HOOK.  enable != 0: every later ipcgpu_intersection_free also writes, on the device, a flag per surface triangle (1 = an edge crosses
+ * it) and the number of codimension-0 vertices inside each tetrahedron; enable = 0 frees those buffers and leaves the check as it was (the
+ * same launches).  tri_flags (nSF) and tet_hits (nT), nullable, receive the last check's values after a synchronisation; they need the
+ * hook on, and are read before `enable` is applied. */
+int ipcgpu_safeguard_debug_flags(ipcgpu_ctx* ctx, int enable, int* tri_flags, int* tet_hits);
 
 /* ---- CCD step bound (Tight-Inclusion), Optimizer.cpp:1884-2040 ----------------------------------------------------- */
 /* capacity (pairs) of the device CCD candidate list; default 2^23 */

@@ -161,6 +161,7 @@ int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity);
 int pattern_update(ipcgpu_ctx* ctx, const ipcgpu::BarrierArgs& lists, bool with_friction);
 int safeguard_inversion(ipcgpu_ctx* ctx);
 int safeguard_intersections(ipcgpu_ctx* ctx);
+int safeguard_debug_flags(ipcgpu_ctx* ctx, bool on); // test hook: per-triangle flags and per-tet point counts of the intersection check
 int safeguard_set_points(ipcgpu_ctx* ctx, const int* vCoDim); // the codimension-0 vertices of the point-in-tetrahedron check (vCoDim nullable)
 
 // A gradient / Hessian term.  NULL output: the term on `chain`; host output: the caller's array in, the term added on the main stream,

@@ -236,6 +236,20 @@ int ipcgpu_intersection_free(ipcgpu_ctx* ctx, int* ok)
     return IPCGPU_OK;
 }
 
+int ipcgpu_safeguard_debug_flags(ipcgpu_ctx* ctx, int enable, int* tri_flags, int* tet_hits)
+{
+    ENTER(kSerial);
+    if (tri_flags || tet_hits) {
+        REQUIRE(ctx->debug_safeguard_flags, IPCGPU_ERR_STATE, "ipcgpu_safeguard_debug_flags(ctx, 1, ...) before the check");
+        CK(cudaStreamSynchronize(ctx->stream));
+        if (tri_flags && ctx->nSF > 0) CK(cudaMemcpy(tri_flags, ctx->dbg_tri_flags.p, sizeof(int) * ctx->nSF, cudaMemcpyDeviceToHost));
+        if (tet_hits && ctx->nT > 0) CK(cudaMemcpy(tet_hits, ctx->dbg_tet_hits.p, sizeof(int) * ctx->nT, cudaMemcpyDeviceToHost));
+    }
+    const int rc = safeguard_debug_flags(ctx, enable != 0);
+    REQUIRE(rc == 0, rc, "safeguard debug buffer allocation failed");
+    return IPCGPU_OK;
+}
+
 // ---- step control: CFL branch and line search (step_control.cu holds the decision kernel) ----------------------------------------
 // Each loop body and loop condition is written once: a sequence of entry points plus one step_decide.  Outside a capture the
 // host loops and reads the decision word (one synchronisation per decision); inside one the body is captured into a conditional node.

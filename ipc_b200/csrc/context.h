@@ -260,6 +260,8 @@ struct ipcgpu_ctx {
     std::vector<int> h_SVI;                // host copy (pSize of the swept build is a serial host sum, SpatialHash.hpp:603-612)
     double debug_prune_seed = -1.0;        // test hook, see ipcgpu_ccd_debug_seed_bound
     long long debug_ti_budget = -1;        // test hook, see ipcgpu_ccd_debug_thread_budget
+    bool debug_safeguard_flags = false;    // test hook, see ipcgpu_safeguard_debug_flags
+    ipcgpu::DevBuf<int> dbg_tri_flags, dbg_tet_hits;
 
     // gradient gather map (local tets)
     ipcgpu::DevBuf<int> inc_ptr, inc;

@@ -157,16 +157,19 @@ DEV void full_piv_solve3(double (&m)[3][3], const double* b, double* x)
     int rank = 0;
     for (int k = 0; k < nz; ++k)
         if (fabs(m[k][k]) > maxpiv * 2.220446049250313e-16 * 3.0) ++rank;
-    for (int i = 1; i < 3; ++i)
-        for (int j = 0; j < i; ++j) rhs[i] -= m[i][j] * rhs[j];
-    double y[3] = { 0.0, 0.0, 0.0 };
-    for (int i = rank - 1; i >= 0; --i) {
-        double s = rhs[i];
-        for (int j = i + 1; j < rank; ++j) s -= m[i][j] * y[j];
-        y[i] = s / m[i][i];
-    }
+    // both triangular solves by columns, as Eigen's triangular_solve_vector runs them on the runtime-sized blocks FullPivLU::_solve_impl
+    // passes: a solved entry is subtracted from the rows it feeds, an exactly zero one is skipped.  Row 0 of the back substitution rounds
+    // as (r0 - U02 y2) - U01 y1 (DESIGN 3.6).
+    for (int j = 0; j < 3; ++j)
+        if (rhs[j] != 0.0)
+            for (int i = j + 1; i < 3; ++i) rhs[i] -= rhs[j] * m[i][j];
+    for (int j = rank - 1; j >= 0; --j)
+        if (rhs[j] != 0.0) {
+            rhs[j] /= m[j][j];
+            for (int i = 0; i < j; ++i) rhs[i] -= rhs[j] * m[i][j];
+        }
     x[0] = x[1] = x[2] = 0.0;
-    for (int k = 0; k < 3; ++k) x[cq[k]] = y[k];
+    for (int k = 0; k < rank; ++k) x[cq[k]] = rhs[k];
 }
 
 // IglUtils::segTriIntersect (IglUtils.hpp:214-265)
@@ -191,8 +194,9 @@ DEV bool seg_tri_intersect(const double* ve0, const double* ve1, const double* v
 // one warp per query triangle (kPairQueriesPerWarp in a row): scan the edge grid for boxes that overlap the triangle's box, run the
 // exact test on the lanes that hold a candidate, count the triangles with at least one intersecting edge (the reference stops at
 // the first per triangle: same count)
+// tri_flags (nullable, test hook ipcgpu_safeguard_debug_flags): 1 / 0 per triangle of [first, last)
 __global__ void __launch_bounds__(256) k_tri_edge_intersect(SurfArgs s, const Grid* __restrict__ gp, SortedGrid eg, const Box* __restrict__ tboxes, int first, int last,
-    int* __restrict__ n_hit)
+    int* __restrict__ n_hit, int* __restrict__ tri_flags)
 {
     const int lane = threadIdx.x & 31;
     const Grid g = *gp;
@@ -224,7 +228,9 @@ __global__ void __launch_bounds__(256) k_tri_edge_intersect(SurfArgs s, const Gr
             }
             if (seg_tri_intersect(p0, p1, t[0], t[1], t[2])) any = true;
         });
-        if (__any_sync(0xffffffffu, any) && lane == 0) atomicAdd(n_hit, 1);
+        const bool hit = __any_sync(0xffffffffu, any);
+        if (hit && lane == 0) atomicAdd(n_hit, 1);
+        if (tri_flags && lane == 0) tri_flags[f] = hit ? 1 : 0;
     }
 }
 
@@ -305,9 +311,10 @@ __global__ void __launch_bounds__(256) k_pit_keys(const double* __restrict__ V, 
 
 // one thread per tetrahedron [t_begin, t_end) (every tet: no Dirichlet and no mu / lambda filter, the reference loops over all of F): the
 // rows of cells its box covers are consecutive key ranges of the sorted points, found by binary search; every point in them that lies in
-// the tet's box (inclusive, as the reference compares) gets the exact test.  Counts (point, tet) pairs.
+// the tet's box (inclusive, as the reference compares) gets the exact test.  Counts (point, tet) pairs; tet_hits (nullable, test hook
+// ipcgpu_safeguard_debug_flags) receives each tet's own count.
 __global__ void __launch_bounds__(256) k_points_in_tets(ElasticArgs p, const PointGrid* __restrict__ gp, const unsigned* __restrict__ key, const int* __restrict__ id, int n,
-    int* __restrict__ n_hit)
+    int* __restrict__ n_hit, int* __restrict__ tet_hits)
 {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     int hits = 0;
@@ -355,6 +362,7 @@ __global__ void __launch_bounds__(256) k_points_in_tets(ElasticArgs p, const Poi
                     }
                 }
         }
+        if (tet_hits) tet_hits[tt] = hits;
     }
     const int tot = warp_sum(hits);
     if (tot && (threadIdx.x & 31) == 0) atomicAdd(n_hit, tot);
@@ -389,6 +397,20 @@ __global__ void __launch_bounds__(256) k_count_inverted(ElasticArgs p, int* __re
 } // namespace ipcgpu
 
 using namespace ipcgpu;
+
+// test hook behind ipcgpu_safeguard_debug_flags: on, the intersection checks also write per-triangle flags (nSF) and per-tet point counts (nT)
+int safeguard_debug_flags(ipcgpu_ctx* ctx, bool on)
+{
+    ctx->debug_safeguard_flags = false;
+    if (!on) {
+        ctx->dbg_tri_flags.release();
+        ctx->dbg_tet_hits.release();
+        return 0;
+    }
+    if (!ctx->dbg_tri_flags.reserve(std::max(ctx->nSF, 1)) || !ctx->dbg_tet_hits.reserve(std::max(ctx->nT, 1))) return IPCGPU_ERR_CUDA;
+    ctx->debug_safeguard_flags = true;
+    return 0;
+}
 
 // enqueue the inversion count of this rank's tets into IterState::checks[0]
 int safeguard_inversion(ipcgpu_ctx* ctx)
@@ -436,12 +458,22 @@ int safeguard_intersections(ipcgpu_ctx* ctx)
     const SurfArgs s = surf_args(ctx);
     int* cnt = &ctx->iter.p->checks[1];
     if (cudaMemsetAsync(cnt, 0, sizeof(int), st) != cudaSuccess) return IPCGPU_ERR_CUDA;
+    int* tri_flags = nullptr;
+    int* tet_hits = nullptr;
+    if (ctx->debug_safeguard_flags) { // (test hook: every flag and count of this check, zeros where nothing ran)
+        if (!ctx->dbg_tri_flags.reserve(std::max(ctx->nSF, 1)) || !ctx->dbg_tet_hits.reserve(std::max(ctx->nT, 1))) return IPCGPU_ERR_CUDA;
+        tri_flags = ctx->dbg_tri_flags.p;
+        tet_hits = ctx->dbg_tet_hits.p;
+        if (cudaMemsetAsync(tri_flags, 0, ctx->dbg_tri_flags.n * sizeof(int), st) != cudaSuccess
+            || cudaMemsetAsync(tet_hits, 0, ctx->dbg_tet_hits.n * sizeof(int), st) != cudaSuccess)
+            return IPCGPU_ERR_CUDA;
+    }
     if (s.nSF > 0 && s.nSE > 0) {
         int rc = boxes_and_grid(ctx, 0.0, false);
         if (rc) return rc;
         const SortedGrid eg = edge_grid(ctx);
         const int f0 = (int)((long long)s.nSF * ctx->rank / ctx->nranks), f1 = (int)((long long)s.nSF * (ctx->rank + 1) / ctx->nranks);
-        if (f1 > f0) k_tri_edge_intersect<<<nblk(f1 - f0, 8 * kPairQueriesPerWarp), 256, 0, st>>>(s, w.grid.p, eg, w.tbox.p, f0, f1, cnt);
+        if (f1 > f0) k_tri_edge_intersect<<<nblk(f1 - f0, 8 * kPairQueriesPerWarp), 256, 0, st>>>(s, w.grid.p, eg, w.tbox.p, f0, f1, cnt, tri_flags);
         ++ctx->launches;
         if (cudaGetLastError() != cudaSuccess) return IPCGPU_ERR_CUDA;
     }
@@ -452,7 +484,7 @@ int safeguard_intersections(ipcgpu_ctx* ctx)
     k_pit_keys<<<nblk(pw.n, 256), 256, 0, st>>>(ctx->V.p, ctx->nV, pw.pts.p, pw.n, pw.grid.p, pw.key.p, pw.id.p);
     size_t bytes = pw.sort_bytes;
     if (cub::DeviceRadixSort::SortPairs(pw.sort_tmp.p, bytes, pw.key.p, pw.key_sorted.p, pw.id.p, pw.id_sorted.p, pw.n, 0, 24, st) != cudaSuccess) return IPCGPU_ERR_CUDA;
-    k_points_in_tets<<<nblk(p.t_end - p.t_begin, 256), 256, 0, st>>>(p, pw.grid.p, pw.key_sorted.p, pw.id_sorted.p, pw.n, cnt);
+    k_points_in_tets<<<nblk(p.t_end - p.t_begin, 256), 256, 0, st>>>(p, pw.grid.p, pw.key_sorted.p, pw.id_sorted.p, pw.n, cnt, tet_hits);
     ctx->launches += 4; // (the sort counts as one)
     return cudaGetLastError() == cudaSuccess ? 0 : IPCGPU_ERR_CUDA;
 }

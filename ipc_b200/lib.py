@@ -40,6 +40,7 @@ SIGNATURES = {
     "ipcgpu_step_bound_set": (C.c_int, [_ctxp, C.c_double]),
     "ipcgpu_check_inversion": (C.c_int, [_ctxp, _ip]),
     "ipcgpu_intersection_free": (C.c_int, [_ctxp, _ip]),
+    "ipcgpu_safeguard_debug_flags": (C.c_int, [_ctxp, C.c_int, _ip, _ip]),
     "ipcgpu_constraint_set_sizes": (C.c_int, [_ctxp, _ip, _ip, _ip]),
     "ipcgpu_ccd_debug_seed_bound": (C.c_int, [_ctxp, C.c_double]),
     "ipcgpu_ccd_debug_thread_budget": (C.c_int, [_ctxp, C.c_int64]),
@@ -383,6 +384,13 @@ class Context:
         self._ck(self.lib.ipcgpu_intersection_free(self.h, C.byref(ok) if want else None))
         return bool(ok.value) if want else None
 
+    def safeguard_debug_flags(self, enable, read=False):
+        """test hook: enable the per-triangle flags / per-tet point counts of the intersection check; read=True returns the last check's
+        (tri_flags[nSF], tet_hits[nT]) before applying `enable`"""
+        out = (np.zeros(max(self.nSF, 1), np.int32), np.zeros(max(self.nT, 1), np.int32)) if read else (None, None)
+        self._ck(self.lib.ipcgpu_safeguard_debug_flags(self.h, int(enable), *(None if x is None else _i(x) for x in out)))
+        return (out[0][: self.nSF], out[1][: self.nT]) if read else None
+
     def step_bound_set(self, alpha):
         self._ck(self.lib.ipcgpu_step_bound_set(self.h, float(alpha)))
 
@@ -656,6 +664,7 @@ class Context:
     # ---- contact ------------------------------------------------------------------------------
     def set_surface(self, SVI, SFEdges, SF_soa, vCoDim=None):
         SVI, SE, SF = i32(SVI).ravel(), i32(SFEdges).ravel(), i32(SF_soa).ravel()
+        self.nSF = SF.size // 3
         self._ck(self.lib.ipcgpu_set_surface(self.h, SVI.size, _i(SVI), SE.size // 2, _i(SE), SF.size // 3, _i(SF), _i(i32(vCoDim))))
 
     def set_obstacle_tail(self, first_obstacle_vertex, ee_through_vf_routine=1):

@@ -11,7 +11,8 @@
  * the determinant evaluated exactly with floating-point expansions (two-sum / two-product, grow-expansion, scale-expansion).
  * Pinned by tests/test_oracle_intersect.py against exact rational arithmetic (Python fractions) incl. exactly coplanar inputs.
  * Eigen's fullPivLu (IglUtils.hpp:258) is restated as Gaussian elimination with full pivoting in Eigen's pivot order
- * (first maximum in column-major order of the remaining corner); unpinned by the reference's tests, unique up to rounding.
+ * (first maximum in column-major order of the remaining corner), rank threshold 3 eps * max pivot, and both triangular solves by columns
+ * as Eigen 3.4 runs them; pinned by tests/test_safeguard_regimes.py to a Python restatement of the same operations, bit for bit.
  */
 #include "oracle.h"
 #include <algorithm>
@@ -89,8 +90,11 @@ int prod_diff(double x, double y, double z, double w, double* h)
     return expansion_sum(2, e, 2, f, h);
 }
 
-/* exact sign of det [a-d; b-d; c-d] via the 4x4 cofactor expansion on the UNtranslated coordinates */
-int orient3d_exact(const double* pa, const double* pb, const double* pc, const double* pd)
+/* exact sign of det [a-d; b-d; c-d] via the 4x4 cofactor expansion on the UNtranslated coordinates.  The four scaled terms are summed in
+ * the device's order (adet + bdet, then every component of cdet and of ddet grown in); lens (nullable) receives the component counts the
+ * device's fixed buffers must hold: cda, dab, abc, bcd, the longest pairwise sum before them, adet, bdet, cdet, ddet, the longest running
+ * sum and the final sum (orc_orient3d_trace) */
+int orient3d_exact(const double* pa, const double* pb, const double* pc, const double* pd, int* lens = nullptr)
 {
     double ab[4], bc[4], cd[4], da[4], ac[4], bd[4];
     const int nab = prod_diff(pa[0], pb[1], pb[0], pa[1], ab), nbc = prod_diff(pb[0], pc[1], pc[0], pb[1], bc), ncd = prod_diff(pc[0], pd[1], pd[0], pc[1], cd);
@@ -98,29 +102,33 @@ int orient3d_exact(const double* pa, const double* pb, const double* pc, const d
     double t[16], cda[16], dab[16], abc[16], bcd[16], nac_[4], nbd_[4];
     for (int i = 0; i < nac; ++i) nac_[i] = -ac[i];
     for (int i = 0; i < nbd; ++i) nbd_[i] = -bd[i];
-    int nt = expansion_sum(ncd, cd, nda, da, t);
+    int nt = expansion_sum(ncd, cd, nda, da, t), ntmax = nt;
     const int ncda = expansion_sum(nt, t, nac, ac, cda);
-    nt = expansion_sum(nda, da, nab, ab, t);
+    nt = expansion_sum(nda, da, nab, ab, t), ntmax = std::max(ntmax, nt);
     const int ndab = expansion_sum(nt, t, nbd, bd, dab);
-    nt = expansion_sum(nab, ab, nbc, bc, t);
+    nt = expansion_sum(nab, ab, nbc, bc, t), ntmax = std::max(ntmax, nt);
     const int nabc = expansion_sum(nt, t, nac, nac_, abc);
-    nt = expansion_sum(nbc, bc, ncd, cd, t);
+    nt = expansion_sum(nbc, bc, ncd, cd, t), ntmax = std::max(ntmax, nt);
     const int nbcd = expansion_sum(nt, t, nbd, nbd_, bcd);
-    double adet[32], bdet[32], cdet[32], ddet[32], s1[64], s2[64], det[128];
+    double adet[32], bdet[32], cdet[32], ddet[32], det[128], nxt[128];
     const int na = scale_expansion(nbcd, bcd, pa[2], adet), nb = scale_expansion(ncda, cda, -pb[2], bdet);
     const int nc = scale_expansion(ndab, dab, pc[2], cdet), nd = scale_expansion(nabc, abc, -pd[2], ddet);
-    const int n1 = expansion_sum(na, adet, nb, bdet, s1), n2 = expansion_sum(nc, cdet, nd, ddet, s2);
-    const int n = expansion_sum(n1, s1, n2, s2, det);
+    int n = expansion_sum(na, adet, nb, bdet, det), nmax = n;
+    for (int j = 0; j < nc + nd; ++j) {
+        n = grow_expansion(n, det, j < nc ? cdet[j] : ddet[j - nc], nxt);
+        std::memcpy(det, nxt, sizeof(double) * n);
+        nmax = std::max(nmax, n);
+    }
+    if (lens) {
+        const int l[11] = { ncda, ndab, nabc, nbcd, ntmax, na, nb, nc, nd, nmax, n };
+        std::memcpy(lens, l, sizeof(l));
+    }
     const double top = det[n - 1]; /* the largest-magnitude component carries the sign */
     return (top > 0.0) - (top < 0.0);
 }
 
-} // namespace
-
-extern "C" {
-
-/* sign (+1 / 0 / -1) of orient3d(pa, pb, pc, pd) in Shewchuk's convention (positive when pd lies below the plane pa pb pc) */
-int orc_orient3d(const double* pa, const double* pb, const double* pc, const double* pd)
+/* the floating-point filter: +1 / -1 when it decides, 2 when the input goes to the exact stage */
+int orient3d_filter(const double* pa, const double* pb, const double* pc, const double* pd)
 {
     const double adx = pa[0] - pd[0], bdx = pb[0] - pd[0], cdx = pc[0] - pd[0];
     const double ady = pa[1] - pd[1], bdy = pb[1] - pd[1], cdy = pc[1] - pd[1];
@@ -134,9 +142,32 @@ int orc_orient3d(const double* pa, const double* pb, const double* pc, const dou
     const double errbound = 1.7763568394002505e-15 * permanent;
     if (det > errbound) return 1;
     if (-det > errbound) return -1;
-    return orient3d_exact(pa, pb, pc, pd);
+    return 2;
+}
+
+} // namespace
+
+extern "C" {
+
+/* sign (+1 / 0 / -1) of orient3d(pa, pb, pc, pd) in Shewchuk's convention (positive when pd lies below the plane pa pb pc) */
+int orc_orient3d(const double* pa, const double* pb, const double* pc, const double* pd)
+{
+    const int f = orient3d_filter(pa, pb, pc, pd);
+    return f != 2 ? f : orient3d_exact(pa, pb, pc, pd);
 }
 int orc_orient3d_exact(const double* pa, const double* pb, const double* pc, const double* pd) { return orient3d_exact(pa, pb, pc, pd); }
+/* orc_orient3d with the path it took: info[0] = 1 when the filter decided (info[1..11] = 0), else 0 and info[1..11] the component counts of
+ * the exact stage (cda, dab, abc, bcd, longest pairwise sum, adet, bdet, cdet, ddet, longest running sum, final sum) */
+int orc_orient3d_trace(const double* pa, const double* pb, const double* pc, const double* pd, int* info)
+{
+    std::memset(info, 0, 12 * sizeof(int));
+    const int f = orient3d_filter(pa, pb, pc, pd);
+    if (f != 2) {
+        info[0] = 1;
+        return f;
+    }
+    return orient3d_exact(pa, pb, pc, pd, info + 1);
+}
 
 /* x = M^-1 b by Gaussian elimination with full pivoting (Eigen::FullPivLU order); M column-major 3x3.  returns the rank */
 static int full_piv_solve3(const double* Mcm, const double* b, double* x)
@@ -166,34 +197,45 @@ static int full_piv_solve3(const double* Mcm, const double* b, double* x)
     int rank = 0;
     for (int k = 0; k < nz; ++k)
         if (std::fabs(m[k][k]) > maxpiv * 2.220446049250313e-16 * 3.0) ++rank;
-    for (int i = 1; i < 3; ++i) /* forward: unit lower */
-        for (int j = 0; j < i; ++j) rhs[i] -= m[i][j] * rhs[j];
-    double y[3] = { 0, 0, 0 };
-    for (int i = rank - 1; i >= 0; --i) { /* back substitution on the leading rank x rank block */
-        double s = rhs[i];
-        for (int j = i + 1; j < rank; ++j) s -= m[i][j] * y[j];
-        y[i] = s / m[i][i];
-    }
+    /* both triangular solves by columns, as Eigen's triangular_solve_vector does for a column-major block (FullPivLU::_solve_impl passes
+     * runtime-sized blocks, so nothing is unrolled): a solved entry is subtracted from every row above/below it at once, and an entry that is
+     * exactly zero is skipped.  Row 0 of the back substitution thus rounds as (r0 - U02 y2) - U01 y1. */
+    for (int j = 0; j < 3; ++j) /* forward: unit lower */
+        if (rhs[j] != 0.0)
+            for (int i = j + 1; i < 3; ++i) rhs[i] -= rhs[j] * m[i][j];
+    for (int j = rank - 1; j >= 0; --j) /* back substitution on the leading rank x rank block */
+        if (rhs[j] != 0.0) {
+            rhs[j] /= m[j][j];
+            for (int i = 0; i < j; ++i) rhs[i] -= rhs[j] * m[i][j];
+        }
     x[0] = x[1] = x[2] = 0.0;
-    for (int k = 0; k < 3; ++k) x[cq[k]] = y[k];
+    for (int k = 0; k < rank; ++k) x[cq[k]] = rhs[k];
     return rank;
 }
 
-/* IglUtils::segTriIntersect (IglUtils.hpp:214-265, USE_PREDICATES) */
-int orc_seg_tri_intersect(const double* ve0, const double* ve1, const double* vt0, const double* vt1, const double* vt2)
+/* IglUtils::segTriIntersect (IglUtils.hpp:214-265, USE_PREDICATES) with the path it took: exit 0 = an endpoint in the triangle's plane,
+ * 1 = both endpoints on one side, 2 = solved (rank and uvt filled; both nullable) */
+int orc_seg_tri_trace(const double* ve0, const double* ve1, const double* vt0, const double* vt1, const double* vt2, int* exit, int* rank, double* uvt)
 {
     const int o1 = orc_orient3d(vt0, vt1, vt2, ve0), o2 = orc_orient3d(vt0, vt1, vt2, ve1);
-    if (o1 == 0 || o2 == 0) return 0; /* coplanar: detected through d(EE) = 0 or d(PT) = 0 instead */
-    if (o1 == o2) return 0;           /* the edge is on one side of the triangle's plane */
-    double M[9], b[3], uvt[3];
+    *exit = (o1 == 0 || o2 == 0) ? 0 : (o1 == o2 ? 1 : 2);
+    if (*exit != 2) return 0; /* coplanar: detected through d(EE) = 0 or d(PT) = 0 instead; or the edge is on one side of the plane */
+    double M[9], b[3], x[3];
     for (int i = 0; i < 3; ++i) {
         M[i] = vt1[i] - vt0[i];
         M[3 + i] = vt2[i] - vt0[i];
         M[6 + i] = ve0[i] - ve1[i];
         b[i] = ve0[i] - vt0[i];
     }
-    full_piv_solve3(M, b, uvt);
-    return (uvt[0] >= 0.0 && uvt[1] >= 0.0 && uvt[0] + uvt[1] <= 1.0 && uvt[2] >= 0.0 && uvt[2] <= 1.0) ? 1 : 0;
+    const int r = full_piv_solve3(M, b, x);
+    if (rank) *rank = r;
+    if (uvt) std::memcpy(uvt, x, sizeof(x));
+    return (x[0] >= 0.0 && x[1] >= 0.0 && x[0] + x[1] <= 1.0 && x[2] >= 0.0 && x[2] <= 1.0) ? 1 : 0;
+}
+int orc_seg_tri_intersect(const double* ve0, const double* ve1, const double* vt0, const double* vt1, const double* vt2)
+{
+    int exit;
+    return orc_seg_tri_trace(ve0, ve1, vt0, vt1, vt2, &exit, nullptr, nullptr);
 }
 
 /* SelfCollisionHandler::checkEdgeTriIntersectionIfAny (:3254-3296): 1 = intersection free.  The candidate edges of a triangle come from a

@@ -213,8 +213,13 @@ int orc_meshco_ccd_full(const orc_surf* s, const orc_obstacle* o, const double* 
 /* igl::predicates::orient3d restated (filter + exact expansion arithmetic): +1 / 0 / -1 */
 int orc_orient3d(const double* pa, const double* pb, const double* pc, const double* pd);
 int orc_orient3d_exact(const double* pa, const double* pb, const double* pc, const double* pd);
+/* orc_orient3d and its path: info[0] = 1 if the filter decided; else info[1..11] = component counts of the exact stage (cda, dab, abc, bcd,
+ * longest pairwise sum, adet, bdet, cdet, ddet, longest running sum, final sum), summed in the device's order */
+int orc_orient3d_trace(const double* pa, const double* pb, const double* pc, const double* pd, int* info /* 12 */);
 /* IglUtils::segTriIntersect (IglUtils.hpp:214-265) */
 int orc_seg_tri_intersect(const double* ve0, const double* ve1, const double* vt0, const double* vt1, const double* vt2);
+/* the same with its exit (0 coplanar endpoint, 1 one side, 2 solved), and for exit 2 the rank and uvt of the full-pivot solve (nullable) */
+int orc_seg_tri_trace(const double* ve0, const double* ve1, const double* vt0, const double* vt1, const double* vt2, int* exit, int* rank, double* uvt);
 /* SelfCollisionHandler::checkEdgeTriIntersectionIfAny (:3254-3296): 1 = intersection free; hits = intersected triangles */
 int orc_intersection_free(const orc_surf* s, double cell, int* hits, int* tri_flags /* nSF, nullable */, int nthreads);
 /* Mesh::checkInversion (Mesh.cpp:715-763): tets with mu, lambda != 0 and det(current edge matrix) < 0 */

@@ -449,9 +449,28 @@ def orient3d(a, b, c, d_, exact=False):
     return int(f(d(a), d(b), d(c), d(d_)))
 
 
+ORIENT3D_TRACE_FIELDS = ("cda", "dab", "abc", "bcd", "pair_sum", "adet", "bdet", "cdet", "ddet", "running_sum", "det")
+
+
+def orient3d_trace(a, b, c, d_):
+    """(sign, filter decided, {component counts of the exact stage}; empty when the filter decided)"""
+    a, b, c, d_ = (np.ascontiguousarray(x, dtype=np.float64) for x in (a, b, c, d_))
+    info = np.zeros(12, np.int32)
+    s = int(lib().orc_orient3d_trace(d(a), d(b), d(c), d(d_), i(info)))
+    return s, bool(info[0]), ({} if info[0] else dict(zip(ORIENT3D_TRACE_FIELDS, info[1:].tolist())))
+
+
 def seg_tri_intersect(e0, e1, t0, t1, t2):
     v = [np.ascontiguousarray(x, dtype=np.float64) for x in (e0, e1, t0, t1, t2)]
     return int(lib().orc_seg_tri_intersect(*[d(x) for x in v]))
+
+
+def seg_tri_trace(e0, e1, t0, t1, t2):
+    """(decision, exit: 0 coplanar endpoint / 1 one side / 2 solved, rank, uvt) -- rank and uvt only for exit 2"""
+    v = [np.ascontiguousarray(x, dtype=np.float64) for x in (e0, e1, t0, t1, t2)]
+    ex, rk, uvt = C.c_int(), C.c_int(-1), np.full(3, np.nan)
+    r = int(lib().orc_seg_tri_trace(*[d(x) for x in v], C.byref(ex), C.byref(rk), d(uvt)))
+    return r, ex.value, (rk.value if ex.value == 2 else None), (uvt if ex.value == 2 else None)
 
 
 # ---- kinematic mesh obstacles: MeshCO<3> (oracle/meshco.cpp) ----------------------------------------------------------------------
