@@ -50,7 +50,8 @@ enum {
     IPCGPU_ERR_STATE = 7,
     IPCGPU_ERR_LINE_SEARCH = 8, /* step 0: a line search whose entry state fails a safeguard (the reference loops forever, Optimizer.cpp:2710-2811),
                                    or a zero step bound (Optimizer.cpp:2031-2033 would exit(-1)) */
-    IPCGPU_ERR_SOLVE = 9 /* ipcgpu_solve_pcg_multilevel: a domain matrix of the preconditioner has a pivot <= 0 (the matrix is not positive definite) */
+    IPCGPU_ERR_SOLVE = 9 /* ipcgpu_solve_pcg_multilevel: a domain matrix of the preconditioner has a pivot <= 0 (the matrix is not positive definite);
+                            a deferred solve: that, or a non-finite residual (ipcgpu_solve_info, ipcgpu_fetch_iteration) */
 };
 
 enum { IPCGPU_NEOHOOKEAN = 0, IPCGPU_FIXED_COROT = 1 };
@@ -533,7 +534,15 @@ int ipcgpu_ccd_debug_thread_budget(ipcgpu_ctx* ctx, int64_t boxes);
  * preconditioned CG on the upper-triangular CSR.  rhs == NULL solves H p = -g with the device-resident gradient; x == NULL keeps the
  * solution on the device; adopt_as_search_dir != 0 makes it the search direction of the step-bound stages (as if uploaded by
  * ipcgpu_set_search_dir; mean|p| of SpatialHash.hpp:603-612 is then a fixed-order device sum).  Single rank.
- * iters / rel_residual (nullable) report the iteration count and |r| / |b|. */
+ * iters / rel_residual (nullable) report the iteration count and |r| / |b|.  The residual is tested every 25 iterations: the loop stops at
+ * sqrt(rr) <= rel_tol sqrt(bb), at max_iter or on a NaN residual (returned as IPCGPU_OK with that residual).  Both triangles' row structure
+ * is built on the device, again whenever the pattern changed (ipcgpu_update_pattern), with nothing on the host.
+ * Deferred form: rhs, x, iters and rel_residual all NULL.  Nothing is returned but errors of the call itself; the result is read by
+ * ipcgpu_solve_info, and a failure (a non-finite residual; a pivot <= 0 of the multilevel preconditioner) is reported there and by
+ * ipcgpu_fetch_iteration as IPCGPU_ERR_SOLVE, and a line search started after it runs nothing (V stays V0; its status is IPCGPU_ERR_SOLVE).
+ * It is the only form accepted inside ipcgpu_capture_begin / _end (others: IPCGPU_ERR_STATE): the Krylov loops become conditional graph
+ * nodes and nothing synchronises; rel_tol and max_iter are baked into the graph.  Run the solver once outside a capture first (lazy
+ * allocations; IPCGPU_ERR_STATE otherwise).  Outside a capture every form reads the residual test back once per 25 iterations. */
 int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual);
 /* The same Krylov method and the same contract as ipcgpu_solve_pcg (rhs == NULL: H p = -g on the resident gradient; x == NULL: the solution
  * stays on the device; adopt_as_search_dir; iters / rel_residual nullable; single rank), preconditioned by a multilevel additive Schwarz
@@ -542,9 +551,19 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
  * domain matrix (96 x 96, piecewise-constant translations as coarse space) inverted and stored dense, z = sum_l P_l^T A_l^-1 P_l r.  Every
  * sum is taken in a fixed order: two calls on the same state return identical bits.  Memory: 73,728 bytes per domain, about 2.4 KB per
  * vertex, kept for the life of the context.  Dirichlet vertices (the dbc flags of ipcgpu_set_mesh) and the obstacle tail are left out of the
- * coarse levels: with a zero right-hand side on their identity rows their solution entries are exactly 0.  A domain matrix with a pivot <= 0 (the matrix is not positive definite) returns IPCGPU_ERR_SOLVE; nothing is NaN and nothing hangs. */
+ * coarse levels: with a zero right-hand side on their identity rows their solution entries are exactly 0.  A domain matrix with a pivot <= 0 (the matrix is not positive definite) returns IPCGPU_ERR_SOLVE
+ * (deferred form: raises it, see above); nothing is NaN and nothing hangs. */
 int ipcgpu_solve_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters,
     double* rel_residual);
+/* result of the last solve of either solver (deferred or not) */
+typedef struct ipcgpu_solve_result {
+    int iterations;               /* Krylov iterations run */
+    double rel_residual;          /* |r| / |b| after them (0 for b = 0) */
+    double max_abs_x;             /* max_i |x_i| of the solution, exact (searchDir.cwiseAbs().maxCoeff(), Optimizer.cpp:1870, :2189) */
+    int status;                   /* IPCGPU_OK or IPCGPU_ERR_SOLVE */
+} ipcgpu_solve_result;
+/* synchronises only when a solve was enqueued since the last read; returns out->status */
+int ipcgpu_solve_info(ipcgpu_ctx* ctx, ipcgpu_solve_result* out);
 /* what the last multilevel solve built: number of levels, domains per level (8 entries, 0 beyond the last level), bytes of the stored
  * inverses; any pointer may be NULL.  IPCGPU_ERR_STATE before the first ipcgpu_solve_pcg_multilevel and after one that failed. */
 int ipcgpu_multilevel_info(ipcgpu_ctx* ctx, int* levels, int64_t* domains_per_level, uint64_t* bytes);

@@ -151,10 +151,97 @@ int ccd_build_swept(ipcgpu_ctx* ctx, double h);
 int ccd_full(ipcgpu_ctx* ctx, double tol, const double* err_vf, const double* err_ee);
 int ccd_read_back(ipcgpu_ctx* ctx, double* alpha_out);
 
+// ---- api_step.cu: the decisions of the step control and of the Krylov loops ----------------------------------------------------
+// one step_decide(op) on the main stream; word != NULL: read back (with the solve's words, IterState::ls_cond + kDecisionBytes) and returned
+int decide(ipcgpu_ctx* ctx, int op, double a, int b, cudaGraphConditionalHandle h, bool* word, const double* aux = nullptr);
+int cond_prepare(ipcgpu_ctx* ctx, const char* what); // the streams of cond_node's bodies (refused inside a capture before an eager run)
+
+// if (decision) body  /  while (decision) body, where the decision is step_decide(op) before the node and, for a loop, at the end of each pass.
+// Captured: the handle is created on the graph being captured, the decision before the node sets it, the node is added behind the
+// capture's current dependencies, and the body is captured into the node's body graph on a stream of its own (ctx->stream points to it
+// meanwhile, so that the entry points the body calls enqueue there).
+template <typename Body>
+int cond_node(ipcgpu_ctx* ctx, bool loop, int op, double a, int b, Body body)
+{
+    int rc;
+    if (!ctx->capturing) {
+        bool go = false;
+        if ((rc = decide(ctx, op, a, b, 0, &go))) return rc;
+        while (go) {
+            if ((rc = body())) return rc;
+            if (!loop) break;
+            if ((rc = decide(ctx, op, a, b, 0, &go))) return rc;
+        }
+        return IPCGPU_OK;
+    }
+    REQUIRE(ctx->cond_depth < ipcgpu_ctx::kCondDepth, IPCGPU_ERR_STATE, "conditional nodes nested too deeply");
+    cudaStreamCaptureStatus cs;
+    cudaGraph_t g = nullptr;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t nd = 0;
+    CK(cudaStreamGetCaptureInfo(ctx->stream, &cs, nullptr, &g, &deps, &nd));
+    cudaGraphConditionalHandle h = 0;
+    const cudaError_t eh = cudaGraphConditionalHandleCreate(&h, g, 0, 0);
+    if (eh != cudaSuccess) {
+        cudaGetLastError();
+        ctx->err = std::string("conditional graph nodes need CUDA 12.4 or newer in the driver: ") + cudaGetErrorString(eh);
+        return IPCGPU_ERR_CUDA;
+    }
+    if ((rc = decide(ctx, op, a, b, h, nullptr))) return rc;
+    CK(cudaStreamGetCaptureInfo(ctx->stream, &cs, nullptr, &g, &deps, &nd));
+    cudaGraphNodeParams np = {};
+    np.type = cudaGraphNodeTypeConditional;
+    np.conditional.handle = h;
+    np.conditional.type = loop ? cudaGraphCondTypeWhile : cudaGraphCondTypeIf;
+    np.conditional.size = 1;
+    cudaGraphNode_t node;
+    CK(cudaGraphAddNode(&node, g, deps, nd, &np));
+    cudaGraph_t bg = np.conditional.phGraph_out[0];
+    ctx->capture_bodies.push_back(bg);
+    cudaStream_t outer = ctx->stream, inner = ctx->cond_streams[ctx->cond_depth];
+    CK(cudaStreamBeginCaptureToGraph(inner, bg, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    ctx->stream = inner;
+    ++ctx->cond_depth;
+    ctx->inputs_marked = false;
+    rc = body();
+    if (!rc && loop) rc = decide(ctx, op, a, b, h, nullptr);
+    --ctx->cond_depth;
+    ctx->stream = outer;
+    cudaGraph_t captured = nullptr;
+    const cudaError_t ee = cudaStreamEndCapture(inner, &captured);
+    if (rc) return rc;
+    CK(ee);
+    CK(cudaStreamUpdateCaptureDependencies(outer, &node, 1, cudaStreamSetCaptureDependencies));
+    ctx->mark_inputs(); // an event recorded inside the body cannot be waited on out here: the positions / sets changed at this node
+    return IPCGPU_OK;
+}
+
 // ---- solve.cu, multilevel.cu, pattern.cu, safeguard.cu ----------------------------------------------------------------------
-int solver_build_full_pattern(ipcgpu_ctx* ctx, const int* ia, const int* ja);
-int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int* iters_out, double* rel_res_out);
-int solver_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int* iters_out, double* rel_res_out);
+// The Krylov loops of both solvers, after their set-up and a step_decide(kSolveStart): bursts of kKrylovBurst iterations as the body of a
+// WHILE whose decision (kSolveBurst) stops on a non-finite residual, on sqrt(rr) <= rel_tol sqrt(bb) or when the next burst would pass
+// max_iter, then the max_iter % kKrylovBurst iterations left as a second WHILE that runs at most once.  `iteration` enqueues one iteration
+// on ctx->stream (read it there: inside a capture it is the body's stream).  The set-up check (|b| > 0, no pivot <= 0) is the first
+// decision of the first WHILE.  Eager: one read per burst plus the one before the first, as many as a host loop needs.
+constexpr int kKrylovBurst = 25;
+int solver_finish(ipcgpu_ctx* ctx); // max |x_i| into IterState::sv_xmax_ord
+template <typename Iteration>
+int krylov_loops(ipcgpu_ctx* ctx, int max_iter, Iteration iteration)
+{
+    for (const int burst : { kKrylovBurst, max_iter % kKrylovBurst }) {
+        if (burst == 0 || burst > max_iter) continue;
+        int rc = cond_node(ctx, true, ipcgpu::kSolveBurst, 0.0, burst, [&]() {
+            for (int k = 0; k < burst; ++k) iteration();
+            CK(cudaGetLastError());
+            return IPCGPU_OK;
+        });
+        if (rc) return rc;
+    }
+    return solver_finish(ctx);
+}
+int solver_full_pattern(ipcgpu_ctx* ctx);        // fia / fja / fpos of the pattern in ia / ja, rebuilt on the device when its version moved
+int solver_forget_full_pattern(ipcgpu_ctx* ctx); // a new pattern (ipcgpu_set_csr / ipcgpu_enable_device_pattern): the next solve rebuilds
+int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter);
+int solver_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter);
 int solver_multilevel_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count);
 int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src); // src NULL: the direction already in ctx->dir
 int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity);

@@ -46,7 +46,6 @@ static int refresh_pattern_mirror(ipcgpu_ctx* ctx)
     ctx->nnz = (int)h.pat_nnz;
     CK(cudaMemcpyAsync(ctx->h_ia.data(), ctx->ia.p, ctx->h_ia.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->full_pattern_ready = false;
     owned_value_range(ctx);
     return IPCGPU_OK;
 }
@@ -81,6 +80,10 @@ static int status_from_flags(ipcgpu_ctx* ctx, const int* f)
         ctx->err = "device-built sparsity pattern exceeds its capacity (raise it with ipcgpu_enable_device_pattern); the previous pattern is kept";
         return IPCGPU_ERR_CAPACITY;
     }
+    if (f[FLAG_SOLVE]) {
+        ctx->err = "the deferred linear solve failed: a non-positive pivot of the multilevel preconditioner or a non-finite residual (the matrix is not positive definite)";
+        return IPCGPU_ERR_SOLVE;
+    }
     if (f[FLAG_PATTERN]) {
         ctx->err = "CSR pattern misses a contact block: call ipcgpu_set_csr with the augmented pattern (augmentConnectivity, SelfCollisionHandler.cpp:330-415)";
         return IPCGPU_ERR_PATTERN;
@@ -92,8 +95,8 @@ static int status_from_flags(ipcgpu_ctx* ctx, const int* f)
 // the flags of `mask` that the (fresh) h_iter shows raised: cleared on the device, returned as a status
 int flag_status(ipcgpu_ctx* ctx, unsigned mask)
 {
-    int f[8] = { 0 };
-    for (int i = 0; i < 8; ++i)
+    int f[kFlagSlots] = { 0 };
+    for (int i = 0; i < kFlagSlots; ++i)
         if (((mask >> i) & 1u) && ctx->h_iter->flags[i]) {
             f[i] = ctx->h_iter->flags[i];
             CK(cudaMemsetAsync(&ctx->iter.p->flags[i], 0, sizeof(int), ctx->stream));
@@ -348,7 +351,7 @@ int ipcgpu_fetch_iteration(ipcgpu_ctx* ctx, ipcgpu_iteration* out)
         status = IPCGPU_ERR_LINE_SEARCH;
     }
     out->status = status;
-    CK(cudaMemsetAsync(ctx->iter.p->flags, 0, 8 * sizeof(int), ctx->stream)); // flags are per fetch
+    CK(cudaMemsetAsync(ctx->iter.p->flags, 0, sizeof(ctx->iter.p->flags), ctx->stream)); // flags are per fetch
     if (h.hs_zero_step) CK(cudaMemsetAsync(&ctx->iter.p->hs_zero_step, 0, sizeof(int), ctx->stream));
     if (h.grid_axis_cells > 0) { // sort width of the next iteration's grid builds: enough bits for 1.5x the cells this one wanted
         int bits = 3;

@@ -359,8 +359,8 @@ int ipcgpu_enable_device_pattern(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_c
     ctx->pat_changed_host = 0;
     ctx->a_all_dirty = false;
     ctx->offsets_ready = false;
-    ctx->full_pattern_ready = false;
     owned_value_range(ctx);
+    if ((rc = solver_forget_full_pattern(ctx))) return rc;
     return ensure_offsets(ctx);
 }
 

@@ -3,6 +3,7 @@
 #include "abi.h"
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <numeric>
 #include <vector>
 
@@ -271,9 +272,8 @@ int ipcgpu_set_csr(ipcgpu_ctx* ctx, int n_rows, const int* ia, const int* ja, in
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->a_all_dirty = false;
     ctx->offsets_ready = false;
-    ctx->full_pattern_ready = false;
     owned_value_range(ctx);
-    return IPCGPU_OK;
+    return solver_forget_full_pattern(ctx);
 }
 
 int ipcgpu_set_state(ipcgpu_ctx* ctx, const double* V)
@@ -464,38 +464,52 @@ int ipcgpu_inversion_step(ipcgpu_ctx* ctx, const double* p, double slack, double
 }
 
 // ---- device-resident linear solve hand-off (SURVEY 8(f) rank 1) ----------------------------------------------------------
-// (both built-in solvers: the preconditioner is the only difference)
+// (both built-in solvers: the preconditioner is the only difference).  The deferred form (rhs, x, iters, rel_residual all NULL) enqueues
+// everything, the Krylov loops as conditional graph nodes inside a capture; its result is read by ipcgpu_solve_info, its failure raises
+// FLAG_SOLVE.  Any other form synchronises and returns what it always did.
 static int solve_pcg(ipcgpu_ctx* ctx, bool multilevel, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
 {
     REQUIRE(ctx->nnz > 0 && ctx->n_rows == 3 * ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
     REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the built-in solver runs on one rank (a distributed solver takes each rank's rows: ipcgpu_partition_info)");
     REQUIRE(rel_tol > 0.0 && max_iter > 0, IPCGPU_ERR_ARG, "bad tolerance / iteration limit");
+    const bool deferred = !rhs && !x && !iters && !rel_residual;
+    REQUIRE(deferred || !ctx->capturing, IPCGPU_ERR_STATE, "inside a capture the solve takes its deferred form: rhs, x, iters and rel_residual all NULL");
+    REQUIRE(!ctx->capturing || ctx->solve_epoch[multilevel] == ctx->epoch, IPCGPU_ERR_STATE,
+        multilevel ? "run ipcgpu_solve_pcg_multilevel once outside a capture first (it makes its allocations and creates its streams)"
+                   : "run ipcgpu_solve_pcg once outside a capture first (it makes its allocations and creates its streams)");
     ENTER(kSerial);
-    {
-        int rcp = sync_pattern_mirror(ctx);
-        if (rcp) return rcp;
-    }
-    if (!ctx->full_pattern_ready) { // once per sparsity pattern: rows of both triangles, gathered through a position map
-        std::vector<int> ia((size_t)ctx->n_rows + 1), ja((size_t)ctx->nnz);
-        CK(cudaMemcpyAsync(ia.data(), ctx->ia.p, ia.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaMemcpyAsync(ja.data(), ctx->ja.p, ja.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        int rc = solver_build_full_pattern(ctx, ia.data(), ja.data());
-        if (rc) return rc;
-    }
+    int rc = cond_prepare(ctx, multilevel ? "ipcgpu_solve_pcg_multilevel" : "ipcgpu_solve_pcg");
+    if (rc) return rc;
+    const int n = ctx->n_rows;
+    bool ok = ctx->sol.reserve(n) && ctx->pcg_r.reserve(n) && ctx->pcg_p.reserve(n) && ctx->pcg_q.reserve(n) && ctx->pcg_scal.reserve(8)
+        && (multilevel || ctx->pcg_minv.reserve((size_t)6 * ctx->nV));
+    REQUIRE(ok, IPCGPU_ERR_CUDA, "PCG workspace allocation failed");
+    if ((rc = solver_full_pattern(ctx))) return rc; // (rows of both triangles, gathered through a position map; rebuilt when the pattern moved)
     const double* rhs_dev = ctx->g.p;
     double sign = -1.0; // Newton: H p = -g (Optimizer.cpp:2350-2352)
     if (rhs) { // a host right-hand side is staged in a buffer of its own
-        ALLOC(ctx->pcg_b, (size_t)ctx->n_rows);
-        CK(cudaMemcpyAsync(ctx->pcg_b.p, rhs, (size_t)ctx->n_rows * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        ALLOC(ctx->pcg_b, (size_t)n);
+        CK(cudaMemcpyAsync(ctx->pcg_b.p, rhs, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
         rhs_dev = ctx->pcg_b.p;
         sign = 1.0;
     }
-    int rc = (multilevel ? solver_pcg_multilevel : solver_pcg)(ctx, rhs_dev, sign, rel_tol, max_iter, iters, rel_residual);
+    rc = (multilevel ? solver_pcg_multilevel : solver_pcg)(ctx, rhs_dev, sign, rel_tol, max_iter);
     if (rc) return rc;
+    ctx->sv_pending = true;
+    if (!ctx->capturing) ctx->solve_epoch[multilevel] = ctx->epoch;
+    // outside a capture the host loops have read the solve's words (h_iter) with their last decision; inside one they are in device memory
+    const IterState& h = *ctx->h_iter;
+    const bool bad_pivot = !ctx->capturing && multilevel && h.sv_status != 0 && h.sv_iters == 0; // (the set-up failed: no iteration ran)
+    if (multilevel) ctx->ml.built = !bad_pivot;
+    if (!deferred) { // the host-output forms report a failure by their return value alone, as before: no deferred flag
+        if (h.sv_status != 0) CK(cudaMemsetAsync(&ctx->iter.p->flags[FLAG_SOLVE], 0, sizeof(int), ctx->stream));
+        REQUIRE(!bad_pivot, IPCGPU_ERR_SOLVE, "multilevel preconditioner: a domain matrix has a non-positive pivot (the matrix is not positive definite)");
+    }
     if (adopt_as_search_dir && (rc = solver_adopt_direction(ctx, ctx->sol.p))) return rc;
+    if (iters) *iters = h.sv_iters;
+    if (rel_residual) *rel_residual = h.sv_bb > 0.0 ? std::sqrt(h.sv_rr / h.sv_bb) : 0.0;
     if (x) {
-        CK(cudaMemcpyAsync(x, ctx->sol.p, (size_t)ctx->n_rows * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(x, ctx->sol.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
     }
     return IPCGPU_OK;
@@ -509,6 +523,26 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
 int ipcgpu_solve_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
 {
     return solve_pcg(ctx, true, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
+}
+
+int ipcgpu_solve_info(ipcgpu_ctx* ctx, ipcgpu_solve_result* out)
+{
+    REQUIRE(out != nullptr, IPCGPU_ERR_ARG, "null output");
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is in progress");
+    if (ctx->sv_pending) {
+        ENTER(kSerial);
+        int rc = fetch_iter_state(ctx);
+        if (rc) return rc;
+        ctx->sv_pending = false;
+    }
+    else CK(cudaSetDevice(ctx->device)); // (reads the host mirror)
+    const IterState& h = *ctx->h_iter;
+    out->iterations = h.sv_iters;
+    out->rel_residual = h.sv_bb > 0.0 ? std::sqrt(h.sv_rr / h.sv_bb) : 0.0;
+    std::memcpy(&out->max_abs_x, &h.sv_xmax_ord, sizeof(double));
+    out->status = h.sv_status;
+    if (h.sv_status) ctx->err = "the linear solve failed: a non-positive pivot of the multilevel preconditioner or a non-finite residual (the matrix is not positive definite)";
+    return h.sv_status;
 }
 
 int ipcgpu_multilevel_info(ipcgpu_ctx* ctx, int* levels, int64_t* domains_per_level, uint64_t* bytes)

@@ -86,6 +86,8 @@ int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
     ctx->pat_pending = false;
     ctx->sc_pending_at_capture = ctx->sc_pending;
     ctx->sc_pending = false;
+    ctx->sv_pending_at_capture = ctx->sv_pending;
+    ctx->sv_pending = false;
     ctx->capture_bodies.clear();
     CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
     ctx->capturing = true;
@@ -137,6 +139,8 @@ int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id)
     ctx->pat_pending = ctx->pat_pending_at_capture; // nothing ran yet
     rec.step_control = ctx->sc_pending;
     ctx->sc_pending = ctx->sc_pending_at_capture;
+    rec.solve = ctx->sv_pending;
+    ctx->sv_pending = ctx->sv_pending_at_capture;
     rec.bodies.swap(ctx->capture_bodies);
     rec.hs = snapshot_host_state(ctx);
     ctx->launches = ctx->launches_at_capture; // nothing ran yet
@@ -159,6 +163,7 @@ int ipcgpu_graph_launch(ipcgpu_ctx* ctx, int graph_id)
     CK(cudaGraphLaunch(rec.exec, ctx->stream));
     if (rec.updates_pattern) ctx->pat_pending = true;
     if (rec.step_control) ctx->sc_pending = true;
+    if (rec.solve) ctx->sv_pending = true;
     ctx->a_all_dirty = false;
     apply_host_state(ctx, rec.hs);
     ctx->launches += rec.launches;
@@ -250,81 +255,32 @@ int ipcgpu_safeguard_debug_flags(ipcgpu_ctx* ctx, int enable, int* tri_flags, in
     return IPCGPU_OK;
 }
 
+} // extern "C"
+
 // ---- step control: CFL branch and line search (step_control.cu holds the decision kernel) ----------------------------------------
 // Each loop body and loop condition is written once: a sequence of entry points plus one step_decide.  Outside a capture the
-// host loops and reads the decision word (one synchronisation per decision); inside one the body is captured into a conditional node.
-static int decide(ipcgpu_ctx* ctx, int op, double a, int b, cudaGraphConditionalHandle h, bool* word)
+// host loops and reads the decision word (one synchronisation per decision); inside one the body is captured into a conditional node
+// (cond_node, abi.h).  The linear solves drive their Krylov loops the same way (krylov_loops, abi.h).
+int decide(ipcgpu_ctx* ctx, int op, double a, int b, cudaGraphConditionalHandle h, bool* word, const double* aux)
 {
-    step_decide(ctx->iter.p, op, a, b, (unsigned long long)h, ctx->stream);
+    step_decide(ctx->iter.p, op, a, b, (unsigned long long)h, ctx->stream, aux);
     ++ctx->launches;
     CK(cudaGetLastError());
-    if (word) {
-        CK(cudaMemcpyAsync(&ctx->staging->decision, &ctx->iter.p->ls_cond, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    if (word) { // (the solve's words come along: an eager solve reads its result here)
+        CK(cudaMemcpyAsync(&ctx->h_iter->ls_cond, &ctx->iter.p->ls_cond, kDecisionBytes, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        *word = ctx->staging->decision != 0;
+        *word = ctx->h_iter->ls_cond != 0;
     }
     return IPCGPU_OK;
 }
 
-} // extern "C"
-
-// if (decision) body  /  while (decision) body, where the decision is step_decide(op) before the node and, for a loop, at the end of each pass.
-// Captured: the handle is created on the graph being captured, the decision before the node sets it, the node is added behind the
-// capture's current dependencies, and the body is captured into the node's body graph on a stream of its own (ctx->stream points to it
-// meanwhile, so that the entry points the body calls enqueue there).
-template <typename Body>
-static int cond_node(ipcgpu_ctx* ctx, bool loop, int op, double a, int b, Body body)
+// the streams the bodies of conditional nodes are captured on: created by the first eager call (`what` names it in the refusal)
+int cond_prepare(ipcgpu_ctx* ctx, const char* what)
 {
-    int rc;
-    if (!ctx->capturing) {
-        bool go = false;
-        if ((rc = decide(ctx, op, a, b, 0, &go))) return rc;
-        while (go) {
-            if ((rc = body())) return rc;
-            if (!loop) break;
-            if ((rc = decide(ctx, op, a, b, 0, &go))) return rc;
-        }
-        return IPCGPU_OK;
+    if (!ctx->cond_streams[0]) {
+        REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, std::string("run ") + what + " once outside a capture first (it creates its streams)");
+        for (cudaStream_t& s : ctx->cond_streams) CK(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, ctx->prio_high));
     }
-    REQUIRE(ctx->cond_depth < ipcgpu_ctx::kCondDepth, IPCGPU_ERR_STATE, "conditional nodes nested too deeply");
-    cudaStreamCaptureStatus cs;
-    cudaGraph_t g = nullptr;
-    const cudaGraphNode_t* deps = nullptr;
-    size_t nd = 0;
-    CK(cudaStreamGetCaptureInfo(ctx->stream, &cs, nullptr, &g, &deps, &nd));
-    cudaGraphConditionalHandle h = 0;
-    const cudaError_t eh = cudaGraphConditionalHandleCreate(&h, g, 0, 0);
-    if (eh != cudaSuccess) {
-        cudaGetLastError();
-        ctx->err = std::string("conditional graph nodes need CUDA 12.4 or newer in the driver: ") + cudaGetErrorString(eh);
-        return IPCGPU_ERR_CUDA;
-    }
-    if ((rc = decide(ctx, op, a, b, h, nullptr))) return rc;
-    CK(cudaStreamGetCaptureInfo(ctx->stream, &cs, nullptr, &g, &deps, &nd));
-    cudaGraphNodeParams np = {};
-    np.type = cudaGraphNodeTypeConditional;
-    np.conditional.handle = h;
-    np.conditional.type = loop ? cudaGraphCondTypeWhile : cudaGraphCondTypeIf;
-    np.conditional.size = 1;
-    cudaGraphNode_t node;
-    CK(cudaGraphAddNode(&node, g, deps, nd, &np));
-    cudaGraph_t bg = np.conditional.phGraph_out[0];
-    ctx->capture_bodies.push_back(bg);
-    cudaStream_t outer = ctx->stream, inner = ctx->cond_streams[ctx->cond_depth];
-    CK(cudaStreamBeginCaptureToGraph(inner, bg, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    ctx->stream = inner;
-    ++ctx->cond_depth;
-    ctx->inputs_marked = false;
-    rc = body();
-    if (!rc && loop) rc = decide(ctx, op, a, b, h, nullptr);
-    --ctx->cond_depth;
-    ctx->stream = outer;
-    cudaGraph_t captured = nullptr;
-    const cudaError_t ee = cudaStreamEndCapture(inner, &captured);
-    if (rc) return rc;
-    CK(ee);
-    CK(cudaStreamUpdateCaptureDependencies(outer, &node, 1, cudaStreamSetCaptureDependencies));
-    ctx->mark_inputs(); // an event recorded inside the body cannot be waited on out here: the positions / sets changed at this node
     return IPCGPU_OK;
 }
 
@@ -335,17 +291,15 @@ static int step_control_prepare(ipcgpu_ctx* ctx)
     REQUIRE(ctx->surface_ready && ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh and ipcgpu_set_surface first");
     REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the CFL branch and the line search run on one rank");
     REQUIRE(ctx->dir_valid && ctx->pSize_surface, IPCGPU_ERR_STATE, "no search direction for this surface: ipcgpu_set_search_dir first");
-    if (!ctx->cond_streams[0]) {
-        REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "run the CFL branch / line search once outside a capture first (it creates its streams)");
-        for (cudaStream_t& s : ctx->cond_streams) CK(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, ctx->prio_high));
-    }
-    return IPCGPU_OK;
+    return cond_prepare(ctx, "the CFL branch / line search");
 }
 
 static int step_control_status(ipcgpu_ctx* ctx, int status)
 {
     if (status == IPCGPU_ERR_LINE_SEARCH)
         ctx->err = "step 0: the line search's entry state fails a safeguard (inversion / intersection), or the step bound or the entry step is 0";
+    else if (status == IPCGPU_ERR_SOLVE)
+        ctx->err = "the line search did not start: the linear solve that produced the search direction failed";
     else if (status == IPCGPU_ERR_NONPOSITIVE_DISTANCE)
         ctx->err = "a line-search trial has a constraint with d <= 0 (the reference exits here, Optimizer.cpp:3296-3306)";
     return status;

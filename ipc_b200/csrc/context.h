@@ -155,9 +155,7 @@ struct HostStaging {
     double scalar;   // a read-back double: energy_result, ipcgpu_dirichlet_completed_step
     int count;       // a read-back count: the lagged friction pairs
     int contact[16]; // ContactWork::counters read back (contact_sync_counts, the sort-based duplicate merge) or uploaded (ipcgpu_set_constraint_set)
-    double pcg[8];   // the PCG scalars (solve.cu), then its residual history entry
     double pSize;    // source of upload_dir's asynchronous H2D copy into pSize_dev, which nothing waits on: never reused for anything else
-    int decision;    // the step-control decision word (IterState::ls_cond) of the host loop of a CFL branch / line search
     int hs_count[2]; // half-space counts: [0] active, [1] lagged
 };
 
@@ -284,11 +282,16 @@ struct ipcgpu_ctx {
     uint64_t pat_seen_version = 0;
     int pat_changed_host = 0;
     ipcgpu::PatternWork pw;
-    // device-resident linear solve (solve.cu): full-row structure of the symmetric matrix + PCG workspace
-    ipcgpu::DevBuf<int> fia, fja, fpos;
-    bool full_pattern_ready = false;
-    ipcgpu::DevBuf<double> sol, pcg_b, pcg_r, pcg_p, pcg_q, pcg_minv, pcg_scal, pcg_hist;
+    // device-resident linear solve (solve.cu): full-row structure of the symmetric matrix, built on the device whenever the pattern's
+    // version differs from the one it was built for (fp_cnt / fp_start / fp_cur / fp_tmp: counts, scan, scatter cursors, scan scratch),
+    // + PCG workspace.  solve_epoch[m]: the epoch of the last eager solve of the block-Jacobi (0) / multilevel (1) solver, whose lazy
+    // allocations a capture relies on; sv_pending: a solve was enqueued since ipcgpu_solve_info read it
+    ipcgpu::DevBuf<int> fia, fja, fpos, fp_cnt, fp_start, fp_cur;
+    ipcgpu::DevBuf<unsigned char> fp_tmp;
+    ipcgpu::DevBuf<double> sol, pcg_b, pcg_r, pcg_p, pcg_q, pcg_minv, pcg_scal;
     ipcgpu::MultilevelWork ml;
+    uint64_t solve_epoch[2] = { ~0ull, ~0ull };
+    bool sv_pending = false, sv_pending_at_capture = false;
 
     // work / result buffers
     ipcgpu::DevBuf<double> gcont, hblk, g, e_per_tet, partials, inv_steps, dir, in_partials, e_partials2;
@@ -310,12 +313,13 @@ struct ipcgpu_ctx {
         bool dirty_at_begin = false;
         bool updates_pattern = false; // the sequence contains ipcgpu_update_pattern
         bool step_control = false;    // ... a CFL branch or a line search
+        bool solve = false;           // ... a linear solve
         std::vector<cudaGraph_t> bodies; // bodies of its conditional nodes (owned by `graph`)
         HostState hs;
     };
     std::vector<GraphRec> graphs;
     std::vector<cudaGraph_t> capture_bodies; // conditional-node bodies of the capture in progress
-    // step control (api_step.cu: cond_node): the bodies of nested conditional nodes are captured on these high-priority streams, one per depth
+    // conditional graph nodes (abi.h: cond_node): the bodies of nested conditional nodes are captured on these high-priority streams, one per depth
     static constexpr int kCondDepth = 3;
     cudaStream_t cond_streams[kCondDepth] = { nullptr, nullptr, nullptr };
     int cond_depth = 0;

@@ -660,7 +660,7 @@ void step_set(IterState* st_dev, double alpha, cudaStream_t st) { k_step_set<<<1
 
 // Deferred cross-rank scalars of one iteration in ONE collective (kernels.h: kPackedScalars): buf = the energies, the flags, the checks and
 // the crossing count; a scalar that is not a local share (local_mask) packs as 0 and keeps its value.
-constexpr int kFlags = kEnergySlots, kChecks = kFlags + 8, kCrossings = kChecks + 2;
+constexpr int kFlags = kEnergySlots, kChecks = kFlags + kFlagSlots, kCrossings = kChecks + 2;
 static_assert(kCrossings + 1 == kPackedScalars && kPackedScalars <= 32, "one warp packs the scalars");
 __global__ void k_pack_scalars(const IterState* __restrict__ st, unsigned local_mask, double* __restrict__ buf)
 {

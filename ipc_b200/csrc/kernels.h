@@ -1,9 +1,12 @@
 // kernels.h -- launcher declarations shared between the .cu translation units and the C-ABI (api*.cu)
 #pragma once
 #include <cuda_runtime.h>
+#include <cstddef>
 #include <cstdint>
 
 namespace ipcgpu {
+
+constexpr int kFlagSlots = 9; // IterState::flags (FLAG_*)
 
 // slots of IterState::energy
 enum { kEnergyElastic = 0, kEnergyBarrier, kEnergyFriction, kEnergyInertia, kEnergyPlaneBarrier, kEnergyPlaneFriction, kEnergyDamping, kEnergyNeumann,
@@ -24,9 +27,8 @@ struct IterState {
     double energy[kEnergySlots];      // kEnergy* slots (this rank's share, then cross-rank sums)
     int ref_count[3];
     int n_set[3];                     // active / mollified / candidate counts of the last constraint set (this rank's lists)
-    int flags[8];                     // IPCGPU_FLAG_* slots (nonzero = raised); cleared by ipcgpu_fetch_iteration
+    int flags[kFlagSlots];            // FLAG_* slots (nonzero = raised); cleared by ipcgpu_fetch_iteration
     int grid_axis_cells;              // cells per axis the broad-phase grids built since the last fetch would have liked (sort-width tuning)
-    int pad_;
     int checks[2];                    // line-search safeguards: inverted tets, surface triangles crossed by an edge (this rank's share, then sums)
     unsigned long long ccd_stats[8];  // survivors, warnings, deferred, longest / total pair cycles, boxes (thread pass, warp pass), candidates
     // step control (step_control.cu): the CFL branch of the step bound and the line search
@@ -38,6 +40,16 @@ struct IterState {
     int ls_count[4];                  // halvings: inversion guard, intersection pre-check, Armijo loop, post-check
     int ls_stopped, ls_rebuilt, ls_post_ran;
     int ls_cond;                      // the decision word of the last step_decide
+    // linear solve (solve.cu, multilevel.cu): the Krylov loops' state, read with ls_cond by the host loop of an eager solve (kDecisionWords)
+    int sv_iters;                     // iterations run by the solve in flight
+    int sv_status;                    // IPCGPU_OK or IPCGPU_ERR_SOLVE (a pivot <= 0 of the multilevel set-up, a non-finite residual)
+    int sv_run;                       // the loop goes on: the set-up passed, no stop yet
+    int sv_max_iter;
+    double sv_rr, sv_bb, sv_tol;      // |r|^2 after the last iteration, |b|^2, rel_tol
+    unsigned long long sv_xmax_ord;   // max |x_i| of the solution (order-preserving image)
+    unsigned long long sv_fp_version; // pat_version the full-row structure (fia / fja / fpos) was built for; ~0 = none
+    int sv_fp_build;                  // the full-row build in flight runs (pat_version != sv_fp_version)
+    int sv_pad_;
     // Dirichlet penalty and Neumann forces (damping.cu; before the half-space words, which ipcgpu_set_halfspaces clears as one range)
     double dbc_rho;                   // rho_DBC (ipcgpu_set_dirichlet_penalty), read by the penalty kernels at run time
     double dbc_step;                  // the last computeCompletedStepSize
@@ -56,16 +68,20 @@ struct IterState {
     int pat_diff;                     // the extra blocks of the update in flight differ from the previous ones
     int pat_pad_;
 };
-// step_decide operations (step_control.cu) and the energy terms of a line search
-enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersection, kLsArmijo, kLsPostCheck, kLsPostLoop, kLsRebuild, kWsEntry };
+// step_decide operations (step_control.cu) and the energy terms of a line search.  kSolveStart / kSolveBurst: the Krylov loops of both
+// built-in solvers (solve.cu, multilevel.cu)
+enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersection, kLsArmijo, kLsPostCheck, kLsPostLoop, kLsRebuild, kWsEntry, kSolveStart,
+    kSolveBurst };
+// bytes of IterState from ls_cond on that an eager decision reads back: the decision word and the solve's words (one copy)
+constexpr size_t kDecisionBytes = offsetof(IterState, sv_tol) - offsetof(IterState, ls_cond);
 enum { kTermInertia = 1, kTermFriction = 2, kTermHalfSpace = 4, kTermHalfSpaceFriction = 8, kTermDamping = 16, kTermNeumann = 32, kTermDirichlet = 64 };
 enum { FLAG_NONPOSITIVE_DISTANCE = 0, FLAG_SET_CAPACITY = 1, FLAG_CCD_CAPACITY = 2, FLAG_ZERO_CCD_DISTANCE = 3, FLAG_PATTERN = 4, FLAG_TI_WARNINGS = 5, FLAG_EXCHANGE_CAPACITY = 6,
-    FLAG_PATTERN_CAPACITY = 7 };
+    FLAG_PATTERN_CAPACITY = 7, FLAG_SOLVE = 8 };
 // Scalars that may still hold this rank's share (ipcgpu_ctx::local_scalars): bit s = energy[s], then checks and hs_crossings.  The fetch
-// completes them in one sum-allreduce of kPackedScalars doubles: the energies, the 8 flags (a flag is raised iff any rank raised it), the
+// completes them in one sum-allreduce of kPackedScalars doubles: the energies, the flags (a flag is raised iff any rank raised it), the
 // 2 checks and the crossing count (integer counts are exact in a double).
 enum : unsigned { kLocalChecks = 1u << kEnergySlots, kLocalCrossings = 1u << (kEnergySlots + 1) };
-constexpr int kPackedScalars = kEnergySlots + 8 + 2 + 1;
+constexpr int kPackedScalars = kEnergySlots + kFlagSlots + 2 + 1;
 
 struct ElasticArgs {
     int nV, nT;
@@ -184,7 +200,8 @@ void step_forward(int nV, const double* x0_soa, const double* p_interleaved, dou
 // step_control.cu: IterState::sc_pmax_ord = max |p| over the surface vertices below nVdof; one decision of the step control (handle != 0:
 // also the value of that conditional graph node)
 void cfl_pmax(int nSV, const int* SVI, int nVdof, const double* dir, IterState* st_dev, cudaStream_t st);
-void step_decide(IterState* st_dev, int op, double a, int b, unsigned long long handle, cudaStream_t st);
+// aux: kSolveStart reads the solver's scalars there ([4] |b|^2, [6] a non-positive pivot)
+void step_decide(IterState* st_dev, int op, double a, int b, unsigned long long handle, cudaStream_t st, const double* aux = nullptr);
 // inertia term of Optimizer::computeEnergyVal / computeGradient (Optimizer.cpp:3227-3239, :3439-3450)
 int inertia_energy_blocks(int nV);
 void inertia_energy(int v0, int v1, int nV, const double* x_soa, const double* xtilde_soa, const double* mass, double* partials, cudaStream_t st);

@@ -19,21 +19,22 @@
 //          one; at the levels >= 1 a second kernel adds the chunks of every aggregate in chunk order.  No floating-point atomics: the
 //          matrices are bit-identical from call to call.  One CTA per domain then inverts its tile in shared memory by
 //          unpivoted Gauss-Jordan elimination (its pivots are the squares of the Cholesky pivots of the tile: the same positivity test) and
-//          stores the inverse dense and exactly symmetric.  A pivot <= 0 raises a flag the solve reports as IPCGPU_ERR_SOLVE; the domain
+//          stores the inverse dense and exactly symmetric.  A pivot <= 0 raises a word the solve reports as IPCGPU_ERR_SOLVE; the domain
 //          then stores the identity, so nothing downstream is NaN.
 // Apply.   z = sum_l P_l^T A_l^-1 P_l r.  One kernel per level, one CTA per domain: restrict (level 0 reads r through the order, level l
 //          sums the 32 children of each aggregate from level l-1's restricted vector: a fixed shuffle tree), multiply by the stored inverse
 //          (coalesced rows, warp reductions).  One kernel per vertex then adds the levels' contributions in level order and leaves the
 //          per-CTA partials of r.z and r.r.
 // Krylov.  Every dot product is a fixed-order two-level sum (per-CTA partials, then one CTA), so two solves of one system give identical
-//          bits: the direction feeds Armijo decisions (DESIGN 3.13).  The host reads the residual every 25 iterations, as solve.cu does, and
-//          decides nothing else; set-up and application never synchronise.
+//          bits: the direction feeds Armijo decisions (DESIGN 3.13).  The loop is solve.cu's (krylov_loops, abi.h): the residual test runs
+//          on the device every 25 iterations, read by the host outside a capture, a conditional graph node inside one; set-up and
+//          application never synchronise.
 //
 // Memory: the stored inverses (73,728 bytes per domain, 0.61 GB at 257 k vertices) and the level vectors stay allocated for the life of the
 // context after the first call, like every workspace of the context.
 //
-// Follow-ups this layout leaves open: capturing the loop in a graph (no host decision but the residual read-back), a block-CSR SpMV, and
-// single-precision storage of the inverses (the 0.6 GB read per application at 257 k vertices).
+// Follow-ups this layout leaves open: a block-CSR SpMV, and single-precision storage of the inverses (the 0.6 GB read per application at
+// 257 k vertices).
 #include "common.cuh"
 #include "abi.h"
 #include <algorithm>
@@ -398,8 +399,9 @@ __global__ void __launch_bounds__(256) k_ml_update(int n, const double* __restri
     r[i] -= alpha * Ap[i];
 }
 
-// after an application: r.z and |r|^2 from the partials, beta = r.z / (the previous r.z) (0 at the start), the residual history
-__global__ void __launch_bounds__(1024) k_ml_roll(const double* __restrict__ part, int n_part, double* __restrict__ scal, double* __restrict__ history, int it)
+// after an application: r.z and |r|^2 from the partials, beta = r.z / (the previous r.z) (0 at the start), |r|^2 and the count of the
+// solve in flight (start: |b|^2 instead)
+__global__ void __launch_bounds__(1024) k_ml_roll(const double* __restrict__ part, int n_part, double* __restrict__ scal, IterState* __restrict__ st, int start)
 {
     __shared__ double sm[2][32];
     double s0 = 0.0, s1 = 0.0;
@@ -422,8 +424,11 @@ __global__ void __launch_bounds__(1024) k_ml_roll(const double* __restrict__ par
             scal[5] = rz_old != 0.0 ? s0 / rz_old : 0.0;
             scal[0] = s0;
             scal[3] = s1;
-            if (it < 0) scal[4] = s1; // the start: r = b
-            else history[it] = s1;
+            if (start) scal[4] = s1; // r = b
+            else {
+                st->sv_rr = s1;
+                ++st->sv_iters;
+            }
         }
     }
 }
@@ -531,54 +536,32 @@ static void multilevel_apply(ipcgpu_ctx* ctx, const double* r, double* z, double
 }
 
 // PCG on the device-resident matrix with the multilevel preconditioner.  rhs_dev: device vector (3 nV) scaled by `sign`.  The solution is
-// left in ctx->sol.
-int solver_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int* iters_out, double* rel_res_out)
+// left in ctx->sol, the result in IterState (sv_*); a pivot <= 0 of the set-up is the solve's failure (kSolveStart).  The Krylov workspace is
+// reserved by the caller (solve_pcg in api_mesh.cu), ml.part here.
+int solver_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter)
 {
     cudaStream_t st = ctx->stream;
-    const int n = ctx->n_rows, nV = ctx->nV;
-    const int spmv_blocks = kSMs * 8, vec_blocks = nblk(nV, 256);
-    bool ok = ctx->sol.reserve(n) && ctx->pcg_r.reserve(n) && ctx->pcg_p.reserve(n) && ctx->pcg_q.reserve(n) && ctx->pcg_scal.reserve(8)
-        && ctx->pcg_hist.reserve((size_t)std::max(max_iter, 1) + 1) && ctx->ml.part.reserve((size_t)std::max(spmv_blocks, 2 * vec_blocks));
-    REQUIRE(ok, IPCGPU_ERR_CUDA, "PCG workspace allocation failed");
+    const int n = ctx->n_rows;
+    const int spmv_blocks = kSMs * 8, vec_blocks = nblk(ctx->nV, 256);
+    REQUIRE(ctx->ml.part.reserve((size_t)std::max(spmv_blocks, 2 * vec_blocks)), IPCGPU_ERR_CUDA, "PCG workspace allocation failed");
     CK(cudaMemsetAsync(ctx->pcg_scal.p, 0, 8 * sizeof(double), st));
     int rc = multilevel_build(ctx, ctx->pcg_scal.p + 6);
     if (rc) return rc;
     double *x = ctx->sol.p, *r = ctx->pcg_r.p, *p = ctx->pcg_p.p, *q = ctx->pcg_q.p, *scal = ctx->pcg_scal.p, *part = ctx->ml.part.p;
     k_ml_init<<<nblk(n, 256), 256, 0, st>>>(n, rhs_dev, sign, x, r, p);
     multilevel_apply(ctx, r, q, part);
-    k_ml_roll<<<1, 1024, 0, st>>>(part, vec_blocks, scal, ctx->pcg_hist.p, -1);
+    k_ml_roll<<<1, 1024, 0, st>>>(part, vec_blocks, scal, ctx->iter.p, 1);
     k_ml_direction<<<nblk(n, 256), 256, 0, st>>>(n, q, p, scal);
     ctx->launches += 3;
-    double* h = ctx->staging->pcg;
-    CK(cudaMemcpyAsync(h, scal, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    REQUIRE(h[6] == 0.0, IPCGPU_ERR_SOLVE, "multilevel preconditioner: a domain matrix has a non-positive pivot (the matrix is not positive definite)");
-    ctx->ml.built = true;
-    const double bb = h[4];
-    int it = 0;
-    double rr = bb;
-    const int check_every = 25; // the host looks at the residual every 25 iterations (one small read-back)
-    if (bb > 0.0) {
-        while (it < max_iter) {
-            const int burst = std::min(check_every, max_iter - it);
-            for (int b = 0; b < burst; ++b, ++it) {
-                k_ml_spmv<<<spmv_blocks, 256, 0, st>>>(n, ctx->fia.p, ctx->fja.p, ctx->fpos.p, ctx->a.p, p, q, part);
-                reduce_sum(part, spmv_blocks, 1.0, scal + 1, st);
-                k_ml_update<<<nblk(n, 256), 256, 0, st>>>(n, p, q, x, r, scal);
-                multilevel_apply(ctx, r, q, part); // z in Ap's storage
-                k_ml_roll<<<1, 1024, 0, st>>>(part, vec_blocks, scal, ctx->pcg_hist.p, it);
-                k_ml_direction<<<nblk(n, 256), 256, 0, st>>>(n, q, p, scal);
-                ctx->launches += 5;
-            }
-            CK(cudaMemcpyAsync(h, ctx->pcg_hist.p + (it - 1), sizeof(double), cudaMemcpyDeviceToHost, st));
-            CK(cudaStreamSynchronize(st));
-            rr = h[0];
-            if (!(rr == rr)) break; // NaN: the matrix was not positive definite
-            if (std::sqrt(rr) <= rel_tol * std::sqrt(bb)) break;
-        }
-    }
-    CK(cudaGetLastError());
-    if (iters_out) *iters_out = it;
-    if (rel_res_out) *rel_res_out = bb > 0.0 ? std::sqrt(rr / bb) : 0.0;
-    return IPCGPU_OK;
+    if ((rc = decide(ctx, kSolveStart, rel_tol, max_iter, 0, nullptr, scal))) return rc;
+    return krylov_loops(ctx, max_iter, [&]() {
+        cudaStream_t s = ctx->stream; // (the body's stream inside a capture)
+        k_ml_spmv<<<spmv_blocks, 256, 0, s>>>(n, ctx->fia.p, ctx->fja.p, ctx->fpos.p, ctx->a.p, p, q, part);
+        reduce_sum(part, spmv_blocks, 1.0, scal + 1, s);
+        k_ml_update<<<nblk(n, 256), 256, 0, s>>>(n, p, q, x, r, scal);
+        multilevel_apply(ctx, r, q, part); // z in Ap's storage
+        k_ml_roll<<<1, 1024, 0, s>>>(part, vec_blocks, scal, ctx->iter.p, 0);
+        k_ml_direction<<<nblk(n, 256), 256, 0, s>>>(n, q, p, scal);
+        ctx->launches += 5;
+    });
 }

@@ -8,14 +8,23 @@
 // It takes its right-hand side from the device-resident gradient and leaves the search direction where the step-bound stages read it,
 // so that a whole Newton iteration (assembly -> solve -> CCD) needs no host transfer of any vertex- or matrix-sized array.
 //
-// SpMV on a symmetric matrix stored by its upper triangle: at ipcgpu_set_csr time the host builds the FULL row structure once
-// (col index + position of the value inside the upper-triangular array for every entry of both triangles), so the product is a plain
-// deterministic row-parallel CSR SpMV that gathers a[] through that position map -- no atomics, no transposed pass.
+// SpMV on a symmetric matrix stored by its upper triangle: the device builds the FULL row structure once per pattern (col index + position
+// of the value inside the upper-triangular array for every entry of both triangles), so the product is a plain deterministic row-parallel
+// CSR SpMV that gathers a[] through that position map -- no atomics, no transposed pass.
+//
+// Full-row build (solver_full_pattern).  Row i of the full matrix is its transposed (lower) entries in ascending source row, then its own
+// upper entries in storage order: the order every SpMV and the multilevel set-up sum a row in.  Five launches of sizes fixed by n_rows,
+// gated on the device by IterState::pat_version against the version the structure was built for (sv_fp_version), so that a captured solve
+// rebuilds it exactly when a replayed ipcgpu_update_pattern rewrote the pattern, and otherwise nothing:
+//   k_fp_gate (one thread) -> k_fp_count (own lengths, +1 per transposed entry: integer atomics) -> exclusive scan into fp_start ->
+//   k_fp_scatter (own entries at their place, transposed ones behind per-row cursors: in any order) -> k_fp_sort (each row's transposed
+//   part sorted by source row -- distinct within a column, so the result does not depend on the order of the scatter's atomics -- and
+//   fia = fp_start).  The scan runs ungated into scratch; fia, fja and fpos are written only by gated kernels.
 #include "common.cuh"
 #include "abi.h"
 #include <algorithm>
 #include <cmath>
-#include <vector>
+#include <cub/cub.cuh>
 
 namespace ipcgpu {
 
@@ -120,12 +129,97 @@ __global__ void __launch_bounds__(256) k_pcg_direction(int n, const double* __re
     const double beta = rz != 0.0 ? scal[2] / rz : 0.0;
     if (i < n) p[i] = z[i] + beta * p[i];
 }
-__global__ void k_pcg_roll(double* scal, double* history, int it)
+__global__ void k_pcg_roll(double* scal, IterState* st)
 {
     if (threadIdx.x == 0) {
-        history[it] = scal[3]; // |r|^2 after this iteration
+        st->sv_rr = scal[3]; // |r|^2 after this iteration
+        ++st->sv_iters;
         scal[0] = scal[2];
         scal[1] = scal[2] = scal[3] = 0.0;
+    }
+}
+// max |x_i| (exact, so the order does not matter; NaN entries are skipped)
+__global__ void __launch_bounds__(256) k_abs_max(int n, const double* __restrict__ x, unsigned long long* __restrict__ out)
+{
+    double m = 0.0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) m = fmax(m, fabs(x[i]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0 && m > 0.0) atomicMax(out, dbl_to_ord(m)); // (non-negative doubles order like their bit patterns)
+}
+
+// ---- full-row structure -------------------------------------------------------------------------------------------------------
+__global__ void k_fp_gate(IterState* st)
+{
+    if (threadIdx.x == 0) st->sv_fp_build = st->pat_version != st->sv_fp_version;
+}
+// cnt[i] += entries of full row i (cnt zeroed by k_fp_zero); the scatter cursors zeroed
+__global__ void __launch_bounds__(256) k_fp_count(int n, const int* __restrict__ ia, const int* __restrict__ ja, int base, int* __restrict__ cnt,
+    int* __restrict__ cur, const IterState* __restrict__ st)
+{
+    if (!st->sv_fp_build) return;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int k0 = ia[i] - base, k1 = ia[i + 1] - base;
+        int own = 0;
+        for (int k = k0; k < k1; ++k) {
+            const int j = ja[k] - base;
+            ++own;
+            if (j != i) atomicAdd(cnt + j, 1);
+        }
+        atomicAdd(cnt + i, own);
+        cur[i] = 0;
+    }
+}
+__global__ void __launch_bounds__(256) k_fp_zero(int n, int* __restrict__ cnt, const IterState* __restrict__ st)
+{
+    if (!st->sv_fp_build) return;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += gridDim.x * blockDim.x) cnt[i] = 0;
+}
+__global__ void __launch_bounds__(256) k_fp_scatter(int n, const int* __restrict__ ia, const int* __restrict__ ja, int base, const int* __restrict__ start,
+    const int* __restrict__ cnt, int* __restrict__ cur, int* __restrict__ fja, int* __restrict__ fpos, const IterState* __restrict__ st)
+{
+    if (!st->sv_fp_build) return;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int k0 = ia[i] - base, k1 = ia[i + 1] - base;
+        const int own0 = start[i] + cnt[i] - (k1 - k0); // the row's own entries come after its transposed ones
+        for (int k = k0; k < k1; ++k) {
+            const int j = ja[k] - base;
+            fja[own0 + k - k0] = j;
+            fpos[own0 + k - k0] = k;
+            if (j != i) {
+                const int e = start[j] + atomicAdd(cur + j, 1);
+                fja[e] = i;
+                fpos[e] = k;
+            }
+        }
+    }
+}
+// each row's transposed part by source row (insertion sort: a few dozen entries), fia = start; the version the structure now holds
+__global__ void __launch_bounds__(256) k_fp_sort(int n, const int* __restrict__ start, const int* __restrict__ cur, int* __restrict__ fja, int* __restrict__ fpos,
+    int* __restrict__ fia, IterState* __restrict__ st)
+{
+    if (!st->sv_fp_build) return;
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    for (int i = t; i < n; i += gridDim.x * blockDim.x) {
+        int* c = fja + start[i];
+        int* q = fpos + start[i];
+        const int m = cur[i];
+        for (int a = 1; a < m; ++a) {
+            const int cj = c[a], qa = q[a];
+            int b = a - 1;
+            while (b >= 0 && c[b] > cj) {
+                c[b + 1] = c[b];
+                q[b + 1] = q[b];
+                --b;
+            }
+            c[b + 1] = cj;
+            q[b + 1] = qa;
+        }
+        fia[i] = start[i];
+    }
+    if (t == 0) {
+        fia[n] = start[n];
+        st->sv_fp_version = st->pat_version;
     }
 }
 // mean |p| over the surface vertices (SpatialHash.hpp:603-612) for a direction that was produced on the device: fixed-order two-level sum
@@ -160,83 +254,72 @@ __global__ void k_psize_mean(const double* __restrict__ partials, int n, long lo
 
 using namespace ipcgpu;
 
-// full row structure of the symmetric matrix from its upper-triangular CSR (host, once per pattern)
-int solver_build_full_pattern(ipcgpu_ctx* ctx, const int* ia, const int* ja)
+// fia / fja / fpos of the pattern in ia / ja, rebuilt on the device when IterState::pat_version differs from the version they hold.  Nothing
+// synchronises.  fja / fpos hold 2 nnz entries of the host pattern, 2 nnz_capacity - n_rows of the device-built one (every row has its diagonal).
+int solver_full_pattern(ipcgpu_ctx* ctx)
 {
+    cudaStream_t st = ctx->stream;
     const int n = ctx->n_rows, base = ctx->index_base;
-    std::vector<int> cnt((size_t)n + 1, 0);
-    for (int i = 0; i < n; ++i)
-        for (int k = ia[i] - base; k < ia[i + 1] - base; ++k) {
-            const int j = ja[k] - base;
-            ++cnt[i + 1];
-            if (j != i) ++cnt[j + 1];
-        }
-    for (int i = 0; i < n; ++i) cnt[i + 1] += cnt[i];
-    const size_t nf = (size_t)cnt[n];
-    std::vector<int> fja(nf), fpos(nf), cur(cnt.begin(), cnt.end() - 1);
-    // lower part first per row (transposed entries arrive in ascending source row = ascending column), then the row's own upper entries
-    for (int i = 0; i < n; ++i)
-        for (int k = ia[i] - base; k < ia[i + 1] - base; ++k) {
-            const int j = ja[k] - base;
-            if (j != i) { fja[cur[j]] = i; fpos[cur[j]] = k; ++cur[j]; }
-        }
-    for (int i = 0; i < n; ++i)
-        for (int k = ia[i] - base; k < ia[i + 1] - base; ++k) {
-            fja[cur[i]] = ja[k] - base; fpos[cur[i]] = k; ++cur[i];
-        }
-    bool ok = ctx->fia.upload(cnt.data(), cnt.size(), ctx->stream) && ctx->fja.upload(fja.data(), nf, ctx->stream) && ctx->fpos.upload(fpos.data(), nf, ctx->stream);
-    if (!ok) {
-        ctx->err = "upload of the full-row pattern failed";
-        return IPCGPU_ERR_CUDA;
+    const size_t nf = ctx->device_pattern ? (size_t)(2 * ctx->pw.nnz_cap - n) : (size_t)2 * ctx->nnz;
+    size_t scan_bytes = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int*)nullptr, (int*)nullptr, n + 1, st));
+    const size_t n1 = (size_t)n + 1;
+    // (sizes fixed within an epoch: inside a capture, after an eager solve of the same epoch, nothing is allocated here)
+    bool ok = ctx->fia.reserve(n1) && ctx->fja.reserve(nf) && ctx->fpos.reserve(nf) && ctx->fp_start.reserve(n1) && ctx->fp_cur.reserve(n1)
+        && ctx->fp_tmp.reserve(std::max<size_t>(scan_bytes, 1));
+    if (ctx->fp_cnt.n < n1) { // (the ungated scan reads it: defined contents from the start)
+        ok = ok && ctx->fp_cnt.reserve(n1);
+        if (ok) CK(cudaMemsetAsync(ctx->fp_cnt.p, 0, n1 * sizeof(int), st));
     }
-    CK(cudaStreamSynchronize(ctx->stream));
-    ctx->full_pattern_ready = true;
-    return 0;
+    REQUIRE(ok, IPCGPU_ERR_CUDA, "allocation of the full-row pattern failed");
+    IterState* it = ctx->iter.p;
+    const int grid = std::min(nblk(n1, 256), kSMs * 8);
+    k_fp_gate<<<1, 32, 0, st>>>(it);
+    k_fp_zero<<<grid, 256, 0, st>>>(n, ctx->fp_cnt.p, it);
+    k_fp_count<<<grid, 256, 0, st>>>(n, ctx->ia.p, ctx->ja.p, base, ctx->fp_cnt.p, ctx->fp_cur.p, it);
+    CK(cub::DeviceScan::ExclusiveSum(ctx->fp_tmp.p, scan_bytes, ctx->fp_cnt.p, ctx->fp_start.p, n + 1, st));
+    k_fp_scatter<<<grid, 256, 0, st>>>(n, ctx->ia.p, ctx->ja.p, base, ctx->fp_start.p, ctx->fp_cnt.p, ctx->fp_cur.p, ctx->fja.p, ctx->fpos.p, it);
+    k_fp_sort<<<grid, 256, 0, st>>>(n, ctx->fp_start.p, ctx->fp_cur.p, ctx->fja.p, ctx->fpos.p, ctx->fia.p, it);
+    ctx->launches += 6; // (the scan counts as one)
+    CK(cudaGetLastError());
+    return IPCGPU_OK;
 }
 
-// PCG on the device-resident matrix.  rhs_dev: device vector (3 nV) scaled by `sign`.  The solution is left in ctx->sol.
-int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int* iters_out, double* rel_res_out)
+int solver_forget_full_pattern(ipcgpu_ctx* ctx)
+{
+    CK(cudaMemsetAsync(&ctx->iter.p->sv_fp_version, 0xff, sizeof(unsigned long long), ctx->stream));
+    return IPCGPU_OK;
+}
+
+int solver_finish(ipcgpu_ctx* ctx)
+{
+    const int n = ctx->n_rows;
+    k_abs_max<<<std::min(nblk(n, 256), kSMs * 4), 256, 0, ctx->stream>>>(n, ctx->sol.p, &ctx->iter.p->sv_xmax_ord);
+    ++ctx->launches;
+    CK(cudaGetLastError());
+    return IPCGPU_OK;
+}
+
+// PCG on the device-resident matrix.  rhs_dev: device vector (3 nV) scaled by `sign`.  The solution is left in ctx->sol, the result in
+// IterState (sv_*).  The workspace is reserved by the caller (solve_pcg in api_mesh.cu).
+int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter)
 {
     cudaStream_t st = ctx->stream;
     const int n = ctx->n_rows, nV = ctx->nV;
-    bool ok = ctx->sol.reserve(n) && ctx->pcg_r.reserve(n) && ctx->pcg_p.reserve(n) && ctx->pcg_q.reserve(n) && ctx->pcg_minv.reserve((size_t)6 * nV) && ctx->pcg_scal.reserve(8)
-        && ctx->pcg_hist.reserve((size_t)std::max(max_iter, 1) + 1);
-    if (!ok) {
-        ctx->err = "PCG workspace allocation failed";
-        return IPCGPU_ERR_CUDA;
-    }
     CK(cudaMemsetAsync(ctx->pcg_scal.p, 0, 8 * sizeof(double), st));
     k_block_jacobi<<<nblk(nV, 256), 256, 0, st>>>(nV, ctx->ia.p, ctx->index_base, ctx->a.p, ctx->pcg_minv.p);
     k_pcg_init<<<nblk(nV, 256), 256, 0, st>>>(nV, rhs_dev, sign, ctx->pcg_minv.p, ctx->sol.p, ctx->pcg_r.p, ctx->pcg_p.p, ctx->pcg_scal.p);
     ctx->launches += 2;
-    double* h = ctx->staging->pcg;
-    CK(cudaMemcpyAsync(h, ctx->pcg_scal.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    const double bb = h[4];
-    int it = 0;
-    double rr = bb;
-    const int check_every = 25; // the host looks at the residual every 25 iterations (one small read-back)
-    if (bb > 0.0) {
-        while (it < max_iter) {
-            const int burst = std::min(check_every, max_iter - it);
-            for (int b = 0; b < burst; ++b, ++it) {
-                k_spmv_dot<<<kSMs * 8, 256, 0, st>>>(n, ctx->fia.p, ctx->fja.p, ctx->fpos.p, ctx->a.p, ctx->pcg_p.p, ctx->pcg_q.p, ctx->pcg_scal.p, 1);
-                k_pcg_update<<<nblk(nV, 256), 256, 0, st>>>(nV, ctx->pcg_minv.p, ctx->pcg_p.p, ctx->pcg_q.p, ctx->sol.p, ctx->pcg_r.p, ctx->pcg_scal.p);
-                k_pcg_direction<<<nblk(n, 256), 256, 0, st>>>(n, ctx->pcg_q.p, ctx->pcg_p.p, ctx->pcg_scal.p);
-                k_pcg_roll<<<1, 32, 0, st>>>(ctx->pcg_scal.p, ctx->pcg_hist.p, it);
-                ctx->launches += 4;
-            }
-            CK(cudaMemcpyAsync(h, ctx->pcg_hist.p + (it - 1), sizeof(double), cudaMemcpyDeviceToHost, st));
-            CK(cudaStreamSynchronize(st));
-            rr = h[0];
-            if (!(rr == rr)) break; // NaN: the matrix was not positive definite
-            if (std::sqrt(rr) <= rel_tol * std::sqrt(bb)) break;
-        }
-    }
-    CK(cudaGetLastError());
-    if (iters_out) *iters_out = it;
-    if (rel_res_out) *rel_res_out = bb > 0.0 ? std::sqrt(rr / bb) : 0.0;
-    return 0;
+    int rc = decide(ctx, kSolveStart, rel_tol, max_iter, 0, nullptr, ctx->pcg_scal.p);
+    if (rc) return rc;
+    return krylov_loops(ctx, max_iter, [&]() {
+        cudaStream_t s = ctx->stream; // (the body's stream inside a capture)
+        k_spmv_dot<<<kSMs * 8, 256, 0, s>>>(n, ctx->fia.p, ctx->fja.p, ctx->fpos.p, ctx->a.p, ctx->pcg_p.p, ctx->pcg_q.p, ctx->pcg_scal.p, 1);
+        k_pcg_update<<<nblk(nV, 256), 256, 0, s>>>(nV, ctx->pcg_minv.p, ctx->pcg_p.p, ctx->pcg_q.p, ctx->sol.p, ctx->pcg_r.p, ctx->pcg_scal.p);
+        k_pcg_direction<<<nblk(n, 256), 256, 0, s>>>(n, ctx->pcg_q.p, ctx->pcg_p.p, ctx->pcg_scal.p);
+        k_pcg_roll<<<1, 32, 0, s>>>(ctx->pcg_scal.p, ctx->iter.p);
+        ctx->launches += 4;
+    });
 }
 
 // a direction produced on the device (src, or `dir` itself when src is NULL) becomes the search direction of the step-bound stages: pSize
@@ -246,7 +329,9 @@ int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src)
     cudaStream_t st = ctx->stream;
     if (src) CK(cudaMemcpyAsync(ctx->dir.p, src, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyDeviceToDevice, st));
     const int nb = ctx->nSV > 0 ? 64 : 0;
-    if (!ctx->partials.reserve(nb + 8) || !ctx->pSize_dev.reserve(1)) return IPCGPU_ERR_CUDA;
+    REQUIRE(!ctx->capturing || (ctx->partials.n >= (size_t)nb + 8 && ctx->pSize_dev.n >= 1), IPCGPU_ERR_STATE,
+        "adopt a search direction once outside a capture first (it sizes its workspace)");
+    REQUIRE(ctx->partials.reserve(nb + 8) && ctx->pSize_dev.reserve(1), IPCGPU_ERR_CUDA, "search-direction workspace allocation failed");
     long long nMeshSV = 0;
     for (int v : ctx->h_SVI) nMeshSV += v < ctx->nVdof ? 1 : 0;
     if (nb) k_psize<<<nb, 256, 0, st>>>(ctx->nSV, ctx->SVI.p, ctx->nVdof, ctx->dir.p, ctx->partials.p);

@@ -5,7 +5,9 @@
 //
 // Every decision is one single-thread kernel that reads IterState (energies, safeguard counts, flags), computes the next step in place
 // (IterState::step_ord) and writes the decision word IterState::ls_cond.  Outside a capture the host reads that word; inside one the kernel
-// also hands it to the conditional graph node that runs the loop body (cudaGraphSetConditional).  api_step.cu holds the two drivers.
+// also hands it to the conditional graph node that runs the loop body (cudaGraphSetConditional).  abi.h holds the two drivers (cond_node).
+// The Krylov loops of the linear solves (kSolveStart, kSolveBurst) are decided here too: their residual test is the host loop's, so
+// the iterations and the bits do not depend on which driver runs them.
 #include "common.cuh"
 #include "kernels.h"
 #include "../../include/ipcgpu.h"
@@ -64,7 +66,15 @@ DEV double energy_sum(const IterState* st, int terms)
 // the intersection safeguard: surface triangles crossed by an edge, and with half-spaces the vertices with d <= 0 (isIntersected, :2627-2642)
 DEV bool intersected(const IterState* st, int terms) { return st->checks[1] > 0 || ((terms & kTermHalfSpace) && st->hs_crossings > 0); }
 
-__global__ void k_step_decide(IterState* st, int op, double a, int b, cudaGraphConditionalHandle h)
+// the solve fails: the status its result reports and the flag the fetch reports (a line search refuses to start while it is raised)
+DEV void solve_fail(IterState* st)
+{
+    st->sv_run = 0;
+    st->sv_status = IPCGPU_ERR_SOLVE;
+    st->flags[FLAG_SOLVE] = 1;
+}
+
+__global__ void k_step_decide(IterState* st, int op, double a, int b, cudaGraphConditionalHandle h, const double* __restrict__ aux)
 {
     if (threadIdx.x != 0) return;
     int cond = 0;
@@ -100,6 +110,10 @@ __global__ void k_step_decide(IterState* st, int op, double a, int b, cudaGraphC
         st->ls_LF = alpha;
         cond = alpha > 0.0;
         if (!cond) st->sc_status = IPCGPU_ERR_LINE_SEARCH;
+        if (st->flags[FLAG_SOLVE]) { // the direction is that of a failed solve: V stays V0
+            cond = 0;
+            st->sc_status = IPCGPU_ERR_SOLVE;
+        }
         break;
     }
     case kLsStart: // :2681 E0 = E(V) with the sets held on entry;  b = energy terms
@@ -147,6 +161,26 @@ __global__ void k_step_decide(IterState* st, int op, double a, int b, cudaGraphC
         st->ls_LF = a;
         st->alpha_stage[0] = a; // the step the inversion filter starts from (it lowers it on Neo-Hookean meshes; no filter otherwise)
         break;
+    case kSolveStart: // after the solver's set-up;  a = rel_tol, b = max_iter, aux = the solver's scalars ([4] |b|^2, [6] a pivot <= 0)
+        st->sv_iters = 0;
+        st->sv_status = 0;
+        st->sv_max_iter = b;
+        st->sv_tol = a;
+        st->sv_bb = st->sv_rr = aux[4];
+        st->sv_xmax_ord = 0;
+        st->sv_run = aux[4] > 0.0;
+        if (aux[6] != 0.0) solve_fail(st);
+        break;
+    case kSolveBurst: // before a burst of b iterations, and after each: stop on a non-finite residual, on convergence (checked after a burst
+                      // only) or when the burst would pass max_iter.  Evaluated twice at one count (end of a loop, entry of the next), it
+                      // decides the same.
+        if (st->sv_run && st->sv_iters > 0) {
+            const double rr = st->sv_rr;
+            if (!(rr == rr)) solve_fail(st);
+            else if (sqrt(rr) <= st->sv_tol * sqrt(st->sv_bb)) st->sv_run = 0;
+        }
+        cond = st->sv_run && st->sv_iters + b <= st->sv_max_iter;
+        break;
     }
     st->ls_cond = cond;
     if (h) cudaGraphSetConditional(h, (unsigned)cond);
@@ -158,9 +192,9 @@ void cfl_pmax(int nSV, const int* SVI, int nVdof, const double* dir, IterState* 
     if (nSV > 0) k_cfl_pmax<<<std::min((nSV + 255) / 256, kSMs * 4), 256, 0, st>>>(nSV, SVI, nVdof, dir, &st_dev->sc_pmax_ord);
 }
 
-void step_decide(IterState* st_dev, int op, double a, int b, unsigned long long handle, cudaStream_t st)
+void step_decide(IterState* st_dev, int op, double a, int b, unsigned long long handle, cudaStream_t st, const double* aux)
 {
-    k_step_decide<<<1, 32, 0, st>>>(st_dev, op, a, b, (cudaGraphConditionalHandle)handle);
+    k_step_decide<<<1, 32, 0, st>>>(st_dev, op, a, b, (cudaGraphConditionalHandle)handle, aux);
 }
 
 } // namespace ipcgpu

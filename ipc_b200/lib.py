@@ -104,6 +104,7 @@ SIGNATURES = {
     "ipcgpu_csr_set_zero": (C.c_int, [_ctxp]),
     "ipcgpu_solve_pcg": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
     "ipcgpu_solve_pcg_multilevel": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
+    "ipcgpu_solve_info": (C.c_int, [_ctxp, C.c_void_p]),
     "ipcgpu_multilevel_info": (C.c_int, [_ctxp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]),
     "ipcgpu_multilevel_debug_matrices": (C.c_int, [_ctxp, _dp, C.c_uint64]),
     "ipcgpu_allreduce_grad_hess": (C.c_int, [_ctxp, C.c_int, C.c_int]),
@@ -180,6 +181,11 @@ class StepControl(C.Structure):
     _fields_ = [("alpha_cfl", C.c_double), ("alpha_feasible", C.c_double), ("alpha", C.c_double), ("energy_start", C.c_double), ("energy", C.c_double),
                 ("full_ccd", C.c_int), ("stopped", C.c_int), ("halvings_inversion", C.c_int), ("halvings_intersection", C.c_int),
                 ("halvings_armijo", C.c_int), ("halvings_post_check", C.c_int), ("post_check_rebuilt", C.c_int), ("status", C.c_int)]
+
+
+class SolveResult(C.Structure):
+    """ipcgpu_solve_result (include/ipcgpu.h)"""
+    _fields_ = [("iterations", C.c_int), ("rel_residual", C.c_double), ("max_abs_x", C.c_double), ("status", C.c_int)]
 
 
 class IpcGpuError(RuntimeError):
@@ -828,21 +834,32 @@ class Context:
     def allreduce_grad_hess(self, with_gradient=1, with_hessian=1):
         self._ck(self.lib.ipcgpu_allreduce_grad_hess(self.h, with_gradient, with_hessian))
 
-    def solve_pcg(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False):
-        """H x = rhs (None: -gradient, both device resident); returns (x or None, iterations, relative residual)"""
+    def _solve(self, fn, rhs, rel_tol, max_iter, want_x, adopt, deferred):
+        if deferred:  # H x = -g on the device, capturable; the result comes from solve_info()
+            if rhs is not None or want_x is True:
+                raise ValueError("the deferred solve takes the resident gradient and leaves x on the device: rhs=None, want_x=False")
+            self._ck(fn(self.h, None, rel_tol, int(max_iter), None, int(adopt), None, None))
+            return None
         x = np.empty(3 * self.nV) if want_x else None
         it, res = C.c_int(), C.c_double()
-        self._ck(self.lib.ipcgpu_solve_pcg(self.h, _d(f64(rhs)) if rhs is not None else None, rel_tol, int(max_iter), _d(x) if want_x else None, int(adopt),
-                                           C.byref(it), C.byref(res)))
+        self._ck(fn(self.h, _d(f64(rhs)) if rhs is not None else None, rel_tol, int(max_iter), _d(x) if want_x else None, int(adopt), C.byref(it),
+                    C.byref(res)))
         return x, it.value, res.value
 
-    def solve_pcg_multilevel(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False):
+    def solve_pcg(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False, deferred=False):
+        """H x = rhs (None: -gradient, both device resident); returns (x or None, iterations, relative residual).  deferred=True (rhs=None,
+        want_x=False): enqueued only, capturable; returns None, the result is solve_info()"""
+        return self._solve(self.lib.ipcgpu_solve_pcg, rhs, rel_tol, max_iter, want_x, adopt, deferred)
+
+    def solve_pcg_multilevel(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False, deferred=False):
         """solve_pcg with the multilevel additive Schwarz preconditioner (rebuilt from the resident matrix and positions at every call)"""
-        x = np.empty(3 * self.nV) if want_x else None
-        it, res = C.c_int(), C.c_double()
-        self._ck(self.lib.ipcgpu_solve_pcg_multilevel(self.h, _d(f64(rhs)) if rhs is not None else None, rel_tol, int(max_iter), _d(x) if want_x else None,
-                                                      int(adopt), C.byref(it), C.byref(res)))
-        return x, it.value, res.value
+        return self._solve(self.lib.ipcgpu_solve_pcg_multilevel, rhs, rel_tol, max_iter, want_x, adopt, deferred)
+
+    def solve_info(self):
+        """ipcgpu_solve_result of the last solve (its status is out.status, not raised)"""
+        out = SolveResult()
+        self.lib.ipcgpu_solve_info(self.h, C.byref(out))
+        return out
 
     def multilevel_info(self):
         """(domains per level, bytes of the stored inverses) of the last multilevel solve"""
