@@ -2,6 +2,7 @@
 // macros, the two chains of an iteration, and the prototypes of every host helper that crosses a file boundary.  Not installed.
 #pragma once
 #include "../../include/ipcgpu.h"
+#include "common.cuh"
 #include "context.h"
 #include <cstddef>
 #include <string>
@@ -240,8 +241,12 @@ int krylov_loops(ipcgpu_ctx* ctx, int max_iter, Iteration iteration)
 }
 int solver_full_pattern(ipcgpu_ctx* ctx);        // fia / fja / fpos of the pattern in ia / ja, rebuilt on the device when its version moved
 int solver_forget_full_pattern(ipcgpu_ctx* ctx); // a new pattern (ipcgpu_set_csr / ipcgpu_enable_device_pattern): the next solve rebuilds
-int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter);
-int solver_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter);
+// PCG with the block-Jacobi or the multilevel preconditioner; its workspace pcg_part holds kPcgSpmvBlocks SpMV partials, then 2 per CTA
+// of one thread per vertex
+constexpr int kPcgSpmvBlocks = ipcgpu::kSMs * 8;
+int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, bool multilevel);
+int solver_multilevel_build(ipcgpu_ctx* ctx, double* bad_pivot); // the hierarchy at the current matrix and positions (set-up)
+void solver_multilevel_step(ipcgpu_ctx* ctx, bool start);        // (iteration: the CG update first) z = M^-1 r, partials of r.z and r.r
 int solver_multilevel_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count);
 int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src); // src NULL: the direction already in ctx->dir
 int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity);

@@ -482,7 +482,7 @@ static int solve_pcg(ipcgpu_ctx* ctx, bool multilevel, const double* rhs, double
     if (rc) return rc;
     const int n = ctx->n_rows;
     bool ok = ctx->sol.reserve(n) && ctx->pcg_r.reserve(n) && ctx->pcg_p.reserve(n) && ctx->pcg_q.reserve(n) && ctx->pcg_scal.reserve(8)
-        && (multilevel || ctx->pcg_minv.reserve((size_t)6 * ctx->nV));
+        && ctx->pcg_part.reserve((size_t)kPcgSpmvBlocks + 2 * nblk(ctx->nV, 256)) && (multilevel || ctx->pcg_minv.reserve((size_t)6 * ctx->nV));
     REQUIRE(ok, IPCGPU_ERR_CUDA, "PCG workspace allocation failed");
     if ((rc = solver_full_pattern(ctx))) return rc; // (rows of both triangles, gathered through a position map; rebuilt when the pattern moved)
     const double* rhs_dev = ctx->g.p;
@@ -493,7 +493,7 @@ static int solve_pcg(ipcgpu_ctx* ctx, bool multilevel, const double* rhs, double
         rhs_dev = ctx->pcg_b.p;
         sign = 1.0;
     }
-    rc = (multilevel ? solver_pcg_multilevel : solver_pcg)(ctx, rhs_dev, sign, rel_tol, max_iter);
+    rc = solver_pcg(ctx, rhs_dev, sign, rel_tol, max_iter, multilevel);
     if (rc) return rc;
     ctx->sv_pending = true;
     if (!ctx->capturing) ctx->solve_epoch[multilevel] = ctx->epoch;

@@ -121,15 +121,7 @@ __global__ void __launch_bounds__(256) k_barrier_energy(BarrierArgs p, double* _
             }
         }
     }
-    __shared__ double sm[8];
-    double w = warp_sum(val);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = w;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-        for (int i = 0; i < 8; ++i) s += sm[i];
-        partials[blockIdx.x] = s;
-    }
+    cta_sum(&val, partials + blockIdx.x);
 }
 
 // -----------------------------------------------------------------------------------------------------------

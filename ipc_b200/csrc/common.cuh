@@ -46,4 +46,25 @@ DEV double warp_min(double v)
     return v;
 }
 
+// The fixed-order sum over a 256-thread CTA of N per-thread values v[0..N): warp shuffles, then the 8 warp sums in warp order starting
+// from +0.0; thread c writes the sum of v[c] to out[c].  Every thread of the CTA calls it.  The per-CTA partials of every deterministic
+// two-level sum come from here, so they all round alike.
+template <int N = 1>
+DEV void cta_sum(const double* v, double* out)
+{
+    __shared__ double sm[N][8];
+#pragma unroll
+    for (int c = 0; c < N; ++c) {
+        const double w = warp_sum(v[c]);
+        if ((threadIdx.x & 31) == 0) sm[c][threadIdx.x >> 5] = w;
+    }
+    __syncthreads();
+    if (threadIdx.x < N) {
+        double s = 0.0;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) s += sm[threadIdx.x][w];
+        out[threadIdx.x] = s;
+    }
+}
+
 } // namespace ipcgpu

@@ -121,7 +121,7 @@ struct PatternWork {
 // (96 x 96 doubles per domain, the levels one after the other) and the per-level restricted / coarse-solved vectors (96 per domain)
 constexpr int kMultilevelMax = 8; // levels: 32^8 vertices and more are out of reach of an int
 struct MultilevelWork {
-    DevBuf<double> box, inv, R, Y, part, chunk; // (part: per-CTA partials of the dot products; chunk: per-chunk shares of a level's assembly)
+    DevBuf<double> box, inv, R, Y, chunk; // (chunk: per-chunk shares of a level's assembly)
     DevBuf<unsigned> code, code_sorted;
     DevBuf<int> id, order, rank;
     DevBuf<unsigned char> sort_tmp, fixed; // (fixed: 1 for a vertex without degrees of freedom -- Dirichlet or obstacle tail)
@@ -288,7 +288,7 @@ struct ipcgpu_ctx {
     // allocations a capture relies on; sv_pending: a solve was enqueued since ipcgpu_solve_info read it
     ipcgpu::DevBuf<int> fia, fja, fpos, fp_cnt, fp_start, fp_cur;
     ipcgpu::DevBuf<unsigned char> fp_tmp;
-    ipcgpu::DevBuf<double> sol, pcg_b, pcg_r, pcg_p, pcg_q, pcg_minv, pcg_scal;
+    ipcgpu::DevBuf<double> sol, pcg_b, pcg_r, pcg_p, pcg_q, pcg_minv, pcg_scal, pcg_part; // (pcg_part: per-CTA partials of the dot products)
     ipcgpu::MultilevelWork ml;
     uint64_t solve_epoch[2] = { ~0ull, ~0ull };
     bool sv_pending = false, sv_pending_at_capture = false;

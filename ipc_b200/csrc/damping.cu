@@ -22,21 +22,6 @@ DEV void displacement(int nV, const double* __restrict__ x, const double* __rest
     for (int c = 0; c < 3; ++c) d[c] = zero ? 0.0 : x[(size_t)c * nV + v] - xp[(size_t)c * nV + v];
 }
 
-// per-CTA partial of a 256-thread block
-DEV void block_partial(double e, double* __restrict__ partials)
-{
-    __shared__ double sm[8];
-    const double w = warp_sum(e);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = w;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s += sm[i];
-        partials[blockIdx.x] = s;
-    }
-}
-
 // ---- damping ---------------------------------------------------------------------------------------------------------------------
 // computeDampingMtr's assembly (Energy.cpp:317-330 with projectDBC = 1 -> IglUtils::addBlockToMatrix, IglUtils.hpp:44-80) into slot storage:
 // the per-tet blocks of k_elastic_grad_hess (Hessian only, coef, projected) summed in ascending tet order as k_assemble_csr sums them; a block
@@ -84,7 +69,7 @@ __global__ void __launch_bounds__(256) k_damping_energy(int nSlots, const int* _
         for (int r = 0; r < 3; ++r) e += dv[r] * ((B[3 * r] * du[0] + B[3 * r + 1] * du[1]) + B[3 * r + 2] * du[2]);
         if (v != u) e *= 2.0;
     }
-    block_partial(e, partials);
+    cta_sum(&e, partials + blockIdx.x);
 }
 
 // g += D d (:3519-3540), d zeroed on the projected Dirichlet vertices: one thread per vertex gathers its row of the symmetric product over
@@ -143,7 +128,7 @@ __global__ void __launch_bounds__(256) k_neumann_energy(int nV, const double* __
         const double dot = (x[v] * f[3 * (size_t)v] + x[(size_t)nV + v] * f[3 * (size_t)v + 1]) + x[2 * (size_t)nV + v] * f[3 * (size_t)v + 2];
         e = -((coef * mass[v]) * dot);
     }
-    block_partial(e, partials);
+    cta_sum(&e, partials + blockIdx.x);
 }
 __global__ void __launch_bounds__(256) k_neumann_gradient(int nV, const double* __restrict__ f, const double* __restrict__ mass, const uint8_t* __restrict__ dbc,
     const double* __restrict__ coef, double* __restrict__ g)
@@ -177,7 +162,7 @@ __global__ void __launch_bounds__(256) k_dirichlet_energy(int n, const int* __re
         const double m = mass[v];
         e = rho / 2.0 * m * sq - sqrt(m) * ((l[0] * dx[0] + l[1] * dx[1]) + l[2] * dx[2]);
     }
-    block_partial(e, partials);
+    cta_sum(&e, partials + blockIdx.x);
 }
 __global__ void __launch_bounds__(256) k_dirichlet_gradient(int n, const int* __restrict__ vid, const double* __restrict__ tgt, const double* __restrict__ lam,
     int nV, const double* __restrict__ x, const double* __restrict__ mass, const double* __restrict__ rho_p, double* __restrict__ g)
@@ -227,7 +212,7 @@ __global__ void __launch_bounds__(256) k_dirichlet_sqnorm(int n, const int* __re
         double dx[3];
         e = sq_dist(nV, x, vid[i], tgt + 3 * (size_t)i, dx);
     }
-    block_partial(e, partials);
+    cta_sum(&e, partials + blockIdx.x);
 }
 __global__ void k_dirichlet_step(const double* __restrict__ tol_p, double* __restrict__ s)
 {

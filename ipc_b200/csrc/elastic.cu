@@ -79,16 +79,7 @@ __global__ void __launch_bounds__(256) k_elastic_energy(ElasticArgs p, double* _
         e = psi<ENERGY>(s, in.mu, in.lam) * in.vol;
         if (e_per_tet) e_per_tet[tt] = e;
     }
-    __shared__ double sm[8];
-    double w = warp_sum(e);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = w;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s += sm[i];
-        partials[blockIdx.x] = s;
-    }
+    cta_sum(&e, partials + blockIdx.x);
 }
 
 // single-CTA fixed-order reduction of the per-CTA partials: out[0] = scale * sum

@@ -146,15 +146,7 @@ __global__ void __launch_bounds__(256) k_friction_energy(FrictionArgs p, double*
         const double x2 = f.u0 * f.u0 + f.u1 * f.u1;
         val += (x2 > p.eps2) ? p.lambda[c] * sqrt(x2) : p.lambda[c] * f0_SF(x2, eps);
     }
-    __shared__ double sm[8];
-    const double w = warp_sum(val);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = w;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-        for (int i = 0; i < 8; ++i) s += sm[i];
-        partials[blockIdx.x] = s;
-    }
+    cta_sum(&val, partials + blockIdx.x);
 }
 
 __global__ void __launch_bounds__(128) k_friction_gradient(FrictionArgs p, double* __restrict__ g)

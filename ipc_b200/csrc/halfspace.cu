@@ -35,20 +35,6 @@ DEV bool codim3(const int* vCoDim, int v) { return !vCoDim || vCoDim[v] == 3; }
 DEV bool is_dbc(const uint8_t* dbc, int v) { return dbc && dbc[v] != 0; }
 DEV bool owned(const HalfSpaceArgs& p, int v) { return v >= p.row_lo && v < p.row_hi; }
 
-template <int kThreads>
-DEV void block_partial(double val, double* partials)
-{
-    __shared__ double sm[kThreads / 32];
-    const double w = warp_sum(val);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = w;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-        for (int i = 0; i < kThreads / 32; ++i) s += sm[i];
-        partials[blockIdx.x] = s;
-    }
-}
-
 // ---- active set: flag, scan, scatter ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_hs_flags(HalfSpaceArgs p, double dHat, int* __restrict__ flags)
 {
@@ -95,7 +81,7 @@ __global__ void __launch_bounds__(256) k_hs_energy(HalfSpaceArgs p, double dHat,
         barrier_all(d, dHat, b, db, d2b);
         val += b;
     }
-    block_partial<256>(val, partials);
+    cta_sum(&val, partials + blockIdx.x);
 }
 
 __global__ void __launch_bounds__(128) k_hs_gradient(HalfSpaceArgs p, double dHat, double kappa, double* __restrict__ g)
@@ -241,7 +227,7 @@ __global__ void __launch_bounds__(256) k_hs_fric_energy(HalfSpaceArgs p, double 
         const double m = pl[7] * p.lam[c];
         val += (s.mag2 > eps2) ? m * (sqrt(s.mag2) - eps * 0.5) : m * s.mag2 / eps * 0.5; // HalfSpace.cpp:289-294
     }
-    block_partial<256>(val, partials);
+    cta_sum(&val, partials + blockIdx.x);
 }
 
 __global__ void __launch_bounds__(128) k_hs_fric_gradient(HalfSpaceArgs p, double eps2, double* __restrict__ g)

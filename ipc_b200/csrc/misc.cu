@@ -38,16 +38,7 @@ __global__ void __launch_bounds__(256) k_inertia_energy(int v0, int v1, int nV, 
         }
         e = s * mass[v] / 2.0;
     }
-    __shared__ double sm[8];
-    const double w = warp_sum(e);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = w;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s += sm[i];
-        partials[blockIdx.x] = s;
-    }
+    cta_sum(&e, partials + blockIdx.x);
 }
 // ... and of computeGradient (:3439-3450): g_v += m_v (x_v - xtilde_v) unless v is a projected Dirichlet vertex
 __global__ void __launch_bounds__(256) k_inertia_gradient(int nV, const double* __restrict__ x, const double* __restrict__ xt, const double* __restrict__ mass,

@@ -1,7 +1,8 @@
 // multilevel.cu -- conjugate gradients on the device-resident matrix, preconditioned by a multilevel additive Schwarz hierarchy (MAS: Wu,
 // Wang, Wang, "A GPU-based multilevel additive Schwarz preconditioner for cloth and deformable body simulation", 2022) that is rebuilt from
-// the matrix and the current positions at every solve.  The second built-in solver next to solve.cu's block-Jacobi PCG: same Krylov
-// recurrences, same contract (right-hand side from the resident gradient, solution left where the step-bound stages read it).
+// the matrix and the current positions at every solve.  This file holds the hierarchy and its step of solve.cu's Krylov loop (solver_pcg),
+// which it shares with the block-Jacobi preconditioner: same recurrences, same contract (right-hand side from the resident gradient,
+// solution left where the step-bound stages read it).
 //
 // Order.   Vertices (obstacle tail included) are sorted by a 30-bit Morton code of their current position: 10 bits per axis of the cube
 //          that spans the largest extent of their bounding box (one cell size on every axis, so that a thin body is not cut into layers),
@@ -25,10 +26,9 @@
 //          sums the 32 children of each aggregate from level l-1's restricted vector: a fixed shuffle tree), multiply by the stored inverse
 //          (coalesced rows, warp reductions).  One kernel per vertex then adds the levels' contributions in level order and leaves the
 //          per-CTA partials of r.z and r.r.
-// Krylov.  Every dot product is a fixed-order two-level sum (per-CTA partials, then one CTA), so two solves of one system give identical
-//          bits: the direction feeds Armijo decisions (DESIGN 3.13).  The loop is solve.cu's (krylov_loops, abi.h): the residual test runs
-//          on the device every 25 iterations, read by the host outside a capture, a conditional graph node inside one; set-up and
-//          application never synchronise.
+// Step.    In an iteration: p.Ap = k_reduce_sum of the SpMV's partials, then x += alpha p, r -= alpha Ap (k_ml_update); then the levels
+//          and k_ml_prolong.  6 + L launches per iteration with the SpMV, roll and direction of solve.cu; set-up and step never
+//          synchronise.
 //
 // Memory: the stored inverses (73,728 bytes per domain, 0.61 GB at 257 k vertices) and the level vectors stay allocated for the life of the
 // context after the first call, like every workspace of the context.
@@ -302,24 +302,6 @@ __global__ void __launch_bounds__(256) k_ml_level(int nV, int level, long long n
     }
 }
 
-// fixed-order sum of two per-thread values over a 256-thread CTA: warp shuffles, then the 8 warps in order
-DEV void cta_partials2(double s0, double s1, double* __restrict__ out)
-{
-    __shared__ double sm[2][8];
-    s0 = warp_sum(s0);
-    s1 = warp_sum(s1);
-    if ((threadIdx.x & 31) == 0) {
-        sm[0][threadIdx.x >> 5] = s0;
-        sm[1][threadIdx.x >> 5] = s1;
-    }
-    __syncthreads();
-    if (threadIdx.x < 2) {
-        double t = 0.0;
-        for (int w = 0; w < 8; ++w) t += sm[threadIdx.x][w];
-        out[threadIdx.x] = t;
-    }
-}
-
 // z = sum over the levels, in level order, of the coarse solution of the vertex's aggregate (level 0 alone for a vertex without degrees of
 // freedom); partials of r.z and r.r (2 per CTA)
 __global__ void __launch_bounds__(256) k_ml_prolong(int nV, MlLevels lv, const int* __restrict__ rank, const unsigned char* __restrict__ fixed, const double* __restrict__ Y,
@@ -327,7 +309,7 @@ __global__ void __launch_bounds__(256) k_ml_prolong(int nV, MlLevels lv, const i
     double* __restrict__ z, double* __restrict__ part)
 {
     const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    double rz = 0.0, rr = 0.0;
+    double rz_rr[2] = { 0.0, 0.0 };
     if (v < nV) {
         const long long rk = rank[v];
         const int n_lv = fixed[v] ? 1 : lv.n;
@@ -343,51 +325,14 @@ __global__ void __launch_bounds__(256) k_ml_prolong(int nV, MlLevels lv, const i
         for (int c = 0; c < 3; ++c) {
             const double rc = r[3 * (size_t)v + c];
             z[3 * (size_t)v + c] = s[c];
-            rz += rc * s[c];
-            rr += rc * rc;
+            rz_rr[0] += rc * s[c];
+            rz_rr[1] += rc * rc;
         }
     }
-    cta_partials2(rz, rr, part + 2 * blockIdx.x);
+    cta_sum<2>(rz_rr, part + 2 * blockIdx.x);
 }
 
-// ---- the Krylov loop --------------------------------------------------------------------------------------------------------
-// scal: [0] r.z, [1] p.Ap, [3] |r|^2, [4] |b|^2, [5] beta, [6] a domain had a non-positive pivot
-__global__ void __launch_bounds__(256) k_ml_init(int n, const double* __restrict__ src, double sign, double* __restrict__ x, double* __restrict__ r, double* __restrict__ p)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    x[i] = 0.0;
-    p[i] = 0.0;
-    r[i] = sign * src[i];
-}
-
-// y = A x over full rows (one warp per row, rows dealt to the warps of a fixed grid), partial of x.y per CTA
-__global__ void __launch_bounds__(256) k_ml_spmv(int n, const int* __restrict__ fia, const int* __restrict__ fja, const int* __restrict__ fpos, const double* __restrict__ a,
-    const double* __restrict__ x, double* __restrict__ y, double* __restrict__ part)
-{
-    const int lane = threadIdx.x & 31;
-    const int row0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    double acc = 0.0;
-    for (int row = row0; row < n; row += (gridDim.x * blockDim.x) >> 5) {
-        double s = 0.0;
-        for (int k = fia[row] + lane; k < fia[row + 1]; k += 32) s += __ldg(a + fpos[k]) * __ldg(x + fja[k]);
-        s = warp_sum(s);
-        if (lane == 0) {
-            y[row] = s;
-            acc += x[row] * s;
-        }
-    }
-    __shared__ double sm[8];
-    if (lane == 0) sm[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0.0;
-        for (int w = 0; w < 8; ++w) t += sm[w];
-        part[blockIdx.x] = t;
-    }
-}
-
-// x += alpha p ; r -= alpha Ap       with alpha = r.z / p.Ap
+// the CG update of an iteration: x += alpha p ; r -= alpha Ap       with alpha = r.z / p.Ap (scal: solve.cu's layout)
 __global__ void __launch_bounds__(256) k_ml_update(int n, const double* __restrict__ p, const double* __restrict__ Ap, double* __restrict__ x, double* __restrict__ r,
     const double* __restrict__ scal)
 {
@@ -397,48 +342,6 @@ __global__ void __launch_bounds__(256) k_ml_update(int n, const double* __restri
     if (i >= n) return;
     x[i] += alpha * p[i];
     r[i] -= alpha * Ap[i];
-}
-
-// after an application: r.z and |r|^2 from the partials, beta = r.z / (the previous r.z) (0 at the start), |r|^2 and the count of the
-// solve in flight (start: |b|^2 instead)
-__global__ void __launch_bounds__(1024) k_ml_roll(const double* __restrict__ part, int n_part, double* __restrict__ scal, IterState* __restrict__ st, int start)
-{
-    __shared__ double sm[2][32];
-    double s0 = 0.0, s1 = 0.0;
-    for (int i = threadIdx.x; i < n_part; i += blockDim.x) {
-        s0 += part[2 * i];
-        s1 += part[2 * i + 1];
-    }
-    s0 = warp_sum(s0);
-    s1 = warp_sum(s1);
-    if ((threadIdx.x & 31) == 0) {
-        sm[0][threadIdx.x >> 5] = s0;
-        sm[1][threadIdx.x >> 5] = s1;
-    }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        s0 = warp_sum(sm[0][threadIdx.x]);
-        s1 = warp_sum(sm[1][threadIdx.x]);
-        if (threadIdx.x == 0) {
-            const double rz_old = scal[0];
-            scal[5] = rz_old != 0.0 ? s0 / rz_old : 0.0;
-            scal[0] = s0;
-            scal[3] = s1;
-            if (start) scal[4] = s1; // r = b
-            else {
-                st->sv_rr = s1;
-                ++st->sv_iters;
-            }
-        }
-    }
-}
-
-// p = z + beta p
-__global__ void __launch_bounds__(256) k_ml_direction(int n, const double* __restrict__ z, double* __restrict__ p, const double* __restrict__ scal)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const double beta = scal[5];
-    if (i < n) p[i] = z[i] + beta * p[i];
 }
 
 } // namespace ipcgpu
@@ -492,8 +395,8 @@ static int multilevel_matrices(ipcgpu_ctx* ctx)
     return IPCGPU_OK;
 }
 
-// ... and their inverses in place; a pivot <= 0 leaves 1.0 in *bad_pivot
-static int multilevel_build(ipcgpu_ctx* ctx, double* bad_pivot)
+// ... and their inverses in place: the set-up of a multilevel solve; a pivot <= 0 leaves 1.0 in *bad_pivot
+int solver_multilevel_build(ipcgpu_ctx* ctx, double* bad_pivot)
 {
     MultilevelWork& w = ctx->ml;
     int rc = multilevel_matrices(ctx);
@@ -519,11 +422,19 @@ int solver_multilevel_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count)
     return IPCGPU_OK;
 }
 
-// z = M^-1 r, and the partials of r.z and r.r
-static void multilevel_apply(ipcgpu_ctx* ctx, const double* r, double* z, double* part)
+// the multilevel step of solver_pcg (solve.cu).  In an iteration: p.Ap = the sum of the SpMV's partials, then the CG update.  Then
+// z = M^-1 r in pcg_q, and the partials of r.z and r.r behind the SpMV's.
+void solver_multilevel_step(ipcgpu_ctx* ctx, bool start)
 {
     cudaStream_t st = ctx->stream;
     MultilevelWork& w = ctx->ml;
+    const double* r = ctx->pcg_r.p;
+    double *z = ctx->pcg_q.p, *part = ctx->pcg_part.p;
+    if (!start) {
+        reduce_sum(part, kPcgSpmvBlocks, 1.0, ctx->pcg_scal.p + 1, st);
+        k_ml_update<<<nblk(ctx->n_rows, 256), 256, 0, st>>>(ctx->n_rows, ctx->pcg_p.p, z, ctx->sol.p, ctx->pcg_r.p, ctx->pcg_scal.p);
+        ctx->launches += 2;
+    }
     MlLevels lv;
     lv.n = w.levels;
     for (int l = 0; l < w.levels; ++l) {
@@ -531,37 +442,6 @@ static void multilevel_apply(ipcgpu_ctx* ctx, const double* r, double* z, double
         k_ml_level<<<(unsigned)w.domains[l], 256, 0, st>>>(ctx->nV, l, l ? w.domains[l - 1] * kAgg : 0, w.order.p, w.fixed.p, r, l ? w.R.p + lv.off[l - 1] : nullptr, w.R.p + lv.off[l],
             w.inv.p + w.tile_off[l] * kTile2, w.Y.p + lv.off[l]);
     }
-    k_ml_prolong<<<nblk(ctx->nV, 256), 256, 0, st>>>(ctx->nV, lv, w.rank.p, w.fixed.p, w.Y.p, r, z, part);
+    k_ml_prolong<<<nblk(ctx->nV, 256), 256, 0, st>>>(ctx->nV, lv, w.rank.p, w.fixed.p, w.Y.p, r, z, part + kPcgSpmvBlocks);
     ctx->launches += w.levels + 1;
-}
-
-// PCG on the device-resident matrix with the multilevel preconditioner.  rhs_dev: device vector (3 nV) scaled by `sign`.  The solution is
-// left in ctx->sol, the result in IterState (sv_*); a pivot <= 0 of the set-up is the solve's failure (kSolveStart).  The Krylov workspace is
-// reserved by the caller (solve_pcg in api_mesh.cu), ml.part here.
-int solver_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter)
-{
-    cudaStream_t st = ctx->stream;
-    const int n = ctx->n_rows;
-    const int spmv_blocks = kSMs * 8, vec_blocks = nblk(ctx->nV, 256);
-    REQUIRE(ctx->ml.part.reserve((size_t)std::max(spmv_blocks, 2 * vec_blocks)), IPCGPU_ERR_CUDA, "PCG workspace allocation failed");
-    CK(cudaMemsetAsync(ctx->pcg_scal.p, 0, 8 * sizeof(double), st));
-    int rc = multilevel_build(ctx, ctx->pcg_scal.p + 6);
-    if (rc) return rc;
-    double *x = ctx->sol.p, *r = ctx->pcg_r.p, *p = ctx->pcg_p.p, *q = ctx->pcg_q.p, *scal = ctx->pcg_scal.p, *part = ctx->ml.part.p;
-    k_ml_init<<<nblk(n, 256), 256, 0, st>>>(n, rhs_dev, sign, x, r, p);
-    multilevel_apply(ctx, r, q, part);
-    k_ml_roll<<<1, 1024, 0, st>>>(part, vec_blocks, scal, ctx->iter.p, 1);
-    k_ml_direction<<<nblk(n, 256), 256, 0, st>>>(n, q, p, scal);
-    ctx->launches += 3;
-    if ((rc = decide(ctx, kSolveStart, rel_tol, max_iter, 0, nullptr, scal))) return rc;
-    return krylov_loops(ctx, max_iter, [&]() {
-        cudaStream_t s = ctx->stream; // (the body's stream inside a capture)
-        k_ml_spmv<<<spmv_blocks, 256, 0, s>>>(n, ctx->fia.p, ctx->fja.p, ctx->fpos.p, ctx->a.p, p, q, part);
-        reduce_sum(part, spmv_blocks, 1.0, scal + 1, s);
-        k_ml_update<<<nblk(n, 256), 256, 0, s>>>(n, p, q, x, r, scal);
-        multilevel_apply(ctx, r, q, part); // z in Ap's storage
-        k_ml_roll<<<1, 1024, 0, s>>>(part, vec_blocks, scal, ctx->iter.p, 0);
-        k_ml_direction<<<nblk(n, 256), 256, 0, s>>>(n, q, p, scal);
-        ctx->launches += 5;
-    });
 }

@@ -4,9 +4,14 @@
 // Optimizer::computeSearchDir (src/TimeStepper/Optimizer.cpp:2324-2355), i.e. CHOLMODSolver.cpp:123-154.  The north star keeps the sparse
 // Cholesky a black box (CHOLMOD / cuDSS); cuDSS is not in this image, so the production binding is documented in INTEGRATION.md
 // (ipcgpu_device_ptr hands cuDSS the device-resident ia / ja / a) and what is BUILT here is the hand-off itself plus a reference solver
-// that runs entirely on the device: a block-Jacobi preconditioned conjugate gradient on the upper-triangular CSR the assembly stages fill.
-// It takes its right-hand side from the device-resident gradient and leaves the search direction where the step-bound stages read it,
-// so that a whole Newton iteration (assembly -> solve -> CCD) needs no host transfer of any vertex- or matrix-sized array.
+// that runs entirely on the device: a preconditioned conjugate gradient on the upper-triangular CSR the assembly stages fill, with the
+// block-Jacobi preconditioner (here) or the multilevel one (multilevel.cu).  It takes its right-hand side from the device-resident gradient
+// and leaves the search direction where the step-bound stages read it, so that a whole Newton iteration (assembly -> solve -> CCD) needs no
+// host transfer of any vertex- or matrix-sized array.
+//
+// One Krylov loop (solver_pcg) for both preconditioners: init, SpMV with per-CTA partials, the preconditioner's step, roll, direction.
+// Every dot product is a fixed-order two-level sum (per-CTA partials, then one order for every launch), so two solves of one system give
+// identical bits with either preconditioner: an adopted direction feeds the Armijo and step-bound decisions (DESIGN 3.13 / 3.17).
 //
 // SpMV on a symmetric matrix stored by its upper triangle: the device builds the FULL row structure once per pattern (col index + position
 // of the value inside the upper-triangular array for every entry of both triangles), so the product is a plain deterministic row-parallel
@@ -27,25 +32,6 @@
 #include <cub/cub.cuh>
 
 namespace ipcgpu {
-
-// y = A x over full rows; dot(x, y) accumulated into scal[slot] (one warp per row)
-__global__ void __launch_bounds__(256) k_spmv_dot(int n, const int* __restrict__ fia, const int* __restrict__ fja, const int* __restrict__ fpos, const double* __restrict__ a,
-    const double* __restrict__ x, double* __restrict__ y, double* __restrict__ scal, int slot)
-{
-    const int lane = threadIdx.x & 31;
-    const int row0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    double acc = 0.0;
-    for (int row = row0; row < n; row += (gridDim.x * blockDim.x) >> 5) {
-        double s = 0.0;
-        for (int k = fia[row] + lane; k < fia[row + 1]; k += 32) s += __ldg(a + fpos[k]) * __ldg(x + fja[k]);
-        s = warp_sum(s);
-        if (lane == 0) {
-            y[row] = s;
-            acc += x[row] * s;
-        }
-    }
-    if (lane == 0 && acc != 0.0) atomicAdd(scal + slot, acc);
-}
 
 // block-Jacobi preconditioner: inverse of the 3x3 diagonal block of every vertex (row 3v: [d00 d01 d02], row 3v+1: [d11 d12], row 3v+2: [d22])
 __global__ void __launch_bounds__(256) k_block_jacobi(int nV, const int* __restrict__ ia, int base, const double* __restrict__ a, double* __restrict__ Minv /* 6 per vertex */)
@@ -68,76 +54,115 @@ __global__ void __launch_bounds__(256) k_block_jacobi(int nV, const int* __restr
     m[5] = (d00 * d11 - d01 * d01) * id;
 }
 
-// scal: [0] rz, [1] pAp, [2] rz_new, [3] |r|^2, [4] |b|^2
-// init: r = b (= sign * src), x = 0, z = Minv r, p = z, rz = r.z
-__global__ void __launch_bounds__(256) k_pcg_init(int nV, const double* __restrict__ src, double sign, const double* __restrict__ Minv, double* __restrict__ x, double* __restrict__ r,
-    double* __restrict__ p, double* __restrict__ scal)
+// block-Jacobi step, one thread per vertex.  In an iteration (dot != NULL): x += alpha p, r -= alpha Ap with alpha = r.z / p.Ap, p.Ap the
+// sum of the SpMV's n_dot partials, added by every CTA in the same order (so every CTA has the same alpha, with no launch of its own).
+// Then z = Minv r in Ap's storage, and the partials of r.z and r.r.
+__global__ void __launch_bounds__(256) k_block_jacobi_step(int nV, const double* __restrict__ Minv, const double* __restrict__ p, double* __restrict__ Ap_z,
+    double* __restrict__ x, double* __restrict__ r, const double* __restrict__ scal, const double* __restrict__ dot, int n_dot, double* __restrict__ part)
 {
     const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    double rz = 0.0, bb = 0.0;
-    if (v < nV) {
-        const double r0 = sign * src[3 * (size_t)v], r1 = sign * src[3 * (size_t)v + 1], r2 = sign * src[3 * (size_t)v + 2];
-        const double* m = Minv + 6 * (size_t)v;
-        const double z0 = m[0] * r0 + m[1] * r1 + m[2] * r2, z1 = m[1] * r0 + m[3] * r1 + m[4] * r2, z2 = m[2] * r0 + m[4] * r1 + m[5] * r2;
-        for (int c = 0; c < 3; ++c) x[3 * (size_t)v + c] = 0.0;
-        r[3 * (size_t)v] = r0; r[3 * (size_t)v + 1] = r1; r[3 * (size_t)v + 2] = r2;
-        p[3 * (size_t)v] = z0; p[3 * (size_t)v + 1] = z1; p[3 * (size_t)v + 2] = z2;
-        rz = r0 * z0 + r1 * z1 + r2 * z2;
-        bb = r0 * r0 + r1 * r1 + r2 * r2;
+    __shared__ double pAp;
+    if (dot) {
+        double s = 0.0;
+        for (int i = threadIdx.x; i < n_dot; i += blockDim.x) s += dot[i];
+        cta_sum(&s, &pAp);
+        __syncthreads();
     }
-    rz = warp_sum(rz);
-    bb = warp_sum(bb);
-    if ((threadIdx.x & 31) == 0) {
-        if (rz != 0.0) atomicAdd(scal + 0, rz);
-        if (bb != 0.0) atomicAdd(scal + 4, bb);
-    }
-}
-// x += alpha p ; r -= alpha Ap ; z = Minv r (kept in Ap's storage) ; rz_new = r.z ; |r|^2       with alpha = rz / pAp
-__global__ void __launch_bounds__(256) k_pcg_update(int nV, const double* __restrict__ Minv, const double* __restrict__ p, double* __restrict__ Ap_z, double* __restrict__ x,
-    double* __restrict__ r, double* __restrict__ scal)
-{
-    const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    const double pAp = scal[1];
-    const double alpha = pAp != 0.0 ? scal[0] / pAp : 0.0;
-    double rz = 0.0, rr = 0.0;
+    double rz_rr[2] = { 0.0, 0.0 };
     if (v < nV) {
+        const double alpha = dot && pAp != 0.0 ? scal[0] / pAp : 0.0;
         double rv[3];
         for (int c = 0; c < 3; ++c) {
             const size_t i = 3 * (size_t)v + c;
-            x[i] += alpha * p[i];
-            rv[c] = r[i] - alpha * Ap_z[i];
-            r[i] = rv[c];
+            rv[c] = r[i];
+            if (dot) {
+                x[i] += alpha * p[i];
+                rv[c] -= alpha * Ap_z[i];
+                r[i] = rv[c];
+            }
         }
         const double* m = Minv + 6 * (size_t)v;
         const double z0 = m[0] * rv[0] + m[1] * rv[1] + m[2] * rv[2], z1 = m[1] * rv[0] + m[3] * rv[1] + m[4] * rv[2], z2 = m[2] * rv[0] + m[4] * rv[1] + m[5] * rv[2];
         Ap_z[3 * (size_t)v] = z0; Ap_z[3 * (size_t)v + 1] = z1; Ap_z[3 * (size_t)v + 2] = z2;
-        rz = rv[0] * z0 + rv[1] * z1 + rv[2] * z2;
-        rr = rv[0] * rv[0] + rv[1] * rv[1] + rv[2] * rv[2];
+        rz_rr[0] = rv[0] * z0 + rv[1] * z1 + rv[2] * z2;
+        rz_rr[1] = rv[0] * rv[0] + rv[1] * rv[1] + rv[2] * rv[2];
     }
-    rz = warp_sum(rz);
-    rr = warp_sum(rr);
+    cta_sum<2>(rz_rr, part + 2 * blockIdx.x);
+}
+
+// ---- the Krylov loop of both solvers ----------------------------------------------------------------------------------------
+// scal: [0] r.z, [1] p.Ap (multilevel), [3] |r|^2, [4] |b|^2, [5] beta, [6] a domain of the multilevel set-up had a non-positive pivot
+// x = 0, p = 0, r = sign * src
+__global__ void __launch_bounds__(256) k_pcg_init(int n, const double* __restrict__ src, double sign, double* __restrict__ x, double* __restrict__ r, double* __restrict__ p)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    x[i] = 0.0;
+    p[i] = 0.0;
+    r[i] = sign * src[i];
+}
+
+// y = A x over full rows (one warp per row, rows dealt to the warps of a fixed grid), partial of x.y per CTA
+__global__ void __launch_bounds__(256) k_pcg_spmv(int n, const int* __restrict__ fia, const int* __restrict__ fja, const int* __restrict__ fpos, const double* __restrict__ a,
+    const double* __restrict__ x, double* __restrict__ y, double* __restrict__ part)
+{
+    const int lane = threadIdx.x & 31;
+    const int row0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    double acc = 0.0; // (lane 0's; the other lanes add +0.0)
+    for (int row = row0; row < n; row += (gridDim.x * blockDim.x) >> 5) {
+        double s = 0.0;
+        for (int k = fia[row] + lane; k < fia[row + 1]; k += 32) s += __ldg(a + fpos[k]) * __ldg(x + fja[k]);
+        s = warp_sum(s);
+        if (lane == 0) {
+            y[row] = s;
+            acc += x[row] * s;
+        }
+    }
+    cta_sum(&acc, part + blockIdx.x);
+}
+
+// after a preconditioner step: r.z and |r|^2 from its partials, beta = r.z / (the previous r.z) (0 at the start), |r|^2 and the count of
+// the solve in flight (start: |b|^2 instead)
+__global__ void __launch_bounds__(1024) k_pcg_roll(const double* __restrict__ part, int n_part, double* __restrict__ scal, IterState* __restrict__ st, int start)
+{
+    __shared__ double sm[2][32];
+    double s0 = 0.0, s1 = 0.0;
+    for (int i = threadIdx.x; i < n_part; i += blockDim.x) {
+        s0 += part[2 * i];
+        s1 += part[2 * i + 1];
+    }
+    s0 = warp_sum(s0);
+    s1 = warp_sum(s1);
     if ((threadIdx.x & 31) == 0) {
-        if (rz != 0.0) atomicAdd(scal + 2, rz);
-        if (rr != 0.0) atomicAdd(scal + 3, rr);
+        sm[0][threadIdx.x >> 5] = s0;
+        sm[1][threadIdx.x >> 5] = s1;
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        s0 = warp_sum(sm[0][threadIdx.x]);
+        s1 = warp_sum(sm[1][threadIdx.x]);
+        if (threadIdx.x == 0) {
+            const double rz_old = scal[0];
+            scal[5] = rz_old != 0.0 ? s0 / rz_old : 0.0;
+            scal[0] = s0;
+            scal[3] = s1;
+            if (start) scal[4] = s1; // r = b
+            else {
+                st->sv_rr = s1;
+                ++st->sv_iters;
+            }
+        }
     }
 }
-// p = z + beta p with beta = rz_new / rz ; then roll the scalars for the next iteration (one thread)
+
+// p = z + beta p
 __global__ void __launch_bounds__(256) k_pcg_direction(int n, const double* __restrict__ z, double* __restrict__ p, const double* __restrict__ scal)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const double rz = scal[0];
-    const double beta = rz != 0.0 ? scal[2] / rz : 0.0;
+    const double beta = scal[5];
     if (i < n) p[i] = z[i] + beta * p[i];
 }
-__global__ void k_pcg_roll(double* scal, IterState* st)
-{
-    if (threadIdx.x == 0) {
-        st->sv_rr = scal[3]; // |r|^2 after this iteration
-        ++st->sv_iters;
-        scal[0] = scal[2];
-        scal[1] = scal[2] = scal[3] = 0.0;
-    }
-}
+
 // max |x_i| (exact, so the order does not matter; NaN entries are skipped)
 __global__ void __launch_bounds__(256) k_abs_max(int n, const double* __restrict__ x, unsigned long long* __restrict__ out)
 {
@@ -231,15 +256,7 @@ __global__ void __launch_bounds__(256) k_psize(int nSV, const int* __restrict__ 
         if (v >= nVdof) continue; // the obstacle's surface vertices do not count (SpatialHash::build sees the mesh alone)
         s += fabs(p[3 * (size_t)v]) + fabs(p[3 * (size_t)v + 1]) + fabs(p[3 * (size_t)v + 2]);
     }
-    s = warp_sum(s);
-    __shared__ double sm[8];
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0.0;
-        for (int w = 0; w < 8; ++w) t += sm[w];
-        partials[blockIdx.x] = t;
-    }
+    cta_sum(&s, partials + blockIdx.x);
 }
 // ... then the partials in block order, over the 3 nMeshSV components (0 without mesh surface vertices)
 __global__ void k_psize_mean(const double* __restrict__ partials, int n, long long n3, double* __restrict__ out)
@@ -300,25 +317,47 @@ int solver_finish(ipcgpu_ctx* ctx)
     return IPCGPU_OK;
 }
 
-// PCG on the device-resident matrix.  rhs_dev: device vector (3 nV) scaled by `sign`.  The solution is left in ctx->sol, the result in
-// IterState (sv_*).  The workspace is reserved by the caller (solve_pcg in api_mesh.cu).
-int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter)
+// block-Jacobi step (start: z = Minv r alone)
+static void block_jacobi_step(ipcgpu_ctx* ctx, bool start)
+{
+    double* part = ctx->pcg_part.p;
+    k_block_jacobi_step<<<nblk(ctx->nV, 256), 256, 0, ctx->stream>>>(ctx->nV, ctx->pcg_minv.p, ctx->pcg_p.p, ctx->pcg_q.p, ctx->sol.p, ctx->pcg_r.p,
+        ctx->pcg_scal.p, start ? nullptr : part, kPcgSpmvBlocks, part + kPcgSpmvBlocks);
+    ++ctx->launches;
+}
+
+// PCG on the device-resident matrix, preconditioned by block-Jacobi or by the multilevel hierarchy (multilevel.cu).  rhs_dev: device vector
+// (3 nV) scaled by `sign`.  The solution is left in ctx->sol, the result in IterState (sv_*); a pivot <= 0 of the multilevel set-up is the
+// solve's failure (kSolveStart).  The workspace is reserved by the caller (solve_pcg in api_mesh.cu).  pcg_part holds the SpMV's partials
+// of p.Ap, then the preconditioner step's partials of r.z and r.r (2 per CTA of one thread per vertex).  The step is all the two solvers
+// differ in: in an iteration it finishes the CG update from the SpMV's partials, then it leaves z = M^-1 r in pcg_q.
+int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, bool multilevel)
 {
     cudaStream_t st = ctx->stream;
-    const int n = ctx->n_rows, nV = ctx->nV;
-    CK(cudaMemsetAsync(ctx->pcg_scal.p, 0, 8 * sizeof(double), st));
-    k_block_jacobi<<<nblk(nV, 256), 256, 0, st>>>(nV, ctx->ia.p, ctx->index_base, ctx->a.p, ctx->pcg_minv.p);
-    k_pcg_init<<<nblk(nV, 256), 256, 0, st>>>(nV, rhs_dev, sign, ctx->pcg_minv.p, ctx->sol.p, ctx->pcg_r.p, ctx->pcg_p.p, ctx->pcg_scal.p);
-    ctx->launches += 2;
-    int rc = decide(ctx, kSolveStart, rel_tol, max_iter, 0, nullptr, ctx->pcg_scal.p);
+    const int n = ctx->n_rows, n_pre = nblk(ctx->nV, 256);
+    double *x = ctx->sol.p, *r = ctx->pcg_r.p, *p = ctx->pcg_p.p, *q = ctx->pcg_q.p, *scal = ctx->pcg_scal.p, *pre = ctx->pcg_part.p + kPcgSpmvBlocks;
+    CK(cudaMemsetAsync(scal, 0, 8 * sizeof(double), st));
+    if (multilevel) {
+        int rc = solver_multilevel_build(ctx, scal + 6);
+        if (rc) return rc;
+    } else {
+        k_block_jacobi<<<n_pre, 256, 0, st>>>(ctx->nV, ctx->ia.p, ctx->index_base, ctx->a.p, ctx->pcg_minv.p);
+        ++ctx->launches;
+    }
+    k_pcg_init<<<nblk(n, 256), 256, 0, st>>>(n, rhs_dev, sign, x, r, p);
+    multilevel ? solver_multilevel_step(ctx, true) : block_jacobi_step(ctx, true);
+    k_pcg_roll<<<1, 1024, 0, st>>>(pre, n_pre, scal, ctx->iter.p, 1);
+    k_pcg_direction<<<nblk(n, 256), 256, 0, st>>>(n, q, p, scal);
+    ctx->launches += 3;
+    int rc = decide(ctx, kSolveStart, rel_tol, max_iter, 0, nullptr, scal);
     if (rc) return rc;
     return krylov_loops(ctx, max_iter, [&]() {
         cudaStream_t s = ctx->stream; // (the body's stream inside a capture)
-        k_spmv_dot<<<kSMs * 8, 256, 0, s>>>(n, ctx->fia.p, ctx->fja.p, ctx->fpos.p, ctx->a.p, ctx->pcg_p.p, ctx->pcg_q.p, ctx->pcg_scal.p, 1);
-        k_pcg_update<<<nblk(nV, 256), 256, 0, s>>>(nV, ctx->pcg_minv.p, ctx->pcg_p.p, ctx->pcg_q.p, ctx->sol.p, ctx->pcg_r.p, ctx->pcg_scal.p);
-        k_pcg_direction<<<nblk(n, 256), 256, 0, s>>>(n, ctx->pcg_q.p, ctx->pcg_p.p, ctx->pcg_scal.p);
-        k_pcg_roll<<<1, 32, 0, s>>>(ctx->pcg_scal.p, ctx->iter.p);
-        ctx->launches += 4;
+        k_pcg_spmv<<<kPcgSpmvBlocks, 256, 0, s>>>(n, ctx->fia.p, ctx->fja.p, ctx->fpos.p, ctx->a.p, p, q, ctx->pcg_part.p);
+        multilevel ? solver_multilevel_step(ctx, false) : block_jacobi_step(ctx, false);
+        k_pcg_roll<<<1, 1024, 0, s>>>(pre, n_pre, scal, ctx->iter.p, 0);
+        k_pcg_direction<<<nblk(n, 256), 256, 0, s>>>(n, q, p, scal);
+        ctx->launches += 3;
     });
 }
 

@@ -1,7 +1,8 @@
 """ipcgpu_solve_pcg_multilevel: PCG on the device-resident Hessian with the multilevel additive Schwarz preconditioner.  The solution equals
 a host direct solve, the stored inverses, the application and the iteration count equal the host mirror's (tests/multilevel_mirror.py),
-two calls give identical bits, the device-built pattern, an obstacle tail and Dirichlet vertices are covered, a non-positive pivot is an
-error and not a hang, and the iterations are at most half of block-Jacobi's on ball_on_mat."""
+two calls of either solver give identical bits and make 6 + L (multilevel) or 4 (block-Jacobi) launches per iteration, the device-built
+pattern, an obstacle tail and Dirichlet vertices are covered, a non-positive pivot is an error and not a hang, and the iterations are at most
+half of block-Jacobi's on ball_on_mat."""
 import numpy as np
 import pytest
 import scipy.sparse.linalg as spla
@@ -131,6 +132,16 @@ def test_hierarchy_application_and_iterations_equal_the_mirror(gpu_ctx):
         ctx.multilevel_info()
 
 
+def launches_of_25_more_iterations(ctx, solve):
+    """launches of a solve to max_iter 50 minus those of one to 25, at an unreachable tolerance: 25 iterations and one burst decision"""
+    counts = []
+    for max_iter in (25, 50):
+        n0 = ctx.launch_count()
+        assert solve(None, rel_tol=1e-30, max_iter=max_iter, want_x=False)[1] == max_iter
+        counts.append(ctx.launch_count() - n0)
+    return counts[1] - counts[0]
+
+
 def test_two_solves_give_identical_bits(gpu_ctx):
     ctx = gpu_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
@@ -141,6 +152,20 @@ def test_two_solves_give_identical_bits(gpu_ctx):
     x2, it2, res2 = ctx.solve_pcg_multilevel(None, rel_tol=1e-8, max_iter=5000)
     inv2 = ctx.download(L.BUF_MULTILEVEL_INVERSES, 9216 * sum(ctx.multilevel_info()[0]))
     assert res1 <= 1e-8 and it1 == it2 and same_bits(res1, res2) and same_bits(x1, x2) and same_bits(inv1, inv2)
+    # 6 + L launches per iteration: SpMV, reduce, update, L levels, prolongation, roll, direction
+    assert launches_of_25_more_iterations(ctx, ctx.solve_pcg_multilevel) == 25 * (6 + len(ctx.multilevel_info()[0])) + 1
+
+
+def test_two_block_jacobi_solves_give_identical_bits(gpu_ctx):
+    ctx = gpu_ctx
+    m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
+    assemble(ctx, m, info["dHat"], 1e8)
+    x1, it1, res1 = ctx.solve_pcg(None, rel_tol=1e-8, max_iter=5000)
+    ctx.solve_pcg_multilevel(None, rel_tol=1e-3, max_iter=50)  # (another solver in between shares the workspace)
+    x2, it2, res2 = ctx.solve_pcg(None, rel_tol=1e-8, max_iter=5000)
+    assert res1 <= 1e-8 and it1 == it2 and same_bits(res1, res2) and same_bits(x1, x2)
+    # 4 launches per iteration: SpMV, block-Jacobi step (alpha summed inside), roll, direction
+    assert launches_of_25_more_iterations(ctx, ctx.solve_pcg) == 25 * 4 + 1
 
 
 def test_device_built_pattern_after_a_pattern_change(gpu_ctx):
