@@ -781,7 +781,7 @@ DEV bool library_leaves_at_max_itr(const DBox* cur, int n, int lane, bool has_k2
 // box-parallel root finder of the warp-level pass, one box per lane, level buffers in global memory: 0 no collision, 1 collision (toi set),
 // -1 a level outgrew the buffers (toi / out_tol hold the conservative estimate of the level before)
 __device__ int ti_root_finder(bool VF, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err, double ms, int max_itr, DBox* bufA,
-    DBox* bufB, int cap, int lane, double& toi, double& out_tol, int* __restrict__ warn, const unsigned long long* best)
+    DBox* bufB, int cap, int lane, double& toi, double& out_tol, int* __restrict__ warn, unsigned long long& boxes, const unsigned long long* best)
 {
     const bool check_t = (max_t != 1.0);
     const double INF = __longlong_as_double(0x7ff0000000000000ll);
@@ -860,7 +860,7 @@ __device__ int ti_root_finder(bool VF, const TiPair& P, const double* tol, const
             return 1;
         }
         const bool has_k2 = k2.t != INF;
-        if (lane == 0) atomicAdd(reinterpret_cast<unsigned long long*>(warn + 7), (unsigned long long)visited); // diagnostics: boxes evaluated
+        boxes += (unsigned)visited; // diagnostics: boxes evaluated (the same on every lane)
         if (max_itr > 0) {
             temp_toi = k1.t;
             temp_out_tol = fmax(a1, co_tol);
@@ -977,7 +977,7 @@ __device__ int ti_root_finder(bool VF, const TiPair& P, const double* tol, const
 // lane with a warp scan.  Level buffers live in shared memory.  Same arithmetic per corner, same decisions => same result as the
 // box-parallel variant.  Returns -1 when a level outgrows the shared-memory buffer (the caller restarts with the box-parallel variant).
 __device__ int ti_root_finder_cp(bool VF, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err, double ms, int max_itr, DBox* sA, DBox* sB,
-    int lane, double& toi, double& out_tol, int* __restrict__ warn, const unsigned long long* best)
+    int lane, double& toi, double& out_tol, int* __restrict__ warn, unsigned long long& boxes, const unsigned long long* best)
 {
     const bool check_t = (max_t != 1.0);
     const double INF = __longlong_as_double(0x7ff0000000000000ll);
@@ -1123,7 +1123,7 @@ __device__ int ti_root_finder_cp(bool VF, const TiPair& P, const double* tol, co
         if (p1 & 1u) { toi = k1.t; return 1; }
         const bool has_k2 = k2.t != INF;
         if (has_k2 && (p2 & 1u)) { toi = k2.t; return 1; }
-        if (lane == 0) atomicAdd(reinterpret_cast<unsigned long long*>(warn + 7), (unsigned long long)visited);
+        boxes += (unsigned)visited;
         if (max_itr > 0) {
             temp_toi = k1.t;
             temp_out_tol = fmax(a1max, co_tol);
@@ -1219,28 +1219,29 @@ __device__ int ti_root_finder_cp(bool VF, const TiPair& P, const double* tol, co
 // corner evaluation (a few instructions differ), the retry is a second trip through ONE call site, and the split rule multiplies by exact
 // reciprocals instead of dividing (below): one copy of each root finder.
 __device__ __noinline__ int ti_root_finder_cp_call(bool vf, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err, double ms,
-    int max_itr, DBox* sA, DBox* sB, int lane, double& toi, double& out_tol, int* __restrict__ warn, const unsigned long long* best)
+    int max_itr, DBox* sA, DBox* sB, int lane, double& toi, double& out_tol, int* __restrict__ warn, unsigned long long& boxes, const unsigned long long* best)
 {
-    return ti_root_finder_cp(vf, P, tol, inv_tol, co_tol, max_t, err, ms, max_itr, sA, sB, lane, toi, out_tol, warn, best);
+    return ti_root_finder_cp(vf, P, tol, inv_tol, co_tol, max_t, err, ms, max_itr, sA, sB, lane, toi, out_tol, warn, boxes, best);
 }
 __device__ __noinline__ int ti_root_finder_warp_call(bool vf, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err, double ms,
-    int max_itr, DBox* bufA, DBox* bufB, int cap, int lane, double& toi, double& out_tol, int* __restrict__ warn, const unsigned long long* best)
+    int max_itr, DBox* bufA, DBox* bufB, int cap, int lane, double& toi, double& out_tol, int* __restrict__ warn, unsigned long long& boxes,
+    const unsigned long long* best)
 {
-    return ti_root_finder(vf, P, tol, inv_tol, co_tol, max_t, err, ms, max_itr, bufA, bufB, cap, lane, toi, out_tol, warn, best);
+    return ti_root_finder(vf, P, tol, inv_tol, co_tol, max_t, err, ms, max_itr, bufA, bufB, cap, lane, toi, out_tol, warn, boxes, best);
 }
 
 // A search that outgrows the per-warp level buffers runs again in the context's overflow arena (two levels of kArenaLevel boxes), which one
 // warp holds at a time: such searches are rare, and the library itself runs them to max_itr.  The arena run does not prune against the
 // running minimum, so its count of evaluated boxes -- and with it the max_itr exit -- is the library's own.
 __device__ __noinline__ int ti_root_finder_arena(bool vf, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err,
-    double ms, int max_itr, DBox* arena, int* arena_lock, int lane, double& toi, double& out_tol, int* __restrict__ warn)
+    double ms, int max_itr, DBox* arena, int* arena_lock, int lane, double& toi, double& out_tol, int* __restrict__ warn, unsigned long long& boxes)
 {
     if (lane == 0) {
         while (atomicCAS(arena_lock, 0, 1) != 0) __nanosleep(1000);
         __threadfence();
     }
     __syncwarp();
-    int rc = ti_root_finder_warp_call(vf, P, tol, inv_tol, co_tol, max_t, err, ms, max_itr, arena, arena + kArenaLevel, kArenaLevel, lane, toi, out_tol, warn, nullptr);
+    int rc = ti_root_finder_warp_call(vf, P, tol, inv_tol, co_tol, max_t, err, ms, max_itr, arena, arena + kArenaLevel, kArenaLevel, lane, toi, out_tol, warn, boxes, nullptr);
     __syncwarp();
     if (lane == 0) {
         __threadfence();
@@ -1257,7 +1258,7 @@ __device__ __noinline__ int ti_root_finder_arena(bool vf, const TiPair& P, const
 // in the shared-memory level buffers sA / sB; a search that outgrows them restarts box-parallel in the global buffers bufA / bufB, and one
 // that outgrows those in the overflow arena.
 __device__ int ti_ccd(bool vf, const TiPair& P, const double* err, double ms, double tolerance, double t_max, int max_itr, DBox* bufA, DBox* bufB, int cap, int lane,
-    double& toi, int* __restrict__ warn, DBox* sA, DBox* sB, const unsigned long long* best, DBox* arena, int* arena_lock)
+    double& toi, int* __restrict__ warn, unsigned long long& boxes, DBox* sA, DBox* sB, const unsigned long long* best, DBox* arena, int* arena_lock)
 {
     double tolerance_in = tolerance, ms_in = ms, out_tol = tolerance;
     bool is_impacting = false, tmp = false;
@@ -1270,9 +1271,9 @@ __device__ int ti_ccd(bool vf, const TiPair& P, const double* err, double ms, do
         // for bit: one division per axis and search instead of three per box.
 #pragma unroll
         for (int d = 0; d < 3; ++d) inv_tol[d] = 1.0 / tol[d];
-        int rc = ti_root_finder_cp_call(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, sA, sB, lane, toi, out_tol, warn, best);
-        if (rc == -1) rc = ti_root_finder_warp_call(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, bufA, bufB, cap, lane, toi, out_tol, warn, best);
-        if (rc == -1) rc = ti_root_finder_arena(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, arena, arena_lock, lane, toi, out_tol, warn);
+        int rc = ti_root_finder_cp_call(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, sA, sB, lane, toi, out_tol, warn, boxes, best);
+        if (rc == -1) rc = ti_root_finder_warp_call(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, bufA, bufB, cap, lane, toi, out_tol, warn, boxes, best);
+        if (rc == -1) rc = ti_root_finder_arena(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, max_itr, arena, arena_lock, lane, toi, out_tol, warn, boxes);
         tmp = rc == 1;
         if (iter == 0) is_impacting = tmp;
         else toi = tmp ? toi : t_max;
@@ -1287,7 +1288,8 @@ __device__ int ti_ccd(bool vf, const TiPair& P, const double* err, double ms, do
 }
 
 // one candidate end to end (SelfCollisionHandler.cpp:740-790): 0 / 1 (toi set)
-__device__ int pair_ccd(bool vf, const TiPair& P, const NarrowArgs& a, DBox* bufA, DBox* bufB, int cap, int lane, double& toi, int* __restrict__ warn, DBox* sA, DBox* sB)
+__device__ int pair_ccd(bool vf, const TiPair& P, const NarrowArgs& a, DBox* bufA, DBox* bufB, int cap, int lane, double& toi, int* __restrict__ warn, unsigned long long& boxes,
+    DBox* sA, DBox* sB)
 {
     const double d = pair_distance_sqrt(vf, P);
     const double max_t = a.st->max_t;                 // canonical semantics: every pair sees the step on entry (SURVEY 8a row 10)
@@ -1300,7 +1302,7 @@ __device__ int pair_ccd(bool vf, const TiPair& P, const NarrowArgs& a, DBox* buf
     for (int attempt = 0; attempt < 2; ++attempt) {
         const double ms = attempt ? 0.0 : fmin(0.2 * d, 1e-6);
         const unsigned long long* best = attempt ? nullptr : &a.st->ccd_ord;
-        hit = ti_ccd(vf, P, err, ms, a.tol, max_t, a.max_itr, bufA, bufB, cap, lane, toi, warn, sA, sB, best, a.arena, a.arena_lock);
+        hit = ti_ccd(vf, P, err, ms, a.tol, max_t, a.max_itr, bufA, bufB, cap, lane, toi, warn, boxes, sA, sB, best, a.arena, a.arena_lock);
         if (attempt == 1) {
             if (hit) toi *= 0.8;
             break;
@@ -1340,7 +1342,7 @@ DEV void bfs1_init(Bfs1& b, DBox* bufA, DBox* bufB, double co_tol, const unsigne
 // one level of the thread pass (ti_root_finder's level loop run by one lane): 0 no collision, 1 collision (toi set), 2 deferred, 3 go on
 // with the next level
 DEV int bfs1_level(bool VF, const TiPair& P, const double* tol, const double* inv_tol, double co_tol, double max_t, const double* err, double ms, int max_itr,
-    int cap, long long thread_budget, const unsigned long long* best, Bfs1& b, double& toi, double& out_tol, int* __restrict__ warn)
+    int cap, long long thread_budget, const unsigned long long* best, Bfs1& b, double& toi, double& out_tol, int* __restrict__ warn, unsigned long long& boxes)
 {
     const bool check_t = (max_t != 1.0);
     const double INF = __longlong_as_double(0x7ff0000000000000ll);
@@ -1381,7 +1383,7 @@ DEV int bfs1_level(bool VF, const TiPair& P, const double* tol, const double* in
     if (p1 & 1u) { toi = k1.t; return 1; }
     const bool has_k2 = k2.t != INF;
     if (has_k2 && (p2 & 1u)) { toi = k2.t; return 1; }
-    atomicAdd(reinterpret_cast<unsigned long long*>(warn + 5), (unsigned long long)visited); // diagnostics: boxes evaluated by the thread pass
+    boxes += (unsigned)visited; // diagnostics: boxes evaluated by the thread pass
     if (b.refine + visited > thread_budget) return 2; // over budget: handed to the warp pass
     if (max_itr > 0) {
         b.temp_toi = k1.t;
@@ -1445,7 +1447,9 @@ DEV int bfs1_level(bool VF, const TiPair& P, const double* tol, const double* in
 }
 
 constexpr int kThreadLevel = 8;  // boxes per level buffer of a lane of the thread pass (2 buffers per lane, in shared memory)
-constexpr int kRefillBatch = 16; // idle lanes of a warp refill together once this many are idle (H100 SXM, 400 W, C5: batch 1 / 8 / 16 / 32 -> 1.06 / 1.05 / 1.03 / 1.03 ms)
+// idle lanes of a warp refill together once this many are idle (H100 SXM, 400 W, C5: batch 1 / 8 / 16 / 32 -> 1.06 / 1.05 / 1.03 / 1.03 ms;
+// again with the box counter in registers, 700 W, budget 64, iteration ms: 8 / 16 / 32 -> 2.54 / 2.52 / 2.53)
+constexpr int kRefillBatch = 16;
 __global__ void __launch_bounds__(128, 2) k_ti_stage15_refill(NarrowArgs a, const unsigned* __restrict__ survivors, const unsigned* __restrict__ nSurvPtr, unsigned* __restrict__ work,
     unsigned* __restrict__ deferred, unsigned* __restrict__ nDeferred, long long budget, unsigned long long* __restrict__ min_ord, int* __restrict__ warn)
 {
@@ -1470,6 +1474,9 @@ __global__ void __launch_bounds__(128, 2) k_ti_stage15_refill(NarrowArgs a, cons
     const double* err = a.err_vf;
     const unsigned long long* best = nullptr;
     bool drained = false;
+    // diagnostics: the boxes this lane evaluated over all its searches.  A count per lane and one atomic per warp when it leaves: an add to
+    // the pass's single counter at every level of every search was a serial chain of same-address reductions on one L2 slice.
+    unsigned long long boxes = 0;
     for (;;) {
         // Refill in batches: fetching a pair is two dependent rounds of global loads (candidate -> vertex ids -> positions, directions), and the
         // whole warp waits for them -- refilling whenever any lane is idle made every iteration pay that latency (ncu: long scoreboard 3.0 per
@@ -1503,9 +1510,14 @@ __global__ void __launch_bounds__(128, 2) k_ti_stage15_refill(NarrowArgs a, cons
             else drained = true;
         }
         __syncwarp();
-        if (__all_sync(0xffffffffu, !busy)) break; // the lanes of a warp leave together: all idle and the list exhausted
+        if (__all_sync(0xffffffffu, !busy)) { // the lanes of a warp leave together: all idle and the list exhausted
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) boxes += __shfl_xor_sync(0xffffffffu, boxes, o);
+            if (lane == 0 && boxes) atomicAdd(reinterpret_cast<unsigned long long*>(warn + 5), boxes);
+            break;
+        }
         if (busy) {
-            const int rc = bfs1_level(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, a.max_itr, kThreadLevel, budget, best, bf, toi, out_tol, warn);
+            const int rc = bfs1_level(vf, P, tol, inv_tol, tolerance_in, t_max, err, ms_in, a.max_itr, kThreadLevel, budget, best, bf, toi, out_tol, warn, boxes);
             if (rc != 3) {
                 bool restart = false, finished = false;
                 int hit = 0;
@@ -1563,11 +1575,16 @@ __global__ void __launch_bounds__(128, 2) k_ti_stage2(NarrowArgs a, const unsign
     DBox* bufA = scratch + (size_t)warp_global * 2 * cap;
     DBox* bufB = bufA + cap;
     const unsigned nSurv = *nSurvPtr;
+    // diagnostics: the boxes this warp's searches evaluated (the same count on every lane), added to the pass's total once, when the warp leaves
+    unsigned long long boxes = 0;
     for (;;) {
         unsigned w = 0;
         if (lane == 0) w = atomicAdd(work, 1u);
         w = __shfl_sync(0xffffffffu, w, 0);
-        if (w >= nSurv) break;
+        if (w >= nSurv) {
+            if (lane == 0 && boxes) atomicAdd(reinterpret_cast<unsigned long long*>(warn + 7), boxes);
+            break;
+        }
         bool vf;
         {
             // the pair's 24 coordinates live in shared memory: the warp-level search only needs them 8 at a time per lane
@@ -1580,7 +1597,7 @@ __global__ void __launch_bounds__(128, 2) k_ti_stage2(NarrowArgs a, const unsign
         const TiPair& P = sPair[threadIdx.x >> 5];
         double toi;
         const long long t0 = clock64();
-        const int hit = pair_ccd(vf, P, a, bufA, bufB, cap, lane, toi, warn, sA, sB);
+        const int hit = pair_ccd(vf, P, a, bufA, bufB, cap, lane, toi, warn, boxes, sA, sB);
         if (hit && lane == 0) atomicMin(min_ord, dbl_to_ord(toi));
         if (lane == 0) { // diagnostics: the longest pair bounds this pass from below
             const unsigned dt = (unsigned)((clock64() - t0) >> 6);
@@ -1711,10 +1728,11 @@ int ccd_narrow(ipcgpu_ctx* ctx, const int2* cand, const int* n32, const unsigned
         unsigned* nDefA = reinterpret_cast<unsigned*>(flags + 2);
         unsigned* refill_work = reinterpret_cast<unsigned*>(flags + 3);
         // pass A (thread per survivor): the shallow majority (2-3 boxes) at 32 pairs per warp; pass B (warp per pair): the searches pass A hands on.
-        // boxes a thread may evaluate before it hands its pair on (H100 SXM, 700 W, C5, iteration ms with the warp pass above: 24 -> 3.26 (2,871 pairs
-        // handed on in the full CCD), 32 -> 3.15 (950), 40 -> 3.14, 64 -> 3.16; the narrow phase alone barely moves, the iteration gains because
-        // the shorter warp pass leaves the SMs to the derivative chain sooner).  The test hook ipcgpu_ccd_debug_thread_budget overrides it.
-        constexpr long long kThreadBudget = 32;
+        // boxes a thread may evaluate before it hands its pair on (H100 SXM, 700 W, C5, iteration ms with the box counters in registers: 24 -> 2.64
+        // (2,871 pairs handed on in the full CCD), 32 -> 2.58 (950), 48 -> 2.55, 64 -> 2.52 (444), 96 -> 2.49 (440), 128 -> 2.50; the eager narrow
+        // phase grows from 0.79 to 0.90 ms between 32 and 96, the iteration gains because the shorter warp pass leaves the SMs to the derivative
+        // chain sooner).  The test hook ipcgpu_ccd_debug_thread_budget overrides it.
+        constexpr long long kThreadBudget = 96;
         const long long budget = ctx->debug_ti_budget >= 0 ? ctx->debug_ti_budget : kThreadBudget;
         constexpr int bytes = 2 * 128 * (kThreadLevel * (int)sizeof(DBox) + 8);
         static bool attr = false;
