@@ -56,6 +56,12 @@ enum {
 
 enum { IPCGPU_NEOHOOKEAN = 0, IPCGPU_FIXED_COROT = 1 };
 
+/* A kappa argument exactly equal to this value means "the barrier stiffness held in device memory, read at run time" (ipcgpu_set_kappa and
+ * the calls after it).  Accepted by ipcgpu_barrier_energy / _gradient / _hessian, ipcgpu_para_ee_gradient, ipcgpu_friction_lag, the
+ * half-space barrier calls and ipcgpu_line_search (ipcgpu_line_search_terms.kappa).  A graph captured with it reads the current value at every
+ * replay, so a new kappa needs no new capture.  Single rank: IPCGPU_ERR_STATE with several.  Every other value is a host kappa as before. */
+#define IPCGPU_KAPPA_DEVICE (-1.0)
+
 /* device-resident result buffers that ipcgpu_download() can fetch */
 enum {
     IPCGPU_BUF_GRADIENT = 0,      /* 3*nV doubles, interleaved */
@@ -137,7 +143,7 @@ int ipcgpu_step_bound_set(ipcgpu_ctx* ctx, double alpha);
  * What it does not: positions (ipcgpu_set_state), search direction (ipcgpu_set_search_dir), previous state / xTilta, the contact sets,
  * list sizes and step bounds -- they live in device memory and are read at replay time.  So one capture serves every Newton iteration
  * of a solve; capture again after ipcgpu_set_mesh / _set_surface / _set_csr / _set_*_capacity / _comm_init / _set_canonical_order /
- * _set_contact_partition (older graphs are refused with IPCGPU_ERR_STATE) or when dHat / kappa change.  Run the sequence once eagerly
+ * _set_contact_partition (older graphs are refused with IPCGPU_ERR_STATE) or when dHat / a host kappa change (IPCGPU_KAPPA_DEVICE is read at replay).  Run the sequence once eagerly
  * before capturing it (lazy allocations), with ipcgpu_set_canonical_order(ctx, 0): the canonical sort of the contact lists needs their sizes
  * on the host.  Collective: with several ranks every rank captures and launches the same sequence.
  * ipcgpu_fetch_iteration stays outside the graph. */
@@ -442,6 +448,41 @@ typedef struct ipcgpu_step_control {
 } ipcgpu_step_control;
 /* synchronises only when a CFL branch or a line search was enqueued since the last read; returns out->status */
 int ipcgpu_step_control_info(ipcgpu_ctx* ctx, ipcgpu_step_control* out);
+
+/* ---- adaptive barrier stiffness (ADAPTIVE_KAPPA, src/Utils/Types.hpp:41; DESIGN.md section 3.18) -------------------------------------------
+ * kappa held in device memory and adapted there, read by the calls given IPCGPU_KAPPA_DEVICE.  A time step: ipcgpu_set_kappa (the start rule of
+ * Optimizer.cpp:1540-1547 applied by the caller), ipcgpu_kappa_init, ipcgpu_kappa_clear_close_set, then Newton iterations that each end with
+ * ipcgpu_kappa_post_line_search.  Every call but ipcgpu_kappa_bounds and ipcgpu_kappa_info enqueues in stream order without synchronising and
+ * can be captured.  Single rank: IPCGPU_ERR_STATE with several. */
+/* suggestKappa and upperBoundKappa (Optimizer.cpp:2216-2233) with H_b = b''(1e-16 bbox_diag2) at dHat (BarrierFunctions.hpp:73-83):
+ * suggest = kappa_min_multiplier * avg_node_mass / (4e-16 * bbox_diag2 * H_b), max = 100 * the same.  avg_node_mass is Mesh::avgNodeMass(3),
+ * bbox_diag2 the squared diagonal of the rest bounding box (bboxDiagSize2).  Host-only. */
+int ipcgpu_kappa_bounds(double dHat, double kappa_min_multiplier, double avg_node_mass, double bbox_diag2, double* suggest, double* max);
+/* the device kappa and its two bounds; resets the doubling count */
+int ipcgpu_set_kappa(ipcgpu_ctx* ctx, double kappa, double suggest, double max);
+/* initKappa (Optimizer.cpp:2236-2313).  g_E is the device gradient as the caller left it (the NULL-output elastic, inertia, Neumann, damping and
+ * Dirichlet-penalty gradients: computeGradient with solveIP off); g_c = J^T g_b(d) over the self / obstacle active set and the planes' active
+ * set, without the mollified pairs and friction, with the rows of every Dirichlet vertex (dbc != 0) zeroed.  With no active entry nothing
+ * changes; otherwise minKappa = -g_c.g_E / |g_c|^2, kappa = minKappa if minKappa > 0, then kappa = max(kappa, suggest), min(kappa, max)
+ * (|g_c| = 0 gives a NaN minKappa: kappa stays, then the floor applies).  Clears needs_init.  The gradient is left as it was. */
+int ipcgpu_kappa_init(ipcgpu_ctx* ctx, double dHat);
+/* initSubProb_IP (Optimizer.cpp:2316-2322): empties the close set */
+int ipcgpu_kappa_clear_close_set(ipcgpu_ctx* ctx);
+/* postLineSearch (Optimizer.cpp:2357-2445).  kappa == 0: needs_init is set and nothing else changes (the caller runs ipcgpu_kappa_init).
+ * Otherwise every saved close entry is evaluated at the current positions; if any has d <= its saved d, kappa doubles and is capped at max.
+ * Then the close set becomes the active entries (self / obstacle, planes; no mollified pairs) of the sets held with d < dTol. */
+int ipcgpu_kappa_post_line_search(ipcgpu_ctx* ctx, double dTol);
+typedef struct ipcgpu_kappa {
+    double kappa;
+    double min_kappa;             /* minKappa of the last ipcgpu_kappa_init with active entries (NaN for g_c = 0) */
+    double suggest, max;          /* as set by ipcgpu_set_kappa */
+    double close_min_dist2;       /* min d^2 over the active entries at the last snapshot (the reference logs it); inf without entries */
+    int doublings;                /* since the last ipcgpu_set_kappa */
+    int n_close;                  /* entries of the close set */
+    int needs_init;               /* ipcgpu_kappa_post_line_search met kappa == 0 */
+} ipcgpu_kappa;
+/* synchronises only when a kappa call was enqueued since the last read */
+int ipcgpu_kappa_info(ipcgpu_ctx* ctx, ipcgpu_kappa* out);
 
 /* ---- kinematic mesh obstacle: MeshCO<3> (src/CollisionObject/MeshCO.hpp:39-233; SURVEY 8 row f3, barrier / Tight-Inclusion path) --------------------
  * An obstacle is a triangle mesh without degrees of freedom (MeshCO's Base::V, edges, Base::F).  It rides at the TAIL of the mesh's arrays: the

@@ -69,6 +69,11 @@ static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
 //   - time integration (timestep.cu): ipcgpu_compute_xtilde, ipcgpu_end_time_step and ipcgpu_warm_start write xtilde, Vprev, V, dir and the
 //     dynamic state (vel, acc, dxe), which the derivative chain reads (inertia, damping, friction) or the step-bound chain does (dir): all
 //     three are kSerial.
+//   - the device-resident kappa (kappa.cu): the barrier / plane derivative calls given IPCGPU_KAPPA_DEVICE read IterState::kappa; every call
+//     that writes it or the other kappa words -- ipcgpu_set_kappa, _kappa_init (which also reads g and V), _kappa_clear_close_set and
+//     _kappa_post_line_search (which reads V and the contact sets) -- is kSerial, which orders it before the derivative chain.  The pair-Hessian
+//     build of ipcgpu_barrier_hessian runs on the side stream, which waits on ev_inputs only: the three calls that write kappa mark the
+//     inputs (mark_inputs) as a position or set change does.  The step-bound chain touches none of them.
 //   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, e_partials2, bHraw, brows, bpsd:
 //     derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };
@@ -108,8 +113,15 @@ int sync_pattern_mirror(ipcgpu_ctx* ctx);
 int flag_status(ipcgpu_ctx* ctx, unsigned mask);
 void set_local(ipcgpu_ctx* ctx, unsigned bits, bool local);
 int energy_result(ipcgpu_ctx* ctx, int slot, double* E, bool fetch = false, unsigned check = 0);
+// scale_dev != nullptr: the scale is read on the device from there (the device-resident kappa)
 int energy_tail(ipcgpu_ctx* ctx, int slot, const double* partials, int n_partials, double scale, cudaEvent_t pe, double* E, bool fetch = false,
-    unsigned check = 0);
+    unsigned check = 0, const double* scale_dev = nullptr);
+
+// ---- the barrier stiffness: a kappa argument equal to IPCGPU_KAPPA_DEVICE stands for IterState::kappa, read at run time (one rank only) ----
+inline bool kappa_on_device(double kappa) { return kappa == IPCGPU_KAPPA_DEVICE; }
+inline const double* kappa_ptr(ipcgpu_ctx* ctx, double kappa) { return kappa_on_device(kappa) ? &ctx->iter.p->kappa : nullptr; }
+#define REQUIRE_KAPPA(kappa)                                                                                                        \
+    REQUIRE(!kappa_on_device(kappa) || ctx->nranks == 1, IPCGPU_ERR_STATE, "the device-resident kappa (IPCGPU_KAPPA_DEVICE) runs on one rank")
 int gradient_roundtrip_begin(ipcgpu_ctx* ctx, const double* g_in);
 int gradient_roundtrip_end(ipcgpu_ctx* ctx, double* g_out);
 int hessian_begin(ipcgpu_ctx* ctx, Chain chain, const double* a_inout);
@@ -141,6 +153,8 @@ int contact_sync_counts(ipcgpu_ctx* ctx);
 void contact_pack_lists(ipcgpu_ctx* ctx);
 void contact_unpack_lists(ipcgpu_ctx* ctx);
 ipcgpu::SurfArgs surf_args(const ipcgpu_ctx* ctx);
+ipcgpu::BarrierArgs barrier_args(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC); // (api_contact.cu; kappa may be IPCGPU_KAPPA_DEVICE)
+ipcgpu::HalfSpaceArgs halfspace_args(ipcgpu_ctx* ctx);                                      // (api_terms.cu)
 ipcgpu::SortedGrid edge_grid(const ipcgpu_ctx* ctx);
 int boxes_and_grid(ipcgpu_ctx* ctx, double radius, bool with_vertex_boxes);
 

@@ -130,9 +130,9 @@ int energy_result(ipcgpu_ctx* ctx, int slot, double* E, bool fetch, unsigned che
 }
 // the tail of an energy term on the main stream: its partial sums reduced into the slot, the stage timer `pe` stopped, energy_result
 int energy_tail(ipcgpu_ctx* ctx, int slot, const double* partials, int n_partials, double scale, cudaEvent_t pe, double* E, bool fetch,
-    unsigned check)
+    unsigned check, const double* scale_dev)
 {
-    reduce_sum(partials, n_partials, scale, &ctx->iter.p->energy[slot], ctx->stream);
+    reduce_sum(partials, n_partials, scale, &ctx->iter.p->energy[slot], ctx->stream, scale_dev);
     ctx->prof_end(pe);
     ctx->launches += 2; // the term's partial kernel and the reduce
     CK(cudaGetLastError());

@@ -321,7 +321,9 @@ int ipcgpu_set_constraint_set(ipcgpu_ctx* ctx, int nC, const int* mm, int nP, co
     return IPCGPU_OK;
 }
 
-static BarrierArgs barrier_args(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC)
+} // extern "C"
+
+BarrierArgs barrier_args(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC)
 {
     BarrierArgs p;
     ContactWork& w = ctx->cw;
@@ -340,8 +342,11 @@ static BarrierArgs barrier_args(ipcgpu_ctx* ctx, double dHat, double kappa, int 
     p.row_hi = ctx->nranks > 1 ? ctx->v_end : ctx->nV;
     p.dHat = dHat; p.kappa = kappa; p.projectDBC = projectDBC;
     p.ia = ctx->ia.p; p.ja = ctx->ja.p; p.base = ctx->index_base;
+    p.kappa_dev = kappa_ptr(ctx, kappa);
     return p;
 }
+
+extern "C" {
 
 // ---- device-built sparsity pattern (pattern.cu) -------------------------------------------------------------------------
 int ipcgpu_enable_device_pattern(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity)
@@ -407,17 +412,19 @@ int ipcgpu_get_pattern(ipcgpu_ctx* ctx, int* ia, int* ja)
 int ipcgpu_barrier_energy(ipcgpu_ctx* ctx, double dHat, double kappa, double* E)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    REQUIRE_KAPPA(kappa);
     ENTER(kSerial);
     BarrierArgs p = barrier_args(ctx, dHat, kappa, 0);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     barrier_energy(p, ctx->cw.bpartials.p, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE], ctx->stream);
     // synchronous form: the d <= 0 flag is checked right here (every rank checks its own share of the pairs)
-    return energy_tail(ctx, kEnergyBarrier, ctx->cw.bpartials.p, barrier_energy_blocks(), kappa, pe, E, true, 1u << FLAG_NONPOSITIVE_DISTANCE);
+    return energy_tail(ctx, kEnergyBarrier, ctx->cw.bpartials.p, barrier_energy_blocks(), kappa, pe, E, true, 1u << FLAG_NONPOSITIVE_DISTANCE, p.kappa_dev);
 }
 
 int ipcgpu_barrier_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* g_inout)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    REQUIRE_KAPPA(kappa);
     const BarrierArgs p = barrier_args(ctx, dHat, kappa, 0);
     return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { barrier_gradient(p, ctx->g.p, st); });
 }
@@ -471,6 +478,7 @@ int ipcgpu_para_ee_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE(g_inout != nullptr, IPCGPU_ERR_ARG, "null gradient");
+    REQUIRE_KAPPA(kappa);
     ENTER(kSerial);
     int rc = gradient_roundtrip_begin(ctx, g_inout);
     if (rc) return rc;
@@ -483,6 +491,7 @@ int ipcgpu_para_ee_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
 int ipcgpu_barrier_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC, double* a_inout)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    REQUIRE_KAPPA(kappa);
     int rc = hessian_begin(ctx, kDerivative, a_inout);
     if (rc) return rc;
     ContactWork& w = ctx->cw;
@@ -535,6 +544,7 @@ static int friction_alloc(ipcgpu_ctx* ctx)
 int ipcgpu_friction_lag(ipcgpu_ctx* ctx, double dHat, double kappa, int* n_pairs)
 {
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    REQUIRE_KAPPA(kappa);
     ENTER(kSerial);
     int rc = friction_alloc(ctx);
     if (rc) return rc;

@@ -88,6 +88,8 @@ int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
     ctx->sc_pending = false;
     ctx->sv_pending_at_capture = ctx->sv_pending;
     ctx->sv_pending = false;
+    ctx->kp_pending_at_capture = ctx->kp_pending;
+    ctx->kp_pending = false;
     ctx->capture_bodies.clear();
     CK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
     ctx->capturing = true;
@@ -141,6 +143,8 @@ int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id)
     ctx->sc_pending = ctx->sc_pending_at_capture;
     rec.solve = ctx->sv_pending;
     ctx->sv_pending = ctx->sv_pending_at_capture;
+    rec.kappa = ctx->kp_pending;
+    ctx->kp_pending = ctx->kp_pending_at_capture;
     rec.bodies.swap(ctx->capture_bodies);
     rec.hs = snapshot_host_state(ctx);
     ctx->launches = ctx->launches_at_capture; // nothing ran yet
@@ -164,6 +168,7 @@ int ipcgpu_graph_launch(ipcgpu_ctx* ctx, int graph_id)
     if (rec.updates_pattern) ctx->pat_pending = true;
     if (rec.step_control) ctx->sc_pending = true;
     if (rec.solve) ctx->sv_pending = true;
+    if (rec.kappa) ctx->kp_pending = true;
     ctx->a_all_dirty = false;
     apply_host_state(ctx, rec.hs);
     ctx->launches += rec.launches;
@@ -429,7 +434,7 @@ static int line_search_body(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms& t)
 int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* t, double* alpha_inout)
 {
     REQUIRE(t != nullptr, IPCGPU_ERR_ARG, "null terms");
-    REQUIRE(t->dHat > 0.0 && t->kappa >= 0.0, IPCGPU_ERR_ARG, "dHat must be positive");
+    REQUIRE(t->dHat > 0.0 && (t->kappa >= 0.0 || kappa_on_device(t->kappa)), IPCGPU_ERR_ARG, "dHat must be positive, kappa >= 0 or IPCGPU_KAPPA_DEVICE");
     REQUIRE(!t->inertia || (ctx->xtilde_set && ctx->has_mass), IPCGPU_ERR_STATE, "inertia: ipcgpu_set_xtilde and a mass diagonal first");
     REQUIRE(!(t->fric_coef > 0.0) || (ctx->cw.fr_ready && ctx->prev_set && t->fric_eps2 > 0.0), IPCGPU_ERR_STATE,
         "friction: ipcgpu_friction_lag, ipcgpu_set_prev_state and fric_eps2 > 0 first");

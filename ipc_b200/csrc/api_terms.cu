@@ -447,7 +447,9 @@ int ipcgpu_dirichlet_completed_step(ipcgpu_ctx* ctx, double* s)
 }
 
 // ---- analytic half-space collision objects (halfspace.cu; which chain each call runs on: see enter()) ------------------------------------
-static HalfSpaceArgs halfspace_args(ipcgpu_ctx* ctx)
+} // extern "C"
+
+HalfSpaceArgs halfspace_args(ipcgpu_ctx* ctx)
 {
     HalfSpaceArgs p;
     p.nV = ctx->nV; p.nSV = ctx->nSV; p.nP = ctx->n_hs;
@@ -461,6 +463,8 @@ static HalfSpaceArgs halfspace_args(ipcgpu_ctx* ctx)
     p.ia = ctx->ia.p; p.base = ctx->index_base;
     return p;
 }
+
+extern "C" {
 
 int ipcgpu_set_halfspaces(ipcgpu_ctx* ctx, int n, const double* origin, const double* normal, const double* velocitydt, const double* friction)
 {
@@ -556,27 +560,33 @@ int ipcgpu_halfspace_energy(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
     if (E) *E = 0.0;
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_SET();
+    REQUIRE_KAPPA(kappa);
     ENTER(kSerial);
     const HalfSpaceArgs p = halfspace_args(ctx);
     cudaEvent_t pe = ctx->prof_begin(IPCGPU_STAGE_BARRIER);
     halfspace_energy(p, dHat, ctx->hs_partials.p, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE], ctx->stream);
-    return energy_tail(ctx, kEnergyPlaneBarrier, ctx->hs_partials.p, halfspace_energy_blocks(), kappa, pe, E, true, 1u << FLAG_NONPOSITIVE_DISTANCE);
+    return energy_tail(ctx, kEnergyPlaneBarrier, ctx->hs_partials.p, halfspace_energy_blocks(), kappa, pe, E, true, 1u << FLAG_NONPOSITIVE_DISTANCE,
+        kappa_ptr(ctx, kappa));
 }
 
 int ipcgpu_halfspace_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* g_inout)
 {
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_SET();
+    REQUIRE_KAPPA(kappa);
     const HalfSpaceArgs p = halfspace_args(ctx);
-    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { halfspace_gradient(p, dHat, kappa, ctx->g.p, st); });
+    const double* kd = kappa_ptr(ctx, kappa);
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { halfspace_gradient(p, dHat, kappa, kd, ctx->g.p, st); });
 }
 
 int ipcgpu_halfspace_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC, double* a_inout)
 {
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_SET();
+    REQUIRE_KAPPA(kappa);
     const HalfSpaceArgs p = halfspace_args(ctx);
-    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) { halfspace_hessian(p, dHat, kappa, projectDBC, ctx->a.p, st); });
+    const double* kd = kappa_ptr(ctx, kappa);
+    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) { halfspace_hessian(p, dHat, kappa, kd, projectDBC, ctx->a.p, st); });
 }
 
 int ipcgpu_halfspace_step(ipcgpu_ctx* ctx, const double* p_dir, double slackness, double* alpha_inout)
@@ -621,8 +631,9 @@ int ipcgpu_halfspace_friction_lag(ipcgpu_ctx* ctx, double dHat, double kappa, in
     if (n_lagged) *n_lagged = 0;
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_SET();
+    REQUIRE_KAPPA(kappa);
     ENTER(kSerial);
-    halfspace_lag(halfspace_args(ctx), dHat, kappa, ctx->hs_pstart.p, ctx->hs_lag.p, ctx->hs_lam.p, ctx->hs_cnt.p + 1, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE],
+    halfspace_lag(halfspace_args(ctx), dHat, kappa, kappa_ptr(ctx, kappa), ctx->hs_pstart.p, ctx->hs_lag.p, ctx->hs_lam.p, ctx->hs_cnt.p + 1, &ctx->iter.p->flags[FLAG_NONPOSITIVE_DISTANCE],
         ctx->iter.p, ctx->stream);
     ++ctx->launches;
     CK(cudaGetLastError());

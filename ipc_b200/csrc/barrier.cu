@@ -127,6 +127,12 @@ __global__ void __launch_bounds__(256) k_barrier_energy(BarrierArgs p, double* _
 // -----------------------------------------------------------------------------------------------------------
 // gradient: g += kappa*mult*b'(d) grad d   (+ para-EE: kappa*b*grad e + kappa*e*b' grad d)
 // -----------------------------------------------------------------------------------------------------------
+// kDevKappa: kappa is the device-resident one (BarrierArgs::kappa_dev).  A template parameter rather than a run-time test, and read where
+// p.kappa was, so that the host-kappa instantiations compile to the same code (registers, spills) as without the device kappa
+template <bool kDevKappa>
+DEV double barrier_kappa(const BarrierArgs& p) { return kDevKappa ? *p.kappa_dev : p.kappa; }
+
+template <bool kDevKappa>
 __global__ void __launch_bounds__(128) k_barrier_gradient(BarrierArgs p, double* __restrict__ g)
 {
     const ListRange lr = list_range(p, false);
@@ -143,7 +149,7 @@ __global__ void __launch_bounds__(128) k_barrier_gradient(BarrierArgs p, double*
     double b, db, d2b;
     barrier_all(d, p.dHat, b, db, d2b);
     double w;
-    if (!is_para) w = p.kappa * s.mult * db;
+    if (!is_para) w = barrier_kappa<kDevKappa>(p) * s.mult * db;
     else {
         int ev[4];
         para_edge_stencil(mm, p.para_e[c], p.SE, ev);
@@ -152,8 +158,8 @@ __global__ void __launch_bounds__(128) k_barrier_gradient(BarrierArgs p, double*
         double eg[12];
         const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, false, [](int, int, double) {});
         for (int k = 0; k < 4; ++k)
-            for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)ev[k] + q, p.kappa * b * eg[3 * k + q]);
-        w = p.kappa * e * db; // slot 3 is -1 (or a vertex id): multiplicity 1
+            for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)ev[k] + q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
+        w = barrier_kappa<kDevKappa>(p) * e * db; // slot 3 is -1 (or a vertex id): multiplicity 1
     }
     for (int k = 0; k < s.nv; ++k)
         for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)s.v[k] + q, w * gd[3 * k + q]);
@@ -190,6 +196,7 @@ __global__ void __launch_bounds__(128) k_constraint_jacobian_t(BarrierArgs p, co
     }
 }
 // augmentParaEEGradient (:2990-3045) alone: the mollified pairs' share of k_barrier_gradient
+template <bool kDevKappa>
 __global__ void __launch_bounds__(128) k_para_gradient(BarrierArgs p, double* __restrict__ g)
 {
     const ListRange lr = list_range(p, false);
@@ -209,8 +216,8 @@ __global__ void __launch_bounds__(128) k_para_gradient(BarrierArgs p, double* __
         double eg[12];
         const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, false, [](int, int, double) {});
         for (int k = 0; k < 4; ++k)
-            for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)ev[k] + q, p.kappa * b * eg[3 * k + q]);
-        const double w = p.kappa * e * db;
+            for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)ev[k] + q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
+        const double w = barrier_kappa<kDevKappa>(p) * e * db;
         for (int k = 0; k < s.nv; ++k)
             for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)s.v[k] + q, w * gd[3 * k + q]);
     }
@@ -224,6 +231,7 @@ __global__ void __launch_bounds__(128) k_para_gradient(BarrierArgs p, double* __
 // -----------------------------------------------------------------------------------------------------------
 DEV bool owns_row(const BarrierArgs& p, int v) { return v >= p.row_lo && v < p.row_hi; }
 
+template <bool kDevKappa>
 __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, double* __restrict__ Hraw, int* __restrict__ rows_out, int* __restrict__ n_owned,
     int capacity, int* __restrict__ flags)
 {
@@ -256,7 +264,7 @@ __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, dou
         const double d = pair_derivs(s, x, gd, true, [&](int i, int j, double v) { HE(i, j) = v; });
         double b, db, d2b;
         barrier_all(d, p.dHat, b, db, d2b);
-        const double coef = p.kappa * s.mult;
+        const double coef = barrier_kappa<kDevKappa>(p) * s.mult;
         for (int i = 0; i < n; ++i)
             for (int j = 0; j < n; ++j) HE(i, j) = ((coef * d2b) * gd[i]) * gd[j] + (coef * db) * HE(i, j);
     }
@@ -289,7 +297,7 @@ __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, dou
         double b, db, d2b;
         barrier_all(d, p.dHat, b, db, d2b);
         const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, true, [&](int i, int j, double v) { HE(i, j) = v; });
-        const double k = p.kappa;
+        const double k = barrier_kappa<kDevKappa>(p);
         for (int i = 0; i < 12; ++i)
             for (int j = 0; j < 12; ++j)
                 HE(i, j) = ((k * db) * gd[i]) * eg[j] + ((k * db) * gd[j]) * eg[i] + (k * b) * HE(i, j) + ((k * e * d2b) * gd[i]) * gd[j] + (k * e * db) * VE[i * 12 + j];
@@ -582,15 +590,21 @@ void barrier_energy(const BarrierArgs& p, double* partials, int* bad, cudaStream
 int barrier_energy_blocks() { return kBarrierEnergyBlocks; }
 void barrier_gradient(const BarrierArgs& p, double* g, cudaStream_t st)
 {
-    k_barrier_gradient<<<kSMs * 4, 128, 0, st>>>(p, g);
+    if (p.kappa_dev) k_barrier_gradient<true><<<kSMs * 4, 128, 0, st>>>(p, g);
+    else k_barrier_gradient<false><<<kSMs * 4, 128, 0, st>>>(p, g);
 }
 void evaluate_constraints(const BarrierArgs& p, double* val, cudaStream_t st) { k_evaluate_constraints<<<kSMs * 2, 256, 0, st>>>(p, val); }
 void constraint_jacobian_t(const BarrierArgs& p, const double* input, double coef, double* g, cudaStream_t st) { k_constraint_jacobian_t<<<kSMs * 4, 128, 0, st>>>(p, input, coef, g); }
-void para_gradient(const BarrierArgs& p, double* g, cudaStream_t st) { k_para_gradient<<<kSMs, 128, 0, st>>>(p, g); }
+void para_gradient(const BarrierArgs& p, double* g, cudaStream_t st)
+{
+    if (p.kappa_dev) k_para_gradient<true><<<kSMs, 128, 0, st>>>(p, g);
+    else k_para_gradient<false><<<kSMs, 128, 0, st>>>(p, g);
+}
 void barrier_hessian_build_project(const BarrierArgs& p, int* flags, double* Hraw, int* rows, int* psd, int* n_owned, int capacity, cudaStream_t st)
 {
     cudaMemsetAsync(n_owned, 0, sizeof(int), st);
-    k_barrier_hessian_build<<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
+    if (p.kappa_dev) k_barrier_hessian_build<true><<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
+    else k_barrier_hessian_build<false><<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
     k_barrier_hessian_project<<<kSMs * 4, 32 * kProjWarps, 0, st>>>(n_owned, capacity, Hraw, psd);
 }
 void barrier_hessian_scatter(const BarrierArgs& p, double* a, int* flags, const double* Hraw, const int* rows, const int* psd, const int* n_owned, int capacity, cudaStream_t st)

@@ -254,6 +254,13 @@ struct ipcgpu_ctx {
     ipcgpu::DevBuf<double> vel, acc, dxe;
     bool time_set = false;
     int dyn_nV = 0;
+    // device-resident barrier stiffness (kappa.cu): g_c of initKappa and the per-CTA partials of its two dot products, and the close set of
+    // postLineSearch (self / obstacle entries and plane entries, each with its saved d).  kp_pending: a kappa call was enqueued since the
+    // last ipcgpu_kappa_info
+    ipcgpu::DevBuf<double> kp_gc, kp_part, kp_close_mm_val, kp_close_hs_val;
+    ipcgpu::DevBuf<int4> kp_close_mm;
+    ipcgpu::DevBuf<int2> kp_close_hs;
+    bool kp_pending = false, kp_pending_at_capture = false;
     size_t ccd_capacity = (size_t)1 << 23; // candidate pairs
     std::vector<int> h_SVI;                // host copy (pSize of the swept build is a serial host sum, SpatialHash.hpp:603-612)
     double debug_prune_seed = -1.0;        // test hook, see ipcgpu_ccd_debug_seed_bound
@@ -314,6 +321,7 @@ struct ipcgpu_ctx {
         bool updates_pattern = false; // the sequence contains ipcgpu_update_pattern
         bool step_control = false;    // ... a CFL branch or a line search
         bool solve = false;           // ... a linear solve
+        bool kappa = false;           // ... a call that writes the device-resident kappa
         std::vector<cudaGraph_t> bodies; // bodies of its conditional nodes (owned by `graph`)
         HostState hs;
     };

@@ -82,8 +82,11 @@ __global__ void __launch_bounds__(256) k_elastic_energy(ElasticArgs p, double* _
     cta_sum(&e, partials + blockIdx.x);
 }
 
-// single-CTA fixed-order reduction of the per-CTA partials: out[0] = scale * sum
-__global__ void __launch_bounds__(1024) k_reduce_sum(const double* __restrict__ partials, int n, double scale, double* __restrict__ out)
+// single-CTA fixed-order reduction of the per-CTA partials: out[0] = scale * sum.  kDevScale: the scale is read from scale_dev (the
+// device-resident kappa of a barrier energy); a template parameter, so that the host-scale instantiation compiles as without it
+template <bool kDevScale>
+__global__ void __launch_bounds__(1024) k_reduce_sum(const double* __restrict__ partials, int n, double scale, double* __restrict__ out,
+    const double* __restrict__ scale_dev)
 {
     __shared__ double sm[32];
     double s = 0.0;
@@ -94,7 +97,7 @@ __global__ void __launch_bounds__(1024) k_reduce_sum(const double* __restrict__ 
     if (threadIdx.x < 32) {
         double v = (threadIdx.x < (blockDim.x >> 5)) ? sm[threadIdx.x] : 0.0;
         v = warp_sum(v);
-        if (threadIdx.x == 0) out[0] = scale * v;
+        if (threadIdx.x == 0) out[0] = (kDevScale ? *scale_dev : scale) * v;
     }
 }
 
@@ -583,7 +586,11 @@ void elastic_energy(const ElasticArgs& p, double* e_per_tet, double* partials, c
     else k_elastic_energy<1><<<nb, 256, 0, st>>>(p, e_per_tet, partials);
 }
 int elastic_energy_blocks(int nTets) { return (nTets + 255) / 256; }
-void reduce_sum(const double* partials, int n, double scale, double* out, cudaStream_t st) { k_reduce_sum<<<1, 1024, 0, st>>>(partials, n, scale, out); }
+void reduce_sum(const double* partials, int n, double scale, double* out, cudaStream_t st, const double* scale_dev)
+{
+    if (scale_dev) k_reduce_sum<true><<<1, 1024, 0, st>>>(partials, n, scale, out, scale_dev);
+    else k_reduce_sum<false><<<1, 1024, 0, st>>>(partials, n, scale, out, nullptr);
+}
 
 int elastic_grad_hess_blocks(int n_list) { return (n_list + kHessTile - 1) / kHessTile; }
 template <int ENERGY, bool G, bool H>

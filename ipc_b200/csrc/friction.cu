@@ -69,6 +69,7 @@ __global__ void __launch_bounds__(128) k_friction_lag(BarrierArgs p, int4* __res
     double2* __restrict__ coord, double* __restrict__ basis, int capacity, int* __restrict__ bad)
 {
     const int n = min(*p.nC, capacity);
+    const double kappa = p.kappa_dev ? *p.kappa_dev : p.kappa;
     if (blockIdx.x == 0 && threadIdx.x == 0) *n_out = n;
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) {
         const int4 mm = p.cs[c];
@@ -80,7 +81,7 @@ __global__ void __launch_bounds__(128) k_friction_lag(BarrierArgs p, int4* __res
         double b, db, d2b;
         barrier_all(d, p.dHat, b, db, d2b);
         double lam = db;
-        lam *= -p.kappa * 2.0 * sqrt(d);
+        lam *= -kappa * 2.0 * sqrt(d);
         if (mm.x < 0 && mm.w < -1) lam *= (double)(-mm.w); // PP or PE duplication (Optimizer.cpp:1588-1591)
         // no friction against a mesh obstacle: the reference's MeshCO does not implement the friction functions (CollisionObject.h:403-423 throw),
         // Optimizer.cpp:1582-1600 lags the self-contact set only.  A zero normal force switches the pair's E / g / H off.

@@ -84,8 +84,10 @@ __global__ void __launch_bounds__(256) k_hs_energy(HalfSpaceArgs p, double dHat,
     cta_sum(&val, partials + blockIdx.x);
 }
 
-__global__ void __launch_bounds__(128) k_hs_gradient(HalfSpaceArgs p, double dHat, double kappa, double* __restrict__ g)
+// kappa_dev != nullptr (the barrier kernels below): kappa is the device-resident one
+__global__ void __launch_bounds__(128) k_hs_gradient(HalfSpaceArgs p, double dHat, double kappa, const double* __restrict__ kappa_dev, double* __restrict__ g)
 {
+    if (kappa_dev) kappa = *kappa_dev;
     const int n = *p.n_act;
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) {
         const int2 e = p.act[c];
@@ -108,8 +110,10 @@ DEV void add_diag_block(const HalfSpaceArgs& p, int v, const double* M, double* 
     }
 }
 
-__global__ void __launch_bounds__(128) k_hs_hessian(HalfSpaceArgs p, double dHat, double kappa, int projectDBC, double* __restrict__ a)
+__global__ void __launch_bounds__(128) k_hs_hessian(HalfSpaceArgs p, double dHat, double kappa, const double* __restrict__ kappa_dev, int projectDBC,
+    double* __restrict__ a)
 {
+    if (kappa_dev) kappa = *kappa_dev;
     const int n = *p.n_act;
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) {
         const int2 e = p.act[c];
@@ -171,9 +175,10 @@ __global__ void __launch_bounds__(256) k_hs_crossings(HalfSpaceArgs p, int* __re
 
 // ---- friction ------------------------------------------------------------------------------------------------------------
 // lag: the active entries of the planes with friction > 0, in order; lambda = -kappa 2 sqrt(d) b'(d)
-__global__ void __launch_bounds__(128) k_hs_lag(HalfSpaceArgs p, double dHat, double kappa, const int* __restrict__ pstart, int2* __restrict__ lag, double* __restrict__ lam,
-    int* __restrict__ n_lag, int* __restrict__ bad, IterState* __restrict__ st)
+__global__ void __launch_bounds__(128) k_hs_lag(HalfSpaceArgs p, double dHat, double kappa, const double* __restrict__ kappa_dev, const int* __restrict__ pstart,
+    int2* __restrict__ lag, double* __restrict__ lam, int* __restrict__ n_lag, int* __restrict__ bad, IterState* __restrict__ st)
 {
+    if (kappa_dev) kappa = *kappa_dev;
     const int n = pstart[p.nP];
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         int m = 0;
@@ -303,13 +308,13 @@ void halfspace_energy(const HalfSpaceArgs& p, double dHat, double* partials, int
 {
     k_hs_energy<<<kHsEnergyBlocks, 256, 0, st>>>(p, dHat, partials, bad);
 }
-void halfspace_gradient(const HalfSpaceArgs& p, double dHat, double kappa, double* g, cudaStream_t st)
+void halfspace_gradient(const HalfSpaceArgs& p, double dHat, double kappa, const double* kappa_dev, double* g, cudaStream_t st)
 {
-    k_hs_gradient<<<kSMs, 128, 0, st>>>(p, dHat, kappa, g);
+    k_hs_gradient<<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, g);
 }
-void halfspace_hessian(const HalfSpaceArgs& p, double dHat, double kappa, int projectDBC, double* a, cudaStream_t st)
+void halfspace_hessian(const HalfSpaceArgs& p, double dHat, double kappa, const double* kappa_dev, int projectDBC, double* a, cudaStream_t st)
 {
-    k_hs_hessian<<<kSMs, 128, 0, st>>>(p, dHat, kappa, projectDBC, a);
+    k_hs_hessian<<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, projectDBC, a);
 }
 void halfspace_step(const HalfSpaceArgs& p, const double* dir, double slack, IterState* st_dev, cudaStream_t st)
 {
@@ -321,9 +326,10 @@ void halfspace_crossings(const HalfSpaceArgs& p, IterState* st_dev, cudaStream_t
     zero_words(&st_dev->hs_crossings, 1, st);
     k_hs_crossings<<<grid_for(p.nV, 256), 256, 0, st>>>(p, &st_dev->hs_crossings);
 }
-void halfspace_lag(const HalfSpaceArgs& p, double dHat, double kappa, const int* pstart, int2* lag, double* lam, int* n_lag, int* bad, IterState* st_dev, cudaStream_t st)
+void halfspace_lag(const HalfSpaceArgs& p, double dHat, double kappa, const double* kappa_dev, const int* pstart, int2* lag, double* lam, int* n_lag, int* bad,
+    IterState* st_dev, cudaStream_t st)
 {
-    k_hs_lag<<<kSMs, 128, 0, st>>>(p, dHat, kappa, pstart, lag, lam, n_lag, bad, st_dev);
+    k_hs_lag<<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, pstart, lag, lam, n_lag, bad, st_dev);
 }
 void halfspace_friction_energy(const HalfSpaceArgs& p, double eps2, double* partials, cudaStream_t st)
 {

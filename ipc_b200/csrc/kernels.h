@@ -67,6 +67,18 @@ struct IterState {
     int pat_ok;                       // the raw contact keys of the update in flight fit the key buffer
     int pat_diff;                     // the extra blocks of the update in flight differ from the previous ones
     int pat_pad_;
+    // barrier stiffness held on the device (kappa.cu): read by the barrier / plane calls given IPCGPU_KAPPA_DEVICE, adapted by initKappa and
+    // postLineSearch's close-pair doubling
+    double kappa;                     // kappa
+    double kappa_suggest, kappa_max;  // suggestKappa / upperBoundKappa at the current dHat (ipcgpu_set_kappa)
+    double kappa_min_last;            // minKappa = -g_c.g_E / |g_c|^2 of the last initKappa (NaN for g_c = 0)
+    double kappa_dot[2];              // g_c.g_E and g_c.g_c of the initKappa in flight
+    unsigned long long kappa_dmin_ord;// min d^2 over the active entries of the last snapshot (order-preserving image)
+    int kappa_doublings;              // doublings since the last ipcgpu_set_kappa
+    int kappa_n_close[2];             // close set: self / obstacle entries, plane entries
+    int kappa_needs_init;             // postLineSearch met kappa == 0: initKappa is due
+    int kappa_hit;                    // a saved close entry is not farther than its snapshot (the check in flight)
+    int kappa_skip;                   // the check in flight found kappa == 0: no snapshot
 };
 // step_decide operations (step_control.cu) and the energy terms of a line search.  kSolveStart / kSolveBurst: the Krylov loops of both
 // built-in solvers (solve.cu, multilevel.cu)
@@ -156,6 +168,7 @@ struct BarrierArgs {
     int projectDBC;
     const int* ia; const int* ja; int base;
     int nVdof; // first obstacle vertex (SurfArgs::nVdof)
+    const double* kappa_dev; // nullptr: kappa above; else the device-resident kappa (IterState::kappa), read at run time
 };
 
 // barrier.cu
@@ -192,7 +205,8 @@ void friction_hessian(const FrictionArgs& p, double* a, int* err, cudaStream_t s
 // pattern.cu: a[ia[row0] - base, ia[row1] - base) = 0 with the range read on the device (the value-array clear of the device-built pattern)
 void zero_csr_rows(const int* ia, int base, int row0, int row1, double* a, cudaStream_t st);
 // elastic.cu (shared fixed-order reduction)
-void reduce_sum(const double* partials, int n, double scale, double* out, cudaStream_t st);
+// scale_dev != nullptr: the scale is read on the device from there instead of `scale`
+void reduce_sum(const double* partials, int n, double scale, double* out, cudaStream_t st, const double* scale_dev = nullptr);
 
 // misc.cu.  alpha_ord != nullptr: the step is read on the device from there (an IterState::step_ord) instead of `alpha`
 void step_forward(int nV, const double* x0_soa, const double* p_interleaved, double alpha, double* x_soa, cudaStream_t st,
@@ -228,11 +242,12 @@ size_t halfspace_scan_bytes(int n);
 cudaError_t halfspace_active_set(const HalfSpaceArgs& p, double dHat, int* flags, int* offs, void* scan_tmp, size_t scan_bytes, int2* act, int* n_act,
     int* pstart, IterState* st_dev, cudaStream_t st);
 void halfspace_energy(const HalfSpaceArgs& p, double dHat, double* partials, int* bad, cudaStream_t st);
-void halfspace_gradient(const HalfSpaceArgs& p, double dHat, double kappa, double* g, cudaStream_t st);
-void halfspace_hessian(const HalfSpaceArgs& p, double dHat, double kappa, int projectDBC, double* a, cudaStream_t st);
+// kappa_dev != nullptr: kappa is read on the device from there (IterState::kappa)
+void halfspace_gradient(const HalfSpaceArgs& p, double dHat, double kappa, const double* kappa_dev, double* g, cudaStream_t st);
+void halfspace_hessian(const HalfSpaceArgs& p, double dHat, double kappa, const double* kappa_dev, int projectDBC, double* a, cudaStream_t st);
 void halfspace_step(const HalfSpaceArgs& p, const double* dir, double slack, IterState* st_dev, cudaStream_t st);
 void halfspace_crossings(const HalfSpaceArgs& p, IterState* st_dev, cudaStream_t st);
-void halfspace_lag(const HalfSpaceArgs& p, double dHat, double kappa, const int* pstart, int2* lag, double* lam, int* n_lag, int* bad, IterState* st_dev, cudaStream_t st);
+void halfspace_lag(const HalfSpaceArgs& p, double dHat, double kappa, const double* kappa_dev, const int* pstart, int2* lag, double* lam, int* n_lag, int* bad, IterState* st_dev, cudaStream_t st);
 void halfspace_friction_energy(const HalfSpaceArgs& p, double eps2, double* partials, cudaStream_t st);
 void halfspace_friction_gradient(const HalfSpaceArgs& p, double eps2, double* g, cudaStream_t st);
 void halfspace_friction_hessian(const HalfSpaceArgs& p, double eps2, int projectDBC, double* a, cudaStream_t st);

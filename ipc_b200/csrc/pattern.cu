@@ -263,7 +263,7 @@ int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity)
     for (int* p : { w.row_cnt.p, w.ucnt.p, w.prev_ptr.p }) CK(cudaMemsetAsync(p, 0, n1 * sizeof(int), ctx->stream)); // no extra blocks yet
     {   // result of the "last update": the mesh pattern, unchanged, version 0
         struct { long long nnz; unsigned long long version; int changed, ok, diff, pad; } r = { mesh_nnz, 0ull, 0, 1, 0, 0 };
-        static_assert(sizeof(r) == sizeof(IterState) - offsetof(IterState, pat_nnz), "IterState pattern words");
+        static_assert(sizeof(r) == offsetof(IterState, kappa) - offsetof(IterState, pat_nnz), "IterState pattern words");
         CK(cudaMemcpyAsync(reinterpret_cast<char*>(ctx->iter.p) + offsetof(IterState, pat_nnz), &r, sizeof(r), cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream)); // (host vectors and r go out of scope)
     }

@@ -150,7 +150,15 @@ SIGNATURES = {
     "ipcgpu_compute_xtilde": (C.c_int, [_ctxp]),
     "ipcgpu_end_time_step": (C.c_int, [_ctxp]),
     "ipcgpu_warm_start": (C.c_int, [_ctxp, C.c_int, C.c_double, C.c_double, _dp, _dp, _dp]),
+    "ipcgpu_kappa_bounds": (C.c_int, [C.c_double, C.c_double, C.c_double, C.c_double, _dp, _dp]),
+    "ipcgpu_set_kappa": (C.c_int, [_ctxp, C.c_double, C.c_double, C.c_double]),
+    "ipcgpu_kappa_init": (C.c_int, [_ctxp, C.c_double]),
+    "ipcgpu_kappa_clear_close_set": (C.c_int, [_ctxp]),
+    "ipcgpu_kappa_post_line_search": (C.c_int, [_ctxp, C.c_double]),
+    "ipcgpu_kappa_info": (C.c_int, [_ctxp, C.c_void_p]),
 }
+# IPCGPU_KAPPA_DEVICE: as a kappa argument, the barrier stiffness held in device memory (Context.set_kappa)
+KAPPA_DEVICE = -1.0
 TIT_BE, TIT_NM = 0, 1
 
 STAGES = ["elastic_energy", "elastic_tet", "gather_gradient", "assemble_csr", "inversion", "hash", "constraint_set", "barrier",
@@ -181,6 +189,12 @@ class StepControl(C.Structure):
     _fields_ = [("alpha_cfl", C.c_double), ("alpha_feasible", C.c_double), ("alpha", C.c_double), ("energy_start", C.c_double), ("energy", C.c_double),
                 ("full_ccd", C.c_int), ("stopped", C.c_int), ("halvings_inversion", C.c_int), ("halvings_intersection", C.c_int),
                 ("halvings_armijo", C.c_int), ("halvings_post_check", C.c_int), ("post_check_rebuilt", C.c_int), ("status", C.c_int)]
+
+
+class KappaInfo(C.Structure):
+    """ipcgpu_kappa (include/ipcgpu.h)"""
+    _fields_ = [("kappa", C.c_double), ("min_kappa", C.c_double), ("suggest", C.c_double), ("max", C.c_double), ("close_min_dist2", C.c_double),
+                ("doublings", C.c_int), ("n_close", C.c_int), ("needs_init", C.c_int)]
 
 
 class SolveResult(C.Structure):
@@ -782,6 +796,33 @@ class Context:
         """ipcgpu_step_control of the last CFL branch / line search (its status is out.status, not raised)"""
         out = StepControl()
         self.lib.ipcgpu_step_control_info(self.h, C.byref(out))
+        return out
+
+    # ---- adaptive barrier stiffness (kappa held on the device; pass KAPPA_DEVICE as the kappa of the barrier calls) --------------
+    @staticmethod
+    def kappa_bounds(dHat, kappa_min_multiplier, avg_node_mass, bbox_diag2):
+        """(suggestKappa, upperBoundKappa's kappaMax); host-only"""
+        s, m = C.c_double(), C.c_double()
+        rc = load().ipcgpu_kappa_bounds(float(dHat), float(kappa_min_multiplier), float(avg_node_mass), float(bbox_diag2), C.byref(s), C.byref(m))
+        if rc:
+            raise IpcGpuError(f"ipcgpu_kappa_bounds failed with {ERR_NAMES.get(rc, rc)}")
+        return s.value, m.value
+
+    def set_kappa(self, kappa, suggest, kmax):
+        self._ck(self.lib.ipcgpu_set_kappa(self.h, float(kappa), float(suggest), float(kmax)))
+
+    def kappa_init(self, dHat):
+        self._ck(self.lib.ipcgpu_kappa_init(self.h, float(dHat)))
+
+    def kappa_clear_close_set(self):
+        self._ck(self.lib.ipcgpu_kappa_clear_close_set(self.h))
+
+    def kappa_post_line_search(self, dTol):
+        self._ck(self.lib.ipcgpu_kappa_post_line_search(self.h, float(dTol)))
+
+    def kappa_info(self):
+        out = KappaInfo()
+        self._ck(self.lib.ipcgpu_kappa_info(self.h, C.byref(out)))
         return out
 
     def hash_build_swept(self, p, alpha, h):
