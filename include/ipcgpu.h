@@ -484,6 +484,38 @@ typedef struct ipcgpu_kappa {
 /* synchronises only when a kappa call was enqueued since the last read */
 int ipcgpu_kappa_info(ipcgpu_ctx* ctx, ipcgpu_kappa* out);
 
+/* ---- end-of-step diagnostics (DESIGN.md section 3.19, INTEGRATION.md section 10) ---------------------------------------------------------
+ * The per-step reductions the reference takes over full-size state, so that a binding needs no download of V, V_prev or the per-tet energies
+ * at every step.  Single rank: IPCGPU_ERR_STATE with several.  Every sum has one fixed order (no value atomics): the same state gives the same
+ * bits, eagerly or replayed from a graph. */
+/* The components of the mesh, as the reference's cumulative compVAccSize / compFAccSize (main.cpp:1107-1112): one entry per `shapes` line, in
+ * order; a codimensional component repeats the previous tet_end.  The obstacle tail belongs to no component: vertex_end[n - 1] must be the
+ * mesh's own vertex count (the first obstacle vertex of ipcgpu_set_obstacle_tail, else nV) and tet_end[n - 1] the tet count.  IPCGPU_ERR_ARG
+ * for n < 1, a negative first entry, decreasing ends or other last entries.  Builds and uploads the segment table once; graphs captured
+ * before are refused (as after ipcgpu_set_mesh, which removes the components). */
+int ipcgpu_set_components(ipcgpu_ctx* ctx, int n, const int* vertex_end, const int* tet_end);
+/* Optimizer::computeSystemEnergy (Optimizer.cpp:3746-3778), which fullyImplicit_IP calls once per time step (:1799-1816): per component c,
+ *   sysE[c] = sum over its tets of vol psi(F) at V + sum over its vertices of m (|V - V_prev|^2 / dtSq / 2 - g.V),
+ *   sysM[c] = sum p, sysL[c] = sum V x p, with p = m / dt (V - V_prev)   (sysM, sysL: n rows of xyz),
+ * with m the mass diagonal of ipcgpu_set_mesh, dt, dtSq and g of ipcgpu_set_time_integration; Dirichlet vertices count.  Call it where the
+ * reference does, after the Newton iterations and before ipcgpu_end_time_step (V_prev is the previous step's V).  Overwrites the per-tet
+ * energies (IPCGPU_BUF_ENERGY_PER_TET).  Host outputs: synchronises and copies; all three NULL: deferred and capturable, read later with
+ * ipcgpu_get_system_energy.  IPCGPU_ERR_STATE without components, time integration, a mass diagonal or V_prev. */
+int ipcgpu_system_energy(ipcgpu_ctx* ctx, double* sysE, double* sysM, double* sysL);
+int ipcgpu_get_system_energy(ipcgpu_ctx* ctx, double* sysE, double* sysM, double* sysL); /* the last ipcgpu_system_energy; synchronises */
+typedef struct ipcgpu_constraint_summary_result {
+    int n;                        /* entries: the planes' active entries + the self / obstacle active entries; 0 = "no collision" */
+    double d_min, d_max;          /* min and max squared distance over them (0 for n = 0) */
+    double fb_norm;               /* |fb|, fb_i = dual_i + d_i - sqrt(dual_i^2 + d_i^2), dual_i = -kappa g_b(d_i, dHat) (0 for n = 0) */
+} ipcgpu_constraint_summary_result;
+/* The read-back after each solveSub_IP (Optimizer.cpp:1619-1757 with USE_DISCRETE_CMS, HOMOTOPY_VAR 1): the constraint values of every
+ * handler -- the planes' active (plane, vertex) entries with d as the half-space kernels evaluate it, then the self / obstacle active entries
+ * with the values of ipcgpu_evaluate_constraints; no mollified entries -- reduced to their count, range (the dTol fail-safe, dHatTarget,
+ * fricDHatThres) and the Fischer-Burmeister norm the reference logs (:1681-1692).  The decisions stay with the caller.  kappa may be
+ * IPCGPU_KAPPA_DEVICE.  out NULL: deferred and capturable, read later with ipcgpu_get_constraint_summary; otherwise synchronises. */
+int ipcgpu_constraint_summary(ipcgpu_ctx* ctx, double dHat, double kappa, ipcgpu_constraint_summary_result* out);
+int ipcgpu_get_constraint_summary(ipcgpu_ctx* ctx, ipcgpu_constraint_summary_result* out); /* the last ipcgpu_constraint_summary; synchronises */
+
 /* ---- kinematic mesh obstacle: MeshCO<3> (src/CollisionObject/MeshCO.hpp:39-233; SURVEY 8 row f3, barrier / Tight-Inclusion path) --------------------
  * An obstacle is a triangle mesh without degrees of freedom (MeshCO's Base::V, edges, Base::F).  It rides at the TAIL of the mesh's arrays: the
  * caller appends the obstacle's vertices to the vertex arrays of ipcgpu_set_mesh (rest = current positions, Dirichlet flag 1, mass 0, no

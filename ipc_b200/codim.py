@@ -169,3 +169,12 @@ def codim_scene(components, YM=1e5, PR=0.4, density=1000.0, energy=0):
     m.bbox_diag2 = float(((m.V_rest.max(0) - m.V_rest.min(0)) ** 2).sum())
     m._nbr = None
     return m
+
+
+def component_ends(m):
+    """(vertex_end, tet_end): the cumulative compVAccSize / compFAccSize of ipcgpu_set_components from componentNodeRange.  A tet belongs
+    to the component of its first vertex (codim_scene appends the tets in component order); codimensional components add no tet."""
+    rng = np.asarray(m.componentNodeRange, dtype=np.int64)
+    comp_of_tet = np.searchsorted(rng, np.asarray(m.T)[:, 0], side="right") - 1
+    tets = np.bincount(comp_of_tet, minlength=len(rng) - 1)
+    return rng[1:].astype(np.int32), np.cumsum(tets).astype(np.int32)

@@ -74,6 +74,10 @@ static inline int nblk(long long n, int b) { return (int)((n + b - 1) / b); }
 //     _kappa_post_line_search (which reads V and the contact sets) -- is kSerial, which orders it before the derivative chain.  The pair-Hessian
 //     build of ipcgpu_barrier_hessian runs on the side stream, which waits on ev_inputs only: the three calls that write kappa mark the
 //     inputs (mark_inputs) as a position or set change does.  The step-bound chain touches none of them.
+//   - end-of-step diagnostics (diagnostics.cu): ipcgpu_system_energy reads V, Vprev, mass and TimeParams and writes e_per_tet and partials
+//     (the per-tet elastic energy, as ipcgpu_elastic_energy does) and diag_part / diag_sys; ipcgpu_constraint_summary reads V, the self /
+//     obstacle active list, the plane set and IterState::kappa and writes cw.bval and diag_sum*.  Both are kSerial: e_per_tet and bval are
+//     no input of either chain, and the chains' writes to V and the lists are ordered before them.
 //   - V, Vrest, SE, dbc, ia, ja: read by both, written by neither (ia / ja / slot_off are written only by ipcgpu_update_pattern, which joins).  g, a, gcont, hblk, e_partials2, bHraw, brows, bpsd:
 //     derivative chain only.  dir, pSize_dev, inv_steps: step-bound chain only.
 enum Chain { kSerial, kStepBound, kDerivative };

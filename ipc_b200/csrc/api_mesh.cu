@@ -225,6 +225,7 @@ int ipcgpu_set_mesh(ipcgpu_ctx* ctx, int nV, int nT, const double* Vrest, const 
     ctx->energy = energy;
     ctx->hs_set_built = ctx->hs_lag_ready = false; // the plane sets index the old vertices
     ctx->nVdof = 0x7fffffff; // a new mesh has no obstacle tail until ipcgpu_set_obstacle_tail names one
+    ctx->n_comp = 0;         // ... and no components until ipcgpu_set_components names them
     ctx->h_T.assign(tets, tets + (size_t)4 * nT);
     ctx->h_ia.clear();
     ctx->nnz = 0;

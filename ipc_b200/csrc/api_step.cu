@@ -1,6 +1,7 @@
 // api_step.cu -- entry points that drive a whole sequence: CUDA-graph capture and replay, the line-search safeguards, and the step control
 // (CFL branch and line search) built from conditional graph nodes.
 #include "abi.h"
+#include <algorithm>
 #include <cstring>
 #include <vector>
 
@@ -523,6 +524,145 @@ int ipcgpu_step_control_info(ipcgpu_ctx* ctx, ipcgpu_step_control* out)
     out->post_check_rebuilt = h.ls_rebuilt;
     out->status = h.sc_status;
     return step_control_status(ctx, h.sc_status);
+}
+
+} // extern "C"
+
+// ---- end-of-step diagnostics (diagnostics.cu): Optimizer::computeSystemEnergy (:3746-3778) and the constraint summary of the homotopy
+// read-back after solveSub_IP (:1619-1691).  Both run on one rank and enter kSerial (abi.h); the reductions are fixed-order sums.
+static int diag_copy(ipcgpu_ctx* ctx, void* dst, const void* src, size_t bytes)
+{
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (bytes) CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
+    return IPCGPU_OK;
+}
+
+extern "C" {
+
+int ipcgpu_set_components(ipcgpu_ctx* ctx, int n, const int* vertex_end, const int* tet_end)
+{
+    REQUIRE(ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh first");
+    REQUIRE(n >= 1 && vertex_end && tet_end, IPCGPU_ERR_ARG, "ipcgpu_set_components: n >= 1 components and both arrays");
+    const int nv_own = std::min(ctx->nV, ctx->nVdof); // (the obstacle tail belongs to no component)
+    REQUIRE(vertex_end[0] >= 0 && tet_end[0] >= 0, IPCGPU_ERR_ARG, "ipcgpu_set_components: negative first entry");
+    for (int c = 1; c < n; ++c)
+        REQUIRE(vertex_end[c] >= vertex_end[c - 1] && tet_end[c] >= tet_end[c - 1], IPCGPU_ERR_ARG, "ipcgpu_set_components: the ends must not decrease");
+    REQUIRE(vertex_end[n - 1] == nv_own && tet_end[n - 1] == ctx->nT, IPCGPU_ERR_ARG,
+        "ipcgpu_set_components: the last ends must be the mesh's own vertex count (without the obstacle tail) and its tet count");
+    ENTER(kSerial);
+    ++ctx->epoch; // graphs captured before this call are refused (the segment table and its buffers change)
+    // every component's tet range, then its vertex range, cut at the multiples of kDiagChunk
+    std::vector<DiagSegment> seg;
+    std::vector<int> first((size_t)n + 1);
+    auto cut = [&](int lo, int hi, int kind) {
+        for (int b = lo; b < hi;) {
+            const int e = std::min(hi, (b / kDiagChunk + 1) * kDiagChunk);
+            seg.push_back(DiagSegment{ b, e, kind, 0 });
+            b = e;
+        }
+    };
+    for (int c = 0; c < n; ++c) {
+        first[c] = (int)seg.size();
+        cut(c ? tet_end[c - 1] : 0, tet_end[c], kSegTets);
+        cut(c ? vertex_end[c - 1] : 0, vertex_end[c], kSegVertices);
+    }
+    first[n] = (int)seg.size();
+    REQUIRE(ctx->diag_seg.upload(seg.data(), seg.size(), ctx->stream) && ctx->diag_comp_seg.upload(first.data(), first.size(), ctx->stream),
+        IPCGPU_ERR_CUDA, "component table upload failed");
+    ALLOC(ctx->diag_part, (size_t)7 * std::max(seg.size(), (size_t)1));
+    ALLOC(ctx->diag_sys, (size_t)7 * n);
+    CK(cudaMemsetAsync(ctx->diag_sys.p, 0, (size_t)7 * n * sizeof(double), ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream)); // (the table's host copy goes out of scope)
+    ctx->n_comp = n;
+    ctx->n_seg = (int)seg.size();
+    ctx->comp_v_end = nv_own;
+    return IPCGPU_OK;
+}
+
+int ipcgpu_system_energy(ipcgpu_ctx* ctx, double* sysE, double* sysM, double* sysL)
+{
+    const bool host = sysE || sysM || sysL;
+    REQUIRE(!host || (sysE && sysM && sysL), IPCGPU_ERR_ARG, "ipcgpu_system_energy: all three outputs or none (deferred)");
+    REQUIRE(!(host && ctx->capturing), IPCGPU_ERR_STATE, "inside a capture: NULL outputs, read later with ipcgpu_get_system_energy");
+    REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the system energy runs on one rank");
+    REQUIRE(ctx->maps_ready && ctx->n_comp > 0, IPCGPU_ERR_STATE, "ipcgpu_set_components first");
+    REQUIRE(ctx->comp_v_end == std::min(ctx->nV, ctx->nVdof), IPCGPU_ERR_STATE, "the obstacle tail moved since ipcgpu_set_components: set the components again");
+    REQUIRE(ctx->time_set, IPCGPU_ERR_STATE, "ipcgpu_set_time_integration first");
+    REQUIRE(ctx->has_mass, IPCGPU_ERR_STATE, "no mass diagonal: ipcgpu_set_mesh with a mass");
+    REQUIRE(ctx->prev_set && ctx->Vprev.n >= (size_t)3 * ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_prev_state first");
+    ENTER(kSerial);
+    cudaStream_t st = ctx->stream;
+    elastic_energy(ctx->eargs(), ctx->e_per_tet.p, ctx->partials.p, st); // vol psi per tet at V (getEnergyValPerElemBySVD, :3750)
+    if (ctx->nT > 0) ++ctx->launches;
+    SystemEnergyArgs a;
+    a.nV = ctx->nV; a.n_comp = ctx->n_comp; a.n_seg = ctx->n_seg;
+    a.seg = ctx->diag_seg.p; a.comp_seg = ctx->diag_comp_seg.p;
+    a.e_per_tet = ctx->e_per_tet.p; a.V = ctx->V.p; a.Vprev = ctx->Vprev.p; a.mass = ctx->mass.p; a.tp = ctx->tparams.p;
+    a.part = ctx->diag_part.p; a.out = ctx->diag_sys.p;
+    system_energy(a, st);
+    ctx->launches += (ctx->n_seg > 0) + 1;
+    CK(cudaGetLastError());
+    return host ? ipcgpu_get_system_energy(ctx, sysE, sysM, sysL) : IPCGPU_OK;
+}
+
+int ipcgpu_get_system_energy(ipcgpu_ctx* ctx, double* sysE, double* sysM, double* sysL)
+{
+    REQUIRE(sysE && sysM && sysL, IPCGPU_ERR_ARG, "null output");
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is in progress");
+    REQUIRE(ctx->n_comp > 0, IPCGPU_ERR_STATE, "ipcgpu_set_components first");
+    ENTER(kSerial);
+    const size_t n = (size_t)ctx->n_comp;
+    int rc = diag_copy(ctx, sysE, ctx->diag_sys.p, n * sizeof(double));
+    if (!rc) rc = diag_copy(ctx, sysM, ctx->diag_sys.p + n, 3 * n * sizeof(double));
+    if (!rc) rc = diag_copy(ctx, sysL, ctx->diag_sys.p + 4 * n, 3 * n * sizeof(double));
+    return rc;
+}
+
+int ipcgpu_constraint_summary(ipcgpu_ctx* ctx, double dHat, double kappa, ipcgpu_constraint_summary_result* out)
+{
+    REQUIRE(dHat > 0.0 && (kappa >= 0.0 || kappa_on_device(kappa)), IPCGPU_ERR_ARG, "dHat must be positive, kappa >= 0 or IPCGPU_KAPPA_DEVICE");
+    REQUIRE(!(out && ctx->capturing), IPCGPU_ERR_STATE, "inside a capture: a NULL output, read later with ipcgpu_get_constraint_summary");
+    REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the constraint summary runs on one rank");
+    REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
+    REQUIRE(ctx->n_hs == 0 || ctx->hs_set_built, IPCGPU_ERR_STATE, "half-spaces: ipcgpu_halfspace_constraint_set first");
+    ENTER(kSerial);
+    ContactWork& w = ctx->cw;
+    ALLOC(w.bval, (size_t)std::max(w.cap, 1));
+    ALLOC(ctx->diag_sum_part, (size_t)kDiagSummaryBlocks);
+    ALLOC(ctx->diag_sum_ord, (size_t)2 * kDiagSummaryBlocks);
+    ALLOC(ctx->diag_sum, 4);
+    cudaStream_t st = ctx->stream;
+    // the self / obstacle values as ipcgpu_evaluate_constraints computes them, over the same list
+    BarrierArgs p = barrier_args(ctx, dHat, 1.0, 0);
+    p.cs = w.act.p; p.nC = w.counters.p + 0;
+    evaluate_constraints(p, w.bval.p, st);
+    SummaryArgs s;
+    s.nV = ctx->nV; s.V = ctx->V.p;
+    const bool planes = ctx->n_hs > 0;
+    s.par = planes ? ctx->hs_par.p : nullptr; s.act = planes ? ctx->hs_act.p : nullptr; s.n_act = planes ? ctx->hs_cnt.p : nullptr;
+    s.val = w.bval.p; s.nC = w.counters.p + 0;
+    s.dHat = dHat; s.kappa = kappa; s.kappa_dev = kappa_ptr(ctx, kappa);
+    s.part = ctx->diag_sum_part.p; s.part_ord = ctx->diag_sum_ord.p; s.out = ctx->diag_sum.p;
+    constraint_summary(s, st);
+    ctx->launches += 3;
+    CK(cudaGetLastError());
+    return out ? ipcgpu_get_constraint_summary(ctx, out) : IPCGPU_OK;
+}
+
+int ipcgpu_get_constraint_summary(ipcgpu_ctx* ctx, ipcgpu_constraint_summary_result* out)
+{
+    REQUIRE(out != nullptr, IPCGPU_ERR_ARG, "null output");
+    REQUIRE(!ctx->capturing, IPCGPU_ERR_STATE, "a capture is in progress");
+    REQUIRE(ctx->diag_sum.n >= 4, IPCGPU_ERR_STATE, "ipcgpu_constraint_summary first");
+    ENTER(kSerial);
+    double v[4];
+    int rc = diag_copy(ctx, v, ctx->diag_sum.p, sizeof(v));
+    if (rc) return rc;
+    out->n = (int)v[0];
+    out->d_min = v[1];
+    out->d_max = v[2];
+    out->fb_norm = v[3];
+    return IPCGPU_OK;
 }
 
 } // extern "C"

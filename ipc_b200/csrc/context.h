@@ -261,6 +261,14 @@ struct ipcgpu_ctx {
     ipcgpu::DevBuf<int4> kp_close_mm;
     ipcgpu::DevBuf<int2> kp_close_hs;
     bool kp_pending = false, kp_pending_at_capture = false;
+    // end-of-step diagnostics (diagnostics.cu): the components of ipcgpu_set_components (n_comp = 0: none; a new mesh removes them) as a
+    // segment table with each component's first segment, the per-segment partials and the results of ipcgpu_system_energy (7 n_comp); the
+    // partials and the result (n, d_min, d_max, |fb|) of ipcgpu_constraint_summary
+    int n_comp = 0, n_seg = 0, comp_v_end = 0;
+    ipcgpu::DevBuf<ipcgpu::DiagSegment> diag_seg;
+    ipcgpu::DevBuf<int> diag_comp_seg;
+    ipcgpu::DevBuf<double> diag_part, diag_sys, diag_sum_part, diag_sum;
+    ipcgpu::DevBuf<unsigned long long> diag_sum_ord;
     size_t ccd_capacity = (size_t)1 << 23; // candidate pairs
     std::vector<int> h_SVI;                // host copy (pSize of the swept build is a serial host sum, SpatialHash.hpp:603-612)
     double debug_prune_seed = -1.0;        // test hook, see ipcgpu_ccd_debug_seed_bound

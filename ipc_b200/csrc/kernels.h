@@ -306,6 +306,39 @@ void timestep_xtilde(const DynamicsArgs& p, cudaStream_t st);
 void timestep_end(const DynamicsArgs& p, cudaStream_t st);
 void timestep_predictor(const DynamicsArgs& p, int option, double* dir, cudaStream_t st); // option 0-4 into dir (interleaved)
 
+// diagnostics.cu -- the end-of-step diagnostics: Optimizer::computeSystemEnergy per component and the constraint summary of the homotopy
+// read-back.  A segment is the part of one component's tet range or vertex range inside one cell of the global chunk grid (kDiagChunk
+// elements); the table lists every component's tet segments, then its vertex segments, in index order, component after component.
+constexpr int kDiagChunk = 2048;
+enum { kSegTets = 0, kSegVertices = 1 };
+struct DiagSegment {
+    int begin, end, kind, pad_;
+};
+struct SystemEnergyArgs {
+    int nV, n_comp, n_seg;
+    const DiagSegment* seg;
+    const int* comp_seg;      // n_comp + 1 starts of each component's segments in `seg`
+    const double* e_per_tet;  // vol psi per tet at the current V (k_elastic_energy)
+    const double* V; const double* Vprev; const double* mass; // SoA, SoA, mass_diag
+    const TimeParams* tp;
+    double* part;             // 7 doubles per segment: E, p (3), V x p (3)
+    double* out;              // sysE (n_comp), sysM (3 n_comp), sysL (3 n_comp)
+};
+void system_energy(const SystemEnergyArgs& p, cudaStream_t st); // 2 launches
+struct SummaryArgs {
+    int nV;
+    const double* V;                         // SoA
+    const double* par; const int2* act; const int* n_act; // planes (nullptrs without planes)
+    const double* val; const int* nC;        // pair_distance of the self / obstacle active entries (k_evaluate_constraints)
+    double dHat, kappa;
+    const double* kappa_dev;                 // nullptr: kappa above; else IterState::kappa
+    double* part;                            // kDiagSummaryBlocks partial sums of fb^2
+    unsigned long long* part_ord;            // 2 kDiagSummaryBlocks: min and max image of d per CTA
+    double* out;                             // n, d_min, d_max, fb_norm
+};
+void constraint_summary(const SummaryArgs& p, cudaStream_t st); // 2 launches
+constexpr int kDiagSummaryBlocks = 264;
+
 // zero n_words 4-byte words.  A kernel rather than cudaMemsetAsync where the two chains of an iteration overlap (abi.h: enter): replayed from a
 // graph, a memset node has no priority of its own and queues behind whatever low-priority grids are pending, which held the step-bound
 // chain up for the length of the CSR assembly

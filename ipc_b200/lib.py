@@ -156,6 +156,11 @@ SIGNATURES = {
     "ipcgpu_kappa_clear_close_set": (C.c_int, [_ctxp]),
     "ipcgpu_kappa_post_line_search": (C.c_int, [_ctxp, C.c_double]),
     "ipcgpu_kappa_info": (C.c_int, [_ctxp, C.c_void_p]),
+    "ipcgpu_set_components": (C.c_int, [_ctxp, C.c_int, _ip, _ip]),
+    "ipcgpu_system_energy": (C.c_int, [_ctxp, _dp, _dp, _dp]),
+    "ipcgpu_get_system_energy": (C.c_int, [_ctxp, _dp, _dp, _dp]),
+    "ipcgpu_constraint_summary": (C.c_int, [_ctxp, C.c_double, C.c_double, C.c_void_p]),
+    "ipcgpu_get_constraint_summary": (C.c_int, [_ctxp, C.c_void_p]),
 }
 # IPCGPU_KAPPA_DEVICE: as a kappa argument, the barrier stiffness held in device memory (Context.set_kappa)
 KAPPA_DEVICE = -1.0
@@ -195,6 +200,11 @@ class KappaInfo(C.Structure):
     """ipcgpu_kappa (include/ipcgpu.h)"""
     _fields_ = [("kappa", C.c_double), ("min_kappa", C.c_double), ("suggest", C.c_double), ("max", C.c_double), ("close_min_dist2", C.c_double),
                 ("doublings", C.c_int), ("n_close", C.c_int), ("needs_init", C.c_int)]
+
+
+class ConstraintSummary(C.Structure):
+    """ipcgpu_constraint_summary_result (include/ipcgpu.h)"""
+    _fields_ = [("n", C.c_int), ("d_min", C.c_double), ("d_max", C.c_double), ("fb_norm", C.c_double)]
 
 
 class SolveResult(C.Structure):
@@ -267,6 +277,7 @@ class Context:
         if rc:
             raise IpcGpuError(f"ipcgpu_create(device={device}) failed with {ERR_NAMES.get(rc, rc)}: a CUDA device is required (no CPU fallback)")
         self.nV = self.nT = self.nnz = 0
+        self.n_components = 0
         self._keep = []
 
     def close(self):
@@ -823,6 +834,44 @@ class Context:
     def kappa_info(self):
         out = KappaInfo()
         self._ck(self.lib.ipcgpu_kappa_info(self.h, C.byref(out)))
+        return out
+
+    # ---- end-of-step diagnostics (computeSystemEnergy, the constraint summary after solveSub_IP) ----------------------------------
+    def set_components(self, vertex_end, tet_end):
+        """the cumulative compVAccSize / compFAccSize: one entry per component, in order"""
+        ve, te = i32(np.asarray(vertex_end).ravel()), i32(np.asarray(tet_end).ravel())
+        if ve.size != te.size:
+            raise ValueError("vertex_end and tet_end must have one entry per component")
+        self._ck(self.lib.ipcgpu_set_components(self.h, int(ve.size), _i(ve), _i(te)))
+        self.n_components = int(ve.size)
+
+    def _system_energy_arrays(self):
+        n = self.n_components
+        return np.empty(n), np.empty((n, 3)), np.empty((n, 3))
+
+    def system_energy(self, want=True):
+        """(sysE (n,), sysM (n, 3), sysL (n, 3)); want=False: deferred and capturable (get_system_energy reads it)"""
+        if not want:
+            self._ck(self.lib.ipcgpu_system_energy(self.h, None, None, None))
+            return None
+        E, Mo, Lo = self._system_energy_arrays()
+        self._ck(self.lib.ipcgpu_system_energy(self.h, _d(E), _d(Mo), _d(Lo)))
+        return E, Mo, Lo
+
+    def get_system_energy(self):
+        E, Mo, Lo = self._system_energy_arrays()
+        self._ck(self.lib.ipcgpu_get_system_energy(self.h, _d(E), _d(Mo), _d(Lo)))
+        return E, Mo, Lo
+
+    def constraint_summary(self, dHat, kappa, want=True):
+        """ConstraintSummary (n, d_min, d_max, fb_norm); want=False: deferred and capturable (get_constraint_summary reads it)"""
+        out = ConstraintSummary()
+        self._ck(self.lib.ipcgpu_constraint_summary(self.h, float(dHat), float(kappa), C.byref(out) if want else None))
+        return out if want else None
+
+    def get_constraint_summary(self):
+        out = ConstraintSummary()
+        self._ck(self.lib.ipcgpu_get_constraint_summary(self.h, C.byref(out)))
         return out
 
     def hash_build_swept(self, p, alpha, h):
