@@ -144,8 +144,8 @@ int ipcgpu_step_bound_set(ipcgpu_ctx* ctx, double alpha);
  * list sizes and step bounds -- they live in device memory and are read at replay time.  So one capture serves every Newton iteration
  * of a solve; capture again after ipcgpu_set_mesh / _set_surface / _set_csr / _set_*_capacity / _comm_init / _set_canonical_order /
  * _set_contact_partition (older graphs are refused with IPCGPU_ERR_STATE) or when dHat / a host kappa change (IPCGPU_KAPPA_DEVICE is read at replay).  Run the sequence once eagerly
- * before capturing it (lazy allocations), with ipcgpu_set_canonical_order(ctx, 0): the canonical sort of the contact lists needs their sizes
- * on the host.  Collective: with several ranks every rank captures and launches the same sequence.
+ * before capturing it (lazy allocations), with ipcgpu_set_canonical_order(ctx, 0) or (ctx, 2): the level-1 sort of the contact lists needs
+ * their sizes on the host.  Collective: with several ranks every rank captures and launches the same sequence.
  * ipcgpu_fetch_iteration stays outside the graph. */
 int ipcgpu_capture_begin(ipcgpu_ctx* ctx);
 int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id);
@@ -236,10 +236,18 @@ int ipcgpu_set_exchange_capacity(ipcgpu_ctx* ctx, int pairs_per_rank);
 int ipcgpu_constraint_set(ipcgpu_ctx* ctx, double dHat, int getPTEE, int* nC, int* nPara, int* nCand);
 /* sizes of the last set (synchronises if it was built with NULL size pointers) */
 int ipcgpu_constraint_set_sizes(ipcgpu_ctx* ctx, int* nC, int* nPara, int* nCand);
-/* enable=1 (default): the lists are returned in canonical (lexicographic) order, so two runs give bitwise identical sets and sums.
- * enable=0: the order is whatever the atomic appends produced -- the same freedom the reference has (its order depends on
- * unordered_set iteration and TBB scheduling); saves the sorting passes when the sets are only consumed on the device. */
-int ipcgpu_set_canonical_order(ipcgpu_ctx* ctx, int enable);
+/* Order of the contact lists and of the contact sums.
+ * level=1 (default): the lists are returned in canonical (lexicographic) order, so two runs give bitwise identical sets.  The sorts are
+ *   sized on the host: refused inside a capture.
+ * level=0: the order is whatever the atomic appends produced -- the same freedom the reference has (its order depends on
+ *   unordered_set iteration and TBB scheduling); saves the sorting passes when the sets are only consumed on the device.
+ * level=2 (reproducible mode): the canonical order of level 1 from device-sized sorts wherever a list is produced (the constraint set,
+ *   ipcgpu_set_constraint_set, ipcgpu_friction_lag, ipcgpu_set_friction_data), inside a capture as well, and every contact term (barrier,
+ *   mollified, Jacobian^T, friction, planes; E, g and H) summed in an order fixed by the lists alone, with no floating-point atomic on g or
+ *   the CSR values: a captured time step gives the same bits on every run and for every order the lists were handed in.  Lists built
+ *   before the switch keep their order until they are built again.  One rank only (IPCGPU_ERR_STATE otherwise); a pair capacity of at
+ *   most 2^27.  Every level change refuses older graphs. */
+int ipcgpu_set_canonical_order(ipcgpu_ctx* ctx, int level);
 /* Multi-rank only. enable=1: ipcgpu_constraint_set issues only this rank's share of the PT/EE queries, so every rank holds a disjoint
  * part of the sets (PP/PE multiplicities may be split between ranks, which leaves the summed E/g/H unchanged because
  * makePD(c*M) = c*makePD(M) for c > 0); the counts returned are local.  enable=0 (default): every rank builds the whole set

@@ -160,6 +160,14 @@ ipcgpu::SurfArgs surf_args(const ipcgpu_ctx* ctx);
 ipcgpu::BarrierArgs barrier_args(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC); // (api_contact.cu; kappa may be IPCGPU_KAPPA_DEVICE)
 ipcgpu::HalfSpaceArgs halfspace_args(ipcgpu_ctx* ctx);                                      // (api_terms.cu)
 ipcgpu::SortedGrid edge_grid(const ipcgpu_ctx* ctx);
+
+// ---- repro.cu: the reproducible mode (canonical order level 2) -----------------------------------------------------------------------
+int repro_alloc(ipcgpu_ctx* ctx);                        // its workspace, sized by the pair capacity and the mesh (outside a capture)
+bool repro_on(const ipcgpu_ctx* ctx);                    // level 2 on one rank, workspace allocated
+int repro_contact_lists(ipcgpu_ctx* ctx);                // act / para in canonical order (device-sized), their gather indices
+int repro_friction_list(ipcgpu_ctx* ctx, bool sort);     // fr_cs (+ companions) in canonical order if `sort`, its gather indices
+ipcgpu::ReproArgs repro_barrier_args(ipcgpu_ctx* ctx);   // on = 0 unless the indices belong to the lists in act / para
+ipcgpu::ReproArgs repro_friction_args(ipcgpu_ctx* ctx);  // ... to the list in fr_cs
 int boxes_and_grid(ipcgpu_ctx* ctx, double radius, bool with_vertex_boxes);
 
 // ---- ccd.cu -----------------------------------------------------------------------------------------------------------------

@@ -97,6 +97,7 @@ int ipcgpu_comm_init(ipcgpu_ctx* ctx, int rank, int nranks, const void* id128)
     ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
     REQUIRE(nranks >= 1 && rank >= 0 && rank < nranks, IPCGPU_ERR_ARG, "bad rank/nranks");
+    REQUIRE(nranks == 1 || ctx->canonical_order != 2, IPCGPU_ERR_STATE, "the reproducible mode (canonical order level 2) runs on one rank");
     ctx->rank = rank;
     ctx->nranks = nranks;
     if (nranks > 1) {

@@ -250,11 +250,16 @@ int ipcgpu_constraint_set(ipcgpu_ctx* ctx, double dHat, int getPTEE, int* nC, in
     return rc;
 }
 
-int ipcgpu_set_canonical_order(ipcgpu_ctx* ctx, int enable)
+int ipcgpu_set_canonical_order(ipcgpu_ctx* ctx, int level)
 {
+    REQUIRE(level >= 0 && level <= 2, IPCGPU_ERR_ARG, "ipcgpu_set_canonical_order: level 0, 1 or 2");
+    REQUIRE(level != 2 || ctx->nranks == 1, IPCGPU_ERR_STATE, "the reproducible mode (level 2) runs on one rank");
     ENTER(kSerial);
     ++ctx->epoch; // graphs captured before this call are refused (buffers, partition or list order may change)
-    ctx->canonical_order = enable != 0;
+    ctx->canonical_order = level;
+    // the lists held now keep the order they were built in: the fixed-order sums start with the next lists built at level 2
+    ctx->rw.lists_ready = ctx->rw.fr_ready = false;
+    if (level == 2 && ctx->surface_ready) return repro_alloc(ctx);
     return IPCGPU_OK;
 }
 
@@ -317,6 +322,11 @@ int ipcgpu_set_constraint_set(ipcgpu_ctx* ctx, int nC, const int* mm, int nP, co
     w.want_cand = nK > 0;
     ctx->lists_local = false; // uploaded sets are the global ones
     w.lists_global = false;
+    ctx->rw.lists_ready = false;
+    if (repro_on(ctx)) {
+        int rc = repro_contact_lists(ctx);
+        if (rc) return rc;
+    }
     ctx->mark_inputs();
     return IPCGPU_OK;
 }
@@ -343,6 +353,7 @@ BarrierArgs barrier_args(ipcgpu_ctx* ctx, double dHat, double kappa, int project
     p.dHat = dHat; p.kappa = kappa; p.projectDBC = projectDBC;
     p.ia = ctx->ia.p; p.ja = ctx->ja.p; p.base = ctx->index_base;
     p.kappa_dev = kappa_ptr(ctx, kappa);
+    p.rep = repro_barrier_args(ctx);
     return p;
 }
 
@@ -426,7 +437,10 @@ int ipcgpu_barrier_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
     REQUIRE(ctx->surface_ready, IPCGPU_ERR_STATE, "ipcgpu_set_surface first");
     REQUIRE_KAPPA(kappa);
     const BarrierArgs p = barrier_args(ctx, dHat, kappa, 0);
-    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { barrier_gradient(p, ctx->g.p, st); });
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) {
+        barrier_gradient(p, ctx->g.p, st);
+        ctx->launches += p.rep.on; // (the reproducible mode's gather)
+    });
 }
 
 int ipcgpu_evaluate_constraints(ipcgpu_ctx* ctx, double* val, int n)
@@ -469,7 +483,7 @@ int ipcgpu_constraint_jacobian_t(ipcgpu_ctx* ctx, const double* input, int n, do
     BarrierArgs p = barrier_args(ctx, 1.0, 1.0, 0);
     p.cs = w.act.p; p.nC = w.counters.p + 0;
     constraint_jacobian_t(p, w.bval.p, coef, ctx->g.p, ctx->stream);
-    ++ctx->launches;
+    ctx->launches += 1 + p.rep.on;
     CK(cudaGetLastError());
     return gradient_roundtrip_end(ctx, g_inout);
 }
@@ -482,8 +496,9 @@ int ipcgpu_para_ee_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double* 
     ENTER(kSerial);
     int rc = gradient_roundtrip_begin(ctx, g_inout);
     if (rc) return rc;
-    para_gradient(barrier_args(ctx, dHat, kappa, 0), ctx->g.p, ctx->stream);
-    ++ctx->launches;
+    const BarrierArgs p = barrier_args(ctx, dHat, kappa, 0);
+    para_gradient(p, ctx->g.p, ctx->stream);
+    ctx->launches += 1 + p.rep.on;
     CK(cudaGetLastError());
     return gradient_roundtrip_end(ctx, g_inout);
 }
@@ -556,6 +571,8 @@ int ipcgpu_friction_lag(ipcgpu_ctx* ctx, double dHat, double kappa, int* n_pairs
     CK(cudaGetLastError());
     w.fr_ready = true;
     w.fr_host_n = -1;
+    ctx->rw.fr_ready = false;
+    if (repro_on(ctx) && (rc = repro_friction_list(ctx, !ctx->rw.lists_ready))) return rc; // (a copy of the active list: sorted already at level 2)
     if (n_pairs) {
         CK(cudaMemcpyAsync(&ctx->staging->count, w.fr_n.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
@@ -613,6 +630,8 @@ int ipcgpu_set_friction_data(ipcgpu_ctx* ctx, int n_pairs, const int* mmcvid4, c
     CK(cudaStreamSynchronize(ctx->stream)); // n_pairs lives on the caller's stack
     w.fr_host_n = n_pairs;
     w.fr_ready = true;
+    ctx->rw.fr_ready = false;
+    if (repro_on(ctx)) return repro_friction_list(ctx, true);
     return IPCGPU_OK;
 }
 
@@ -627,6 +646,7 @@ static FrictionArgs friction_args(ipcgpu_ctx* ctx, double eps2, double coef, int
     p.rank = ctx->rank; p.nranks = ctx->nranks;
     p.row_lo = ctx->nranks > 1 ? ctx->v_begin : 0;
     p.row_hi = ctx->nranks > 1 ? ctx->v_end : ctx->nV;
+    p.rep = repro_friction_args(ctx);
     return p;
 }
 #define REQUIRE_FRICTION() \
@@ -648,7 +668,10 @@ int ipcgpu_friction_gradient(ipcgpu_ctx* ctx, double eps2, double coef, double* 
     REQUIRE_FRICTION();
     REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive");
     const FrictionArgs p = friction_args(ctx, eps2, coef, 0);
-    return gradient_call(ctx, kSerial, g_inout, [&](cudaStream_t st) { friction_gradient(p, ctx->g.p, st); });
+    return gradient_call(ctx, kSerial, g_inout, [&](cudaStream_t st) {
+        friction_gradient(p, ctx->g.p, st);
+        ctx->launches += p.rep.on;
+    });
 }
 
 int ipcgpu_friction_hessian(ipcgpu_ctx* ctx, double eps2, double coef, int projectDBC, double* a_inout)
@@ -657,7 +680,10 @@ int ipcgpu_friction_hessian(ipcgpu_ctx* ctx, double eps2, double coef, int proje
     REQUIRE(eps2 > 0.0, IPCGPU_ERR_ARG, "fricDHat must be positive");
     const FrictionArgs p = friction_args(ctx, eps2, coef, projectDBC);
     return hessian_call(ctx, kSerial, a_inout, 1u << FLAG_PATTERN,
-        [&](cudaStream_t st) { friction_hessian(p, ctx->a.p, ctx->iter.p->flags + FLAG_PATTERN, st); });
+        [&](cudaStream_t st) {
+            friction_hessian(p, ctx->a.p, ctx->iter.p->flags + FLAG_PATTERN, st);
+            ctx->launches += p.rep.on;
+        });
 }
 
 } // extern "C"

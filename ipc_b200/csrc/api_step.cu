@@ -56,6 +56,8 @@ static ipcgpu_ctx::HostState snapshot_host_state(const ipcgpu_ctx* ctx)
     h.nC = ctx->cw.nC; h.nP = ctx->cw.nP; h.nK = ctx->cw.nK; h.fr_host_n = ctx->cw.fr_host_n;
     h.hs_set_built = ctx->hs_set_built;
     h.hs_lag_ready = ctx->hs_lag_ready;
+    h.rep_lists = ctx->rw.lists_ready;
+    h.rep_fr = ctx->rw.fr_ready;
     return h;
 }
 static void apply_host_state(ipcgpu_ctx* ctx, const ipcgpu_ctx::HostState& h)
@@ -71,6 +73,8 @@ static void apply_host_state(ipcgpu_ctx* ctx, const ipcgpu_ctx::HostState& h)
     ctx->cw.nC = h.nC; ctx->cw.nP = h.nP; ctx->cw.nK = h.nK; ctx->cw.fr_host_n = h.fr_host_n;
     ctx->hs_set_built = h.hs_set_built;
     ctx->hs_lag_ready = h.hs_lag_ready;
+    ctx->rw.lists_ready = h.rep_lists;
+    ctx->rw.fr_ready = h.rep_fr;
 }
 
 int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
@@ -442,7 +446,7 @@ int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* t, doubl
     REQUIRE(ctx->n_hs == 0 || ctx->hs_set_built, IPCGPU_ERR_STATE, "half-spaces: ipcgpu_halfspace_constraint_set first (E0 takes the sets held on entry)");
     REQUIRE(!(ls_terms(ctx, *t) & kTermHalfSpaceFriction) || ctx->prev_set, IPCGPU_ERR_STATE, "half-space friction: ipcgpu_set_prev_state first");
     REQUIRE(!ctx->damp_on || ctx->prev_set, IPCGPU_ERR_STATE, "damping: ipcgpu_set_prev_state first");
-    REQUIRE(!(ctx->capturing && ctx->canonical_order), IPCGPU_ERR_STATE, "inside a capture the line search needs ipcgpu_set_canonical_order(ctx, 0)");
+    REQUIRE(!(ctx->capturing && ctx->canonical_order == 1), IPCGPU_ERR_STATE, "inside a capture the line search needs ipcgpu_set_canonical_order(ctx, 0) or (ctx, 2)");
     ENTER(kSerial);
     int rc = step_control_prepare(ctx);
     if (rc) return rc;

@@ -461,6 +461,11 @@ HalfSpaceArgs halfspace_args(ipcgpu_ctx* ctx)
     p.row_lo = ctx->nranks > 1 ? ctx->v_begin : 0;
     p.row_hi = ctx->nranks > 1 ? ctx->v_end : ctx->nV;
     p.ia = ctx->ia.p; p.base = ctx->index_base;
+    if (repro_on(ctx) && ctx->rw.nV >= ctx->nV && ctx->rw.nSV >= ctx->nSV) { // the reproducible mode: every vertex adds its planes in plane order
+        p.rep_mask = ctx->rw.hs_mask.p;
+        p.rep_pos = ctx->rw.hs_pos.p;
+        p.rep_stage = ctx->rw.hs_stage.p;
+    }
     return p;
 }
 
@@ -576,7 +581,10 @@ int ipcgpu_halfspace_gradient(ipcgpu_ctx* ctx, double dHat, double kappa, double
     REQUIRE_KAPPA(kappa);
     const HalfSpaceArgs p = halfspace_args(ctx);
     const double* kd = kappa_ptr(ctx, kappa);
-    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { halfspace_gradient(p, dHat, kappa, kd, ctx->g.p, st); });
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) {
+        halfspace_gradient(p, dHat, kappa, kd, ctx->g.p, st);
+        ctx->launches += p.rep_mask != nullptr; // (the reproducible mode's per-vertex add)
+    });
 }
 
 int ipcgpu_halfspace_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int projectDBC, double* a_inout)
@@ -586,7 +594,10 @@ int ipcgpu_halfspace_hessian(ipcgpu_ctx* ctx, double dHat, double kappa, int pro
     REQUIRE_KAPPA(kappa);
     const HalfSpaceArgs p = halfspace_args(ctx);
     const double* kd = kappa_ptr(ctx, kappa);
-    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) { halfspace_hessian(p, dHat, kappa, kd, projectDBC, ctx->a.p, st); });
+    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) {
+        halfspace_hessian(p, dHat, kappa, kd, projectDBC, ctx->a.p, st);
+        ctx->launches += p.rep_mask != nullptr;
+    });
 }
 
 int ipcgpu_halfspace_step(ipcgpu_ctx* ctx, const double* p_dir, double slackness, double* alpha_inout)
@@ -667,7 +678,10 @@ int ipcgpu_halfspace_friction_gradient(ipcgpu_ctx* ctx, double eps2, double* g_i
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_LAG();
     const HalfSpaceArgs p = halfspace_args(ctx);
-    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) { halfspace_friction_gradient(p, eps2, ctx->g.p, st); });
+    return gradient_call(ctx, kDerivative, g_inout, [&](cudaStream_t st) {
+        halfspace_friction_gradient(p, eps2, ctx->g.p, st);
+        ctx->launches += p.rep_mask != nullptr;
+    });
 }
 
 int ipcgpu_halfspace_friction_hessian(ipcgpu_ctx* ctx, double eps2, int projectDBC, double* a_inout)
@@ -675,7 +689,10 @@ int ipcgpu_halfspace_friction_hessian(ipcgpu_ctx* ctx, double eps2, int projectD
     if (ctx->n_hs == 0) return IPCGPU_OK;
     REQUIRE_HS_LAG();
     const HalfSpaceArgs p = halfspace_args(ctx);
-    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) { halfspace_friction_hessian(p, eps2, projectDBC, ctx->a.p, st); });
+    return hessian_call(ctx, kDerivative, a_inout, 0, [&](cudaStream_t st) {
+        halfspace_friction_hessian(p, eps2, projectDBC, ctx->a.p, st);
+        ctx->launches += p.rep_mask != nullptr;
+    });
 }
 
 int ipcgpu_get_halfspace_sets(ipcgpu_ctx* ctx, int* n_active, int* active2, int* n_lagged, int* lagged2, double* lambda)

@@ -10,8 +10,7 @@
 //    access of a warp is conflict-free even though p,q are data dependent per sweep position only;
 //  * gradients and CSR values are accumulated with FP64 red.global.add (pair counts are orders of magnitude below the
 //    tet count; the elastic path stays deterministic, the barrier scatter is order-free to ~1 ulp of the sum).
-#include "pair_common.cuh"
-#include "kernels.h"
+#include "repro.cuh"
 #include <algorithm>
 
 namespace ipcgpu {
@@ -59,15 +58,6 @@ __device__ inline double mollifier(const V3* ex, double eps_x, double* eg, bool 
         diff_to_vertices(C, 3, 4, false, true, [](int, double) {}, [&](int i, int j, double v) { puth(i, j, v * qg + (qH * cg[i]) * cg[j]); });
     const double r = C.val / eps_x;
     return (-r + 2.0) * r;
-}
-
-DEV void para_edge_stencil(int4 mm, int2 e, const int* __restrict__ SE, int* ev)
-{
-    if (mm.w >= 0 && mm.x >= 0) { ev[0] = mm.x; ev[1] = mm.y; ev[2] = mm.z; ev[3] = mm.w; }
-    else {
-        ev[0] = SE[2 * e.x]; ev[1] = SE[2 * e.x + 1];
-        ev[2] = SE[2 * e.y]; ev[3] = SE[2 * e.y + 1];
-    }
 }
 
 // The list sizes live on the device (the constraint set is built there and nothing is read back inside an iteration), so every
@@ -132,9 +122,20 @@ __global__ void __launch_bounds__(256) k_barrier_energy(BarrierArgs p, double* _
 template <bool kDevKappa>
 DEV double barrier_kappa(const BarrierArgs& p) { return kDevKappa ? *p.kappa_dev : p.kappa; }
 
-template <bool kDevKappa>
+// kStage (reproducible mode): contribution k of a pair goes to its own slot g[3 key + q] of the staging array (ReproArgs: key 4c + k for
+// active entry c; 4 cap + 8c + k for the edge stencil and 4 cap + 8c + 4 + k for the distance stencil of mollified entry c) instead of being
+// added at its vertex; k_repro_gather_g sums them
+template <bool kStage>
+DEV void put_g(double* __restrict__ g, int v, unsigned long long key, int q, double val)
+{
+    if (kStage) g[3 * key + q] = val;
+    else atomicAdd(g + 3 * (size_t)v + q, val);
+}
+
+template <bool kDevKappa, bool kStage>
 __global__ void __launch_bounds__(128) k_barrier_gradient(BarrierArgs p, double* __restrict__ g)
 {
+    const unsigned long long para0 = 4ull * p.rep.cap;
     const ListRange lr = list_range(p, false);
     const int nA = lr.ce - lr.cb, n = nA + (lr.pe - lr.pb);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -158,11 +159,12 @@ __global__ void __launch_bounds__(128) k_barrier_gradient(BarrierArgs p, double*
         double eg[12];
         const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, false, [](int, int, double) {});
         for (int k = 0; k < 4; ++k)
-            for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)ev[k] + q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
+            for (int q = 0; q < 3; ++q) put_g<kStage>(g, ev[k], para0 + 8ull * c + k, q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
         w = barrier_kappa<kDevKappa>(p) * e * db; // slot 3 is -1 (or a vertex id): multiplicity 1
     }
+    const unsigned long long key0 = is_para ? para0 + 8ull * c + 4 : 4ull * c;
     for (int k = 0; k < s.nv; ++k)
-        for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)s.v[k] + q, w * gd[3 * k + q]);
+        for (int q = 0; q < 3; ++q) put_g<kStage>(g, s.v[k], key0 + k, q, w * gd[3 * k + q]);
     }
 }
 
@@ -181,6 +183,7 @@ __global__ void __launch_bounds__(256) k_evaluate_constraints(BarrierArgs p, dou
         val[c] = pair_distance(s, x);
     }
 }
+template <bool kStage>
 __global__ void __launch_bounds__(128) k_constraint_jacobian_t(BarrierArgs p, const double* __restrict__ input, double coef, double* __restrict__ g)
 {
     const ListRange lr = list_range(p, false);
@@ -192,13 +195,14 @@ __global__ void __launch_bounds__(128) k_constraint_jacobian_t(BarrierArgs p, co
         pair_derivs(s, x, gd, false, [](int, int, double) {});
         const double w = coef * s.mult * input[c];
         for (int k = 0; k < s.nv; ++k)
-            for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)s.v[k] + q, w * gd[3 * k + q]);
+            for (int q = 0; q < 3; ++q) put_g<kStage>(g, s.v[k], 4ull * c + k, q, w * gd[3 * k + q]);
     }
 }
 // augmentParaEEGradient (:2990-3045) alone: the mollified pairs' share of k_barrier_gradient
-template <bool kDevKappa>
+template <bool kDevKappa, bool kStage>
 __global__ void __launch_bounds__(128) k_para_gradient(BarrierArgs p, double* __restrict__ g)
 {
+    const unsigned long long para0 = 4ull * p.rep.cap;
     const ListRange lr = list_range(p, false);
     for (int c = lr.pb + blockIdx.x * blockDim.x + threadIdx.x; c < lr.pe; c += gridDim.x * blockDim.x) {
         const int4 mm = p.para[c];
@@ -216,10 +220,10 @@ __global__ void __launch_bounds__(128) k_para_gradient(BarrierArgs p, double* __
         double eg[12];
         const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, false, [](int, int, double) {});
         for (int k = 0; k < 4; ++k)
-            for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)ev[k] + q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
+            for (int q = 0; q < 3; ++q) put_g<kStage>(g, ev[k], para0 + 8ull * c + k, q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
         const double w = barrier_kappa<kDevKappa>(p) * e * db;
         for (int k = 0; k < s.nv; ++k)
-            for (int q = 0; q < 3; ++q) atomicAdd(g + 3 * (size_t)s.v[k] + q, w * gd[3 * k + q]);
+            for (int q = 0; q < 3; ++q) put_g<kStage>(g, s.v[k], para0 + 8ull * c + 4 + k, q, w * gd[3 * k + q]);
     }
 }
 
@@ -231,11 +235,14 @@ __global__ void __launch_bounds__(128) k_para_gradient(BarrierArgs p, double* __
 // -----------------------------------------------------------------------------------------------------------
 DEV bool owns_row(const BarrierArgs& p, int v) { return v >= p.row_lo && v < p.row_hi; }
 
-template <bool kDevKappa>
+// kFixedSlot (reproducible mode, one rank): the pair of list position c (active, then mollified) keeps slot c, so that the slot order is the
+// list order; *n_owned = the number of pairs
+template <bool kDevKappa, bool kFixedSlot>
 __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, double* __restrict__ Hraw, int* __restrict__ rows_out, int* __restrict__ n_owned,
     int capacity, int* __restrict__ flags)
 {
     const int nC = *p.nC, nTot = nC + *p.nP;
+    if (kFixedSlot && blockIdx.x == 0 && threadIdx.x == 0) *n_owned = min(nTot, capacity);
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < nTot; c += gridDim.x * blockDim.x) {
     // the matrix is assembled in thread-local memory (interleaved across the warp by the hardware: every access is one coalesced
     // transaction) and shipped to its pair-major slot once at the end; read-modify-write straight on the 1152-byte-strided slots
@@ -303,8 +310,8 @@ __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, dou
                 HE(i, j) = ((k * db) * gd[i]) * eg[j] + ((k * db) * gd[j]) * eg[i] + (k * b) * HE(i, j) + ((k * e * d2b) * gd[i]) * gd[j] + (k * e * db) * VE[i * 12 + j];
     }
     // compacted output slot (one atomic per warp iteration)
-    int slot;
-    {
+    int slot = c;
+    if (!kFixedSlot) {
         const unsigned m = __activemask();
         const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
         int base = 0;
@@ -582,6 +589,32 @@ __global__ void __launch_bounds__(32 * kScatWarps) k_barrier_hessian_scatter(Bar
     }
 }
 
+// reproducible mode: the scatter above as a per-row gather (repro.cuh), one thread per row vertex; slot c holds list entry c
+__global__ void __launch_bounds__(128) k_barrier_hessian_gather(BarrierArgs p, const int* __restrict__ n_ptr, int capacity, const double* __restrict__ H,
+    const int* __restrict__ psd, double* __restrict__ a, int* __restrict__ err)
+{
+    const int n = min(*n_ptr, capacity);
+    for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < p.nV; v += gridDim.x * blockDim.x)
+        repro_gather_row(v, p.rep.h, p.dbc, p.projectDBC, p.ia, p.ja, p.base, a, err, [&](int c, int bi, int bj, double* acc) {
+            if (c >= n) return;
+            const double* H0 = H + (size_t)c * 144;
+            if (psd[c] != 0) {
+                for (int r = 0; r < 3; ++r)
+                    for (int q = 0; q < 3; ++q) acc[3 * r + q] += H0[(3 * bi + r) * 12 + 3 * bj + q];
+                return;
+            }
+            for (int r = 0; r < 3; ++r)
+                for (int q = 0; q < 3; ++q) {
+                    double t = 0.0;
+                    for (int ka = 0; ka < 3; ++ka) {
+                        const double qa = helmert(ka, bi);
+                        for (int kb = 0; kb < 3; ++kb) t += (qa * helmert(kb, bj)) * H0[(3 * ka + r) * 9 + 3 * kb + q];
+                    }
+                    acc[3 * r + q] += t;
+                }
+        });
+}
+
 // -----------------------------------------------------------------------------------------------------------
 void barrier_energy(const BarrierArgs& p, double* partials, int* bad, cudaStream_t st)
 {
@@ -590,26 +623,48 @@ void barrier_energy(const BarrierArgs& p, double* partials, int* bad, cudaStream
 int barrier_energy_blocks() { return kBarrierEnergyBlocks; }
 void barrier_gradient(const BarrierArgs& p, double* g, cudaStream_t st)
 {
-    if (p.kappa_dev) k_barrier_gradient<true><<<kSMs * 4, 128, 0, st>>>(p, g);
-    else k_barrier_gradient<false><<<kSMs * 4, 128, 0, st>>>(p, g);
+    if (p.rep.on) {
+        if (p.kappa_dev) k_barrier_gradient<true, true><<<kSMs * 4, 128, 0, st>>>(p, p.rep.stage);
+        else k_barrier_gradient<false, true><<<kSMs * 4, 128, 0, st>>>(p, p.rep.stage);
+        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 0ull, ~0ull, g, st);
+    }
+    else if (p.kappa_dev) k_barrier_gradient<true, false><<<kSMs * 4, 128, 0, st>>>(p, g);
+    else k_barrier_gradient<false, false><<<kSMs * 4, 128, 0, st>>>(p, g);
 }
 void evaluate_constraints(const BarrierArgs& p, double* val, cudaStream_t st) { k_evaluate_constraints<<<kSMs * 2, 256, 0, st>>>(p, val); }
-void constraint_jacobian_t(const BarrierArgs& p, const double* input, double coef, double* g, cudaStream_t st) { k_constraint_jacobian_t<<<kSMs * 4, 128, 0, st>>>(p, input, coef, g); }
+void constraint_jacobian_t(const BarrierArgs& p, const double* input, double coef, double* g, cudaStream_t st)
+{
+    if (p.rep.on) {
+        k_constraint_jacobian_t<true><<<kSMs * 4, 128, 0, st>>>(p, input, coef, p.rep.stage);
+        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 0ull, 4ull * p.rep.cap, g, st); // the active list's contributions
+    }
+    else k_constraint_jacobian_t<false><<<kSMs * 4, 128, 0, st>>>(p, input, coef, g);
+}
 void para_gradient(const BarrierArgs& p, double* g, cudaStream_t st)
 {
-    if (p.kappa_dev) k_para_gradient<true><<<kSMs, 128, 0, st>>>(p, g);
-    else k_para_gradient<false><<<kSMs, 128, 0, st>>>(p, g);
+    if (p.rep.on) {
+        if (p.kappa_dev) k_para_gradient<true, true><<<kSMs, 128, 0, st>>>(p, p.rep.stage);
+        else k_para_gradient<false, true><<<kSMs, 128, 0, st>>>(p, p.rep.stage);
+        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 4ull * p.rep.cap, ~0ull, g, st); // the mollified list's contributions
+    }
+    else if (p.kappa_dev) k_para_gradient<true, false><<<kSMs, 128, 0, st>>>(p, g);
+    else k_para_gradient<false, false><<<kSMs, 128, 0, st>>>(p, g);
 }
 void barrier_hessian_build_project(const BarrierArgs& p, int* flags, double* Hraw, int* rows, int* psd, int* n_owned, int capacity, cudaStream_t st)
 {
     cudaMemsetAsync(n_owned, 0, sizeof(int), st);
-    if (p.kappa_dev) k_barrier_hessian_build<true><<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
-    else k_barrier_hessian_build<false><<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
+    if (p.rep.on) {
+        if (p.kappa_dev) k_barrier_hessian_build<true, true><<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
+        else k_barrier_hessian_build<false, true><<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
+    }
+    else if (p.kappa_dev) k_barrier_hessian_build<true, false><<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
+    else k_barrier_hessian_build<false, false><<<kSMs * 8, 64, 0, st>>>(p, Hraw, rows, n_owned, capacity, flags);
     k_barrier_hessian_project<<<kSMs * 4, 32 * kProjWarps, 0, st>>>(n_owned, capacity, Hraw, psd);
 }
 void barrier_hessian_scatter(const BarrierArgs& p, double* a, int* flags, const double* Hraw, const int* rows, const int* psd, const int* n_owned, int capacity, cudaStream_t st)
 {
-    k_barrier_hessian_scatter<<<kSMs * 4, 32 * kScatWarps, 0, st>>>(p, n_owned, capacity, Hraw, rows, psd, a, flags + FLAG_PATTERN);
+    if (p.rep.on) k_barrier_hessian_gather<<<kSMs * 4, 128, 0, st>>>(p, n_owned, capacity, Hraw, psd, a, flags + FLAG_PATTERN);
+    else k_barrier_hessian_scatter<<<kSMs * 4, 32 * kScatWarps, 0, st>>>(p, n_owned, capacity, Hraw, rows, psd, a, flags + FLAG_PATTERN);
 }
 
 } // namespace ipcgpu

@@ -812,6 +812,7 @@ int contact_alloc(ipcgpu_ctx* ctx)
         return IPCGPU_ERR_CUDA;
     }
     w.cap = cap;
+    if (ctx->canonical_order == 2) return repro_alloc(ctx);
     return 0;
 }
 
@@ -968,7 +969,7 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
     }
     w.want_cand = wantCand != 0;
     w.nC = w.nP = w.nK = -1; // unknown on the host until somebody asks
-    const bool need_host = !hashed_merge || ctx->canonical_order || nC || nPara || nCand;
+    const bool need_host = !hashed_merge || ctx->canonical_order == 1 || nC || nPara || nCand;
     if (need_host) {
         int* h = ctx->staging->contact;
         if (!hashed_merge) { // huge meshes: sort-based merge, sized on the host
@@ -982,12 +983,15 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
             }
         }
         if ((rc = contact_sync_counts(ctx))) return rc;
-        if (ctx->canonical_order) { // deterministic output order (the reference's own order is scheduling dependent, :2176, :2282)
+        if (ctx->canonical_order == 1) { // deterministic output order (the reference's own order is scheduling dependent, :2176, :2282)
             if ((rc = sort_lex(ctx, w.act.p, nullptr, w.nC, w.tmp4.p, nullptr))) return rc;
             if ((rc = sort_lex(ctx, w.para.p, w.para_e.p, w.nP, w.tmp4.p, w.tmp2.p))) return rc;
             if (wantCand && (rc = sort_int2(ctx, w.cand.p, w.nK, w.tmp2.p))) return rc;
         }
     }
+    // the reproducible mode: the same order from device-sized sorts (also inside a capture), and the gather indices of the contact sums
+    ctx->rw.lists_ready = false;
+    if (repro_on(ctx) && (rc = repro_contact_lists(ctx))) return rc;
     k_publish_counts<<<1, 32, 0, st>>>(w.counters.p, wantCand, ctx->iter.p);
     ++ctx->launches;
     ctx->prof_end(pe);

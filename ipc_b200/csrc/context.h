@@ -81,6 +81,25 @@ struct ContactWork {
     bool fr_ready = false;
 };
 
+// reproducible mode (ipcgpu_set_canonical_order(ctx, 2), repro.cu), allocated when the level is selected: the scratch of the device-sized
+// lexicographic sort and of the index builds (bucket counts / offsets over 2 nV + 1 buckets, the permutation, a word buffer for the
+// permuted companions), the per-vertex gather indices of the barrier (bg / bh) and friction (fg / fh) gradients and Hessians with their
+// staging, and the plane terms' per-vertex masks, positions and staging.  lists_ready / fr_ready: the indices belong to the lists in act /
+// para and fr_cs (built where the lists were produced at level 2)
+struct ReproWork {
+    DevBuf<int> cnt, off, perm;
+    DevBuf<unsigned long long> words;
+    DevBuf<unsigned char> scan_tmp;
+    size_t scan_bytes = 0;
+    DevBuf<int> bg_ptr, bh_ptr, fg_ptr, fh_ptr;
+    DevBuf<unsigned long long> bg_key, bh_key, fg_key, fh_key;
+    DevBuf<double> bstage, fstage, fhstage;
+    DevBuf<int> hs_mask, hs_pos;
+    DevBuf<double> hs_stage;
+    int cap = 0, nV = 0, nSV = 0; // what the buffers are sized for
+    bool lists_ready = false, fr_ready = false;
+};
+
 // device workspace of the CCD stage (ccd.cu)
 struct CcdWork {
     DevBuf<int> vmin, vmax, counters;
@@ -227,7 +246,10 @@ struct ipcgpu_ctx {
     bool has_codim = false, surface_ready = false;
     int pair_capacity = 1 << 20;
     int exchange_capacity = 1 << 16; // pairs per rank and list in the fixed-size message of the cross-rank pair-list exchange
-    bool canonical_order = true; // sort the contact lists lexicographically after the build
+    // order of the contact lists (ipcgpu_set_canonical_order): 0 build order, 1 sorted lexicographically by host-sized sorts, 2 sorted by
+    // device-sized sorts and every contact sum taken in list order (the reproducible mode, ReproWork)
+    int canonical_order = 1;
+    ipcgpu::ReproWork rw;
     bool partition_contact = false, lists_local = false; // multi-rank: build only this rank's share of the contact sets
     ipcgpu::ContactWork cw;
     ipcgpu::CcdWork ccd;
@@ -318,7 +340,7 @@ struct ipcgpu_ctx {
     // capture and re-applied at every replay.  `epoch` is bumped by every call that may reallocate or re-partition: older graphs are refused.
     struct HostState {
         unsigned local_scalars;
-        bool lists_local, lists_global, want_cand, swept_ready, fr_ready, inputs_marked, scatter_marked, hs_set_built, hs_lag_ready;
+        bool lists_local, lists_global, want_cand, swept_ready, fr_ready, inputs_marked, scatter_marked, hs_set_built, hs_lag_ready, rep_lists, rep_fr;
         int nC, nP, nK, fr_host_n;
     };
     struct GraphRec {

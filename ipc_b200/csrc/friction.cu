@@ -15,8 +15,7 @@
 // The reference forms the 12x12 matrix T^T S T and eigen-decomposes it (makePD); its non-zero spectrum is (sum w^2) * eig(S), so the
 // projection is the clamp of the two eigenvalues of S -- done here in closed form on e_perp, e_par.  One thread per pair, ten 3x3 blocks
 // w_k w_l M (M = B S B^T is symmetric, so no orientation case) added straight into the CSR rows this rank owns.
-#include "pair_common.cuh"
-#include "kernels.h"
+#include "repro.cuh"
 
 namespace ipcgpu {
 
@@ -35,6 +34,9 @@ DEV void fric_weights(int kind, double c0, double c1, double* w)
     else { w[0] = 1.0; w[1] = -1.0; w[2] = 0.0; w[3] = 0.0; }                              // PP  :246-252
 }
 
+// kUnrolled: the stencil loop unrolled with a guard, so that dx stays in registers (the reproducible mode's staging kernel; the other
+// kernels keep the loop they were tuned with)
+template <bool kUnrolled = false>
 DEV FricPair fric_pair(const FrictionArgs& p, int c)
 {
     FricPair f;
@@ -45,7 +47,13 @@ DEV FricPair fric_pair(const FrictionArgs& p, int c)
     f.b0 = { B[0], B[1], B[2] };
     f.b1 = { B[3], B[4], B[5] };
     V3 dx[4];
-    for (int k = 0; k < f.s.nv; ++k) dx[k] = load_vertex(p.V, p.nV, f.s.v[k]) - load_vertex(p.Vt, p.nV, f.s.v[k]);
+    if (kUnrolled) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (k < f.s.nv) dx[k] = load_vertex(p.V, p.nV, f.s.v[k]) - load_vertex(p.Vt, p.nV, f.s.v[k]);
+    }
+    else
+        for (int k = 0; k < f.s.nv; ++k) dx[k] = load_vertex(p.V, p.nV, f.s.v[k]) - load_vertex(p.Vt, p.nV, f.s.v[k]);
     V3 r; // relDX3D in the reference's own association (FrictionUtils.hpp:48-57, 131-140, 183-191, 246-252)
     if (f.s.kind == 0) r = dx[0] - (dx[1] + co.x * (dx[2] - dx[1]) + co.y * (dx[3] - dx[1]));
     else if (f.s.kind == 1) r = dx[0] + co.x * (dx[1] - dx[0]) - (dx[2] + co.y * (dx[3] - dx[2]));
@@ -150,24 +158,65 @@ __global__ void __launch_bounds__(256) k_friction_energy(FrictionArgs p, double*
     cta_sum(&val, partials + blockIdx.x);
 }
 
+// kStage (reproducible mode): the vector of stencil vertex k of pair c goes to g[3 (4c + k) + q] of the staging array (k_repro_gather_g sums it)
+template <bool kStage>
 __global__ void __launch_bounds__(128) k_friction_gradient(FrictionArgs p, double* __restrict__ g)
 {
     const FricRange r = fric_range(p);
     const double eps = sqrt(p.eps2);
     for (int c = r.b + blockIdx.x * blockDim.x + threadIdx.x; c < r.e; c += gridDim.x * blockDim.x) {
-        const FricPair f = fric_pair(p, c);
+        const FricPair f = fric_pair<kStage>(p, c);
         const double x2 = f.u0 * f.u0 + f.u1 * f.u1;
         double u0 = f.u0, u1 = f.u1;
         if (x2 > p.eps2) { const double n = sqrt(x2); u0 /= n; u1 /= n; }
         else { const double s = f1_SF_div(x2, eps); u0 *= s; u1 *= s; }
         const V3 t = u0 * f.b0 + u1 * f.b1;
         const double cl = p.coef * p.lambda[c];
-        for (int k = 0; k < f.s.nv; ++k) {
-            const double wk = f.w[k] * cl;
-            atomicAdd(g + 3 * (size_t)f.s.v[k], wk * t.x);
-            atomicAdd(g + 3 * (size_t)f.s.v[k] + 1, wk * t.y);
-            atomicAdd(g + 3 * (size_t)f.s.v[k] + 2, wk * t.z);
+        if (kStage) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { // (unrolled with a guard: the stencil stays in registers)
+                if (k >= f.s.nv) continue;
+                const double wk = f.w[k] * cl;
+                double* out = g + 3 * (4 * (size_t)c + k);
+                out[0] = wk * t.x;
+                out[1] = wk * t.y;
+                out[2] = wk * t.z;
+            }
         }
+        else
+            for (int k = 0; k < f.s.nv; ++k) {
+                const double wk = f.w[k] * cl;
+                atomicAdd(g + 3 * (size_t)f.s.v[k], wk * t.x);
+                atomicAdd(g + 3 * (size_t)f.s.v[k] + 1, wk * t.y);
+                atomicAdd(g + 3 * (size_t)f.s.v[k] + 2, wk * t.z);
+            }
+    }
+}
+
+// the projected tangent-plane block M = B S B^T of pair f (symmetric, row-major)
+DEV void fric_block(const FrictionArgs& p, const FricPair& f, int c, double eps, double* M)
+{
+    const double x2 = f.u0 * f.u0 + f.u1 * f.u1, xn = sqrt(x2);
+    const double cl = p.coef * p.lambda[c];
+    // eigenvalues of S across / along the slip direction
+    double e_perp, e_par;
+    if (x2 > p.eps2) { e_perp = cl / xn; e_par = 0.0; }                 // :2776-2786  c lam (I/|u| - uu^T/|u|^3)
+    else {                                                               // :2787-2804
+        const double f1 = f1_SF_div(x2, eps), f2 = f2_SF(x2, eps);
+        e_perp = cl * f1;
+        e_par = (f2 != f1 && x2 != 0.0) ? cl * f2 : e_perp;
+    }
+    // makePD (IglUtils.hpp:119-133): clamp of the spectrum -- here the two eigenvalues of S
+    e_perp = fmax(e_perp, 0.0);
+    e_par = fmax(e_par, 0.0);
+    // M = B S B^T = e_perp (b0 b0^T + b1 b1^T) + (e_par - e_perp) t t^T,  t = B u / |u|
+    {
+        V3 t = { 0.0, 0.0, 0.0 };
+        if (x2 > 0.0) t = (f.u0 / xn) * f.b0 + (f.u1 / xn) * f.b1;
+        const double de = e_par - e_perp;
+        const double b0v[3] = { f.b0.x, f.b0.y, f.b0.z }, b1v[3] = { f.b1.x, f.b1.y, f.b1.z }, tv[3] = { t.x, t.y, t.z };
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) M[3 * i + j] = e_perp * (b0v[i] * b0v[j] + b1v[i] * b1v[j]) + de * (tv[i] * tv[j]);
     }
 }
 
@@ -180,29 +229,8 @@ __global__ void __launch_bounds__(128) k_friction_hessian(FrictionArgs p, double
         bool mine = false; // row-owner rule: a rank adds only the block rows it owns
         for (int k = 0; k < f.s.nv; ++k) mine = mine || (f.s.v[k] >= p.row_lo && f.s.v[k] < p.row_hi);
         if (!mine) continue;
-        const double x2 = f.u0 * f.u0 + f.u1 * f.u1, xn = sqrt(x2);
-        const double cl = p.coef * p.lambda[c];
-        // eigenvalues of S across / along the slip direction
-        double e_perp, e_par;
-        if (x2 > p.eps2) { e_perp = cl / xn; e_par = 0.0; }                 // :2776-2786  c lam (I/|u| - uu^T/|u|^3)
-        else {                                                               // :2787-2804
-            const double f1 = f1_SF_div(x2, eps), f2 = f2_SF(x2, eps);
-            e_perp = cl * f1;
-            e_par = (f2 != f1 && x2 != 0.0) ? cl * f2 : e_perp;
-        }
-        // makePD (IglUtils.hpp:119-133): clamp of the spectrum -- here the two eigenvalues of S
-        e_perp = fmax(e_perp, 0.0);
-        e_par = fmax(e_par, 0.0);
-        // M = B S B^T = e_perp (b0 b0^T + b1 b1^T) + (e_par - e_perp) t t^T,  t = B u / |u|
         double M[9];
-        {
-            V3 t = { 0.0, 0.0, 0.0 };
-            if (x2 > 0.0) t = (f.u0 / xn) * f.b0 + (f.u1 / xn) * f.b1;
-            const double de = e_par - e_perp;
-            const double b0v[3] = { f.b0.x, f.b0.y, f.b0.z }, b1v[3] = { f.b1.x, f.b1.y, f.b1.z }, tv[3] = { t.x, t.y, t.z };
-            for (int i = 0; i < 3; ++i)
-                for (int j = 0; j < 3; ++j) M[3 * i + j] = e_perp * (b0v[i] * b0v[j] + b1v[i] * b1v[j]) + de * (tv[i] * tv[j]);
-        }
+        fric_block(p, f, c, eps, M);
         for (int bi = 0; bi < f.s.nv; ++bi) {
             for (int bj = bi; bj < f.s.nv; ++bj) {
                 const int vi = min(f.s.v[bi], f.s.v[bj]), vj = max(f.s.v[bi], f.s.v[bj]);
@@ -220,6 +248,29 @@ __global__ void __launch_bounds__(128) k_friction_hessian(FrictionArgs p, double
     }
 }
 
+// reproducible mode: M and the stencil weights of every pair to hstage (13 doubles per pair), then a per-row gather (repro.cuh) of the blocks
+// w_bi w_bj M, one thread per row vertex
+__global__ void __launch_bounds__(128) k_friction_hessian_stage(FrictionArgs p)
+{
+    const int n = *p.n;
+    const double eps = sqrt(p.eps2);
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) {
+        const FricPair f = fric_pair<true>(p, c);
+        double* out = p.rep.hstage + 13 * (size_t)c;
+        fric_block(p, f, c, eps, out);
+        for (int k = 0; k < 4; ++k) out[9 + k] = f.w[k];
+    }
+}
+__global__ void __launch_bounds__(128) k_friction_hessian_gather(FrictionArgs p, double* __restrict__ a, int* __restrict__ err)
+{
+    for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < p.nV; v += gridDim.x * blockDim.x)
+        repro_gather_row(v, p.rep.h, p.dbc, p.projectDBC, p.ia, p.ja, p.base, a, err, [&](int c, int bi, int bj, double* acc) {
+            const double* S = p.rep.hstage + 13 * (size_t)c;
+            const double ww = S[9 + bi] * S[9 + bj];
+            for (int i = 0; i < 9; ++i) acc[i] += ww * S[i];
+        });
+}
+
 // -----------------------------------------------------------------------------------------------------------
 void friction_lag(const BarrierArgs& p, int4* cs_out, int* n_out, double* lambda, double2* coord, double* basis, int capacity, int* bad, cudaStream_t st)
 {
@@ -227,7 +278,21 @@ void friction_lag(const BarrierArgs& p, int4* cs_out, int* n_out, double* lambda
 }
 void friction_energy(const FrictionArgs& p, double* partials, cudaStream_t st) { k_friction_energy<<<kFricEnergyBlocks, 256, 0, st>>>(p, partials); }
 int friction_energy_blocks() { return kFricEnergyBlocks; }
-void friction_gradient(const FrictionArgs& p, double* g, cudaStream_t st) { k_friction_gradient<<<kSMs * 4, 128, 0, st>>>(p, g); }
-void friction_hessian(const FrictionArgs& p, double* a, int* err, cudaStream_t st) { k_friction_hessian<<<kSMs * 4, 128, 0, st>>>(p, a, err); }
+void friction_gradient(const FrictionArgs& p, double* g, cudaStream_t st)
+{
+    if (p.rep.on) {
+        k_friction_gradient<true><<<kSMs * 4, 128, 0, st>>>(p, p.rep.stage);
+        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 0ull, ~0ull, g, st);
+    }
+    else k_friction_gradient<false><<<kSMs * 4, 128, 0, st>>>(p, g);
+}
+void friction_hessian(const FrictionArgs& p, double* a, int* err, cudaStream_t st)
+{
+    if (p.rep.on) {
+        k_friction_hessian_stage<<<kSMs * 4, 128, 0, st>>>(p);
+        k_friction_hessian_gather<<<kSMs * 4, 128, 0, st>>>(p, a, err);
+    }
+    else k_friction_hessian<<<kSMs * 4, 128, 0, st>>>(p, a, err);
+}
 
 } // namespace ipcgpu

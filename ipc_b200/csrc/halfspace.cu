@@ -84,7 +84,18 @@ __global__ void __launch_bounds__(256) k_hs_energy(HalfSpaceArgs p, double dHat,
     cta_sum(&val, partials + blockIdx.x);
 }
 
+// reproducible mode (kStage): entry c of plane q at vertex v leaves its vector (3 doubles) or the upper part of its block (6) in rep_stage[c]
+// and marks itself in rep_mask[v] / rep_pos; k_hs_repro_add then adds the entries of every vertex in plane order
+template <int kWidth>
+DEV void hs_stage(const HalfSpaceArgs& p, int c, int2 e, const double* val)
+{
+    for (int i = 0; i < kWidth; ++i) p.rep_stage[(size_t)kWidth * c + i] = val[i];
+    p.rep_pos[kMaxPlanes * (size_t)e.y + e.x] = c;
+    atomicOr(p.rep_mask + e.y, 1 << e.x);
+}
+
 // kappa_dev != nullptr (the barrier kernels below): kappa is the device-resident one
+template <bool kStage>
 __global__ void __launch_bounds__(128) k_hs_gradient(HalfSpaceArgs p, double dHat, double kappa, const double* __restrict__ kappa_dev, double* __restrict__ g)
 {
     if (kappa_dev) kappa = *kappa_dev;
@@ -97,19 +108,59 @@ __global__ void __launch_bounds__(128) k_hs_gradient(HalfSpaceArgs p, double dHa
         double b, db, d2b;
         barrier_all(d, dHat, b, db, d2b);
         const double s = kappa * db * 2.0 * dist; // coef * input[cI] * 2.0 * dist (HalfSpace.cpp:138)
-        for (int r = 0; r < 3; ++r) atomicAdd(g + 3 * (size_t)e.y + r, s * pl[r]);
+        if (kStage) {
+            const double val[3] = { s * pl[0], s * pl[1], s * pl[2] };
+            hs_stage<3>(p, c, e, val);
+        }
+        else
+            for (int r = 0; r < 3; ++r) atomicAdd(g + 3 * (size_t)e.y + r, s * pl[r]);
     }
 }
 
 // upper part of a symmetric 3x3 block M (row-major) onto the diagonal block of vertex v: row 3v+r starts with column 3v+r
-DEV void add_diag_block(const HalfSpaceArgs& p, int v, const double* M, double* a)
+template <bool kStage>
+DEV void add_diag_block(const HalfSpaceArgs& p, int c, int2 e, const double* M, double* a)
 {
-    for (int r = 0; r < 3; ++r) {
-        const int o = p.ia[3 * v + r] - p.base;
-        for (int q = r; q < 3; ++q) atomicAdd(a + o + (q - r), M[3 * r + q]);
+    if (kStage) {
+        const double val[6] = { M[0], M[1], M[2], M[4], M[5], M[8] };
+        hs_stage<6>(p, c, e, val);
+    }
+    else
+        for (int r = 0; r < 3; ++r) {
+            const int o = p.ia[3 * e.y + r] - p.base;
+            for (int q = r; q < 3; ++q) atomicAdd(a + o + (q - r), M[3 * r + q]);
+        }
+}
+
+// the entry of the lowest plane of its vertex adds the staged entries of that vertex in plane order, once, and clears the vertex's mask.
+// kWidth 3: into g[v]; 6: into the upper part of v's diagonal block of a
+template <int kWidth>
+__global__ void __launch_bounds__(128) k_hs_repro_add(HalfSpaceArgs p, const int2* __restrict__ list, const int* __restrict__ n_ptr, double* __restrict__ out)
+{
+    const int n = *n_ptr;
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) {
+        const int2 e = list[c];
+        const int m = p.rep_mask[e.y];
+        if (m == 0 || __ffs(m) - 1 != e.x) continue;
+        double sum[kWidth];
+        for (int i = 0; i < kWidth; ++i) sum[i] = 0.0;
+        for (int q = 0; q < kMaxPlanes; ++q) {
+            if (!((m >> q) & 1)) continue;
+            const double* val = p.rep_stage + (size_t)kWidth * p.rep_pos[kMaxPlanes * (size_t)e.y + q];
+            for (int i = 0; i < kWidth; ++i) sum[i] += val[i];
+        }
+        p.rep_mask[e.y] = 0;
+        if (kWidth == 3)
+            for (int r = 0; r < 3; ++r) out[3 * (size_t)e.y + r] += sum[r];
+        else
+            for (int r = 0, i = 0; r < 3; ++r) {
+                const int o = p.ia[3 * e.y + r] - p.base;
+                for (int q = r; q < 3; ++q, ++i) out[o + (q - r)] += sum[i];
+            }
     }
 }
 
+template <bool kStage>
 __global__ void __launch_bounds__(128) k_hs_hessian(HalfSpaceArgs p, double dHat, double kappa, const double* __restrict__ kappa_dev, int projectDBC,
     double* __restrict__ a)
 {
@@ -128,7 +179,7 @@ __global__ void __launch_bounds__(128) k_hs_hessian(HalfSpaceArgs p, double dHat
         double M[9];
         for (int i = 0; i < 3; ++i)
             for (int j = 0; j < 3; ++j) M[3 * i + j] = s * (pl[i] * pl[j]);
-        add_diag_block(p, e.y, M, a);
+        add_diag_block<kStage>(p, c, e, M, a);
     }
 }
 
@@ -235,6 +286,7 @@ __global__ void __launch_bounds__(256) k_hs_fric_energy(HalfSpaceArgs p, double 
     cta_sum(&val, partials + blockIdx.x);
 }
 
+template <bool kStage>
 __global__ void __launch_bounds__(128) k_hs_fric_gradient(HalfSpaceArgs p, double eps2, double* __restrict__ g)
 {
     const int n = *p.n_lag;
@@ -246,10 +298,16 @@ __global__ void __launch_bounds__(128) k_hs_fric_gradient(HalfSpaceArgs p, doubl
         const Slip s = slip(p, pl, e.y);
         const double m = pl[7] * p.lam[c];
         const double f = (s.mag2 > eps2) ? m / sqrt(s.mag2) : m / eps; // HalfSpace.cpp:317-322
-        for (int r = 0; r < 3; ++r) atomicAdd(g + 3 * (size_t)e.y + r, f * s.u[r]);
+        if (kStage) {
+            const double val[3] = { f * s.u[0], f * s.u[1], f * s.u[2] };
+            hs_stage<3>(p, c, e, val);
+        }
+        else
+            for (int r = 0; r < 3; ++r) atomicAdd(g + 3 * (size_t)e.y + r, f * s.u[r]);
     }
 }
 
+template <bool kStage>
 __global__ void __launch_bounds__(128) k_hs_fric_hessian(HalfSpaceArgs p, double eps2, int projectDBC, double* __restrict__ a)
 {
     const int n = *p.n_lag;
@@ -276,7 +334,7 @@ __global__ void __launch_bounds__(128) k_hs_fric_hessian(HalfSpaceArgs p, double
             for (int i = 0; i < 3; ++i)
                 for (int j = 0; j < 3; ++j) M[3 * i + j] = ((i == j ? 1.0 : 0.0) - pl[i] * pl[j]) * k;
         }
-        add_diag_block(p, e.y, M, a);
+        add_diag_block<kStage>(p, c, e, M, a);
     }
 }
 
@@ -310,11 +368,19 @@ void halfspace_energy(const HalfSpaceArgs& p, double dHat, double* partials, int
 }
 void halfspace_gradient(const HalfSpaceArgs& p, double dHat, double kappa, const double* kappa_dev, double* g, cudaStream_t st)
 {
-    k_hs_gradient<<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, g);
+    if (p.rep_mask) {
+        k_hs_gradient<true><<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, g);
+        k_hs_repro_add<3><<<kSMs, 128, 0, st>>>(p, p.act, p.n_act, g);
+    }
+    else k_hs_gradient<false><<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, g);
 }
 void halfspace_hessian(const HalfSpaceArgs& p, double dHat, double kappa, const double* kappa_dev, int projectDBC, double* a, cudaStream_t st)
 {
-    k_hs_hessian<<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, projectDBC, a);
+    if (p.rep_mask) {
+        k_hs_hessian<true><<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, projectDBC, a);
+        k_hs_repro_add<6><<<kSMs, 128, 0, st>>>(p, p.act, p.n_act, a);
+    }
+    else k_hs_hessian<false><<<kSMs, 128, 0, st>>>(p, dHat, kappa, kappa_dev, projectDBC, a);
 }
 void halfspace_step(const HalfSpaceArgs& p, const double* dir, double slack, IterState* st_dev, cudaStream_t st)
 {
@@ -337,11 +403,19 @@ void halfspace_friction_energy(const HalfSpaceArgs& p, double eps2, double* part
 }
 void halfspace_friction_gradient(const HalfSpaceArgs& p, double eps2, double* g, cudaStream_t st)
 {
-    k_hs_fric_gradient<<<kSMs, 128, 0, st>>>(p, eps2, g);
+    if (p.rep_mask) {
+        k_hs_fric_gradient<true><<<kSMs, 128, 0, st>>>(p, eps2, g);
+        k_hs_repro_add<3><<<kSMs, 128, 0, st>>>(p, p.lag, p.n_lag, g);
+    }
+    else k_hs_fric_gradient<false><<<kSMs, 128, 0, st>>>(p, eps2, g);
 }
 void halfspace_friction_hessian(const HalfSpaceArgs& p, double eps2, int projectDBC, double* a, cudaStream_t st)
 {
-    k_hs_fric_hessian<<<kSMs, 128, 0, st>>>(p, eps2, projectDBC, a);
+    if (p.rep_mask) {
+        k_hs_fric_hessian<true><<<kSMs, 128, 0, st>>>(p, eps2, projectDBC, a);
+        k_hs_repro_add<6><<<kSMs, 128, 0, st>>>(p, p.lag, p.n_lag, a);
+    }
+    else k_hs_fric_hessian<false><<<kSMs, 128, 0, st>>>(p, eps2, projectDBC, a);
 }
 
 } // namespace ipcgpu

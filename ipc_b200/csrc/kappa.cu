@@ -265,10 +265,11 @@ int ipcgpu_kappa_init(ipcgpu_ctx* ctx, double dHat)
     evaluate_constraints(p, ctx->cw.bval.p, st);
     k_kappa_gb<<<kKappaBlocks, kKappaThreads, 0, st>>>(p.nC, dHat, ctx->cw.bval.p);
     constraint_jacobian_t(p, ctx->cw.bval.p, 1.0, gc, st);
-    ctx->launches += 3;
+    ctx->launches += 3 + p.rep.on; // (+ the reproducible mode's gather)
     if (ps.n) {
-        halfspace_gradient(halfspace_args(ctx), dHat, 1.0, nullptr, gc, st);
-        ++ctx->launches;
+        const HalfSpaceArgs hp = halfspace_args(ctx);
+        halfspace_gradient(hp, dHat, 1.0, nullptr, gc, st);
+        ctx->launches += 1 + (hp.rep_mask != nullptr);
     }
     if (ctx->has_dbc) {
         k_kappa_zero_dbc<<<std::min(nblk(ctx->nV, kKappaThreads), kKappaBlocks), kKappaThreads, 0, st>>>(ctx->nV, ctx->dbc.p, gc);

@@ -151,7 +151,23 @@ struct SurfArgs {
 // which body a surface primitive belongs to is decided by any one of its vertices (primitives do not straddle bodies)
 __device__ __forceinline__ bool obstacle_vertex(const SurfArgs& s, int v) { return v >= s.nVdof; }
 
+// Reproducible mode (ipcgpu_set_canonical_order(ctx, 2), repro.cu): the contact terms add into g and a in an order fixed by the lists alone.
+// A term kernel writes each pair's per-vertex vectors to `stage` (3 doubles per contribution index); a gather then sums the entries of
+// every vertex in ascending key order and adds the result to g once.  The Hessians go through a per-row gather of the same form.
+struct VertexIndex {
+    const int* ptr;                  // nV + 1 starts: the entries of vertex v are key[ptr[v], ptr[v + 1]), ascending
+    const unsigned long long* key;   // gradient: contribution index; Hessian: column vertex << 32 | list index << 4 | block (bi << 2 | bj)
+};
+struct ReproArgs {
+    int on = 0;                      // 0: the atomic scatter (levels 0 and 1); nothing below is read
+    int cap = 0;                     // list capacity: the active list's contributions are [0, 4 cap), the mollified list's [4 cap, 12 cap)
+    double* stage = nullptr;         // per-contribution gradient vectors
+    double* hstage = nullptr;        // friction Hessian: M (9) and the stencil weights (4) per pair
+    VertexIndex g = {}, h = {};      // gradient and Hessian indices
+};
+
 struct BarrierArgs {
+    ReproArgs rep;
     int nV;
     const double* V;
     const double* Vrest;
@@ -181,8 +197,11 @@ void para_gradient(const BarrierArgs& p, double* g, cudaStream_t st);
 // Hraw: 144 doubles per owned pair; rows: 4 vertex ids per owned pair; psd: makePD "unchanged" flag per owned pair; n_owned: device counter
 void barrier_hessian_build_project(const BarrierArgs& p, int* flags, double* Hraw, int* rows, int* psd, int* n_owned, int capacity, cudaStream_t st);
 void barrier_hessian_scatter(const BarrierArgs& p, double* a, int* flags, const double* Hraw, const int* rows, const int* psd, const int* n_owned, int capacity, cudaStream_t st);
+// repro.cu -- the reproducible mode.  g[v] += the staged contributions of v with lo <= key < hi, in index order (one thread per vertex)
+void repro_gather_g(int nV, const VertexIndex& idx, const double* stage, unsigned long long lo, unsigned long long hi, double* g, cudaStream_t st);
 // friction.cu -- lagged friction of the self-contact pairs (SelfCollisionHandler.cpp:2481-2987)
 struct FrictionArgs {
+    ReproArgs rep;
     int nV;
     const double* V;       // current positions (SoA)
     const double* Vt;      // positions at the start of the time step, result.V_prev (SoA)
@@ -235,6 +254,11 @@ struct HalfSpaceArgs {
     const int2* lag; const double* lam; const int* n_lag; // lagged set (friction planes only), lambda, size
     int row_lo, row_hi;     // rows (energies, gradient, Hessian, crossings) this rank owns
     const int* ia; int base;
+    // reproducible mode: an entry (plane q, vertex v) at list position c leaves its vector / block in rep_stage[c], sets bit q of rep_mask[v]
+    // and c in rep_pos[kMaxPlanes v + q]; the entry of the lowest plane of v then adds them in plane order (and clears rep_mask[v])
+    int* rep_mask = nullptr;
+    int* rep_pos = nullptr;
+    double* rep_stage = nullptr;
 };
 int halfspace_energy_blocks();
 size_t halfspace_scan_bytes(int n);

@@ -50,6 +50,16 @@ DEV int csr_find(const int* __restrict__ ia, const int* __restrict__ ja, int bas
     return (lo < end && ja[lo] == target) ? lo : -1;
 }
 
+// the two-edge stencil of a mollified (nearly parallel EE) entry: its own four vertices, or the edges (eI, eJ) it came from
+DEV void para_edge_stencil(int4 mm, int2 e, const int* __restrict__ SE, int* ev)
+{
+    if (mm.w >= 0 && mm.x >= 0) { ev[0] = mm.x; ev[1] = mm.y; ev[2] = mm.z; ev[3] = mm.w; }
+    else {
+        ev[0] = SE[2 * e.x]; ev[1] = SE[2 * e.x + 1];
+        ev[2] = SE[2 * e.y]; ev[3] = SE[2 * e.y + 1];
+    }
+}
+
 DEV bool proj_dbc(const uint8_t* dbc, int v, int projectDBC) { return dbc && (dbc[v] == 1 || (dbc[v] == 2 && projectDBC)); }
 
 } // namespace ipcgpu
