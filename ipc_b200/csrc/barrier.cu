@@ -91,9 +91,9 @@ __global__ void __launch_bounds__(256) k_barrier_energy(BarrierArgs p, double* _
         const bool is_para = i >= nA;
         const int c = is_para ? lr.pb + (i - nA) : lr.cb + i;
         const int4 mm = is_para ? p.para[c] : p.cs[c];
-        PairStencil s = decode(mm);
+        const PairStencil s = decode(mm);
         V3 x[4];
-        for (int k = 0; k < s.nv; ++k) x[k] = load_vertex(p.V, p.nV, s.v[k]);
+        load_stencil(s, p.V, p.nV, x);
         const double d = pair_distance(s, x);
         if (!(d > 0.0)) atomicExch(bad, 1);
         else {
@@ -102,11 +102,10 @@ __global__ void __launch_bounds__(256) k_barrier_energy(BarrierArgs p, double* _
             if (!is_para) val += (mm.x < 0 && mm.w < -1) ? b * (double)(-mm.w) : b;
             else {
                 int ev[4];
-                para_edge_stencil(mm, p.para_e[c], p.SE, ev);
                 V3 ex[4];
-                for (int k = 0; k < 4; ++k) ex[k] = load_vertex(p.V, p.nV, ev[k]);
+                const double eps_x = load_para_edges(mm, p.para_e[c], p.SE, p.V, p.Vrest, p.nV, ev, ex);
                 double eg[12];
-                const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, false, [](int, int, double) {});
+                const double e = mollifier(ex, eps_x, eg, false, [](int, int, double) {});
                 val += b * e;
             }
         }
@@ -122,29 +121,20 @@ __global__ void __launch_bounds__(256) k_barrier_energy(BarrierArgs p, double* _
 template <bool kDevKappa>
 DEV double barrier_kappa(const BarrierArgs& p) { return kDevKappa ? *p.kappa_dev : p.kappa; }
 
-// kStage (reproducible mode): contribution k of a pair goes to its own slot g[3 key + q] of the staging array (ReproArgs: key 4c + k for
-// active entry c; 4 cap + 8c + k for the edge stencil and 4 cap + 8c + 4 + k for the distance stencil of mollified entry c) instead of being
-// added at its vertex; k_repro_gather_g sums them
-template <bool kStage>
-DEV void put_g(double* __restrict__ g, int v, unsigned long long key, int q, double val)
-{
-    if (kStage) g[3 * key + q] = val;
-    else atomicAdd(g + 3 * (size_t)v + q, val);
-}
-
-template <bool kDevKappa, bool kStage>
+// kStage: the contributions go to the staging array under their gradient keys (repro.cuh).  kParaOnly: the mollified list alone, the
+// reference's augmentParaEEGradient (:2990-3045)
+template <bool kDevKappa, bool kStage, bool kParaOnly = false>
 __global__ void __launch_bounds__(128) k_barrier_gradient(BarrierArgs p, double* __restrict__ g)
 {
-    const unsigned long long para0 = 4ull * p.rep.cap;
     const ListRange lr = list_range(p, false);
-    const int nA = lr.ce - lr.cb, n = nA + (lr.pe - lr.pb);
+    const int nA = kParaOnly ? 0 : lr.ce - lr.cb, n = nA + (lr.pe - lr.pb);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const bool is_para = i >= nA;
     const int c = is_para ? lr.pb + (i - nA) : lr.cb + i;
     const int4 mm = is_para ? p.para[c] : p.cs[c];
-    PairStencil s = decode(mm);
+    const PairStencil s = decode(mm);
     V3 x[4];
-    for (int k = 0; k < s.nv; ++k) x[k] = load_vertex(p.V, p.nV, s.v[k]);
+    load_stencil(s, p.V, p.nV, x);
     double gd[12];
     const double d = pair_derivs(s, x, gd, false, [](int, int, double) {});
     double b, db, d2b;
@@ -153,18 +143,16 @@ __global__ void __launch_bounds__(128) k_barrier_gradient(BarrierArgs p, double*
     if (!is_para) w = barrier_kappa<kDevKappa>(p) * s.mult * db;
     else {
         int ev[4];
-        para_edge_stencil(mm, p.para_e[c], p.SE, ev);
         V3 ex[4];
-        for (int k = 0; k < 4; ++k) ex[k] = load_vertex(p.V, p.nV, ev[k]);
+        const double eps_x = load_para_edges(mm, p.para_e[c], p.SE, p.V, p.Vrest, p.nV, ev, ex);
         double eg[12];
-        const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, false, [](int, int, double) {});
+        const double e = mollifier(ex, eps_x, eg, false, [](int, int, double) {});
         for (int k = 0; k < 4; ++k)
-            for (int q = 0; q < 3; ++q) put_g<kStage>(g, ev[k], para0 + 8ull * c + k, q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
+            for (int q = 0; q < 3; ++q) put_g<kStage>(g, ev[k], gkey_para_edge(p.rep.cap, c, k), q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
         w = barrier_kappa<kDevKappa>(p) * e * db; // slot 3 is -1 (or a vertex id): multiplicity 1
     }
-    const unsigned long long key0 = is_para ? para0 + 8ull * c + 4 : 4ull * c;
     for (int k = 0; k < s.nv; ++k)
-        for (int q = 0; q < 3; ++q) put_g<kStage>(g, s.v[k], key0 + k, q, w * gd[3 * k + q]);
+        for (int q = 0; q < 3; ++q) put_g<kStage>(g, s.v[k], is_para ? gkey_para_dist(p.rep.cap, c, k) : gkey_active(c, k), q, w * gd[3 * k + q]);
     }
 }
 
@@ -176,12 +164,7 @@ __global__ void __launch_bounds__(128) k_barrier_gradient(BarrierArgs p, double*
 __global__ void __launch_bounds__(256) k_evaluate_constraints(BarrierArgs p, double* __restrict__ val)
 {
     const int n = *p.nC;
-    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) {
-        const PairStencil s = decode(p.cs[c]);
-        V3 x[4];
-        for (int k = 0; k < s.nv; ++k) x[k] = load_vertex(p.V, p.nV, s.v[k]);
-        val[c] = pair_distance(s, x);
-    }
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) val[c] = pair_distance(p.cs[c], p.V, p.nV);
 }
 template <bool kStage>
 __global__ void __launch_bounds__(128) k_constraint_jacobian_t(BarrierArgs p, const double* __restrict__ input, double coef, double* __restrict__ g)
@@ -190,40 +173,12 @@ __global__ void __launch_bounds__(128) k_constraint_jacobian_t(BarrierArgs p, co
     for (int c = lr.cb + blockIdx.x * blockDim.x + threadIdx.x; c < lr.ce; c += gridDim.x * blockDim.x) {
         const PairStencil s = decode(p.cs[c]);
         V3 x[4];
-        for (int k = 0; k < s.nv; ++k) x[k] = load_vertex(p.V, p.nV, s.v[k]);
+        load_stencil(s, p.V, p.nV, x);
         double gd[12];
         pair_derivs(s, x, gd, false, [](int, int, double) {});
         const double w = coef * s.mult * input[c];
         for (int k = 0; k < s.nv; ++k)
-            for (int q = 0; q < 3; ++q) put_g<kStage>(g, s.v[k], 4ull * c + k, q, w * gd[3 * k + q]);
-    }
-}
-// augmentParaEEGradient (:2990-3045) alone: the mollified pairs' share of k_barrier_gradient
-template <bool kDevKappa, bool kStage>
-__global__ void __launch_bounds__(128) k_para_gradient(BarrierArgs p, double* __restrict__ g)
-{
-    const unsigned long long para0 = 4ull * p.rep.cap;
-    const ListRange lr = list_range(p, false);
-    for (int c = lr.pb + blockIdx.x * blockDim.x + threadIdx.x; c < lr.pe; c += gridDim.x * blockDim.x) {
-        const int4 mm = p.para[c];
-        const PairStencil s = decode(mm);
-        V3 x[4];
-        for (int k = 0; k < s.nv; ++k) x[k] = load_vertex(p.V, p.nV, s.v[k]);
-        double gd[12];
-        const double d = pair_derivs(s, x, gd, false, [](int, int, double) {});
-        double b, db, d2b;
-        barrier_all(d, p.dHat, b, db, d2b);
-        int ev[4];
-        para_edge_stencil(mm, p.para_e[c], p.SE, ev);
-        V3 ex[4];
-        for (int k = 0; k < 4; ++k) ex[k] = load_vertex(p.V, p.nV, ev[k]);
-        double eg[12];
-        const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, false, [](int, int, double) {});
-        for (int k = 0; k < 4; ++k)
-            for (int q = 0; q < 3; ++q) put_g<kStage>(g, ev[k], para0 + 8ull * c + k, q, barrier_kappa<kDevKappa>(p) * b * eg[3 * k + q]);
-        const double w = barrier_kappa<kDevKappa>(p) * e * db;
-        for (int k = 0; k < s.nv; ++k)
-            for (int q = 0; q < 3; ++q) put_g<kStage>(g, s.v[k], para0 + 8ull * c + 4 + k, q, w * gd[3 * k + q]);
+            for (int q = 0; q < 3; ++q) put_g<kStage>(g, s.v[k], gkey_active(c, k), q, w * gd[3 * k + q]);
     }
 }
 
@@ -249,9 +204,10 @@ __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, dou
     // cost 32 sectors per warp access
     const bool is_para = c >= nC;
     const int4 mm = is_para ? p.para[c - nC] : p.cs[c];
-    PairStencil s = decode(mm);
+    const PairStencil s = decode(mm);
     int rows[4];
-    {   // row ownership (multi-rank): this rank assembles the pair only if it owns a row of its stencil
+    {   // row ownership (multi-rank): this rank assembles the pair only if it owns a row of its stencil.  The rows are hessian_rows',
+        // written out: the call raises this kernel's spill loads
         bool mine = false;
         if (!is_para) {
             for (int k = 0; k < 4; ++k) rows[k] = (k < s.nv) ? s.v[k] : -1;
@@ -264,7 +220,7 @@ __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, dou
 #define HE(i, j) H[(i) * 12 + (j)]
     for (int i = 0; i < 144; ++i) H[i] = 0.0;
     V3 x[4];
-    for (int k = 0; k < s.nv; ++k) x[k] = load_vertex(p.V, p.nV, s.v[k]);
+    load_stencil(s, p.V, p.nV, x);
     if (!is_para) {
         const int n = 3 * s.nv;
         double gd[12];
@@ -278,9 +234,8 @@ __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, dou
     else {
         // mollified pair on the two-edge stencil (:3049-3173)
         int ev[4];
-        para_edge_stencil(mm, p.para_e[c - nC], p.SE, ev);
         V3 ex[4];
-        for (int k = 0; k < 4; ++k) ex[k] = load_vertex(p.V, p.nV, ev[k]);
+        const double eps_x = load_para_edges(mm, p.para_e[c - nC], p.SE, p.V, p.Vrest, p.nV, ev, ex);
         double gd0[12], gd[12], eg[12];
         double AE[144], VE[144]; // distance Hessian on its own stencil / embedded in the edge stencil
         const double d = pair_derivs(s, x, gd0, true, [&](int i, int j, double v) { AE[i * 12 + j] = v; });
@@ -303,7 +258,7 @@ __global__ void __launch_bounds__(64) k_barrier_hessian_build(BarrierArgs p, dou
         }
         double b, db, d2b;
         barrier_all(d, p.dHat, b, db, d2b);
-        const double e = mollifier(ex, eps_x_rest(p.Vrest, p.nV, ev[0], ev[1], ev[2], ev[3]), eg, true, [&](int i, int j, double v) { HE(i, j) = v; });
+        const double e = mollifier(ex, eps_x, eg, true, [&](int i, int j, double v) { HE(i, j) = v; });
         const double k = barrier_kappa<kDevKappa>(p);
         for (int i = 0; i < 12; ++i)
             for (int j = 0; j < 12; ++j)
@@ -532,6 +487,22 @@ __global__ void __launch_bounds__(32 * kProjWarps) k_barrier_hessian_project(con
     }
 }
 
+// entry (i, j) of a pair slot's projected Hessian: the raw 12x12 where makePD returned its input (psd flag), else
+// (Q^T M Q)[i][j] = sum_{a,b} Q4[a][bi] Q4[b][bj] M[3a+r][3b+q] from the 9x9 M that k_barrier_hessian_project left in the slot
+DEV double pair_hessian_entry(const double* __restrict__ H0, bool raw, int i, int j)
+{
+    if (raw) return H0[i * 12 + j];
+    const int bi = i / 3, r = i % 3, bj = j / 3, q = j % 3;
+    double v = 0.0;
+#pragma unroll
+    for (int ka = 0; ka < 3; ++ka) {
+        const double qa = helmert(ka, bi);
+#pragma unroll
+        for (int kb = 0; kb < 3; ++kb) v += (qa * helmert(kb, bj)) * H0[(3 * ka + r) * 9 + 3 * kb + q];
+    }
+    return v;
+}
+
 // scatter of the projected pair Hessians into the CSR values (upper-triangular 3x3 blocks, LinSysSolver.hpp:207-265)
 constexpr int kScatWarps = 8;
 __global__ void __launch_bounds__(32 * kScatWarps) k_barrier_hessian_scatter(BarrierArgs p, const int* __restrict__ n_ptr, int capacity, const double* __restrict__ H,
@@ -542,7 +513,7 @@ __global__ void __launch_bounds__(32 * kScatWarps) k_barrier_hessian_scatter(Bar
     const int n = min(*n_ptr, capacity);
     for (int c = blockIdx.x * kScatWarps + wib; c < n; c += gridDim.x * kScatWarps) {
     const double* H0 = H + (size_t)c * 144;
-    const bool raw = psd[c] != 0; // makePD returned its input: the slot still holds the unprojected 12x12
+    const bool raw = psd[c] != 0;
     // CSR offsets of the 16 vertex blocks x 3 rows (upper-triangular blocks only); -1 = skip, -2 = missing in the pattern
     int rows[4];
 #pragma unroll
@@ -551,7 +522,7 @@ __global__ void __launch_bounds__(32 * kScatWarps) k_barrier_hessian_scatter(Bar
         const int bi = t / 12, bj = (t / 3) % 4, r = t % 3;
         int o = -1;
         const int vi = rows[bi], vj = rows[bj];
-        if (vi >= 0 && vj >= 0 && vi <= vj && !(vi == vj && bi != bj) && owns_row(p, vi) && !proj_dbc(p.dbc, vi, p.projectDBC) && !proj_dbc(p.dbc, vj, p.projectDBC)) {
+        if (upper_block(rows, bi, bj) && owns_row(p, vi) && !proj_dbc(p.dbc, vi, p.projectDBC) && !proj_dbc(p.dbc, vj, p.projectDBC)) {
             const int c0 = (vi == vj) ? r : 0;
             o = csr_find(p.ia, p.ja, p.base, 3 * vi + r, 3 * vj + c0);
             if (o < 0) o = -2;
@@ -570,18 +541,7 @@ __global__ void __launch_bounds__(32 * kScatWarps) k_barrier_hessian_scatter(Bar
             if (o == -2) atomicExch(err, 1);
             else if (o != -1) {
                 if (rows[bi] == rows[bj] && q < r) continue; // strictly lower part of a diagonal block
-                // (Q^T M Q)[i][j] = sum_{a,b} Q4[a][bi] Q4[b][bj] M[3a+r][3b+q]
-                double v = 0.0;
-                if (raw) v = H0[i * 12 + j];
-                else {
-#pragma unroll
-                    for (int ka = 0; ka < 3; ++ka) {
-                        const double qa = helmert(ka, bi);
-#pragma unroll
-                        for (int kb = 0; kb < 3; ++kb) v += (qa * helmert(kb, bj)) * H0[(3 * ka + r) * 9 + 3 * kb + q];
-                    }
-                }
-                atomicAdd(a + o + q, v);
+                atomicAdd(a + o + q, pair_hessian_entry(H0, raw, i, j));
             }
         }
     }
@@ -598,20 +558,9 @@ __global__ void __launch_bounds__(128) k_barrier_hessian_gather(BarrierArgs p, c
         repro_gather_row(v, p.rep.h, p.dbc, p.projectDBC, p.ia, p.ja, p.base, a, err, [&](int c, int bi, int bj, double* acc) {
             if (c >= n) return;
             const double* H0 = H + (size_t)c * 144;
-            if (psd[c] != 0) {
-                for (int r = 0; r < 3; ++r)
-                    for (int q = 0; q < 3; ++q) acc[3 * r + q] += H0[(3 * bi + r) * 12 + 3 * bj + q];
-                return;
-            }
+            const bool raw = psd[c] != 0;
             for (int r = 0; r < 3; ++r)
-                for (int q = 0; q < 3; ++q) {
-                    double t = 0.0;
-                    for (int ka = 0; ka < 3; ++ka) {
-                        const double qa = helmert(ka, bi);
-                        for (int kb = 0; kb < 3; ++kb) t += (qa * helmert(kb, bj)) * H0[(3 * ka + r) * 9 + 3 * kb + q];
-                    }
-                    acc[3 * r + q] += t;
-                }
+                for (int q = 0; q < 3; ++q) acc[3 * r + q] += pair_hessian_entry(H0, raw, 3 * bi + r, 3 * bj + q);
         });
 }
 
@@ -626,7 +575,7 @@ void barrier_gradient(const BarrierArgs& p, double* g, cudaStream_t st)
     if (p.rep.on) {
         if (p.kappa_dev) k_barrier_gradient<true, true><<<kSMs * 4, 128, 0, st>>>(p, p.rep.stage);
         else k_barrier_gradient<false, true><<<kSMs * 4, 128, 0, st>>>(p, p.rep.stage);
-        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 0ull, ~0ull, g, st);
+        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 0ull, kAllKeys, g, st);
     }
     else if (p.kappa_dev) k_barrier_gradient<true, false><<<kSMs * 4, 128, 0, st>>>(p, g);
     else k_barrier_gradient<false, false><<<kSMs * 4, 128, 0, st>>>(p, g);
@@ -636,19 +585,19 @@ void constraint_jacobian_t(const BarrierArgs& p, const double* input, double coe
 {
     if (p.rep.on) {
         k_constraint_jacobian_t<true><<<kSMs * 4, 128, 0, st>>>(p, input, coef, p.rep.stage);
-        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 0ull, 4ull * p.rep.cap, g, st); // the active list's contributions
+        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 0ull, para_keys(p.rep.cap), g, st); // the active list's contributions
     }
     else k_constraint_jacobian_t<false><<<kSMs * 4, 128, 0, st>>>(p, input, coef, g);
 }
 void para_gradient(const BarrierArgs& p, double* g, cudaStream_t st)
 {
     if (p.rep.on) {
-        if (p.kappa_dev) k_para_gradient<true, true><<<kSMs, 128, 0, st>>>(p, p.rep.stage);
-        else k_para_gradient<false, true><<<kSMs, 128, 0, st>>>(p, p.rep.stage);
-        repro_gather_g(p.nV, p.rep.g, p.rep.stage, 4ull * p.rep.cap, ~0ull, g, st); // the mollified list's contributions
+        if (p.kappa_dev) k_barrier_gradient<true, true, true><<<kSMs, 128, 0, st>>>(p, p.rep.stage);
+        else k_barrier_gradient<false, true, true><<<kSMs, 128, 0, st>>>(p, p.rep.stage);
+        repro_gather_g(p.nV, p.rep.g, p.rep.stage, para_keys(p.rep.cap), kAllKeys, g, st); // the mollified list's contributions
     }
-    else if (p.kappa_dev) k_para_gradient<true, false><<<kSMs, 128, 0, st>>>(p, g);
-    else k_para_gradient<false, false><<<kSMs, 128, 0, st>>>(p, g);
+    else if (p.kappa_dev) k_barrier_gradient<true, false, true><<<kSMs, 128, 0, st>>>(p, g);
+    else k_barrier_gradient<false, false, true><<<kSMs, 128, 0, st>>>(p, g);
 }
 void barrier_hessian_build_project(const BarrierArgs& p, int* flags, double* Hraw, int* rows, int* psd, int* n_owned, int capacity, cudaStream_t st)
 {

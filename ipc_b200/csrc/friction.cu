@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(128) k_friction_lag(BarrierArgs p, int4* __res
         const int4 mm = p.cs[c];
         const PairStencil s = decode(mm);
         V3 x[4];
-        for (int k = 0; k < s.nv; ++k) x[k] = load_vertex(p.V, p.nV, s.v[k]);
+        load_stencil(s, p.V, p.nV, x);
         const double d = pair_distance(s, x);
         if (!(d > 0.0)) atomicExch(bad, 1);
         double b, db, d2b;
@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(256) k_friction_energy(FrictionArgs p, double*
     cta_sum(&val, partials + blockIdx.x);
 }
 
-// kStage (reproducible mode): the vector of stencil vertex k of pair c goes to g[3 (4c + k) + q] of the staging array (k_repro_gather_g sums it)
+// kStage: the contributions go to the staging array under their gradient keys (repro.cuh)
 template <bool kStage>
 __global__ void __launch_bounds__(128) k_friction_gradient(FrictionArgs p, double* __restrict__ g)
 {
@@ -172,24 +172,14 @@ __global__ void __launch_bounds__(128) k_friction_gradient(FrictionArgs p, doubl
         else { const double s = f1_SF_div(x2, eps); u0 *= s; u1 *= s; }
         const V3 t = u0 * f.b0 + u1 * f.b1;
         const double cl = p.coef * p.lambda[c];
-        if (kStage) {
 #pragma unroll
-            for (int k = 0; k < 4; ++k) { // (unrolled with a guard: the stencil stays in registers)
-                if (k >= f.s.nv) continue;
-                const double wk = f.w[k] * cl;
-                double* out = g + 3 * (4 * (size_t)c + k);
-                out[0] = wk * t.x;
-                out[1] = wk * t.y;
-                out[2] = wk * t.z;
-            }
+        for (int k = 0; k < 4; ++k) { // (unrolled with a guard: the stencil stays in registers)
+            if (k >= f.s.nv) continue;
+            const double wk = f.w[k] * cl;
+            put_g<kStage>(g, f.s.v[k], gkey_active(c, k), 0, wk * t.x);
+            put_g<kStage>(g, f.s.v[k], gkey_active(c, k), 1, wk * t.y);
+            put_g<kStage>(g, f.s.v[k], gkey_active(c, k), 2, wk * t.z);
         }
-        else
-            for (int k = 0; k < f.s.nv; ++k) {
-                const double wk = f.w[k] * cl;
-                atomicAdd(g + 3 * (size_t)f.s.v[k], wk * t.x);
-                atomicAdd(g + 3 * (size_t)f.s.v[k] + 1, wk * t.y);
-                atomicAdd(g + 3 * (size_t)f.s.v[k] + 2, wk * t.z);
-            }
     }
 }
 

@@ -32,13 +32,6 @@ DEV double plane_d2(const double* __restrict__ par, const double* __restrict__ V
     const double dist = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(pl[0], x), __dmul_rn(pl[1], y)), __dmul_rn(pl[2], z)), pl[3]);
     return __dmul_rn(dist, dist);
 }
-DEV double pair_d2(const BarrierArgs& p, int4 mm)
-{
-    const PairStencil s = decode(mm);
-    V3 x[4];
-    for (int k = 0; k < s.nv; ++k) x[k] = load_vertex(p.V, p.nV, s.v[k]);
-    return pair_distance(s, x);
-}
 
 // the plane active set of postLineSearch / initKappa (nullptrs without planes)
 struct PlaneSet {
@@ -115,7 +108,7 @@ __global__ void __launch_bounds__(kKappaThreads) k_kappa_check(BarrierArgs p, Pl
     const int n_mm = min(st->kappa_n_close[0], cap_mm), n = n_mm + min(st->kappa_n_close[1], cap_hs);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const bool plane = i >= n_mm;
-        const double d = plane ? plane_d2(ps.par, p.V, p.nV, hs[i - n_mm]) : pair_d2(p, mm[i]);
+        const double d = plane ? plane_d2(ps.par, p.V, p.nV, hs[i - n_mm]) : pair_distance(mm[i], p.V, p.nV);
         if (d <= (plane ? hs_val[i - n_mm] : mm_val[i])) st->kappa_hit = 1;
     }
 }
@@ -152,7 +145,7 @@ __global__ void __launch_bounds__(kKappaThreads) k_kappa_snapshot(BarrierArgs p,
         const bool plane = i >= nC;
         const int4 e = plane ? make_int4(0, 0, 0, 0) : p.cs[i];
         const int2 q = plane ? ps.act[i - nC] : make_int2(0, 0);
-        const double d = plane ? plane_d2(ps.par, p.V, p.nV, q) : pair_d2(p, e);
+        const double d = plane ? plane_d2(ps.par, p.V, p.nV, q) : pair_distance(e, p.V, p.nV);
         dmin = fmin(dmin, d);
         if (!(d < dTol)) continue;
         if (!plane) {

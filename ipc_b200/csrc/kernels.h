@@ -156,11 +156,11 @@ __device__ __forceinline__ bool obstacle_vertex(const SurfArgs& s, int v) { retu
 // every vertex in ascending key order and adds the result to g once.  The Hessians go through a per-row gather of the same form.
 struct VertexIndex {
     const int* ptr;                  // nV + 1 starts: the entries of vertex v are key[ptr[v], ptr[v + 1]), ascending
-    const unsigned long long* key;   // gradient: contribution index; Hessian: column vertex << 32 | list index << 4 | block (bi << 2 | bj)
+    const unsigned long long* key;   // gradient key or Hessian block key (repro.cuh: gkey_*, hkey)
 };
 struct ReproArgs {
     int on = 0;                      // 0: the atomic scatter (levels 0 and 1); nothing below is read
-    int cap = 0;                     // list capacity: the active list's contributions are [0, 4 cap), the mollified list's [4 cap, 12 cap)
+    int cap = 0;                     // list capacity, which places the mollified list's gradient keys (repro.cuh: para_keys)
     double* stage = nullptr;         // per-contribution gradient vectors
     double* hstage = nullptr;        // friction Hessian: M (9) and the stencil weights (4) per pair
     VertexIndex g = {}, h = {};      // gradient and Hessian indices

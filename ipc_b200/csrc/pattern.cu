@@ -17,7 +17,7 @@
 //   6. only when changed: k_pattern_write merges mesh and extra neighbours of every vertex into ia / ja and keeps the extra lists for the
 //      next comparison; k_slot_offsets (elastic.cu) recomputes the CSR offsets of the elastic block slots.
 // Every launch has a size fixed by nV and the capacities and reads its counts and gates from device memory, so an update is capturable.
-#include "common.cuh"
+#include "pair_common.cuh"
 #include "abi.h"
 #include <algorithm>
 #include <cstddef>
@@ -48,17 +48,6 @@ DEV bool mesh_neighbour(const int* __restrict__ mptr, const int* __restrict__ mn
     return a < end && mnbr[a] == hi;
 }
 
-// vertices of a stencil: the first entry decoded (-v-1 -> v), the others where non-negative (negative ones are multiplicities)
-DEV int stencil_vertices(int4 q, int* v)
-{
-    int n = 0;
-    v[n++] = q.x < 0 ? -q.x - 1 : q.x;
-    if (q.y >= 0) v[n++] = q.y;
-    if (q.z >= 0) v[n++] = q.z;
-    if (q.w >= 0) v[n++] = q.w;
-    return n;
-}
-
 template <bool FILL>
 DEV void emit_pairs(const PatArgs& p, const int* v, int n, int* row_cnt, const int* row_off, int* bucket)
 {
@@ -79,18 +68,14 @@ __global__ void __launch_bounds__(256) k_pattern_keys(PatArgs p, int* __restrict
     const int nC = min(*p.nC, p.cap), nP = min(*p.nP, p.cap), nF = p.fr ? min(*p.nF, p.capF) : 0;
     const int total = nC + nP + nF;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        int v[4];
-        if (i < nC) emit_pairs<FILL>(p, v, stencil_vertices(p.cs[i], v), row_cnt, row_off, bucket);
-        else if (i < nC + nP) {
-            const int k = i - nC;
-            emit_pairs<FILL>(p, v, stencil_vertices(p.para[k], v), row_cnt, row_off, bucket);
-            const int2 e = p.para_e[k];
-            if (e.x >= 0 && e.y >= 0) { // the two edges of a mollified pair
-                v[0] = p.SE[2 * e.x]; v[1] = p.SE[2 * e.x + 1]; v[2] = p.SE[2 * e.y]; v[3] = p.SE[2 * e.y + 1];
-                emit_pairs<FILL>(p, v, 4, row_cnt, row_off, bucket);
-            }
+        const bool para = i >= nC && i < nC + nP;
+        const PairStencil s = decode(i < nC ? p.cs[i] : para ? p.para[i - nC] : p.fr[i - nC - nP]);
+        emit_pairs<FILL>(p, s.v, s.nv, row_cnt, row_off, bucket);
+        const int2 e = para ? p.para_e[i - nC] : make_int2(-1, -1);
+        if (e.x >= 0 && e.y >= 0) { // the two edges of a mollified pair
+            const int v[4] = { p.SE[2 * e.x], p.SE[2 * e.x + 1], p.SE[2 * e.y], p.SE[2 * e.y + 1] };
+            emit_pairs<FILL>(p, v, 4, row_cnt, row_off, bucket);
         }
-        else emit_pairs<FILL>(p, v, stencil_vertices(p.fr[i - nC - nP], v), row_cnt, row_off, bucket);
     }
 }
 

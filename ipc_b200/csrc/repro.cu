@@ -120,41 +120,27 @@ DEV void index_item(const IndexSrc& s, int t, int nC, Emit emit)
     const PairStencil ps = decode(mm);
     if (kMode == kIdxGrad) { // keys as k_barrier_gradient / k_friction_gradient stage them
         // (unrolled with a guard: the stencil arrays stay in registers)
-        if (!is_para) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if (k < ps.nv) emit(ps.v[k], 4ull * c + k);
-        }
-        else {
+        if (is_para) {
             int ev[4];
             para_edge_stencil(mm, s.para_e[c], s.SE, ev);
-            const unsigned long long b = 4ull * s.cap + 8ull * c;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) emit(ev[k], b + k);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if (k < ps.nv) emit(ps.v[k], b + 4 + k);
+            for (int k = 0; k < 4; ++k) emit(ev[k], gkey_para_edge(s.cap, c, k));
         }
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (k < ps.nv) emit(ps.v[k], is_para ? gkey_para_dist(s.cap, c, k) : gkey_active(c, k));
     }
     else if (kMode == kIdxBarrierH) { // the blocks k_barrier_hessian_scatter adds, slot t (active, then mollified) of the fixed-slot build
         if (t >= s.cap) return;        // (beyond the slots: the build raises FLAG_SET_CAPACITY)
         int rows[4];
-        if (!is_para)
-            for (int k = 0; k < 4; ++k) rows[k] = (k < ps.nv) ? ps.v[k] : -1;
-        else para_edge_stencil(mm, s.para_e[c], s.SE, rows);
+        hessian_rows(mm, ps, is_para, s.para_e, c, s.SE, rows);
         for (int bi = 0; bi < 4; ++bi)
-            for (int bj = 0; bj < 4; ++bj) {
-                const int vi = rows[bi], vj = rows[bj];
-                if (vi >= 0 && vj >= 0 && vi <= vj && !(vi == vj && bi != bj))
-                    emit(vi, ((unsigned long long)vj << 32) | ((unsigned)t << 4) | (unsigned)(bi << 2 | bj));
-            }
+            for (int bj = 0; bj < 4; ++bj)
+                if (upper_block(rows, bi, bj)) emit(rows[bi], hkey(rows[bj], t, bi, bj));
     }
     else { // the blocks k_friction_hessian adds
         for (int bi = 0; bi < ps.nv; ++bi)
-            for (int bj = bi; bj < ps.nv; ++bj) {
-                const int vi = min(ps.v[bi], ps.v[bj]), vj = max(ps.v[bi], ps.v[bj]);
-                emit(vi, ((unsigned long long)vj << 32) | ((unsigned)c << 4) | (unsigned)(bi << 2 | bj));
-            }
+            for (int bj = bi; bj < ps.nv; ++bj) emit(min(ps.v[bi], ps.v[bj]), hkey(max(ps.v[bi], ps.v[bj]), c, bi, bj));
     }
 }
 // kScatter false: cnt[v] += entries of v; true: key[atomicAdd(cur[v], 1)] = key (the order inside a vertex is fixed by k_index_sort)
