@@ -326,7 +326,13 @@ int ipcgpu_end_time_step(ipcgpu_ctx* ctx);
  * state that fails a check at step 0 gives IPCGPU_ERR_LINE_SEARCH with V = V0.  Results: the stage steps in ipcgpu_iteration (alpha_inversion,
  * alpha_halfspace, alpha_swept_grid, alpha_full_ccd), the accepted step as the device-resident step, the halvings and the status in
  * ipcgpu_step_control (alpha_feasible = alpha = the accepted step).  alpha_out NULL: deferred and capturable (conditional nodes; run it once
- * outside a capture first); otherwise synchronises and returns the accepted step.  Option 5 or out of range: IPCGPU_ERR_ARG.  Single rank. */
+ * outside a capture first); otherwise synchronises and returns the accepted step.  Option 5 (Jacobi, :1082-1110): p_i = -g_i / H_ii from the
+ * device-resident gradient and matrix, one division per row as ipcgpu_precondition_diag, and p = 0 on Dirichlet vertices and the obstacle tail;
+ * the caller assembles g and H at the entry state first (computeGradient(result, true, g) and computePrecondMtr(result, false, ...), :1084-1088:
+ * the calls at the head of a Newton iteration), and the call reads what is resident.  Option 5 on a context without a sparsity pattern
+ * (neither ipcgpu_set_csr nor ipcgpu_enable_device_pattern: no linear system) is refused with IPCGPU_ERR_ARG, as it always was; with a
+ * pattern but no gradient and matrix assembled since the last ipcgpu_set_state, ipcgpu_set_mesh or pattern change: IPCGPU_ERR_STATE.
+ * Option 5 needs no time integration.  Options outside 0-5: IPCGPU_ERR_ARG.  Single rank. */
 int ipcgpu_warm_start(ipcgpu_ctx* ctx, int option, double voxel_size, double tolerance, const double err_vf[3], const double err_ee[3], double* alpha_out);
 
 /* ---- Rayleigh damping, Neumann forces and the augmented-Lagrangian Dirichlet penalty: the last terms of Optimizer::computeEnergyVal /
@@ -645,6 +651,20 @@ typedef struct ipcgpu_solve_result {
 } ipcgpu_solve_result;
 /* synchronises only when a solve was enqueued since the last read; returns out->status */
 int ipcgpu_solve_info(ipcgpu_ctx* ctx, ipcgpu_solve_result* out);
+/* LinSysSolver::precondition_diag (LinSysSolver.hpp:411-420) on the device-resident gradient g and CSR values a (host or device-built
+ * pattern): out_i = (sign g_i) / a(i,i) for every row, a(i,i) the first stored entry of row i, one correctly rounded division with no fused
+ * operation (bit-identical to numpy's (sign * g) / diag).  sign = -1: computeSearchDir's direction when useGD is set or the factorization
+ * fails (Optimizer.cpp:2331-2346); sign = +1: the friction convergence test's (:1724), which compares max_abs_x with targetGRes.  The
+ * caller decides when to take it.  Rows are not skipped: with projectDBC = 1 the Dirichlet and obstacle rows are identity rows, divided by 1
+ * (0 where the projected terms leave their gradient at 0); in penalty mode (projectDBC = 0) they are divided like any other row.  A zero or negative diagonal is divided, not
+ * clamped, as the reference divides it; only a non-finite entry (a zero diagonal under a nonzero gradient, a NaN) fails the result.
+ * adopt_as_search_dir != 0: out becomes the search direction exactly as ipcgpu_solve_pcg's adopted solution does.  x != NULL: synchronises,
+ * copies out (3 nV doubles) and returns IPCGPU_ERR_SOLVE for a non-finite result.  x NULL: deferred and capturable (run it once outside a
+ * capture first); a non-finite result raises IPCGPU_ERR_SOLVE as a failed deferred solve does.  Either way ipcgpu_solve_info reads the
+ * result: iterations = 0, rel_residual = 0, max_abs_x = max_i |out_i| (the solvers' exact maximum; NaN entries skipped), status.
+ * IPCGPU_ERR_STATE without a gradient and a matrix assembled since the last ipcgpu_set_state, ipcgpu_set_mesh or pattern change, and on
+ * more than one rank; IPCGPU_ERR_ARG for a sign other than +1 / -1. */
+int ipcgpu_precondition_diag(ipcgpu_ctx* ctx, int sign, double* x, int adopt_as_search_dir);
 /* what the last multilevel solve built: number of levels, domains per level (8 entries, 0 beyond the last level), bytes of the stored
  * inverses; any pointer may be NULL.  IPCGPU_ERR_STATE before the first ipcgpu_solve_pcg_multilevel and after one that failed. */
 int ipcgpu_multilevel_info(ipcgpu_ctx* ctx, int* levels, int64_t* domains_per_level, uint64_t* bytes);

@@ -275,6 +275,8 @@ int solver_multilevel_build(ipcgpu_ctx* ctx, double* bad_pivot); // the hierarch
 void solver_multilevel_step(ipcgpu_ctx* ctx, bool start);        // (iteration: the CG update first) z = M^-1 r, partials of r.z and r.r
 int solver_multilevel_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count);
 int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src); // src NULL: the direction already in ctx->dir
+// (sign g_i) / a(i,i) into out; jacobi: initX option 5's predictor (0 on Dirichlet vertices and the obstacle tail, no status words)
+void solver_precondition_diag(ipcgpu_ctx* ctx, double sign, double* out, bool jacobi);
 int pattern_enable(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_capacity);
 int pattern_update(ipcgpu_ctx* ctx, const ipcgpu::BarrierArgs& lists, bool with_friction);
 int safeguard_inversion(ipcgpu_ctx* ctx);

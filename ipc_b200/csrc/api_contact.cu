@@ -375,6 +375,7 @@ int ipcgpu_enable_device_pattern(ipcgpu_ctx* ctx, int index_base, uint64_t nnz_c
     ctx->pat_changed_host = 0;
     ctx->a_all_dirty = false;
     ctx->offsets_ready = false;
+    ctx->g_assembled = ctx->a_assembled = false;
     owned_value_range(ctx);
     if ((rc = solver_forget_full_pattern(ctx))) return rc;
     return ensure_offsets(ctx);
@@ -389,6 +390,7 @@ int ipcgpu_update_pattern(ipcgpu_ctx* ctx, int with_friction, int* changed, int6
     int rc = pattern_update(ctx, barrier_args(ctx, 1.0, 1.0, 0), with_friction != 0);
     if (rc) return rc;
     ctx->pat_pending = true;
+    ctx->g_assembled = ctx->a_assembled = false;
     if (!changed && !nnz) return IPCGPU_OK;
     if ((rc = sync_pattern_mirror(ctx))) return rc;
     if (changed) *changed = ctx->pat_changed_host;

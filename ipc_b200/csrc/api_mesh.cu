@@ -232,6 +232,7 @@ int ipcgpu_set_mesh(ipcgpu_ctx* ctx, int nV, int nT, const double* Vrest, const 
     ctx->device_pattern = ctx->pat_pending = false;
     ctx->surface_ready = false;
     ctx->dir_valid = false;
+    ctx->g_assembled = ctx->a_assembled = false;
     // Dm^-1: reference layout is per-tet column-major; device layout is SoA over the row-major index q=3i+j
     std::vector<double> A((size_t)9 * std::max(nT, 1));
     for (int t = 0; t < nT; ++t)
@@ -273,6 +274,7 @@ int ipcgpu_set_csr(ipcgpu_ctx* ctx, int n_rows, const int* ia, const int* ja, in
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->a_all_dirty = false;
     ctx->offsets_ready = false;
+    ctx->g_assembled = ctx->a_assembled = false;
     owned_value_range(ctx);
     return solver_forget_full_pattern(ctx);
 }
@@ -283,6 +285,7 @@ int ipcgpu_set_state(ipcgpu_ctx* ctx, const double* V)
     ENTER(kSerial);
     if (V) CK(cudaMemcpyAsync(ctx->V.p, V, (size_t)3 * ctx->nV * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     ctx->mark_inputs();
+    ctx->g_assembled = ctx->a_assembled = false;
     return IPCGPU_OK;
 }
 
@@ -361,6 +364,8 @@ static int run_grad_hess(ipcgpu_ctx* ctx, double coef, int projectSPD, int proje
     }
     elastic_grad_hess(ctx->eargs(), coef, projectSPD, need_g, need_h, ctx->gcont.p, ctx->hblk.p, st, e_part);
     ctx->hblk_valid = need_h;
+    ctx->g_assembled = ctx->g_assembled || need_g;
+    ctx->a_assembled = ctx->a_assembled || need_h;
     ctx->prof_end(pe);
     ++ctx->launches;
     if (with_energy) { // (which rank's share it is: energy_result, once the call knows whether the host wants it)
@@ -524,6 +529,41 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
 int ipcgpu_solve_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
 {
     return solve_pcg(ctx, true, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
+}
+
+// LinSysSolver::precondition_diag on the resident system: computeSearchDir's fallback (sign -1, Optimizer.cpp:2331-2346) and the friction
+// convergence test's (sign +1, :1724).  Its result takes the solvers' words (kSolveStart with |b|^2 = 0: 0 iterations, rel_residual 0) and
+// their max |x_i| (solver_finish), so ipcgpu_solve_info reads it as it reads a solve's.
+int ipcgpu_precondition_diag(ipcgpu_ctx* ctx, int sign, double* x, int adopt_as_search_dir)
+{
+    REQUIRE(sign == 1 || sign == -1, IPCGPU_ERR_ARG, "ipcgpu_precondition_diag: sign must be +1 or -1");
+    REQUIRE(ctx->nnz > 0 && ctx->n_rows == 3 * ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
+    REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the diagonal preconditioning runs on one rank, like the built-in solvers");
+    REQUIRE(ctx->g_assembled && ctx->a_assembled, IPCGPU_ERR_STATE,
+        "no gradient and matrix assembled since the last ipcgpu_set_state, ipcgpu_set_mesh or pattern change");
+    REQUIRE(!x || !ctx->capturing, IPCGPU_ERR_STATE, "inside a capture the diagonal preconditioning takes its deferred form: x NULL");
+    const int n = ctx->n_rows;
+    REQUIRE(!ctx->capturing || (ctx->sol.n >= (size_t)n && ctx->pcg_scal.n >= 8), IPCGPU_ERR_STATE,
+        "run ipcgpu_precondition_diag once outside a capture first (it sizes its workspace)");
+    ENTER(kSerial);
+    REQUIRE(ctx->sol.reserve(n) && ctx->pcg_scal.reserve(8), IPCGPU_ERR_CUDA, "diagonal preconditioning workspace allocation failed");
+    CK(cudaMemsetAsync(ctx->pcg_scal.p, 0, 8 * sizeof(double), ctx->stream));
+    int rc = decide(ctx, kSolveStart, 0.0, 0, 0, nullptr, ctx->pcg_scal.p);
+    if (rc) return rc;
+    solver_precondition_diag(ctx, (double)sign, ctx->sol.p, false);
+    CK(cudaGetLastError());
+    if ((rc = solver_finish(ctx))) return rc;
+    ctx->sv_pending = true;
+    if (adopt_as_search_dir && (rc = solver_adopt_direction(ctx, ctx->sol.p))) return rc;
+    if (x) { // the host form reports a non-finite result by its return value alone, as the solvers' host forms do: no deferred flag
+        IterState& h = *ctx->h_iter;
+        CK(cudaMemcpyAsync(x, ctx->sol.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(&h.sv_status, &ctx->iter.p->sv_status, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        if (h.sv_status != 0) CK(cudaMemsetAsync(&ctx->iter.p->flags[FLAG_SOLVE], 0, sizeof(int), ctx->stream));
+        REQUIRE(h.sv_status == 0, IPCGPU_ERR_SOLVE, "diagonal preconditioning: a non-finite entry (a zero or non-finite diagonal or gradient entry)");
+    }
+    return IPCGPU_OK;
 }
 
 int ipcgpu_solve_info(ipcgpu_ctx* ctx, ipcgpu_solve_result* out)

@@ -58,6 +58,8 @@ static ipcgpu_ctx::HostState snapshot_host_state(const ipcgpu_ctx* ctx)
     h.hs_lag_ready = ctx->hs_lag_ready;
     h.rep_lists = ctx->rw.lists_ready;
     h.rep_fr = ctx->rw.fr_ready;
+    h.g_assembled = ctx->g_assembled;
+    h.a_assembled = ctx->a_assembled;
     return h;
 }
 static void apply_host_state(ipcgpu_ctx* ctx, const ipcgpu_ctx::HostState& h)
@@ -75,6 +77,8 @@ static void apply_host_state(ipcgpu_ctx* ctx, const ipcgpu_ctx::HostState& h)
     ctx->hs_lag_ready = h.hs_lag_ready;
     ctx->rw.lists_ready = h.rep_lists;
     ctx->rw.fr_ready = h.rep_fr;
+    ctx->g_assembled = h.g_assembled;
+    ctx->a_assembled = h.a_assembled;
 }
 
 int ipcgpu_capture_begin(ipcgpu_ctx* ctx)
@@ -456,21 +460,30 @@ int ipcgpu_line_search(ipcgpu_ctx* ctx, const ipcgpu_line_search_terms* t, doubl
     return alpha_inout ? step_control_host_result(ctx, alpha_inout) : IPCGPU_OK;
 }
 
-// Optimizer::initX (:925-1233) for options 0-4 with the barrier solver (solveIP): the predictor becomes the search direction, its step is
+// Optimizer::initX (:925-1233) for options 0-5 with the barrier solver (solveIP): the predictor becomes the search direction, its step is
 // bounded (inversion filter, planes with slackness 0.9, swept hash + full CCD: initX always takes the full CCD, :1132) and applied with the
 // two backtracking loops of the line search (kLsInversion, kLsIntersection).  Nothing here synchronises outside the host loops of cond_node.
+// Option 5 (Jacobi, :1082-1110) divides the resident gradient by the resident matrix's diagonal, which the caller assembled at this state.
 int ipcgpu_warm_start(ipcgpu_ctx* ctx, int option, double voxel_size, double tol, const double err_vf[3], const double err_ee[3], double* alpha_out)
 {
-    REQUIRE(option >= 0 && option <= 4, IPCGPU_ERR_ARG, "warm start option 0-4 (initX option 5, Jacobi, is not supported)");
+    REQUIRE(option >= 0 && option <= 5, IPCGPU_ERR_ARG, "warm start option 0-5");
+    // (a context without a sparsity pattern holds no linear system: option 5 is no option of it, as before the Jacobi predictor existed)
+    REQUIRE(option != 5 || (ctx->nnz > 0 && ctx->n_rows == 3 * ctx->nV), IPCGPU_ERR_ARG,
+        "warm start option 5 needs a linear system: ipcgpu_set_csr or ipcgpu_enable_device_pattern first");
     REQUIRE(option == 0 || (err_vf && err_ee && voxel_size > 0.0), IPCGPU_ERR_ARG, "the warm start needs the Tight-Inclusion errors and a positive voxel size");
     REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the warm start runs on one rank");
     REQUIRE(ctx->surface_ready && ctx->maps_ready, IPCGPU_ERR_STATE, "ipcgpu_set_mesh and ipcgpu_set_surface first");
+    REQUIRE(option != 5 || (ctx->g_assembled && ctx->a_assembled), IPCGPU_ERR_STATE,
+        "warm start option 5: assemble the gradient and the matrix at the entry state first (since the last ipcgpu_set_state, ipcgpu_set_mesh or pattern change)");
     ENTER(kSerial);
-    DynamicsArgs dyn;
-    int rc = timestep_prepare(ctx, &dyn);
-    if (rc) return rc;
-    timestep_predictor(dyn, option, ctx->dir.p, ctx->stream);
-    ++ctx->launches;
+    int rc;
+    if (option == 5) solver_precondition_diag(ctx, -1.0, ctx->dir.p, true);
+    else {
+        DynamicsArgs dyn;
+        if ((rc = timestep_prepare(ctx, &dyn))) return rc;
+        timestep_predictor(dyn, option, ctx->dir.p, ctx->stream);
+        ++ctx->launches;
+    }
     CK(cudaGetLastError());
     if ((rc = solver_adopt_direction(ctx, nullptr)) || (rc = step_control_prepare(ctx))) return rc;
     if ((rc = decide(ctx, kWsEntry, option ? 1.0 : 0.0, 0, 0, nullptr))) return rc; // stepSize = 1.0 (:1123)

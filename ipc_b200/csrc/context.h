@@ -329,6 +329,9 @@ struct ipcgpu_ctx {
     ipcgpu::MultilevelWork ml;
     uint64_t solve_epoch[2] = { ~0ull, ~0ull };
     bool sv_pending = false, sv_pending_at_capture = false;
+    // an elastic gradient / Hessian call wrote g / a since the last ipcgpu_set_state, ipcgpu_set_mesh or pattern change: what the diagonal
+    // preconditioning (ipcgpu_precondition_diag, ipcgpu_warm_start option 5) reads is the system at the current state
+    bool g_assembled = false, a_assembled = false;
 
     // work / result buffers
     ipcgpu::DevBuf<double> gcont, hblk, g, e_per_tet, partials, inv_steps, dir, in_partials, e_partials2;
@@ -341,6 +344,7 @@ struct ipcgpu_ctx {
     struct HostState {
         unsigned local_scalars;
         bool lists_local, lists_global, want_cand, swept_ready, fr_ready, inputs_marked, scatter_marked, hs_set_built, hs_lag_ready, rep_lists, rep_fr;
+        bool g_assembled, a_assembled;
         int nC, nP, nK, fr_host_n;
     };
     struct GraphRec {

@@ -28,6 +28,7 @@
 #include "common.cuh"
 #include "abi.h"
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cub/cub.cuh>
 
@@ -161,6 +162,24 @@ __global__ void __launch_bounds__(256) k_pcg_direction(int n, const double* __re
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const double beta = scal[5];
     if (i < n) p[i] = z[i] + beta * p[i];
+}
+
+// out_i = (sign g_i) / a(i,i) on every row (LinSysSolver::precondition_diag, LinSysSolver.hpp:411-420): the diagonal is the first stored
+// entry of its row, read as k_block_jacobi reads it, and the quotient is one correctly rounded division, as the reference's.  Rows of
+// vertices flagged in dbc (nullable) or from v_fixed on are 0 (initX option 5, Optimizer.cpp:1096-1097).  st != NULL: a non-finite entry
+// fails the result as a solve fails (step_control.cu: solve_fail)
+__global__ void __launch_bounds__(256) k_precondition_diag(int n, const int* __restrict__ ia, int base, const double* __restrict__ a,
+    const double* __restrict__ g, double sign, const uint8_t* __restrict__ dbc, int v_fixed, double* __restrict__ out, IterState* __restrict__ st)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int v = i / 3;
+    const double r = (v >= v_fixed || (dbc && dbc[v])) ? 0.0 : (sign * g[i]) / a[ia[i] - base];
+    out[i] = r;
+    if (st && !isfinite(r)) {
+        st->sv_status = IPCGPU_ERR_SOLVE;
+        st->flags[FLAG_SOLVE] = 1;
+    }
 }
 
 // max |x_i| (exact, so the order does not matter; NaN entries are skipped)
@@ -315,6 +334,16 @@ int solver_finish(ipcgpu_ctx* ctx)
     ++ctx->launches;
     CK(cudaGetLastError());
     return IPCGPU_OK;
+}
+
+// the diagonally preconditioned gradient into `out` (3 nV), one thread per row.  jacobi: initX option 5's predictor (0 on Dirichlet vertices
+// and the obstacle tail; no status); otherwise the result ipcgpu_precondition_diag reports, whose status words kSolveStart has reset
+void solver_precondition_diag(ipcgpu_ctx* ctx, double sign, double* out, bool jacobi)
+{
+    const int n = ctx->n_rows;
+    k_precondition_diag<<<nblk(n, 256), 256, 0, ctx->stream>>>(n, ctx->ia.p, ctx->index_base, ctx->a.p, ctx->g.p, sign,
+        jacobi && ctx->has_dbc ? ctx->dbc.p : nullptr, jacobi ? ctx->nVdof : INT_MAX, out, jacobi ? nullptr : ctx->iter.p);
+    ++ctx->launches;
 }
 
 // block-Jacobi step (start: z = Minv r alone)

@@ -105,6 +105,7 @@ SIGNATURES = {
     "ipcgpu_solve_pcg": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
     "ipcgpu_solve_pcg_multilevel": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
     "ipcgpu_solve_info": (C.c_int, [_ctxp, C.c_void_p]),
+    "ipcgpu_precondition_diag": (C.c_int, [_ctxp, C.c_int, _dp, C.c_int]),
     "ipcgpu_multilevel_info": (C.c_int, [_ctxp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]),
     "ipcgpu_multilevel_debug_matrices": (C.c_int, [_ctxp, _dp, C.c_uint64]),
     "ipcgpu_allreduce_grad_hess": (C.c_int, [_ctxp, C.c_int, C.c_int]),
@@ -947,6 +948,13 @@ class Context:
     def solve_pcg_multilevel(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False, deferred=False):
         """solve_pcg with the multilevel additive Schwarz preconditioner (rebuilt from the resident matrix and positions at every call)"""
         return self._solve(self.lib.ipcgpu_solve_pcg_multilevel, rhs, rel_tol, max_iter, want_x, adopt, deferred)
+
+    def precondition_diag(self, sign=-1, want_x=True, adopt=False):
+        """(sign g_i) / a(i,i) over the resident gradient and CSR values; want_x=True returns it (3 nV), want_x=False is deferred and
+        capturable and returns None.  Either way solve_info() reads max_abs_x and the status"""
+        x = np.empty(3 * self.nV) if want_x else None
+        self._ck(self.lib.ipcgpu_precondition_diag(self.h, int(sign), _d(x), int(adopt)))
+        return x
 
     def solve_info(self):
         """ipcgpu_solve_result of the last solve (its status is out.status, not raised)"""
