@@ -144,8 +144,7 @@ int ipcgpu_step_bound_set(ipcgpu_ctx* ctx, double alpha);
  * list sizes and step bounds -- they live in device memory and are read at replay time.  So one capture serves every Newton iteration
  * of a solve; capture again after ipcgpu_set_mesh / _set_surface / _set_csr / _set_*_capacity / _comm_init / _set_canonical_order /
  * _set_contact_partition (older graphs are refused with IPCGPU_ERR_STATE) or when dHat / a host kappa change (IPCGPU_KAPPA_DEVICE is read at replay).  Run the sequence once eagerly
- * before capturing it (lazy allocations), with ipcgpu_set_canonical_order(ctx, 0) or (ctx, 2): the level-1 sort of the contact lists needs
- * their sizes on the host.  Collective: with several ranks every rank captures and launches the same sequence.
+ * before capturing it (lazy allocations).  Collective: with several ranks every rank captures and launches the same sequence.
  * ipcgpu_fetch_iteration stays outside the graph. */
 int ipcgpu_capture_begin(ipcgpu_ctx* ctx);
 int ipcgpu_capture_end(ipcgpu_ctx* ctx, int* graph_id);
@@ -238,13 +237,13 @@ int ipcgpu_constraint_set(ipcgpu_ctx* ctx, double dHat, int getPTEE, int* nC, in
 int ipcgpu_constraint_set_sizes(ipcgpu_ctx* ctx, int* nC, int* nPara, int* nCand);
 /* Order of the contact lists and of the contact sums.
  * level=1 (default): the lists are returned in canonical (lexicographic) order, so two runs give bitwise identical sets.  The sorts are
- *   sized on the host: refused inside a capture.
+ *   sized on the device (the counts are read there), so this level runs inside a capture as well.
  * level=0: the order is whatever the atomic appends produced -- the same freedom the reference has (its order depends on
  *   unordered_set iteration and TBB scheduling); saves the sorting passes when the sets are only consumed on the device.
- * level=2 (reproducible mode): the canonical order of level 1 from device-sized sorts wherever a list is produced (the constraint set,
- *   ipcgpu_set_constraint_set, ipcgpu_friction_lag, ipcgpu_set_friction_data), inside a capture as well, and every contact term (barrier,
- *   mollified, Jacobian^T, friction, planes; E, g and H) summed in an order fixed by the lists alone, with no floating-point atomic on g or
- *   the CSR values: a captured time step gives the same bits on every run and for every order the lists were handed in.  Lists built
+ * level=2 (reproducible mode): the canonical order of level 1 wherever a list is produced (the constraint set, ipcgpu_set_constraint_set,
+ *   ipcgpu_friction_lag, ipcgpu_set_friction_data), and every contact term (barrier, mollified, Jacobian^T, friction, planes; E, g and H)
+ *   summed in an order fixed by the lists alone, with no floating-point atomic on g or the CSR values: a captured time step gives the
+ *   same bits on every run and for every order the lists were handed in.  Lists built
  *   before the switch keep their order until they are built again.  One rank only (IPCGPU_ERR_STATE otherwise); a pair capacity of at
  *   most 2^27.  Every level change refuses older graphs. */
 int ipcgpu_set_canonical_order(ipcgpu_ctx* ctx, int level);

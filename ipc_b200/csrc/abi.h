@@ -154,6 +154,13 @@ struct SortedGrid; // broadphase.cuh
 int contact_alloc(ipcgpu_ctx* ctx);
 int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, int* nPara, int* nCand);
 int contact_sync_counts(ipcgpu_ctx* ctx);
+int contact_scan(ipcgpu_ctx* ctx, const int* in, int* out, int n); // exclusive sum of n ints through the cub_tmp scratch
+// canonical order (lexicographic on the signed components, companion last) of a list of min(*n, cap) entries, sized on the device:
+// lex_order leaves the sorting permutation in ContactWork::perm, permute applies it to the list or a companion of `words` 8-byte words
+int lex_order(ipcgpu_ctx* ctx, const int4* list, const int2* comp, const int* n, int cap);
+int lex_order(ipcgpu_ctx* ctx, const int2* list, const int* n, int cap);
+void permute(ipcgpu_ctx* ctx, void* data, int words, const int* n, int cap);
+int contact_sort_lists(ipcgpu_ctx* ctx); // act, para + para_e and (want_cand) cand in canonical order
 void contact_pack_lists(ipcgpu_ctx* ctx);
 void contact_unpack_lists(ipcgpu_ctx* ctx);
 ipcgpu::SurfArgs surf_args(const ipcgpu_ctx* ctx);
@@ -164,7 +171,7 @@ ipcgpu::SortedGrid edge_grid(const ipcgpu_ctx* ctx);
 // ---- repro.cu: the reproducible mode (canonical order level 2) -----------------------------------------------------------------------
 int repro_alloc(ipcgpu_ctx* ctx);                        // its workspace, sized by the pair capacity and the mesh (outside a capture)
 bool repro_on(const ipcgpu_ctx* ctx);                    // level 2 on one rank, workspace allocated
-int repro_contact_lists(ipcgpu_ctx* ctx);                // act / para in canonical order (device-sized), their gather indices
+int repro_contact_lists(ipcgpu_ctx* ctx);                // the gather indices of act / para (in canonical order)
 int repro_friction_list(ipcgpu_ctx* ctx, bool sort);     // fr_cs (+ companions) in canonical order if `sort`, its gather indices
 ipcgpu::ReproArgs repro_barrier_args(ipcgpu_ctx* ctx);   // on = 0 unless the indices belong to the lists in act / para
 ipcgpu::ReproArgs repro_friction_args(ipcgpu_ctx* ctx);  // ... to the list in fr_cs

@@ -324,7 +324,8 @@ int ipcgpu_set_constraint_set(ipcgpu_ctx* ctx, int nC, const int* mm, int nP, co
     w.lists_global = false;
     ctx->rw.lists_ready = false;
     if (repro_on(ctx)) {
-        int rc = repro_contact_lists(ctx);
+        int rc = contact_sort_lists(ctx);
+        if (!rc) rc = repro_contact_lists(ctx);
         if (rc) return rc;
     }
     ctx->mark_inputs();

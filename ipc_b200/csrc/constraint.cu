@@ -5,9 +5,9 @@
 // (:2411-2424) and the serial std::map merge with PP/PE multiplicities (:2434-2476), including the three sentinel
 // encodings for nearly parallel edge pairs (:2305-2311, :2383-2388, :2455-2468).
 //
-// Pipeline (one stream, one host sync at the end to return the counts):
+// Pipeline (one stream; a host sync only when the caller asks for the counts):
 //   boxes+bounds -> grid params -> emit (cell,id) -> CUB radix sort -> PT / EE queries (atomic append)
-//   -> run-length merge of PP/PE duplicates -> canonical lexicographic sort of every output list.
+//   -> merge of PP/PE duplicates -> canonical order of every output list (levels 1 and 2, sized on the device: lex_order / permute).
 // The output ORDER is canonical (sorted), unlike the reference whose order depends on unordered_set iteration and TBB
 // scheduling (:2176, :2282 "different constraint order will result in numerically different results").
 #include "broadphase.cuh"
@@ -559,56 +559,91 @@ __global__ void __launch_bounds__(128) k_classify_ee(SurfArgs s, const int2* __r
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// lexicographic sorts (signed int components) via stable LSD radix passes on packed 64-bit keys
+// canonical order of a contact list, sized on the device: lexicographic on the signed components, the companion (eI, eJ) last.  A bucket
+// pass on the first component (count, exclusive scan, scatter of positions; x + nV is the bucket: x is -v - 1 in the PT/PP/PE encodings
+// and in the PT candidates, a vertex or an edge index otherwise), then an insertion sort of every bucket on the rest.
 // ------------------------------------------------------------------------------------------------------------
-DEV unsigned long long pack2(int hi, int lo) { return ((unsigned long long)((unsigned)hi ^ 0x80000000u) << 32) | (unsigned long long)((unsigned)lo ^ 0x80000000u); }
-
-__global__ void k_iota(int n, int* idx)
+constexpr int kLexBlocks = kSMs * 4;
+DEV bool lex_less(int4 a, int2 ac, int4 b, int2 bc)
 {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) idx[i] = i;
+    if (a.y != b.y) return a.y < b.y;
+    if (a.z != b.z) return a.z < b.z;
+    if (a.w != b.w) return a.w < b.w;
+    if (ac.x != bc.x) return ac.x < bc.x;
+    return ac.y < bc.y;
 }
-__global__ void k_key_from4(int n, const int4* __restrict__ data, const int* __restrict__ idx, int which, unsigned long long* __restrict__ keys)
+DEV bool lex_less(int2 a, int2, int2 b, int2) { return a.y < b.y; }
+template <typename T>
+__global__ void __launch_bounds__(256) k_lex_count(const T* __restrict__ list, const int* __restrict__ n_ptr, int cap, int nV, int* __restrict__ cnt)
 {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int4 v = data[idx[i]];
-    keys[i] = which ? pack2(v.x, v.y) : pack2(v.z, v.w);
-}
-__global__ void k_key_from2(int n, const int2* __restrict__ data, const int* __restrict__ idx, unsigned long long* __restrict__ keys)
-{
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int2 v = data[idx[i]];
-    keys[i] = pack2(v.x, v.y);
+    const int n = min(*n_ptr, cap);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) atomicAdd(cnt + list[i].x + nV, 1);
 }
 template <typename T>
-__global__ void k_gather(int n, const T* __restrict__ src, const int* __restrict__ idx, T* __restrict__ dst)
+__global__ void __launch_bounds__(256) k_lex_scatter(const T* __restrict__ list, const int* __restrict__ n_ptr, int cap, int nV, int* __restrict__ cur,
+    int* __restrict__ perm)
 {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dst[i] = src[idx[i]];
+    const int n = min(*n_ptr, cap);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) perm[atomicAdd(cur + list[i].x + nV, 1)] = i;
+}
+// one thread per bucket: insertion sort of its positions on (y, z, w, companion)
+template <typename T>
+__global__ void __launch_bounds__(256) k_lex_bucket_sort(int nB, const int* __restrict__ off, const T* __restrict__ list, const int2* __restrict__ comp,
+    int* __restrict__ perm)
+{
+    for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nB; b += gridDim.x * blockDim.x) {
+        const int s = off[b], e = off[b + 1];
+        for (int i = s + 1; i < e; ++i) {
+            const int pi = perm[i];
+            const T key = list[pi];
+            const int2 kc = comp ? comp[pi] : make_int2(0, 0);
+            int j = i - 1;
+            while (j >= s) {
+                const int pj = perm[j];
+                if (!lex_less(key, kc, list[pj], comp ? comp[pj] : make_int2(0, 0))) break;
+                perm[j + 1] = pj;
+                --j;
+            }
+            perm[j + 1] = pi;
+        }
+    }
+}
+// dst[i] = src[perm[i]] for i < n, `words` 8-byte words per element (k_copy_words then copies dst back)
+__global__ void __launch_bounds__(256) k_permute_words(const unsigned long long* __restrict__ src, const int* __restrict__ perm, const int* __restrict__ n_ptr,
+    int cap, int words, unsigned long long* __restrict__ dst)
+{
+    const long long n = (long long)min(*n_ptr, cap) * words;
+    for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[(long long)perm[i / words] * words + i % words];
+}
+__global__ void __launch_bounds__(256) k_copy_words(const unsigned long long* __restrict__ src, const int* __restrict__ n_ptr, int cap, int words,
+    unsigned long long* __restrict__ dst)
+{
+    const long long n = (long long)min(*n_ptr, cap) * words;
+    for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i];
 }
 // heads of runs of equal (x,y,z) in a sorted dup list emit (x,y,z,-count) into the active list (:2434-2476)
-__global__ void k_merge_dups(int n, const int4* __restrict__ sorted, int4* __restrict__ act, int* __restrict__ nAct, int cap, int* __restrict__ overflow)
+__global__ void __launch_bounds__(256) k_merge_dups(const int* __restrict__ n_ptr, int cap, const int4* __restrict__ sorted, int4* __restrict__ act, int* __restrict__ nAct,
+    int* __restrict__ overflow)
 {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int4 v = sorted[i];
-    if (i > 0) {
-        const int4 u = sorted[i - 1];
-        if (u.x == v.x && u.y == v.y && u.z == v.z) return;
+    const int n = min(*n_ptr, cap);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int4 v = sorted[i];
+        if (i > 0) {
+            const int4 u = sorted[i - 1];
+            if (u.x == v.x && u.y == v.y && u.z == v.z) continue;
+        }
+        int cnt = 1;
+        while (i + cnt < n) {
+            const int4 w = sorted[i + cnt];
+            if (w.x != v.x || w.y != v.y || w.z != v.z) break;
+            ++cnt;
+        }
+        push4(act, nAct, cap, overflow, make_int4(v.x, v.y, v.z, -cnt));
     }
-    int cnt = 1;
-    while (i + cnt < n) {
-        const int4 w = sorted[i + cnt];
-        if (w.x != v.x || w.y != v.y || w.z != v.z) break;
-        ++cnt;
-    }
-    push4(act, nAct, cap, overflow, make_int4(v.x, v.y, v.z, -cnt));
 }
 
 // sort-free variant of the same merge for meshes below 2^21 vertices: (x,y,z) packs into one 64-bit key, an open-addressing table
-// counts the multiplicities (2 short kernels instead of 16 radix passes over a list of a few thousand entries)
+// counts the multiplicities (2 short kernels instead of sorting the list)
 DEV unsigned long long dup_key(int4 v) { return ((unsigned long long)(unsigned)(-v.x - 1) << 42) | ((unsigned long long)(unsigned)v.y << 21) | (unsigned long long)(unsigned)(v.z + 1); }
 __global__ void k_dup_insert(const int* __restrict__ n_ptr, int cap, const int4* __restrict__ dup, unsigned long long* __restrict__ tab_key, int* __restrict__ tab_cnt,
     unsigned mask, int* __restrict__ overflow)
@@ -719,61 +754,65 @@ static void cell_pairs_ee(const Grid* gp, const SortedGrid& eg, const SurfArgs& 
     if (last > first) k_cell_pairs_ee<<<nblk(last - first, 32 * kCellPairWarps), 32 * kCellPairWarps, 0, st>>>(gp, eg, s.SE, radius, first, last, out);
 }
 
-// stable radix sort of (keys, idx) pairs, result back in (keys, idx)
-static int sort_pass(ipcgpu_ctx* ctx, int n)
+int contact_scan(ipcgpu_ctx* ctx, const int* in, int* out, int n)
 {
     ContactWork& w = ctx->cw;
     size_t bytes = w.cub_tmp.n;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(w.cub_tmp.p, bytes, w.skey.p, w.skey2.p, w.sidx.p, w.sidx2.p, n, 0, 64, ctx->stream);
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, bytes, in, out, n, ctx->stream);
     if (e != cudaSuccess) {
-        ctx->err = std::string("cub sort: ") + cudaGetErrorString(e);
+        ctx->err = std::string("cub scan: ") + cudaGetErrorString(e);
         return IPCGPU_ERR_CUDA;
     }
-    std::swap(w.skey.p, w.skey2.p);
-    std::swap(w.sidx.p, w.sidx2.p);
-    ++ctx->launches;
-    return 0;
+    return IPCGPU_OK;
 }
 
-// sort int4 list lexicographically (optionally with an int2 companion as the least significant key)
-static int sort_lex(ipcgpu_ctx* ctx, int4* data, int2* comp, int n, int4* tmp4, int2* tmp2)
+// buckets of the canonical order: first components in [-nV, max(nV, nSE)) (candidates: -svI - 1 or an edge index)
+static int lex_buckets(const ipcgpu_ctx* ctx) { return std::max(ctx->nV, 1) + std::max(std::max(ctx->nV, ctx->nSE), 1); }
+
+// perm = the permutation that sorts list[0, min(*n, cap)) lexicographically (companion last)
+template <typename T>
+static int lex_order_impl(ipcgpu_ctx* ctx, const T* list, const int2* comp, const int* n, int cap)
 {
-    if (n <= 1) return 0;
     ContactWork& w = ctx->cw;
     cudaStream_t st = ctx->stream;
-    k_iota<<<nblk(n, 256), 256, 0, st>>>(n, w.sidx.p);
-    int rc;
-    if (comp) {
-        k_key_from2<<<nblk(n, 256), 256, 0, st>>>(n, comp, w.sidx.p, w.skey.p);
-        if ((rc = sort_pass(ctx, n))) return rc;
-    }
-    k_key_from4<<<nblk(n, 256), 256, 0, st>>>(n, data, w.sidx.p, 0, w.skey.p);
-    if ((rc = sort_pass(ctx, n))) return rc;
-    k_key_from4<<<nblk(n, 256), 256, 0, st>>>(n, data, w.sidx.p, 1, w.skey.p);
-    if ((rc = sort_pass(ctx, n))) return rc;
-    k_gather<int4><<<nblk(n, 256), 256, 0, st>>>(n, data, w.sidx.p, tmp4);
-    CK(cudaMemcpyAsync(data, tmp4, (size_t)n * sizeof(int4), cudaMemcpyDeviceToDevice, st));
-    if (comp) {
-        k_gather<int2><<<nblk(n, 256), 256, 0, st>>>(n, comp, w.sidx.p, tmp2);
-        CK(cudaMemcpyAsync(comp, tmp2, (size_t)n * sizeof(int2), cudaMemcpyDeviceToDevice, st));
-    }
+    const int nB = lex_buckets(ctx);
+    zero_words(w.cnt.p, (size_t)nB + 1, st);
+    k_lex_count<<<kLexBlocks, 256, 0, st>>>(list, n, cap, ctx->nV, w.cnt.p);
+    int rc = contact_scan(ctx, w.cnt.p, w.off.p, nB + 1);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(w.cnt.p, w.off.p, (size_t)nB * sizeof(int), cudaMemcpyDeviceToDevice, st)); // scatter cursors
+    k_lex_scatter<<<kLexBlocks, 256, 0, st>>>(list, n, cap, ctx->nV, w.cnt.p, w.perm.p);
+    k_lex_bucket_sort<<<nblk(nB, 256), 256, 0, st>>>(nB, w.off.p, list, comp, w.perm.p);
     ctx->launches += 6;
-    return 0;
+    return IPCGPU_OK;
+}
+int lex_order(ipcgpu_ctx* ctx, const int4* list, const int2* comp, const int* n, int cap) { return lex_order_impl(ctx, list, comp, n, cap); }
+int lex_order(ipcgpu_ctx* ctx, const int2* list, const int* n, int cap) { return lex_order_impl(ctx, list, (const int2*)nullptr, n, cap); }
+
+// data[0, min(*n, cap)) = data[perm[i]], `words` 8-byte words per element
+void permute(ipcgpu_ctx* ctx, void* data, int words, const int* n, int cap)
+{
+    ContactWork& w = ctx->cw;
+    k_permute_words<<<kLexBlocks, 256, 0, ctx->stream>>>(static_cast<const unsigned long long*>(data), w.perm.p, n, cap, words, w.words.p);
+    k_copy_words<<<kLexBlocks, 256, 0, ctx->stream>>>(w.words.p, n, cap, words, static_cast<unsigned long long*>(data));
+    ctx->launches += 2;
 }
 
-static int sort_int2(ipcgpu_ctx* ctx, int2* data, int n, int2* tmp2)
+// act, para (with para_e) and, when the candidates were wanted, cand in canonical order, sized by the device counters
+int contact_sort_lists(ipcgpu_ctx* ctx)
 {
-    if (n <= 1) return 0;
     ContactWork& w = ctx->cw;
-    cudaStream_t st = ctx->stream;
-    k_iota<<<nblk(n, 256), 256, 0, st>>>(n, w.sidx.p);
-    k_key_from2<<<nblk(n, 256), 256, 0, st>>>(n, data, w.sidx.p, w.skey.p);
     int rc;
-    if ((rc = sort_pass(ctx, n))) return rc;
-    k_gather<int2><<<nblk(n, 256), 256, 0, st>>>(n, data, w.sidx.p, tmp2);
-    CK(cudaMemcpyAsync(data, tmp2, (size_t)n * sizeof(int2), cudaMemcpyDeviceToDevice, st));
-    ctx->launches += 3;
-    return 0;
+    if ((rc = lex_order(ctx, w.act.p, nullptr, w.counters.p + 0, w.cap))) return rc;
+    permute(ctx, w.act.p, 2, w.counters.p + 0, w.cap);
+    if ((rc = lex_order(ctx, w.para.p, w.para_e.p, w.counters.p + 2, w.cap))) return rc;
+    permute(ctx, w.para.p, 2, w.counters.p + 2, w.cap);
+    permute(ctx, w.para_e.p, 1, w.counters.p + 2, w.cap);
+    if (w.want_cand) {
+        if ((rc = lex_order(ctx, w.cand.p, w.counters.p + 3, 4 * w.cap))) return rc;
+        permute(ctx, w.cand.p, 1, w.counters.p + 3, 4 * w.cap);
+    }
+    return IPCGPU_OK;
 }
 
 int contact_alloc(ipcgpu_ctx* ctx)
@@ -784,10 +823,12 @@ int contact_alloc(ipcgpu_ctx* ctx)
     const int cap = std::max(ctx->pair_capacity, 1024);
     bool ok = w.vbox.reserve(std::max(nSV, 1)) && w.ebox.reserve(std::max(nSE, 1)) && w.tbox.reserve(std::max(nSF, 1)) && w.bounds.reserve(8) && w.grid.reserve(2)
         && w.centries.reserve(nAll) && w.ckeys.reserve(nAll) && w.cvals.reserve(nAll) && w.key_tmp.reserve(nAll) && w.val_tmp.reserve(nAll)
-        && w.act.reserve(cap) && w.dup.reserve(cap) && w.para.reserve(cap) && w.para_e.reserve(cap) && w.cand.reserve((size_t)4 * cap) && w.tmp4.reserve(cap)
-        && w.tmp2.reserve((size_t)4 * cap) && w.counters.reserve(16) && w.skey.reserve((size_t)4 * cap) && w.skey2.reserve((size_t)4 * cap) && w.sidx.reserve((size_t)4 * cap)
-        && w.sidx2.reserve((size_t)4 * cap);
-    // PP/PE duplicate-merge table: the largest power of two that fits the sort scratch, at most 2^20 slots (cleared every build)
+        && w.act.reserve(cap) && w.dup.reserve(cap) && w.para.reserve(cap) && w.para_e.reserve(cap) && w.cand.reserve((size_t)4 * cap)
+        && w.counters.reserve(16) && w.skey.reserve((size_t)4 * cap) && w.sidx.reserve((size_t)4 * cap);
+    // canonical order: bucket counts and offsets, the permutation (up to 4 cap candidates), the permuted words (up to 6 per friction basis)
+    const size_t nB = (size_t)lex_buckets(ctx) + 1;
+    ok = ok && w.cnt.reserve(nB) && w.off.reserve(nB) && w.perm.reserve((size_t)4 * cap) && w.words.reserve((size_t)6 * cap);
+    // PP/PE duplicate-merge table: the largest power of two that fits skey / sidx, at most 2^20 slots (cleared every build)
     w.dup_tab = 1024;
     while (w.dup_tab * 2 <= (unsigned)std::min<size_t>((size_t)4 * cap, (size_t)1 << 20)) w.dup_tab *= 2;
     // pair Hessians of the barrier stage (144 doubles per pair) + stencil rows + makePD flags, sized by the pair capacity so that the
@@ -806,7 +847,7 @@ int contact_alloc(ipcgpu_ctx* ctx)
     }
     size_t b1 = 0, b2 = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, b1, (int*)nullptr, (int*)nullptr, (int)(3 * kGridCells + 1)); // dense cell-offset table
-    cub::DeviceRadixSort::SortPairs(nullptr, b2, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, 4 * cap);
+    cub::DeviceScan::ExclusiveSum(nullptr, b2, (int*)nullptr, (int*)nullptr, (int)nB);                   // bucket offsets of the order
     if (!w.cub_tmp.reserve(std::max(b1, b2) + 256)) {
         ctx->err = "cub temp allocation failed";
         return IPCGPU_ERR_CUDA;
@@ -915,8 +956,7 @@ int contact_sync_counts(ipcgpu_ctx* ctx)
 }
 
 // SelfCollisionHandler::computeConstraintSet on the device.  Nothing is read back unless the caller asks for the sizes (nC / nPara /
-// nCand non-NULL) or for the canonical order (whose sorts are sized on the host): the lists and their counts stay on the device and
-// every consumer (barrier_*, partial CCD) takes the counts from there.
+// nCand non-NULL): the lists and their counts stay on the device and every consumer (barrier_*, partial CCD) takes the counts from there.
 int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, int* nPara, int* nCand)
 {
     ContactWork& w = ctx->cw;
@@ -959,37 +999,24 @@ int contact_constraint_set(ipcgpu_ctx* ctx, double dHat, int wantCand, int* nC, 
         ctx->launches += 2;
     }
     // merge PP/PE duplicates into the active list with negative multiplicities (:2434-2476)
-    const bool hashed_merge = ctx->nV < (1 << 21) - 2;
-    if (hashed_merge) { // (x,y,z) packs into one 64-bit key: fixed-size table, no host-side size needed
+    if (ctx->nV < (1 << 21) - 2) { // (x,y,z) packs into one 64-bit key: fixed-size table
         CK(cudaMemsetAsync(w.skey.p, 0xff, (size_t)w.dup_tab * sizeof(unsigned long long), st));
         CK(cudaMemsetAsync(w.sidx.p, 0, (size_t)w.dup_tab * sizeof(int), st));
         k_dup_insert<<<kSMs * 2, 256, 0, st>>>(w.counters.p + 1, w.cap, w.dup.p, w.skey.p, w.sidx.p, w.dup_tab - 1, w.counters.p + 4);
         k_dup_emit<<<nblk(w.dup_tab, 256), 256, 0, st>>>(w.dup_tab, w.skey.p, w.sidx.p, w.act.p, w.counters.p + 0, w.cap, w.counters.p + 4);
         ctx->launches += 2;
     }
+    else { // huge meshes: equal entries are adjacent in canonical order
+        if ((rc = lex_order(ctx, w.dup.p, nullptr, w.counters.p + 1, w.cap))) return rc;
+        permute(ctx, w.dup.p, 2, w.counters.p + 1, w.cap);
+        k_merge_dups<<<kLexBlocks, 256, 0, st>>>(w.counters.p + 1, w.cap, w.dup.p, w.act.p, w.counters.p + 0, w.counters.p + 4);
+        ++ctx->launches;
+    }
     w.want_cand = wantCand != 0;
     w.nC = w.nP = w.nK = -1; // unknown on the host until somebody asks
-    const bool need_host = !hashed_merge || ctx->canonical_order == 1 || nC || nPara || nCand;
-    if (need_host) {
-        int* h = ctx->staging->contact;
-        if (!hashed_merge) { // huge meshes: sort-based merge, sized on the host
-            CK(cudaMemcpyAsync(h, w.counters.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
-            CK(cudaStreamSynchronize(st));
-            const int nDup = std::min(h[1], w.cap);
-            if (nDup > 0) {
-                if ((rc = sort_lex(ctx, w.dup.p, nullptr, nDup, w.tmp4.p, nullptr))) return rc;
-                k_merge_dups<<<nblk(nDup, 256), 256, 0, st>>>(nDup, w.dup.p, w.act.p, w.counters.p + 0, w.cap, w.counters.p + 4);
-                ++ctx->launches;
-            }
-        }
-        if ((rc = contact_sync_counts(ctx))) return rc;
-        if (ctx->canonical_order == 1) { // deterministic output order (the reference's own order is scheduling dependent, :2176, :2282)
-            if ((rc = sort_lex(ctx, w.act.p, nullptr, w.nC, w.tmp4.p, nullptr))) return rc;
-            if ((rc = sort_lex(ctx, w.para.p, w.para_e.p, w.nP, w.tmp4.p, w.tmp2.p))) return rc;
-            if (wantCand && (rc = sort_int2(ctx, w.cand.p, w.nK, w.tmp2.p))) return rc;
-        }
-    }
-    // the reproducible mode: the same order from device-sized sorts (also inside a capture), and the gather indices of the contact sums
+    if ((nC || nPara || nCand) && (rc = contact_sync_counts(ctx))) return rc;
+    // deterministic output order (the reference's own order is scheduling dependent, :2176, :2282); at level 2 the gather indices too
+    if (ctx->canonical_order >= 1 && (rc = contact_sort_lists(ctx))) return rc;
     ctx->rw.lists_ready = false;
     if (repro_on(ctx) && (rc = repro_contact_lists(ctx))) return rc;
     k_publish_counts<<<1, 32, 0, st>>>(w.counters.p, wantCand, ctx->iter.p);

@@ -44,13 +44,14 @@ struct DevBuf {
 struct ContactWork {
     DevBuf<Box> vbox, ebox, tbox;   // per-primitive boxes (primitive order)
     DevBuf<QEntry> centries;        // grid-sorted entries (triangles first, then edges): quantised box + id
-    DevBuf<unsigned long long> bounds, skey, skey2;
+    DevBuf<unsigned long long> bounds, skey, words; // skey / sidx: the PP/PE duplicate-merge table; words: permuted list entries
     DevBuf<unsigned> ckeys, key_tmp; // ckeys: sorted 32-bit cell keys (cell | type bits) of the combined triangle + edge + vertex grid
     DevBuf<Grid> grid;
-    DevBuf<int> cvals, val_tmp, counters, sidx, sidx2;
-    DevBuf<int4> act, dup, para, tmp4;
-    DevBuf<int2> para_e, cand, tmp2;
-    DevBuf<unsigned char> cub_tmp;
+    DevBuf<int> cvals, val_tmp, counters, sidx;
+    DevBuf<int> cnt, off, perm;     // canonical order: bucket counts / offsets over [-nV, max(nV, nSE)), the sorting permutation
+    DevBuf<int4> act, dup, para;
+    DevBuf<int2> para_e, cand;
+    DevBuf<unsigned char> cub_tmp;  // scans: the cell offsets, the order's bucket offsets, the reproducible mode's index offsets
     DevBuf<int> cell_cnt, cell_off; // dense per-(type, cell) counters and their exclusive prefix sum: entry range of a cell = two adjacent offsets
     DevBuf<int2> bp_pairs; // broad-phase pair lists (PT then EE), bp_cap each
     size_t bp_cap = 0;
@@ -81,16 +82,11 @@ struct ContactWork {
     bool fr_ready = false;
 };
 
-// reproducible mode (ipcgpu_set_canonical_order(ctx, 2), repro.cu), allocated when the level is selected: the scratch of the device-sized
-// lexicographic sort and of the index builds (bucket counts / offsets over 2 nV + 1 buckets, the permutation, a word buffer for the
-// permuted companions), the per-vertex gather indices of the barrier (bg / bh) and friction (fg / fh) gradients and Hessians with their
-// staging, and the plane terms' per-vertex masks, positions and staging.  lists_ready / fr_ready: the indices belong to the lists in act /
-// para and fr_cs (built where the lists were produced at level 2)
+// reproducible mode (ipcgpu_set_canonical_order(ctx, 2), repro.cu), allocated when the level is selected: the per-vertex gather indices of
+// the barrier (bg / bh) and friction (fg / fh) gradients and Hessians with their staging, and the plane terms' per-vertex masks, positions
+// and staging (the index builds count and scan in ContactWork's cnt / cub_tmp).  lists_ready / fr_ready: the indices belong to the lists
+// in act / para and fr_cs (built where the lists were produced at level 2)
 struct ReproWork {
-    DevBuf<int> cnt, off, perm;
-    DevBuf<unsigned long long> words;
-    DevBuf<unsigned char> scan_tmp;
-    size_t scan_bytes = 0;
     DevBuf<int> bg_ptr, bh_ptr, fg_ptr, fh_ptr;
     DevBuf<unsigned long long> bg_key, bh_key, fg_key, fh_key;
     DevBuf<double> bstage, fstage, fhstage;
@@ -173,7 +169,7 @@ struct PointTetWork {
 struct HostStaging {
     double scalar;   // a read-back double: energy_result, ipcgpu_dirichlet_completed_step
     int count;       // a read-back count: the lagged friction pairs
-    int contact[16]; // ContactWork::counters read back (contact_sync_counts, the sort-based duplicate merge) or uploaded (ipcgpu_set_constraint_set)
+    int contact[16]; // ContactWork::counters read back (contact_sync_counts) or uploaded (ipcgpu_set_constraint_set)
     double pSize;    // source of upload_dir's asynchronous H2D copy into pSize_dev, which nothing waits on: never reused for anything else
     int hs_count[2]; // half-space counts: [0] active, [1] lagged
 };
@@ -246,8 +242,8 @@ struct ipcgpu_ctx {
     bool has_codim = false, surface_ready = false;
     int pair_capacity = 1 << 20;
     int exchange_capacity = 1 << 16; // pairs per rank and list in the fixed-size message of the cross-rank pair-list exchange
-    // order of the contact lists (ipcgpu_set_canonical_order): 0 build order, 1 sorted lexicographically by host-sized sorts, 2 sorted by
-    // device-sized sorts and every contact sum taken in list order (the reproducible mode, ReproWork)
+    // order of the contact lists (ipcgpu_set_canonical_order): 0 build order, 1 sorted lexicographically (lex_order), 2 sorted and every
+    // contact sum taken in list order (the reproducible mode, ReproWork)
     int canonical_order = 1;
     ipcgpu::ReproWork rw;
     bool partition_contact = false, lists_local = false; // multi-rank: build only this rank's share of the contact sets

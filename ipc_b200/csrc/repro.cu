@@ -1,16 +1,11 @@
-// repro.cu -- the reproducible mode (ipcgpu_set_canonical_order(ctx, 2)), sm_90a: device-sized canonical order of the contact lists and
-// the per-vertex gather indices of the fixed-order contact sums (repro.cuh, DESIGN.md section 3.20).
-//
-// Order.  The lists are sorted into the order sort_lex gives (lexicographic on the signed components, the companion (eI, eJ) last) without
-// a host read-back: a bucket pass on the first component -- count, exclusive scan over 2 nV + 1 buckets (x is -v - 1 in the PT/PP/PE
-// encodings), scatter -- then an insertion sort of every bucket on the rest.  Grids are sized by capacities, counts are read on the device.
+// repro.cu -- the reproducible mode (ipcgpu_set_canonical_order(ctx, 2)), sm_90a: the per-vertex gather indices of the fixed-order contact
+// sums (repro.cuh, DESIGN.md section 3.20).  The lists arrive in canonical order (constraint.cu's lex_order / permute).
 //
 // Index.  The contributions of a list (gradient: one per stencil vertex, key = list position and local vertex; Hessian: one per upper
 // 3x3 block, row = its lower vertex, key = column vertex, list position, block) are counted per vertex, scanned, scattered and sorted per
-// vertex on the same pattern.  Built where the list is produced; the term calls then only stage and gather.
+// vertex on the pattern of the canonical order.  Built where the list is produced; the term calls then only stage and gather.
 #include "repro.cuh"
 #include "abi.h"
-#include <cub/cub.cuh>
 #include <algorithm>
 
 namespace ipcgpu {
@@ -46,61 +41,6 @@ void repro_gather_g(int nV, const VertexIndex& idx, const double* stage, unsigne
 namespace {
 
 constexpr int kReproBlocks = kSMs * 4;
-
-// ---- device-sized lexicographic order ------------------------------------------------------------------------------------------------
-DEV bool lex_less(int4 a, int2 ac, int4 b, int2 bc)
-{
-    if (a.y != b.y) return a.y < b.y;
-    if (a.z != b.z) return a.z < b.z;
-    if (a.w != b.w) return a.w < b.w;
-    if (ac.x != bc.x) return ac.x < bc.x;
-    return ac.y < bc.y;
-}
-__global__ void __launch_bounds__(256) k_lex_count(const int4* __restrict__ list, const int* __restrict__ n_ptr, int cap, int nV, int* __restrict__ cnt)
-{
-    const int n = min(*n_ptr, cap);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) atomicAdd(cnt + list[i].x + nV, 1);
-}
-__global__ void __launch_bounds__(256) k_lex_scatter(const int4* __restrict__ list, const int* __restrict__ n_ptr, int cap, int nV, int* __restrict__ cur,
-    int* __restrict__ perm)
-{
-    const int n = min(*n_ptr, cap);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) perm[atomicAdd(cur + list[i].x + nV, 1)] = i;
-}
-// one thread per bucket: insertion sort of its positions on (y, z, w, companion)
-__global__ void __launch_bounds__(256) k_lex_bucket_sort(int nB, const int* __restrict__ off, const int4* __restrict__ list, const int2* __restrict__ comp,
-    int* __restrict__ perm)
-{
-    for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nB; b += gridDim.x * blockDim.x) {
-        const int s = off[b], e = off[b + 1];
-        for (int i = s + 1; i < e; ++i) {
-            const int pi = perm[i];
-            const int4 key = list[pi];
-            const int2 kc = comp ? comp[pi] : make_int2(0, 0);
-            int j = i - 1;
-            while (j >= s) {
-                const int pj = perm[j];
-                if (!lex_less(key, kc, list[pj], comp ? comp[pj] : make_int2(0, 0))) break;
-                perm[j + 1] = pj;
-                --j;
-            }
-            perm[j + 1] = pi;
-        }
-    }
-}
-// dst[i] = src[perm[i]] for i < n, `words` 8-byte words per element (k_copy_words then copies dst back)
-__global__ void __launch_bounds__(256) k_permute_words(const unsigned long long* __restrict__ src, const int* __restrict__ perm, const int* __restrict__ n_ptr,
-    int cap, int words, unsigned long long* __restrict__ dst)
-{
-    const long long n = (long long)min(*n_ptr, cap) * words;
-    for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[(long long)perm[i / words] * words + i % words];
-}
-__global__ void __launch_bounds__(256) k_copy_words(const unsigned long long* __restrict__ src, const int* __restrict__ n_ptr, int cap, int words,
-    unsigned long long* __restrict__ dst)
-{
-    const long long n = (long long)min(*n_ptr, cap) * words;
-    for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i];
-}
 
 // ---- per-vertex gather indices -------------------------------------------------------------------------------------------------------
 enum { kIdxGrad = 0, kIdxBarrierH, kIdxFrictionH };
@@ -175,55 +115,18 @@ __global__ void __launch_bounds__(256) k_index_sort(int nV, const int* __restric
 
 using namespace ipcgpu;
 
-static int scan(ipcgpu_ctx* ctx, const int* in, int* out, int n)
-{
-    ReproWork& r = ctx->rw;
-    size_t bytes = r.scan_bytes;
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(r.scan_tmp.p, bytes, in, out, n, ctx->stream);
-    if (e != cudaSuccess) {
-        ctx->err = std::string("cub scan (reproducible mode): ") + cudaGetErrorString(e);
-        return IPCGPU_ERR_CUDA;
-    }
-    return IPCGPU_OK;
-}
-
-// perm = the permutation that sorts list[0, *n) lexicographically (companion last)
-static int lex_order(ipcgpu_ctx* ctx, const int4* list, const int2* comp, const int* n)
-{
-    ReproWork& r = ctx->rw;
-    cudaStream_t st = ctx->stream;
-    const int nB = 2 * ctx->nV + 1;
-    zero_words(r.cnt.p, (size_t)nB + 1, st);
-    k_lex_count<<<kReproBlocks, 256, 0, st>>>(list, n, r.cap, ctx->nV, r.cnt.p);
-    int rc = scan(ctx, r.cnt.p, r.off.p, nB + 1);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(r.cnt.p, r.off.p, (size_t)nB * sizeof(int), cudaMemcpyDeviceToDevice, st)); // scatter cursors
-    k_lex_scatter<<<kReproBlocks, 256, 0, st>>>(list, n, r.cap, ctx->nV, r.cnt.p, r.perm.p);
-    k_lex_bucket_sort<<<nblk(nB, 256), 256, 0, st>>>(nB, r.off.p, list, comp, r.perm.p);
-    ctx->launches += 6;
-    return IPCGPU_OK;
-}
-// data[0, *n) = data[perm[i]], `words` 8-byte words per element
-static void permute(ipcgpu_ctx* ctx, void* data, int words, const int* n)
-{
-    ReproWork& r = ctx->rw;
-    k_permute_words<<<kReproBlocks, 256, 0, ctx->stream>>>(static_cast<const unsigned long long*>(data), r.perm.p, n, r.cap, words, r.words.p);
-    k_copy_words<<<kReproBlocks, 256, 0, ctx->stream>>>(r.words.p, n, r.cap, words, static_cast<unsigned long long*>(data));
-    ctx->launches += 2;
-}
-
 template <int kMode>
 static int build_index(ipcgpu_ctx* ctx, const IndexSrc& s, int* ptr, unsigned long long* key)
 {
-    ReproWork& r = ctx->rw;
+    int* cnt = ctx->cw.cnt.p;
     cudaStream_t st = ctx->stream;
     const int nV = ctx->nV;
-    zero_words(r.cnt.p, (size_t)nV + 1, st);
-    k_index_emit<kMode, false><<<kReproBlocks, 128, 0, st>>>(s, r.cnt.p, nullptr);
-    int rc = scan(ctx, r.cnt.p, ptr, nV + 1);
+    zero_words(cnt, (size_t)nV + 1, st);
+    k_index_emit<kMode, false><<<kReproBlocks, 128, 0, st>>>(s, cnt, nullptr);
+    int rc = contact_scan(ctx, cnt, ptr, nV + 1);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(r.cnt.p, ptr, (size_t)nV * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    k_index_emit<kMode, true><<<kReproBlocks, 128, 0, st>>>(s, r.cnt.p, key);
+    CK(cudaMemcpyAsync(cnt, ptr, (size_t)nV * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    k_index_emit<kMode, true><<<kReproBlocks, 128, 0, st>>>(s, cnt, key);
     k_index_sort<<<nblk(nV, 256), 256, 0, st>>>(nV, ptr, key);
     ctx->launches += 6;
     return IPCGPU_OK;
@@ -236,12 +139,7 @@ int repro_alloc(ipcgpu_ctx* ctx)
     const size_t cap = (size_t)std::max(ctx->cw.cap, 1);
     if (r.cap == (int)cap && r.nV == nV && r.nSV == nSV) return IPCGPU_OK;
     REQUIRE(cap <= ((size_t)1 << 27), IPCGPU_ERR_CAPACITY, "the reproducible mode keys list positions on 28 bits: a pair capacity of at most 2^27");
-    const size_t nB = 2 * (size_t)nV + 2;
-    size_t scan_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int*)nullptr, (int*)nullptr, (int)nB);
-    r.scan_bytes = scan_bytes;
-    bool ok = r.cnt.reserve(nB) && r.off.reserve(nB) && r.perm.reserve(cap) && r.words.reserve(6 * cap) && r.scan_tmp.reserve(scan_bytes + 256)
-        && r.bg_ptr.reserve((size_t)nV + 1) && r.bh_ptr.reserve((size_t)nV + 1) && r.fg_ptr.reserve((size_t)nV + 1) && r.fh_ptr.reserve((size_t)nV + 1)
+    bool ok = r.bg_ptr.reserve((size_t)nV + 1) && r.bh_ptr.reserve((size_t)nV + 1) && r.fg_ptr.reserve((size_t)nV + 1) && r.fh_ptr.reserve((size_t)nV + 1)
         && r.bg_key.reserve(12 * cap) && r.bh_key.reserve(10 * cap) && r.fg_key.reserve(4 * cap) && r.fh_key.reserve(10 * cap)
         && r.bstage.reserve(36 * cap) && r.fstage.reserve(12 * cap) && r.fhstage.reserve(13 * cap)
         && r.hs_mask.reserve((size_t)nV) && r.hs_pos.reserve((size_t)kMaxPlanes * nV) && r.hs_stage.reserve((size_t)6 * kMaxPlanes * nSV);
@@ -256,17 +154,12 @@ int repro_alloc(ipcgpu_ctx* ctx)
 
 bool repro_on(const ipcgpu_ctx* ctx) { return ctx->canonical_order == 2 && ctx->nranks == 1 && ctx->rw.cap > 0; }
 
-// the active and mollified lists in canonical order, then their gradient and Hessian indices
+// the gradient and Hessian indices of the active and mollified lists (in canonical order already)
 int repro_contact_lists(ipcgpu_ctx* ctx)
 {
     ContactWork& w = ctx->cw;
     ReproWork& r = ctx->rw;
     int rc;
-    if ((rc = lex_order(ctx, w.act.p, nullptr, w.counters.p + 0))) return rc;
-    permute(ctx, w.act.p, 2, w.counters.p + 0);
-    if ((rc = lex_order(ctx, w.para.p, w.para_e.p, w.counters.p + 2))) return rc;
-    permute(ctx, w.para.p, 2, w.counters.p + 2);
-    permute(ctx, w.para_e.p, 1, w.counters.p + 2);
     const IndexSrc s{ w.act.p, w.counters.p + 0, w.para.p, w.para_e.p, w.counters.p + 2, ctx->SE.p, r.cap };
     if ((rc = build_index<kIdxGrad>(ctx, s, r.bg_ptr.p, r.bg_key.p))) return rc;
     if ((rc = build_index<kIdxBarrierH>(ctx, s, r.bh_ptr.p, r.bh_key.p))) return rc;
@@ -282,11 +175,11 @@ int repro_friction_list(ipcgpu_ctx* ctx, bool sort)
     ReproWork& r = ctx->rw;
     int rc;
     if (sort) {
-        if ((rc = lex_order(ctx, w.fr_cs.p, nullptr, w.fr_n.p))) return rc;
-        permute(ctx, w.fr_cs.p, 2, w.fr_n.p);
-        permute(ctx, w.fr_lambda.p, 1, w.fr_n.p);
-        permute(ctx, w.fr_coord.p, 2, w.fr_n.p);
-        permute(ctx, w.fr_basis.p, 6, w.fr_n.p);
+        if ((rc = lex_order(ctx, w.fr_cs.p, nullptr, w.fr_n.p, r.cap))) return rc;
+        permute(ctx, w.fr_cs.p, 2, w.fr_n.p, r.cap);
+        permute(ctx, w.fr_lambda.p, 1, w.fr_n.p, r.cap);
+        permute(ctx, w.fr_coord.p, 2, w.fr_n.p, r.cap);
+        permute(ctx, w.fr_basis.p, 6, w.fr_n.p, r.cap);
     }
     const IndexSrc s{ w.fr_cs.p, w.fr_n.p, nullptr, nullptr, nullptr, ctx->SE.p, r.cap };
     if ((rc = build_index<kIdxGrad>(ctx, s, r.fg_ptr.p, r.fg_key.p))) return rc;

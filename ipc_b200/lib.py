@@ -709,9 +709,9 @@ class Context:
         self._ck(self.lib.ipcgpu_set_obstacle_positions(self.h, _d(f64(np.ascontiguousarray(np.asarray(Vo, dtype=np.float64).T).ravel()))))
 
     def set_canonical_order(self, level):
-        """0: contact lists in build order; 1 (default): sorted lexicographically (host-sized sorts, refused inside a capture);
-        2: the reproducible mode -- the same order from device-sized sorts, also inside a capture, and every contact sum (E, g, H) in an
-        order fixed by the lists alone, so a captured time step gives the same bits on every run.  One rank only."""
+        """0: contact lists in build order; 1 (default): sorted lexicographically (sorts sized on the device, also inside a capture);
+        2: the reproducible mode -- the same order, and every contact sum (E, g, H) in an order fixed by the lists alone, so a captured
+        time step gives the same bits on every run.  One rank only."""
         self._ck(self.lib.ipcgpu_set_canonical_order(self.h, int(level)))
 
     def set_contact_partition(self, enable):

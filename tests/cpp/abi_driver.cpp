@@ -83,7 +83,7 @@ int main(int argc, char** argv)
         CHECK(ipcgpu_ccd_full_ti(ctx, tol, evf, eee, nullptr, nullptr));
         return 0;
     };
-    CHECK(ipcgpu_set_canonical_order(ctx, 0)); // the sets are consumed on the device: no canonical sort (it needs the list sizes on the host)
+    CHECK(ipcgpu_set_canonical_order(ctx, 0)); // the sets are consumed on the device: no canonical sort
     ipcgpu_iteration it;
     if (enqueue()) return 1; // eager once (lazy allocations)
     CHECK(ipcgpu_fetch_iteration(ctx, &it));

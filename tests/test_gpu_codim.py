@@ -8,6 +8,7 @@ import pytest
 
 import oracle as orc
 import oracle_codim as oc
+from ipc_b200 import codim
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from stagecheck import check_every_stage
@@ -143,6 +144,40 @@ def soup_mesh(V, T, pts):
     m.vCoDim = np.full(m.nV, 3, dtype=np.int32)
     m.vCoDim[pts] = 0
     return m
+
+
+def sheet_under_ball(n=60, span=3.0):
+    """a scripted codimension-2 sheet of 2 n^2 triangles 0.01 under a tet ball.  The sheet comes first, so its edges hold the low edge
+    indices: the EE candidates of the ball against it have first components (sheet edges) up to nSE, which is about three times nV.
+    (Cells of 0.05, wider than the contact distance: the sheet's own box pairs stay within the broad phase's capacity.)"""
+    g = np.linspace(-span / 2, span / 2, n + 1)
+    X, Z = np.meshgrid(g, g, indexing="ij")
+    V = np.stack([X.ravel(), np.zeros(X.size), Z.ravel()], 1)
+    idx = np.arange((n + 1) ** 2).reshape(n + 1, n + 1)
+    a, b, c, d = idx[:-1, :-1].ravel(), idx[1:, :-1].ravel(), idx[1:, 1:].ravel(), idx[:-1, 1:].ravel()
+    F = np.concatenate([np.stack([a, b, c], 1), np.stack([a, c, d], 1)])
+    ball = oc._ball(6, 0.45, (0.0, 0.0, 0.0))
+    ball["V"][:, 1] += 0.01 - ball["V"][:, 1].min()
+    m = codim.codim_scene([dict(codim=2, V=V, F=F, dbc=True), ball], density=1000.0, YM=1e4, PR=0.4)
+    m.V = m.V_rest.copy()
+    return m
+
+
+@pytest.mark.parametrize("level", [1, 2])
+def test_candidates_beyond_nv_in_canonical_order(gpu_ctx, level):
+    """the candidate list sorted on a scene with more surface edges than vertices: its first components reach past nV"""
+    m = sheet_under_ball()
+    dHat = 0.03 ** 2
+    upload(gpu_ctx, m)
+    gpu_ctx.set_canonical_order(level)
+    try:
+        got = gpu_ctx.constraint_set(dHat, 1)
+    finally:
+        gpu_ctx.set_canonical_order(1)
+    ref = orc.Surf(m).constraint_set(dHat)
+    cand = ref[3]
+    assert len(m.SFEdges) > m.nV and cand[:, 0].max() >= m.nV and cand[:, 0].min() < 0
+    assert all(np.array_equal(x, y) for x, y in zip(got, ref))
 
 
 def test_point_in_tet_crafted_soup(gpu_ctx):

@@ -7,6 +7,7 @@ import oracle as orc
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from ipc_b200 import scenes
+from stagecheck import sort_rows
 
 pytestmark = pytest.mark.gpu
 RTOL = 1e-10
@@ -127,6 +128,41 @@ def test_ball_pile_sets_match_oracle(gpu_ctx):
     kappa = 1e9
     E_ref, bad = orc.Surf(m).barrier_energy(mm_r, pa_r, pe_r, info["dHat"], kappa)
     assert bad == 0 and abs(gpu_ctx.barrier_energy(info["dHat"], kappa) - E_ref) <= RTOL * abs(E_ref)
+
+
+def padded(m, nV):
+    """m with unreferenced vertices appended up to nV: the surface arrays and the tets keep their indices"""
+    k = nV - m.nV
+    p = M.Mesh.__new__(M.Mesh)
+    p.__dict__.update(m.__dict__)
+    pad = lambda a, v: np.concatenate([np.asarray(a), np.full((k,) + np.shape(a)[1:], v, dtype=np.asarray(a).dtype)])
+    p.V_rest, p.V, p.mass, p.dbc, p.vCoDim = pad(m.V_rest, 0.0), pad(m.V, 0.0), pad(m.mass, 1.0), pad(m.dbc, 0), pad(m.vCoDim, 3)
+    p.nV = nV
+    return p
+
+
+def test_duplicate_merge_on_a_huge_mesh(gpu_ctx):
+    """from nV = 2^21 - 2 on, the PP/PE multiplicities are merged in canonical order instead of through the 64-bit key table: the same
+    lists as the small mesh's, bit for bit at levels 1 and 2, as sorted multisets at level 0"""
+    m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
+    dHat = info["dHat"]
+    big = padded(m, (1 << 21) - 2)
+    out = {}
+    try:
+        for level in (1, 2, 0):
+            for name, mesh in (("small", m), ("huge", big)):
+                upload(gpu_ctx, mesh)
+                gpu_ctx.set_canonical_order(level)
+                out[name, level] = gpu_ctx.constraint_set(dHat, 1)
+    finally:
+        gpu_ctx.set_canonical_order(1)
+    mm = out["small", 1][0]
+    assert (mm[:, 3] <= -2).any()  # PP / PE entries counted more than once
+    for level in (1, 2):
+        assert all(np.array_equal(x, y) for x, y in zip(out["huge", level], out["small", level])), level
+    s, h = out["small", 0], out["huge", 0]
+    assert all(np.array_equal(x, y) for x, y in zip(sort_rows(h[0]) + sort_rows(h[1], h[2]) + sort_rows(h[3]),
+                                                    sort_rows(s[0]) + sort_rows(s[1], s[2]) + sort_rows(s[3])))
 
 
 def test_reference_two_step_gradient_form(gpu_ctx):

@@ -275,11 +275,6 @@ def test_contract(gpu_ctx):
     with pytest.raises(L.IpcGpuError):
         ctx.graph_launch(gid)
     ctx.graph_destroy(gid)
-    ctx.set_canonical_order(1)  # level 1 inside a capture: still refused
-    ctx.capture_begin()
-    with pytest.raises(L.IpcGpuError, match="STATE"):
-        ctx.line_search(DT2, info["dHat"], KAPPA)
-    ctx.graph_destroy(ctx.capture_end())
     other = L.Context(0)  # level 2 and several ranks: refused (before any collective is set up)
     try:
         other.set_canonical_order(2)
@@ -287,6 +282,51 @@ def test_contract(gpu_ctx):
             other.comm_init(0, 2, bytes(128))
     finally:
         other.close()
+
+
+def held_lists(ctx):
+    """the lists the context holds, without a rebuild"""
+    nC, nP, nK = ctx.constraint_set_sizes()
+    mm, pa, pe, cand = (np.empty((n, k), dtype=np.int32) for n, k in ((nC, 4), (nP, 4), (nP, 2), (nK, 2)))
+    ctx._ck(ctx.lib.ipcgpu_get_constraint_set(ctx.h, L._i(mm), L._i(pa), L._i(pe), L._i(cand)))
+    return mm, pa, pe, cand
+
+
+def test_level1_inside_a_capture(gpu_ctx):
+    """level 1 sorts sized on the device: a captured constraint set and line search replay to the eager calls' lists, which are the
+    oracle's at the accepted step"""
+    ctx = gpu_ctx
+    m, info, _, Vprev = pile_scene()
+    dHat = info["dHat"]
+    upload(ctx, m, None, Vprev, 1)
+    g = ctx.elastic_gradient(DT2) + ctx.barrier_gradient(dHat, KAPPA, np.zeros(3 * m.nV))
+    p = -g / np.abs(g).max() * 0.5 * np.sqrt(dHat)  # a descent direction, at most half a contact distance per coordinate
+    ctx.set_search_dir(p)
+
+    def sequence():
+        ctx.constraint_set(dHat, 1, fetch=False, sizes=False)
+        ctx.step_bound_set(1.0)
+        ctx.line_search(DT2, dHat, KAPPA)
+
+    runs = []
+    for captured in (False, True):
+        ctx.set_state(soa(m.V))
+        if captured:
+            ctx.capture_begin()
+            sequence()
+            gid = ctx.capture_end()
+            ctx.set_state(soa(m.V))
+            ctx.graph_launch(gid)
+            ctx.graph_destroy(gid)
+        else:
+            sequence()  # (also the eager run before the capture)
+        s = ctx.step_control_info()
+        assert s.status == 0 and s.alpha > 0.0
+        runs.append((ctx.download(L.BUF_POSITIONS, 3 * m.nV), held_lists(ctx)))
+    (V_e, eager), (V_g, replay) = runs
+    assert same_bits(V_g, V_e) and all(np.array_equal(x, y) for x, y in zip(replay, eager))
+    assert all(np.array_equal(x, y) for x, y in zip(eager, orc.Surf(m, V_e.reshape(3, -1).T).constraint_set(dHat)))
+    assert len(eager[0]) > 0 and len(eager[3]) > 0
 
 
 # ---- 4. five time steps: the time-integration frame, kappa on the device, a host-driven Newton loop over the captured iteration ----
