@@ -641,7 +641,21 @@ int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max
  * (deferred form: raises it, see above); nothing is NaN and nothing hangs. */
 int ipcgpu_solve_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters,
     double* rel_residual);
-/* result of the last solve of either solver (deferred or not) */
+/* `linearSolver AMGCL` (AMGCLSolver.cpp:24-44; rebuilt at every call as AMGCLSolver::factorize rebuilds it, :173-191): the same Krylov
+ * method and contract as ipcgpu_solve_pcg_multilevel (rhs == NULL: H p = -g on the resident gradient; x == NULL: the solution stays on the
+ * device; adopt_as_search_dir; iters / rel_residual nullable; ipcgpu_solve_info reads the result, max_abs_x exact; single rank),
+ * preconditioned by one W-cycle of smoothed-aggregation algebraic multigrid: vertices aggregated by a distance-2 maximal independent set
+ * of the kept 3 x 3 blocks, 3 x 3 blocks at every level with the translations of each aggregate as the coarse space (the block form of the
+ * reference's scalar hierarchy), P = (I - omega D^-1 A) P_tent, Galerkin coarse matrices, degree-16 D^-1-scaled Chebyshev smoothing over
+ * [rho / 60, 2 rho] (rho by 100 power steps), at most 6 levels, the coarsest (at most 1000 block rows) smoothed.  Every sum is taken in a
+ * fixed order: two calls on the same state return identical bits.  Dirichlet vertices and the obstacle tail (identity rows) are in no
+ * aggregate: with a zero right-hand side there their solution entries are exactly 0.  A diagonal block with a pivot <= 0 or a non-finite
+ * spectral radius (the matrix is not positive definite) returns IPCGPU_ERR_SOLVE; nothing is NaN and nothing hangs.  The set-up reads
+ * sizes back: inside a capture, and on more than one rank, the call returns IPCGPU_ERR_STATE.  Its workspace (ipcgpu_amg_info) is kept for
+ * the life of the context. */
+int ipcgpu_solve_pcg_amg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters,
+    double* rel_residual);
+/* result of the last solve of any solver (deferred or not) */
 typedef struct ipcgpu_solve_result {
     int iterations;               /* Krylov iterations run */
     double rel_residual;          /* |r| / |b| after them (0 for b = 0) */
@@ -671,6 +685,13 @@ int ipcgpu_multilevel_info(ipcgpu_ctx* ctx, int* levels, int64_t* domains_per_le
  * again from the resident matrix and the current positions and copied out before any inversion.  It overwrites the stored inverses: the
  * hierarchy counts as not built until the next ipcgpu_solve_pcg_multilevel.  count: 96*96 times the domains of ipcgpu_multilevel_info. */
 int ipcgpu_multilevel_debug_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count);
+/* what the last ipcgpu_solve_pcg_amg built (AMGCLSolver.cpp:173-191): levels; per level (6 entries, 0 beyond the last) block rows, kept
+ * 3 x 3 blocks, the spectral radius rho of D^-1 A and the prolongator damping omega (0 on the last level); device bytes the AMG workspace
+ * holds.  Any pointer may be NULL.  IPCGPU_ERR_STATE before the first ipcgpu_solve_pcg_amg and after one that failed. */
+int ipcgpu_amg_info(ipcgpu_ctx* ctx, int* levels, int64_t* rows, int64_t* blocks, double* rho, double* omega, uint64_t* bytes);
+/* TEST HOOK.  Level `level` of the last AMG hierarchy: aggregate (rows; the aggregate of every row, -1 for a row without a connection and on
+ * the last level), ia (rows + 1), ja (blocks) and blocks (9 per block, row-major) of its block CSR matrix.  Any pointer may be NULL. */
+int ipcgpu_amg_debug_level(ipcgpu_ctx* ctx, int level, int* aggregate, int* ia, int* ja, double* blocks);
 /* LinSysSolver::setZero (LinSysSolver.hpp:348) on the device-resident value array */
 int ipcgpu_csr_set_zero(ipcgpu_ctx* ctx);
 /* cross-rank completion over NVLink (no-op on a single rank).  with_gradient: sum-allreduce of the gradient (needed every iteration).

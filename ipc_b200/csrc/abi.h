@@ -277,10 +277,14 @@ int solver_forget_full_pattern(ipcgpu_ctx* ctx); // a new pattern (ipcgpu_set_cs
 // PCG with the block-Jacobi or the multilevel preconditioner; its workspace pcg_part holds kPcgSpmvBlocks SpMV partials, then 2 per CTA
 // of one thread per vertex
 constexpr int kPcgSpmvBlocks = ipcgpu::kSMs * 8;
-int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, bool multilevel);
+enum { kPrecondJacobi = 0, kPrecondMultilevel = 1, kPrecondAmg = 2 }; // solver_pcg's preconditioner
+int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int precond);
 int solver_multilevel_build(ipcgpu_ctx* ctx, double* bad_pivot); // the hierarchy at the current matrix and positions (set-up)
 void solver_multilevel_step(ipcgpu_ctx* ctx, bool start);        // (iteration: the CG update first) z = M^-1 r, partials of r.z and r.r
 int solver_multilevel_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count);
+int solver_amg_build(ipcgpu_ctx* ctx, double* bad_pivot); // the smoothed-aggregation hierarchy of the resident matrix (eager set-up)
+void solver_amg_step(ipcgpu_ctx* ctx, bool start);        // (iteration: the CG update first) one W-cycle z = M^-1 r, partials of r.z and r.r
+size_t solver_amg_bytes(const ipcgpu_ctx* ctx);           // device memory the AMG workspace holds
 int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src); // src NULL: the direction already in ctx->dir
 // (sign g_i) / a(i,i) into out; jacobi: initX option 5's predictor (0 on Dirichlet vertices and the obstacle tail, no status words)
 void solver_precondition_diag(ipcgpu_ctx* ctx, double sign, double* out, bool jacobi);

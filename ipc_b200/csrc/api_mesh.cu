@@ -470,25 +470,29 @@ int ipcgpu_inversion_step(ipcgpu_ctx* ctx, const double* p, double slack, double
 }
 
 // ---- device-resident linear solve hand-off (SURVEY 8(f) rank 1) ----------------------------------------------------------
-// (both built-in solvers: the preconditioner is the only difference).  The deferred form (rhs, x, iters, rel_residual all NULL) enqueues
+// (the three built-in solvers: the preconditioner is the only difference).  The deferred form (rhs, x, iters, rel_residual all NULL) enqueues
 // everything, the Krylov loops as conditional graph nodes inside a capture; its result is read by ipcgpu_solve_info, its failure raises
 // FLAG_SOLVE.  Any other form synchronises and returns what it always did.
-static int solve_pcg(ipcgpu_ctx* ctx, bool multilevel, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
+static int solve_pcg(ipcgpu_ctx* ctx, int precond, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
 {
     REQUIRE(ctx->nnz > 0 && ctx->n_rows == 3 * ctx->nV, IPCGPU_ERR_STATE, "ipcgpu_set_csr first");
     REQUIRE(ctx->nranks == 1, IPCGPU_ERR_STATE, "the built-in solver runs on one rank (a distributed solver takes each rank's rows: ipcgpu_partition_info)");
     REQUIRE(rel_tol > 0.0 && max_iter > 0, IPCGPU_ERR_ARG, "bad tolerance / iteration limit");
     const bool deferred = !rhs && !x && !iters && !rel_residual;
     REQUIRE(deferred || !ctx->capturing, IPCGPU_ERR_STATE, "inside a capture the solve takes its deferred form: rhs, x, iters and rel_residual all NULL");
+    static const char* const name[] = { "ipcgpu_solve_pcg", "ipcgpu_solve_pcg_multilevel", "ipcgpu_solve_pcg_amg" };
+    const bool multilevel = precond == kPrecondMultilevel;
+    // (the AMG set-up reads its sizes back: it cannot be captured)
+    REQUIRE(!ctx->capturing || precond != kPrecondAmg, IPCGPU_ERR_STATE, "ipcgpu_solve_pcg_amg cannot run inside a capture (its set-up reads sizes back)");
     REQUIRE(!ctx->capturing || ctx->solve_epoch[multilevel] == ctx->epoch, IPCGPU_ERR_STATE,
         multilevel ? "run ipcgpu_solve_pcg_multilevel once outside a capture first (it makes its allocations and creates its streams)"
                    : "run ipcgpu_solve_pcg once outside a capture first (it makes its allocations and creates its streams)");
     ENTER(kSerial);
-    int rc = cond_prepare(ctx, multilevel ? "ipcgpu_solve_pcg_multilevel" : "ipcgpu_solve_pcg");
+    int rc = cond_prepare(ctx, name[precond]);
     if (rc) return rc;
     const int n = ctx->n_rows;
     bool ok = ctx->sol.reserve(n) && ctx->pcg_r.reserve(n) && ctx->pcg_p.reserve(n) && ctx->pcg_q.reserve(n) && ctx->pcg_scal.reserve(8)
-        && ctx->pcg_part.reserve((size_t)kPcgSpmvBlocks + 2 * nblk(ctx->nV, 256)) && (multilevel || ctx->pcg_minv.reserve((size_t)6 * ctx->nV));
+        && ctx->pcg_part.reserve((size_t)kPcgSpmvBlocks + 2 * nblk(ctx->nV, 256)) && (precond != kPrecondJacobi || ctx->pcg_minv.reserve((size_t)6 * ctx->nV));
     REQUIRE(ok, IPCGPU_ERR_CUDA, "PCG workspace allocation failed");
     if ((rc = solver_full_pattern(ctx))) return rc; // (rows of both triangles, gathered through a position map; rebuilt when the pattern moved)
     const double* rhs_dev = ctx->g.p;
@@ -499,17 +503,19 @@ static int solve_pcg(ipcgpu_ctx* ctx, bool multilevel, const double* rhs, double
         rhs_dev = ctx->pcg_b.p;
         sign = 1.0;
     }
-    rc = solver_pcg(ctx, rhs_dev, sign, rel_tol, max_iter, multilevel);
+    rc = solver_pcg(ctx, rhs_dev, sign, rel_tol, max_iter, precond);
     if (rc) return rc;
     ctx->sv_pending = true;
-    if (!ctx->capturing) ctx->solve_epoch[multilevel] = ctx->epoch;
+    if (!ctx->capturing && precond != kPrecondAmg) ctx->solve_epoch[multilevel] = ctx->epoch;
     // outside a capture the host loops have read the solve's words (h_iter) with their last decision; inside one they are in device memory
     const IterState& h = *ctx->h_iter;
-    const bool bad_pivot = !ctx->capturing && multilevel && h.sv_status != 0 && h.sv_iters == 0; // (the set-up failed: no iteration ran)
+    const bool bad_pivot = !ctx->capturing && precond != kPrecondJacobi && h.sv_status != 0 && h.sv_iters == 0; // (the set-up failed: no iteration ran)
     if (multilevel) ctx->ml.built = !bad_pivot;
+    if (precond == kPrecondAmg) ctx->amg.built = ctx->amg.built && !bad_pivot;
     if (!deferred) { // the host-output forms report a failure by their return value alone, as before: no deferred flag
         if (h.sv_status != 0) CK(cudaMemsetAsync(&ctx->iter.p->flags[FLAG_SOLVE], 0, sizeof(int), ctx->stream));
-        REQUIRE(!bad_pivot, IPCGPU_ERR_SOLVE, "multilevel preconditioner: a domain matrix has a non-positive pivot (the matrix is not positive definite)");
+        REQUIRE(!bad_pivot || precond == kPrecondAmg, IPCGPU_ERR_SOLVE, "multilevel preconditioner: a domain matrix has a non-positive pivot (the matrix is not positive definite)");
+        REQUIRE(!bad_pivot, IPCGPU_ERR_SOLVE, "AMG preconditioner: a diagonal block with a non-positive pivot or a non-finite spectral radius (the matrix is not positive definite)");
     }
     if (adopt_as_search_dir && (rc = solver_adopt_direction(ctx, ctx->sol.p))) return rc;
     if (iters) *iters = h.sv_iters;
@@ -523,12 +529,18 @@ static int solve_pcg(ipcgpu_ctx* ctx, bool multilevel, const double* rhs, double
 
 int ipcgpu_solve_pcg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
 {
-    return solve_pcg(ctx, false, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
+    return solve_pcg(ctx, kPrecondJacobi, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
 }
 
 int ipcgpu_solve_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
 {
-    return solve_pcg(ctx, true, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
+    return solve_pcg(ctx, kPrecondMultilevel, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
+}
+
+// smoothed-aggregation multigrid (amg.cu, AMGCLSolver.cpp:24-44, :173-191): eager, single rank, not capturable
+int ipcgpu_solve_pcg_amg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters, double* rel_residual)
+{
+    return solve_pcg(ctx, kPrecondAmg, rhs, rel_tol, max_iter, x, adopt_as_search_dir, iters, rel_residual);
 }
 
 // LinSysSolver::precondition_diag on the resident system: computeSearchDir's fallback (sign -1, Optimizer.cpp:2331-2346) and the friction
@@ -602,6 +614,41 @@ int ipcgpu_multilevel_debug_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t coun
     REQUIRE(ctx->ml.built, IPCGPU_ERR_STATE, "ipcgpu_solve_pcg_multilevel first");
     ENTER(kSerial);
     return solver_multilevel_matrices(ctx, dst, count);
+}
+
+int ipcgpu_amg_info(ipcgpu_ctx* ctx, int* levels, int64_t* rows, int64_t* blocks, double* rho, double* omega, uint64_t* bytes)
+{
+    const ipcgpu::AmgWork& w = ctx->amg;
+    REQUIRE(w.built, IPCGPU_ERR_STATE, "ipcgpu_solve_pcg_amg first (a call that failed leaves no hierarchy)");
+    if (levels) *levels = w.levels;
+    for (int l = 0; l < ipcgpu::kAmgMaxLevels; ++l) {
+        const bool in = l < w.levels;
+        if (rows) rows[l] = in ? w.lv[l].n : 0;
+        if (blocks) blocks[l] = in ? w.lv[l].nnzb : 0;
+        if (rho) rho[l] = in ? w.lv[l].rho : 0.0;
+        if (omega) omega[l] = in ? w.lv[l].omega : 0.0;
+    }
+    if (bytes) *bytes = solver_amg_bytes(ctx);
+    return IPCGPU_OK;
+}
+
+int ipcgpu_amg_debug_level(ipcgpu_ctx* ctx, int level, int* aggregate, int* ia, int* ja, double* blocks)
+{
+    const ipcgpu::AmgWork& w = ctx->amg;
+    REQUIRE(w.built, IPCGPU_ERR_STATE, "ipcgpu_solve_pcg_amg first (a call that failed leaves no hierarchy)");
+    REQUIRE(level >= 0 && level < w.levels, IPCGPU_ERR_ARG, "level out of range (ipcgpu_amg_info gives the levels)");
+    ENTER(kSerial);
+    const ipcgpu::AmgLevel& L = w.lv[level];
+    cudaStream_t st = ctx->stream;
+    if (aggregate) {
+        if (L.np > 0) CK(cudaMemcpyAsync(aggregate, L.agg.p, (size_t)L.n * sizeof(int), cudaMemcpyDeviceToHost, st));
+        else std::fill(aggregate, aggregate + L.n, -1); // (the last level is not aggregated)
+    }
+    if (ia) CK(cudaMemcpyAsync(ia, L.ia.p, ((size_t)L.n + 1) * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (ja && L.nnzb) CK(cudaMemcpyAsync(ja, L.ja.p, (size_t)L.nnzb * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (blocks && L.nnzb) CK(cudaMemcpyAsync(blocks, L.blk.p, 9 * (size_t)L.nnzb * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return IPCGPU_OK;
 }
 
 int ipcgpu_csr_set_zero(ipcgpu_ctx* ctx)

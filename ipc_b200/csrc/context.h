@@ -147,6 +147,29 @@ struct MultilevelWork {
     bool smem_opted = false;              // the inversion kernel's dynamic shared memory has been opted in
 };
 
+// smoothed-aggregation multigrid preconditioner (amg.cu): per level the block CSR matrix (3 x 3 blocks), the inverses of its diagonal
+// blocks, the aggregates, the prolongator P and its transpose R (block CSR), the cycle's vectors; shared scratch of the set-up
+constexpr int kAmgMaxLevels = 6;
+struct AmgLevel {
+    DevBuf<int> ia, ja, agg, pia, pja, ria, rja;
+    DevBuf<double> blk, dinv, pblk, rblk;
+    DevBuf<double> f, x, r, d0, d1, t; // (level 0 takes f and x from the Krylov loop: r and z)
+    int n = 0, nnzb = 0, np = 0;       // block rows, kept blocks, blocks of P (0 on the last level)
+    double rho = 0.0, omega = 0.0;     // spectral radius of D^-1 A (power iteration), prolongator damping (0 on the last level)
+    double theta = 0.0, c1[16] = {}, c2[16] = {}; // Chebyshev: 1 / theta for the first direction, the recurrence's coefficients
+};
+struct AmgWork {
+    AmgLevel lv[kAmgMaxLevels];
+    int levels = 0;
+    bool built = false;                                 // the last AMG solve built the whole hierarchy (every pivot positive, rho finite)
+    DevBuf<int> cnt, scan_out, m1, m2, key, pos, lidx, ridx, skey, spos, prow;
+    DevBuf<unsigned long long> tkey, tkey_sorted;
+    DevBuf<unsigned char> state0, state1, tmp;
+    DevBuf<int> flags;                                  // [0] undecided rows, [1] bad layout, [2] bad pivot
+    DevBuf<unsigned long long> absrow;                  // max absolute row sum of D^-1 A (ordered bits)
+    DevBuf<double> part, sq;                            // power iteration: per-CTA partials, squared norms of every step
+};
+
 // point-in-tetrahedron half of the intersection check (safeguard.cu): the codimension-0 vertices (vCoDim == 0) of ipcgpu_set_surface, and
 // a grid over them rebuilt at every check -- cell key per point, the (key, vertex) pairs sorted by key, the grid's geometry, sort scratch
 struct PointGrid {
@@ -323,6 +346,7 @@ struct ipcgpu_ctx {
     ipcgpu::DevBuf<unsigned char> fp_tmp;
     ipcgpu::DevBuf<double> sol, pcg_b, pcg_r, pcg_p, pcg_q, pcg_minv, pcg_scal, pcg_part; // (pcg_part: per-CTA partials of the dot products)
     ipcgpu::MultilevelWork ml;
+    ipcgpu::AmgWork amg;
     uint64_t solve_epoch[2] = { ~0ull, ~0ull };
     bool sv_pending = false, sv_pending_at_capture = false;
     // an elastic gradient / Hessian call wrote g / a since the last ipcgpu_set_state, ipcgpu_set_mesh or pattern change: what the diagonal

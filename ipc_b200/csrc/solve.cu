@@ -5,13 +5,13 @@
 // Cholesky a black box (CHOLMOD / cuDSS); cuDSS is not in this image, so the production binding is documented in INTEGRATION.md
 // (ipcgpu_device_ptr hands cuDSS the device-resident ia / ja / a) and what is BUILT here is the hand-off itself plus a reference solver
 // that runs entirely on the device: a preconditioned conjugate gradient on the upper-triangular CSR the assembly stages fill, with the
-// block-Jacobi preconditioner (here) or the multilevel one (multilevel.cu).  It takes its right-hand side from the device-resident gradient
+// block-Jacobi preconditioner (here), the multilevel one (multilevel.cu) or smoothed-aggregation multigrid (amg.cu).  It takes its right-hand side from the device-resident gradient
 // and leaves the search direction where the step-bound stages read it, so that a whole Newton iteration (assembly -> solve -> CCD) needs no
 // host transfer of any vertex- or matrix-sized array.
 //
-// One Krylov loop (solver_pcg) for both preconditioners: init, SpMV with per-CTA partials, the preconditioner's step, roll, direction.
+// One Krylov loop (solver_pcg) for the three preconditioners: init, SpMV with per-CTA partials, the preconditioner's step, roll, direction.
 // Every dot product is a fixed-order two-level sum (per-CTA partials, then one order for every launch), so two solves of one system give
-// identical bits with either preconditioner: an adopted direction feeds the Armijo and step-bound decisions (DESIGN 3.13 / 3.17).
+// identical bits with any preconditioner: an adopted direction feeds the Armijo and step-bound decisions (DESIGN 3.13 / 3.17).
 //
 // SpMV on a symmetric matrix stored by its upper triangle: the device builds the FULL row structure once per pattern (col index + position
 // of the value inside the upper-triangular array for every entry of both triangles), so the product is a plain deterministic row-parallel
@@ -355,26 +355,34 @@ static void block_jacobi_step(ipcgpu_ctx* ctx, bool start)
     ++ctx->launches;
 }
 
-// PCG on the device-resident matrix, preconditioned by block-Jacobi or by the multilevel hierarchy (multilevel.cu).  rhs_dev: device vector
-// (3 nV) scaled by `sign`.  The solution is left in ctx->sol, the result in IterState (sv_*); a pivot <= 0 of the multilevel set-up is the
-// solve's failure (kSolveStart).  The workspace is reserved by the caller (solve_pcg in api_mesh.cu).  pcg_part holds the SpMV's partials
-// of p.Ap, then the preconditioner step's partials of r.z and r.r (2 per CTA of one thread per vertex).  The step is all the two solvers
+static void preconditioner_step(ipcgpu_ctx* ctx, int precond, bool start)
+{
+    if (precond == kPrecondAmg) solver_amg_step(ctx, start);
+    else if (precond == kPrecondMultilevel) solver_multilevel_step(ctx, start);
+    else block_jacobi_step(ctx, start);
+}
+
+// PCG on the device-resident matrix, preconditioned by block-Jacobi, the multilevel hierarchy (multilevel.cu) or smoothed-aggregation
+// multigrid (amg.cu).  rhs_dev: device vector
+// (3 nV) scaled by `sign`.  The solution is left in ctx->sol, the result in IterState (sv_*); a pivot <= 0 of the multilevel or AMG set-up is
+// the solve's failure (kSolveStart).  The workspace is reserved by the caller (solve_pcg in api_mesh.cu).  pcg_part holds the SpMV's partials
+// of p.Ap, then the preconditioner step's partials of r.z and r.r (2 per CTA of one thread per vertex).  The step is all the three solvers
 // differ in: in an iteration it finishes the CG update from the SpMV's partials, then it leaves z = M^-1 r in pcg_q.
-int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, bool multilevel)
+int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_tol, int max_iter, int precond)
 {
     cudaStream_t st = ctx->stream;
     const int n = ctx->n_rows, n_pre = nblk(ctx->nV, 256);
     double *x = ctx->sol.p, *r = ctx->pcg_r.p, *p = ctx->pcg_p.p, *q = ctx->pcg_q.p, *scal = ctx->pcg_scal.p, *pre = ctx->pcg_part.p + kPcgSpmvBlocks;
     CK(cudaMemsetAsync(scal, 0, 8 * sizeof(double), st));
-    if (multilevel) {
-        int rc = solver_multilevel_build(ctx, scal + 6);
+    if (precond != kPrecondJacobi) {
+        int rc = precond == kPrecondAmg ? solver_amg_build(ctx, scal + 6) : solver_multilevel_build(ctx, scal + 6);
         if (rc) return rc;
     } else {
         k_block_jacobi<<<n_pre, 256, 0, st>>>(ctx->nV, ctx->ia.p, ctx->index_base, ctx->a.p, ctx->pcg_minv.p);
         ++ctx->launches;
     }
     k_pcg_init<<<nblk(n, 256), 256, 0, st>>>(n, rhs_dev, sign, x, r, p);
-    multilevel ? solver_multilevel_step(ctx, true) : block_jacobi_step(ctx, true);
+    preconditioner_step(ctx, precond, true);
     k_pcg_roll<<<1, 1024, 0, st>>>(pre, n_pre, scal, ctx->iter.p, 1);
     k_pcg_direction<<<nblk(n, 256), 256, 0, st>>>(n, q, p, scal);
     ctx->launches += 3;
@@ -383,7 +391,7 @@ int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_t
     return krylov_loops(ctx, max_iter, [&]() {
         cudaStream_t s = ctx->stream; // (the body's stream inside a capture)
         k_pcg_spmv<<<kPcgSpmvBlocks, 256, 0, s>>>(n, ctx->fia.p, ctx->fja.p, ctx->fpos.p, ctx->a.p, p, q, ctx->pcg_part.p);
-        multilevel ? solver_multilevel_step(ctx, false) : block_jacobi_step(ctx, false);
+        preconditioner_step(ctx, precond, false);
         k_pcg_roll<<<1, 1024, 0, s>>>(pre, n_pre, scal, ctx->iter.p, 0);
         k_pcg_direction<<<nblk(n, 256), 256, 0, s>>>(n, q, p, scal);
         ctx->launches += 3;

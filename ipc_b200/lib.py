@@ -108,6 +108,9 @@ SIGNATURES = {
     "ipcgpu_precondition_diag": (C.c_int, [_ctxp, C.c_int, _dp, C.c_int]),
     "ipcgpu_multilevel_info": (C.c_int, [_ctxp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]),
     "ipcgpu_multilevel_debug_matrices": (C.c_int, [_ctxp, _dp, C.c_uint64]),
+    "ipcgpu_solve_pcg_amg": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
+    "ipcgpu_amg_info": (C.c_int, [_ctxp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _dp, _dp, C.POINTER(C.c_uint64)]),
+    "ipcgpu_amg_debug_level": (C.c_int, [_ctxp, C.c_int, _ip, _ip, _ip, _dp]),
     "ipcgpu_allreduce_grad_hess": (C.c_int, [_ctxp, C.c_int, C.c_int]),
     "ipcgpu_download": (C.c_int, [_ctxp, C.c_int, _dp, C.c_uint64]),
     "ipcgpu_device_ptr": (C.c_void_p, [_ctxp, C.c_int]),
@@ -974,6 +977,28 @@ class Context:
         out = np.empty(9216 * sum(domains))
         self._ck(self.lib.ipcgpu_multilevel_debug_matrices(self.h, _d(out), out.size))
         return [a.reshape(-1, 96, 96) for a in np.split(out, np.cumsum([9216 * d for d in domains])[:-1])]
+
+    def solve_pcg_amg(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False):
+        """solve_pcg with the smoothed-aggregation multigrid preconditioner (linearSolver AMGCL, rebuilt from the resident matrix at every
+        call; not capturable).  want_x=False with rhs=None leaves the solution on the device; the result is also solve_info()"""
+        return self._solve(self.lib.ipcgpu_solve_pcg_amg, rhs, rel_tol, max_iter, want_x, adopt, False)
+
+    def amg_info(self):
+        """dict of the last AMG hierarchy: rows, blocks, rho, omega (one entry per level) and bytes"""
+        lv, rows, blocks = C.c_int(), (C.c_int64 * 6)(), (C.c_int64 * 6)()
+        rho, omega, nb = (C.c_double * 6)(), (C.c_double * 6)(), C.c_uint64()
+        self._ck(self.lib.ipcgpu_amg_info(self.h, C.byref(lv), rows, blocks, rho, omega, C.byref(nb)))
+        n = lv.value
+        return {"rows": list(rows[:n]), "blocks": list(blocks[:n]), "rho": list(rho[:n]), "omega": list(omega[:n]), "bytes": nb.value}
+
+    def amg_debug_level(self, level):
+        """test hook: (aggregate, ia, ja, blocks (nnzb, 3, 3)) of level `level` of the last AMG hierarchy"""
+        info = self.amg_info()
+        n, nb = info["rows"][level], info["blocks"][level]
+        agg, ia = np.empty(n, dtype=np.int32), np.empty(n + 1, dtype=np.int32)
+        ja, blk = np.empty(max(nb, 1), dtype=np.int32), np.empty(9 * max(nb, 1))
+        self._ck(self.lib.ipcgpu_amg_debug_level(self.h, int(level), _i(agg), _i(ia), _i(ja), _d(blk)))
+        return agg, ia, ja[:nb], blk[: 9 * nb].reshape(-1, 3, 3)
 
     def csr_set_zero(self):
         self._ck(self.lib.ipcgpu_csr_set_zero(self.h))

@@ -1,6 +1,7 @@
-"""Cost of the two built-in linear solvers on C5 (146 x sphere1K.msh, 1M tets) at the state and right-hand side of step_control_timing.py
-(one implicit-Euler step under gravity, H p = -g on the device-resident matrix): block-Jacobi PCG (ipcgpu_solve_pcg) against PCG with the
-multilevel additive Schwarz preconditioner (ipcgpu_solve_pcg_multilevel), alternating, both to 1e-6.  Per solver: iterations, the time of a
+"""Cost of the three built-in linear solvers on C5 (146 x sphere1K.msh, 1M tets) at the state and right-hand side of step_control_timing.py
+(one implicit-Euler step under gravity, H p = -g on the device-resident matrix): block-Jacobi PCG (ipcgpu_solve_pcg), PCG with the
+multilevel additive Schwarz preconditioner (ipcgpu_solve_pcg_multilevel) and PCG with smoothed-aggregation multigrid
+(ipcgpu_solve_pcg_amg), alternating, all to 1e-6.  Per solver: iterations, the time of a
 whole solve, the set-up (a solve limited to one iteration: hierarchy or block inverses, the start of the loop and that iteration) and the
 time per iteration from the two, as device-event medians with min-max.  Prints one JSON line with the card's name, SM clock and power limit
 read in the same run; no device setting is changed.
@@ -45,7 +46,7 @@ def main():
     ctx.barrier_gradient(dHat, kappa, None)
     ctx.barrier_hessian(dHat, kappa, 1, None)
     ctx.inertia_gradient(1, None)
-    solvers = {"block_jacobi": ctx.solve_pcg, "multilevel": ctx.solve_pcg_multilevel}
+    solvers = {"block_jacobi": ctx.solve_pcg, "multilevel": ctx.solve_pcg_multilevel, "amg": ctx.solve_pcg_amg}
     out = {"gpu": gpu_info(), "scene": f"C5, {m.nT} tets, {m.nV} vertices", "rel_tol": TOL, "reps": args.reps}
 
     def timed(solve, max_iter):
@@ -57,7 +58,7 @@ def main():
     runs = {k: {"solve": [], "setup": []} for k in solvers}
     iters = {}
     for r in range(args.reps + 1):  # (the first repetition warms up: allocations, the full-row structure, module loads)
-        for name in (list(solvers) if r % 2 else list(solvers)[::-1]):
+        for name in list(solvers)[r % 3:] + list(solvers)[:r % 3]:  # (each solver first in turn)
             t_all, it, res = timed(solvers[name], 20000)
             t_one, _, _ = timed(solvers[name], 1)
             assert res <= TOL, (name, it, res)
@@ -74,6 +75,7 @@ def main():
     domains, nbytes = ctx.multilevel_info()
     out["multilevel"]["domains_per_level"] = domains
     out["multilevel"]["inverse_bytes"] = nbytes
+    out["amg"]["hierarchy"] = ctx.amg_info()
     out["gpu_after"] = gpu_info()
     print(json.dumps(out))
     ctx.close()
