@@ -650,9 +650,12 @@ int ipcgpu_solve_pcg_multilevel(ipcgpu_ctx* ctx, const double* rhs, double rel_t
  * [rho / 60, 2 rho] (rho by 100 power steps), at most 6 levels, the coarsest (at most 1000 block rows) smoothed.  Every sum is taken in a
  * fixed order: two calls on the same state return identical bits.  Dirichlet vertices and the obstacle tail (identity rows) are in no
  * aggregate: with a zero right-hand side there their solution entries are exactly 0.  A diagonal block with a pivot <= 0 or a non-finite
- * spectral radius (the matrix is not positive definite) returns IPCGPU_ERR_SOLVE; nothing is NaN and nothing hangs.  The set-up reads
- * sizes back: inside a capture, and on more than one rank, the call returns IPCGPU_ERR_STATE.  Its workspace (ipcgpu_amg_info) is kept for
- * the life of the context. */
+ * spectral radius (the matrix is not positive definite) returns IPCGPU_ERR_SOLVE; nothing is NaN and nothing hangs.  Every size of the
+ * hierarchy lives in device memory.  Unreserved, the set-up reads the sizes back to grow its buffers: inside a capture the call returns
+ * IPCGPU_ERR_STATE.  After ipcgpu_amg_reserve nothing is allocated or read back before the Krylov loop, and the deferred form runs inside a
+ * capture under the contract of the other two solvers (one eager call of this solver after the reservation first; ipcgpu_solve_info; a
+ * failure raises IPCGPU_ERR_SOLVE at the fetch).  On more than one rank the call returns IPCGPU_ERR_STATE.  Its workspace (ipcgpu_amg_info)
+ * is kept for the life of the context. */
 int ipcgpu_solve_pcg_amg(ipcgpu_ctx* ctx, const double* rhs, double rel_tol, int max_iter, double* x, int adopt_as_search_dir, int* iters,
     double* rel_residual);
 /* result of the last solve of any solver (deferred or not) */
@@ -687,11 +690,33 @@ int ipcgpu_multilevel_info(ipcgpu_ctx* ctx, int* levels, int64_t* domains_per_le
 int ipcgpu_multilevel_debug_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count);
 /* what the last ipcgpu_solve_pcg_amg built (AMGCLSolver.cpp:173-191): levels; per level (6 entries, 0 beyond the last) block rows, kept
  * 3 x 3 blocks, the spectral radius rho of D^-1 A and the prolongator damping omega (0 on the last level); device bytes the AMG workspace
- * holds.  Any pointer may be NULL.  IPCGPU_ERR_STATE before the first ipcgpu_solve_pcg_amg and after one that failed. */
+ * holds.  Any pointer may be NULL.  IPCGPU_ERR_STATE before the first ipcgpu_solve_pcg_amg, after one that failed, and inside a capture.  The
+ * sizes live in device memory (a replayed graph sets them): the call synchronises to read them. */
 int ipcgpu_amg_info(ipcgpu_ctx* ctx, int* levels, int64_t* rows, int64_t* blocks, double* rho, double* omega, uint64_t* bytes);
 /* TEST HOOK.  Level `level` of the last AMG hierarchy: aggregate (rows; the aggregate of every row, -1 for a row without a connection and on
- * the last level), ia (rows + 1), ja (blocks) and blocks (9 per block, row-major) of its block CSR matrix.  Any pointer may be NULL. */
+ * the last level), ia (rows + 1), ja (blocks) and blocks (9 per block, row-major) of its block CSR matrix.  Any pointer may be NULL.
+ * Synchronises; IPCGPU_ERR_STATE inside a capture. */
 int ipcgpu_amg_debug_level(ipcgpu_ctx* ctx, int level, int* aggregate, int* ia, int* ja, double* blocks);
+/* Reserve every buffer of the AMG set-up, so that ipcgpu_solve_pcg_amg allocates and reads back nothing before its Krylov loop and runs
+ * inside a capture.  The reserved depth is the level count the last set-up built (never less than an earlier reservation).  Level 0 holds nV
+ * block rows and every block of the full pattern (for the device-built pattern: what its nnz_capacity allows); a coarse level holds 4/5 of
+ * the rows above, floored, which the 4/5 stopping rule never exceeds.  The entry counts of each coarsening (blocks of P and R, both product
+ * expansions, blocks of A P and of the coarse matrix) get headroom x what the last set-up needed, never less than an earlier reservation.
+ * A set-up that would exceed a count, or go deeper than the reserved depth, ends the hierarchy at that level (ipcgpu_amg_capacity_info
+ * reports it): the cycle stays symmetric positive definite, CG still reaches rel_tol, only the iteration count grows.  Called again, it
+ * re-sizes for what the last set-up needed: a cut set-up counts nothing beyond the count that cut it, and a depth cut adds one level whose
+ * counts are not known yet, so removing a cut can take a few rounds of reserve, eager solve, ipcgpu_amg_capacity_info.  Bumps the epoch: graphs captured before are refused.  A new mesh or a larger pattern drops the
+ * reservation.  IPCGPU_ERR_STATE without a hierarchy built by an earlier ipcgpu_solve_pcg_amg, inside a capture and on more than one rank;
+ * IPCGPU_ERR_ARG for a headroom that is not finite or below 1. */
+int ipcgpu_amg_reserve(ipcgpu_ctx* ctx, double headroom);
+/* What the last AMG set-up needed against what its buffers hold, per level l and count q (needed / reserved: 6 x 5 entries, index 5 l + q;
+ * q = 0 blocks of P, 1 entries of the A P expansion, 2 blocks of A P, 3 entries of the R (A P) expansion, 4 blocks of the coarse matrix).
+ * *cut_at_level: the level at which a capacity or the reserved depth ended the hierarchy, -1 if none.  Any pointer may be NULL.  Synchronises.
+ * IPCGPU_ERR_STATE before the first ipcgpu_solve_pcg_amg. */
+int ipcgpu_amg_capacity_info(ipcgpu_ctx* ctx, int* cut_at_level, int64_t* needed, int64_t* reserved);
+/* TEST HOOK.  A level with at most `rows` block rows is the last (default 1000).  Held in device memory and read by every set-up, so one
+ * graph can be replayed at another level count. */
+int ipcgpu_amg_debug_coarse_enough(ipcgpu_ctx* ctx, int rows);
 /* LinSysSolver::setZero (LinSysSolver.hpp:348) on the device-resident value array */
 int ipcgpu_csr_set_zero(ipcgpu_ctx* ctx);
 /* cross-rank completion over NVLink (no-op on a single rank).  with_gradient: sum-allreduce of the gradient (needed every iteration).

@@ -282,9 +282,13 @@ int solver_pcg(ipcgpu_ctx* ctx, const double* rhs_dev, double sign, double rel_t
 int solver_multilevel_build(ipcgpu_ctx* ctx, double* bad_pivot); // the hierarchy at the current matrix and positions (set-up)
 void solver_multilevel_step(ipcgpu_ctx* ctx, bool start);        // (iteration: the CG update first) z = M^-1 r, partials of r.z and r.r
 int solver_multilevel_matrices(ipcgpu_ctx* ctx, double* dst, uint64_t count);
-int solver_amg_build(ipcgpu_ctx* ctx, double* bad_pivot); // the smoothed-aggregation hierarchy of the resident matrix (eager set-up)
+int solver_amg_build(ipcgpu_ctx* ctx, double* bad_pivot); // the smoothed-aggregation hierarchy of the resident matrix (set-up)
 void solver_amg_step(ipcgpu_ctx* ctx, bool start);        // (iteration: the CG update first) one W-cycle z = M^-1 r, partials of r.z and r.r
 size_t solver_amg_bytes(const ipcgpu_ctx* ctx);           // device memory the AMG workspace holds
+int solver_amg_reserve(ipcgpu_ctx* ctx, double headroom);  // ipcgpu_amg_reserve (the hierarchy of the last set-up read back first)
+bool solver_amg_reserved(ipcgpu_ctx* ctx);                 // a reservation that still fits the mesh and pattern (another one is dropped)
+int solver_amg_read(ipcgpu_ctx* ctx);                      // AmgDev into AmgWork::h (synchronises)
+int solver_amg_coarse_enough(ipcgpu_ctx* ctx, int rows);   // the "at most rows block rows is the last level" rule, in device memory
 int solver_adopt_direction(ipcgpu_ctx* ctx, const double* src); // src NULL: the direction already in ctx->dir
 // (sign g_i) / a(i,i) into out; jacobi: initX option 5's predictor (0 on Dirichlet vertices and the obstacle tail, no status words)
 void solver_precondition_diag(ipcgpu_ctx* ctx, double sign, double* out, bool jacobi);

@@ -149,25 +149,46 @@ struct MultilevelWork {
 
 // smoothed-aggregation multigrid preconditioner (amg.cu): per level the block CSR matrix (3 x 3 blocks), the inverses of its diagonal
 // blocks, the aggregates, the prolongator P and its transpose R (block CSR), the cycle's vectors; shared scratch of the set-up
+// Every size of the hierarchy lives in device memory (AmgDev), so that a reserved set-up runs inside a graph; the host reads it back
+// only to grow buffers (unreserved) or to answer a getter.
 constexpr int kAmgMaxLevels = 6;
+constexpr int kAmgDegree = 16;
+// the entry counts of one coarsening (level l -> l + 1) that a reservation bounds: blocks of P (and R), entries of the A P expansion, blocks
+// of A P, entries of the R (A P) expansion, blocks of A_{l+1}
+enum { kAmgQP = 0, kAmgQApExp, kAmgQAp, kAmgQRapExp, kAmgQCoarse, kAmgQty };
+struct AmgDev {
+    int n[kAmgMaxLevels];                 // block rows (0: not built by the last set-up)
+    int nnzb[kAmgMaxLevels];              // kept blocks
+    int np[kAmgMaxLevels];                // blocks of P (0 on the last level)
+    int na[kAmgMaxLevels];                // aggregates of the coarsening of level l
+    int go[kAmgMaxLevels];                // level l is coarsened (cleared by a stopping rule or a capacity cut)
+    int levels, fail, cut_level, coarse_enough; // fail: a pivot <= 0, a non-finite rho or bound, a bad layout; cut_level: -1 = not cut
+    int cut_depth, pad_;                  // cut_depth: the cut is the reserved depth (the set-up wanted one more level)
+    long long need[kAmgMaxLevels][kAmgQty]; // what the last set-up needed (counted even where it was cut)
+    double rho[kAmgMaxLevels], rho_g[kAmgMaxLevels], omega[kAmgMaxLevels]; // rho_g: the Gershgorin bound of D^-1 A
+    double inv_theta[kAmgMaxLevels], c[kAmgMaxLevels][kAmgDegree][2]; // Chebyshev: 1 / theta, (c1, c2) of step k
+};
 struct AmgLevel {
     DevBuf<int> ia, ja, agg, pia, pja, ria, rja;
     DevBuf<double> blk, dinv, pblk, rblk;
     DevBuf<double> f, x, r, d0, d1, t; // (level 0 takes f and x from the Krylov loop: r and z)
-    int n = 0, nnzb = 0, np = 0;       // block rows, kept blocks, blocks of P (0 on the last level)
-    double rho = 0.0, omega = 0.0;     // spectral radius of D^-1 A (power iteration), prolongator damping (0 on the last level)
-    double theta = 0.0, c1[16] = {}, c2[16] = {}; // Chebyshev: 1 / theta for the first direction, the recurrence's coefficients
+    long long cap_n = 0, cap_nnzb = 0, cap[kAmgQty] = {}; // the sizes the buffers hold (rows, kept blocks, the coarsening's counts)
 };
 struct AmgWork {
     AmgLevel lv[kAmgMaxLevels];
-    int levels = 0;
-    bool built = false;                                 // the last AMG solve built the whole hierarchy (every pivot positive, rho finite)
-    DevBuf<int> cnt, scan_out, m1, m2, key, pos, lidx, ridx, skey, spos, prow;
-    DevBuf<unsigned long long> tkey, tkey_sorted;
+    int levels = 0;                                     // levels of the cycle: the built ones (unreserved), the reserved depth otherwise
+    int reserved = 0;                                   // reserved depth L_r (ipcgpu_amg_reserve); 0: the set-up reads sizes back and grows
+    int res_nV = 0;                                     // the mesh the reservation was sized for (another one drops it)
+    bool ran = false;                                   // a set-up was enqueued (AmgDev holds its result)
+    DevBuf<AmgDev> dev;
+    AmgDev h{};                                         // host copy of dev (read by the getters)
+    DevBuf<int> cnt, scan_out, m1, m2, pos, lidx, ridx, spos, prow, api, apj;
+    DevBuf<double> apb;                                 // A P of the coarsening in flight
+    DevBuf<unsigned long long> key, skey, tkey, tkey_sorted; // (row, column) keys of a product's entries; (column, row) keys of R
     DevBuf<unsigned char> state0, state1, tmp;
-    DevBuf<int> flags;                                  // [0] undecided rows, [1] bad layout, [2] bad pivot
+    DevBuf<int> flags;                                  // [1] bad layout, [2] bad pivot
     DevBuf<unsigned long long> absrow;                  // max absolute row sum of D^-1 A (ordered bits)
-    DevBuf<double> part, sq;                            // power iteration: per-CTA partials, squared norms of every step
+    DevBuf<double> part, sq;                            // power iteration: per-chunk partials, squared norms of every step
 };
 
 // point-in-tetrahedron half of the intersection check (safeguard.cu): the codimension-0 vertices (vCoDim == 0) of ipcgpu_set_surface, and
@@ -340,14 +361,14 @@ struct ipcgpu_ctx {
     ipcgpu::PatternWork pw;
     // device-resident linear solve (solve.cu): full-row structure of the symmetric matrix, built on the device whenever the pattern's
     // version differs from the one it was built for (fp_cnt / fp_start / fp_cur / fp_tmp: counts, scan, scatter cursors, scan scratch),
-    // + PCG workspace.  solve_epoch[m]: the epoch of the last eager solve of the block-Jacobi (0) / multilevel (1) solver, whose lazy
+    // + PCG workspace.  solve_epoch[m]: the epoch of the last eager solve of the block-Jacobi (0) / multilevel (1) / reserved AMG (2) solver, whose lazy
     // allocations a capture relies on; sv_pending: a solve was enqueued since ipcgpu_solve_info read it
     ipcgpu::DevBuf<int> fia, fja, fpos, fp_cnt, fp_start, fp_cur;
     ipcgpu::DevBuf<unsigned char> fp_tmp;
     ipcgpu::DevBuf<double> sol, pcg_b, pcg_r, pcg_p, pcg_q, pcg_minv, pcg_scal, pcg_part; // (pcg_part: per-CTA partials of the dot products)
     ipcgpu::MultilevelWork ml;
     ipcgpu::AmgWork amg;
-    uint64_t solve_epoch[2] = { ~0ull, ~0ull };
+    uint64_t solve_epoch[3] = { ~0ull, ~0ull, ~0ull };
     bool sv_pending = false, sv_pending_at_capture = false;
     // an elastic gradient / Hessian call wrote g / a since the last ipcgpu_set_state, ipcgpu_set_mesh or pattern change: what the diagonal
     // preconditioning (ipcgpu_precondition_diag, ipcgpu_warm_start option 5) reads is the system at the current state

@@ -79,11 +79,14 @@ struct IterState {
     int kappa_needs_init;             // postLineSearch met kappa == 0: initKappa is due
     int kappa_hit;                    // a saved close entry is not farther than its snapshot (the check in flight)
     int kappa_skip;                   // the check in flight found kappa == 0: no snapshot
+    // aggregation rounds of the AMG set-up (amg.cu, kAmgRound): passes run, the pass limit (0: the level is not coarsened), rows left
+    // undecided by the last pass, the limit was reached
+    int amg_round, amg_limit, amg_undecided, amg_stuck;
 };
 // step_decide operations (step_control.cu) and the energy terms of a line search.  kSolveStart / kSolveBurst: the Krylov loops of both
-// built-in solvers (solve.cu, multilevel.cu)
+// built-in solvers (solve.cu, multilevel.cu); kAmgRound: the aggregation rounds of the AMG set-up (amg.cu)
 enum { kCflBranch = 0, kCflClamp, kLsEntry, kLsStart, kLsInversion, kLsIntersection, kLsArmijo, kLsPostCheck, kLsPostLoop, kLsRebuild, kWsEntry, kSolveStart,
-    kSolveBurst };
+    kSolveBurst, kAmgRound };
 // bytes of IterState from ls_cond on that an eager decision reads back: the decision word and the solve's words (one copy)
 constexpr size_t kDecisionBytes = offsetof(IterState, sv_tol) - offsetof(IterState, ls_cond);
 enum { kTermInertia = 1, kTermFriction = 2, kTermHalfSpace = 4, kTermHalfSpaceFriction = 8, kTermDamping = 16, kTermNeumann = 32, kTermDirichlet = 64 };

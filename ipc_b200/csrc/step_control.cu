@@ -181,6 +181,18 @@ __global__ void k_step_decide(IterState* st, int op, double a, int b, cudaGraphC
         }
         cond = st->sv_run && st->sv_iters + b <= st->sv_max_iter;
         break;
+    case kAmgRound: // before each pass of aggregation rounds: the first pass of a coarsened level, then while a row is undecided.  A pass
+                    // beyond amg_limit (the level's rows: every round decides a row) stops the loop and raises amg_stuck
+        cond = st->amg_limit > 0 && (st->amg_round == 0 || st->amg_undecided > 0);
+        if (cond && st->amg_round > st->amg_limit) {
+            cond = 0;
+            st->amg_stuck = 1;
+        }
+        if (cond) {
+            ++st->amg_round;
+            st->amg_undecided = 0;
+        }
+        break;
     }
     st->ls_cond = cond;
     if (h) cudaGraphSetConditional(h, (unsigned)cond);

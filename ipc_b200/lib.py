@@ -111,6 +111,9 @@ SIGNATURES = {
     "ipcgpu_solve_pcg_amg": (C.c_int, [_ctxp, _dp, C.c_double, C.c_int, _dp, C.c_int, _ip, _dp]),
     "ipcgpu_amg_info": (C.c_int, [_ctxp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _dp, _dp, C.POINTER(C.c_uint64)]),
     "ipcgpu_amg_debug_level": (C.c_int, [_ctxp, C.c_int, _ip, _ip, _ip, _dp]),
+    "ipcgpu_amg_reserve": (C.c_int, [_ctxp, C.c_double]),
+    "ipcgpu_amg_capacity_info": (C.c_int, [_ctxp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "ipcgpu_amg_debug_coarse_enough": (C.c_int, [_ctxp, C.c_int]),
     "ipcgpu_allreduce_grad_hess": (C.c_int, [_ctxp, C.c_int, C.c_int]),
     "ipcgpu_download": (C.c_int, [_ctxp, C.c_int, _dp, C.c_uint64]),
     "ipcgpu_device_ptr": (C.c_void_p, [_ctxp, C.c_int]),
@@ -978,10 +981,25 @@ class Context:
         self._ck(self.lib.ipcgpu_multilevel_debug_matrices(self.h, _d(out), out.size))
         return [a.reshape(-1, 96, 96) for a in np.split(out, np.cumsum([9216 * d for d in domains])[:-1])]
 
-    def solve_pcg_amg(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False):
+    def solve_pcg_amg(self, rhs=None, rel_tol=1e-8, max_iter=2000, want_x=True, adopt=False, deferred=False):
         """solve_pcg with the smoothed-aggregation multigrid preconditioner (linearSolver AMGCL, rebuilt from the resident matrix at every
-        call; not capturable).  want_x=False with rhs=None leaves the solution on the device; the result is also solve_info()"""
-        return self._solve(self.lib.ipcgpu_solve_pcg_amg, rhs, rel_tol, max_iter, want_x, adopt, False)
+        call; capturable in its deferred form after amg_reserve()).  want_x=False with rhs=None leaves the solution on the device; the
+        result is also solve_info()"""
+        return self._solve(self.lib.ipcgpu_solve_pcg_amg, rhs, rel_tol, max_iter, want_x, adopt, deferred)
+
+    def amg_reserve(self, headroom=1.5):
+        """size every AMG set-up buffer from the last hierarchy (headroom x its entry counts): the solve then runs inside a capture"""
+        self._ck(self.lib.ipcgpu_amg_reserve(self.h, float(headroom)))
+
+    def amg_capacity_info(self):
+        """(cut_at_level, needed, reserved) of the last AMG set-up: needed / reserved are (6 levels, 5 counts) arrays"""
+        cut, need, res = C.c_int(), (C.c_int64 * 30)(), (C.c_int64 * 30)()
+        self._ck(self.lib.ipcgpu_amg_capacity_info(self.h, C.byref(cut), need, res))
+        return cut.value, np.array(need[:]).reshape(6, 5), np.array(res[:]).reshape(6, 5)
+
+    def amg_debug_coarse_enough(self, rows=1000):
+        """test hook: a level with at most `rows` block rows is the last"""
+        self._ck(self.lib.ipcgpu_amg_debug_coarse_enough(self.h, int(rows)))
 
     def amg_info(self):
         """dict of the last AMG hierarchy: rows, blocks, rho, omega (one entry per level) and bytes"""
