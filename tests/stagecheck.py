@@ -2,22 +2,14 @@
 reference-style (hashed) drivers on all host cores.  Integer sets identical (as sorted multisets when the device order is not canonical),
 E / g <= 1e-10 relative, CSR values <= 1e-9, step bounds bit-exact.  Size-independent properties ride along."""
 import os
-import struct
 
 import numpy as np
 
 import oracle as orc
+from gpu_common import load_scene, rel, scalar_bits
 from ipc_b200 import lib as L
 
 RTOL = 1e-10
-
-
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
-def rel(a, b):
-    return np.linalg.norm(np.asarray(a) - np.asarray(b)) / max(np.linalg.norm(b), 1e-300)
 
 
 def sort_rows(a, *companions):
@@ -42,9 +34,7 @@ def check_every_stage(ctx, m, info, kappa=1e8, dt2=0.025 ** 2, tol=1e-6, canonic
     nth = os.cpu_count() or 8
     dHat, p = info["dHat"], info["p"]
     hvox = m.avgEdgeLen / 3.0
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
     ctx.set_canonical_order(1 if canonical else 0)
     ctx.set_contact_partition(0 if canonical else 1)  # (a no-op on one rank; this is the exact mode bench.py times)
     o, s = orc.Elastic(m), orc.Surf(m)
@@ -101,11 +91,11 @@ def check_every_stage(ctx, m, info, kappa=1e8, dt2=0.025 ** 2, tol=1e-6, canonic
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)  # computeTightInclusionError uses mesh.V only (CCDUtils.cpp:29-46)
     al = ctx.ccd_partial(p, tol, evf, eee, al_r)
     al_r, _ = orc.ccd_partial(s, p, cand_r, tol, evf, eee, al_r, nth)
-    assert bits(al) == bits(al_r), (al, al_r)
+    assert scalar_bits(al) == scalar_bits(al_r), (al, al_r)
     ag = ctx.hash_build_swept(p, al, hvox)
     al2, ncand = ctx.ccd_full(tol, evf, eee, ag)
     al2_r, _, npairs = orc.ccd_full_hashed(s, p, al_r, hvox, tol, evf, eee, nth)
-    assert ncand == npairs and bits(al2) == bits(al2_r), (ncand, npairs, al2, al2_r)
+    assert ncand == npairs and scalar_bits(al2) == scalar_bits(al2_r), (ncand, npairs, al2, al2_r)
     assert ctx.ccd_stats()[2] == 0  # no conservative early-out was needed
     assert 0.0 < al2 <= 1.0
     out["alpha"], out["n_full_cand"] = al2, int(ncand)

@@ -10,8 +10,8 @@ import scipy.sparse.linalg as spla
 
 import amg_mirror as am
 import multilevel_mirror as mlm
+from gpu_common import rel
 from ipc_b200 import scenes
-from stagecheck import rel
 from test_multilevel_cpu import DT2, ball_on_mat_system
 
 

@@ -23,12 +23,12 @@ on the device.
 """
 import importlib.util
 import os
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import load_scene, own_context, scalar_bits
 from ipc_b200 import mesh as M
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -41,10 +41,6 @@ EXCLUDED = {0, 1, 9, 48, 49}
 # exits and no_zero_toi branches no finishing pair of the fixture takes (DESIGN §4)
 UNCOVERED_EXITS = {"k2", "skip", "depth60"}
 OLD_LEVEL_CAP = 4096  # the device's per-warp level buffers, which used to end a search that outgrew them
-
-
-def bits(x):
-    return struct.pack("<d", x)
 
 
 def gold():
@@ -209,12 +205,6 @@ def test_old_level_cap_rule_spins_where_the_library_stops():
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------------------------------
-def upload(ctx, m):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
-
-
 def expected(r, toi, mt):
     return 0.0 if r < 0 else (toi if r == 1 else mt)
 
@@ -230,17 +220,15 @@ def bounded(tr, keys):
 def own_ctx():
     """a context of its own: the early-outs these searches take add to the warning count that the next fetch_iteration of the same
     context reports, and the other tests' contexts must not see them"""
-    from ipc_b200 import lib as L
-    ctx = L.Context(0)
-    yield ctx
-    ctx.close()
+    with own_context() as ctx:
+        yield ctx
 
 
 @pytest.mark.gpu
 def test_each_pair_alone_matches_the_oracle(own_ctx):
-    gpu_ctx = own_ctx
+    ctx = own_ctx
     z, m, tr = fixture_traces()
-    upload(gpu_ctx, m)
+    load_scene(ctx, m)
     p = z["p"].ravel()
     mm0, pe0 = np.empty((0, 4), dtype=np.int32), np.empty((0, 2), dtype=np.int32)
     cands = candidates(m, z)
@@ -251,29 +239,29 @@ def test_each_pair_alone_matches_the_oracle(own_ctx):
     try:
         for k in run:
             cand = np.array([cands[k][0]], dtype=np.int32)
-            gpu_ctx.set_constraint_set(mm0, mm0, pe0, cand)
+            ctx.set_constraint_set(mm0, mm0, pe0, cand)
             for q, mt in enumerate(z["max_t"]):
                 r, toi, t, err = tr[(k, q)]
                 want = expected(r, toi, float(mt))
                 a_ref, _ = orc.ccd_partial(s, p, cand, TOL, err, err, float(mt))
-                assert bits(a_ref) == bits(want), (k, q)  # the traced pair is the pair the narrow phase reads
+                assert scalar_bits(a_ref) == scalar_bits(want), (k, q)  # the traced pair is the pair the narrow phase reads
                 for budget in (-1, 0, 1 << 40):
-                    gpu_ctx.ccd_debug_thread_budget(budget)
-                    a = gpu_ctx.ccd_partial(p, TOL, err, err, float(mt))
-                    warn = gpu_ctx.ccd_stats()[2]
-                    if bits(a) != bits(want) or warn != t["early_outs"]:
+                    ctx.ccd_debug_thread_budget(budget)
+                    a = ctx.ccd_partial(p, TOL, err, err, float(mt))
+                    warn = ctx.ccd_stats()[2]
+                    if scalar_bits(a) != scalar_bits(want) or warn != t["early_outs"]:
                         bad.append((k, q, budget, a, want, warn, t["early_outs"]))
     finally:
-        gpu_ctx.ccd_debug_thread_budget(-1)
+        ctx.ccd_debug_thread_budget(-1)
     assert not bad, bad
 
 
 @pytest.mark.gpu
 def test_whole_soup_in_one_call(own_ctx):
     """all pairs in one candidate list with one err: the minimum over the pairs, twice, at each budget"""
-    gpu_ctx = own_ctx
+    ctx = own_ctx
     z, m, tr = fixture_traces()
-    upload(gpu_ctx, m)
+    load_scene(ctx, m)
     p = z["p"].ravel()
     cands = candidates(m, z)
     err = np.full(3, 1e-13)
@@ -291,15 +279,15 @@ def test_whole_soup_in_one_call(own_ctx):
     assert len(keep) >= 40
     cand = np.array([cands[k][0] for k in keep], dtype=np.int32)
     mm0, pe0 = np.empty((0, 4), dtype=np.int32), np.empty((0, 2), dtype=np.int32)
-    gpu_ctx.set_constraint_set(mm0, mm0, pe0, cand)
+    ctx.set_constraint_set(mm0, mm0, pe0, cand)
     s = orc.Surf(m)
     try:
         for q, mt in enumerate(z["max_t"]):
             a_ref, _ = orc.ccd_partial(s, p, cand, TOL, err, err, float(mt), nthreads=8)
-            assert bits(a_ref) == bits(best[q])
+            assert scalar_bits(a_ref) == scalar_bits(best[q])
             for budget in (-1, 0, 1 << 40):
-                gpu_ctx.ccd_debug_thread_budget(budget)
+                ctx.ccd_debug_thread_budget(budget)
                 for _ in range(2):
-                    assert bits(gpu_ctx.ccd_partial(p, TOL, err, err, float(mt))) == bits(a_ref), (q, budget)
+                    assert scalar_bits(ctx.ccd_partial(p, TOL, err, err, float(mt))) == scalar_bits(a_ref), (q, budget)
     finally:
-        gpu_ctx.ccd_debug_thread_budget(-1)
+        ctx.ccd_debug_thread_budget(-1)

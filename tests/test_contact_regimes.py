@@ -42,6 +42,7 @@ import scipy.sparse as sps
 
 import oracle as orc
 import refpairs
+from gpu_common import load_scene, shared_ctx
 from ipc_b200 import mesh as M
 from test_elastic_regimes import csr_of_blocks
 
@@ -350,15 +351,6 @@ def test_reference_codegen_matches_fixture():
 # ---------------------------------------------------------------------------------------------------------------------------------------
 # GPU (through the C ABI only)
 # ---------------------------------------------------------------------------------------------------------------------------------------
-def upload(ctx, m):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, None, None, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
-    ia, ja = m.csr_pattern(1)
-    ctx.set_csr(ia, ja, 1)
-    return ia, ja
-
-
 def gpu_hessian(ctx, m, ia, ja, mm, pa, pe, dHat, kappa):
     ctx.set_constraint_set(mm, pa, pe)
     a = np.zeros(ja.size)
@@ -367,29 +359,31 @@ def gpu_hessian(ctx, m, ia, ja, mm, pa, pe, dHat, kappa):
 
 
 @pytest.mark.gpu
-def test_barrier_kernels_match_fixture(gpu_ctx):
+def test_barrier_kernels_match_fixture(shared_ctx):
     z = gold()
     m = soup_mesh(z)
-    ia, ja = upload(gpu_ctx, m)
+    load_scene(shared_ctx, m, mass=False, dbc=False)
+    ia, ja = m.csr_pattern(1)
+    shared_ctx.set_csr(ia, ja, 1)
     rep = Report(z, "gpu")
     n = z["E"].size
     for (dHat, kappa), ks in groups(z, range(n)).items():
         a_idx, p_idx, mm, pa, pe = lists(z, ks)
         # d of every pair (the mollified pairs' encodings are valid active encodings of the same distance)
-        gpu_ctx.set_constraint_set(np.concatenate([mm, pa]), pa[:0], pe[:0])
-        d = dict(zip(np.concatenate([a_idx, p_idx]), gpu_ctx.evaluate_constraints(len(ks))))
+        shared_ctx.set_constraint_set(np.concatenate([mm, pa]), pa[:0], pe[:0])
+        d = dict(zip(np.concatenate([a_idx, p_idx]), shared_ctx.evaluate_constraints(len(ks))))
         # energy one pair at a time, and of the whole group
         E = {}
         for k in ks:
             one = (z["mm"][k][None], pa[:0], pe[:0]) if not z["moll"][k] else (mm[:0], z["mm"][k][None], z["pe"][k][None])
-            gpu_ctx.set_constraint_set(*one)
-            E[k] = gpu_ctx.barrier_energy(dHat, kappa)
-        gpu_ctx.set_constraint_set(mm, pa, pe)
-        E_sum = gpu_ctx.barrier_energy(dHat, kappa)
+            shared_ctx.set_constraint_set(*one)
+            E[k] = shared_ctx.barrier_energy(dHat, kappa)
+        shared_ctx.set_constraint_set(mm, pa, pe)
+        E_sum = shared_ctx.barrier_energy(dHat, kappa)
         tot = sum(abs(v) for v in E.values())
         assert abs(E_sum - sum(E.values())) <= 4 * len(ks) * EPS * tot, (dHat, kappa)
-        g = gpu_ctx.barrier_gradient(dHat, kappa, np.zeros(3 * m.nV)).reshape(-1, 3)
-        a = gpu_hessian(gpu_ctx, m, ia, ja, mm, pa, pe, dHat, kappa)
+        g = shared_ctx.barrier_gradient(dHat, kappa, np.zeros(3 * m.nV)).reshape(-1, 3)
+        a = gpu_hessian(shared_ctx, m, ia, ja, mm, pa, pe, dHat, kappa)
         Hb = blocks_of_csr(a, ia, ja, m.nV, m.T)
         # one contribution per CSR entry: the group's blocks rebuild the CSR exactly, nothing lands outside them
         only = np.zeros((n, 12, 12))
@@ -408,7 +402,7 @@ def rotations(n):
 
 
 @pytest.mark.gpu
-def test_projection_does_not_depend_on_the_slot(gpu_ctx):
+def test_projection_does_not_depend_on_the_slot(shared_ctx):
     """the whole soup under one dHat and kappa.  dHat is the d of the early_return stencils, so their blocks are exactly zero and take
     makePD's early return whatever the rounding (their projection groups leave the shuffles early); they share warps with clamped blocks
     of widely spread spectra (d / dHat down to 1e-23) and slow-converging ones, and with pairs beyond dHat.  The CSR values are
@@ -416,48 +410,52 @@ def test_projection_does_not_depend_on_the_slot(gpu_ctx):
     stencils are disjoint)."""
     z = gold()
     m = soup_mesh(z)
-    ia, ja = upload(gpu_ctx, m)
+    load_scene(shared_ctx, m, mass=False, dbc=False)
+    ia, ja = m.csr_pattern(1)
+    shared_ctx.set_csr(ia, ja, 1)
     n = z["E"].size
     er = np.flatnonzero(z["family"] == list(z["families"]).index("early_return"))
     dHat, kappa = float(z["dHat"][er[0]]), 1.0
     assert np.all(z["d"][er] == dHat)
     a_idx, p_idx, mm, pa, pe = lists(z, range(n))
-    ref = gpu_hessian(gpu_ctx, m, ia, ja, mm, pa, pe, dHat, kappa)
+    ref = gpu_hessian(shared_ctx, m, ia, ja, mm, pa, pe, dHat, kappa)
     assert np.count_nonzero(ref) > 0 and np.all(np.isfinite(ref))
     assert not np.any(blocks_of_csr(ref, ia, ja, m.nV, m.T[er]))
     for oa, op in zip(rotations(len(mm)), rotations(len(pa))[::-1]):
-        a = gpu_hessian(gpu_ctx, m, ia, ja, mm[oa], pa[op], pe[op], dHat, kappa)
+        a = gpu_hessian(shared_ctx, m, ia, ja, mm[oa], pa[op], pe[op], dHat, kappa)
         assert np.array_equal(a, ref)
-    act = gpu_hessian(gpu_ctx, m, ia, ja, mm, pa[:0], pe[:0], dHat, kappa)
-    par = gpu_hessian(gpu_ctx, m, ia, ja, mm[:0], pa, pe, dHat, kappa)
+    act = gpu_hessian(shared_ctx, m, ia, ja, mm, pa[:0], pe[:0], dHat, kappa)
+    par = gpu_hessian(shared_ctx, m, ia, ja, mm[:0], pa, pe, dHat, kappa)
     assert not np.any((act != 0) & (par != 0))
     assert np.array_equal(act + par, ref)
 
 
 @pytest.mark.gpu
-def test_friction_kernels_match_fixture(gpu_ctx):
+def test_friction_kernels_match_fixture(shared_ctx):
     z = gold()
     m = soup_mesh(z)
-    ia, ja = upload(gpu_ctx, m)
-    gpu_ctx.set_prev_state(np.ascontiguousarray(z["V_prev"].T).ravel())
+    load_scene(shared_ctx, m, mass=False, dbc=False)
+    ia, ja = m.csr_pattern(1)
+    shared_ctx.set_csr(ia, ja, 1)
+    shared_ctx.set_prev_state(np.ascontiguousarray(z["V_prev"].T).ravel())
     rep = Report(z, "gpu")
     coef = float(z["coef"])
     for (dHat, kappa), ks in groups(z, np.flatnonzero(z["fric"])).items():
         mm = z["mm"][ks]
-        gpu_ctx.set_constraint_set(mm, np.zeros((0, 4), np.int32), np.zeros((0, 2), np.int32))
-        assert gpu_ctx.friction_lag(dHat, kappa) == len(ks)
-        mm_l, lam, co, ba = gpu_ctx.get_friction_data()
+        shared_ctx.set_constraint_set(mm, np.zeros((0, 4), np.int32), np.zeros((0, 2), np.int32))
+        assert shared_ctx.friction_lag(dHat, kappa) == len(ks)
+        mm_l, lam, co, ba = shared_ctx.get_friction_data()
         assert np.array_equal(mm_l, mm)
         for j, k in enumerate(ks):
             check_lag(rep, z, k, lam[j], co[j], ba[j])
             for dev, data in ((True, (lam[j], co[j], ba[j])), (False, (z["lam"][k], z["coord"][k], z["basis"][k]))):
                 if dev and z["near_branch"][k]:
                     continue
-                gpu_ctx.set_friction_data(mm[j:j + 1], np.atleast_1d(data[0]), data[1][None], data[2][None])
+                shared_ctx.set_friction_data(mm[j:j + 1], np.atleast_1d(data[0]), data[1][None], data[2][None])
                 eps2 = float(z["eps2"][k])
-                E = gpu_ctx.friction_energy(eps2, coef)
-                g = gpu_ctx.friction_gradient(eps2, coef, np.zeros(3 * m.nV)).reshape(-1, 3)
-                a = gpu_ctx.friction_hessian(eps2, coef, 1, np.zeros(ja.size))
+                E = shared_ctx.friction_energy(eps2, coef)
+                g = shared_ctx.friction_gradient(eps2, coef, np.zeros(3 * m.nV)).reshape(-1, 3)
+                a = shared_ctx.friction_hessian(eps2, coef, 1, np.zeros(ja.size))
                 H = blocks_of_csr(a, ia, ja, m.nV, m.T[k:k + 1])[0]
                 assert np.count_nonzero(g) == np.count_nonzero(g[m.T[k]])
                 check_friction(rep, z, k, E, g[m.T[k]].ravel(), H, dev)

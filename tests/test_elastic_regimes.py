@@ -29,6 +29,7 @@ import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import shared_ctx
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 
@@ -237,10 +238,10 @@ def csr_of_blocks(m, H, ia, ja):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("et", [0, 1])
-def test_kernels_match_fixture(gpu_ctx, et):
+def test_kernels_match_fixture(shared_ctx, et):
     z = gold()
     idx, m = subset(z, et)
-    out = run_gpu(gpu_ctx, m)
+    out = run_gpu(shared_ctx, m)
     worst = check(z, idx, out["E"], out["g"], out["H"], out["Hp"], "gpu")
     print(f"energy {et}: {fixture_counts(z)}; worst error / bar per family:")
     for (f, kind), r in sorted(worst.items()):
@@ -261,7 +262,7 @@ def test_kernels_match_fixture(gpu_ctx, et):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("et", [0, 1])
-def test_tile_slot_does_not_change_a_tet(gpu_ctx, et):
+def test_tile_slot_does_not_change_a_tet(shared_ctx, et):
     """the same soup uploaded in an order that moves every tet to another slot of its 64-tet tile gives bit-identical per-tet results"""
     z = gold()
     n = int((z["energy"] == et).sum())
@@ -273,8 +274,8 @@ def test_tile_slot_does_not_change_a_tet(gpu_ctx, et):
             break
     assert order is not None and np.array_equal(np.sort(order), np.arange(n))
     _, m0 = subset(z, et)
-    a = run_gpu(gpu_ctx, m0)
+    a = run_gpu(shared_ctx, m0)
     _, m1 = subset(z, et, order)
-    b = run_gpu(gpu_ctx, m1)
+    b = run_gpu(shared_ctx, m1)
     for k in ("E", "g", "H78", "Hp78"):
         assert np.array_equal(a[k][order], b[k]), k

@@ -8,11 +8,11 @@ import scipy.sparse.linalg as spla
 
 import amg_mirror as am
 import multilevel_mirror as mlm
+from gpu_common import own_context, rel, same_bits, shared_ctx, soa
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from ipc_b200 import scenes
-from stagecheck import rel
-from test_gpu_multilevel import DT2, assemble, launches_of_25_more_iterations, resident_system, same_bits, soa, states, upload
+from test_gpu_multilevel import DT2, assemble, launches_of_25_more_iterations, load_sorted, resident_system, states
 
 pytestmark = pytest.mark.gpu
 
@@ -33,8 +33,8 @@ def compare_hierarchy(ctx, A):
         assert abs(h["omega"][l] - om) <= 1e-12 * max(om, 1e-300), (l, h["omega"][l], om)
 
 
-def test_hierarchy_application_and_iterations_equal_the_mirror(gpu_ctx):
-    ctx = gpu_ctx
+def test_hierarchy_application_and_iterations_equal_the_mirror(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
     ia, ja = assemble(ctx, m, info["dHat"], 1e6)
     n = 3 * m.nV
@@ -58,8 +58,8 @@ def test_hierarchy_application_and_iterations_equal_the_mirror(gpu_ctx):
     assert abs(iters - it_m) <= 25 and rel(x, xm) <= 1e-8
 
 
-def test_two_solves_give_identical_bits_and_the_launches_of_the_cycle(gpu_ctx):
-    ctx = gpu_ctx
+def test_two_solves_give_identical_bits_and_the_launches_of_the_cycle(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     assemble(ctx, m, info["dHat"], 1e8)
     x1, it1, res1 = ctx.solve_pcg_amg(None, rel_tol=1e-8, max_iter=5000)
@@ -76,11 +76,11 @@ def test_two_solves_give_identical_bits_and_the_launches_of_the_cycle(gpu_ctx):
     assert launches_of_25_more_iterations(ctx, ctx.solve_pcg_amg) == 25 * (67 * 2 ** (Lv - 1) - 32) + 1
 
 
-def test_device_built_pattern_after_a_pattern_change(gpu_ctx):
-    ctx = gpu_ctx
+def test_device_built_pattern_after_a_pattern_change(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
     dHat, kappa = info["dHat"], 1e6
-    upload(ctx, m)
+    load_sorted(ctx, m)
     S = states(ctx, m, info)
     ctx.enable_device_pattern(1)
     for name in ("A", "B"):
@@ -101,15 +101,15 @@ def test_device_built_pattern_after_a_pattern_change(gpu_ctx):
     assert abs(mlm.pcg(H, -g, A.apply, 1e-10, 5000)[1] - iters) <= 25
 
 
-def test_obstacle_tail_and_dirichlet_vertices(gpu_ctx):
+def test_obstacle_tail_and_dirichlet_vertices(shared_ctx):
     from ipc_b200 import obstacle as OB
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = scenes.balls_on_obstacle(plate_angle=0.0, res=4, plate=12)
     ob = info["obstacle"]
     M2 = OB.with_obstacle(m, ob["V"], ob["E"], ob["F"])
     M2.dbc = M2.dbc.copy()
     M2.dbc[:5] = 1
-    upload(ctx, M2)
+    load_sorted(ctx, M2)
     ctx.set_obstacle_tail(M2.nV_dof, 1)
     try:
         ctx.enable_device_pattern(1)
@@ -144,8 +144,7 @@ def test_obstacle_tail_and_dirichlet_vertices(gpu_ctx):
 
 
 def test_not_positive_definite_is_an_error_and_not_a_hang():
-    ctx = L.Context(0)
-    try:
+    with own_context() as ctx:
         V, T = M.grid_tets(2, 2, 2)
         m = M.Mesh(V, T, energy=0)
         ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, 0)
@@ -160,13 +159,10 @@ def test_not_positive_definite_is_an_error_and_not_a_hang():
         ctx.elastic_grad_hess(DT2, 1, 1, 1, None, None)
         x, iters, res = ctx.solve_pcg_amg(np.ones(3 * m.nV), rel_tol=1e-10, max_iter=1000)
         assert res <= 1e-10 and np.isfinite(x).all()
-    finally:
-        ctx.close()
 
 
 def test_capture_and_arguments_are_rejected():
-    ctx = L.Context(0)
-    try:
+    with own_context() as ctx:
         with pytest.raises(L.IpcGpuError, match="STATE"):
             ctx.solve_pcg_amg(None)  # no matrix yet
         with pytest.raises(L.IpcGpuError, match="STATE"):
@@ -188,5 +184,3 @@ def test_capture_and_arguments_are_rejected():
         rc = ctx.lib.ipcgpu_solve_pcg_amg(ctx.h, None, 1e-8, 100, None, 0, None, None)  # (the deferred form)
         ctx.capture_end()
         assert rc == L.ERR_STATE
-    finally:
-        ctx.close()

@@ -6,15 +6,18 @@ pattern, also after contacts changed the device-built pattern; a whole captured 
 iterations; the level count moves inside one graph with the coarse-enough hook; a set-up deeper than reserved, or one that outgrows a count,
 is cut short, reported and still converges, and new reservations restore the unreserved bits; a failed solve inside a graph is reported at
 the fetch and leaves V = V0; and the reservation's refusals hold."""
+import contextlib
+
 import numpy as np
 import pytest
 
+from gpu_common import load_scene, own_context, same_bits, soa
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from ipc_b200 import scenes
 from stagecheck import contact_pattern_pairs
 from test_gpu_reproducible import snapshot
-from test_gpu_solve_capture import DT2, pile, same_bits, small_context, soa
+from test_gpu_solve_capture import DT2, pile, small_context
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-8
@@ -36,9 +39,7 @@ SCENES = {"ball_pile": pile, "ball_on_mat": mat}
 
 
 def start(ctx, m, device_pattern):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
     ctx.set_canonical_order(2)
     if device_pattern:
         ctx.enable_device_pattern(1)
@@ -106,11 +107,12 @@ def reserve_until_it_fits(r, headroom):
     raise AssertionError("the set-up is still cut after 24 reservations")
 
 
+@contextlib.contextmanager
 def contexts(m, device_pattern):
-    r, u = L.Context(0), L.Context(0)
-    for c in (r, u):
-        start(c, m, device_pattern)
-    return r, u
+    with own_context() as r, own_context() as u:
+        for c in (r, u):
+            start(c, m, device_pattern)
+        yield r, u
 
 
 # ---- 1, 2. reserved eager and replays equal unreserved eager ---------------------------------------------------------------------------
@@ -119,8 +121,7 @@ def contexts(m, device_pattern):
 def test_reserved_and_replayed_equal_unreserved(name, pattern):
     m, info, S = SCENES[name]()
     dHat, n, dev = info["dHat"], 3 * m.nV, pattern == "device"
-    r, u = contexts(m, dev)
-    try:
+    with contexts(m, dev) as (r, u):
         for c in (r, u):
             assemble(c, m, S["A"], dHat, dev)
         x0, it0, res0 = eager(r)  # (unreserved in both: the two contexts hold one system)
@@ -142,9 +143,6 @@ def test_reserved_and_replayed_equal_unreserved(name, pattern):
             replay_equals_unreserved(r, gid, u, n)
             assert r.amg_capacity_info()[0] == -1
         r.graph_destroy(gid)
-    finally:
-        r.close()
-        u.close()
 
 
 # ---- 3. the whole Newton iteration in one graph --------------------------------------------------------------------------------------
@@ -167,8 +165,7 @@ def test_captured_newton_iteration_equals_unreserved_eager():
     m, info, _ = pile()
     dHat = info["dHat"]
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
-    g, e = contexts(m, True)
-    try:
+    with contexts(m, True) as (g, e):
         newton_iteration(g, m, dHat, evf, eee)  # unreserved: the hierarchy the reservation is sized from
         g.fetch_iteration()
         g.amg_reserve(1.5)
@@ -191,18 +188,13 @@ def test_captured_newton_iteration_equals_unreserved_eager():
                 assert same_bits(sg[key], se[key]), (k, key)
             assert sg["counts"] == se["counts"], k  # (halvings and Krylov iterations)
         g.graph_destroy(gid)
-    finally:
-        g.close()
-        e.close()
 
 
 # ---- 4. the level count moves inside one graph ---------------------------------------------------------------------------------------
 def test_level_count_moves_inside_one_graph():
     m, info, S = pile()
     dHat, n = info["dHat"], 3 * m.nV
-    r, u = contexts(m, True)
-    d = L.Context(0)
-    try:
+    with contexts(m, True) as (r, u), own_context() as d:
         start(d, m, True)
         for c in (r, u, d):
             assemble(c, m, S["A"], dHat)
@@ -241,17 +233,13 @@ def test_level_count_moves_inside_one_graph():
         gid = capture_solve(d, adopt=True)
         replay_equals_unreserved(d, gid, u, n)
         d.graph_destroy(gid)
-    finally:
-        for c in (r, u, d):
-            c.close()
 
 
 # ---- 5. a set-up that outgrows its reservation ---------------------------------------------------------------------------------------
 def test_overflow_is_cut_short_and_new_reservations_restore_the_bits():
     m, info, S = pile()
     dHat, n = info["dHat"], 3 * m.nV
-    r, u = contexts(m, True)
-    try:
+    with contexts(m, True) as (r, u):
         assemble(r, m, S["A"], 1e-8 * dHat)  # (a contact distance of 1e-4 of the scene's: no contact)
         eager(r)
         r.amg_reserve(1.0)  # exactly what the contact-free set-up needed
@@ -272,15 +260,11 @@ def test_overflow_is_cut_short_and_new_reservations_restore_the_bits():
         gid = capture_solve(r, adopt=True)
         replay_equals_unreserved(r, gid, u, n)
         r.graph_destroy(gid)
-    finally:
-        r.close()
-        u.close()
 
 
 # ---- 6. failure, 7. refusals -----------------------------------------------------------------------------------------------------------
 def test_failed_solve_inside_a_graph():
-    ctx, m, nnz = small_context()
-    try:
+    with small_context() as (ctx, m, nnz):
         n, dHat = 3 * m.nV, 1e-8
 
         def sequence():
@@ -307,13 +291,10 @@ def test_failed_solve_inside_a_graph():
             ctx.fetch_iteration()
         assert same_bits(ctx.download(L.BUF_POSITIONS, n), V0)
         ctx.graph_destroy(gid)
-    finally:
-        ctx.close()
 
 
 def test_refusals():
-    ctx = L.Context(0)
-    try:
+    with own_context() as ctx:
         V, T = M.grid_tets(4, 4, 4)
         m = M.Mesh(V, T, energy=0)
         ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, 0)
@@ -336,5 +317,3 @@ def test_refusals():
         with pytest.raises(L.IpcGpuError, match="STATE"):
             ctx.graph_launch(gid)
         ctx.graph_destroy(gid)
-    finally:
-        ctx.close()

@@ -10,6 +10,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from gpu_common import load_scene, own_context, same_bits
 from ipc_b200 import lib as L  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -20,20 +21,13 @@ class _Args:
     tets, res, scene = 1_000_000, 10, "c5"
 
 
-def same_bits(x, y):
-    return np.array_equal(np.asarray(x, dtype=np.float64).view(np.uint64), np.asarray(y, dtype=np.float64).view(np.uint64))
-
-
 def test_c5_captured_amg_solve_equals_the_unreserved_one():
     import bench
     m, info = bench.build_scene(_Args())
     dHat, kappa, n = info["dHat"], bench.KAPPA, 3 * m.nV
-    ctx = L.Context(0)  # (a context of its own: the reservation does not reach the shared one)
-    try:
-        ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-        ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
+    with own_context() as ctx:  # (a context of its own: the reservation does not reach the shared one)
+        load_scene(ctx, m)
         ctx.set_canonical_order(0)
-        ctx.set_state(m.V_soa)
         ctx.enable_device_pattern(1)
         xt = m.V.copy()
         xt[:, 2] -= 9.81 * DT2
@@ -66,5 +60,3 @@ def test_c5_captured_amg_solve_equals_the_unreserved_one():
         assert r.status == 0 and same_bits(p, x0) and r.iterations == it0 and same_bits(r.rel_residual, res0) and h2 == h0
         assert ctx.amg_capacity_info()[0] == -1
         ctx.graph_destroy(gid)
-    finally:
-        ctx.close()

@@ -8,6 +8,8 @@ import sys
 import numpy as np
 import pytest
 
+from gpu_common import load_scene, shared_ctx
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
@@ -19,15 +21,13 @@ class _Args:
     tets, res, scene = 1_000_000, 10, "c5"
 
 
-def test_c5_amg_direction(gpu_ctx):
+def test_c5_amg_direction(shared_ctx):
     import bench
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = bench.build_scene(_Args())
     dHat, kappa = info["dHat"], bench.KAPPA
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
+    load_scene(ctx, m)
     ctx.set_canonical_order(0)
-    ctx.set_state(m.V_soa)
     ctx.enable_device_pattern(1)
     xt = m.V.copy()
     xt[:, 2] -= 9.81 * DT2
@@ -50,4 +50,3 @@ def test_c5_amg_direction(gpu_ctx):
     print(f"C5 iterations to 1e-6: AMG {it_amg}, multilevel {it_ml}, block-Jacobi {it_bj}; AMG levels {h['rows']}, blocks {h['blocks']}, "
           f"rho {h['rho']}, {h['bytes'] / 2**20:.0f} MiB")
     assert it_amg < it_ml, (it_amg, it_ml)
-    ctx.set_canonical_order(1)

@@ -5,6 +5,7 @@ Dirichlet vertices must be dropped (+0.0), with 1.0 on their diagonal."""
 import numpy as np
 import pytest
 
+from gpu_common import shared_ctx
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 
@@ -53,20 +54,20 @@ def reference(m, ia, ja, hblk, dropped):
 
 
 @pytest.mark.parametrize("energy", [0, 1])
-def test_written_assembly_is_the_ordered_sum_of_the_tet_blocks(gpu_ctx, energy):
+def test_written_assembly_is_the_ordered_sum_of_the_tet_blocks(shared_ctx, energy):
     V, T = M.grid_tets(9, 8, 7)
     m = M.Mesh(V, T, energy=energy)
     M.deform(m, 2)
     m.dbc[::17] = 1
     m.dbc[5::23] = 2
-    gpu_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
+    shared_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
     ia, ja = m.csr_pattern(1)
-    gpu_ctx.set_csr(ia, ja, 1)
-    gpu_ctx.set_state(m.V_soa)
+    shared_ctx.set_csr(ia, ja, 1)
+    shared_ctx.set_state(m.V_soa)
     for projectDBC in (0, 1):
         g, a = np.empty(3 * m.nV), np.full(ja.size, np.nan)
-        gpu_ctx.elastic_grad_hess(DT2, 1, projectDBC, 0, g, a)
-        hblk = gpu_ctx.download(L.BUF_TET_HESSIANS, 78 * 64 * ((m.nT + 63) // 64))
+        shared_ctx.elastic_grad_hess(DT2, 1, projectDBC, 0, g, a)
+        hblk = shared_ctx.download(L.BUF_TET_HESSIANS, 78 * 64 * ((m.nT + 63) // 64))
         dropped = (m.dbc == 1) | ((m.dbc == 2) & bool(projectDBC))
         a_ref = reference(m, ia, ja, hblk, dropped)
         assert np.array_equal(a.view(np.uint64), a_ref.view(np.uint64)), projectDBC

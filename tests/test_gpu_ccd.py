@@ -1,25 +1,15 @@
 """GPU parity of the CCD step bound (through the C ABI): BIT-EXACT against the oracle (BASELINE.json north_star)."""
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import load_scene, scalar_bits, shared_ctx
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from ipc_b200 import scenes
 
 pytestmark = pytest.mark.gpu
-
-
-def bits(x):
-    return struct.pack("<d", x)
-
-
-def upload(ctx, m):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
 
 
 def two_body(seed, n=4, gap=0.01, speed=0.05):
@@ -48,43 +38,43 @@ def test_ti_error_matches_oracle():
 
 
 @pytest.mark.parametrize("seed,speed", [(1, 0.05), (2, 0.5), (3, 0.004)])
-def test_partial_ccd_bit_exact(gpu_ctx, seed, speed):
+def test_partial_ccd_bit_exact(shared_ctx, seed, speed):
     m, p = two_body(seed, speed=speed)
     dHat = 0.02 ** 2
-    upload(gpu_ctx, m)
-    mm, pa, pe, cand = gpu_ctx.constraint_set(dHat, 1)
+    load_scene(shared_ctx, m)
+    mm, pa, pe, cand = shared_ctx.constraint_set(dHat, 1)
     s = orc.Surf(m)
     _, _, _, cand_r = s.constraint_set(dHat)
     assert np.array_equal(cand, cand_r) and len(cand) > 0
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, p)
     for alpha0 in (1.0, 0.37):
         a_ref, z = orc.ccd_partial(s, p, cand_r, 1e-6, evf, eee, alpha0, nthreads=8)
-        a = gpu_ctx.ccd_partial(p, 1e-6, evf, eee, alpha0)
-        assert bits(a) == bits(a_ref), (a, a_ref)
-        assert gpu_ctx.ccd_stats()[2] == 0  # no conservative early-outs were taken
-    a_sep = gpu_ctx.ccd_partial(-p, 1e-6, evf, eee, 1.0)  # separating motion: step unchanged
+        a = shared_ctx.ccd_partial(p, 1e-6, evf, eee, alpha0)
+        assert scalar_bits(a) == scalar_bits(a_ref), (a, a_ref)
+        assert shared_ctx.ccd_stats()[2] == 0  # no conservative early-outs were taken
+    a_sep = shared_ctx.ccd_partial(-p, 1e-6, evf, eee, 1.0)  # separating motion: step unchanged
     assert a_sep == 1.0 == orc.ccd_partial(s, -p, cand_r, 1e-6, evf, eee, 1.0)[0]
 
 
 @pytest.mark.parametrize("seed,speed", [(4, 0.05), (5, 0.6)])
-def test_full_ccd_bit_exact(gpu_ctx, seed, speed):
+def test_full_ccd_bit_exact(shared_ctx, seed, speed):
     m, p = two_body(seed, n=3, speed=speed)
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     s = orc.Surf(m)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, p)
     h = m.avgEdgeLen / 3
     g, a_grid_ref = orc.grid_swept(s, p, 1.0, h)
-    a_grid = gpu_ctx.hash_build_swept(p, 1.0, h)
-    assert bits(a_grid) == bits(a_grid_ref)
+    a_grid = shared_ctx.hash_build_swept(p, 1.0, h)
+    assert scalar_bits(a_grid) == scalar_bits(a_grid_ref)
     a_ref, z, npairs = orc.ccd_full(s, p, g, a_grid_ref, 1e-6, evf, eee, a_grid_ref, nthreads=8)
-    a, ncand = gpu_ctx.ccd_full(1e-6, evf, eee, a_grid)
+    a, ncand = shared_ctx.ccd_full(1e-6, evf, eee, a_grid)
     assert ncand == npairs  # the candidate SET is the reference hash's (voxel-range overlap + swept bbox test)
-    assert bits(a) == bits(a_ref), (a, a_ref)
+    assert scalar_bits(a) == scalar_bits(a_ref), (a, a_ref)
     assert 0 < a < a_grid
-    assert gpu_ctx.ccd_stats()[2] == 0
+    assert shared_ctx.ccd_stats()[2] == 0
 
 
-def test_zero_distance_returns_zero_step(gpu_ctx):
+def test_zero_distance_returns_zero_step(shared_ctx):
     m, p = two_body(7, n=2)
     # put a vertex of the upper body exactly onto a face of the lower one
     up = np.nonzero(m.V_rest[:, 2] > 1.0)[0]
@@ -92,37 +82,37 @@ def test_zero_distance_returns_zero_step(gpu_ctx):
     m.V[v] = [0.3, 0.2, 1.0]  # inside a lower triangle, away from its edges (on an edge, pairs at distance ~1e-17 make the
     # no_zero_toi refinement of Tight-Inclusion spin forever -- in the library as well)
     m.V[m.V_rest[:, 2] <= 1.0] = m.V_rest[m.V_rest[:, 2] <= 1.0]
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     s = orc.Surf(m)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, p)
     h = m.avgEdgeLen / 3
     g, ag = orc.grid_swept(s, p, 1.0, h)
     a_ref, z, _ = orc.ccd_full(s, p, g, ag, 1e-6, evf, eee, ag, nthreads=8)
     assert z == 1 and a_ref == 0.0
-    gpu_ctx.hash_build_swept(p, 1.0, h)
-    a, _ = gpu_ctx.ccd_full(1e-6, evf, eee, ag)
+    shared_ctx.hash_build_swept(p, 1.0, h)
+    a, _ = shared_ctx.ccd_full(1e-6, evf, eee, ag)
     assert a == 0.0
 
 
-def test_ball_pile_ccd_bit_exact(gpu_ctx):
+def test_ball_pile_ccd_bit_exact(shared_ctx):
     """BASELINE ball-pile workload at a size the brute-force oracle can sweep (4 balls)."""
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     p = info["p"]
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     s = orc.Surf(m)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, p)
-    mm, pa, pe, cand = gpu_ctx.constraint_set(info["dHat"], 1)
+    mm, pa, pe, cand = shared_ctx.constraint_set(info["dHat"], 1)
     a_part_ref, _ = orc.ccd_partial(s, p, cand, 1e-6, evf, eee, 1.0, nthreads=8)
-    a_part = gpu_ctx.ccd_partial(p, 1e-6, evf, eee, 1.0)
-    assert bits(a_part) == bits(a_part_ref)
+    a_part = shared_ctx.ccd_partial(p, 1e-6, evf, eee, 1.0)
+    assert scalar_bits(a_part) == scalar_bits(a_part_ref)
     h = m.avgEdgeLen / 3
     g, ag_ref = orc.grid_swept(s, p, a_part_ref, h)
-    ag = gpu_ctx.hash_build_swept(p, a_part, h)
-    assert bits(ag) == bits(ag_ref)
+    ag = shared_ctx.hash_build_swept(p, a_part, h)
+    assert scalar_bits(ag) == scalar_bits(ag_ref)
     a_ref, z, npairs = orc.ccd_full(s, p, g, ag_ref, 1e-6, evf, eee, ag_ref, nthreads=8)
-    a, ncand = gpu_ctx.ccd_full(1e-6, evf, eee, ag)
-    assert ncand == npairs and bits(a) == bits(a_ref)
-    assert gpu_ctx.ccd_stats()[2] == 0
+    a, ncand = shared_ctx.ccd_full(1e-6, evf, eee, ag)
+    assert ncand == npairs and scalar_bits(a) == scalar_bits(a_ref)
+    assert shared_ctx.ccd_stats()[2] == 0
     # property: the step is intersection free for the active stencils
     V2 = m.V + 0.999 * a * p.reshape(-1, 3)
     for c in cand[:200]:
@@ -154,12 +144,12 @@ def _retry_scene():
     return m, p.ravel(), np.array([candA], dtype=np.int32), np.array([candB], dtype=np.int32)
 
 
-def test_ms0_retry_is_not_pruned_by_a_competing_impact(gpu_ctx):
+def test_ms0_retry_is_not_pruned_by_a_competing_impact(shared_ctx):
     """ADVICE r1: the running-minimum pruning must not cut the ms = 0 rerun, whose result is rescaled by 0.8 afterwards.  Which pair reports
     first is a race on the device, so the test seeds the running minimum with pair A's impact (ipcgpu_ccd_debug_seed_bound) and runs pair B
     alone: with the rerun pruned B would report nothing and the step would stay at A's 1.0198e-6; the oracle (no pruning) says 2^-20."""
     m, p, candA, candB = _retry_scene()
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     s = orc.Surf(m)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     mm0 = np.empty((0, 4), dtype=np.int32)
@@ -168,13 +158,13 @@ def test_ms0_retry_is_not_pruned_by_a_competing_impact(gpu_ctx):
     a_B, _ = orc.ccd_partial(s, p, candB, 1e-6, evf, eee, 1.0, 1)
     a_AB, _ = orc.ccd_partial(s, p, np.concatenate([candA, candB]), 1e-6, evf, eee, 1.0, 1)
     assert a_B == 2.0 ** -20 and a_A > a_B and a_AB == a_B and 1.25 * a_B > a_A  # the scenario is the intended one
-    gpu_ctx.set_constraint_set(mm0, mm0, pe0, candB)
+    shared_ctx.set_constraint_set(mm0, mm0, pe0, candB)
     try:
-        gpu_ctx.ccd_debug_seed_bound(a_A)  # "pair A has already reported"
-        a = gpu_ctx.ccd_partial(p, 1e-6, evf, eee, 1.0)
+        shared_ctx.ccd_debug_seed_bound(a_A)  # "pair A has already reported"
+        a = shared_ctx.ccd_partial(p, 1e-6, evf, eee, 1.0)
     finally:
-        gpu_ctx.ccd_debug_seed_bound(-1.0)
-    assert bits(a) == bits(a_AB), (a, a_AB)
+        shared_ctx.ccd_debug_seed_bound(-1.0)
+    assert scalar_bits(a) == scalar_bits(a_AB), (a, a_AB)
     # and without the hook, both pairs in one list, whatever the race
-    gpu_ctx.set_constraint_set(mm0, mm0, pe0, np.concatenate([candA, candB]))
-    assert bits(gpu_ctx.ccd_partial(p, 1e-6, evf, eee, 1.0)) == bits(a_AB)
+    shared_ctx.set_constraint_set(mm0, mm0, pe0, np.concatenate([candA, candB]))
+    assert scalar_bits(shared_ctx.ccd_partial(p, 1e-6, evf, eee, 1.0)) == scalar_bits(a_AB)

@@ -5,11 +5,11 @@ every search then prunes against the same value, and the counts are a property o
 captured iteration must count the same boxes, at the default thread budget and at budget 0 (every search that goes past its root box is
 handed to the warp pass)."""
 import os
-import struct
 import sys
 
 import pytest
 
+from gpu_common import load_scene, scalar_bits, shared_ctx
 from ipc_b200 import lib as L
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -25,21 +25,15 @@ class _Args:
         self.scene = scene
 
 
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
 @pytest.mark.parametrize("budget", [-1, 0], ids=["default_budget", "budget0"])
 @pytest.mark.parametrize("scene", ["c5", "pile"])
-def test_box_counts_are_identical_eager_and_replayed(gpu_ctx, scene, budget):
+def test_box_counts_are_identical_eager_and_replayed(shared_ctx, scene, budget):
     import bench
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = bench.build_scene(_Args(scene))
     dHat, p, tol = info["dHat"], info["p"], bench.TI_TOL
     h = m.avgEdgeLen / 3.0
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
     ctx.set_canonical_order(0)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     ctx.constraint_set(dHat, 1)
@@ -57,7 +51,7 @@ def test_box_counts_are_identical_eager_and_replayed(gpu_ctx, scene, budget):
         it = ctx.fetch_iteration()
         _, survivors, warnings = ctx.ccd_stats()
         deferred, boxes_thread, boxes_warp = ctx.ccd_stats_ex()
-        return dict(alpha=bits(it.alpha), survivors=survivors, warnings=warnings, deferred=deferred, boxes_thread=boxes_thread, boxes_warp=boxes_warp)
+        return dict(alpha=scalar_bits(it.alpha), survivors=survivors, warnings=warnings, deferred=deferred, boxes_thread=boxes_thread, boxes_warp=boxes_warp)
 
     ctx.ccd_debug_thread_budget(budget)
     try:
@@ -79,7 +73,7 @@ def test_box_counts_are_identical_eager_and_replayed(gpu_ctx, scene, budget):
         ctx.ccd_debug_thread_budget(-1)
         ctx.set_canonical_order(1)
     print("COUNTS", scene, budget, runs[0])
-    assert runs[0]["alpha"] == bits(alpha), runs
+    assert runs[0]["alpha"] == scalar_bits(alpha), runs
     assert runs[0] == runs[1] == runs[2], runs
     # a handed-on search was counted by the thread pass at its first level (at least its root box) before the warp pass took it
     assert runs[0]["survivors"] > 0 and runs[0]["boxes_thread"] >= runs[0]["deferred"] > 0 and runs[0]["boxes_warp"] > 0, runs

@@ -1,21 +1,17 @@
 """The swept grid of the full CCD registers every primitive in each cell of K x K x K reference voxels its range touches, with K chosen on
 the device from the longest range and from the size of the cell table.  These scenes push K up and make many ranges straddle cell borders:
 the candidate set must still be the reference hash's, every pair exactly once, and the step bound bit-equal to the oracle's."""
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import load_scene, scalar_bits, shared_ctx
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from ipc_b200 import scenes
 
 pytestmark = pytest.mark.gpu
-
-
-def bits(x):
-    return struct.pack("<d", x)
 
 
 def fast_vertices():
@@ -48,20 +44,18 @@ def far_apart():
 
 
 @pytest.mark.parametrize("scene", [fast_vertices, far_apart])
-def test_swept_grid_candidates_and_step_match_oracle(gpu_ctx, scene):
+def test_swept_grid_candidates_and_step_match_oracle(shared_ctx, scene):
     m, p = scene()
-    gpu_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    gpu_ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    gpu_ctx.set_state(m.V_soa)
+    load_scene(shared_ctx, m)
     s = orc.Surf(m)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, p)
     h = m.avgEdgeLen / 3
     g, ag_ref = orc.grid_swept(s, p, 1.0, h)
-    ag = gpu_ctx.hash_build_swept(p, 1.0, h)
-    assert bits(ag) == bits(ag_ref)
+    ag = shared_ctx.hash_build_swept(p, 1.0, h)
+    assert scalar_bits(ag) == scalar_bits(ag_ref)
     a_ref, _, npairs = orc.ccd_full(s, p, g, ag_ref, 1e-6, evf, eee, ag_ref, nthreads=8)
-    a, ncand = gpu_ctx.ccd_full(1e-6, evf, eee, ag)
+    a, ncand = shared_ctx.ccd_full(1e-6, evf, eee, ag)
     assert npairs > 0
     assert ncand == npairs  # no pair found twice, none missed
-    assert bits(a) == bits(a_ref), (a, a_ref)
-    assert gpu_ctx.ccd_stats()[2] == 0
+    assert scalar_bits(a) == scalar_bits(a_ref), (a, a_ref)
+    assert shared_ctx.ccd_stats()[2] == 0

@@ -1,13 +1,13 @@
 """Codimensional scenes on the device: every stage against the oracle on scenes modelled on the reference's codimensional examples, the
 point-in-tetrahedron half of the intersection check against exact arithmetic, the line search with a point entering a tet, and a tet-only
 scene with vCoDim given against one without."""
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
 import oracle_codim as oc
+from gpu_common import load_scene, scalar_bits, shared_ctx, soa
 from ipc_b200 import codim
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
@@ -15,20 +15,6 @@ from stagecheck import check_every_stage
 
 pytestmark = pytest.mark.gpu
 NTH = 8
-
-
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def upload(ctx, m, codim=True):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim if codim else None)
-    ctx.set_state(m.V_soa)
 
 
 def deformed(m, seed, amp):
@@ -59,7 +45,7 @@ SCENES = {"pin_cushion": oc.pin_cushion, "point_roller": oc.point_roller, "point
 
 @pytest.mark.parametrize("seed", [1, 2])
 @pytest.mark.parametrize("name", list(SCENES))
-def test_codim_scene_every_stage(gpu_ctx, name, seed):
+def test_codim_scene_every_stage(shared_ctx, name, seed):
     m = deformed(SCENES[name](), seed, 2e-3)
     dHat = 0.03 ** 2
     rng = np.random.default_rng(seed + 10)
@@ -67,10 +53,10 @@ def test_codim_scene_every_stage(gpu_ctx, name, seed):
     P[m.vCoDim == 3, 1] = -0.05
     P[m.dbc != 0, 1] = 0.03
     P += 0.005 * rng.standard_normal(P.shape)
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     # (the summed CSR Hessian is compared in test_codim_scene_hessian: stagecheck's oracle writes the Dirichlet identity only on rows of
     # vertices that have a tet, as Energy::computeHessian does; the codimensional Dirichlet vertices have none)
-    r = check_every_stage(gpu_ctx, m, dict(dHat=dHat, p=np.ascontiguousarray(P).ravel()), kappa=1e4, min_active=1, h_tol=np.inf)
+    r = check_every_stage(shared_ctx, m, dict(dHat=dHat, p=np.ascontiguousarray(P).ravel()), kappa=1e4, min_active=1, h_tol=np.inf)
     assert r["n_active"] > 0
     s = orc.Surf(m)
     mm_r, pa_r, pe_r, _ = s.constraint_set(dHat)
@@ -79,44 +65,44 @@ def test_codim_scene_every_stage(gpu_ctx, name, seed):
     assert any(min(m.vCoDim[v] for v in vs(q)) < 3 for q in mm_r)
     # lagged friction: the same pairs and the same energy
     Vt = m.V - 1e-3 * P
-    gpu_ctx.set_prev_state(soa(Vt))
-    gpu_ctx.constraint_set(dHat, 0)
-    nfr = gpu_ctx.friction_lag(dHat, 1e4)
+    shared_ctx.set_prev_state(soa(Vt))
+    shared_ctx.constraint_set(dHat, 0)
+    nfr = shared_ctx.friction_lag(dHat, 1e4)
     lam, co, ba = s.friction_lag(mm_r, dHat, 1e4)
     eps2 = (1e-3 * m.avgEdgeLen) ** 2
-    Ef, Ef_r = gpu_ctx.friction_energy(eps2, 0.3), s.friction_energy(Vt, mm_r, lam, co, ba, eps2, 0.3)
+    Ef, Ef_r = shared_ctx.friction_energy(eps2, 0.3), s.friction_energy(Vt, mm_r, lam, co, ba, eps2, 0.3)
     assert nfr == len(mm_r) and abs(Ef - Ef_r) <= 1e-10 * abs(Ef_r)
     # device-built pattern: vNeighbor with the CE / codimension-2 triangle edges, plus the contact pairs
     import bench
     ia_r, ja_r = m.csr_pattern(1, extra_pairs=bench.contact_pattern_pairs(m, mm_r, pa_r, pe_r))
-    gpu_ctx.enable_device_pattern(1, 2 * ja_r.size)
-    gpu_ctx.constraint_set(dHat, 0)
-    gpu_ctx.update_pattern()
-    ia, ja = gpu_ctx.get_pattern()
+    shared_ctx.enable_device_pattern(1, 2 * ja_r.size)
+    shared_ctx.constraint_set(dHat, 0)
+    shared_ctx.update_pattern()
+    ia, ja = shared_ctx.get_pattern()
     assert np.array_equal(ia, ia_r) and np.array_equal(ja, ja_r)
-    gpu_ctx.set_csr(ia_r, ja_r, 1)  # (back to host mode for the next test)
+    shared_ctx.set_csr(ia_r, ja_r, 1)  # (back to host mode for the next test)
     # intersection check (both halves) and inversion check (tets only)
     ok_r, hits_r = s.intersection_free(nthreads=NTH)
     n_pit = oc.points_in_tets(m.V, m.T, pts_of(m), NTH)
-    assert device_count(gpu_ctx) == hits_r + n_pit
-    assert gpu_ctx.intersection_free() == (ok_r and n_pit == 0)
-    assert gpu_ctx.check_inversion() == orc.Elastic(m).count_inverted()
+    assert device_count(shared_ctx) == hits_r + n_pit
+    assert shared_ctx.intersection_free() == (ok_r and n_pit == 0)
+    assert shared_ctx.check_inversion() == orc.Elastic(m).count_inverted()
 
 
 @pytest.mark.parametrize("name", list(SCENES))
-def test_codim_scene_hessian(gpu_ctx, name):
+def test_codim_scene_hessian(shared_ctx, name):
     m = deformed(SCENES[name](), 1, 2e-3)
     dHat, kappa, dt2 = 0.03 ** 2, 1e4, 0.025 ** 2
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     s = orc.Surf(m)
     mm_r, pa_r, pe_r, _ = s.constraint_set(dHat)
-    gpu_ctx.constraint_set(dHat, 0)
+    shared_ctx.constraint_set(dHat, 0)
     import bench
     ia, ja = m.csr_pattern(1, extra_pairs=bench.contact_pattern_pairs(m, mm_r, pa_r, pe_r))
-    gpu_ctx.set_csr(ia, ja, 1)
+    shared_ctx.set_csr(ia, ja, 1)
     a = np.zeros(ja.size)
-    gpu_ctx.elastic_hessian(dt2, 1, 1, 1, a)
-    gpu_ctx.barrier_hessian(dHat, kappa, 1, a)
+    shared_ctx.elastic_hessian(dt2, 1, 1, 1, a)
+    shared_ctx.barrier_hessian(dHat, kappa, 1, a)
     a_r = orc.Elastic(m).hessian_csr(dt2, ia, ja, 1, 1, 1, nthreads=NTH)
     s.barrier_hessian_csr(mm_r, pa_r, pe_r, dHat, kappa, ia, ja, 1, 1, a=a_r, nthreads=NTH)
     # Optimizer::computePrecondMtr (Optimizer.cpp:3634-3660) sets the identity on the diagonal of EVERY projected Dirichlet vertex, also of
@@ -164,35 +150,35 @@ def sheet_under_ball(n=60, span=3.0):
 
 
 @pytest.mark.parametrize("level", [1, 2])
-def test_candidates_beyond_nv_in_canonical_order(gpu_ctx, level):
+def test_candidates_beyond_nv_in_canonical_order(shared_ctx, level):
     """the candidate list sorted on a scene with more surface edges than vertices: its first components reach past nV"""
     m = sheet_under_ball()
     dHat = 0.03 ** 2
-    upload(gpu_ctx, m)
-    gpu_ctx.set_canonical_order(level)
+    load_scene(shared_ctx, m)
+    shared_ctx.set_canonical_order(level)
     try:
-        got = gpu_ctx.constraint_set(dHat, 1)
+        got = shared_ctx.constraint_set(dHat, 1)
     finally:
-        gpu_ctx.set_canonical_order(1)
+        shared_ctx.set_canonical_order(1)
     ref = orc.Surf(m).constraint_set(dHat)
     cand = ref[3]
     assert len(m.SFEdges) > m.nV and cand[:, 0].max() >= m.nV and cand[:, 0].min() < 0
     assert all(np.array_equal(x, y) for x, y in zip(got, ref))
 
 
-def test_point_in_tet_crafted_soup(gpu_ctx):
+def test_point_in_tet_crafted_soup(shared_ctx):
     V, T, pts = oc.crafted_soup()
     m = soup_mesh(V, T, pts)
     n_exact = oc.points_in_tets_exact(V, T, pts)
     assert n_exact == oc.points_in_tets(V, T, pts) and n_exact > 0
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     _, hits_r = orc.Surf(m).intersection_free()
     assert hits_r == 0
-    assert device_count(gpu_ctx) == n_exact
-    assert gpu_ctx.intersection_free() is False
+    assert device_count(shared_ctx) == n_exact
+    assert shared_ctx.intersection_free() is False
 
 
-def test_point_in_tet_one_point_per_tet(gpu_ctx):
+def test_point_in_tet_one_point_per_tet(shared_ctx):
     """every tet of a grid holds its own point (centroid), every point in another slot of the grid, plus points on shared faces"""
     V, T = M.grid_tets(7, 6, 5, h=0.1)
     C = V[T].mean(1)
@@ -206,11 +192,11 @@ def test_point_in_tet_one_point_per_tet(gpu_ctx):
     pts = pts_of(m)
     n_ref = oc.points_in_tets(Vall, T, pts, NTH)
     assert n_ref >= len(T) + len(F[::5])
-    upload(gpu_ctx, m)
-    assert device_count(gpu_ctx) == n_ref + orc.Surf(m).intersection_free()[1]
+    load_scene(shared_ctx, m)
+    assert device_count(shared_ctx) == n_ref + orc.Surf(m).intersection_free()[1]
 
 
-def test_tet_only_vcodim_bit_identical(gpu_ctx):
+def test_tet_only_vcodim_bit_identical(shared_ctx):
     """a tet-only scene with vCoDim (all 3) equals vCoDim = NULL bit for bit with the same launch count"""
     V1, T1 = M.grid_tets(4, 4, 4, h=0.25)
     V2, T2 = M.grid_tets(4, 4, 4, h=0.25, origin=(0.1, 0.05, 1.01))
@@ -223,16 +209,16 @@ def test_tet_only_vcodim_bit_identical(gpu_ctx):
     dHat = 0.02 ** 2
     out = []
     for codim in (True, False):
-        upload(gpu_ctx, m, codim)
-        n0 = gpu_ctx.launch_count()
-        mm, pa, pe, cand = gpu_ctx.constraint_set(dHat, 1)
+        load_scene(shared_ctx, m, vcodim=codim)
+        n0 = shared_ctx.launch_count()
+        mm, pa, pe, cand = shared_ctx.constraint_set(dHat, 1)
         evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
-        a1 = gpu_ctx.ccd_partial(p, 1e-6, evf, eee, 1.0)
-        ag = gpu_ctx.hash_build_swept(p, a1, m.avgEdgeLen / 3)
-        a2, nc = gpu_ctx.ccd_full(1e-6, evf, eee, ag)
-        ok = gpu_ctx.intersection_free()
-        Eb = gpu_ctx.barrier_energy(dHat, 1e4)
-        out.append((mm.tobytes(), pa.tobytes(), cand.tobytes(), bits(a1), bits(a2), nc, ok, bits(Eb), gpu_ctx.launch_count() - n0))
+        a1 = shared_ctx.ccd_partial(p, 1e-6, evf, eee, 1.0)
+        ag = shared_ctx.hash_build_swept(p, a1, m.avgEdgeLen / 3)
+        a2, nc = shared_ctx.ccd_full(1e-6, evf, eee, ag)
+        ok = shared_ctx.intersection_free()
+        Eb = shared_ctx.barrier_energy(dHat, 1e4)
+        out.append((mm.tobytes(), pa.tobytes(), cand.tobytes(), scalar_bits(a1), scalar_bits(a2), nc, ok, scalar_bits(Eb), shared_ctx.launch_count() - n0))
     assert out[0] == out[1]
 
 
@@ -260,7 +246,7 @@ class _OrcWithPoints:
         return s
 
 
-def test_line_search_point_enters_tet(gpu_ctx):
+def test_line_search_point_enters_tet(shared_ctx):
     import test_gpu_step_control as SC
     # a block falls onto a bed of points; at alpha = 1 the points are 0.3 deep inside it
     Vb, Tb = M.grid_tets(3, 3, 3, h=1.0 / 3, origin=(0.0, 0.0, 0.1))
@@ -280,21 +266,20 @@ def test_line_search_point_enters_tet(gpu_ctx):
     finally:
         SC.orc = real
     assert ref["status"] == 0 and ref["counts"][1] > 0  # the point-in-tet half halved the step
-    SC.upload(gpu_ctx, sc)
-    rc, alpha = gpu_ctx.line_search(**sc.terms(), alpha=1.0)
-    info = gpu_ctx.step_control_info()
-    assert rc == 0 and bits(alpha) == bits(ref["alpha"]) and SC.counts(info) == ref["counts"]
+    SC.load_step_scene(shared_ctx, sc)
+    rc, alpha = shared_ctx.line_search(**sc.terms(), alpha=1.0)
+    info = shared_ctx.step_control_info()
+    assert rc == 0 and scalar_bits(alpha) == scalar_bits(ref["alpha"]) and SC.counts(info) == ref["counts"]
     # captured: the same step and counters from a replay (a captured line search keeps the device's list order)
-    gpu_ctx.set_canonical_order(0)
-    SC.prepare(gpu_ctx, sc, m.V, sc.p)
-    gpu_ctx.fetch_iteration()
-    gpu_ctx.capture_begin()
-    gpu_ctx.step_bound_set(1.0)
-    gpu_ctx.line_search(**sc.terms())
-    gid = gpu_ctx.capture_end()
-    SC.prepare(gpu_ctx, sc, m.V, sc.p)
-    gpu_ctx.graph_launch(gid)
-    info = gpu_ctx.step_control_info()
-    assert info.status == 0 and bits(info.alpha) == bits(ref["alpha"]) and SC.counts(info) == ref["counts"]
-    gpu_ctx.graph_destroy(gid)
-    gpu_ctx.set_canonical_order(1)
+    shared_ctx.set_canonical_order(0)
+    SC.prepare(shared_ctx, sc, m.V, sc.p)
+    shared_ctx.fetch_iteration()
+    shared_ctx.capture_begin()
+    shared_ctx.step_bound_set(1.0)
+    shared_ctx.line_search(**sc.terms())
+    gid = shared_ctx.capture_end()
+    SC.prepare(shared_ctx, sc, m.V, sc.p)
+    shared_ctx.graph_launch(gid)
+    info = shared_ctx.step_control_info()
+    assert info.status == 0 and scalar_bits(info.alpha) == scalar_bits(ref["alpha"]) and SC.counts(info) == ref["counts"]
+    shared_ctx.graph_destroy(gid)

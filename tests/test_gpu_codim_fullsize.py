@@ -8,6 +8,7 @@ import pytest
 
 import oracle as orc
 import oracle_codim as oc
+from gpu_common import load_scene, shared_ctx
 from ipc_b200 import codim
 
 pytestmark = pytest.mark.gpu
@@ -28,15 +29,13 @@ def pile_with_points(n_points=100_000, seed=3):
     return mc, info
 
 
-def test_c5_point_cloud_count(gpu_ctx):
+def test_c5_point_cloud_count(shared_ctx):
     m, _ = pile_with_points()
     pts = np.flatnonzero(m.vCoDim == 0).astype(np.int32)
     n_ref = oc.points_in_tets(m.V, m.T, pts, os.cpu_count() or 8)
     assert 1000 < n_ref < len(pts)
     _, hits_r = orc.Surf(m).intersection_free(nthreads=os.cpu_count() or 8)
-    gpu_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    gpu_ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    gpu_ctx.set_state(m.V_soa)
-    gpu_ctx.intersection_free(want=False)
-    assert gpu_ctx.fetch_iteration().n_intersected_triangles == n_ref + hits_r
-    assert gpu_ctx.intersection_free() is False
+    load_scene(shared_ctx, m)
+    shared_ctx.intersection_free(want=False)
+    assert shared_ctx.fetch_iteration().n_intersected_triangles == n_ref + hits_r
+    assert shared_ctx.intersection_free() is False

@@ -1,15 +1,15 @@
 """A C++ program (tests/cpp/abi_driver.cpp), not Python, drives the C ABI end to end -- the position the reference-side adapters are in.
 The test writes a scene file, builds and runs the driver, and compares what it wrote back with the oracle."""
 import os
-import struct
 import subprocess
 
 import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import rel, scalar_bits
 from ipc_b200 import scenes
-from stagecheck import contact_pattern_pairs, rel
+from stagecheck import contact_pattern_pairs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cpp", "abi_driver.cpp")
@@ -68,12 +68,11 @@ def test_cpp_driver_matches_oracle(tmp_path):
     al1, _ = orc.ccd_partial(s, p, cand, tol, evf, eee, al0, 8)
     gr, ag = orc.grid_swept(s, p, al1, h)
     al2, _, npairs = orc.ccd_full(s, p, gr, ag, tol, evf, eee, ag, 8)
-    bits = lambda x: struct.pack("<d", float(x))
     assert tuple(ints[:3]) == (len(mm), len(pa), len(cand)) and ints[3] == npairs == ints[7]
     assert ints[4] == 0 and ints[5] == 1 and ints[6] == 0  # no inverted tet, intersection free, status OK
     assert abs(dbl[0] - E_el) <= 1e-10 * abs(E_el) and abs(dbl[1] - E_b) <= 1e-10 * abs(E_b)
     assert abs(dbl[5] - E_el) <= 1e-10 * abs(E_el) and abs(dbl[6] - E_b) <= 1e-10 * abs(E_b)
-    assert abs(dbl[2] - al0) <= 1e-9 * al0 and bits(dbl[3]) == bits(al1) and bits(dbl[4]) == bits(al2)
-    assert bits(dbl[8]) == bits(al1) and bits(dbl[9]) == bits(al2) and bits(dbl[10]) == bits(al2)
+    assert abs(dbl[2] - al0) <= 1e-9 * al0 and scalar_bits(dbl[3]) == scalar_bits(al1) and scalar_bits(dbl[4]) == scalar_bits(al2)
+    assert scalar_bits(dbl[8]) == scalar_bits(al1) and scalar_bits(dbl[9]) == scalar_bits(al2) and scalar_bits(dbl[10]) == scalar_bits(al2)
     for gg, aa in ((g, a), (g2, a2)):
         assert rel(gg, g_ref) <= 1e-10 and rel(aa, a_ref) <= 1e-9

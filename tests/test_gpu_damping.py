@@ -2,7 +2,6 @@
 tests/oracle_damping.py: D added into the CSR (host pattern and device-built pattern), energies and gradients for projectDBC = 0 and 1, the
 penalty's lambda update and completed step, the line search with each term against an oracle driver, and a captured iteration replayed after
 rho doubles and lambda updates."""
-import struct
 
 import numpy as np
 import pytest
@@ -10,32 +9,16 @@ import pytest
 import oracle as orc
 import oracle_damping as OD
 import test_gpu_step_control as SC
+from gpu_common import own_context, rel, scalar_bits, soa
 from ipc_b200 import lib as L
 
 pytestmark = pytest.mark.gpu
 
 
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def rel(a, b):
-    return abs(a - b) / max(abs(b), 1e-300)
-
-
-def nrel(a, b):
-    return np.linalg.norm(np.asarray(a) - np.asarray(b)) / max(np.linalg.norm(b), 1e-300)
-
-
 @pytest.fixture(scope="module")
 def ctx():
-    c = L.Context(0)
-    yield c
-    c.close()
+    with own_context() as c:
+        yield c
 
 
 def scene(energy):
@@ -58,8 +41,8 @@ def scene(energy):
     return sc
 
 
-def upload(ctx, sc, canonical=1):
-    SC.upload(ctx, sc, canonical=canonical)  # mesh, surface, state, p, xTilta, contact sets, V_prev, friction lag
+def load_step_scene_csr(ctx, sc, canonical=1):
+    SC.load_step_scene(ctx, sc, canonical=canonical)  # mesh, surface, state, p, xTilta, contact sets, V_prev, friction lag
     ia, ja = sc.m.csr_pattern(1)
     ctx.set_csr(ia, ja, 1)
     return ia, ja
@@ -70,12 +53,12 @@ def upload(ctx, sc, canonical=1):
 def test_damping_matrix_host_and_device_pattern(ctx, energy):
     sc = scene(energy)
     m, coef = sc.m, 0.3
-    ia, ja = upload(ctx, sc)
+    ia, ja = load_step_scene_csr(ctx, sc)
     D = OD.damping_matrix(m, m.V, coef)
     assert np.array_equal(D[0], ia) and np.array_equal(D[1], ja)
     ctx.damping_update(coef)
     a = ctx.damping_hessian(np.zeros(ja.size))
-    assert nrel(a, D[2]) <= 1e-9
+    assert rel(a, D[2]) <= 1e-9
     for v in np.flatnonzero(m.dbc):  # the identity of the reference's setCoeff
         for r in range(3):
             assert a[ia[3 * v + r] - 1] == 1.0
@@ -88,7 +71,7 @@ def test_damping_matrix_host_and_device_pattern(ctx, energy):
     ctx.csr_set_zero()
     ctx.damping_hessian(None)
     a2 = ctx.download(L.BUF_CSR_VALUES, nnz)
-    assert nrel(a2, OD.scatter(ia, ja, D[2], ia2, ja2)) <= 1e-9
+    assert rel(a2, OD.scatter(ia, ja, D[2], ia2, ja2)) <= 1e-9
 
 
 # ---- energies and gradients ------------------------------------------------------------------------------------------------------------
@@ -97,28 +80,28 @@ def test_damping_matrix_host_and_device_pattern(ctx, energy):
 def test_energies_and_gradients(ctx, energy, projectDBC):
     sc = scene(energy)
     m, coef, dt2, rho = sc.m, 0.3, 1e-2, 1e3
-    ia, ja = upload(ctx, sc)
+    ia, ja = load_step_scene_csr(ctx, sc)
     V = m.V
     D = OD.damping_matrix(m, V, coef)
     ctx.damping_update(coef)
     assert rel(ctx.damping_energy(), OD.damping_energy(D, V, sc.Vprev, m.dbc)) <= 1e-10
     g = ctx.damping_gradient(projectDBC, np.zeros(3 * m.nV))
-    assert nrel(g, OD.damping_gradient(D, V, sc.Vprev, m.dbc, projectDBC)) <= 1e-10
+    assert rel(g, OD.damping_gradient(D, V, sc.Vprev, m.dbc, projectDBC)) <= 1e-10
     ctx.set_neumann_forces(dt2, sc.f)
     assert rel(ctx.neumann_energy(), OD.neumann_energy(V, sc.f, m.mass, m.dbc, dt2)) <= 1e-10
     g = ctx.neumann_gradient(np.zeros(3 * m.nV))
-    assert nrel(g, OD.neumann_gradient(sc.f, m.mass, m.dbc, dt2)) <= 1e-10
+    assert rel(g, OD.neumann_gradient(sc.f, m.mass, m.dbc, dt2)) <= 1e-10
     ctx.set_dirichlet_targets(sc.vid, sc.tgt, sc.lam, 1e-6)
     ctx.set_dirichlet_penalty(rho)
     assert rel(ctx.dirichlet_energy(), OD.mdbc_energy(V, sc.vid, sc.tgt, sc.lam, m.mass, rho)) <= 1e-10
     g = ctx.dirichlet_gradient(projectDBC, np.zeros(3 * m.nV))
     want = OD.mdbc_gradient(V, sc.vid, sc.tgt, sc.lam, m.mass, rho, m.nV) if not projectDBC else np.zeros(3 * m.nV)
-    assert nrel(g, want) <= 1e-10 if not projectDBC else not g.any()
+    assert rel(g, want) <= 1e-10 if not projectDBC else not g.any()
     a = ctx.dirichlet_hessian(projectDBC, np.zeros(ja.size))
     want = np.zeros(ja.size)
     if not projectDBC:
         want[ia[:-1] - 1] = OD.mdbc_hessian_diag(sc.vid, m.mass, rho, m.nV)
-    assert nrel(a, want) <= 1e-12 if not projectDBC else not a.any()
+    assert rel(a, want) <= 1e-12 if not projectDBC else not a.any()
     # the deferred forms: the fetch reports the same energies
     for f in (ctx.damping_energy, ctx.neumann_energy, ctx.dirichlet_energy):
         f(want=False)
@@ -137,7 +120,7 @@ def test_energies_and_gradients(ctx, energy, projectDBC):
 def test_lambda_update_and_completed_step(ctx):
     sc = scene(1)
     m, rho, tol = sc.m, 2e3, 1e-5
-    upload(ctx, sc)
+    load_step_scene_csr(ctx, sc)
     ctx.set_dirichlet_targets(sc.vid, sc.tgt, sc.lam, tol)
     ctx.set_dirichlet_penalty(rho)
     s = ctx.dirichlet_completed_step()
@@ -146,7 +129,7 @@ def test_lambda_update_and_completed_step(ctx):
     assert rel(ctx.fetch_iteration().dirichlet_completed_step, s) <= 1e-15
     ctx.dirichlet_update_lambda()
     lam1 = OD.mdbc_update_lambda(m.V, sc.vid, sc.tgt, sc.lam, m.mass, rho)
-    assert nrel(ctx.get_dirichlet_lambda(), lam1) <= 1e-14
+    assert rel(ctx.get_dirichlet_lambda(), lam1) <= 1e-14
     ctx.set_dirichlet_targets(sc.vid, sc.tgt, None, 0.0)
     assert ctx.dirichlet_completed_step() == 1.0 and not ctx.get_dirichlet_lambda().any()
     ctx.set_dirichlet_targets([], [])
@@ -156,7 +139,7 @@ def test_refusals_and_a_new_mesh(ctx):
     """repeated target vertices are refused (targetPos is a map); a new mesh removes the three terms and their energies read 0"""
     sc = scene(1)
     m = sc.m
-    upload(ctx, sc)
+    load_step_scene_csr(ctx, sc)
     with pytest.raises(L.IpcGpuError, match="ARG"):
         ctx.set_dirichlet_targets([3, 5, 3], np.zeros((3, 3)))
     ctx.damping_update(0.3)
@@ -249,7 +232,7 @@ def test_line_search_with_each_term_matches_oracle(ctx, term):
     ref0 = oracle_line_search(sc, {})
     assert min(ref["margins"]) > SC.MARGIN and min(ref0["margins"]) > SC.MARGIN
     assert ref["alpha"] <= ref0["alpha"] / 2.0 and ref["counts"][2] > ref0["counts"][2], (ref["counts"], ref0["counts"])
-    upload(ctx, sc)
+    load_step_scene_csr(ctx, sc)
     for with_term, want in ((True, ref), (False, ref0)):
         (on if with_term else off)(ctx)
         ctx.set_state(sc.m.V_soa)
@@ -257,13 +240,13 @@ def test_line_search_with_each_term_matches_oracle(ctx, term):
         rc, alpha = ctx.line_search(**sc.terms(), alpha=1.0)
         e = ctx.step_control_info()
         assert rc == 0 and e.status == 0
-        assert bits(alpha) == bits(want["alpha"]) and SC.counts(e) == want["counts"], (term, with_term, alpha, want["alpha"], SC.counts(e), want["counts"])
+        assert scalar_bits(alpha) == scalar_bits(want["alpha"]) and SC.counts(e) == want["counts"], (term, with_term, alpha, want["alpha"], SC.counts(e), want["counts"])
         assert rel(e.energy_start, want["E0"]) <= 1e-10 and rel(e.energy, want["Et"]) <= 1e-10
 
 
 def test_zero_rho_leaves_the_line_search_bit_identical(ctx):
     sc = scene(1)
-    upload(ctx, sc)
+    load_step_scene_csr(ctx, sc)
     out = []
     for targets in (False, True):
         if targets:
@@ -273,7 +256,7 @@ def test_zero_rho_leaves_the_line_search_bit_identical(ctx):
         ctx.constraint_set(sc.dHat, 1, fetch=False, sizes=False)
         ctx.line_search(**sc.terms(), alpha=1.0)
         e = ctx.step_control_info()
-        out.append((bits(e.alpha), bits(e.energy_start), bits(e.energy), tuple(SC.counts(e))))
+        out.append((scalar_bits(e.alpha), scalar_bits(e.energy_start), scalar_bits(e.energy), tuple(SC.counts(e))))
     assert out[0] == out[1]
     ctx.set_dirichlet_targets([], [])
 
@@ -283,7 +266,7 @@ def test_captured_penalty_iteration_equals_eager(ctx):
     sc = scene(1)
     sc.fric = (sc.fric[0], 0.0, sc.fric[2])  # (friction off in the search: the captured line search needs no lag refresh)
     m = sc.m
-    ia, ja = upload(ctx, sc, canonical=0)
+    ia, ja = load_step_scene_csr(ctx, sc, canonical=0)
     ctx.enable_device_pattern(1)
     ctx.damping_update(0.003)
     ctx.set_neumann_forces(1e-2, sc.f)
@@ -340,12 +323,12 @@ def test_captured_penalty_iteration_equals_eager(ctx):
         ctx.graph_launch(gid)  # (the same graph: refused if anything had required a new capture)
         ig, eg, gg, ag = results()
         assert ig.status == ie.status == 0 and eg.status == ee.status == 0
-        assert bits(eg.alpha) == bits(ee.alpha) and SC.counts(eg) == SC.counts(ee)
+        assert scalar_bits(eg.alpha) == scalar_bits(ee.alpha) and SC.counts(eg) == SC.counts(ee)
         assert rel(eg.energy, ee.energy) <= 1e-12 and rel(eg.energy_start, ee.energy_start) <= 1e-12  # (contact lists in arbitrary order)
-        assert bits(ig.dirichlet_completed_step) == bits(ie.dirichlet_completed_step)
-        assert nrel(gg, ge) <= 1e-12 and nrel(ag, ae) <= 1e-12
-        seen.add(bits(ee.energy_start))
-        steps.add(bits(ie.dirichlet_completed_step))
+        assert scalar_bits(ig.dirichlet_completed_step) == scalar_bits(ie.dirichlet_completed_step)
+        assert rel(gg, ge) <= 1e-12 and rel(ag, ae) <= 1e-12
+        seen.add(scalar_bits(ee.energy_start))
+        steps.add(scalar_bits(ie.dirichlet_completed_step))
     assert len(seen) == 4 and len(steps) == 4  # rho, lambda and the new targets reached the objective and the completed step
     ctx.graph_destroy(gid)
     ctx.set_canonical_order(1)
@@ -362,21 +345,20 @@ def test_c5_damping_matches_oracle():
     class Args:
         tets, res, scene = 1_000_000, 10, "c5"
     m, info = bench.build_scene(Args())
-    ctx = L.Context(0)
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ia, ja = m.csr_pattern(1)
-    ctx.set_csr(ia, ja, 1)
-    ctx.set_state(m.V_soa)
-    P = np.array(info["p"], dtype=np.float64).reshape(-1, 3)
-    Vprev = m.V - 1e-2 * P
-    ctx.set_prev_state(soa(Vprev))
-    coef = 0.1
-    ctx.damping_update(coef)
-    a = ctx.damping_hessian(np.zeros(ja.size))
-    a_ref = orc.Elastic(m).hessian_csr(coef, ia, ja, 1, 1, 1, nthreads=8)
-    assert nrel(a, a_ref) <= 1e-9
-    D = (ia, ja, a_ref)
-    assert rel(ctx.damping_energy(), OD.damping_energy(D, m.V, Vprev, m.dbc)) <= 1e-10
-    g = ctx.damping_gradient(1, np.zeros(3 * m.nV))
-    assert nrel(g, OD.damping_gradient(D, m.V, Vprev, m.dbc, 1)) <= 1e-10
-    ctx.close()
+    with own_context() as ctx:
+        ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
+        ia, ja = m.csr_pattern(1)
+        ctx.set_csr(ia, ja, 1)
+        ctx.set_state(m.V_soa)
+        P = np.array(info["p"], dtype=np.float64).reshape(-1, 3)
+        Vprev = m.V - 1e-2 * P
+        ctx.set_prev_state(soa(Vprev))
+        coef = 0.1
+        ctx.damping_update(coef)
+        a = ctx.damping_hessian(np.zeros(ja.size))
+        a_ref = orc.Elastic(m).hessian_csr(coef, ia, ja, 1, 1, 1, nthreads=8)
+        assert rel(a, a_ref) <= 1e-9
+        D = (ia, ja, a_ref)
+        assert rel(ctx.damping_energy(), OD.damping_energy(D, m.V, Vprev, m.dbc)) <= 1e-10
+        g = ctx.damping_gradient(1, np.zeros(3 * m.nV))
+        assert rel(g, OD.damping_gradient(D, m.V, Vprev, m.dbc, 1)) <= 1e-10

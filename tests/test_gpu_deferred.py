@@ -1,31 +1,25 @@
 """The device-resident iteration (every stage enqueued with NULL outputs, one ipcgpu_fetch_iteration) must give exactly what the
 synchronous calls give: same energies, same gradient / CSR values, bit-identical step after every bound -- and both match the oracle."""
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import load_scene, rel, scalar_bits, shared_ctx
 from ipc_b200 import lib as L
 from ipc_b200 import scenes
-from stagecheck import contact_pattern_pairs, rel
+from stagecheck import contact_pattern_pairs
 
 pytestmark = pytest.mark.gpu
 
 
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
 @pytest.mark.parametrize("canonical", [1, 0])
-def test_deferred_iteration_equals_synchronous_calls(gpu_ctx, canonical):
-    ctx = gpu_ctx
+def test_deferred_iteration_equals_synchronous_calls(shared_ctx, canonical):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     dHat, p, kappa, dt2, tol = info["dHat"], info["p"], 1e8, 0.025 ** 2, 1e-6
     h = m.avgEdgeLen / 3
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
     ctx.set_canonical_order(canonical)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     mm, pa, pe, cand = ctx.constraint_set(dHat, 1)
@@ -57,7 +51,7 @@ def test_deferred_iteration_equals_synchronous_calls(gpu_ctx, canonical):
     assert it.status == 0 and it.ti_warnings == 0
     assert (it.n_active, it.n_mollified, it.n_candidates) == (len(mm), len(pa), len(cand)) == ctx.constraint_set_sizes()
     assert abs(it.energy_elastic - E_el) <= 1e-14 * abs(E_el) and abs(it.energy_barrier - E_b) <= 1e-12 * abs(E_b)
-    assert [bits(x) for x in (it.alpha_inversion, it.alpha_partial_ccd, it.alpha_swept_grid, it.alpha_full_ccd, it.alpha)] == [bits(x) for x in (a0, a1, a2, a3, a3)]
+    assert [scalar_bits(x) for x in (it.alpha_inversion, it.alpha_partial_ccd, it.alpha_swept_grid, it.alpha_full_ccd, it.alpha)] == [scalar_bits(x) for x in (a0, a1, a2, a3, a3)]
     assert it.n_full_ccd_candidates == ncand
     g2, a_2 = ctx.download(L.BUF_GRADIENT, 3 * m.nV), ctx.download(L.BUF_CSR_VALUES, ja.size)
     assert rel(g2, g) <= 1e-13 and rel(a_2, a) <= 1e-13  # (atomics: summation order differs run to run)
@@ -67,17 +61,15 @@ def test_deferred_iteration_equals_synchronous_calls(gpu_ctx, canonical):
     al, _ = orc.ccd_partial(s, p, cand, tol, evf, eee, al, 8)
     gr, ag = orc.grid_swept(s, p, al, h)
     al, _, _ = orc.ccd_full(s, p, gr, ag, tol, evf, eee, ag, 8)
-    assert bits(it.alpha) == bits(al)
-    ctx.set_canonical_order(1)
+    assert scalar_bits(it.alpha) == scalar_bits(al)
 
 
-def test_deferred_errors_surface_at_fetch(gpu_ctx):
+def test_deferred_errors_surface_at_fetch(shared_ctx):
     """d <= 0 in the barrier energy (the reference exits there) is reported by the fetch when nothing was read back in between"""
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = scenes.ball_pile(2, res=4, seed=1, height=2)
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
+    ctx.set_canonical_order(1)
     bad = np.array([[-1, 0, -1, -1]], dtype=np.int32)  # a vertex against itself: d = 0
     ctx.set_constraint_set(bad, bad[:0], np.empty((0, 2), dtype=np.int32))
     ctx.barrier_energy(info["dHat"], 1e3, want=False)
@@ -86,17 +78,15 @@ def test_deferred_errors_surface_at_fetch(gpu_ctx):
     assert ctx.fetch_iteration().status == 0  # flags are per fetch
 
 
-def test_captured_graph_replays_the_iteration_at_new_states(gpu_ctx):
+def test_captured_graph_replays_the_iteration_at_new_states(shared_ctx):
     """ipcgpu_capture_begin/_end: the device-resident iteration captured ONCE into a CUDA graph and replayed at other positions and another
     search direction gives bit-identical step bounds and the same energies / gradient / CSR values as the eager calls at that state.
     A graph is refused after a call that may reallocate or re-partition."""
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     dHat, p, kappa, dt2, tol = info["dHat"], info["p"], 1e8, 0.025 ** 2, 1e-6
     h = m.avgEdgeLen / 3
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
     ctx.set_canonical_order(0)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     mm, pa, pe, cand = ctx.constraint_set(dHat, 1)
@@ -141,8 +131,8 @@ def test_captured_graph_replays_the_iteration_at_new_states(gpu_ctx):
     ctx.graph_launch(gid)
     it1, g1, a1 = result()
     assert ctx.launch_count() - n_before >= 40
-    assert [bits(x) for x in (it1.alpha_inversion, it1.alpha_partial_ccd, it1.alpha_swept_grid, it1.alpha_full_ccd)] == \
-        [bits(x) for x in (it0.alpha_inversion, it0.alpha_partial_ccd, it0.alpha_swept_grid, it0.alpha_full_ccd)]
+    assert [scalar_bits(x) for x in (it1.alpha_inversion, it1.alpha_partial_ccd, it1.alpha_swept_grid, it1.alpha_full_ccd)] == \
+        [scalar_bits(x) for x in (it0.alpha_inversion, it0.alpha_partial_ccd, it0.alpha_swept_grid, it0.alpha_full_ccd)]
     assert (it1.n_active, it1.n_mollified, it1.n_candidates) == (it0.n_active, it0.n_mollified, it0.n_candidates)
     assert rel(g1, g0) <= 1e-13 and rel(a1, a0) <= 1e-13 and abs(it1.energy_barrier - it0.energy_barrier) <= 1e-12 * abs(it0.energy_barrier)
     # another state and another search direction through the SAME graph
@@ -154,8 +144,8 @@ def test_captured_graph_replays_the_iteration_at_new_states(gpu_ctx):
     enqueue()
     it3, g3, a3 = result()
     assert it2.n_active == len(mm2) == it3.n_active and len(mm2) != len(mm)
-    assert [bits(x) for x in (it2.alpha_inversion, it2.alpha_partial_ccd, it2.alpha_swept_grid, it2.alpha_full_ccd, it2.alpha)] == \
-        [bits(x) for x in (it3.alpha_inversion, it3.alpha_partial_ccd, it3.alpha_swept_grid, it3.alpha_full_ccd, it3.alpha)]
+    assert [scalar_bits(x) for x in (it2.alpha_inversion, it2.alpha_partial_ccd, it2.alpha_swept_grid, it2.alpha_full_ccd, it2.alpha)] == \
+        [scalar_bits(x) for x in (it3.alpha_inversion, it3.alpha_partial_ccd, it3.alpha_swept_grid, it3.alpha_full_ccd, it3.alpha)]
     assert rel(g2, g3) <= 1e-13 and rel(a2, a3) <= 1e-13
     assert abs(it2.energy_elastic - it3.energy_elastic) <= 1e-14 * abs(it3.energy_elastic)
     # ... and the oracle at that state
@@ -165,19 +155,18 @@ def test_captured_graph_replays_the_iteration_at_new_states(gpu_ctx):
     al, _ = orc.ccd_partial(s2, p2, cand2, tol, evf, eee, al, 8)
     gr, ag = orc.grid_swept(s2, p2, al, h)
     al, _, _ = orc.ccd_full(s2, p2, gr, ag, tol, evf, eee, ag, 8)
-    assert bits(it2.alpha) == bits(al)
+    assert scalar_bits(it2.alpha) == scalar_bits(al)
     # a call that may reallocate invalidates the graph
     ctx.set_csr(ia, ja, 1)
     with pytest.raises(L.IpcGpuError, match="capture it again"):
         ctx.graph_launch(gid)
     ctx.graph_destroy(gid)
     ctx.set_state(m.V_soa)
-    ctx.set_canonical_order(1)
 
 
-def test_async_download_on_the_copy_stream_eager_and_captured(gpu_ctx):
+def test_async_download_on_the_copy_stream_eager_and_captured(shared_ctx):
     """ipcgpu_download_range_async: the copy is forked behind what produced the buffer and joined by the fetch -- also as part of a graph"""
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = scenes.ball_pile(2, res=6, seed=1, height=2)
     dt2 = 0.025 ** 2
     ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)

@@ -2,7 +2,6 @@
 mirror's set_pattern(vNeighbor + augmentConnectivity(sets)) at every state, `changed` tracking, values equal to the oracle and to host-pattern
 mode, one captured graph across changing contacts, the capacity error, the obstacle tail, the PCG solve after a change, and two ranks."""
 import os
-import struct
 import subprocess
 import sys
 
@@ -12,29 +11,16 @@ import scipy.sparse as sp
 import scipy.sparse.linalg as spla
 
 import oracle as orc
+from gpu_common import rel, scalar_bits, shared_ctx, soa
 from ipc_b200 import lib as L
 from ipc_b200 import scenes
-from stagecheck import contact_pattern_pairs, rel
+from stagecheck import contact_pattern_pairs
+from test_gpu_multilevel import load_sorted
 from test_oracle_meshco import contact_pairs
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KAPPA, DT2, TOL = 1e8, 0.025 ** 2, 1e-6
-
-
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def upload(ctx, m):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
-    ctx.set_canonical_order(1)
 
 
 def states(ctx, m, info):
@@ -62,11 +48,11 @@ def at(ctx, V, dHat):
 
 
 @pytest.mark.parametrize("base", [0, 1])
-def test_exact_pattern_with_and_without_friction(gpu_ctx, base):
-    ctx = gpu_ctx
+def test_exact_pattern_with_and_without_friction(shared_ctx, base):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     dHat = info["dHat"]
-    upload(ctx, m)
+    load_sorted(ctx, m)
     S = states(ctx, m, info)
     ctx.enable_device_pattern(base)
     ia, ja = ctx.get_pattern()
@@ -93,16 +79,16 @@ def test_exact_pattern_with_and_without_friction(gpu_ctx, base):
     assert np.array_equal(ctx.get_pattern()[1], host_pattern(m, [(mm, pa, pe)], base)[1])
 
 
-def test_c5_full_size_pattern(gpu_ctx):
+def test_c5_full_size_pattern(shared_ctx):
     sys.path.insert(0, ROOT)
     import bench
 
     class Args:
         tets, res, scene = 1_000_000, 10, "c5"
 
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = bench.build_scene(Args())
-    upload(ctx, m)
+    load_sorted(ctx, m)
     mm, pa, pe, _ = ctx.constraint_set(info["dHat"], 1)
     assert len(mm) > 1000
     ctx.enable_device_pattern(1)
@@ -113,11 +99,11 @@ def test_c5_full_size_pattern(gpu_ctx):
     assert ctx.update_pattern() == (0, nnz)
 
 
-def test_change_tracking(gpu_ctx):
-    ctx = gpu_ctx
+def test_change_tracking(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     dHat = info["dHat"]
-    upload(ctx, m)
+    load_sorted(ctx, m)
     S = states(ctx, m, info)
     ctx.enable_device_pattern(1)
     seen = []
@@ -139,11 +125,11 @@ def test_change_tracking(gpu_ctx):
     assert seen[-1][1] == m.csr_pattern(1)[1].size  # no contact: back to the mesh pattern
 
 
-def test_values_match_oracle_and_host_mode(gpu_ctx):
-    ctx = gpu_ctx
+def test_values_match_oracle_and_host_mode(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     dHat = info["dHat"]
-    upload(ctx, m)
+    load_sorted(ctx, m)
     S = states(ctx, m, info)
     ctx.enable_device_pattern(1)
     at(ctx, S["A"], dHat)
@@ -174,11 +160,11 @@ def test_values_match_oracle_and_host_mode(gpu_ctx):
     assert np.array_equal(a1, a2) and np.array_equal(g1, g2)
 
 
-def test_one_graph_across_changing_contacts(gpu_ctx):
-    ctx = gpu_ctx
+def test_one_graph_across_changing_contacts(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     dHat, p, h = info["dHat"], info["p"], m.avgEdgeLen / 3
-    upload(ctx, m)
+    load_sorted(ctx, m)
     S = states(ctx, m, info)
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     ctx.enable_device_pattern(1)
@@ -204,7 +190,7 @@ def test_one_graph_across_changing_contacts(gpu_ctx):
         ia, ja = ctx.get_pattern()
         part = ctx.partition_info()
         assert part["value_begin"] == 0 and part["value_end"] == ja.size
-        steps = [bits(x) for x in (it.alpha_inversion, it.alpha_partial_ccd, it.alpha_swept_grid, it.alpha_full_ccd, it.alpha)]
+        steps = [scalar_bits(x) for x in (it.alpha_inversion, it.alpha_partial_ccd, it.alpha_swept_grid, it.alpha_full_ccd, it.alpha)]
         return it, ia, ja, steps, ctx.download(L.BUF_GRADIENT, 3 * m.nV), ctx.download(L.BUF_CSR_VALUES, ja.size)
 
     ctx.set_state(soa(S["A"]))
@@ -235,14 +221,13 @@ def test_one_graph_across_changing_contacts(gpu_ctx):
             assert it1.n_active == 0 and ja1.size == m.csr_pattern(1)[1].size
     ctx.graph_destroy(gid)
     hg.free()
-    ctx.set_canonical_order(1)
 
 
-def test_capacity_error_and_raise(gpu_ctx):
-    ctx = gpu_ctx
+def test_capacity_error_and_raise(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     dHat = info["dHat"]
-    upload(ctx, m)
+    load_sorted(ctx, m)
     S = states(ctx, m, info)
     ctx.enable_device_pattern(1)
     at(ctx, S["A"], dHat)
@@ -267,13 +252,13 @@ def test_capacity_error_and_raise(gpu_ctx):
     assert np.array_equal(ctx.get_pattern()[1], host_pattern(m, [(mmB, paB, peB)])[1])
 
 
-def test_obstacle_tail_rows_stay_diagonal(gpu_ctx):
+def test_obstacle_tail_rows_stay_diagonal(shared_ctx):
     from ipc_b200 import obstacle as OB
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = scenes.balls_on_obstacle(plate_angle=0.0, res=4, plate=12)
     ob = info["obstacle"]
     M2 = OB.with_obstacle(m, ob["V"], ob["E"], ob["F"])
-    upload(ctx, M2)
+    load_sorted(ctx, M2)
     ctx.set_obstacle_tail(M2.nV_dof, 1)
     ctx.enable_device_pattern(1)
     mm, pa, pe, _ = ctx.constraint_set(info["dHat"], 1)
@@ -285,7 +270,6 @@ def test_obstacle_tail_rows_stay_diagonal(gpu_ctx):
     rows = np.arange(3 * M2.nV_dof, 3 * M2.nV)
     assert np.array_equal(np.diff(ia)[rows], 3 - rows % 3)  # the tail's rows: the diagonal block only
     assert (ja[: ia[3 * M2.nV_dof] - 1] <= 3 * M2.nV_dof).all()  # no mesh row reaches into the tail's columns
-    ctx.set_obstacle_tail(-1)
 
 
 def full_matrix(ia, ja, a, n):
@@ -293,11 +277,11 @@ def full_matrix(ia, ja, a, n):
     return (U + sp.triu(U, 1).T).tocsc()
 
 
-def test_pcg_after_a_pattern_change(gpu_ctx):
-    ctx = gpu_ctx
+def test_pcg_after_a_pattern_change(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
     dHat, kappa = info["dHat"], 1e6
-    upload(ctx, m)
+    load_sorted(ctx, m)
     S = states(ctx, m, info)
     ctx.enable_device_pattern(1)
     for name in ("A", "B"):

@@ -1,33 +1,17 @@
 """Half-space collision objects (ipcgpu_set_halfspaces and the ipcgpu_halfspace_* stages, HalfSpace<3>) against the CPU oracle
 (oracle/halfspace.cpp): sets, counts and step bounds bit for bit, energies and gradients to 1e-10, Hessians to 1e-9 -- eagerly, deferred and
 replayed from a graph; the planes inside the line search; and a context with no planes launching exactly what it launched before."""
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
 import oracle_halfspace as OH
+from gpu_common import load_scene, own_context, rel, scalar_bits, soa
 from ipc_b200 import lib as L
 from ipc_b200 import scenes
 
 pytestmark = pytest.mark.gpu
-
-
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def rel(a, b):
-    return abs(a - b) / max(abs(b), 1e-300)
-
-
-def nrel(a, b):
-    return np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-300)
 
 
 class Small:
@@ -63,10 +47,11 @@ class Small:
         self.Vprev = m.V - T
 
 
-def upload(ctx, sc, V=None):
+def upload_with_csr(ctx, sc, V=None):
     m = sc.m
     ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
     ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
+    ctx.set_canonical_order(1)
     ia, ja = m.csr_pattern(1)
     ctx.set_csr(ia, ja, 1)
     ctx.set_state(soa(m.V if V is None else V))
@@ -94,14 +79,13 @@ def oracle_all(sc, V, ia, ja):
 
 @pytest.fixture(scope="module")
 def ctx():
-    c = L.Context(0)
-    yield c
-    c.close()
+    with own_context() as c:
+        yield c
 
 
 def test_small_scene_eager_matches_oracle(ctx):
     sc = Small()
-    ia, ja = upload(ctx, sc)
+    ia, ja = upload_with_csr(ctx, sc)
     ctx.set_halfspaces(sc.origin, sc.normal, sc.vdt, sc.friction)
     ref = oracle_all(sc, sc.m.V, ia, ja)
     assert len(ref["act"]) >= 4 and {0, 1} <= set(ref["act"][:, 0]) and ref["bad"] == 0
@@ -110,15 +94,15 @@ def test_small_scene_eager_matches_oracle(ctx):
     assert n == len(ref["act"]) and np.array_equal(act, ref["act"])
     assert rel(ctx.halfspace_energy(sc.dHat, sc.kappa), ref["E"]) <= 1e-10
     g = ctx.halfspace_gradient(sc.dHat, sc.kappa, np.zeros(3 * sc.m.nV))
-    assert nrel(g, ref["g"]) <= 1e-10
+    assert rel(g, ref["g"]) <= 1e-10
     a = ctx.halfspace_hessian(sc.dHat, sc.kappa, 1, np.zeros(ja.size))
-    assert nrel(a, ref["a"]) <= 1e-9 and np.linalg.norm(ref["a"]) > 0
+    assert rel(a, ref["a"]) <= 1e-9 and np.linalg.norm(ref["a"]) > 0
     alpha, rc = ctx.halfspace_step(None, 0.9, 1.0)
-    assert rc == 0 and bits(alpha) == bits(ref["alpha"]) and 0.0 < alpha < 1.0
+    assert rc == 0 and scalar_bits(alpha) == scalar_bits(ref["alpha"]) and 0.0 < alpha < 1.0
     assert ctx.halfspace_crossings() == ref["cross"] == 0
     assert ctx.halfspace_friction_lag(sc.dHat, sc.kappa) == len(ref["lag"])
     _, lag, lam = ctx.get_halfspace_sets()
-    assert np.array_equal(lag, ref["lag"]) and nrel(lam, ref["lam"]) <= 1e-13
+    assert np.array_equal(lag, ref["lag"]) and rel(lam, ref["lam"]) <= 1e-13
     # both friction branches occur
     u = (sc.m.V - sc.Vprev)[lag[:, 1]] - sc.vdt[lag[:, 0]]
     nn = sc.par[lag[:, 0], :3]
@@ -127,9 +111,9 @@ def test_small_scene_eager_matches_oracle(ctx):
     assert slide.any() and (~slide).any()
     assert rel(ctx.halfspace_friction_energy(sc.eps2), ref["Ef"]) <= 1e-10
     gf = ctx.halfspace_friction_gradient(sc.eps2, np.zeros(3 * sc.m.nV))
-    assert nrel(gf, ref["gf"]) <= 1e-10
+    assert rel(gf, ref["gf"]) <= 1e-10
     af = ctx.halfspace_friction_hessian(sc.eps2, 1, np.zeros(ja.size))
-    assert nrel(af, ref["af"]) <= 1e-9
+    assert rel(af, ref["af"]) <= 1e-9
     # the plane blocks sit in the vertices' diagonal blocks only
     rows = np.repeat(np.arange(ia.size - 1), np.diff(ia))
     cols = ja - 1
@@ -139,7 +123,7 @@ def test_small_scene_eager_matches_oracle(ctx):
 def test_crossing_and_zero_step(ctx):
     sc = Small()
     V = sc.m.V.copy()
-    ia, ja = upload(ctx, sc, V)
+    ia, ja = upload_with_csr(ctx, sc, V)
     v = int(sc.m.SVI[np.argsort(sc.m.V[sc.m.SVI, 1])][2])  # not Dirichlet, codimension 3
     V[v, 1] = sc.origin[0, 1]                               # exactly on the floor
     ctx.set_state(soa(V))
@@ -184,7 +168,7 @@ def run_eager_reference(ctx, sc, ia, ja):
 @pytest.mark.parametrize("captured", [False, True])
 def test_deferred_and_captured_equal_eager(ctx, captured):
     sc = Small()
-    ia, ja = upload(ctx, sc)
+    ia, ja = upload_with_csr(ctx, sc)
     ctx.set_halfspaces(sc.origin, sc.normal, sc.vdt, sc.friction)
     ctx.set_canonical_order(0)
     ctx.halfspace_constraint_set(sc.dHat)
@@ -203,7 +187,7 @@ def test_deferred_and_captured_equal_eager(ctx, captured):
         ctx.set_state(soa(V))
         n, E, Ef, alpha, g, a, act = run_eager_reference(ctx, sc, ia, ja)
         ref = oracle_all(sc, V, ia, ja)
-        assert n == len(ref["act"]) and bits(alpha) == bits(ref["alpha"]) and rel(E, ref["E"]) <= 1e-10
+        assert n == len(ref["act"]) and scalar_bits(alpha) == scalar_bits(ref["alpha"]) and rel(E, ref["E"]) <= 1e-10
         ctx.set_state(soa(V))
         ctx.fetch_iteration()
         ctx.set_search_dir(sc.p)
@@ -214,22 +198,21 @@ def test_deferred_and_captured_equal_eager(ctx, captured):
             deferred_sequence(ctx, sc)
         it = ctx.fetch_iteration()
         assert it.status == 0 and it.n_halfspace_active == n and it.n_halfspace_crossings == 0
-        assert bits(it.alpha_halfspace) == bits(alpha) and bits(it.alpha) == bits(alpha)
+        assert scalar_bits(it.alpha_halfspace) == scalar_bits(alpha) and scalar_bits(it.alpha) == scalar_bits(alpha)
         assert rel(it.energy_halfspace, E) <= 1e-12 and rel(it.energy_halfspace_friction, Ef) <= 1e-12
         act2, _, _ = ctx.get_halfspace_sets()
         assert np.array_equal(act2, act)
         ctx.download_into(L.BUF_GRADIENT, g_dev)
-        assert nrel(g_dev, g) <= 1e-12
+        assert rel(g_dev, g) <= 1e-12
         a_dev = ctx.download(L.BUF_CSR_VALUES, ja.size)
-        assert nrel(a_dev, a) <= 1e-12
+        assert rel(a_dev, a) <= 1e-12
     if gid is not None:
         ctx.graph_destroy(gid)
-    ctx.set_canonical_order(1)
 
 
 def test_device_pattern_holds_the_plane_blocks(ctx):
     sc = Small()
-    ia, ja = upload(ctx, sc)
+    ia, ja = upload_with_csr(ctx, sc)
     ctx.enable_device_pattern(1)
     ctx.set_halfspaces(sc.origin, sc.normal, sc.vdt, sc.friction)
     ctx.constraint_set(sc.dHat, 1, fetch=False, sizes=False)
@@ -240,7 +223,7 @@ def test_device_pattern_holds_the_plane_blocks(ctx):
     ia2, ja2 = ctx.get_pattern()
     ref = oracle_all(sc, sc.m.V, ia2, ja2)
     a = ctx.halfspace_hessian(sc.dHat, sc.kappa, 1, np.zeros(ja2.size))
-    assert nrel(a, ref["a"]) <= 1e-9
+    assert rel(a, ref["a"]) <= 1e-9
     ctx.set_csr(ia, ja, 1)
 
 
@@ -263,17 +246,16 @@ def test_no_planes_launch_nothing(ctx):
     sc = Small()
     counts, alphas = [], []
     for setting in ("never", "removed"):
-        c = L.Context(0)
-        upload(c, sc)
-        if setting == "removed":
-            c.set_halfspaces(sc.origin, sc.normal, sc.vdt, sc.friction)
-            c.set_halfspaces([], [])
-        n0 = c.launch_count()
-        it = iteration_calls(c, sc, False)
-        counts.append(c.launch_count() - n0)
-        alphas.append(bits(it.alpha))
-        assert it.n_halfspace_active == 0 and it.energy_halfspace == 0.0
-        c.close()
+        with own_context() as c:
+            upload_with_csr(c, sc)
+            if setting == "removed":
+                c.set_halfspaces(sc.origin, sc.normal, sc.vdt, sc.friction)
+                c.set_halfspaces([], [])
+            n0 = c.launch_count()
+            it = iteration_calls(c, sc, False)
+            counts.append(c.launch_count() - n0)
+            alphas.append(scalar_bits(it.alpha))
+            assert it.n_halfspace_active == 0 and it.energy_halfspace == 0.0
     assert counts[0] == counts[1] and alphas[0] == alphas[1]
 
 
@@ -378,7 +360,7 @@ LS_CASE = (0.1, 0.5, 0.3, 0.4)
 
 def ls_upload(ctx, sc, canonical):
     import test_gpu_step_control as SC
-    SC.upload(ctx, sc, canonical=canonical)  # mesh, surface, state, p, xTilta, contact sets, prev state, self-friction lag
+    SC.load_step_scene(ctx, sc, canonical=canonical)  # mesh, surface, state, p, xTilta, contact sets, prev state, self-friction lag
     ctx.set_halfspaces(*sc.plane)
     ctx.halfspace_constraint_set(sc.dHat)
     ctx.halfspace_friction_lag(sc.dHat, sc.kappa)
@@ -411,8 +393,8 @@ def test_line_search_with_planes_matches_oracle(ctx):
             assert ctx.line_search(**t, check=False) == 0
             e = ctx.step_control_info()
             assert e.status == 0
-            assert bits(e.alpha) == bits(want["alpha"]) and SC.counts(e) == want["counts"], (planes, e.alpha, want["alpha"], SC.counts(e), want["counts"])
-            assert bool(e.stopped) == want["stopped"] and bool(e.post_check_rebuilt) == want["rebuilt"] and bits(e.alpha_feasible) == bits(want["LF"])
+            assert scalar_bits(e.alpha) == scalar_bits(want["alpha"]) and SC.counts(e) == want["counts"], (planes, e.alpha, want["alpha"], SC.counts(e), want["counts"])
+            assert bool(e.stopped) == want["stopped"] and bool(e.post_check_rebuilt) == want["rebuilt"] and scalar_bits(e.alpha_feasible) == scalar_bits(want["LF"])
             assert rel(e.energy_start, want["E0"]) <= 1e-10 and rel(e.energy, want["Et"]) <= 1e-10
             if canonical:
                 continue
@@ -425,10 +407,9 @@ def test_line_search_with_planes_matches_oracle(ctx):
             ls_entry(ctx, sc, planes, ref["alpha0"])
             ctx.graph_launch(gid)
             g = ctx.step_control_info()
-            assert g.status == 0 and bits(g.alpha) == bits(want["alpha"]) and SC.counts(g) == want["counts"]
+            assert g.status == 0 and scalar_bits(g.alpha) == scalar_bits(want["alpha"]) and SC.counts(g) == want["counts"]
             assert rel(g.energy, want["Et"]) <= 1e-10 and rel(g.energy_start, want["E0"]) <= 1e-10
             ctx.graph_destroy(gid)
-    ctx.set_canonical_order(1)
 
 
 def test_two_ranks_match_the_oracle():
@@ -452,14 +433,12 @@ def test_two_ranks_match_the_oracle():
 def test_larger_surface_on_the_same_context(ctx):
     """planes on a small surface, then a larger surface on the same context: the scan's temporary storage follows the surface"""
     small = Small()
-    upload(ctx, small)
+    upload_with_csr(ctx, small)
     ctx.set_halfspaces(small.origin, small.normal, small.vdt, small.friction)
     assert ctx.halfspace_constraint_set(small.dHat) == len(oracle_all(small, small.m.V, *small.m.csr_pattern(1))["act"])
     m, info = scenes.ball_pile(64, res=10, seed=7, height=8)
     assert m.SVI.size > 8 * small.m.SVI.size
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
     sq = np.sqrt(info["dHat"])
     origin, normal = [[0.0, m.V[:, 1].min() - 0.5 * sq, 0.0], [m.V[:, 0].max() + 0.5 * sq, 0.0, 0.0]], [[0.0, 1.0, 0.0], [-1.0, 0.0, 0.0]]
     ctx.set_halfspaces(origin, normal, None, [0.0, 0.0])
@@ -485,60 +464,59 @@ def test_c5_captured_iteration_with_a_ground_plane():
     P[:, 1] -= 6.0 * sq
     p = np.ascontiguousarray(P).ravel()
     origin, normal = [[0.0, m.V[:, 1].min() - 0.5 * sq, 0.0]], [[0.0, 1.0, 0.0]]
-    ctx = L.Context(0)
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ia, ja = m.csr_pattern(1)
-    ctx.set_csr(ia, ja, 1)
-    ctx.set_canonical_order(0)
-    ctx.set_state(m.V_soa)
-    ctx.set_search_dir(p)
-    ctx.set_halfspaces(origin, normal, None, [0.0])
-    evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
+    with own_context() as ctx:
+        ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
+        ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
+        ia, ja = m.csr_pattern(1)
+        ctx.set_csr(ia, ja, 1)
+        ctx.set_canonical_order(0)
+        ctx.set_state(m.V_soa)
+        ctx.set_search_dir(p)
+        ctx.set_halfspaces(origin, normal, None, [0.0])
+        evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
 
-    def iteration():
-        ctx.constraint_set(dHat, 1, fetch=False, sizes=False)
-        ctx.halfspace_constraint_set(dHat, want=False)
-        ctx.halfspace_energy(dHat, kappa, want=False)
-        ctx.halfspace_crossings(want=False)
-        ctx.csr_set_zero()
-        ctx.elastic_gradient(0.0, want=False)
-        ctx.halfspace_gradient(dHat, kappa)
-        ctx.halfspace_hessian(dHat, kappa, 1)
-        ctx.step_bound_set(1.0)
-        ctx.inversion_step(None, 0.2, None)
-        ctx.halfspace_step(None, 0.9, None)
-        ctx.ccd_partial(None, tol, evf, eee, None)
-        ctx.hash_build_swept(None, None, h)
-        ctx.ccd_full(tol, evf, eee, None)
+        def iteration():
+            ctx.constraint_set(dHat, 1, fetch=False, sizes=False)
+            ctx.halfspace_constraint_set(dHat, want=False)
+            ctx.halfspace_energy(dHat, kappa, want=False)
+            ctx.halfspace_crossings(want=False)
+            ctx.csr_set_zero()
+            ctx.elastic_gradient(0.0, want=False)
+            ctx.halfspace_gradient(dHat, kappa)
+            ctx.halfspace_hessian(dHat, kappa, 1)
+            ctx.step_bound_set(1.0)
+            ctx.inversion_step(None, 0.2, None)
+            ctx.halfspace_step(None, 0.9, None)
+            ctx.ccd_partial(None, tol, evf, eee, None)
+            ctx.hash_build_swept(None, None, h)
+            ctx.ccd_full(tol, evf, eee, None)
 
-    iteration()  # eager first: lazy allocations
-    ctx.fetch_iteration()
-    ctx.capture_begin()
-    iteration()
-    gid = ctx.capture_end()
-    ctx.graph_launch(gid)
-    it = ctx.fetch_iteration()
-    assert it.status == 0
-    s = orc.Surf(m)
-    hs = OH.HalfSpaces(s, OH.planes(origin, normal, None, [0.0]))
-    act = hs.constraint_set(dHat)
-    assert len(act) > 0 and it.n_halfspace_active == len(act) and np.array_equal(ctx.get_halfspace_sets()[0], act)
-    E_ref, bad = hs.energy(act, dHat, kappa)
-    assert bad == 0 and rel(it.energy_halfspace, E_ref) <= 1e-10 and it.n_halfspace_crossings == hs.crossings() == 0
-    g = np.empty(3 * m.nV)
-    ctx.download_into(L.BUF_GRADIENT, g)
-    assert nrel(g, hs.gradient(act, dHat, kappa)) <= 1e-10
-    a = ctx.download(L.BUF_CSR_VALUES, ja.size)
-    assert nrel(a, hs.hessian_csr(act, dHat, kappa, ia, ja, 1)) <= 1e-9
-    a_inv, _ = orc.Elastic(m).inversion_step(p, 0.2, 1.0)
-    assert rel(it.alpha_inversion, a_inv) <= 1e-9  # (the inversion filter's own tolerance)
-    a_hs = hs.step(p, 0.9, it.alpha_inversion)       # the plane bound of the step that entered it
-    assert bits(it.alpha_halfspace) == bits(a_hs) and a_hs < it.alpha_inversion  # ... binding
-    nC, nP, nK = ctx.constraint_set_sizes()
-    mm, pa, pe, cand = np.empty((nC, 4), np.int32), np.empty((nP, 4), np.int32), np.empty((nP, 2), np.int32), np.empty((nK, 2), np.int32)
-    ctx._ck(ctx.lib.ipcgpu_get_constraint_set(ctx.h, L._i(mm), L._i(pa), L._i(pe), L._i(cand)))
-    a_part, _ = orc.ccd_partial(s, p, cand, tol, evf, eee, a_hs, nthreads=8)
-    assert bits(it.alpha_partial_ccd) == bits(a_part) and it.alpha_full_ccd <= a_part
-    ctx.graph_destroy(gid)
-    ctx.close()
+        iteration()  # eager first: lazy allocations
+        ctx.fetch_iteration()
+        ctx.capture_begin()
+        iteration()
+        gid = ctx.capture_end()
+        ctx.graph_launch(gid)
+        it = ctx.fetch_iteration()
+        assert it.status == 0
+        s = orc.Surf(m)
+        hs = OH.HalfSpaces(s, OH.planes(origin, normal, None, [0.0]))
+        act = hs.constraint_set(dHat)
+        assert len(act) > 0 and it.n_halfspace_active == len(act) and np.array_equal(ctx.get_halfspace_sets()[0], act)
+        E_ref, bad = hs.energy(act, dHat, kappa)
+        assert bad == 0 and rel(it.energy_halfspace, E_ref) <= 1e-10 and it.n_halfspace_crossings == hs.crossings() == 0
+        g = np.empty(3 * m.nV)
+        ctx.download_into(L.BUF_GRADIENT, g)
+        assert rel(g, hs.gradient(act, dHat, kappa)) <= 1e-10
+        a = ctx.download(L.BUF_CSR_VALUES, ja.size)
+        assert rel(a, hs.hessian_csr(act, dHat, kappa, ia, ja, 1)) <= 1e-9
+        a_inv, _ = orc.Elastic(m).inversion_step(p, 0.2, 1.0)
+        assert rel(it.alpha_inversion, a_inv) <= 1e-9  # (the inversion filter's own tolerance)
+        a_hs = hs.step(p, 0.9, it.alpha_inversion)       # the plane bound of the step that entered it
+        assert scalar_bits(it.alpha_halfspace) == scalar_bits(a_hs) and a_hs < it.alpha_inversion  # ... binding
+        nC, nP, nK = ctx.constraint_set_sizes()
+        mm, pa, pe, cand = np.empty((nC, 4), np.int32), np.empty((nP, 4), np.int32), np.empty((nP, 2), np.int32), np.empty((nK, 2), np.int32)
+        ctx._ck(ctx.lib.ipcgpu_get_constraint_set(ctx.h, L._i(mm), L._i(pa), L._i(pe), L._i(cand)))
+        a_part, _ = orc.ccd_partial(s, p, cand, tol, evf, eee, a_hs, nthreads=8)
+        assert scalar_bits(it.alpha_partial_ccd) == scalar_bits(a_part) and it.alpha_full_ccd <= a_part
+        ctx.graph_destroy(gid)

@@ -2,12 +2,14 @@
 results; ipcgpu_kappa_init (initKappa) and ipcgpu_kappa_post_line_search (postLineSearch's close-pair doubling) against the float64
 restatement of tests/oracle_kappa.py; a few time steps of Newton iterations with kappa on the device, eagerly, replayed from one graph and
 driven from the host with the restatement's kappa, take the same doubling decisions."""
-import struct
+
+import contextlib
 
 import numpy as np
 import pytest
 
 import oracle_kappa as ok
+from gpu_common import load_scene, own_context, rel, scalar_bits, soa
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from ipc_b200 import obstacle as OB
@@ -19,26 +21,13 @@ DT2 = 0.025 ** 2
 TOL = 1e-6
 
 
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def rel(a, b):
-    return float(np.linalg.norm(np.asarray(a) - np.asarray(b)) / max(np.linalg.norm(b), 1e-300))
-
-
+@contextlib.contextmanager
 def context(m, nV_dof=None):
-    ctx = L.Context(0)
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
-    if nV_dof is not None:
-        ctx.set_obstacle_tail(nV_dof)
-    return ctx
+    with own_context() as ctx:
+        load_scene(ctx, m)
+        if nV_dof is not None:
+            ctx.set_obstacle_tail(nV_dof)
+        yield ctx
 
 
 def mat_scene(**kw):
@@ -59,8 +48,7 @@ def host_sets(ctx, dHat, planes):
 def test_sentinel_equivalence():
     m, info, dHat, pl = mat_scene()
     K, n = 3.7e5, 3 * m.nV
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         ctx.set_halfspaces(**pl)
         ctx.set_prev_state(soa(m.V - 1e-3 * info["p"].reshape(-1, 3)))
         ctx.enable_device_pattern(1)
@@ -69,7 +57,7 @@ def test_sentinel_equivalence():
         ctx.update_pattern()
         ctx.set_kappa(K, 0.0, 1e300)
         for f in (ctx.barrier_energy, ctx.halfspace_energy):
-            assert bits(f(dHat, KD)) == bits(f(dHat, K))
+            assert scalar_bits(f(dHat, KD)) == scalar_bits(f(dHat, K))
 
         def spread_check(call, size):
             h1, h2, d = (call(k, np.zeros(size)) for k in (K, K, KD))
@@ -99,13 +87,11 @@ def test_sentinel_equivalence():
             ctx.set_search_dir(info["p"])
             rc, a = ctx.line_search(DT2, dHat, k, alpha=1.0, check=False)
             s = ctx.step_control_info()
-            res.append((rc, bits(a), bits(s.energy_start), bits(s.energy), s.halvings_inversion, s.halvings_intersection, s.halvings_armijo,
+            res.append((rc, scalar_bits(a), scalar_bits(s.energy_start), scalar_bits(s.energy), s.halvings_inversion, s.halvings_intersection, s.halvings_armijo,
                         s.halvings_post_check, ctx.download(L.BUF_POSITIONS, n).tobytes()))
         assert res[0] == res[1]
         with pytest.raises(L.IpcGpuError, match="ARG"):
             ctx.line_search(DT2, dHat, -2.0, alpha=1.0)
-    finally:
-        ctx.close()
 
 
 def spread(h1, h2, d):
@@ -121,27 +107,23 @@ def test_sentinel_mollified_pairs():
     ob = inf0["obstacle"]
     m = OB.with_obstacle(m0, ob["V"], ob["E"], ob["F"])
     dHat, K, n = inf0["dHat"], 2.9e7, 3 * m.nV
-    ctx = context(m, m.nV_dof)
-    try:
+    with context(m, m.nV_dof) as ctx:
         ctx.enable_device_pattern(1)
         ctx.constraint_set(dHat, 1)
         assert ctx.nP > 0
         ctx.update_pattern()
         ctx.set_kappa(K, 0.0, 1e300)
-        assert bits(ctx.barrier_energy(dHat, KD)) == bits(ctx.barrier_energy(dHat, K))
+        assert scalar_bits(ctx.barrier_energy(dHat, KD)) == scalar_bits(ctx.barrier_energy(dHat, K))
         for call, size in [(lambda k, g: ctx.para_ee_gradient(dHat, k, g), n), (lambda k, g: ctx.barrier_gradient(dHat, k, g), n),
                            (lambda k, a: ctx.barrier_hessian(dHat, k, 1, a), ctx.nnz)]:
             assert spread(*(call(k, np.zeros(size)) for k in (K, K, KD))) > 0
-    finally:
-        ctx.close()
 
 
 def test_hessian_right_after_a_kappa_write():
     """the reference's order: initKappa, then the Hessian at the same positions and sets; postLineSearch's doubling, then the next
     iteration's Hessian with no set rebuild in between.  The device-kappa Hessian must be the one at the kappa that was just written."""
     m, info, dHat, pl = mat_scene()
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         ctx.enable_device_pattern(1)
         ctx.constraint_set(dHat, 1)
         ctx.update_pattern()
@@ -162,9 +144,7 @@ def test_hessian_right_after_a_kappa_write():
         ctx.kappa_post_line_search(dHat)  # the snapshot
         ctx.kappa_post_line_search(dHat)  # the same positions: every saved d is equal, kappa doubles
         k2 = hessian_matches()
-        assert bits(k2) == bits(2.0 * k1) and ctx.kappa_info().doublings == 1
-    finally:
-        ctx.close()
+        assert scalar_bits(k2) == scalar_bits(2.0 * k1) and ctx.kappa_info().doublings == 1
 
 
 # ---- 2. initKappa ----------------------------------------------------------------------------------------------------------------
@@ -196,15 +176,14 @@ def test_kappa_init_scenes(which):
         m0, inf0 = scenes.balls_on_obstacle(res=4)
         ob = inf0["obstacle"]
         m = OB.with_obstacle(m0, ob["V"], ob["E"], ob["F"])
-        dHat, planes, ctx = inf0["dHat"], None, context(m, m.nV_dof)
+        dHat, planes, nV_dof = inf0["dHat"], None, m.nV_dof
     else:
         m, info, dHat, pl = mat_scene()
-        planes = pl if which == "plane" else None
-        ctx = context(m)
+        planes, nV_dof = (pl if which == "plane" else None), None
+    with context(m, nV_dof) as ctx:
         if planes:
             ctx.set_halfspaces(**planes)
             ctx.halfspace_constraint_set(dHat)
-    try:
         ctx.elastic_gradient(DT2, 1, 1, want=False)
         gE = ctx.download(L.BUF_GRADIENT, 3 * m.nV)
         s, mx = 1.0, 1e30
@@ -213,14 +192,11 @@ def test_kappa_init_scenes(which):
         assert abs(info.kappa - kappa) <= 1e-12 * abs(kappa), (info.kappa, kappa)
         assert abs(info.min_kappa - minK) <= 1e-12 * abs(minK)
         assert info.needs_init == 0
-    finally:
-        ctx.close()
 
 
 def test_kappa_init_branches():
     m, info, dHat, pl = mat_scene()
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         n = 3 * m.nV
         V = m.V
         mm, act = host_sets(ctx, dHat, False)
@@ -229,11 +205,11 @@ def test_kappa_init_branches():
         for K, expect in [(-1.0, k0), (1e9, mx), (10.0, s), (2e5, None)]:  # minK <= 0, above max, below suggest, in between
             got, kappa, minK, _ = init_case(ctx, m, dHat, k0, s, mx, -K * gc)
             exp = kappa if expect is None else expect
-            assert bits(kappa) == bits(exp) or expect is None
+            assert scalar_bits(kappa) == scalar_bits(exp) or expect is None
             if expect is None:
                 assert abs(got.kappa - kappa) <= 1e-12 * kappa
             else:
-                assert bits(got.kappa) == bits(expect), (K, got.kappa, expect)
+                assert scalar_bits(got.kappa) == scalar_bits(expect), (K, got.kappa, expect)
         # no active entries: nothing changes (not even minKappa)
         before = ctx.kappa_info().min_kappa
         ctx.constraint_set(1e-30, 1)
@@ -241,9 +217,7 @@ def test_kappa_init_branches():
         ctx.set_kappa(k0, s, mx)
         ctx.kappa_init(dHat)
         got = ctx.kappa_info()
-        assert bits(got.kappa) == bits(k0) and bits(got.min_kappa) == bits(before)
-    finally:
-        ctx.close()
+        assert scalar_bits(got.kappa) == scalar_bits(k0) and scalar_bits(got.min_kappa) == scalar_bits(before)
     # contact only on Dirichlet vertices against the obstacle (pairs between two Dirichlet mesh vertices are not built, obstacle pairs are):
     # g_c = 0, minKappa = NaN, kappa stays, then the floor
     m0, inf0 = scenes.balls_on_obstacle(res=4)
@@ -251,15 +225,12 @@ def test_kappa_init_branches():
     ob = inf0["obstacle"]
     m = OB.with_obstacle(m0, ob["V"], ob["E"], ob["F"])
     dHat = inf0["dHat"]
-    ctx = context(m, m.nV_dof)
-    try:
+    with context(m, m.nV_dof) as ctx:
         ctx.elastic_gradient(DT2, 1, 1, want=False)
         for k0, expect in [(5e4, 5e4), (10.0, 1e3)]:
             got, kappa, minK, gc = init_case(ctx, m, dHat, k0, 1e3, 1e7, ctx.download(L.BUF_GRADIENT, 3 * m.nV))
             assert ctx.nC > 0 and not np.any(gc) and minK is not None and np.isnan(minK) and np.isnan(got.min_kappa)
-            assert bits(got.kappa) == bits(expect) == bits(kappa)
-    finally:
-        ctx.close()
+            assert scalar_bits(got.kappa) == scalar_bits(expect) == scalar_bits(kappa)
 
 
 # ---- 3. postLineSearch -----------------------------------------------------------------------------------------------------------
@@ -279,7 +250,7 @@ def run_post(ctx, m, ref, V, dHat, dTol, planes=None, par=None):
     ctx.kappa_post_line_search(dTol)
     ref.post_line_search(V, mm, act, dTol, par)
     got = ctx.kappa_info()
-    assert bits(got.kappa) == bits(ref.kappa), (got.kappa, ref.kappa)
+    assert scalar_bits(got.kappa) == scalar_bits(ref.kappa), (got.kappa, ref.kappa)
     assert got.n_close == len(ref.saved) and got.doublings == ref.doublings and bool(got.needs_init) == ref.needs_init
     return got
 
@@ -292,8 +263,7 @@ def test_post_line_search(case):
     dHat = (1.5 * gap) ** 2
     dTol = dHat if case != "new_pair" else (0.5 * gap) ** 2
     k0, mx = 1e4, (1.5e4 if case == "capped" else 1e9)
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         ctx.set_kappa(0.0 if case == "zero" else k0, 1.0, mx)
         ctx.kappa_clear_close_set()
         ref = ok.CloseSet(0.0 if case == "zero" else k0, mx)
@@ -315,15 +285,13 @@ def test_post_line_search(case):
         expect = {"approach": 1, "recede": 0, "equal": 1, "left_set": 1, "new_pair": 0, "at_dTol": 1, "capped": 1, "zero": 0}[case]
         assert got.doublings == expect
         if case == "capped":
-            assert bits(got.kappa) == bits(mx)
+            assert scalar_bits(got.kappa) == scalar_bits(mx)
         if case == "zero":
             assert got.needs_init == 1 and got.kappa == 0.0
         if case == "new_pair":
             assert got.n_close > 0
         if case == "at_dTol":
             assert 0 < got.n_close < ctx.nC
-    finally:
-        ctx.close()
 
 
 def test_post_line_search_plane_and_obstacle():
@@ -335,8 +303,7 @@ def test_post_line_search_plane_and_obstacle():
     planes = dict(origin=[[0.0, 0.0, -gap]], normal=[[0.0, 0.0, 1.0]], friction=[0.0])
     import oracle_halfspace as ohs
     par = ohs.planes(planes["origin"], planes["normal"], None, planes["friction"])
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         ctx.set_halfspaces(**planes)
         ctx.set_kappa(1e4, 1.0, 1e9)
         ref = ok.CloseSet(1e4, 1e9)
@@ -345,15 +312,12 @@ def test_post_line_search_plane_and_obstacle():
         V2 = m.V.copy()
         V2[:, 2] -= 0.2 * gap
         assert run_post(ctx, m, ref, V2, dHat, dHat, True, par).doublings == 1
-    finally:
-        ctx.close()
     # an obstacle: the balls approach the plate
     m0, inf0 = scenes.balls_on_obstacle(res=4)
     ob = inf0["obstacle"]
     m = OB.with_obstacle(m0, ob["V"], ob["E"], ob["F"])
     dHat = inf0["dHat"]
-    ctx = context(m, m.nV_dof)
-    try:
+    with context(m, m.nV_dof) as ctx:
         ctx.set_kappa(1e4, 1.0, 1e9)
         ref = ok.CloseSet(1e4, 1e9)
         got = run_post(ctx, m, ref, m.V, dHat, dHat)
@@ -361,15 +325,12 @@ def test_post_line_search_plane_and_obstacle():
         V2 = m.V.copy()
         V2[: m.nV_dof, 2] -= 0.1 * np.sqrt(dHat)
         assert run_post(ctx, m, ref, V2, dHat, dHat).doublings == 1
-    finally:
-        ctx.close()
 
 
 def test_capture_contract():
     V, T = M.grid_tets(2, 2, 2)
     m = M.Mesh(V, T, energy=0)
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         ctx.set_kappa(1.0, 1.0, 2.0)
         ctx.capture_begin()
         ctx.set_kappa(2.0, 1.0, 2.0)
@@ -380,8 +341,6 @@ def test_capture_contract():
         ctx.graph_launch(gid)
         assert ctx.kappa_info().kappa == 2.0
         ctx.graph_destroy(gid)
-    finally:
-        ctx.close()
 
 
 # ---- 4. Newton iterations with kappa on the device ---------------------------------------------------------------------------------
@@ -431,8 +390,7 @@ def test_newton_driver_eager_graph_host():
     dTol = dHat
     s, mx = ok.bounds(dHat, 1e-11, float(np.mean(m.mass)), float(np.sum((m.V_rest.max(0) - m.V_rest.min(0)) ** 2)))
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
-    e, g, h = context(m), context(m), context(m)
-    try:
+    with context(m) as e, context(m) as g, context(m) as h:
         for c in (e, g, h):
             prepare(c, m, xt)
 
@@ -484,6 +442,3 @@ def test_newton_driver_eager_graph_host():
             assert rel(ag, ae) <= 1e-6 and rel(ah, ae) <= 1e-6, log
         assert sum(x[0] for x in log["e"]) >= 1, log  # the scene doubles at least once
         g.graph_destroy(gid)
-    finally:
-        for c in (e, g, h):
-            c.close()

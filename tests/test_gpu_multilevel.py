@@ -9,29 +9,24 @@ import scipy.sparse.linalg as spla
 
 import multilevel_mirror as mlm
 import oracle as orc
+from gpu_common import load_scene, own_context, rel, same_bits, shared_ctx, soa
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from ipc_b200 import scenes
-from stagecheck import contact_pattern_pairs, rel
+from stagecheck import contact_pattern_pairs
 
 pytestmark = pytest.mark.gpu
 DT2 = 0.025 ** 2
 
 
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def upload(ctx, m):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+def load_sorted(ctx, m):
+    load_scene(ctx, m)
     ctx.set_canonical_order(1)
 
 
 def assemble(ctx, m, dHat, kappa):
     """g and H on the device (elastic + mass + barrier) on the host-built contact pattern; returns the pattern and the sets"""
-    upload(ctx, m)
+    load_sorted(ctx, m)
     mm, pa, pe, _ = ctx.constraint_set(dHat, 1)
     ia, ja = m.csr_pattern(1, extra_pairs=contact_pattern_pairs(m, mm, pa, pe))
     ctx.set_csr(ia, ja, 1)
@@ -59,12 +54,8 @@ def states(ctx, m, info):
     return {"A": m.V.copy(), "B": m.V + 0.5 * a * p.reshape(-1, 3)}
 
 
-def same_bits(x, y):
-    return np.array_equal(np.asarray(x).view(np.uint64), np.asarray(y).view(np.uint64))
-
-
-def test_multilevel_pcg_on_the_device_resident_hessian(gpu_ctx):
-    ctx = gpu_ctx
+def test_multilevel_pcg_on_the_device_resident_hessian(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
     dHat, kappa = info["dHat"], 1e6
     ia, ja = assemble(ctx, m, dHat, kappa)
@@ -89,8 +80,8 @@ def test_multilevel_pcg_on_the_device_resident_hessian(gpu_ctx):
     assert iters <= ctx.solve_pcg(None, rel_tol=1e-10, max_iter=5000)[1]
 
 
-def test_hierarchy_application_and_iterations_equal_the_mirror(gpu_ctx):
-    ctx = gpu_ctx
+def test_hierarchy_application_and_iterations_equal_the_mirror(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
     ia, ja = assemble(ctx, m, info["dHat"], 1e6)
     n = 3 * m.nV
@@ -142,8 +133,8 @@ def launches_of_25_more_iterations(ctx, solve):
     return counts[1] - counts[0]
 
 
-def test_two_solves_give_identical_bits(gpu_ctx):
-    ctx = gpu_ctx
+def test_two_solves_give_identical_bits(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     assemble(ctx, m, info["dHat"], 1e8)
     x1, it1, res1 = ctx.solve_pcg_multilevel(None, rel_tol=1e-8, max_iter=5000)
@@ -156,8 +147,8 @@ def test_two_solves_give_identical_bits(gpu_ctx):
     assert launches_of_25_more_iterations(ctx, ctx.solve_pcg_multilevel) == 25 * (6 + len(ctx.multilevel_info()[0])) + 1
 
 
-def test_two_block_jacobi_solves_give_identical_bits(gpu_ctx):
-    ctx = gpu_ctx
+def test_two_block_jacobi_solves_give_identical_bits(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
     assemble(ctx, m, info["dHat"], 1e8)
     x1, it1, res1 = ctx.solve_pcg(None, rel_tol=1e-8, max_iter=5000)
@@ -168,11 +159,11 @@ def test_two_block_jacobi_solves_give_identical_bits(gpu_ctx):
     assert launches_of_25_more_iterations(ctx, ctx.solve_pcg) == 25 * 4 + 1
 
 
-def test_device_built_pattern_after_a_pattern_change(gpu_ctx):
-    ctx = gpu_ctx
+def test_device_built_pattern_after_a_pattern_change(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
     dHat, kappa = info["dHat"], 1e6
-    upload(ctx, m)
+    load_sorted(ctx, m)
     S = states(ctx, m, info)
     ctx.enable_device_pattern(1)
     for name in ("A", "B"):
@@ -195,15 +186,15 @@ def test_device_built_pattern_after_a_pattern_change(gpu_ctx):
     assert abs(mlm.pcg(H, -g, mlm.Multilevel(H, S["B"]).apply, 1e-10, 5000)[1] - iters) <= 2
 
 
-def test_obstacle_tail_and_dirichlet_vertices(gpu_ctx):
+def test_obstacle_tail_and_dirichlet_vertices(shared_ctx):
     from ipc_b200 import obstacle as OB
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info = scenes.balls_on_obstacle(plate_angle=0.0, res=4, plate=12)
     ob = info["obstacle"]
     M2 = OB.with_obstacle(m, ob["V"], ob["E"], ob["F"])
     M2.dbc = M2.dbc.copy()
     M2.dbc[:5] = 1  # Dirichlet vertices of the mesh besides the tail
-    upload(ctx, M2)
+    load_sorted(ctx, M2)
     ctx.set_obstacle_tail(M2.nV_dof, 1)
     try:
         ctx.enable_device_pattern(1)
@@ -249,8 +240,7 @@ def test_obstacle_tail_and_dirichlet_vertices(gpu_ctx):
 
 
 def test_nonpositive_pivot_is_an_error_and_not_a_hang():
-    ctx = L.Context(0)  # (a context of its own: the error must not leak into the shared one)
-    try:
+    with own_context() as ctx:  # (a context of its own: the error must not leak into the shared one)
         V, T = M.grid_tets(2, 2, 2)
         m = M.Mesh(V, T, energy=0)
         ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, 0)
@@ -266,23 +256,18 @@ def test_nonpositive_pivot_is_an_error_and_not_a_hang():
         ctx.elastic_grad_hess(DT2, 1, 1, 1, None, None)
         x, iters, res = ctx.solve_pcg_multilevel(np.ones(3 * m.nV), rel_tol=1e-10, max_iter=1000)
         assert res <= 1e-10 and np.isfinite(x).all()
-    finally:
-        ctx.close()
 
 
-def test_single_rank_contract_and_arguments(gpu_ctx):
-    ctx = L.Context(0)
-    try:
+def test_single_rank_contract_and_arguments(shared_ctx):
+    with own_context() as ctx:
         with pytest.raises(L.IpcGpuError, match="STATE"):
             ctx.solve_pcg_multilevel(None)  # no matrix yet
         with pytest.raises(L.IpcGpuError, match="STATE"):
             ctx.multilevel_info()
-    finally:
-        ctx.close()
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
-    assemble(gpu_ctx, m, info["dHat"], 1e6)
+    assemble(shared_ctx, m, info["dHat"], 1e6)
     with pytest.raises(L.IpcGpuError, match="ARG"):
-        gpu_ctx.solve_pcg_multilevel(None, rel_tol=0.0)
+        shared_ctx.solve_pcg_multilevel(None, rel_tol=0.0)
 
 
 def first_iteration_below(solve, tol):
@@ -295,8 +280,8 @@ def first_iteration_below(solve, tol):
     return x, hi
 
 
-def test_half_the_iterations_of_block_jacobi_on_ball_on_mat(gpu_ctx):
-    ctx = gpu_ctx
+def test_half_the_iterations_of_block_jacobi_on_ball_on_mat(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_on_mat()
     assemble(ctx, m, info["dHat"], 1e8)
     for tol in (1e-6, 1e-10):

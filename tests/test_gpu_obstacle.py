@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import load_scene, rel, scalar_bits, shared_ctx
 from ipc_b200 import lib as L
 from ipc_b200 import obstacle as OB
 from ipc_b200 import scenes
@@ -16,23 +17,13 @@ KAPPA = 1e8
 NTH = 8
 
 
-def bits(x):
-    return np.float64(x).view(np.uint64)
-
-
-def rel(a, b):
-    return np.linalg.norm(np.asarray(a) - np.asarray(b)) / max(np.linalg.norm(b), 1e-300)
-
-
 def lex(a):
     a = np.asarray(a)
     return a[np.lexsort(a.T[::-1])] if len(a) else a
 
 
-def upload(ctx, M2, ee_as_vf=1):
-    ctx.set_mesh(M2.V_rest_soa, M2.T_soa, M2.restTriInv, M2.vol, M2.mu, M2.lam, M2.mass, M2.dbc, M2.energy)
-    ctx.set_surface(M2.SVI, M2.SFEdges, M2.SF_soa, M2.vCoDim)
-    ctx.set_state(M2.V_soa)
+def load_with_obstacle(ctx, M2, ee_as_vf=1):
+    load_scene(ctx, M2)
     ctx.set_obstacle_tail(M2.nV_dof, ee_as_vf)
 
 
@@ -41,9 +32,9 @@ def remove_obstacle(ctx):
 
 
 @pytest.fixture
-def ctx(gpu_ctx):
-    yield gpu_ctx
-    remove_obstacle(gpu_ctx)
+def ctx(shared_ctx):
+    yield shared_ctx
+    remove_obstacle(shared_ctx)
 
 
 def build(angle, **kw):
@@ -58,7 +49,7 @@ def build(angle, **kw):
 def test_sets_energy_gradient_hessian(ctx, angle, res):
     m, info, ob, s, o, M2 = build(angle, res=res, plate=12 if res == 4 else 30)
     dHat = info["dHat"]
-    upload(ctx, M2)
+    load_with_obstacle(ctx, M2)
     mm, pa, pe, cand = ctx.constraint_set(dHat, 1)
     (smm, spa, spe), (cmm, cpa, cpe) = OB.split_sets(mm, pa, pe, m.nV, len(m.SFEdges))
     mm_s, pa_s, pe_s, cand_s = s.constraint_set(dHat, NTH)
@@ -104,7 +95,7 @@ def test_step_bounds_bit_exact(ctx, ee_as_vf, angle, res, plate):
     # (on the aligned plate an edge pair sets the partial bound: 0.2597 through the vertex-face routine, 0.2617 through the edge-edge one)
     m, info, ob, s, o, M2 = build(angle, res=res, plate=plate)
     dHat, p = info["dHat"], info["p"]
-    upload(ctx, M2, ee_as_vf)
+    load_with_obstacle(ctx, M2, ee_as_vf)
     p2 = OB.pad_direction(p, M2.nV)
     ctx.constraint_set(dHat, 1)
     _, _, _, cand_s = s.constraint_set(dHat, NTH)
@@ -113,23 +104,23 @@ def test_step_bounds_bit_exact(ctx, ee_as_vf, angle, res, plate):
     a = ctx.ccd_partial(p2, 1e-6, evf, eee, 1.0)
     a_self, _ = orc.ccd_partial(s, p, cand_s, 1e-6, evf, eee, 1.0, NTH)
     a_co, z = o.ccd_partial(p, cand_o, 1e-6, evf, eee, 1.0, ee_as_vf=ee_as_vf, nthreads=NTH)
-    assert not z and bits(a) == bits(min(a_self, a_co)), (a, a_self, a_co)
+    assert not z and scalar_bits(a) == scalar_bits(min(a_self, a_co)), (a, a_self, a_co)
     assert a_co < 1.0
     hvox = m.avgEdgeLen / 3.0
     ag = ctx.hash_build_swept(p2, a, hvox)
     a2, ncand = ctx.ccd_full(1e-6, evf, eee, ag)
     gs = orc.grid_swept(s, p, a, hvox)
-    assert bits(gs[1]) == bits(ag)  # the swept grid's own step only looks at the mesh's motion
+    assert scalar_bits(gs[1]) == scalar_bits(ag)  # the swept grid's own step only looks at the mesh's motion
     a2_self, _, _ = orc.ccd_full(s, p, gs[0], gs[1], 1e-6, evf, eee, gs[1], nthreads=NTH)
     a2_co, z, npairs = o.ccd_full(p, 1e-6, evf, eee, gs[1], ee_as_vf=ee_as_vf, nthreads=NTH)
-    assert not z and bits(a2) == bits(min(a2_self, a2_co)), (a2, a2_self, a2_co)
+    assert not z and scalar_bits(a2) == scalar_bits(min(a2_self, a2_co)), (a2, a2_self, a2_co)
     assert ctx.ccd_stats()[2] == 0 and ncand > 0
 
 
 def test_moving_the_obstacle_and_the_intersection_check(ctx):
     m, info, ob, s, o, M2 = build(0.37, res=4)
     dHat = info["dHat"]
-    upload(ctx, M2)
+    load_with_obstacle(ctx, M2)
     n0 = len(ctx.constraint_set(dHat, 0)[0])
     assert ctx.intersection_free()
     # far away: only the mesh's own pairs are left
@@ -149,18 +140,18 @@ def test_moving_the_obstacle_and_the_intersection_check(ctx):
     assert len(ctx.constraint_set(dHat, 0)[0]) == n0 and ctx.intersection_free()
 
 
-def test_tail_is_validated(gpu_ctx):
+def test_tail_is_validated(shared_ctx):
     m, info, ob, s, o, M2 = build(0.37, res=4)
     bad = OB.with_obstacle(m, ob["V"], ob["E"], ob["F"])
     bad.dbc = bad.dbc.copy()
     bad.dbc[-1] = 0
     with pytest.raises(L.IpcGpuError):
-        upload(gpu_ctx, bad)
-    remove_obstacle(gpu_ctx)
+        load_with_obstacle(shared_ctx, bad)
+    remove_obstacle(shared_ctx)
     with pytest.raises(L.IpcGpuError):  # a tetrahedron would use an obstacle vertex
-        gpu_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, np.ones(m.nV, dtype=np.uint8), m.energy)
-        gpu_ctx.set_obstacle_tail(m.nV - 1)
-    remove_obstacle(gpu_ctx)
+        shared_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, np.ones(m.nV, dtype=np.uint8), m.energy)
+        shared_ctx.set_obstacle_tail(m.nV - 1)
+    remove_obstacle(shared_ctx)
 
 
 @pytest.mark.skipif(not __import__("ipc_b200.msh", fromlist=["msh"]).have_asset("sphere1K"), reason="sphere1K mesh missing")
@@ -172,7 +163,7 @@ def test_c3_ball_over_the_mat_as_obstacle(ctx):
     o = orc.Obstacle(s, ob["V"], ob["E"], ob["F"])
     M2 = OB.with_obstacle(m, ob["V"], ob["E"], ob["F"])
     dHat, p = info["dHat"], info["p"]
-    upload(ctx, M2)
+    load_with_obstacle(ctx, M2)
     mm, pa, pe, cand = ctx.constraint_set(dHat, 1)
     (smm, spa, spe), (cmm, cpa, cpe) = OB.split_sets(mm, pa, pe, m.nV, len(m.SFEdges))
     mm_o, pa_o, pe_o, cand_o = o.constraint_set(dHat, NTH)
@@ -188,13 +179,13 @@ def test_c3_ball_over_the_mat_as_obstacle(ctx):
     p2 = OB.pad_direction(p, M2.nV)
     a = ctx.ccd_partial(p2, 1e-6, evf, eee, 1.0)
     a_co, z = o.ccd_partial(p, cand_o, 1e-6, evf, eee, 1.0, nthreads=NTH)
-    assert not z and a_co < 1.0 and bits(a) == bits(a_co)
+    assert not z and a_co < 1.0 and scalar_bits(a) == scalar_bits(a_co)
     # the full CCD from the untouched step: every swept mesh primitive against the mat
     hvox = m.avgEdgeLen / 3.0
     ag = ctx.hash_build_swept(p2, 1.0, hvox)
     a2, ncand = ctx.ccd_full(1e-6, evf, eee, ag)
     a2_co, z, npairs = o.ccd_full(p, 1e-6, evf, eee, ag, nthreads=NTH)
-    assert not z and npairs > 0 and ncand > 0 and bits(a2) == bits(a2_co), (a2, a2_co)
+    assert not z and npairs > 0 and ncand > 0 and scalar_bits(a2) == scalar_bits(a2_co), (a2, a2_co)
     assert ctx.ccd_stats()[2] == 0 and ctx.intersection_free()
 
 
@@ -206,7 +197,7 @@ def test_no_friction_against_the_obstacle(ctx):
     dHat = info["dHat"]
     rng = np.random.default_rng(3)
     Vt = m.V - 0.3 * np.sqrt(dHat) * rng.standard_normal(m.V.shape)
-    upload(ctx, M2)
+    load_with_obstacle(ctx, M2)
     ctx.set_prev_state(np.ascontiguousarray(np.concatenate([Vt, ob["V"]]).T).ravel())
     mm, _, _, _ = ctx.constraint_set(dHat, 0)
     n = ctx.friction_lag(dHat, KAPPA)
@@ -228,9 +219,9 @@ def test_no_friction_against_the_obstacle(ctx):
 def test_swept_grid_step_ignores_the_obstacle(ctx):
     """SpatialHash::build rescales the step by the mean |p| over mesh.SVI (SpatialHash.hpp:603-618): the obstacle's vertices must not dilute it"""
     m, info, ob, s, o, M2 = build(0.37, res=4)
-    upload(ctx, M2)
+    load_with_obstacle(ctx, M2)
     p = 40.0 * info["p"]
     hvox = m.avgEdgeLen / 3.0
     ag = ctx.hash_build_swept(OB.pad_direction(p, M2.nV), 1.0, hvox)
     g = orc.grid_swept(s, p, 1.0, hvox)
-    assert g[1] < 1.0 and bits(ag) == bits(g[1]), (ag, g[1])
+    assert g[1] < 1.0 and scalar_bits(ag) == scalar_bits(g[1]), (ag, g[1])

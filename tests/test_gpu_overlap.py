@@ -2,30 +2,24 @@
 scatter) runs on a low-priority stream next to the step-bound chain; with the stage timers on, both run one after the other on one stream.
 Either way the iteration gives a bit-identical elastic energy and step bounds, and gradient / CSR values that differ from a serial run by
 no more than two serial runs differ (the atomic sums of the barrier terms).  A call outside both chains waits for the derivative chain."""
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import load_scene, rel, scalar_bits, shared_ctx
 from ipc_b200 import lib as L
 from ipc_b200 import scenes
-from stagecheck import contact_pattern_pairs, rel
+from stagecheck import contact_pattern_pairs
 
 pytestmark = pytest.mark.gpu
 
 KAPPA, DT2, TOL = 1e8, 0.025 ** 2, 1e-6
 
 
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
-def load_scene(ctx):
+def pile_with_contacts(ctx):
     m, info = scenes.ball_pile(4, res=8, seed=5, height=4)
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
     mm, pa, pe, _ = ctx.constraint_set(info["dHat"], 1)
     ia, ja = m.csr_pattern(1, extra_pairs=contact_pattern_pairs(m, mm, pa, pe))
     ctx.set_csr(ia, ja, 1)
@@ -34,9 +28,9 @@ def load_scene(ctx):
     return m, info, ia, ja
 
 
-def test_concurrent_chains_equal_the_serial_order(gpu_ctx):
-    ctx = gpu_ctx
-    m, info, ia, ja = load_scene(ctx)
+def test_concurrent_chains_equal_the_serial_order(shared_ctx):
+    ctx = shared_ctx
+    m, info, ia, ja = pile_with_contacts(ctx)
     dHat, h = info["dHat"], m.avgEdgeLen / 3
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
 
@@ -96,7 +90,7 @@ def test_concurrent_chains_equal_the_serial_order(gpu_ctx):
     hg.free(); ha.free()
 
     def scalars(it):  # (the barrier energy sums the contact lists in the order the atomic appends left them: compared below)
-        return [bits(x) for x in (it.energy_elastic, it.alpha_inversion, it.alpha_partial_ccd, it.alpha_swept_grid, it.alpha_full_ccd, it.alpha)] + \
+        return [scalar_bits(x) for x in (it.energy_elastic, it.alpha_inversion, it.alpha_partial_ccd, it.alpha_swept_grid, it.alpha_full_ccd, it.alpha)] + \
             [it.n_active, it.n_mollified, it.n_candidates, it.n_full_ccd_candidates]
 
     g_noise, a_noise = rel(s2[1], s1[1]), rel(s2[2], s1[2])
@@ -106,14 +100,13 @@ def test_concurrent_chains_equal_the_serial_order(gpu_ctx):
         assert abs(it.energy_barrier - s1[0].energy_barrier) <= 1e-12 * abs(s1[0].energy_barrier)
         # (the floor: two serial runs can happen to add in the same order; 1e-14 is far below any ordering or race error)
         assert rel(g, s1[1]) <= max(g_noise, 1e-14) and rel(a, s1[2]) <= max(a_noise, 1e-14), (rel(g, s1[1]), g_noise, rel(a, s1[2]), a_noise)
-    ctx.set_canonical_order(1)
 
 
-def test_setter_after_the_derivative_chain_waits_for_it(gpu_ctx):
+def test_setter_after_the_derivative_chain_waits_for_it(shared_ctx):
     """ipcgpu_set_state right behind ipcgpu_elastic_energy_grad_hess (NULL outputs, no fetch in between) must not move the positions
     under the derivative chain still running on its own stream: E / g / H are those of the old positions, the next call sees the new ones"""
-    ctx = gpu_ctx
-    m, info, ia, ja = load_scene(ctx)
+    ctx = shared_ctx
+    m, info, ia, ja = pile_with_contacts(ctx)
     V2 = m.V * 1.01
     diag = np.asarray(ia[:-1], dtype=np.int64)[: 3 * m.nV] - 1
 
@@ -131,4 +124,3 @@ def test_setter_after_the_derivative_chain_waits_for_it(gpu_ctx):
         assert abs(it.energy_elastic - E_r) <= 1e-10 * abs(E_r) and rel(g, g_r) <= 1e-10 and rel(a, a_r) <= 1e-9, \
             (it.energy_elastic, E_r, rel(g, g_r), rel(a, a_r))
     ctx.set_state(m.V_soa)
-    ctx.set_canonical_order(1)

@@ -9,6 +9,7 @@ import oracle_codim as oc
 import oracle_halfspace as OH
 import oracle_jacobi as OJ
 import oracle_timestep as OT
+from gpu_common import load_scene, own_context, same_bits, scalar_bits, shared_ctx, soa
 from ipc_b200 import lib as L
 from ipc_b200 import scenes
 
@@ -18,19 +19,6 @@ TOL = 1e-6
 KAPPA = 1e6
 EPS2 = 1e-6
 FRIC = 0.3
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def bits(x):
-    return np.asarray(x, dtype=np.float64).view(np.uint64)
-
-
-def same_bits(x, y):
-    x, y = np.asarray(x, dtype=np.float64), np.asarray(y, dtype=np.float64)
-    return x.shape == y.shape and np.array_equal(bits(x), bits(y))
 
 
 def mat_scene():
@@ -63,19 +51,10 @@ def codim_scene():
 SCENES = {"ball_on_mat_planes": mat_scene, "codim_pin_cushion": codim_scene}
 
 
-@pytest.fixture(autouse=True)
-def restore_shared_context(gpu_ctx):
-    yield
-    gpu_ctx.set_halfspaces([], [])
-    gpu_ctx.set_canonical_order(1)
-
-
 def start(ctx, m, info, planes, Vprev, level=1):
     """scene, contact sets at V, the lagged friction, the device-built pattern (index base 1)"""
     dHat = info["dHat"]
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(soa(m.V))
+    load_scene(ctx, m)
     ctx.set_prev_state(soa(Vprev))
     ctx.set_halfspaces(planes["origin"], planes["normal"], friction=planes["friction"]) if planes is not None else ctx.set_halfspaces([], [])
     ctx.set_canonical_order(level)
@@ -115,8 +94,8 @@ def resident(ctx, m, pattern):
 @pytest.mark.parametrize("projectDBC", [1, 0])
 @pytest.mark.parametrize("pattern", ["device", "host"])
 @pytest.mark.parametrize("name", list(SCENES))
-def test_direction_bit_identical(gpu_ctx, name, pattern, projectDBC):
-    ctx = gpu_ctx
+def test_direction_bit_identical(shared_ctx, name, pattern, projectDBC):
+    ctx = shared_ctx
     m, info, planes, Vprev = SCENES[name]()
     start(ctx, m, info, planes, Vprev)
     ia, ja = ctx.get_pattern()
@@ -159,8 +138,8 @@ def stages(ctx, m, info, evf, eee):
     return out
 
 
-def test_adopted_equals_uploaded(gpu_ctx):
-    ctx = gpu_ctx
+def test_adopted_equals_uploaded(shared_ctx):
+    ctx = shared_ctx
     m, info, planes, Vprev = mat_scene()
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     runs = []
@@ -179,8 +158,8 @@ def test_adopted_equals_uploaded(gpu_ctx):
 
 
 # ---- 3. warm start option 5 against the oracle driver ------------------------------------------------------------------------------
-def test_warm_start_jacobi_matches_oracle(gpu_ctx):
-    ctx = gpu_ctx
+def test_warm_start_jacobi_matches_oracle(shared_ctx):
+    ctx = shared_ctx
     m, info, planes, Vprev = mat_scene()
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     voxel = m.avgEdgeLen / 3.0
@@ -220,8 +199,8 @@ def frame(ctx, info, planes, evf, eee, voxel):
     ctx.warm_start(5, voxel, TOL, evf, eee, want=False)
 
 
-def test_captured_equals_eager(gpu_ctx):
-    ctx = gpu_ctx
+def test_captured_equals_eager(shared_ctx):
+    ctx = shared_ctx
     m, info, planes, Vprev = mat_scene()
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     voxel, n = m.avgEdgeLen / 3.0, 3 * m.nV
@@ -239,8 +218,8 @@ def test_captured_equals_eager(gpu_ctx):
     def snapshot():
         s, v = ctx.step_control_info(), ctx.solve_info()
         it = ctx.fetch_iteration()
-        return (ctx.download(L.BUF_POSITIONS, n).tobytes(), ctx.download(L.BUF_SEARCH_DIR, n).tobytes(), bits(s.alpha).tobytes(),
-                bits(v.max_abs_x).tobytes(), s.halvings_inversion, s.halvings_intersection, s.halvings_armijo, s.halvings_post_check,
+        return (ctx.download(L.BUF_POSITIONS, n).tobytes(), ctx.download(L.BUF_SEARCH_DIR, n).tobytes(), scalar_bits(s.alpha),
+                scalar_bits(v.max_abs_x), s.halvings_inversion, s.halvings_intersection, s.halvings_armijo, s.halvings_post_check,
                 s.status, v.status, it.status)
 
     start(ctx, m, info, planes, Vprev, level=2)
@@ -263,8 +242,7 @@ def test_captured_equals_eager(gpu_ctx):
 
 # ---- 5. refusals and the non-finite status ------------------------------------------------------------------------------------------
 def test_refusals_and_non_finite():
-    ctx = L.Context(0)
-    try:
+    with own_context() as ctx:
         m, info, planes, Vprev = mat_scene()
         evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
         voxel = m.avgEdgeLen / 3.0
@@ -298,6 +276,4 @@ def test_refusals_and_non_finite():
         assert s.status == L.ERR_SOLVE and np.isinf(s.max_abs_x)
         with pytest.raises(L.IpcGpuError, match="SOLVE"):
             ctx.precondition_diag(-1)
-    finally:
-        ctx.close()
 

@@ -7,9 +7,10 @@ import pytest
 import oracle as orc
 import oracle_codim as oc
 import oracle_kappa as ok
+from gpu_common import load_scene, own_context, rel, same_bits, scalar_bits, shared_ctx, soa
 from ipc_b200 import lib as L
 from ipc_b200 import scenes
-from stagecheck import rel, sort_rows
+from stagecheck import sort_rows
 
 pytestmark = pytest.mark.gpu
 DT2 = 0.025 ** 2
@@ -17,18 +18,6 @@ TOL = 1e-6
 KAPPA = 1e6
 EPS2 = 1e-6
 FRIC = 0.3
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def bits(x):
-    return np.asarray(x, dtype=np.float64).view(np.uint64)
-
-
-def same_bits(x, y):
-    return np.array_equal(bits(x), bits(y))
 
 
 def mat_scene():
@@ -66,21 +55,13 @@ def codim_scene():
 SCENES = {"ball_on_mat_planes": mat_scene, "ball_pile": pile_scene, "codim_pin_cushion": codim_scene}
 
 
-@pytest.fixture(autouse=True)
-def restore_shared_context(gpu_ctx):
-    """the session context goes back to no planes and the default order for the modules that follow"""
-    yield
-    gpu_ctx.set_halfspaces([], [])
-    gpu_ctx.set_canonical_order(1)
-
-
-def upload(ctx, m, planes, Vprev, level):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(soa(m.V))
+def load_at_level(ctx, m, planes, Vprev, level):
+    load_scene(ctx, m)
     ctx.set_prev_state(soa(Vprev))
     if planes is not None:
         ctx.set_halfspaces(planes["origin"], planes["normal"], friction=planes["friction"])
+    else:  # (plane definitions outlive set_mesh)
+        ctx.set_halfspaces([], [])
     ctx.set_canonical_order(level)
 
 
@@ -112,10 +93,10 @@ def build_sets(ctx, info, planes):
 
 # ---- 1. order independence ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", list(SCENES))
-def test_order_independence(gpu_ctx, name):
-    ctx = gpu_ctx
+def test_order_independence(shared_ctx, name):
+    ctx = shared_ctx
     m, info, planes, Vprev = SCENES[name]()
-    upload(ctx, m, planes, Vprev, 2)
+    load_at_level(ctx, m, planes, Vprev, 2)
     ctx.enable_device_pattern(1)
     mm, pa, pe, _ = build_sets(ctx, info, planes)
     fr = ctx.get_friction_data()
@@ -133,17 +114,16 @@ def test_order_independence(gpu_ctx, name):
         assert same_bits(E, ref[0]) and same_bits(g, ref[1]) and same_bits(a, ref[2]), (name, trial)
         fr2 = ctx.get_friction_data()
         assert all(np.array_equal(x, y) for x, y in zip(fr2, fr))  # the uploaded list comes back in canonical order
-    ctx.set_canonical_order(1)
 
 
 # ---- 2. parity with level 0 ---------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", list(SCENES))
-def test_level2_matches_level0(gpu_ctx, name):
-    ctx = gpu_ctx
+def test_level2_matches_level0(shared_ctx, name):
+    ctx = shared_ctx
     m, info, planes, Vprev = SCENES[name]()
     out = {}
     for level in (0, 2, 1):
-        upload(ctx, m, planes, Vprev, level)
+        load_at_level(ctx, m, planes, Vprev, level)
         ctx.enable_device_pattern(1)
         mm, pa, pe, _ = build_sets(ctx, info, planes)
         ia, ja = ctx.get_pattern()
@@ -158,7 +138,6 @@ def test_level2_matches_level0(gpu_ctx, name):
     E2, g2, a2 = s2[5:]
     assert np.all(np.abs(E2 - E0) <= 1e-10 * np.maximum(np.abs(E0), 1e-300))
     assert rel(g2, g0) <= 1e-10 and rel(a2, a0) <= 1e-9
-    ctx.set_canonical_order(1)
 
 
 # ---- 3. captured equals eager, 4. two contexts, one trajectory -----------------------------------------------------------------------
@@ -196,7 +175,7 @@ def snapshot(ctx, m):
 
 
 def start(ctx, m, info, planes, Vprev):
-    upload(ctx, m, planes, Vprev, 2)
+    load_at_level(ctx, m, planes, Vprev, 2)
     ctx.enable_device_pattern(1)
     ctx.constraint_set(info["dHat"], 1, fetch=False, sizes=False)
     ctx.friction_lag(info["dHat"], KAPPA, want=False)
@@ -204,11 +183,11 @@ def start(ctx, m, info, planes, Vprev):
     ctx.halfspace_friction_lag(info["dHat"], KAPPA, want=False)
 
 
-def test_captured_iteration_equals_eager(gpu_ctx):
+def test_captured_iteration_equals_eager(shared_ctx):
     m, info, planes, Vprev = mat_scene()
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
-    g_ctx, e_ctx = gpu_ctx, L.Context(0)
-    try:
+    g_ctx = shared_ctx
+    with own_context() as e_ctx:
         for c in (g_ctx, e_ctx):
             start(c, m, info, planes, Vprev)
         newton_iteration(g_ctx, m, info, evf, eee)  # the eager run: lazy allocations
@@ -227,9 +206,6 @@ def test_captured_iteration_equals_eager(gpu_ctx):
                 assert same_bits(g[key], e[key]), (k, key)
             assert g["counts"] == e["counts"], k
         g_ctx.graph_destroy(gid)
-    finally:
-        e_ctx.close()
-        g_ctx.set_canonical_order(1)
 
 
 def test_two_contexts_one_trajectory():
@@ -237,8 +213,7 @@ def test_two_contexts_one_trajectory():
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     runs = []
     for _ in range(2):
-        ctx = L.Context(0)
-        try:
+        with own_context() as ctx:
             start(ctx, m, info, planes, Vprev)
             newton_iteration(ctx, m, info, evf, eee)  # eager first (lazy allocations), then replays from the same start
             ctx.fetch_iteration()
@@ -252,8 +227,6 @@ def test_two_contexts_one_trajectory():
                 traj.append(snapshot(ctx, m))
             ctx.graph_destroy(gid)
             runs.append(traj)
-        finally:
-            ctx.close()
     for k, (x, y) in enumerate(zip(*runs)):
         for key in ("V", "g", "a", "scalars"):
             assert same_bits(x[key], y[key]), (k, key)
@@ -261,8 +234,8 @@ def test_two_contexts_one_trajectory():
 
 
 # ---- 5. contract ---------------------------------------------------------------------------------------------------------------------
-def test_contract(gpu_ctx):
-    ctx = gpu_ctx
+def test_contract(shared_ctx):
+    ctx = shared_ctx
     m, info, planes, Vprev = mat_scene()
     with pytest.raises(L.IpcGpuError):
         ctx.set_canonical_order(3)
@@ -275,13 +248,10 @@ def test_contract(gpu_ctx):
     with pytest.raises(L.IpcGpuError):
         ctx.graph_launch(gid)
     ctx.graph_destroy(gid)
-    other = L.Context(0)  # level 2 and several ranks: refused (before any collective is set up)
-    try:
+    with own_context() as other:  # level 2 and several ranks: refused (before any collective is set up)
         other.set_canonical_order(2)
         with pytest.raises(L.IpcGpuError, match="STATE"):
             other.comm_init(0, 2, bytes(128))
-    finally:
-        other.close()
 
 
 def held_lists(ctx):
@@ -292,13 +262,13 @@ def held_lists(ctx):
     return mm, pa, pe, cand
 
 
-def test_level1_inside_a_capture(gpu_ctx):
+def test_level1_inside_a_capture(shared_ctx):
     """level 1 sorts sized on the device: a captured constraint set and line search replay to the eager calls' lists, which are the
     oracle's at the accepted step"""
-    ctx = gpu_ctx
+    ctx = shared_ctx
     m, info, _, Vprev = pile_scene()
     dHat = info["dHat"]
-    upload(ctx, m, None, Vprev, 1)
+    load_at_level(ctx, m, None, Vprev, 1)
     g = ctx.elastic_gradient(DT2) + ctx.barrier_gradient(dHat, KAPPA, np.zeros(3 * m.nV))
     p = -g / np.abs(g).max() * 0.5 * np.sqrt(dHat)  # a descent direction, at most half a contact distance per coordinate
     ctx.set_search_dir(p)
@@ -385,15 +355,14 @@ def test_five_time_steps_two_contexts():
     s, mx = ok.bounds(info["dHat"], 1e-11, float(np.mean(m.mass)), float(np.sum((m.V_rest.max(0) - m.V_rest.min(0)) ** 2)))
     runs = []
     for _ in range(2):
-        ctx = L.Context(0)  # a fresh context per run
-        try:
+        with own_context() as ctx:  # a fresh context per run
             def reset():  # (nothing here refuses the graphs)
                 ctx.set_state(soa(m.V))
                 ctx.set_prev_state(soa(m.V))
                 ctx.set_dynamics(vel0.ravel(), None, None)
                 ctx.compute_xtilde()
 
-            upload(ctx, m, planes, m.V, 2)
+            load_at_level(ctx, m, planes, m.V, 2)
             ctx.enable_device_pattern(1)
             ctx.set_time_integration(0, 0.025, gravity=(0.0, 0.0, -9.81))
             reset()
@@ -419,15 +388,13 @@ def test_five_time_steps_two_contexts():
                     ctx.graph_launch(gid_it)
                     sc, sv, it = ctx.step_control_info(), ctx.solve_info(), ctx.fetch_iteration()
                     counts.append((sc.status, sv.status, it.status, sv.iterations, *(getattr(sc, f) for f, _ in sc._fields_ if f.startswith("halvings")),
-                                   bits(sc.alpha).item(), ctx.kappa_info().doublings))
+                                   scalar_bits(sc.alpha), ctx.kappa_info().doublings))
                 # (the mollified pairs' term alone, host form: augmentParaEEGradient with the device kappa)
                 gp = ctx.para_ee_gradient(info["dHat"], KD, np.zeros(3 * m.nV))
-                traj.append(dict(V=ctx.download(L.BUF_POSITIONS, 3 * m.nV), gp=gp, kappa=bits(ctx.kappa_info().kappa).item(), counts=counts))
+                traj.append(dict(V=ctx.download(L.BUF_POSITIONS, 3 * m.nV), gp=gp, kappa=scalar_bits(ctx.kappa_info().kappa), counts=counts))
             ctx.graph_destroy(gid_step)
             ctx.graph_destroy(gid_it)
             runs.append(traj)
-        finally:
-            ctx.close()
     a, b = runs
     for k in range(N_STEPS):
         assert same_bits(a[k]["V"], b[k]["V"]) and same_bits(a[k]["gp"], b[k]["gp"]), k

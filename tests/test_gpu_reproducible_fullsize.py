@@ -7,6 +7,7 @@ import sys
 import numpy as np
 import pytest
 
+from gpu_common import load_scene, own_context
 from ipc_b200 import lib as L
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -28,12 +29,9 @@ def test_c5_two_contexts_same_bits():
     xt[:, 2] -= 9.81 * DT2
     out = []
     for _ in range(2):
-        ctx = L.Context(0)
-        try:
-            ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-            ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
+        with own_context() as ctx:
+            load_scene(ctx, m)
             ctx.set_canonical_order(2)
-            ctx.set_state(m.V_soa)
             ctx.enable_device_pattern(1)
             ctx.set_xtilde(np.ascontiguousarray(xt.T).ravel())
             nC, nP, _ = ctx.constraint_set(dHat, 1, fetch=False)
@@ -45,8 +43,6 @@ def test_c5_two_contexts_same_bits():
             x, iters, res = ctx.solve_pcg_multilevel(None, 1e-6, 10000)
             _, ja = ctx.get_pattern()
             out.append(dict(nC=nC, nP=nP, g=ctx.download(L.BUF_GRADIENT, n), a=ctx.download(L.BUF_CSR_VALUES, len(ja)), x=x, iters=iters, res=res))
-        finally:
-            ctx.close()
     a, b = out
     assert a["nC"] > 5000 and (a["nC"], a["nP"]) == (b["nC"], b["nP"])
     assert a["res"] <= 1e-6 and a["iters"] == b["iters"], (a["iters"], b["iters"])

@@ -4,16 +4,11 @@ import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import load_scene, shared_ctx
 from ipc_b200 import mesh as M
 from ipc_b200 import scenes
 
 pytestmark = pytest.mark.gpu
-
-
-def upload(ctx, m):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
 
 
 def two_cubes(dz, n=3):
@@ -23,37 +18,37 @@ def two_cubes(dz, n=3):
 
 
 @pytest.mark.parametrize("dz,free", [(1.05, True), (0.8, False), (0.999, False)])
-def test_intersection_check_matches_oracle(gpu_ctx, dz, free):
+def test_intersection_check_matches_oracle(shared_ctx, dz, free):
     m = two_cubes(dz)
     rng = np.random.default_rng(3)
     m.V = m.V_rest + 0.01 * rng.standard_normal(m.V_rest.shape)
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     ok_ref, hits_ref = orc.Surf(m).intersection_free(nthreads=4)
     assert ok_ref == free
-    assert gpu_ctx.intersection_free() == ok_ref
-    gpu_ctx.intersection_free(want=False)  # deferred form: the count comes back with the iteration
-    gpu_ctx.check_inversion(want=False)
-    it = gpu_ctx.fetch_iteration()
+    assert shared_ctx.intersection_free() == ok_ref
+    shared_ctx.intersection_free(want=False)  # deferred form: the count comes back with the iteration
+    shared_ctx.check_inversion(want=False)
+    it = shared_ctx.fetch_iteration()
     assert it.n_intersected_triangles == hits_ref and it.n_inverted_tets == orc.Elastic(m).count_inverted()
     # all-Dirichlet pairs are skipped (:3282)
     m.dbc[:] = 1
-    upload(gpu_ctx, m)
-    assert gpu_ctx.intersection_free() is True
+    load_scene(shared_ctx, m)
+    assert shared_ctx.intersection_free() is True
     m.dbc[:] = 0
 
 
-def test_inversion_count_matches_oracle(gpu_ctx):
+def test_inversion_count_matches_oracle(shared_ctx):
     m = scenes.twisted_mat(nx=10, ny=10, nz=8, energy=1, invert_frac=0.02)  # FCR scene with flipped tets
-    upload(gpu_ctx, m)
+    load_scene(shared_ctx, m)
     n_ref = orc.Elastic(m).count_inverted()
-    assert n_ref > 0 and gpu_ctx.check_inversion() == n_ref
+    assert n_ref > 0 and shared_ctx.check_inversion() == n_ref
     m.V = m.V_rest.copy()
-    upload(gpu_ctx, m)
-    assert gpu_ctx.check_inversion() == 0
+    load_scene(shared_ctx, m)
+    assert shared_ctx.check_inversion() == 0
 
 
 def check_intersection_counts(ctx, m):
-    upload(ctx, m)
+    load_scene(ctx, m)
     ok_ref, hits_ref = orc.Surf(m).intersection_free(nthreads=64)
     ctx.intersection_free(want=False)
     ctx.check_inversion(want=False)
@@ -62,18 +57,18 @@ def check_intersection_counts(ctx, m):
     assert it.n_inverted_tets == 0
 
 
-def test_c5_pile_intersection_counts(gpu_ctx):
+def test_c5_pile_intersection_counts(shared_ctx):
     """C5 (1M tets) is intersection free: the device must agree with the oracle at the full size."""
     import bench
 
     class A:
         tets, res, scene = 1_000_000, 10, "c5"
 
-    check_intersection_counts(gpu_ctx, bench.build_scene(A)[0])
+    check_intersection_counts(shared_ctx, bench.build_scene(A)[0])
 
 
 @pytest.mark.skipif(not scenes.have_squeeze_out_bodies(), reason=scenes.SQUEEZE_OUT_MISSING)
-def test_full_size_scenes_intersection_counts(gpu_ctx):
+def test_full_size_scenes_intersection_counts(shared_ctx):
     """C4's manufactured shell crosses its core in places (scenes.squeeze_out_tiled): the device must find exactly the triangles the
     oracle finds, degenerate near-coplanar configurations included.  (C5 is test_c5_pile_intersection_counts.)"""
-    check_intersection_counts(gpu_ctx, scenes.squeeze_out_tiled()[0])
+    check_intersection_counts(shared_ctx, scenes.squeeze_out_tiled()[0])

@@ -6,9 +6,9 @@ import scipy.sparse as sp
 import scipy.sparse.linalg as spla
 
 import oracle as orc
-from ipc_b200 import lib as L
+from gpu_common import load_scene, rel, shared_ctx
 from ipc_b200 import scenes
-from stagecheck import contact_pattern_pairs, rel
+from stagecheck import contact_pattern_pairs
 
 pytestmark = pytest.mark.gpu
 
@@ -18,13 +18,11 @@ def full_matrix(ia, ja, a, n):
     return (U + sp.triu(U, 1).T).tocsc()
 
 
-def test_pcg_on_the_device_resident_hessian(gpu_ctx):
-    ctx = gpu_ctx
+def test_pcg_on_the_device_resident_hessian(shared_ctx):
+    ctx = shared_ctx
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
     dHat, p, kappa, dt2 = info["dHat"], info["p"], 1e6, 0.025 ** 2
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+    load_scene(ctx, m)
     mm, pa, pe, cand = ctx.constraint_set(dHat, 1)
     ia, ja = m.csr_pattern(1, extra_pairs=contact_pattern_pairs(m, mm, pa, pe))
     ctx.set_csr(ia, ja, 1)

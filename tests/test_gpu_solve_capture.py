@@ -2,42 +2,33 @@
 a captured solve replays to the bits and the iteration count of a synchronous one, the full-row structure follows a
 pattern change at replay with nothing on the host, a whole Newton iteration with the solve is one graph, a failed solve is reported by
 ipcgpu_fetch_iteration / ipcgpu_solve_info and leaves V = V0, and the capture contract (deferred form only, an eager run first) holds."""
+import contextlib
+
 import numpy as np
 import pytest
 import scipy.sparse.linalg as spla
 
 import multilevel_mirror as mlm
+from gpu_common import load_scene, own_context, rel, same_bits, shared_ctx, soa
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 from ipc_b200 import scenes
-from stagecheck import rel
 
 pytestmark = pytest.mark.gpu
 DT2 = 0.025 ** 2
 TOL = 1e-6
 
 
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
-def same_bits(x, y):
-    return np.array_equal(np.asarray(x, dtype=np.float64).view(np.uint64), np.asarray(y, dtype=np.float64).view(np.uint64))
-
-
-def upload(ctx, m):
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
+def load_unsorted(ctx, m):
+    load_scene(ctx, m)
     ctx.set_canonical_order(0)  # (inside a capture the contact lists stay in build order)
 
 
 def pile():
     """ball_pile and two states: A (the scene) and B (half of the feasible step along the scene's direction: more contacts, another pattern)"""
     m, info = scenes.ball_pile(4, res=6, seed=5, height=4)
-    ctx = L.Context(0)
-    try:
-        upload(ctx, m)
+    with own_context() as ctx:
+        load_unsorted(ctx, m)
         p = info["p"]
         evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
         ctx.constraint_set(info["dHat"], 1, fetch=False)
@@ -45,8 +36,6 @@ def pile():
         a = ctx.ccd_partial(None, 1e-6, evf, eee, a)
         a = ctx.hash_build_swept(None, a, m.avgEdgeLen / 3)
         a, _ = ctx.ccd_full(1e-6, evf, eee, a)
-    finally:
-        ctx.close()
     return m, info, {"A": m.V.copy(), "B": m.V + 0.5 * a * p.reshape(-1, 3)}
 
 
@@ -73,12 +62,12 @@ def scene():
 
 # ---- 1, 2. a graph that holds the solve alone ---------------------------------------------------------------------------------------
 @pytest.mark.parametrize("multilevel", [True, False], ids=["multilevel", "block_jacobi"])
-def test_solve_only_graph(gpu_ctx, scene, multilevel):
-    ctx = gpu_ctx
+def test_solve_only_graph(shared_ctx, scene, multilevel):
+    ctx = shared_ctx
     m, info, S = scene
     dHat, kappa, n, tol = info["dHat"], 1e6, 3 * m.nV, 1e-10
     solve = ctx.solve_pcg_multilevel if multilevel else ctx.solve_pcg
-    upload(ctx, m)
+    load_unsorted(ctx, m)
     ctx.enable_device_pattern(1)
     assemble_at(ctx, S["A"], dHat, kappa)
     solve(None, rel_tol=tol, max_iter=5000, want_x=False, adopt=True)  # the eager run: lazy allocations
@@ -95,12 +84,11 @@ def test_solve_only_graph(gpu_ctx, scene, multilevel):
         assert r.max_abs_x == np.abs(p).max()
         assert same_bits(p, x) and r.iterations == iters and same_bits(r.rel_residual, res)
     ctx.graph_destroy(gid)
-    ctx.set_canonical_order(1)
 
 
 # ---- 3. the pattern changes between replays ------------------------------------------------------------------------------------------
-def test_pattern_change_between_replays(gpu_ctx, scene):
-    ctx = gpu_ctx
+def test_pattern_change_between_replays(shared_ctx, scene):
+    ctx = shared_ctx
     m, info, S = scene
     dHat, kappa, n, tol = info["dHat"], 1e6, 3 * m.nV, 1e-10
 
@@ -108,7 +96,7 @@ def test_pattern_change_between_replays(gpu_ctx, scene):
         assemble_at(ctx, V, dHat, kappa)
         ctx.solve_pcg_multilevel(rel_tol=tol, max_iter=5000, want_x=False, adopt=True, deferred=True)
 
-    upload(ctx, m)
+    load_unsorted(ctx, m)
     ctx.enable_device_pattern(1)
     sequence(S["A"])
     assert ctx.solve_info().status == 0 and ctx.fetch_iteration().status == 0
@@ -143,7 +131,6 @@ def test_pattern_change_between_replays(gpu_ctx, scene):
     x2, iters2, _ = ctx.solve_pcg_multilevel(None, rel_tol=tol, max_iter=5000)
     assert same_bits(p2, x2) and r2.iterations == iters2 and rel(p2, p) <= 1e-9
     ctx.graph_destroy(gid)
-    ctx.set_canonical_order(1)
 
 
 # ---- 4. a whole Newton iteration in one graph ----------------------------------------------------------------------------------------
@@ -163,14 +150,14 @@ def newton_iteration(ctx, m, dHat, kappa, evf, eee):
     ctx.line_search(DT2, dHat, kappa)
 
 
-def test_whole_newton_iteration_graph(gpu_ctx, scene):
+def test_whole_newton_iteration_graph(shared_ctx, scene):
     m, info, _ = scene
     dHat, kappa, n = info["dHat"], 1e6, 3 * m.nV
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
-    g_ctx, e_ctx = gpu_ctx, L.Context(0)
-    try:
+    g_ctx = shared_ctx
+    with own_context() as e_ctx:
         for c in (g_ctx, e_ctx):
-            upload(c, m)
+            load_unsorted(c, m)
             c.enable_device_pattern(1)
         newton_iteration(g_ctx, m, dHat, kappa, evf, eee)  # the eager run: lazy allocations
         g_ctx.fetch_iteration()
@@ -192,27 +179,24 @@ def test_whole_newton_iteration_graph(gpu_ctx, scene):
             Vg, Ve = g_ctx.download(L.BUF_POSITIONS, n), e_ctx.download(L.BUF_POSITIONS, n)
             assert rel(Vg, Ve) <= 1e-9 and not np.array_equal(Vg, soa(m.V))
         g_ctx.graph_destroy(gid)
-    finally:
-        e_ctx.close()
-        g_ctx.set_canonical_order(1)
 
 
 # ---- 5. a failed solve -------------------------------------------------------------------------------------------------------------
+@contextlib.contextmanager
 def small_context():
-    ctx = L.Context(0)  # (a context of its own: the error must not leak into the shared one)
-    V, T = M.grid_tets(2, 2, 2)
-    m = M.Mesh(V, T, energy=0)
-    upload(ctx, m)
-    ia, ja = m.csr_pattern(1)
-    ctx.set_csr(ia, ja, 1)
-    ctx.set_state(soa(m.V * 1.05))  # stretched: a nonzero elastic gradient, no inverted tet
-    return ctx, m, len(ja)
+    with own_context() as ctx:  # (a context of its own: the error must not leak into the shared one)
+        V, T = M.grid_tets(2, 2, 2)
+        m = M.Mesh(V, T, energy=0)
+        load_unsorted(ctx, m)
+        ia, ja = m.csr_pattern(1)
+        ctx.set_csr(ia, ja, 1)
+        ctx.set_state(soa(m.V * 1.05))  # stretched: a nonzero elastic gradient, no inverted tet
+        yield ctx, m, len(ja)
 
 
 @pytest.mark.parametrize("multilevel", [True, False], ids=["multilevel_pivot", "block_jacobi_nan"])
 def test_failed_deferred_solve(multilevel):
-    ctx, m, nnz = small_context()
-    try:
+    with small_context() as (ctx, m, nnz):
         n, dHat = 3 * m.nV, 1e-8
         solve = ctx.solve_pcg_multilevel if multilevel else ctx.solve_pcg
 
@@ -252,14 +236,11 @@ def test_failed_deferred_solve(multilevel):
         x, iters, res = solve(np.ones(n), rel_tol=1e-10, max_iter=1000)
         assert res <= 1e-10 and np.isfinite(x).all()
         ctx.graph_destroy(gid)
-    finally:
-        ctx.close()
 
 
 # ---- 6. the capture contract -------------------------------------------------------------------------------------------------------
 def test_capture_contract():
-    ctx, m, _ = small_context()
-    try:
+    with small_context() as (ctx, m, _):
         n = 3 * m.nV
         ctx.elastic_grad_hess(DT2, 1, 1, 1, None, None)
         for solve in (ctx.solve_pcg, ctx.solve_pcg_multilevel):  # a capture before any eager run
@@ -287,5 +268,3 @@ def test_capture_contract():
             ctx.graph_destroy(gid)
         with pytest.raises(ValueError):
             ctx.solve_pcg(np.ones(n), deferred=True)
-    finally:
-        ctx.close()

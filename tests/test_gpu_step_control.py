@@ -1,12 +1,12 @@
 """The CFL branch of the step bound (ipcgpu_ccd_cfl_ti) and the line search (ipcgpu_line_search) against oracle drivers restated from
 Optimizer.cpp:1947-2027 and Optimizer::lineSearch (Optimizer.cpp:2662-2916, armijoParam = 0, lowerBound = 0), eagerly and replayed from a
 graph with conditional nodes."""
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import load_scene, own_context, rel, scalar_bits, soa
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 
@@ -14,14 +14,6 @@ pytestmark = pytest.mark.gpu
 
 TOL = 1e-6
 MARGIN = 1e-9  # every energy comparison of the oracle driver must be decided by more than this (relative)
-
-
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
 
 
 # ---- scenes -------------------------------------------------------------------------------------------------------------------
@@ -184,12 +176,9 @@ def oracle_cfl(sc, first, alpha_partial, evf, eee, voxel):
 
 
 # ---- device side --------------------------------------------------------------------------------------------------------------
-def upload(ctx, sc, canonical=1):
-    m = sc.m
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
+def load_step_scene(ctx, sc, canonical=1):
+    load_scene(ctx, sc.m)
     ctx.set_canonical_order(canonical)
-    ctx.set_state(m.V_soa)
     ctx.set_search_dir(sc.p)
     if sc.xtilde is not None:
         ctx.set_xtilde(soa(sc.xtilde))
@@ -201,9 +190,8 @@ def upload(ctx, sc, canonical=1):
 
 @pytest.fixture(scope="module")
 def ctx():
-    c = L.Context(0)
-    yield c
-    c.close()
+    with own_context() as c:
+        yield c
 
 
 def fingerprint(ctx, sc):
@@ -213,7 +201,7 @@ def fingerprint(ctx, sc):
     fp = [ctx.download(L.BUF_ENERGY_PER_TET, m.nT).tobytes()]
     for k in range(2):
         ctx.set_xtilde(soa(m.V_rest + 0.37 * (k + 1)))
-        fp.append(bits(ctx.inertia_energy()))
+        fp.append(scalar_bits(ctx.inertia_energy()))
     if sc.xtilde is not None:
         ctx.set_xtilde(soa(sc.xtilde))
     return fp
@@ -229,10 +217,6 @@ def stepped_fingerprint(ctx, sc, V0, alpha):
 
 def counts(info):
     return [info.halvings_inversion, info.halvings_intersection, info.halvings_armijo, info.halvings_post_check]
-
-
-def rel(a, b):
-    return abs(a - b) / abs(b)
 
 
 # ---- 1. the CFL branch ------------------------------------------------------------------------------------------------------------
@@ -264,21 +248,21 @@ def test_cfl_branch_matches_oracle(ctx, case):
         assert not first and cfl < a_part <= 2.0 * cfl and a_ref == cfl
     if case == "unchanged":
         assert a_part <= cfl and a_ref == a_part
-    upload(ctx, sc)
+    load_step_scene(ctx, sc)
     ctx.constraint_set(dhat_cs, 1, fetch=False, sizes=False)
     a = ctx.ccd_partial(None, TOL, evf, eee, 1.0)
-    assert bits(a) == bits(a_part)
-    assert bits(ctx.ccd_cfl(sc.dHat, first, voxel, TOL, evf, eee, a)) == bits(a_ref)
+    assert scalar_bits(a) == scalar_bits(a_part)
+    assert scalar_bits(ctx.ccd_cfl(sc.dHat, first, voxel, TOL, evf, eee, a)) == scalar_bits(a_ref)
     info = ctx.step_control_info()
-    assert info.status == 0 and bool(info.full_ccd) == full and bits(info.alpha_cfl) == bits(cfl)
+    assert info.status == 0 and bool(info.full_ccd) == full and scalar_bits(info.alpha_cfl) == scalar_bits(cfl)
     # the device-resident form: the same step in ipcgpu_fetch_iteration, the stages of a skipped branch report it
     ctx.step_bound_set(1.0)
     ctx.ccd_partial(None, TOL, evf, eee, None)
     ctx.ccd_cfl(sc.dHat, first, voxel, TOL, evf, eee, None)
     it = ctx.fetch_iteration()
-    assert it.status == 0 and bits(it.alpha) == bits(a_ref)
+    assert it.status == 0 and scalar_bits(it.alpha) == scalar_bits(a_ref)
     if not full:
-        assert bits(it.alpha_swept_grid) == bits(it.alpha_full_ccd) == bits(a_ref)
+        assert scalar_bits(it.alpha_swept_grid) == scalar_bits(it.alpha_full_ccd) == scalar_bits(a_ref)
     assert bool(ctx.step_control_info().full_ccd) == full
 
 
@@ -289,18 +273,18 @@ def test_line_search_matches_oracle(ctx, name):
     orc_lag(sc)
     ref = oracle_line_search(sc, 1.0)
     assert ref["status"] == 0 and min(ref["margins"]) > MARGIN
-    upload(ctx, sc)
+    load_step_scene(ctx, sc)
     rc, alpha = ctx.line_search(**sc.terms(), alpha=1.0)
     info = ctx.step_control_info()
     assert rc == 0 and info.status == 0
-    assert bits(alpha) == bits(ref["alpha"]) == bits(info.alpha)
+    assert scalar_bits(alpha) == scalar_bits(ref["alpha"]) == scalar_bits(info.alpha)
     assert counts(info) == ref["counts"] and bool(info.stopped) == ref["stopped"] and bool(info.post_check_rebuilt) == ref["rebuilt"]
-    assert bits(info.alpha_feasible) == bits(ref["LF"])
+    assert scalar_bits(info.alpha_feasible) == scalar_bits(ref["LF"])
     assert rel(info.energy_start, ref["E0"]) <= 1e-10 and rel(info.energy, ref["Et"]) <= 1e-10
     mm, pa, pe, cand = held_sets(ctx)
     for got, want in zip((mm, pa, pe, cand), ref["sets"]):
         assert np.array_equal(got, want)
-    assert bits(ctx.fetch_iteration().alpha) == bits(ref["alpha"])
+    assert scalar_bits(ctx.fetch_iteration().alpha) == scalar_bits(ref["alpha"])
     fp = fingerprint(ctx, sc)
     assert fp == stepped_fingerprint(ctx, sc, sc.m.V, alpha)
 
@@ -333,7 +317,7 @@ def prepare(ctx, sc, V, p):
 def test_captured_line_search_equals_eager(ctx):
     sc = scene_armijo()
     sc.fric = None
-    upload(ctx, sc, canonical=0)
+    load_step_scene(ctx, sc, canonical=0)
     evf, eee = L.Context.ti_error(sc.m.V_soa, sc.m.nV, None)
     # halvings of the Armijo loop on the oracle: 1, 0 and 2
     pairs = [(sc.m.V, sc.p), (sc.m.V, 0.05 * sc.p), (sc.m.V + 0.1 * sc.P, 2.0 * sc.p)]
@@ -355,14 +339,13 @@ def test_captured_line_search_equals_eager(ctx):
         g = ctx.step_control_info()
         assert ctx.launch_count() > n0
         assert g.status == e.status == 0
-        assert bits(g.alpha) == bits(e.alpha) and bits(g.alpha_cfl) == bits(e.alpha_cfl) and g.full_ccd == e.full_ccd
+        assert scalar_bits(g.alpha) == scalar_bits(e.alpha) and scalar_bits(g.alpha_cfl) == scalar_bits(e.alpha_cfl) and g.full_ccd == e.full_ccd
         assert counts(g) == counts(e) and g.stopped == e.stopped and g.post_check_rebuilt == e.post_check_rebuilt
         assert rel(g.energy, e.energy) <= 1e-12 and rel(g.energy_start, e.energy_start) <= 1e-12
         assert fingerprint(ctx, sc) == fe
         seen.append(tuple(counts(e)))
     assert len(set(seen)) >= 3 and any(c[2] == 0 for c in seen), seen
     ctx.graph_destroy(gid)
-    ctx.set_canonical_order(1)
 
 
 def whole_iteration(ctx, sc, evf, eee):
@@ -377,7 +360,7 @@ def whole_iteration(ctx, sc, evf, eee):
 def test_whole_iteration_graph(ctx):
     sc = scene_armijo()
     sc.fric = None
-    upload(ctx, sc, canonical=0)
+    load_step_scene(ctx, sc, canonical=0)
     ctx.enable_device_pattern(1)
     evf, eee = L.Context.ti_error(sc.m.V_soa, sc.m.nV, None)
     prepare(ctx, sc, sc.m.V, sc.p)
@@ -409,12 +392,11 @@ def test_whole_iteration_graph(ctx):
         ctx.graph_launch(gid)
         g, ig = ctx.step_control_info(), ctx.fetch_iteration()
         assert ig.status == ie.status == 0 and g.status == e.status == 0
-        assert bits(g.alpha) == bits(e.alpha) == bits(ig.alpha) == bits(ie.alpha) and counts(g) == counts(e)
+        assert scalar_bits(g.alpha) == scalar_bits(e.alpha) == scalar_bits(ig.alpha) == scalar_bits(ie.alpha) and counts(g) == counts(e)
         assert rel(ig.energy_elastic, ie.energy_elastic) <= 1e-12 and rel(g.energy, e.energy) <= 1e-12
         assert fingerprint(ctx, sc) == fe
     ctx.graph_destroy(gid)
     ctx.graph_destroy(gid0)
-    ctx.set_canonical_order(1)
 
 
 # ---- 4. termination and refusals (eager) ------------------------------------------------------------------------------------------
@@ -422,7 +404,7 @@ def test_intersecting_entry_state_returns_zero_step(ctx):
     sc = scene_intersection()
     sc.m.V[sc.m.nV // 2:, 2] -= 0.4
     V0 = sc.m.V.copy()
-    upload(ctx, sc)
+    load_step_scene(ctx, sc)
     rc, alpha = ctx.line_search(**sc.terms(), alpha=1.0, check=False)
     info = ctx.step_control_info()
     assert rc == info.status == L.ERR_LINE_SEARCH and alpha == 0.0 and info.alpha == 0.0
@@ -432,7 +414,7 @@ def test_intersecting_entry_state_returns_zero_step(ctx):
 
 def test_zero_entry_step_runs_nothing(ctx):
     sc = scene_tunnel()
-    upload(ctx, sc)
+    load_step_scene(ctx, sc)
     fp0 = fingerprint(ctx, sc)
     n0 = ctx.launch_count()
     rc, alpha = ctx.line_search(**sc.terms(), alpha=0.0, check=False)
@@ -443,7 +425,7 @@ def test_zero_entry_step_runs_nothing(ctx):
 
 def test_line_search_refused_without_a_search_direction(ctx):
     sc = scene_tunnel()
-    upload(ctx, sc, canonical=1)
+    load_step_scene(ctx, sc, canonical=1)
     m = sc.m
     ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)  # forgets the search direction
     ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)

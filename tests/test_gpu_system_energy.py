@@ -3,6 +3,8 @@ tests/oracle_diagnostics.py on multi-body piles (NH and FCR), a codimensional sc
 with an obstacle tail; identical bits for repeated, captured and replayed calls; a few time steps through ipcgpu_end_time_step; the
 component table's edge cases and refusals; and ipcgpu_constraint_summary against numpy over ipcgpu_evaluate_constraints and the plane
 distances of the downloaded positions."""
+import contextlib
+
 import numpy as np
 import pytest
 
@@ -11,6 +13,7 @@ import oracle_diagnostics as od
 import oracle_halfspace as ohs
 import oracle_kappa as ok
 import oracle_timestep as ot
+from gpu_common import load_scene, own_context, same_bits, scalar_bits, soa
 from ipc_b200 import codim
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
@@ -24,24 +27,15 @@ GRAVITY = (0.0, 0.0, -9.81)
 EPS = np.finfo(np.float64).eps
 
 
-def bits(a):
-    return np.ascontiguousarray(np.asarray(a, dtype=np.float64)).tobytes()
-
-
-def soa(V):
-    return np.ascontiguousarray(np.asarray(V).T).ravel()
-
-
+@contextlib.contextmanager
 def context(m, nV_dof=None, time=True):
-    ctx = L.Context(0)
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
-    if nV_dof is not None:
-        ctx.set_obstacle_tail(nV_dof)
-    if time:
-        ctx.set_time_integration(L.TIT_BE, DT, gravity=GRAVITY)
-    return ctx
+    with own_context() as ctx:
+        load_scene(ctx, m)
+        if nV_dof is not None:
+            ctx.set_obstacle_tail(nV_dof)
+        if time:
+            ctx.set_time_integration(L.TIT_BE, DT, gravity=GRAVITY)
+        yield ctx
 
 
 def moved(V, seed, amp):
@@ -88,13 +82,10 @@ def codim_mix():
 def test_pile_components(energy):
     m, ve, te = pile(energy)
     Vp = moved(m.V, 1, 1e-3)
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         ctx.set_prev_state(soa(Vp))
         ctx.set_components(ve, te)
         check_energy(ctx, m, m.V, Vp, m.mass, ve, te)
-    finally:
-        ctx.close()
 
 
 def test_codim_components():
@@ -104,13 +95,10 @@ def test_codim_components():
     V = m.V_rest + 1e-3 * np.random.default_rng(4).standard_normal(m.V_rest.shape)
     m.V = V
     Vp = moved(V, 5, 1e-3)
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         ctx.set_prev_state(soa(Vp))
         ctx.set_components(ve, te)
         check_energy(ctx, m, V, Vp, m.mass, ve, te)
-    finally:
-        ctx.close()
 
 
 def test_obstacle_tail_excluded():
@@ -120,22 +108,18 @@ def test_obstacle_tail_excluded():
     ve = np.arange(1, nb + 1, dtype=np.int32) * (m.nV // nb)
     te = np.arange(1, nb + 1, dtype=np.int32) * (m.nT // nb)
     Vp = moved(mm.V, 6, 1e-3)
-    ctx = context(mm, nV_dof=mm.nV_dof)
-    try:
+    with context(mm, nV_dof=mm.nV_dof) as ctx:
         ctx.set_prev_state(soa(Vp))
         with pytest.raises(L.IpcGpuError, match="ARG"):  # the tail belongs to no component
             ctx.set_components(np.append(ve[:-1], mm.nV), te)
         ctx.set_components(ve, te)
         check_energy(ctx, m, mm.V, Vp, mm.mass, ve, te)
-    finally:
-        ctx.close()
 
 
 def test_bits_repeat_capture_and_edge_ranges():
     m, _, _ = pile(0)
     Vp = moved(m.V, 7, 1e-3)
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         ctx.set_prev_state(soa(Vp))
         assert m.nV > 4200 and m.nT > 4200
         layouts = [
@@ -147,27 +131,24 @@ def test_bits_repeat_capture_and_edge_ranges():
             ctx.set_components(ve, te)
             a = check_energy(ctx, m, m.V, Vp, m.mass, np.asarray(ve), np.asarray(te))
             b = ctx.system_energy()
-            assert all(bits(x) == bits(y) for x, y in zip(a, b))
+            assert all(same_bits(x, y) for x, y in zip(a, b))
             n0 = ctx.launch_count()
             ctx.capture_begin()
             ctx.system_energy(want=False)
             gid = ctx.capture_end()
             ctx.graph_launch(gid)
             c = ctx.get_system_energy()
-            assert all(bits(x) == bits(y) for x, y in zip(a, c))
+            assert all(same_bits(x, y) for x, y in zip(a, c))
             assert ctx.launch_count() - n0 == 3
         # a new component table refuses the graphs captured before it
         ctx.set_components([m.nV], [m.nT])
         with pytest.raises(L.IpcGpuError, match="STATE"):
             ctx.graph_launch(gid)
-    finally:
-        ctx.close()
 
 
 def test_time_steps_through_end_time_step():
     m, ve, te = pile(1)
-    ctx = context(m)
-    try:
+    with context(m) as ctx:
         Vprev = m.V_rest.copy()
         ctx.set_prev_state(soa(Vprev))
         ctx.compute_xtilde()  # (the x~ that ipcgpu_end_time_step reads)
@@ -180,14 +161,11 @@ def test_time_steps_through_end_time_step():
             ctx.end_time_step()  # V_prev := V on the device
             Vprev = V.copy()
             V = V + 1e-3 * rng.standard_normal(V.shape)
-    finally:
-        ctx.close()
 
 
 def test_refusals():
     m, ve, te = pile(0)
-    ctx = context(m, time=False)
-    try:
+    with context(m, time=False) as ctx:
         ctx.set_prev_state(m.V_soa)
         with pytest.raises(L.IpcGpuError, match="STATE"):  # no components yet
             ctx.system_energy()
@@ -204,8 +182,6 @@ def test_refusals():
         ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
         with pytest.raises(L.IpcGpuError, match="STATE"):
             ctx.system_energy()
-    finally:
-        ctx.close()
 
 
 # ---- the constraint summary --------------------------------------------------------------------------------------------------------
@@ -221,7 +197,7 @@ def summary_check(ctx, m, dHat, kappa, par=None):
         act = ctx.get_halfspace_sets()[0]
         d = np.concatenate([od.plane_d2(par, V, act), vals])
     n, lo, hi, fbn, scale = od.summary(d, dHat, kappa)
-    assert (got.n, bits(got.d_min), bits(got.d_max)) == (n, bits(lo), bits(hi))
+    assert (got.n, scalar_bits(got.d_min), scalar_bits(got.d_max)) == (n, scalar_bits(lo), scalar_bits(hi))
     assert abs(got.fb_norm - fbn) <= max(1e-13 * fbn, 8 * EPS * scale), (got.fb_norm, fbn, scale)
     return got
 
@@ -239,8 +215,7 @@ def planes_par(pl):
 
 def test_summary_self_and_planes_host_and_device_kappa():
     m, dHat, pl = mat_with_plane()
-    ctx = context(m, time=False)
-    try:
+    with context(m, time=False) as ctx:
         ctx.set_halfspaces(**pl)
         ctx.constraint_set(dHat, 1)
         assert ctx.halfspace_constraint_set(dHat) > 0 and ctx.nC > 0
@@ -252,24 +227,21 @@ def test_summary_self_and_planes_host_and_device_kappa():
         gid = ctx.capture_end()
         ctx.graph_launch(gid)
         b = ctx.get_constraint_summary()
-        assert (a.n, bits(a.d_min), bits(a.d_max), bits(a.fb_norm)) == (b.n, bits(b.d_min), bits(b.d_max), bits(b.fb_norm))
+        assert (a.n, scalar_bits(a.d_min), scalar_bits(a.d_max), scalar_bits(a.fb_norm)) == (b.n, scalar_bits(b.d_min), scalar_bits(b.d_max), scalar_bits(b.fb_norm))
         # kappa on the device after initKappa: the host-kappa call at the kappa read back
         ctx.barrier_gradient(1e-30, 0.0, np.zeros(3 * m.nV))  # (a defined device gradient g_E for initKappa)
         ctx.set_kappa(1.0, 1e3, 1e12)
         ctx.kappa_init(dHat)
         k = ctx.kappa_info().kappa
         dev, host = ctx.constraint_summary(dHat, KD), ctx.constraint_summary(dHat, k)
-        assert (dev.n, bits(dev.d_min), bits(dev.d_max), bits(dev.fb_norm)) == (host.n, bits(host.d_min), bits(host.d_max), bits(host.fb_norm))
-    finally:
-        ctx.close()
+        assert (dev.n, scalar_bits(dev.d_min), scalar_bits(dev.d_max), scalar_bits(dev.fb_norm)) == (host.n, scalar_bits(host.d_min), scalar_bits(host.d_max), scalar_bits(host.fb_norm))
 
 
 def test_summary_planes_only_and_empty():
     V, T = M.grid_tets(4, 4, 4, h=0.25)
     m = M.Mesh(V, T, energy=0)
     dHat = 1e-4
-    ctx = context(m, time=False)
-    try:
+    with context(m, time=False) as ctx:
         ctx.constraint_set(dHat, 1)
         assert ctx.nC == 0
         e = ctx.constraint_summary(dHat, 1e4)  # no plane, no pair: "no collision in this time step"
@@ -278,32 +250,24 @@ def test_summary_planes_only_and_empty():
         ctx.set_halfspaces(**pl)
         assert ctx.halfspace_constraint_set(dHat) > 0
         assert summary_check(ctx, m, dHat, 1e4, planes_par(pl)).n > 0
-    finally:
-        ctx.close()
 
 
 def test_summary_obstacle_pairs():
     m, info = scenes.balls_on_obstacle(3, res=4)
     mm = OB.with_obstacle(m, info["obstacle"]["V"], info["obstacle"]["E"], info["obstacle"]["F"])
     dHat = info["dHat"]
-    ctx = context(mm, nV_dof=mm.nV_dof, time=False)
-    try:
+    with context(mm, nV_dof=mm.nV_dof, time=False) as ctx:
         mm_set = ctx.constraint_set(dHat, 1)[0]
         assert any(OB.involves_obstacle(q, mm.nV_dof) for q in mm_set)
         summary_check(ctx, mm, dHat, 2e5)
-    finally:
-        ctx.close()
 
 
 def test_summary_codim_pairs():
     m = codim_mix()
     m.V = m.V_rest.copy()
     dHat = 0.1 ** 2
-    ctx = context(m, time=False)
-    try:
+    with context(m, time=False) as ctx:
         mm_set = ctx.constraint_set(dHat, 1)[0]
         codim_v = set(np.flatnonzero(m.vCoDim < 3).tolist())
         assert any(codim_v & set(ok.stencil(q)[1]) for q in mm_set)
         assert summary_check(ctx, m, dHat, 1e3).n == len(mm_set)
-    finally:
-        ctx.close()

@@ -1,7 +1,6 @@
 """The time-integration frame of a time step on the device -- ipcgpu_compute_xtilde, ipcgpu_end_time_step, ipcgpu_warm_start -- against the
 float64 restatement of tests/oracle_timestep.py, bit for bit; captured against eager; a multi-step run against the same frame driven from the
 host through the existing entry points; the refusals."""
-import struct
 
 import numpy as np
 import pytest
@@ -9,6 +8,7 @@ import pytest
 import oracle as orc
 import oracle_halfspace as OH
 import oracle_timestep as OT
+from gpu_common import load_scene, own_context, same_bits, scalar_bits, soa
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 
@@ -19,24 +19,10 @@ G = (0.2, -9.81, -0.4)
 PARAMS = {"BE": (OT.BE, 0.25, 0.5), "NM": (OT.NM, 0.25, 0.5), "NM_nondefault": (OT.NM, 0.3, 0.6)}
 
 
-def soa(A):
-    return np.ascontiguousarray(np.asarray(A).T).ravel()
-
-
-def same(a, b):
-    a, b = np.ascontiguousarray(a, dtype=np.float64), np.ascontiguousarray(b, dtype=np.float64)
-    return a.shape == b.shape and a.tobytes() == b.tobytes()
-
-
-def bits(x):
-    return struct.pack("<d", float(x))
-
-
 @pytest.fixture(scope="module")
 def ctx():
-    c = L.Context(0)
-    yield c
-    c.close()
+    with own_context() as c:
+        yield c
 
 
 def upload_mesh(ctx, Vr, m, mass, dbc):
@@ -71,10 +57,10 @@ def test_xtilde_and_end_of_step_bit_identical(ctx, name):
     ctx.set_state(soa(V1))
     ctx.set_prev_state(soa(Vp))
     ctx.set_dynamics(vel.ravel(), soa(acc), soa(dxe))
-    assert all(same(a, b) for a, b in zip(dynamics(ctx, nV), (vel, acc, dxe)))
+    assert all(same_bits(a, b) for a, b in zip(dynamics(ctx, nV), (vel, acc, dxe)))
     ctx.compute_xtilde()
     xt = OT.xtilde(P, Vp, vel, acc, dbc)
-    assert same(ctx.download(L.BUF_XTILDE, 3 * nV).reshape(3, nV).T, xt)
+    assert same_bits(ctx.download(L.BUF_XTILDE, 3 * nV).reshape(3, nV).T, xt)
     assert np.array_equal(xt[dbc != 0], Vp[dbc != 0])
     # two ends of a time step: the second one reads what the first one left (V_prev, x~, velocity, acceleration)
     for k in range(2):
@@ -82,14 +68,14 @@ def test_xtilde_and_end_of_step_bit_identical(ctx, name):
         ctx.end_time_step()
         got = dynamics(ctx, nV)
         for g, r in zip(got, ref[:3]):
-            assert same(g, r), (name, k)
-        assert same(ctx.download(L.BUF_XTILDE, 3 * nV).reshape(3, nV).T, ref[4])
+            assert same_bits(g, r), (name, k)
+        assert same_bits(ctx.download(L.BUF_XTILDE, 3 * nV).reshape(3, nV).T, ref[4])
         vel, acc, _, Vp, xt = ref
         V1 = V1 + rng.standard_normal((nV, 3)) * 0.01
         ctx.set_state(soa(V1))
     ctx.set_prev_state(soa(Vp))  # (V_prev is what the last end of step left: set it again from the host, the result must not change)
     ctx.compute_xtilde()
-    assert same(ctx.download(L.BUF_XTILDE, 3 * nV).reshape(3, nV).T, xt)
+    assert same_bits(ctx.download(L.BUF_XTILDE, 3 * nV).reshape(3, nV).T, xt)
 
 
 # ---- 2. the warm start against the oracle driver ------------------------------------------------------------------------------------------
@@ -178,15 +164,15 @@ def test_warm_start_matches_oracle(ctx, scene, option, typ):
     it = ctx.fetch_iteration()
     ref = OT.warm_start(m, P, option, sc.vel, sc.dxe, sc.voxel, TOL, evf, eee, sc.planes(), alpha_inversion=it.alpha_inversion if option else None)
     assert rc == ref["status"] == info.status == 0
-    assert same(ctx.download(L.BUF_SEARCH_DIR, 3 * m.nV), ref["p"])
-    assert bits(a) == bits(ref["alpha"]) == bits(info.alpha) == bits(info.alpha_feasible) == bits(it.alpha)
+    assert same_bits(ctx.download(L.BUF_SEARCH_DIR, 3 * m.nV), ref["p"])
+    assert scalar_bits(a) == scalar_bits(ref["alpha"]) == scalar_bits(info.alpha) == scalar_bits(info.alpha_feasible) == scalar_bits(it.alpha)
     assert [info.halvings_inversion, info.halvings_intersection] == ref["counts"]
-    assert same(positions(ctx, m.nV), ref["V"])
+    assert same_bits(positions(ctx, m.nV), ref["V"])
     if option:
-        assert bits(it.alpha_inversion) == bits(ref["alpha_inversion"])
+        assert scalar_bits(it.alpha_inversion) == scalar_bits(ref["alpha_inversion"])
         if sc.plane is not None:
-            assert bits(it.alpha_halfspace) == bits(ref["alpha_halfspace"])
-        assert bits(it.alpha_swept_grid) == bits(ref["alpha_swept_grid"]) and bits(it.alpha_full_ccd) == bits(ref["alpha_full_ccd"])
+            assert scalar_bits(it.alpha_halfspace) == scalar_bits(ref["alpha_halfspace"])
+        assert scalar_bits(it.alpha_swept_grid) == scalar_bits(ref["alpha_swept_grid"]) and scalar_bits(it.alpha_full_ccd) == scalar_bits(ref["alpha_full_ccd"])
         binding = {"ccd": ref["alpha_full_ccd"] < ref["alpha_swept_grid"], "plane": 0.0 < ref.get("alpha_halfspace", 1.0) < ref["alpha_inversion"],
                    "inversion": ref["alpha_inversion"] < 1.0, "zero": ref["alpha"] == 0.0}
         assert binding[scene], (scene, ref)
@@ -215,7 +201,7 @@ def test_failing_entry_state_keeps_v0(ctx, entry):
     ref = OT.warm_start(m, P, 1, sc.vel, sc.dxe, sc.voxel, TOL, evf, eee, alpha_inversion=ctx.fetch_iteration().alpha_inversion)
     assert rc == info.status == ref["status"] == L.ERR_LINE_SEARCH and a == 0.0
     assert [info.halvings_inversion, info.halvings_intersection] == ref["counts"]
-    assert same(positions(ctx, m.nV), m.V)
+    assert same_bits(positions(ctx, m.nV), m.V)
 
 
 # ---- 3. captured against eager ------------------------------------------------------------------------------------------------------------
@@ -258,12 +244,11 @@ def test_captured_frame_equals_eager(ctx):
                 frame(ctx, sc, evf, eee, dHat)
             info, it = ctx.step_control_info(), ctx.fetch_iteration()
             out.append((positions(ctx, m.nV).tobytes(), ctx.download(L.BUF_XTILDE, 3 * m.nV).tobytes(), *[x.tobytes() for x in ctx.get_dynamics()],
-                        bits(info.alpha), info.halvings_intersection, bits(it.alpha_full_ccd), ctx.constraint_set_sizes()))
+                        scalar_bits(info.alpha), info.halvings_intersection, scalar_bits(it.alpha_full_ccd), ctx.constraint_set_sizes()))
         runs.append(out)
     assert runs[0] == runs[1]
     assert len({r[0] for r in runs[0]}) == 4  # the bodies moved at every step
     ctx.graph_destroy(gid)
-    ctx.set_canonical_order(1)
 
 
 # ---- 4. a multi-step run: the device frame against the host-driven frame --------------------------------------------------------------------
@@ -303,6 +288,7 @@ def host_frame(ctx, m, P, state, option, voxel, evf, eee):
 
 
 def test_multi_step_run_equals_host_driven(ctx):
+    ctx.set_canonical_order(1)  # (the module's context: the captured-frame test above runs at 0)
     V1, T1 = M.grid_tets(3, 3, 3, h=1.0 / 3)
     V2, T2 = M.grid_tets(2, 2, 2, h=0.25, origin=(0.3, 0.3, 1.3))  # (K steps of at most 0.06 leave the bodies apart: no contact pairs)
     m = M.merge_meshes([(V1, T1), (V2, T2)], energy=0, density=1.0)
@@ -314,9 +300,7 @@ def test_multi_step_run_equals_host_driven(ctx):
     evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
     trajectories, alphas = [], []
     for device in (True, False):
-        ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-        ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-        ctx.set_state(m.V_soa)
+        load_scene(ctx, m)
         ctx.set_prev_state(m.V_soa)
         ctx.set_time_integration(P.type, P.dt, P.beta, P.gamma, P.gravity)
         ctx.set_dynamics(vel0.ravel(), None, None)
@@ -341,30 +325,27 @@ def test_multi_step_run_equals_host_driven(ctx):
 
 # ---- 5. refusals ----------------------------------------------------------------------------------------------------------------------------
 def test_refusals():
-    ctx = L.Context(0)  # (a fresh context: no time integration set yet)
-    sc = wscene_plane()
-    m = sc.m
-    evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
-    ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, m.energy)
-    ctx.set_surface(m.SVI, m.SFEdges, m.SF_soa, m.vCoDim)
-    ctx.set_state(m.V_soa)
-    ctx.set_prev_state(m.V_soa)
-    ctx.set_dynamics(sc.vel.ravel(), None, None)
-    with pytest.raises(L.IpcGpuError, match="STATE"):  # no set_time_integration on this context yet
-        ctx.warm_start(1, sc.voxel, TOL, evf, eee)
-    with pytest.raises(L.IpcGpuError, match="ARG"):
-        ctx.set_time_integration(2, 0.01)
-    ctx.set_time_integration(OT.BE, 0.01)
-    for option in (5, -1, 6):
+    with own_context() as ctx:  # (a fresh context: no time integration set yet)
+        sc = wscene_plane()
+        m = sc.m
+        evf, eee = L.Context.ti_error(m.V_soa, m.nV, None)
+        load_scene(ctx, m)
+        ctx.set_prev_state(m.V_soa)
+        ctx.set_dynamics(sc.vel.ravel(), None, None)
+        with pytest.raises(L.IpcGpuError, match="STATE"):  # no set_time_integration on this context yet
+            ctx.warm_start(1, sc.voxel, TOL, evf, eee)
         with pytest.raises(L.IpcGpuError, match="ARG"):
-            ctx.warm_start(option, sc.voxel, TOL, evf, eee)
-    ctx.warm_start(1, sc.voxel, TOL, evf, eee)
-    # a new mesh forgets nothing of the time integration, but its V_prev must be set again when it has more vertices
-    V, T = M.grid_tets(4, 4, 4, h=0.25)
-    m2 = M.Mesh(V, T, energy=1, density=1.0)
-    ctx.set_mesh(m2.V_rest_soa, m2.T_soa, m2.restTriInv, m2.vol, m2.mu, m2.lam, m2.mass, m2.dbc, m2.energy)
-    ctx.set_surface(m2.SVI, m2.SFEdges, m2.SF_soa, m2.vCoDim)
-    for call in (ctx.compute_xtilde, lambda: ctx.warm_start(1, sc.voxel, TOL, evf, eee)):
-        with pytest.raises(L.IpcGpuError, match="STATE"):
-            call()
-    ctx.close()
+            ctx.set_time_integration(2, 0.01)
+        ctx.set_time_integration(OT.BE, 0.01)
+        for option in (5, -1, 6):
+            with pytest.raises(L.IpcGpuError, match="ARG"):
+                ctx.warm_start(option, sc.voxel, TOL, evf, eee)
+        ctx.warm_start(1, sc.voxel, TOL, evf, eee)
+        # a new mesh forgets nothing of the time integration, but its V_prev must be set again when it has more vertices
+        V, T = M.grid_tets(4, 4, 4, h=0.25)
+        m2 = M.Mesh(V, T, energy=1, density=1.0)
+        ctx.set_mesh(m2.V_rest_soa, m2.T_soa, m2.restTriInv, m2.vol, m2.mu, m2.lam, m2.mass, m2.dbc, m2.energy)
+        ctx.set_surface(m2.SVI, m2.SFEdges, m2.SF_soa, m2.vCoDim)
+        for call in (ctx.compute_xtilde, lambda: ctx.warm_start(1, sc.voxel, TOL, evf, eee)):
+            with pytest.raises(L.IpcGpuError, match="STATE"):
+                call()

@@ -30,13 +30,13 @@ alpha is held bit for bit to that rule applied to its own per-tet bounds, whatev
 """
 import importlib.util
 import os
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
 import refcubic
+from gpu_common import scalar_bits, shared_ctx
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 
@@ -60,16 +60,12 @@ def gen_module():
     return g
 
 
-def bits(x):
-    return struct.unpack("<Q", struct.pack("<d", float(x)))[0]
-
-
 def check(z, idx, got, who):
     """per-tet bounds `got` of tets idx against the fixture's bars; returns the worst error/bar ratio of the value checks"""
     worst, bad = 0.0, []
     for t, r in zip(idx, got):
         if z["exact"][t] and not z["ambiguous"][t]:
-            if bits(r) != bits(z["root"][t]):
+            if scalar_bits(r) != scalar_bits(z["root"][t]):
                 bad.append((t, "exact", r, z["root"][t]))
             continue
         if not z["ambiguous"][t]:
@@ -155,7 +151,7 @@ def test_cubic_branch_coverage():
     for t in range(len(z["family"])):
         a, b, c, d = double_coefs(z, t)
         r, ex, fb, passed, kept = orc.cubic_branch(a, b, c, d)
-        assert bits(r if r >= 0 else NONE) == bits(per_all[t])   # the branch report is the filter's own computation
+        assert scalar_bits(r if r >= 0 else NONE) == scalar_bits(per_all[t])   # the branch report is the filter's own computation
         seen.add(ex)
         if ex == "linear":
             seen.add("linear c>0" if c > 0 else "linear c<0" if c < 0 else "linear c=0")
@@ -217,7 +213,7 @@ def test_reference_root_finder_meets_the_fixture():
         per[t] = r if r >= 0 else NONE
         a, b, c, d = z["coef"][t]
         if abs(a) <= TOL and abs(b) > TOL:
-            assert bits(refcubic.quad_root(b, c, d)) == bits(r)
+            assert scalar_bits(refcubic.quad_root(b, c, d)) == scalar_bits(r)
     # a coefficient that the fixture holds exactly as a signed zero (a flat tet's d, a zero direction's c) is +0.0 in coef: the sign
     # the double arithmetic gives it is not in the rounded value, so those tets are compared by value
     sz = z["exact"] & ~z["ambiguous"] & ((z["root"] == 0) | np.isinf(z["root"]))
@@ -256,11 +252,11 @@ def run_gpu(ctx, X, P, slack, alpha=1.0):
 
 
 @pytest.mark.gpu
-def test_device_matches_fixture(gpu_ctx):
+def test_device_matches_fixture(shared_ctx):
     z = gold()
     worst = 0.0
     for s, idx in groups(z).items():
-        _, per = run_gpu(gpu_ctx, z["X"][idx], z["P"][idx], s)
+        _, per = run_gpu(shared_ctx, z["X"][idx], z["P"][idx], s)
         worst = max(worst, check(z, idx, per, "device"))
     print(f"\ndevice: worst error/bar {worst:.3g}")
 
@@ -282,7 +278,7 @@ def _soup(z, picks, n=3 * 256 + 40):
 
 
 @pytest.mark.gpu
-def test_device_step_follows_the_reference_rule(gpu_ctx):
+def test_device_step_follows_the_reference_rule(shared_ctx):
     """alpha_out == the reference's rule on the device's own per-tet bounds, with zero bounds of either sign in the CTA of the smallest
     positive bound and in another one, and with no bound at all"""
     z = gold()
@@ -304,11 +300,11 @@ def test_device_step_follows_the_reference_rule(gpu_ctx):
     for name, picks in soups.items():
         X, P = _soup(z, picks)
         for alpha in alphas:
-            a, per = run_gpu(gpu_ctx, X, P, 0.2, alpha)
+            a, per = run_gpu(shared_ctx, X, P, 0.2, alpha)
             want = ref_rule(per, alpha)
-            assert bits(a) == bits(want), (name, alpha, a, want)
+            assert scalar_bits(a) == scalar_bits(want), (name, alpha, a, want)
             for pos, t in picks:
-                assert bits(per[pos]) == bits(z["root"][t]) or not z["exact"][t], (name, pos, per[pos], z["root"][t])
+                assert scalar_bits(per[pos]) == scalar_bits(z["root"][t]) or not z["exact"][t], (name, pos, per[pos], z["root"][t])
             if "0.0" in name:
                 assert a == alpha, (name, alpha, a)   # a zero bound leaves the step unchanged
             if name == "no root":
@@ -316,7 +312,7 @@ def test_device_step_follows_the_reference_rule(gpu_ctx):
 
 
 @pytest.mark.gpu
-def test_device_placement_does_not_change_a_tet(gpu_ctx):
+def test_device_placement_does_not_change_a_tet(shared_ctx):
     """the slack-0.2 soup padded past three CTAs, and the same tets shifted by 257 places (cyclically): every tet changes CTA and lane, its
     bound's bits and the step do not"""
     z = gold()
@@ -328,7 +324,7 @@ def test_device_placement_does_not_change_a_tet(gpu_ctx):
     X2, P2 = np.empty_like(X), np.empty_like(P)
     X2[perm], P2[perm] = X, P
     for alpha in (1.0, 0.01):
-        a1, per1 = run_gpu(gpu_ctx, X, P, 0.2, alpha)
-        a2, per2 = run_gpu(gpu_ctx, X2, P2, 0.2, alpha)
+        a1, per1 = run_gpu(shared_ctx, X, P, 0.2, alpha)
+        a2, per2 = run_gpu(shared_ctx, X2, P2, 0.2, alpha)
         assert per1.view(np.uint64).tolist() == per2[perm].view(np.uint64).tolist()
-        assert bits(a1) == bits(a2) == bits(ref_rule(per1, alpha))
+        assert scalar_bits(a1) == scalar_bits(a2) == scalar_bits(ref_rule(per1, alpha))

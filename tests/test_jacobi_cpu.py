@@ -12,17 +12,13 @@ import scipy.sparse as sp
 import oracle as orc
 import oracle_jacobi as OJ
 import oracle_timestep as OT
+from gpu_common import same_bits
 from ipc_b200 import lib as L
 from ipc_b200 import mesh as M
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 COEF = 0.01 ** 2
 N_TAIL = 5
-
-
-def same(a, b):
-    a, b = np.ascontiguousarray(a, dtype=np.float64), np.ascontiguousarray(b, dtype=np.float64)
-    return a.shape == b.shape and a.tobytes() == b.tobytes()
 
 
 def system(base, projectDBC):
@@ -73,13 +69,13 @@ def test_precondition_diag_matches_a_dense_reading(base, projectDBC):
     fixed = np.repeat(m.dbc != 0, 3)
     for sign in (-1, 1):
         out = OJ.precondition_diag(g, ia, a, base, sign)
-        assert same(out, (sign * g) / d)
+        assert same_bits(out, (sign * g) / d)
         assert np.isfinite(out).all()
         if projectDBC:  # identity rows with a zero gradient: 0 without a special case
             assert not out[fixed].any() and (d[fixed] == 1.0).all()
         else:  # penalty mode: those rows are divided like any other
             assert out[fixed].all()
-    assert same(OJ.precondition_diag(g, ia, a, base, -1), -OJ.precondition_diag(g, ia, a, base, 1))
+    assert same_bits(OJ.precondition_diag(g, ia, a, base, -1), -OJ.precondition_diag(g, ia, a, base, 1))
 
 
 def test_zero_and_negative_diagonals_are_divided():
@@ -98,7 +94,7 @@ def test_jacobi_predictor(base, projectDBC):
     p = OJ.jacobi_predictor(g, ia, a, base, m.dbc).reshape(-1, 3)
     q = OJ.precondition_diag(g, ia, a, base, -1).reshape(-1, 3)
     fixed = m.dbc != 0
-    assert same(p[~fixed], q[~fixed])
+    assert same_bits(p[~fixed], q[~fixed])
     assert (p[fixed].view(np.uint64) == 0).all()  # +0.0, whatever the row held (penalty mode: nonzero)
     assert fixed[-N_TAIL:].all()
 
@@ -117,7 +113,7 @@ def test_warm_start_driver_takes_a_predictor():
     got = OJ.warm_start(m, OT.predictor(P, 2, vel, dxe, m.dbc).ravel(), m.avgEdgeLen / 3.0, 1e-6, evf, eee)
     assert ref["alpha"] < 1.0  # the bodies close: the bound binds
     for k in ("p", "V"):
-        assert same(got[k], ref[k]), k
+        assert same_bits(got[k], ref[k]), k
     for k in ("alpha", "alpha_inversion", "alpha_swept_grid", "alpha_full_ccd", "counts", "status"):
         assert got[k] == ref[k], k
 

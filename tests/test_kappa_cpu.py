@@ -1,16 +1,12 @@
 """ipcgpu_kappa_bounds (suggestKappa / upperBoundKappa, Optimizer.cpp:2216-2233) against the float64 restatement, bit for bit, over a grid
 of dHat, bounding box, node mass and multiplier (host-only: no GPU needed)."""
 import itertools
-import struct
 
 import pytest
 
 import oracle_kappa as ok
+from gpu_common import scalar_bits
 from ipc_b200 import lib as L
-
-
-def bits(x):
-    return struct.pack("<d", float(x))
 
 
 @pytest.mark.parametrize("dHat", [1e-8, 3.7e-6, 1e-4, 2.5e-3])
@@ -18,7 +14,7 @@ def test_bounds_bits(dHat):
     for bbox2, mass, mult in itertools.product([1e-2, 1.0, 3.3, 250.0], [1e-6, 0.013, 2.0], [1e-11, 0.1, 1.0]):
         s, m = L.Context.kappa_bounds(dHat, mult, mass, bbox2)
         rs, rm = ok.bounds(dHat, mult, mass, bbox2)
-        assert bits(s) == bits(rs) and bits(m) == bits(rm), (dHat, bbox2, mass, mult, s, rs, m, rm)
+        assert scalar_bits(s) == scalar_bits(rs) and scalar_bits(m) == scalar_bits(rm), (dHat, bbox2, mass, mult, s, rs, m, rm)
         assert 0.0 < s < m
 
 

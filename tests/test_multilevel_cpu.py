@@ -6,8 +6,8 @@ import pytest
 import scipy.sparse.linalg as spla
 
 import multilevel_mirror as mlm
+from gpu_common import rel
 from ipc_b200 import scenes
-from stagecheck import rel
 
 DT2 = 0.025 ** 2
 

@@ -7,12 +7,12 @@ the FullPivLU solve of segTriIntersect (Eigen's order, bit for bit) and the dete
 solve's decisions and the double-vs-exact disagreements."""
 import importlib.util
 import os
-import struct
 
 import numpy as np
 import pytest
 
 import oracle as orc
+from gpu_common import scalar_bits, shared_ctx
 from ipc_b200 import mesh as M
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -31,10 +31,6 @@ def gen_module():
     g = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(g)
     return g
-
-
-def bits(x):
-    return struct.pack("<d", float(x))
 
 
 # ---- CPU --------------------------------------------------------------------------------------------------------------------------------
@@ -77,7 +73,7 @@ def test_oracle_segment_triangle_meets_the_fixture_bit_for_bit():
         dec, ex, rank, uvt = orc.seg_tri_trace(*p)
         assert ex == z["segtri_exit"][k] and dec == z["segtri_dec"][k], k
         if ex == 2:
-            assert rank == z["segtri_rank"][k] and all(bits(a) == bits(b) for a, b in zip(uvt, z["segtri_uvt"][k])), (k, uvt, z["segtri_uvt"][k])
+            assert rank == z["segtri_rank"][k] and all(scalar_bits(a) == scalar_bits(b) for a, b in zip(uvt, z["segtri_uvt"][k])), (k, uvt, z["segtri_uvt"][k])
 
 
 def test_oracle_inversion_count_meets_the_fixture():
@@ -212,62 +208,62 @@ def assert_matches(soup, total, tri, tet):
 
 
 @pytest.mark.gpu
-def test_device_decisions_per_stencil(gpu_ctx):
+def test_device_decisions_per_stencil(shared_ctx):
     z = gold()
     soup = Soup(z)
-    total, tri, tet = run_check(gpu_ctx, soup)
+    total, tri, tet = run_check(shared_ctx, soup)
     assert_matches(soup, total, tri, tet)
     # the eager form agrees with the deferred one
-    assert gpu_ctx.intersection_free() == (total == 0)
+    assert shared_ctx.intersection_free() == (total == 0)
 
 
 @pytest.mark.gpu
-def test_device_stencil_order_changes_no_decision(gpu_ctx):
+def test_device_stencil_order_changes_no_decision(shared_ctx):
     z = gold()
     for seed in (1, 2):
         soup = Soup(z, perm=np.random.default_rng(seed))
-        assert_matches(soup, *run_check(gpu_ctx, soup))
+        assert_matches(soup, *run_check(shared_ctx, soup))
 
 
 @pytest.mark.gpu
-def test_device_point_grid_scenes_alone(gpu_ctx):
+def test_device_point_grid_scenes_alone(shared_ctx):
     """families whose points alone make a degenerate point grid: one z for all points, a single point, duplicate points"""
     z = gold()
     g = gen_module()
     for name in g.ALONE:
         soup = Soup(z, pit_families=[g.FAMILIES["pit"].index(name)])
-        assert_matches(soup, *run_check(gpu_ctx, soup))
+        assert_matches(soup, *run_check(shared_ctx, soup))
 
 
 @pytest.mark.gpu
-def test_debug_buffers_off_keep_the_launch_count(gpu_ctx):
+def test_debug_buffers_off_keep_the_launch_count(shared_ctx):
     z = gold()
     soup = Soup(z)
-    soup.upload(gpu_ctx)
+    soup.upload(shared_ctx)
     counts = []
     for on in (0, 1, 0):
-        gpu_ctx.safeguard_debug_flags(on)
-        n0 = gpu_ctx.launch_count()
-        gpu_ctx.intersection_free(want=False)
-        counts.append((gpu_ctx.launch_count() - n0, gpu_ctx.fetch_iteration().n_intersected_triangles))
+        shared_ctx.safeguard_debug_flags(on)
+        n0 = shared_ctx.launch_count()
+        shared_ctx.intersection_free(want=False)
+        counts.append((shared_ctx.launch_count() - n0, shared_ctx.fetch_iteration().n_intersected_triangles))
     assert counts[0] == counts[1] == counts[2]
 
 
 @pytest.mark.gpu
-def test_device_inversion_count_per_tet(gpu_ctx):
+def test_device_inversion_count_per_tet(shared_ctx):
     """checkInversion's determinant in doubles, bit for bit: det == +0.0 and -0.0 are not inverted, one ulp either way decides"""
     z = gold()
     unit = np.array([[0, 0, 0], [1.0, 0, 0], [0, 1.0, 0], [0, 0, 1.0]])
     bad = []
     for k, t in enumerate(z["inv_tets"]):
         m = M.Mesh(unit, np.arange(4, dtype=np.int32).reshape(1, 4), energy=0)
-        gpu_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, 0)
-        gpu_ctx.set_state(np.ascontiguousarray(t.T).ravel())
-        if gpu_ctx.check_inversion() != int(z["inv_det"][k] < 0):
+        shared_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, 0)
+        shared_ctx.set_state(np.ascontiguousarray(t.T).ravel())
+        if shared_ctx.check_inversion() != int(z["inv_det"][k] < 0):
             bad.append(k)
     assert not bad, bad
     n = len(z["inv_tets"])
     m = M.Mesh(np.tile(unit, (n, 1)), np.arange(4 * n, dtype=np.int32).reshape(n, 4), energy=0)
-    gpu_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, 0)
-    gpu_ctx.set_state(np.ascontiguousarray(z["inv_tets"].reshape(-1, 3).T).ravel())
-    assert gpu_ctx.check_inversion() == int((z["inv_det"] < 0).sum())
+    shared_ctx.set_mesh(m.V_rest_soa, m.T_soa, m.restTriInv, m.vol, m.mu, m.lam, m.mass, m.dbc, 0)
+    shared_ctx.set_state(np.ascontiguousarray(z["inv_tets"].reshape(-1, 3).T).ravel())
+    assert shared_ctx.check_inversion() == int((z["inv_det"] < 0).sum())
